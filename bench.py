@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmarks of the B200 Tacotron-2 hot paths (BASELINE.json metric:
-"WaveNet train audio-samples/sec/GPU; Tacotron mel-frames/sec; 1/2/4/8 B200").
+"""bench.py — headline benchmarks of the H100 Tacotron-2 hot paths (BASELINE.json metric:
+"WaveNet train audio-samples/sec/GPU; Tacotron mel-frames/sec; 1/2/4/8 H100").
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME]      # our arm (CUDA, one process per GPU)
+  python bench.py [...] --dump-outputs DIR                                   # also write the last timed step's results as DIR/*.npy
   python bench.py --impl reference [...]                                     # CPU arm: the oracle restatement of the reference
                                                                              # graph on the host cores (TF1 cannot be installed
                                                                              # here; DESIGN.md §2)
@@ -91,7 +92,7 @@ def taco_batch(hp, B, T_in, T_out, seed):
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -137,14 +138,6 @@ def _peaks():
         return {}
 
 
-def _traffic(key):
-    """measured DRAM bytes (read + write) from the committed ncu pass (profiles/r02_dram_traffic.json), or None"""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r02_dram_traffic.json"))).get(key)
-    except Exception:
-        return None
-
-
 def _pick_threads(fn):
     """fastest torch intra-op thread count for this graph on this host (oversubscribing a 128-core box is ~5x slower)"""
     import torch
@@ -180,7 +173,7 @@ class WaveNetWorkload(object):
                                                     "raw input + MoL-%d NLL" % (hp.out_channels // 3) if self.scalar else "mu-law-256 one-hot + softmax-CE",
                                                     self.B, self.T, hp.wavenet_dropout, world),
                 "per_gpu_batch": self.B, "samples_per_item": self.T, "parallelism": "dp%d" % world,
-                "l2": "per-step working set (activations stashed for backward, GBs) >> 126 MB L2: no explicit flush"}
+                "l2": "per-step working set (activations stashed for backward, GBs) >> 50 MB L2: no explicit flush"}
 
     def setup(self, dev, rank, use_graph):
         import torch
@@ -195,7 +188,7 @@ class WaveNetWorkload(object):
         self.use_graph = use_graph
         if use_graph:
             # data parallel: the step is cut into 3 graphs after each third of the stack's weight gradients so that the NCCL
-            # all-reduce of a third overlaps the next third's GEMM (3 x 8 layers = 3 x 144 tiles = 3 full waves of 148 SMs)
+            # all-reduce of a third overlaps the next third's GEMM
             world = int(os.environ.get("WORLD_SIZE", "1"))
             self.model.capture(*self.static, overlap_groups=3 if (world >= 4 and self.hp.layers % 3 == 0 and os.environ.get("T2_AR_OVERLAP", "1") != "0") else 1)
 
@@ -216,6 +209,12 @@ class WaveNetWorkload(object):
     def loss(self):
         return self.model.loss_value()
 
+    def outputs(self):
+        import numpy as np
+        return {"loss": np.array([self.model.loss_value()], dtype=np.float64),
+                "loss_sum_and_count": self.model.loss_buf.double().cpu().numpy(),
+                "grads": _flat_sample(self.model.export_grads()), "params": _flat_sample(self.model.export_params())}
+
     def launches_per_step(self):
         return int(self.model.launches_per_step)
 
@@ -228,8 +227,8 @@ class WaveNetWorkload(object):
         BT = self.B * self.T
         flops_gate = 2.0 * BT * G * (3 * R + C)
         pk = _peaks()
-        burst, sustained, hbm = float(pk.get("bf16_tflops", 1590.0)), float(pk.get("bf16_tflops_sustained", 1400.0)), float(pk.get("hbm_gbs", 6650.0))
-        src = "MEASURED_PEAKS.json" if pk else "fallback (B200_PROFILING.md)"
+        burst, sustained, hbm = float(pk.get("bf16_tflops", 989.0)), float(pk.get("bf16_tflops_sustained", 989.0)), float(pk.get("hbm_gbs", 3350.0))
+        src = "MEASURED_PEAKS.json" if pk else "H100 SXM data sheet (dense bf16, HBM3)"
         # whole residual stack, SURVEY §8d accounting: FLOPs fwd = 2(3RG + CG + (G/2)S + (G/2)R) per (b,t,layer), x3 for fwd+bwd;
         # algorithmic bytes fwd+bwd = (5R + 2C + 3S) * sizeof(activation); activations are stored as bf16 here
         flops_step = 3.0 * 2.0 * (3 * R * G + C * G + (G // 2) * S + (G // 2) * R) * BT * L
@@ -238,21 +237,19 @@ class WaveNetWorkload(object):
         step = {"algorithmic_tflop": flops_step / 1e12, "tflops": flops_step / sec / 1e12, "frac_of_sustained_bf16": flops_step / sec / 1e12 / sustained,
                 "algorithmic_gb_bf16_act": bytes_step / 1e9, "gbs": bytes_step / sec / 1e9, "frac_of_hbm": bytes_step / sec / 1e9 / hbm,
                 "t_min_ms": 1e3 * max(flops_step / (sustained * 1e12), bytes_step / (hbm * 1e9)),
-                "dram_bytes_measured": _traffic(self.name + "_step_dram_bytes"),
                 "note": "residual stack only (head, upsampling net and optimizer excluded from the algorithmic figures, included in the time)"}
-        gate = {"kernel": "act_gemm_kernel<EPI_GATE,256,NT=2> (per-layer dilated-conv + conditioning gate GEMM, %d launches / step)" % L,
+        gate = {"kernel": "act_gemm_kernel<EPI_GATE,256> (per-layer dilated-conv + conditioning gate GEMM, %d launches / step)" % L,
                 "timing": "CUDA events around 20 back-to-back launches replayed from one CUDA graph on a private stream (kernel timed ALONE), "
                           "averaged over layers %s" % probe,
                 "flops_per_launch": flops_gate, "ms_per_launch": gate_ms, "tflops": flops_gate / (gate_ms * 1e-3) / 1e12,
-                "frac_of_burst_bf16": flops_gate / (gate_ms * 1e-3) / 1e12 / burst,
-                "dram_bytes_measured": _traffic(self.name + "_gate_dram_bytes_per_launch")}
+                "frac_of_burst_bf16": flops_gate / (gate_ms * 1e-3) / 1e12 / burst}
         if self.name == "wavenet_default":
             # the HBM-bound shape: the roofline object is the whole dilated stack against the measured copy bandwidth
             return {"bound": "hbm", "kernel": "residual stack (gate / out / dz / dx / wgrad GEMM chain), whole training step",
-                    "achieved": step["gbs"], "peak": hbm, "unit": "GB/s", "frac": step["frac_of_hbm"], "traffic": step["dram_bytes_measured"],
+                    "achieved": step["gbs"], "peak": hbm, "unit": "GB/s", "frac": step["frac_of_hbm"],
                     "peak_source": src + " hbm_gbs (kernel chain timed inside the long step)", "step": step, "gate_gemm": gate}
         return {"bound": "tensor", "kernel": gate["kernel"], "timing": gate["timing"], "achieved": gate["tflops"], "peak": burst,
-                "unit": "TFLOP/s", "frac": gate["frac_of_burst_bf16"], "traffic": gate["dram_bytes_measured"],
+                "unit": "TFLOP/s", "frac": gate["frac_of_burst_bf16"],
                 "flops_per_launch": flops_gate, "ms_per_launch": gate_ms,
                 "peak_source": src + " bf16_tflops (burst: the kernel is timed in isolation)", "step": step}
 
@@ -306,7 +303,7 @@ class TacotronWorkload(object):
                             "r=1, predict_linear=False, conv dropout 0.5 / prenet dropout 0.5 / zoneout 0.1 ON, fwd+bwd+global-norm clip+Adam, "
                             "batch %d per GPU, T_in %d, T_out %d, bf16 GEMM operands / fp32 state, dp%d" % (self.B, self.Ti, self.To, world),
                 "per_gpu_batch": self.B, "frames_per_item": self.To, "parallelism": "dp%d" % world,
-                "l2": "per-step working set (state histories for BPTT, GBs) >> 126 MB L2: no explicit flush"}
+                "l2": "per-step working set (state histories for BPTT, GBs) >> 50 MB L2: no explicit flush"}
 
     def setup(self, dev, rank, use_graph):
         import torch
@@ -341,6 +338,13 @@ class TacotronWorkload(object):
     def loss(self):
         return self.model.losses()["total"]
 
+    def outputs(self):
+        import numpy as np
+        ls = self.model.losses()
+        return {"losses_before_after_stop_reg_linear_total": np.array([ls[k] for k in ("before", "after", "stop", "reg", "linear", "total")],
+                                                                      dtype=np.float64),
+                "grads": _flat_sample(self.model.export_grads()), "params": _flat_sample(self.model.export_params())}
+
     def launches_per_step(self):
         return int(self.model.launches_per_step)
 
@@ -352,17 +356,16 @@ class TacotronWorkload(object):
         w_params = (2 * H + D) * 4 * D + 2 * D * 4 * D + D * A + (D + 2 * H) * (M + 1)       # per-step recurrent operand set (prenet part batched)
         bytes_step = 2.0 * w_params * 2 * self.To                                           # bf16, forward + BPTT sweeps
         pk = _peaks()
-        hbm = float(pk.get("hbm_gbs", 6650.0))
+        hbm = float(pk.get("hbm_gbs", 3350.0))
         sec = ms_per_step * 1e-3
         flops = 3.0 * 34.0e6 * self.B * self.To + 3.0 * (11.0e6 * self.B * self.Ti + 10.98e6 * self.B * self.To)
         return {"bound": "hbm", "kernel": "decoder recurrence (EPI_LSTM swapped GEMMs + attention, %d dependent steps fwd and bwd)" % self.To,
                 "achieved": bytes_step / sec / 1e9, "peak": hbm, "unit": "GB/s", "frac": bytes_step / sec / 1e9 / hbm,
-                "traffic": _traffic("tacotron_step_dram_bytes"),
                 "algorithmic_bytes_per_step": bytes_step,
-                "peak_source": ("MEASURED_PEAKS.json" if pk else "fallback") + " hbm_gbs; weights are L2-resident in practice, so this is the floor "
+                "peak_source": ("MEASURED_PEAKS.json" if pk else "H100 SXM data sheet") + " hbm_gbs; weights are L2-resident in practice, so this is the floor "
                                "set by re-streaming them once per decoder step (SURVEY §8d), not a DRAM-traffic claim",
                 "step": {"algorithmic_tflop": flops / 1e12, "tflops": flops / sec / 1e12,
-                         "frac_of_sustained_bf16": flops / sec / 1e12 / float(pk.get("bf16_tflops_sustained", 1400.0))}}
+                         "frac_of_sustained_bf16": flops / sec / 1e12 / float(pk.get("bf16_tflops_sustained", 989.0))}}
 
     def cpu_reference(self, steps, warmup):
         import torch
@@ -391,6 +394,19 @@ class TacotronWorkload(object):
                     B, self.To, self.Ti, len(times), nthreads, ncores)}
 
 
+DUMP_SAMPLE = 1 << 22      # elements kept per dumped array (16 MB of float32)
+
+
+def _flat_sample(tensors):
+    """the variables (name -> CPU tensor, in the model's fixed order) concatenated and flattened, as float32; arrays longer than
+    DUMP_SAMPLE are cut to a fixed, seeded sample of positions so that runs stay comparable element for element"""
+    import numpy as np
+    flat = np.concatenate([t.reshape(-1).numpy().astype(np.float32) for t in tensors.values()])
+    if flat.size > DUMP_SAMPLE:
+        flat = flat[np.sort(np.random.default_rng(0).choice(flat.size, DUMP_SAMPLE, replace=False))]
+    return flat
+
+
 def make_workload(name):
     return TacotronWorkload() if name == "tacotron" else WaveNetWorkload(name)
 
@@ -405,6 +421,8 @@ def main():
     ap.add_argument("--workload", default="wavenet_ce", choices=["wavenet_ce", "wavenet_mol", "wavenet_default", "tacotron"])
     ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly instead of replaying a CUDA graph")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the bounded oracle timing on rank 0")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed (losses, gradients, updated variables) as DIR/<name>.npy")
     args = ap.parse_args()
     heavy = args.workload != "wavenet_ce"
     steps = args.steps if args.steps is not None else (20 if heavy else 200)
@@ -464,6 +482,11 @@ def main():
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         results[mode] = t.item()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in wl.outputs().items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
     loss = wl.loss()
     ms_per_step = results["resident"] / steps
     roof = wl.roofline(ms_per_step)
@@ -480,29 +503,10 @@ def main():
                 "e2e": {"value": total_units / (results["e2e"] * 1e-3), "unit": wl.unit, "h2d_bytes_per_step": wl.h2d_bytes(),
                         "d2h_bytes_per_step": wl.d2h_bytes, "ms_per_step": results["e2e"] / steps},
                 "gpu_launches": wl.launches_per_step() * steps,
-                "parity": _parity_record(wl.name),
                 "roofline": roof, "cpu_baseline": cpu}
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
-
-
-def _parity_record(name):
-    """bf16-mode deviation from the fp32 oracle at this workload's shape, from the committed measurement of the GPU parity tests
-    (profiles/r02_measured_parity.jsonl; tests/test_parity_full_gpu.py)"""
-    key = {"wavenet_ce": "wavenet_cfg2_24L_2x7680_ce_dropout", "wavenet_mol": "wavenet_cfg4_24L_2x4096_mol",
-           "wavenet_default": "wavenet_small_mulaw-quantize_L4_R128_B2xT512", "tacotron": "tacotron_cfg3_fullwidth_B32_Tin160_Tout200_stochastic"}[name]
-    try:
-        for ln in open(os.path.join(ROOT, "profiles", "r02_measured_parity.jsonl")):
-            d = json.loads(ln)
-            if d.get("test") == key:
-                keep = ("loss_abs_err", "logits_max_err", "logits_mean_err", "mel_l1", "dec_l1", "align_max_err", "loss_before_err", "loss_after_err")
-                out = {"mode": "bf16 operands + bf16-stored activations, fp32 accumulate; oracle fp32", "measured_at": key}
-                out.update({k: d[k] for k in keep if k in d})
-                return out
-    except Exception:
-        pass
-    return None
 
 
 if __name__ == "__main__":

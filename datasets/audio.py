@@ -1,5 +1,5 @@
 """Drop-in for the reference's datasets/audio.py: same free functions taking (array, hparams), numpy in / numpy out,
-computed by the sm_100a kernels of libt2b200.so (host<->device copies inside each call). No CPU fallback: without
+computed by the sm_90a kernels of libt2b200.so (host<->device copies inside each call). No CPU fallback: without
 a CUDA device or the built library these functions raise.
 
 Covered (reference datasets/audio.py line numbers): preemphasis :22-25, get_hop_size :54-59, linearspectrogram

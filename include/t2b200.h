@@ -1,4 +1,4 @@
-/* t2b200.h — C-ABI of libt2b200.so, the sm_100a compute library behind the Tacotron-2 hot paths.
+/* t2b200.h — C-ABI of libt2b200.so, the sm_90a compute library behind the Tacotron-2 hot paths.
  *
  * The reference (Rayhane-mamah/Tacotron-2) has NO FFI / plugin boundary: its hot paths are Python methods
  * that build TensorFlow-1 graph nodes. This header therefore DEFINES the boundary; each entry point names the
@@ -39,7 +39,7 @@ int t2_struct_size(const char* name);
 long long t2_launch_count(void);
 
 /* ---- engine-level test hooks (tests/test_gemm_engine.py) --------------------------------------------- */
-/* bf16 dilated-conv-as-GEMM on the tcgen05 engine: out[b,t,n] = act(sum_s sum_k a[b,t+shift_s,k] w[n,s*Kp+k] + bias[n])
+/* bf16 dilated-conv-as-GEMM on the wgmma engine: out[b,t,n] = act(sum_s sum_k a[b,t+shift_s,k] w[n,s*Kp+k] + bias[n])
  * (Kp = C rounded up to 64). Replaces tf.layers.Conv1D as used by wavenet_vocoder/models/modules.py:206-224,320. */
 int t2_dbg_conv_gemm(const void* d_a, int B, int T, int C, int ld, const int* shifts, int nshift,
                      const void* d_w, int N, int BN, const float* d_bias, int relu, void* d_out_bf16,

@@ -1,4 +1,4 @@
-"""tacotron-2_b200 — B200-native compute library behind the Tacotron-2 hot paths.
+"""tacotron-2_b200 — H100-native compute library behind the Tacotron-2 hot paths.
 
 The directory name is not a Python identifier; import it through ``t2_import.py`` at the repo root
 (``from t2_import import t2``), which registers this package as ``tacotron2_b200``.

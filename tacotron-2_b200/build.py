@@ -1,7 +1,7 @@
-"""Builds libt2b200.so (hand-written sm_100a CUDA + the C-ABI) in-tree with nvcc.
+"""Builds libt2b200.so (hand-written sm_90a CUDA + the C-ABI) in-tree with nvcc.
 
 The library is plain CUDA C++ with an ``extern "C"`` surface (include/t2b200.h); it links only against the
-CUDA runtime, so it cross-compiles on a GPU-less box and travels to the B200 box inside the repo snapshot.
+CUDA runtime, so it cross-compiles on a machine without a GPU.
 """
 import hashlib
 import os
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libt2b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
           "-Xptxas", "-v"] + ARCH
 

@@ -7,7 +7,7 @@
 // Dataflow (rows = b * T + t, batch-major; N = B * T):
 //   mel_outputs fp32 [N][M] -> bf16
 //   conv bank: k = 1..K convolutions M -> CC ('same' padding, the extra pad of an even kernel on the right) + bias + ReLU, each one a
-//     tap-shifted GEMM on the tcgen05 engine writing its 128-column slice of Y [N][K*CC]; every layer's batch norm runs on its slice
+//     tap-shifted GEMM on the wgmma engine writing its 128-column slice of Y [N][K*CC]; every layer's batch norm runs on its slice
 //   max-pool (2, stride 1, 'same': max(x[t], x[t+1]))
 //   proj1 (k = 3, K*CC -> PJ, ReLU, BN), proj2 (k = 3, PJ -> M, linear, BN), + mel_outputs, dense M -> HU
 //   NH highway layers: one GEMM with N = 2 HU ([H | T] pre-activations) + an elementwise kernel
@@ -654,7 +654,7 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_bwd_kernel(GruBwdArgs a) {
 // ------------------------------------------------------------------------------------------------------
 // host helpers
 // ------------------------------------------------------------------------------------------------------
-// out[pos][n] = act(sum_taps sum_k a[pos + shift][k0 + k] w[n][tap * Cp + k] + bias[n]) on the tcgen05 engine (EPI_BIAS_ACT)
+// out[pos][n] = act(sum_taps sum_k a[pos + shift][k0 + k] w[n][tap * Cp + k] + bias[n]) on the wgmma engine (EPI_BIAS_ACT)
 int gemm(const void* a, int C, int ld, int k0, long long T, int Bn, const void* w, int wN, int wK, int ntaps, const int* shifts, int BN,
          const float* bias, int act, void* out_bf16, float* out_f32, int ldo, int nvalid, cudaStream_t st, const int* k0s = nullptr, int Ctot = 0) {
   ActGemmCall g;

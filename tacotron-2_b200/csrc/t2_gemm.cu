@@ -1,4 +1,4 @@
-// t2_gemm.cu — host side of the tcgen05 GEMM engine: TMA tensor-map encoding and kernel launches.
+// t2_gemm.cu — host side of the wgmma GEMM engine: TMA tensor-map encoding and kernel launches.
 #include <stdlib.h>
 #include <mutex>
 
@@ -49,7 +49,7 @@ static int encode_act_map(CUtensorMap* m, const ActT& a, int box_rows) {
   return T2_OK;
 }
 
-// 3-D map over a channels-last bf16 OUTPUT tensor [B][T][C] for the epilogue's TMA stores: box 64 columns x 32 rows (one TMEM lane
+// 3-D map over a channels-last bf16 OUTPUT tensor [B][T][C] for the epilogue's TMA stores: box 64 columns x 32 rows (one epilogue row
 // quarter), 128-byte swizzle; rows >= T of an item and columns >= C are clipped by the hardware.
 static int encode_out_map(CUtensorMap* m, const void* ptr, int C, int T, int B) {
   EncodeTiledFn fn = get_encode_fn();
@@ -93,8 +93,7 @@ bool pdl_enabled() {
   return v != 0;
 }
 
-// cluster size along M for the weight-tile multicast (T2_CLUSTER in the environment; default 1 = off: measured on B200 the
-// per-layer GEMMs are bound by bytes in flight per SM, not by L2 reads - 2.51 / 2.57 / 2.58 / 2.68 ms per step at 1 / 2 / 4 / 8)
+// cluster size along M for the weight-tile multicast (T2_CLUSTER in the environment; default 1 = off)
 int cluster_pref() {
   static int v = -1;
   if (v < 0) {
@@ -111,16 +110,15 @@ static int pick_cluster(int BN, const dim3& grid) {
   return cs;
 }
 
-template <int EPI, int BN, int NT = 1>
+template <int EPI, int BN>
 static int launch_one(const GemmArgs& g, dim3 grid, int cs, cudaStream_t stream) {
   using Cfg = ActGemmCfg<BN>;
   static bool configured = false;
   if (!configured) {
-    T2_CHECK_CUDA(cudaFuncSetAttribute(act_gemm_kernel<EPI, BN, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    T2_CHECK_CUDA(cudaFuncSetAttribute(act_gemm_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        Cfg::kSmemBytes));
     configured = true;
   }
-  grid.y = (grid.y + NT - 1) / NT;
   // every launch gets its own slice of the timing buffer (so a captured graph stamps each of its kernel nodes separately)
   if (g.dbg) g_timing_buffer = g.dbg + size_t(grid.x) * grid.y * grid.z * kDbgSlots;
   cudaLaunchConfig_t cfg;
@@ -139,36 +137,7 @@ static int launch_one(const GemmArgs& g, dim3 grid, int cs, cudaStream_t stream)
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  T2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, act_gemm_kernel<EPI, BN, NT>, g));
-  t2_count_launch();
-  return T2_OK;
-}
-
-// CTA-pair kernels (tcgen05 cta_group::2): T2_PAIR=0 in the environment keeps the single-CTA kernels
-bool pair_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("T2_PAIR"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v != 0;
-}
-
-template <int EPI, int BN, int NT = 1>
-static int launch_pair(const GemmArgs& g, dim3 grid, cudaStream_t stream) {
-  using Cfg = ActGemm2Cfg<BN>;
-  static bool configured = false;
-  if (!configured) {
-    T2_CHECK_CUDA(cudaFuncSetAttribute(act_gemm2_kernel<EPI, BN, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    configured = true;
-  }
-  grid.y = (grid.y + NT - 1) / NT;
-  if (g.dbg) g_timing_buffer = g.dbg + size_t(grid.x) * grid.y * grid.z * kDbgSlots;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid; cfg.blockDim = dim3(kActGemmThreads); cfg.dynamicSmemBytes = Cfg::kSmemBytes; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;       // the cluster shape (2,1,1) is compiled into the kernel
-  T2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, act_gemm2_kernel<EPI, BN, NT>, g));
+  T2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, act_gemm_kernel<EPI, BN>, g));
   t2_count_launch();
   return T2_OK;
 }
@@ -183,11 +152,9 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) 
     if (rc) return rc;
   }
   dim3 grid((c.T + kBM - 1) / kBM * c.B, c.n_tiles, c.ksplit > 1 ? c.ksplit : 1);
-  // CTA pairs when the M tiles pair up (even count, no split-K) and the tile is wide enough for a half to be a whole swizzle atom
-  const bool pair = pair_enabled() && BN >= 128 && grid.x % 2 == 0 && grid.z == 1;
-  const int cs = pair ? 1 : pick_cluster(BN, grid);
-  // weight-tile rows one TMA box fetches: half a tile per CTA of a pair, 1/cs per CTA of a multicast cluster
-  int rc = encode_wt_map(&g.bmap, c.w, c.wN, c.wK, c.wL, pair ? BN / 2 : BN / cs);
+  const int cs = pick_cluster(BN, grid);
+  // weight-tile rows one TMA box fetches: 1/cs of the tile per CTA of a multicast cluster
+  int rc = encode_wt_map(&g.bmap, c.w, c.wN, c.wK, c.wL, BN / cs);
   if (rc) return rc;
   int ktot = 0;
   for (int s = 0; s < c.nseg; ++s) {
@@ -224,9 +191,7 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) 
                "act_gemm: split-K needs an atomically accumulating epilogue and at least one k-block per slice");
   }
 #define T2_CASE(E, N) \
-  if (epi == E && BN == N) return pair ? launch_pair<E, N>(g, grid, stream) : launch_one<E, N>(g, grid, cs, stream);
-  if (epi == EPI_GATE && BN == 256 && c.n_tiles % 2 == 0)
-    return pair ? launch_pair<EPI_GATE, 256, 2>(g, grid, stream) : launch_one<EPI_GATE, 256, 2>(g, grid, cs, stream);
+  if (epi == E && BN == N) return launch_one<E, N>(g, grid, cs, stream);
   T2_CASE(EPI_GATE, 256)
   T2_CASE(EPI_RES, 128)
   T2_CASE(EPI_RES, 256)
@@ -239,9 +204,6 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) 
   T2_CASE(EPI_GATE_BWD, 256)
   T2_CASE(EPI_DX, 128)
   T2_CASE(EPI_DX, 256)
-#undef T2_CASE
-#define T2_CASE(E, N) \
-  if (epi == E && BN == N) return launch_one<E, N>(g, grid, cs, stream);
   T2_CASE(EPI_MOL, 32)
   T2_CASE(EPI_LSTM, 32)
   T2_CASE(EPI_TOUT, 32)

@@ -1,15 +1,15 @@
-// t2_gemm.cuh — the tcgen05 GEMM engine all dense contractions of the WaveNet / Tacotron paths run on.
+// t2_gemm.cuh — the wgmma GEMM engine all dense contractions of the WaveNet / Tacotron paths run on.
 //
 //   act_gemm  : D[128 positions, BN] = sum over K-segments A_seg[pos + shift, k] * W[n, k]
 //               A = channels-last bf16 activations [L, B, T, C] read by 4-D TMA (negative / past-the-end
 //               time coordinates are zero-filled by the TMA unit, which is exactly the causal left pad of
 //               wavenet_vocoder/models/modules.py:308-313), B = packed bf16 weights [N, Ktot] (K-major).
-//               fp32 accumulators live in TMEM; a fused epilogue (gate / residual / loss / ...) drains them.
+//               fp32 accumulators live in the registers of four consumer warpgroups; once the reduction is done they are
+//               written to a shared fp32 tile that a fused epilogue (gate / residual / loss / ...) drains, one thread per row.
 //   wgrad_gemm: dW[m, n] = sum over positions A[pos + sa, m] * B[pos + sb, n]; both operands are
-//               channels-last activations, i.e. MN-major UMMA operands, reduction over positions.
+//               channels-last activations, i.e. MN-major wgmma operands, reduction over positions.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (TMEM lane quarter = warp_id % 4).
+// Warp roles of act_gemm (544 threads): warps 0..15 = MMA + epilogue, warp 16 = TMA producer.
 #pragma once
 #include "t2_common.cuh"
 #include "t2_gemm_types.h"
@@ -47,12 +47,21 @@ __device__ __forceinline__ void store_f32x32(float* dst, const float (&v)[32]) {
 #pragma unroll
   for (int q = 0; q < 8; ++q) d[q] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
 }
-__device__ __forceinline__ void tmem_ld32f(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  tmem_ld32(taddr, r);
-  tmem_ld_wait();
+// One row of the shared fp32 accumulator tile [128][BN]: the 16-byte chunk c of row r is stored at chunk c ^ (r % 8), so that the
+// 8 rows a quarter-warp reads at the same column land in distinct banks. `row + n` addresses column n (a multiple of 4).
+struct AccRow {
+  const float* row;
+  int col;
+  int sw;
+  __device__ __forceinline__ AccRow operator+(int n) const { return AccRow{row, col + n, sw}; }
+};
+// 32 consecutive fp32 accumulator columns of this thread's row
+__device__ __forceinline__ void acc_ld32f(AccRow a, float (&v)[32]) {
 #pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
+  for (int q = 0; q < 8; ++q) {
+    const float4 f = *reinterpret_cast<const float4*>(a.row + ((((a.col >> 2) + q) ^ a.sw) << 2));
+    v[q * 4] = f.x; v[q * 4 + 1] = f.y; v[q * 4 + 2] = f.z; v[q * 4 + 3] = f.w;
+  }
 }
 
 // Split-bf16 ("fp32-class") mode: an fp32 value travels as hi = bf16(v) and lo = bf16(v - hi) in channels [0,C) and [C,2C) of a row
@@ -78,7 +87,7 @@ __device__ __forceinline__ void load_split32(const __nv_bfloat16* src_hi, const 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Epilogue staging: a thread owns one accumulator ROW (TMEM lane), but global memory wants a warp to touch one
+// Epilogue staging: a thread owns one accumulator ROW, but global memory wants a warp to touch one
 // row's contiguous bytes. Every epilogue therefore moves 32-row x 128-column bf16 tiles through a per-warp
 // shared-memory tile (the pipeline stages are free once the last MMA has committed): rows are written / read by
 // their owning lane, global traffic is issued with 16 lanes covering one 256-byte row segment.
@@ -88,31 +97,31 @@ constexpr int kTileBytes = 32 * kTilePitch;       // 8704
 constexpr int kEpiTilesPerWarp = 2;          // dedicated staging (not aliased with the pipeline stages)
 // TMA-store staging (EPI_GATE / EPI_RES / EPI_GATE_BWD / EPI_DX): a staged 32-row x 128-column bf16 tile is two 64-column boxes of
 // 32 rows x 128 bytes in the 128-byte swizzle (16-byte chunk index XOR row % 8) the output tensor maps are encoded with, so one
-// elected thread per lane quarter hands a finished tile to the TMA engine instead of 4 warps copying it out through registers.
+// elected thread per row quarter hands a finished tile to the TMA engine instead of 4 warps copying it out through registers.
 // Three tiles per quarter rotate: a tile is rewritten two stores after its own (see tile_store).
 constexpr int kSBoxBytes = 32 * 128;
 constexpr int kSTileBytes = 2 * kSBoxBytes;
 constexpr int kSTiles = 3;
-constexpr int kEpiWarpBytes = kSTiles * kSTileBytes;     // 24 KB per lane quarter (also covers the 2 x 8704-byte pitch-272 tiles)
+constexpr int kEpiWarpBytes = kSTiles * kSTileBytes;     // 24 KB per row quarter (also covers the 2 x 8704-byte pitch-272 tiles)
 static_assert(kEpiWarpBytes >= kEpiTilesPerWarp * kTileBytes && kEpiWarpBytes % 1024 == 0, "staging size / swizzle-atom alignment");
 
-constexpr int kActEpiWarps = 16;                               // 4 TMEM lane quarters x 4 column groups
-constexpr int kActGemmThreads = 64 + 32 * kActEpiWarps;        // + producer warp + MMA warp
+constexpr int kActEpiWarps = 16;                               // 4 row quarters x 4 column groups
+constexpr int kActGemmThreads = 32 * kActEpiWarps + 32;        // + producer warp
 
 struct EpiCtx {
   int n_tile, b, t, T;     // output column tile, batch item, this lane's time step, sequence length
   bool valid;              // t < T
   int lane;
   int cg;                  // column group 0..3: this warp owns columns [32*cg, 32*cg+32) of every 128-column group
-  int qbar;                // named barrier shared by the 4 warps of this TMEM lane quarter
+  int qbar;                // named barrier shared by the 4 warps of this row quarter
   size_t row0;             // b*T + (first time step of this warp)
   int nrows;               // valid rows among this warp's 32
-  uint32_t trow;           // TMEM address of this warp's lanes, column 0
-  uint8_t* wbuf;           // kEpiWarpBytes of shared memory shared by the 4 warps of this lane quarter
+  AccRow trow;             // this thread's row of the accumulator tile, column 0
+  uint8_t* wbuf;           // kEpiWarpBytes of shared memory shared by the 4 warps of this row quarter
   uint8_t* smem_all;       // start of the (free after the mainloop) pipeline shared memory, CTA-wide scratch
   int m_tile;              // index of this CTA's 128-row tile
   const CUtensorMap* omap; // output tensor maps (GemmArgs::omap) of the TMA-store epilogues
-  int tq;                  // first time step of this lane quarter (row coordinate of its stores)
+  int tq;                  // first time step of this row quarter (row coordinate of its stores)
   mutable int sk;          // stores issued so far by this quarter (tile rotation)
 };
 
@@ -314,8 +323,8 @@ struct Epilogue<EPI_GATE, 256> {
       float a[32], g[32], ba[32], bb[32];
       load_f32x32(bias + cb + cq * 32, ba);
       load_f32x32(bias + Gh + cb + cq * 32, bb);
-      tmem_ld32f(c.trow + cq * 32, a);
-      tmem_ld32f(c.trow + 128 + cq * 32, g);
+      acc_ld32f(c.trow + cq * 32, a);
+      acc_ld32f(c.trow + 128 + cq * 32, g);
 #pragma unroll
       for (int j = 0; j < 32; ++j) a[j] = tanhf_(a[j] + ba[j]) * sigmoidf_(g[j] + bb[j]);
       if (c.valid) {
@@ -329,8 +338,8 @@ struct Epilogue<EPI_GATE, 256> {
       float a[32], g[32], ba[32], bb[32];
       load_f32x32(bias + cb + cq * 32, ba);
       load_f32x32(bias + Gh + cb + cq * 32, bb);
-      tmem_ld32f(c.trow + cq * 32, a);
-      tmem_ld32f(c.trow + 128 + cq * 32, g);
+      acc_ld32f(c.trow + cq * 32, a);
+      acc_ld32f(c.trow + 128 + cq * 32, g);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         a[j] = tanh_approx_(a[j] + ba[j]);
@@ -386,7 +395,7 @@ struct Epilogue<EPI_RES, BN> {
         const int j0 = gq * 128 + c.cg * 32;
         float acc[32], x[32], bv[32];
         load_f32x32(bias + j0, bv);
-        tmem_ld32f(c.trow + j0, acc);
+        acc_ld32f(c.trow + j0, acc);
         if (c.valid) {
           load_split32(x_in + r2 + j0, x_in + r2 + R + j0, x);
 #pragma unroll
@@ -410,7 +419,7 @@ struct Epilogue<EPI_RES, BN> {
       const int j0 = gq * 128 + cq * 32;
       float acc[32], x[32], bv[32];
       load_f32x32(bias + j0, bv);
-      tmem_ld32f(c.trow + j0, acc);
+      acc_ld32f(c.trow + j0, acc);
       stage_get_sw(tile, c.lane, cq, x);
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = (acc[j] + bv[j] + x[j]) * rs;
@@ -453,7 +462,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
         const int c0 = c.n_tile * BN + gq * 128 + c.cg * 32;
         if (c0 >= nvalid) continue;
         float acc[32];
-        tmem_ld32f(c.trow + gq * 128 + c.cg * 32, acc);
+        acc_ld32f(c.trow + gq * 128 + c.cg * 32, acc);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           float v = acc[j];
@@ -484,7 +493,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
         const int cq = c.cg;
         const int c0 = g0 + cq * 32;
         float acc[32];
-        if (c0 < nvalid) tmem_ld32f(c.trow + gq * 128 + cq * 32, acc);
+        if (c0 < nvalid) acc_ld32f(c.trow + gq * 128 + cq * 32, acc);
         else {
 #pragma unroll
           for (int j = 0; j < 32; ++j) acc[j] = 0.f;
@@ -520,7 +529,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
 template <>
 struct Epilogue<EPI_CE, 256> {
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
-    if (c.cg != 0) return;  // row-wise softmax: one warp per lane quarter walks all 256 columns
+    if (c.cg != 0) return;  // row-wise softmax: one warp per row quarter walks all 256 columns
     const int* tgt = static_cast<const int*>(e.ptr[0]);
     const int* len = static_cast<const int*>(e.ptr[1]);
     const float* bias = static_cast<const float*>(e.ptr[2]);
@@ -534,7 +543,7 @@ struct Epilogue<EPI_CE, 256> {
 #pragma unroll 1
     for (int j0 = 0; j0 < 256; j0 += 32) {
       float v[32];
-      tmem_ld32f(c.trow + j0, v);
+      acc_ld32f(c.trow + j0, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         v[j] += __ldg(bias + j0 + j);
@@ -547,7 +556,7 @@ struct Epilogue<EPI_CE, 256> {
 #pragma unroll 1
     for (int j0 = 0; j0 < 256; j0 += 32) {
       float v[32];
-      tmem_ld32f(c.trow + j0, v);
+      acc_ld32f(c.trow + j0, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) se += __expf(v[j] + __ldg(bias + j0 + j) - mx);
     }
@@ -564,7 +573,7 @@ struct Epilogue<EPI_CE, 256> {
         for (int cq = 0; cq < 4; ++cq) {
           const int j0 = gq * 128 + cq * 32;
           float v[32], lo[32];
-          tmem_ld32f(c.trow + j0, v);
+          acc_ld32f(c.trow + j0, v);
 #pragma unroll
           for (int j = 0; j < 32; ++j) {
             const float pj = __expf(v[j] + __ldg(bias + j0 + j) - mx) * inv;
@@ -614,7 +623,7 @@ struct Epilogue<EPI_MOL, 32> {
     const bool w = c.valid && (c.t + 1 < c.T) && (c.t + 1 < __ldg(len + c.b));
     const float y = w ? __ldg(tgt + size_t(c.b) * c.T + c.t + 1) : 0.f;
     float v[32];
-    tmem_ld32f(c.trow, v);
+    acc_ld32f(c.trow, v);
     if (e.i[2] != 0) {   // ---- single Gaussian ----
       const float lsg = e.f[3];
       const float m = v[0] + __ldg(bias), sraw = v[1] + __ldg(bias + 1);
@@ -739,7 +748,7 @@ struct Epilogue<EPI_MOL, 32> {
 
 // backward through ReLU: out = acc * scale * (h > 0).
 // ptr: 0 out bf16 [pos, ldo], 1 h bf16 [pos, ldo], 2 device scalar fp32* (nullable; multiplies 1/x),
-//      3 fp32 [ldo] column sums of `out` accumulated with atomics (nullable: bias gradient);  f0 const scale; i0 = ldo
+//      3 int64 fixed-point [ldo] column sums of `out` (fx_add; nullable: bias gradient);  f0 const scale; i0 = ldo
 template <int BN>
 struct Epilogue<EPI_SCALE_RELUMASK, BN> {
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
@@ -760,7 +769,7 @@ struct Epilogue<EPI_SCALE_RELUMASK, BN> {
       uint8_t* tile = c.wbuf + gq * kTileBytes;
       const int cq = c.cg;
       float acc[32], hv[32];
-      tmem_ld32f(c.trow + gq * 128 + cq * 32, acc);
+      acc_ld32f(c.trow + gq * 128 + cq * 32, acc);
       stage_get(tile, c.lane, cq, hv);
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = hv[j] > 0.f ? acc[j] * s : 0.f;
@@ -768,14 +777,14 @@ struct Epilogue<EPI_SCALE_RELUMASK, BN> {
       tile_flush<4>(tile, out + off, ldo, c.nrows, c);
       if (e.ptr[3]) {
         const float cs = warp_colsum32(acc, c.lane);
-        atomicAdd(static_cast<float*>(e.ptr[3]) + c.n_tile * BN + gq * 128 + cq * 32 + colsum32_col(c.lane), cs);
+        fx_add(static_cast<long long*>(e.ptr[3]) + c.n_tile * BN + gq * 128 + cq * 32 + colsum32_col(c.lane), cs);
       }
     }
   }
 };
 
-// backward of the gate: dz -> (da, db).  ptr: 0 ta, 1 sb (bf16 [pos,Gh]), 2 dg out (bf16 [pos,2Gh]), 3 / 4 fp32 [2Gh]
-// gate-bias gradients (column sums of dg, atomics; nullable — dilated-conv bias and cin-conv bias get the same sum); i0 = Gh
+// backward of the gate: dz -> (da, db).  ptr: 0 ta, 1 sb (bf16 [pos,Gh]), 2 dg out (bf16 [pos,2Gh]), 3 / 4 int64 fixed-point [2Gh]
+// gate-bias gradients (column sums of dg, fx_add; nullable — dilated-conv bias and cin-conv bias get the same sum); i0 = Gh
 template <int BN>
 struct Epilogue<EPI_GATE_BWD, BN> {
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
@@ -802,7 +811,7 @@ struct Epilogue<EPI_GATE_BWD, BN> {
       }
       stage_get_sw(t0, c.lane, cq, a);
       stage_get_sw(t1, c.lane, cq, s);
-      tmem_ld32f(c.trow + gq * 128 + cq * 32, dz);
+      acc_ld32f(c.trow + gq * 128 + cq * 32, dz);
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const float da = dz[j] * (1.f - a[j] * a[j]) * s[j];
@@ -817,11 +826,11 @@ struct Epilogue<EPI_GATE_BWD, BN> {
       if (e.ptr[3]) {
         const float ca = warp_colsum32(a, c.lane), cb2 = warp_colsum32(s, c.lane);
         const int col = cb + cq * 32 + colsum32_col(c.lane);
-        atomicAdd(static_cast<float*>(e.ptr[3]) + col, ca);
-        atomicAdd(static_cast<float*>(e.ptr[3]) + Gh + col, cb2);
+        fx_add(static_cast<long long*>(e.ptr[3]) + col, ca);
+        fx_add(static_cast<long long*>(e.ptr[3]) + Gh + col, cb2);
         if (e.ptr[4]) {
-          atomicAdd(static_cast<float*>(e.ptr[4]) + col, ca);
-          atomicAdd(static_cast<float*>(e.ptr[4]) + Gh + col, cb2);
+          fx_add(static_cast<long long*>(e.ptr[4]) + col, ca);
+          fx_add(static_cast<long long*>(e.ptr[4]) + Gh + col, cb2);
         }
       }
     }
@@ -829,7 +838,7 @@ struct Epilogue<EPI_GATE_BWD, BN> {
 };
 
 // gradient wrt the block input: dx = dropout_mask/keep * acc + res_scale * dx_out
-// ptr: 0 dxo bf16 [pos,R] (nullable), 1 dx_out bf16 [pos,R], 2 fp32 [R] += f2 * column sums of dx_out (nullable: bias
+// ptr: 0 dxo bf16 [pos,R] (nullable), 1 dx_out bf16 [pos,R], 2 int64 fixed-point [R] += f2 * column sums of dx_out (nullable: bias
 // gradient of the 1x1 that produced this layer's input), 7 device u64 seed offset (nullable);
 // f0 res_scale, f1 dropout p, f2 bias-gradient scale; i1 = layer
 template <int BN>
@@ -855,7 +864,7 @@ struct Epilogue<EPI_DX, BN> {
       const int cq = c.cg;
       const int j0 = gq * 128 + cq * 32;
       float acc[32], g[32];
-      tmem_ld32f(c.trow + j0, acc);
+      acc_ld32f(c.trow + j0, acc);
       if (p > 0.f) {
         const uint32_t thr = uint32_t(p * 65536.f);
 #pragma unroll
@@ -874,7 +883,7 @@ struct Epilogue<EPI_DX, BN> {
       tile_store(tile, c.omap + 0, gq * 128, c);
       if (e.ptr[2]) {
         const float cs = warp_colsum32(acc, c.lane);
-        atomicAdd(static_cast<float*>(e.ptr[2]) + j0 + colsum32_col(c.lane), cs * e.f[2]);
+        fx_add(static_cast<long long*>(e.ptr[2]) + j0 + colsum32_col(c.lane), cs * e.f[2]);
       }
     }
   }
@@ -898,7 +907,7 @@ struct Epilogue<EPI_LSTM, 32> {
     const int q = c.qbar - 1;
     if (c.cg == 0) {
       float v[32];
-      tmem_ld32f(c.trow, v);
+      acc_ld32f(c.trow, v);
 #pragma unroll
       for (int j = 0; j < 32; ++j) ex[(q * 32 + c.lane) * 33 + j] = v[j];
     }
@@ -971,7 +980,7 @@ struct Epilogue<EPI_TOUT, 32> {
     if (c.cg != 0) return;
     const int k = c.t, nb = e.i[6];
     float v[32];
-    tmem_ld32f(c.trow, v);
+    acc_ld32f(c.trow, v);
     float* dst; int ld, acc, kk;
     if (k < e.i[0]) { dst = static_cast<float*>(e.ptr[0]); ld = e.i[1]; acc = e.i[2]; kk = k; }
     else if (k < e.i[3]) { dst = static_cast<float*>(e.ptr[1]); ld = e.i[4]; acc = e.i[5]; kk = k - e.i[0]; }
@@ -991,38 +1000,36 @@ struct Epilogue<EPI_TOUT, 32> {
 
 // ------------------------------------------------------------------------------------------------
 // act_gemm kernel
+//   Consumer warpgroup w (warps 4w..4w+3) computes rows [64 (w >> 1), +64) x columns [BN/2 (w & 1), +BN/2) of the tile with
+//   wgmma, its accumulators in registers. When the reduction is complete the four warpgroups write them to a shared fp32
+//   tile that aliases the (then idle) pipeline stages, and the same 16 warps run the epilogue on it: warp e owns rows
+//   [32 (e % 4), +32) (one per lane) and column group e / 4.
 // ------------------------------------------------------------------------------------------------
 template <int BN>
 struct ActGemmCfg {
   static constexpr int kABytes = kBM * kBK * 2;   // 16 KB
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // latency-bound pipelines: ~2.3k cycles TMA round trip / stages = cycles per k-block; the narrow swapped GEMMs of the
-  // recurrences (BN = 32, 20 KB stages) take 6 stages
-  // (BN = 256 outside a CTA pair - odd tile counts, T2_PAIR=0 - is a fallback: the 96 KB of store staging leave room for 2 stages)
-#ifndef T2_STAGES_256
-#define T2_STAGES_256 2
-#endif
-  static constexpr int kStages = (BN >= 256) ? T2_STAGES_256 : (BN <= 32 ? 6 : 4);
-  static constexpr int kStagingBytes = 4 * kEpiWarpBytes;      // 4 lane quarters x 3 store tiles, never aliased with the stages
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 /*align*/ + 256 /*barriers*/;
-  static_assert(kSmemBytes <= 232448, "shared memory budget");
+  static constexpr int kAccBytes = kBM * BN * 4;
+  static constexpr int kStagingBytes = 4 * kEpiWarpBytes;      // 4 row quarters x 3 store tiles, never aliased with the stages
+  static constexpr int kPipeBudget = 232448 - kStagingBytes - 1024 /*align*/ - 256 /*barriers*/;
+  // as many stages as fit next to the store staging (2 at BN = 256, 4 at 128, 6 for the narrow swapped GEMMs of the recurrences)
+  static constexpr int kStages = kPipeBudget / kStageBytes > 6 ? 6 : kPipeBudget / kStageBytes;
+  static constexpr int kPipeBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
+  static constexpr int kSmemBytes = kPipeBytes + kStagingBytes + 1024 + 256;
+  static_assert(kStages >= 2 && kPipeBytes <= kPipeBudget, "shared memory budget");
 };
 
-// NT = output column tiles processed by one CTA, each with its own TMEM accumulator: the epilogue of tile h overlaps
-// the MMAs of tile h+1 (used by the gate GEMM: 2 x 256 columns per CTA -> 120 CTAs, one wave, instead of 240)
-template <int EPI, int BN, int NT>
+template <int EPI, int BN>
 __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __grid_constant__ GemmArgs g) {
   using Cfg = ActGemmCfg<BN>;
+  constexpr int WN = BN / 2;          // columns per consumer warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + Cfg::kStages * Cfg::kStageBytes;
+  float* acc_s = reinterpret_cast<float*>(smem);
+  uint8_t* staging = smem + Cfg::kPipeBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;      // [NT]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + NT);
-  constexpr int kTmemCols = (NT * BN) < 32 ? 32 : NT * BN;
-  static_assert(kTmemCols <= 512 && (kTmemCols & (kTmemCols - 1)) == 0, "TMEM columns");
 
   const int warp = threadIdx.x >> 5;
   const int m_tile = blockIdx.x;
@@ -1042,97 +1049,57 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
   const int kb_lo = int((long long)all_kb * blockIdx.z / gridDim.z), kb_hi = int((long long)all_kb * (blockIdx.z + 1) / gridDim.z);
   const int total_kb = kb_hi - kb_lo;
 
-  if (warp == 0 && elect_one()) {
+  if (warp == kActEpiWarps && elect_one()) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&g.amap[i]);
     tma_prefetch_desc(&g.bmap);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int i = 0; i < Cfg::kStages; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], cs);     // a stage is free once EVERY CTA of the cluster has consumed it (peers multicast into it)
-      }
-      for (int i = 0; i < NT; ++i) mbar_init(&tmem_full[i], 1);
-      fence_barrier_init();
+    for (int i = 0; i < Cfg::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      // a stage is free once every consumer warp of EVERY CTA of the cluster has consumed it (peers multicast into it)
+      mbar_init(&empty_bar[i], kActEpiWarps * cs);
     }
-    __syncwarp();
-    tmem_alloc<kTmemCols>(tmem_slot);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   if (cs > 1) cluster_sync_all();      // peers' barriers are initialised before any remote arrive / multicast write
-  const uint32_t tmem_base = *tmem_slot;
   // everything above is CTA-local set-up and overlaps the previous kernel's tail under PDL; global memory from here on
   pdl_wait();
   pdl_launch_dependents();
   if (dbg && threadIdx.x == 0) { dbg[1] = clock64(); dbg[9] = globaltimer_ns(); }
 
-  if (warp == 0) {
+  if (warp == kActEpiWarps) {
     if (elect_one()) {
+      const int n_tile = blockIdx.y;
       int stage = 0;
       uint32_t phase = 0;
-      for (int h = 0; h < NT; ++h) {
-        const int n_tile = blockIdx.y * NT + h;
-        int kb_global = 0;
-        for (int s = 0; s < g.nseg; ++s) {
-          const Seg sg = g.seg[s];
-          for (int l = 0; l < sg.nlayers; ++l) {
-            for (int kb = 0; kb < sg.nkb; ++kb, ++kb_global) {
-              if (kb_global < kb_lo || kb_global >= kb_hi) continue;
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-              uint8_t* sa = smem + stage * Cfg::kStageBytes;
-              uint8_t* sb = sa + Cfg::kABytes;
-              tma_load_4d(sa, &g.amap[sg.map], &full_bar[stage], sg.k0 + kb * kBK, t0 + sg.shift, b,
-                          sg.layer0 + l);
-              if (cs == 1) {
-                tma_load_3d(sb, &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK, n_tile * BN, g.b_layer);
-              } else {
-                const int rows = BN / int(cs);     // this CTA's slice of the weight tile (whole 8-row swizzle atoms: 1024-byte aligned)
-                tma_load_3d_mc(sb + crank * rows * (kBK * 2), &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK,
-                               n_tile * BN + int(crank) * rows, g.b_layer, cmask);
-              }
-              if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      int kb_global = 0;
+      for (int s = 0; s < g.nseg; ++s) {
+        const Seg sg = g.seg[s];
+        for (int l = 0; l < sg.nlayers; ++l) {
+          for (int kb = 0; kb < sg.nkb; ++kb, ++kb_global) {
+            if (kb_global < kb_lo || kb_global >= kb_hi) continue;
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+            uint8_t* sa = smem + stage * Cfg::kStageBytes;
+            uint8_t* sb = sa + Cfg::kABytes;
+            tma_load_4d(sa, &g.amap[sg.map], &full_bar[stage], sg.k0 + kb * kBK, t0 + sg.shift, b, sg.layer0 + l);
+            if (cs == 1) {
+              tma_load_3d(sb, &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK, n_tile * BN, g.b_layer);
+            } else {
+              const int rows = BN / int(cs);     // this CTA's slice of the weight tile (whole 8-row swizzle atoms: 1024-byte aligned)
+              tma_load_3d_mc(sb + crank * rows * (kBK * 2), &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK,
+                             n_tile * BN + int(crank) * rows, g.b_layer, cmask);
             }
+            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(kBM, BN < 16 ? 16 : BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int h = 0; h < NT; ++h) {
-        const uint32_t tmem_d = tmem_base + uint32_t(h * BN);
-        for (int kb = 0; kb < total_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (dbg && kb == 0 && h == 0) dbg[2] = clock64();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
-          const uint64_t adesc = make_sdesc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advancing K by 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr>>4) field
-            umma_f16(tmem_d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), idesc,
-                     (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          if (cs == 1) umma_commit(&empty_bar[stage]);
-          else umma_commit_mc(&empty_bar[stage], cmask);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        if (dbg && h == NT - 1) dbg[3] = clock64();
-        umma_commit(&tmem_full[h]);
       }
     }
   } else {
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
+    const int q = warp & 3;  // row quarter of this warp in the epilogue
+    const int lane = threadIdx.x & 31;
     EpiCtx c;
-    c.lane = threadIdx.x & 31;
-    c.cg = (warp - 2) >> 2;
+    c.lane = lane;
+    c.cg = warp >> 2;
     c.qbar = 1 + q;
     c.b = b; c.T = g.T;
     const int tw = t0 + q * 32;          // first time step of this warp
@@ -1144,228 +1111,157 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
     c.smem_all = staging;
     c.m_tile = m_tile;
     c.omap = g.omap; c.tq = tw; c.sk = 0;
-    if constexpr (EpiHasPrefetch<EPI>::value && NT == 1) {
-      c.n_tile = blockIdx.y;
-      Epilogue<EPI, BN>::prefetch(g.epi, c);
+    c.n_tile = blockIdx.y;
+    if constexpr (EpiHasPrefetch<EPI>::value) Epilogue<EPI, BN>::prefetch(g.epi, c);
+
+    // ---- mainloop: this warpgroup's 64 x WN quarter of the tile
+    const int wg = warp >> 2, mh = wg >> 1, nh = wg & 1;
+    float d[WN / 2];
+#pragma unroll
+    for (int i = 0; i < WN / 2; ++i) d[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < total_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      __syncwarp();                    // wgmma is warp-aligned: reconverge after the spin-wait
+      if (dbg && kb == 0 && threadIdx.x == 0) dbg[2] = clock64();
+      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + uint32_t(mh * 64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes) + uint32_t(nh * WN * 128);
+      const uint64_t adesc = make_gdesc_sw128(sa, 16, 1024);
+      const uint64_t bdesc = make_gdesc_sw128(sb, 16, 1024);
+      wgmma_fence();
+      wgmma_fence_regs(d);
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k)
+        // advancing K by 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr>>4) field
+        Wgmma<WN, 0, 0>::mma(d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_fence_regs(d);
+      // the previous k-block's MMAs have finished reading their stage: hand it back to the producer(s)
+      wgmma_wait<1>();
+      if (kb > 0 && lane == 0) {
+        if (cs == 1) mbar_arrive(&empty_bar[prev]);
+        else for (uint32_t r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
     }
-#pragma unroll 1
-    for (int h = 0; h < NT; ++h) {
-      c.n_tile = blockIdx.y * NT + h;
-      mbar_wait(&tmem_full[h], 0);
-      tc_fence_after();
-      c.trow = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(h * BN);
-      if (dbg && threadIdx.x == 64 && h == 0) dbg[4] = clock64();
-      Epilogue<EPI, BN>::run(g.epi, c);
-      if (dbg && threadIdx.x == 64 && h == NT - 1) dbg[5] = clock64();
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+    if (dbg && threadIdx.x == 0) dbg[3] = clock64();
+    // every warpgroup's MMAs are done with the stages: the accumulator tile may overwrite them
+    asm volatile("bar.sync 6, 512;\n" ::: "memory");
+    {
+      const int r0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < WN / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = r0 + 8 * i, col = nh * WN + 8 * j + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc_s + r * BN + ((((col >> 2) ^ (r & 7)) << 2) | (col & 3))) =
+              make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+        }
     }
+    asm volatile("bar.sync 6, 512;\n" ::: "memory");
+    const int row = q * 32 + lane;
+    c.trow = AccRow{acc_s + row * BN, 0, row & 7};
+    if (dbg && threadIdx.x == 0) dbg[4] = clock64();
+    Epilogue<EPI, BN>::run(g.epi, c);
+    if (dbg && threadIdx.x == 0) dbg[5] = clock64();
     tile_store_drain(c);
   }
-  tc_fence_before();
   __syncthreads();
   if (dbg && threadIdx.x == 0) { dbg[6] = clock64(); dbg[10] = globaltimer_ns(); }
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
-  }
-  // no CTA may leave while a peer can still arrive on its barriers (the last multicast commits of the peers' MMA warps)
+  // no CTA may leave while a peer can still arrive on its barriers or multicast into its shared memory
   if (cs > 1) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------------
-// act_gemm2 kernel: the same GEMM on CTA PAIRS (tcgen05 cta_group::2, cluster of 2 along M).
-//   One MMA covers 256 positions (128 per CTA) x BN columns; each CTA stages its own activation rows and only HALF of the weight
-//   tile (BN/2 rows), so a pipeline stage is 16 KB + BN/2*128 B instead of 16 KB + BN*128 B: fewer bytes per MMA cycle AND more
-//   stages in flight (measured on B200: the 1-CTA kernel is bound by bytes in flight per SM - 3 -> 2 stages costs +24..30 %).
-//   Roles: every CTA runs a TMA producer (its loads complete on the LEADER's full barrier) and the 16 epilogue warps (own TMEM
-//   rows); the leader's MMA thread issues for both SMs and commits, by multicast, to the empty / accumulator-ready barriers of both.
-// ------------------------------------------------------------------------------------------------
-template <int BN>
-struct ActGemm2Cfg {
-  static constexpr int kABytes = kBM * kBK * 2;          // 16 KB: this CTA's 128 positions
-  static constexpr int kBBytes = (BN / 2) * kBK * 2;     // this CTA's half of the weight tile rows
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStagingBytes = 4 * kEpiWarpBytes;
-  static constexpr int kStages = (232448 - kStagingBytes - 1024 - 256) / kStageBytes > 6 ? 6 : (232448 - kStagingBytes - 1024 - 256) / kStageBytes;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 1024 + 256;
-  static_assert(kStages >= 3 && kSmemBytes <= 232448, "shared memory budget");
-};
-
-template <int EPI, int BN, int NT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kActGemmThreads, 1) act_gemm2_kernel(const __grid_constant__ GemmArgs g) {
-  using Cfg = ActGemm2Cfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-  uint64_t* tmem_full = empty_bar + Cfg::kStages;      // [NT]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + NT);
-  constexpr int kTmemCols = (NT * BN) < 32 ? 32 : NT * BN;
-  static_assert(kTmemCols <= 512 && (kTmemCols & (kTmemCols - 1)) == 0, "TMEM columns");
-
-  const int warp = threadIdx.x >> 5;
-  const int m_tile = blockIdx.x;
-  const uint32_t crank = cluster_ctarank();      // 0 = leader of the pair
-  long long* dbg = g.dbg ? g.dbg + (size_t(blockIdx.y) * gridDim.x + blockIdx.x) * kDbgSlots : nullptr;
-  if (dbg && threadIdx.x == 0) { dbg[0] = clock64(); dbg[8] = globaltimer_ns(); dbg[11] = smid(); }
-  const int b = m_tile / g.tiles_per_b;
-  const int t0 = (m_tile - b * g.tiles_per_b) * kBM;
-  int total_kb = 0;
-  for (int s = 0; s < g.nseg; ++s) total_kb += g.seg[s].nkb * g.seg[s].nlayers;
-
-  if (warp == 0 && elect_one()) {
-    for (int i = 0; i < 4; ++i) tma_prefetch_desc(&g.amap[i]);
-    tma_prefetch_desc(&g.bmap);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-      for (int i = 0; i < NT; ++i) mbar_init(&tmem_full[i], 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc_pair<kTmemCols>(tmem_slot);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  cluster_sync_all();            // both CTAs' barriers are initialised and both TMEM halves allocated before any cross-CTA signal
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  pdl_launch_dependents();
-  if (dbg && threadIdx.x == 0) { dbg[1] = clock64(); dbg[9] = globaltimer_ns(); }
-
-  if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int h = 0; h < NT; ++h) {
-        const int n_tile = blockIdx.y * NT + h;
-        int kb_global = 0;
-        for (int s = 0; s < g.nseg; ++s) {
-          const Seg sg = g.seg[s];
-          for (int l = 0; l < sg.nlayers; ++l) {
-            for (int kb = 0; kb < sg.nkb; ++kb, ++kb_global) {
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              // both CTAs' bytes for this stage complete on the leader's barrier: the leader arms it with the pair's total
-              if (crank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-              const uint32_t lead_bar = mapa_cluster(&full_bar[stage], 0);
-              uint8_t* sa = smem + stage * Cfg::kStageBytes;
-              uint8_t* sb = sa + Cfg::kABytes;
-              tma_load_4d_pair(sa, &g.amap[sg.map], lead_bar, sg.k0 + kb * kBK, t0 + sg.shift, b, sg.layer0 + l);
-              tma_load_3d_pair(sb, &g.bmap, lead_bar, g.b_k0 + kb_global * kBK, n_tile * BN + int(crank) * (BN / 2), g.b_layer);
-              if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (crank == 0 && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(2 * kBM, BN, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int h = 0; h < NT; ++h) {
-        const uint32_t tmem_d = tmem_base + uint32_t(h * BN);
-        for (int kb = 0; kb < total_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (dbg && kb == 0 && h == 0) dbg[2] = clock64();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t sb = sa + Cfg::kABytes;
-          const uint64_t adesc = make_sdesc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_sdesc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k)
-            umma_f16_pair(tmem_d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit_pair(&empty_bar[stage], 3);     // frees the stage in both CTAs
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        if (dbg && h == NT - 1) dbg[3] = clock64();
-        umma_commit_pair(&tmem_full[h], 3);           // accumulator half h is complete in both CTAs' TMEM
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    EpiCtx c;
-    c.lane = threadIdx.x & 31;
-    c.cg = (warp - 2) >> 2;
-    c.qbar = 1 + q;
-    c.b = b; c.T = g.T;
-    const int tw = t0 + q * 32;
-    c.t = tw + c.lane;
-    c.valid = c.t < g.T;
-    c.row0 = size_t(b) * g.T + tw;
-    c.nrows = g.T - tw < 0 ? 0 : (g.T - tw > 32 ? 32 : g.T - tw);
-    c.wbuf = staging + q * kEpiWarpBytes;
-    c.smem_all = staging;
-    c.m_tile = m_tile;
-    c.omap = g.omap; c.tq = tw; c.sk = 0;
-    if constexpr (EpiHasPrefetch<EPI>::value && NT == 1) {
-      c.n_tile = blockIdx.y;
-      Epilogue<EPI, BN>::prefetch(g.epi, c);
-    }
-#pragma unroll 1
-    for (int h = 0; h < NT; ++h) {
-      c.n_tile = blockIdx.y * NT + h;
-      mbar_wait(&tmem_full[h], 0);
-      tc_fence_after();
-      c.trow = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(h * BN);
-      if (dbg && threadIdx.x == 64 && h == 0) dbg[4] = clock64();
-      Epilogue<EPI, BN>::run(g.epi, c);
-      if (dbg && threadIdx.x == 64 && h == NT - 1) dbg[5] = clock64();
-    }
-    tile_store_drain(c);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (dbg && threadIdx.x == 0) { dbg[6] = clock64(); dbg[10] = globaltimer_ns(); }
-  cluster_sync_all();            // the peer's epilogue has drained its TMEM half / nobody signals this CTA any more
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair<kTmemCols>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // wgrad_gemm kernel: both operands MN-major (channels contiguous), reduction over positions.
+//   Warps 0..7 = two consumer warpgroups (warpgroup w: output rows [64 w, +64), i.e. A channel block w, all N columns),
+//   warp 8 = TMA producer. The accumulators go from registers straight to the fp32 output.
 // ------------------------------------------------------------------------------------------------
 constexpr int kWgBN = 256;      // up to 256 output columns per tile: the A block pair is reused for twice the MMA work
 constexpr int kWgStages = 4;
 constexpr int kWgStageBytes = 6 * (kBK * 128);  // A: 2 blocks of [64 pos x 128 B] (16 KB), B: up to 4 blocks (32 KB)
 constexpr int kWgSmemBytes = kWgStages * kWgStageBytes + 1024 + 256;
+static_assert(kWgSmemBytes <= 232448, "shared memory budget");
+
+template <int N>
+__device__ __forceinline__ void wgrad_consume(const WgradArgs& g, const WgradTile& tile, uint8_t* smem, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int total_kb) {
+  constexpr int kBlk = kBK * 128;  // bytes of one [64 pos x 64 ch] block
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  int stage = 0, prev = 0;
+  uint32_t phase = 0;
+  for (int kb = 0; kb < total_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    __syncwarp();
+    const uint32_t sa = smem_u32(smem + stage * kWgStageBytes) + uint32_t(wg * kBlk);
+    const uint32_t sb = smem_u32(smem + stage * kWgStageBytes + 2 * kBlk);
+    // MN-major SW128: LBO = distance between 64-channel blocks, SBO = distance between 8-position groups
+    const uint64_t adesc = make_gdesc_sw128(sa, kBlk, 1024);
+    const uint64_t bdesc = make_gdesc_sw128(sb, kBlk, 1024);
+    wgmma_fence();
+    wgmma_fence_regs(d);
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k)
+      // 16 positions = 2 swizzle atoms of 8 rows x 128 B = 2048 bytes -> +128 in the (addr>>4) field
+      Wgmma<N, 1, 1>::mma(d, adesc + uint64_t(k * 128), bdesc + uint64_t(k * 128), (kb > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_fence_regs(d);
+    wgmma_wait<1>();
+    if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == kWgStages) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(d);
+  float sc = tile.scale;
+  if (tile.div) sc /= fmaxf(__ldg(tile.div), 1e-20f);
+  float* out = g.out + tile.out_off;
+  const int m0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int m = m0 + 8 * i, n = 8 * j + 2 * (lane & 3) + e;
+        if (m < tile.m_valid && n < tile.n_valid) {
+          float* o = out + size_t(m) * tile.ldc + n;
+          const float r = d[4 * j + 2 * i + e] * sc;
+          if (tile.accumulate == 2) atomicAdd(o, r);
+          else if (tile.accumulate == 1) *o += r;
+          else *o = r;
+        }
+      }
+}
 
 __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradArgs g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kWgStages * kWgStageBytes);
   uint64_t* empty_bar = full_bar + kWgStages;
-  uint64_t* tmem_full = empty_bar + kWgStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
   const int warp = threadIdx.x >> 5;
   const WgradTile tile = g.tiles[blockIdx.x];
   const int kb_per_b = (g.T + kBK - 1) / kBK;
   const int total_kb = kb_per_b * g.B;
   const int nblk = (tile.n_valid + 63) >> 6;   // 64-channel B blocks this tile needs (1..4)
 
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int i = 0; i < kWgStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-      mbar_init(tmem_full, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc<kWgBN>(tmem_slot);
+  if (warp == 8 && elect_one()) {
+    for (int i = 0; i < kWgStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }   // 8 consumer warps
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();               // (the tile table read above is written once at init, never by a preceding kernel)
   pdl_launch_dependents();
-  constexpr int kBlk = kBK * 128;  // bytes of one [64 pos x 64 ch] block
+  constexpr int kBlk = kBK * 128;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {
       int stage = 0; uint32_t phase = 0;
       for (int bb = 0; bb < g.B; ++bb)
@@ -1382,59 +1278,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1) wgrad_gemm_kernel(const __gri
           if (++stage == kWgStages) { stage = 0; phase ^= 1; }
         }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_bf16(kBM, nblk * 64, 1, 1);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * kWgStageBytes);
-        const uint32_t sb = sa + 2 * kBlk;
-        // MN-major SW128: LBO = distance between 64-channel blocks, SBO = distance between 8-position groups
-        const uint64_t adesc = make_sdesc_sw128(sa, kBlk, 1024);
-        const uint64_t bdesc = make_sdesc_sw128(sb, kBlk, 1024);
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          // 16 positions = 2 swizzle atoms of 8 rows x 128 B = 2048 bytes -> +128 in the (addr>>4) field
-          umma_f16(tmem_base, adesc + uint64_t(k * 128), bdesc + uint64_t(k * 128), idesc,
-                   (kb > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (++stage == kWgStages) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
   } else {
-    const int q = warp & 3;
-    const int m = q * 32 + (threadIdx.x & 31);
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const uint32_t trow = tmem_base + (uint32_t(q * 32) << 16);
-    float* out = g.out + tile.out_off + size_t(m) * tile.ldc;
-    float sc = tile.scale;
-    if (tile.div) sc /= fmaxf(__ldg(tile.div), 1e-20f);
-#pragma unroll 1
-    for (int j0 = 0; j0 < tile.n_valid; j0 += 32) {   // (warp-uniform bound)
-      float v[32];
-      tmem_ld32f(trow + j0, v);
-      if (m < tile.m_valid) {
-        for (int j = 0; j < 32; ++j) {
-          if (j0 + j < tile.n_valid) {
-            const float r = v[j] * sc;
-            if (tile.accumulate == 2) atomicAdd(out + j0 + j, r);
-            else if (tile.accumulate == 1) out[j0 + j] += r;
-            else out[j0 + j] = r;
-          }
-        }
-      }
+    switch (nblk) {
+      case 1: wgrad_consume<64>(g, tile, smem, full_bar, empty_bar, total_kb); break;
+      case 2: wgrad_consume<128>(g, tile, smem, full_bar, empty_bar, total_kb); break;
+      case 3: wgrad_consume<192>(g, tile, smem, full_bar, empty_bar, total_kb); break;
+      default: wgrad_consume<256>(g, tile, smem, full_bar, empty_bar, total_kb); break;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kWgBN>(tmem_base);
   }
 }
 

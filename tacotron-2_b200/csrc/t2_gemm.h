@@ -1,4 +1,4 @@
-// t2_gemm.h — host-side interface of the tcgen05 GEMM engine (see t2_gemm.cuh for the kernels).
+// t2_gemm.h — host-side interface of the wgmma GEMM engine (see t2_gemm.cuh for the kernels).
 #pragma once
 #include <cuda_runtime.h>
 #include <string.h>

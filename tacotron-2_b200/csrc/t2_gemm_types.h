@@ -5,10 +5,10 @@
 
 namespace t2 {
 
-constexpr int kBM = 128;      // positions per tile (UMMA M)
+constexpr int kBM = 128;      // positions per tile (two 64-row wgmma warpgroups)
 constexpr int kBK = 64;       // K elements per pipeline stage (= one 128-byte swizzle row of bf16)
 constexpr int kMaxSeg = 16;
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 288;   // wgrad_gemm: two consumer warpgroups + producer warp
 constexpr int kDbgSlots = 16;  // int64 stamps per CTA in the optional timing buffer (t2_dbg_set_timing_buffer)
 
 struct Seg {

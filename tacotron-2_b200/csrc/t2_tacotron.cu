@@ -4,7 +4,7 @@
 // ZoneoutLSTMCell, Prenet, projections, Postnet), attention.py (location-sensitive attention) and
 // Architecture_wrappers.py:169-213 (decoder step order) of the reference.
 //
-// Mapping onto the B200:
+// Mapping onto the H100:
 //   * everything that is batched over time runs on act_gemm_kernel: the k=5 'same' convolutions are 5 row-shifted
 //     K-segments (zero padding = TMA out-of-bounds fill), prenet / LSTM input projections / frame+stop projections /
 //     attention keys are plain 1x1 GEMMs; weight gradients of all of them go through wgrad_gemm_kernel.
@@ -529,7 +529,7 @@ __device__ __forceinline__ void att_query(const bf16* __restrict__ WqT, const fl
 // ---- the location filter bank on tensor cores -------------------------------------------------------------------
 // pl[j][n] = u0[n] + sum_k cum[j + k - half] U[k][n] is a [T_in x 32] Toeplitz matrix times the [32 x A] filter bank
 // (row KA of the bank is the offset u0, matched by a column of ones): per batch item 160 x 32 x 128 - far too small for a
-// tcgen05 tile pipeline, so it runs as warp-level mma.sync.m16n8k8 TF32 (fp32 accumulate) straight out of shared memory;
+// wgmma tile pipeline, so it runs as warp-level mma.sync.m16n8k8 TF32 (fp32 accumulate) straight out of shared memory;
 // the Toeplitz operand is never materialised (fragments read cum[j + k]). The same instruction computes the three
 // products of the backward pass (dU = T^T dE, P = dE U^T for dcum). The scalar FMA form was issue/shared-memory bound:
 // 20 k (forward) / 55 k (backward) cycles per step at T_in = 160 (tools/att_phases.py).

@@ -1,4 +1,4 @@
-// t2_wavenet.cu — WaveNet vocoder (teacher-forced train path) on the tcgen05 GEMM engine.
+// t2_wavenet.cu — WaveNet vocoder (teacher-forced train path) on the wgmma GEMM engine.
 //
 // Replaces wavenet_vocoder/models/wavenet.py:650-721 (step), :476-519 (add_loss) and the layers in
 // wavenet_vocoder/models/modules.py / mixture.py of the reference. HBM data layout (DESIGN.md §3):
@@ -74,6 +74,7 @@ struct Layout {
   // workspace (byte offsets)
   long long w_cup, w_x, w_xd, w_ta, w_sb, w_z, w_h1, w_h2, w_dlog, w_dh2, w_dskip, w_dxin, w_dg, w_dcup;
   long long w_skipsum;
+  long long w_gfx;      // int64 fixed-point accumulators of the gradients summed by many blocks (t2_common.cuh fx_add)
   long long w_upgrad[2], w_scalars, w_tiles_main, w_tiles_head, w_packjobs, w_colsum, w_tables;
   std::vector<long long> w_upout;
   std::vector<int> up_w;  // width after each upsample layer
@@ -221,7 +222,8 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.w_dg = takeb(L * BT * lo.G * 2);
   lo.w_dcup = takeb(BT * (lo.C > 0 ? lo.C : 8) * 4);
   lo.w_scalars = takeb(64 * 4);
-  lo.w_skipsum = takeb(lo.S * 4);
+  lo.w_skipsum = takeb(lo.S * 8);
+  lo.w_gfx = takeb(lo.n_params * 8);
 
   // ---- pack jobs ----
   lo.packjobs.clear();
@@ -466,7 +468,7 @@ __global__ void first_conv_kernel(const void* __restrict__ xin, int scalar_in, c
   }
 }
 __global__ void first_conv_bwd_kernel(const void* __restrict__ xin, int scalar_in, const bf16* __restrict__ dx0,
-                                      float* __restrict__ dW, long long npos, int R) {
+                                      long long* __restrict__ dW, long long npos, int R) {
   // one block = 64 positions x R channels; scalar input reduces in registers first
   const int r = threadIdx.x;
   const long long p0 = (long long)blockIdx.x * 64;
@@ -474,16 +476,16 @@ __global__ void first_conv_bwd_kernel(const void* __restrict__ xin, int scalar_i
     float acc = 0.f;
     for (int i = 0; i < 64 && p0 + i < npos; ++i)
       acc += static_cast<const float*>(xin)[p0 + i] * __bfloat162float(dx0[(p0 + i) * R + r]);
-    atomicAdd(dW + r, acc);
+    fx_add(dW + r, acc);
   } else {
     for (int i = 0; i < 64 && p0 + i < npos; ++i) {
       const int idx = static_cast<const int*>(xin)[p0 + i];
-      atomicAdd(dW + (long long)idx * R + r, __bfloat162float(dx0[(p0 + i) * R + r]));
+      fx_add(dW + (long long)idx * R + r, __bfloat162float(dx0[(p0 + i) * R + r]));
     }
   }
 }
 
-__global__ void colsum_kernel(const uint8_t* __restrict__ ws, float* __restrict__ grads, const ColsumJob* __restrict__ jobs,
+__global__ void colsum_kernel(const uint8_t* __restrict__ ws, long long* __restrict__ grads, const ColsumJob* __restrict__ jobs,
                               const float* __restrict__ scalars) {
   const ColsumJob j = jobs[blockIdx.y];
   const bf16* src = reinterpret_cast<const bf16*>(ws + j.src_off);
@@ -508,11 +510,11 @@ __global__ void colsum_kernel(const uint8_t* __restrict__ ws, float* __restrict_
       a0 += bf16lo(u); a1 += bf16hi(u);
     }
     a0 *= sc; a1 *= sc;
-    atomicAdd(grads + j.dst_off + c, a0);
-    if (c + 1 < j.C) atomicAdd(grads + j.dst_off + c + 1, a1);
+    fx_add(grads + j.dst_off + c, a0);
+    if (c + 1 < j.C) fx_add(grads + j.dst_off + c + 1, a1);
     if (j.dst2_off >= 0) {
-      atomicAdd(grads + j.dst2_off + c, a0);
-      if (c + 1 < j.C) atomicAdd(grads + j.dst2_off + c + 1, a1);
+      fx_add(grads + j.dst2_off + c, a0);
+      if (c + 1 < j.C) fx_add(grads + j.dst2_off + c + 1, a1);
     }
   }
 }
@@ -580,10 +582,10 @@ __global__ void cl_to_chw_kernel(const float* __restrict__ in, float* __restrict
 // thread always meets the same sub-pixel phase k = e % s: it sums its taps in registers, the block merges through a
 // small shared-memory table (10 atomics per thread, once) and issues one global atomic per table entry.
 __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const float* __restrict__ out, const float* __restrict__ dout,
-                                          float* __restrict__ dK, float* __restrict__ dbias, int B, int H, int W, int s, int type) {
-  __shared__ float acc[10 * 32];
+                                          long long* __restrict__ dK, long long* __restrict__ dbias, int B, int H, int W, int s, int type) {
+  __shared__ long long acc[10 * 32];
   const int ntap = type == 0 ? 9 : 3;
-  for (int i = threadIdx.x; i < (ntap + 1) * s; i += blockDim.x) acc[i] = 0.f;
+  for (int i = threadIdx.x; i < (ntap + 1) * s; i += blockDim.x) acc[i] = 0;
   __syncthreads();
   const int Wo = W * s;
   const long long n = (long long)B * H * Wo;
@@ -620,15 +622,15 @@ __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const fl
   }
 #pragma unroll
   for (int i = 0; i < 9; ++i)
-    if (i < ntap && r[i] != 0.f) atomicAdd(&acc[i * s + k], r[i]);
-  if (r[9] != 0.f) atomicAdd(&acc[ntap * s + k], r[9]);
+    if (i < ntap && r[i] != 0.f) fx_add(&acc[i * s + k], r[i]);
+  if (r[9] != 0.f) fx_add(&acc[ntap * s + k], r[9]);
   __syncthreads();
   for (int i = threadIdx.x; i < (ntap + 1) * s; i += blockDim.x) {
-    const float v = acc[i];
-    if (v == 0.f) continue;
-    if (i < ntap * s) atomicAdd(dK + i, v);
-    else if (type == 0) atomicAdd(dbias + (i - ntap * s), v);
-    else atomicAdd(dbias, v);
+    const unsigned long long v = static_cast<unsigned long long>(acc[i]);
+    if (v == 0) continue;
+    if (i < ntap * s) atomicAdd(reinterpret_cast<unsigned long long*>(dK + i), v);
+    else if (type == 0) atomicAdd(reinterpret_cast<unsigned long long*>(dbias + (i - ntap * s)), v);
+    else atomicAdd(reinterpret_cast<unsigned long long*>(dbias), v);
   }
 }
 __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const float* __restrict__ dout, int cl,
@@ -670,12 +672,17 @@ __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const f
   if (live && part == 0) din[e] = acc;
 }
 // skip-conv bias gradients: db_s[l] = skip_scale[l] * column sums of dskip (table layout: offs[3l+2] = skip bias offset)
-__global__ void skip_bias_kernel(const float* __restrict__ skipsum, float* __restrict__ grads, const long long* __restrict__ offs,
+__global__ void skip_bias_kernel(const long long* __restrict__ skipsum, float* __restrict__ grads, const long long* __restrict__ offs,
                                  const float* __restrict__ scales, int L, int S) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L * S) return;
   const int l = i / S, s = i % S;
-  grads[offs[3 * l + 2] + s] = scales[l] * skipsum[s];
+  grads[offs[3 * l + 2] + s] = scales[l] * fx_value(skipsum[s]);
+}
+// grads += the fixed-point totals of the block-summed gradients (first conv, biases, upsampling net)
+__global__ void fx_finalize_kernel(const long long* __restrict__ acc, float* __restrict__ grads, long long n) {
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e < n && acc[e] != 0) grads[e] += fx_value(acc[e]);
 }
 __global__ void f32_to_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -745,7 +752,8 @@ ActGemmCall make_out_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, cons
   return o;
 }
 
-ActGemmCall make_dz_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l, float* grads) {
+// grads: the int64 fixed-point gradient accumulators (w_gfx), or nullptr for no bias gradients
+ActGemmCall make_dz_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l, long long* grads) {
   const long long BT = (long long)lo.B * lo.T;
   const bool top = l == lo.L - 1;
   ActGemmCall g;
@@ -774,7 +782,7 @@ ActGemmCall make_dz_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
 }
 
 ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l, float p, unsigned long long seed,
-                         const unsigned long long* d_step, float* grads) {
+                         const unsigned long long* d_step, long long* grads) {
   const long long BT = (long long)lo.B * lo.T;
   const int d = lo.dil(l);
   const bool top = l == lo.L - 1;
@@ -1058,6 +1066,10 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
       T2_CHECK_CUDA(cudaEventRecord(side->join, side->s));
       T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
     }
+    fx_finalize_kernel<<<grid1d(lo.n_params), 256, 0, st>>>(reinterpret_cast<const long long*>(static_cast<uint8_t*>(d_workspace) + lo.w_gfx),
+                                                           d_grads, lo.n_params);
+    t2_count_launch();
+    T2_CHECK_CUDA(cudaGetLastError());
     return T2_OK;
   }
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
@@ -1066,7 +1078,9 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   float* scalars = reinterpret_cast<float*>(ws + lo.w_scalars);
   const float p = cfg->dropout;
   T2_CHECK_CUDA(cudaMemsetAsync(d_grads, 0, lo.n_params * sizeof(float), st));
-  T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_skipsum, 0, lo.S * sizeof(float), st));
+  T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_skipsum, 0, lo.S * sizeof(long long), st));
+  T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_gfx, 0, lo.n_params * sizeof(long long), st));
+  long long* gfx = reinterpret_cast<long long*>(ws + lo.w_gfx);
   bf16* h1 = reinterpret_cast<bf16*>(ws + lo.w_h1);
   bf16* h2 = reinterpret_cast<bf16*>(ws + lo.w_h2);
   bf16* dlog = reinterpret_cast<bf16*>(ws + lo.w_dlog);
@@ -1085,7 +1099,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     g.w = pk + lo.k_Wf2T; g.wN = lo.S; g.wK = lo.Op; g.wL = 1;
     g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
     g.epi.ptr[0] = dh2; g.epi.ptr[1] = h2; g.epi.ptr[2] = scalars + 1; g.epi.f[0] = 1.f; g.epi.i[0] = lo.S;
-    g.epi.ptr[3] = d_grads + lo.p_f1_b;
+    g.epi.ptr[3] = gfx + lo.p_f1_b;
     rc = launch_act_gemm(EPI_SCALE_RELUMASK, lo.S, g, st);
     if (rc) return rc;
   }
@@ -1101,12 +1115,12 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     rc = launch_act_gemm(EPI_SCALE_RELUMASK, lo.S, g, st);
     if (rc) return rc;
   }
-  skip_bias_kernel<<<grid1d((long long)lo.L * lo.S), 256, 0, st>>>(reinterpret_cast<const float*>(ws + lo.w_skipsum), d_grads,
+  skip_bias_kernel<<<grid1d((long long)lo.L * lo.S), 256, 0, st>>>(reinterpret_cast<const long long*>(ws + lo.w_skipsum), d_grads,
       reinterpret_cast<const long long*>(ws + lo.w_tables), reinterpret_cast<const float*>(ws + lo.w_tables + 3 * lo.L * sizeof(long long)), lo.L, lo.S);
   t2_count_launch();
   // The head's weight gradients (6 tiles with a 15360-long reduction: ~100 us on 6 SMs) and the bias column sums of dlog
   // depend only on the head backward above: they run on the side stream underneath the whole residual-stack chain below,
-  // which leaves 28 SMs idle (120 M tiles on 148 SMs).
+  // which leaves SMs idle (120 M tiles).
   SideStream* side = side_stream();
   cudaStream_t sb = st;
   if (side) {
@@ -1119,7 +1133,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
                      make_act(dlog, lo.ldo, lo.T, lo.B)};
     rc = launch_wgrad(hmaps, 4, reinterpret_cast<const WgradTile*>(ws + lo.w_tiles_head), lo.n_tiles_head, d_grads, lo.T, lo.B, sb);
     if (rc) return rc;
-    colsum_kernel<<<dim3(96, lo.n_colsum), 256, 0, sb>>>(ws, d_grads, reinterpret_cast<const ColsumJob*>(ws + lo.w_colsum), scalars); t2_count_launch();
+    colsum_kernel<<<dim3(96, lo.n_colsum), 256, 0, sb>>>(ws, gfx, reinterpret_cast<const ColsumJob*>(ws + lo.w_colsum), scalars); t2_count_launch();
     T2_CHECK_CUDA(cudaGetLastError());
   }
   // residual stack, top down
@@ -1128,10 +1142,10 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   const ActT a_dg = make_act(dg, lo.G, lo.T, lo.B, lo.L);
   const int bn_z = lo.Gh >= 256 ? 256 : 128;
   for (int l = lo.L - 1; l >= 0; --l) {
-    ActGemmCall gz = make_dz_call(lo, ws, pk, l, d_grads);
+    ActGemmCall gz = make_dz_call(lo, ws, pk, l, gfx);
     rc = launch_act_gemm(EPI_GATE_BWD, bn_z, gz, st);
     if (rc) return rc;
-    ActGemmCall gx = make_dx_call(lo, ws, pk, l, p, seed, d_step, d_grads);
+    ActGemmCall gx = make_dx_call(lo, ws, pk, l, p, seed, d_step, gfx);
     rc = launch_act_gemm(EPI_DX, lo.R, gx, st);
     if (rc) return rc;
   }
@@ -1151,7 +1165,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     if (rc) return rc;
   }
   // first conv
-  first_conv_bwd_kernel<<<dim3((unsigned)((BT + 63) / 64)), lo.R, 0, sb>>>(d_x, lo.scalar_in ? 1 : 0, dxin, d_grads + lo.p_in_k, BT, lo.R); t2_count_launch();
+  first_conv_bwd_kernel<<<dim3((unsigned)((BT + 63) / 64)), lo.R, 0, sb>>>(d_x, lo.scalar_in ? 1 : 0, dxin, gfx + lo.p_in_k, BT, lo.R); t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   // conditioning path
   if (lo.C > 0 && !cfg->c_pre_upsampled) {
@@ -1177,7 +1191,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
       T2_REQUIRE(s <= 32, T2_ERR_UNSUPPORTED_SHAPE, "upsample scale > 32");
       const float* layer_in = i == 0 ? d_c : reinterpret_cast<const float*>(ws + lo.w_upout[i - 1]);
       const float* out = reinterpret_cast<const float*>(ws + lo.w_upout[i]);
-      upsample_bwd_param_kernel<<<s * ((296 + s - 1) / s), 256, 0, sb>>>(layer_in, out, dout, d_grads + lo.p_up_k[i], d_grads + lo.p_up_b[i], lo.B, lo.C, W, s,
+      upsample_bwd_param_kernel<<<s * ((296 + s - 1) / s), 256, 0, sb>>>(layer_in, out, dout, gfx + lo.p_up_k[i], gfx + lo.p_up_b[i], lo.B, lo.C, W, s,
                                                      cfg->upsample_type); t2_count_launch();
       if (i > 0) {
         float* din = reinterpret_cast<float*>(ws + lo.w_upgrad[pp]);
@@ -1192,6 +1206,11 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   if (side && phase == -1) {
     T2_CHECK_CUDA(cudaEventRecord(side->join, sb));
     T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
+  }
+  if (phase == -1) {   // (phased: once the side stream has joined, in phase 100)
+    fx_finalize_kernel<<<grid1d(lo.n_params), 256, 0, st>>>(gfx, d_grads, lo.n_params);
+    t2_count_launch();
+    T2_CHECK_CUDA(cudaGetLastError());
   }
   return T2_OK;
 }

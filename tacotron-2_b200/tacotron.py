@@ -1,4 +1,4 @@
-"""Host side of the B200 Tacotron-2 mel predictor (training graph). Mirrors tacotron/models/tacotron.py: the
+"""Host side of the H100 Tacotron-2 mel predictor (training graph). Mirrors tacotron/models/tacotron.py: the
 reference's ``initialize`` + ``add_loss`` + ``add_optimizer`` become ``forward`` / ``backward`` / ``optimizer_step``."""
 import ctypes
 import math
@@ -81,7 +81,7 @@ def make_config(hp, B, T_in, T_out, precision="bf16"):
         raise L.T2Error("precision must be 'bf16' or 'fp32-class'")
     bad = unsupported_hparams(hp)
     if bad:
-        raise L.T2Error("hparams not implemented on the B200 Tacotron path (they would change the model): " + "; ".join(bad))
+        raise L.T2Error("hparams not implemented on the H100 Tacotron path (they would change the model): " + "; ".join(bad))
     c = TacoConfig()
     c.B, c.T_in, c.T_out = B, T_in, T_out
     c.n_symbols, c.num_mels, c.embedding_dim = N_SYMBOLS, hp.num_mels, hp.embedding_dim

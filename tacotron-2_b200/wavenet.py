@@ -1,4 +1,4 @@
-"""Host side of the B200 WaveNet vocoder: owns device buffers (torch tensors) and drives libt2b200.so.
+"""Host side of the H100 WaveNet vocoder: owns device buffers (torch tensors) and drives libt2b200.so.
 
 Mirrors the reference's model object (wavenet_vocoder/models/wavenet.py): ``WaveNet(hparams)`` then
 ``initialize`` / ``step`` (forward), ``add_loss`` (loss) and ``add_optimizer`` (Adam + clipping + EMA) collapse into
@@ -57,7 +57,7 @@ def unsupported_hparams(hp):
 def make_config(hp, B, T, c_pre_upsampled=False, dropout=None, precision="bf16"):
     bad = unsupported_hparams(hp)
     if bad:
-        raise L.T2Error("hparams not implemented on the B200 WaveNet path (they would change the model): " + "; ".join(bad))
+        raise L.T2Error("hparams not implemented on the H100 WaveNet path (they would change the model): " + "; ".join(bad))
     cfg = WnConfig()
     cfg.layers, cfg.stacks = hp.layers, hp.stacks
     cfg.residual_channels, cfg.gate_channels, cfg.skip_out_channels = (
@@ -70,7 +70,7 @@ def make_config(hp, B, T, c_pre_upsampled=False, dropout=None, precision="bf16")
     if hp.upsample_type == "NearestNeighbor":     # non-learnable repeat (modules.py:524-536, wavenet.py:165-167): done by nn_upsample() below
         c_pre_upsampled = True
     elif hp.upsample_type not in _UPSAMPLE_TYPES:
-        raise L.T2Error("upsample_type %r is not implemented on the B200 path" % hp.upsample_type)
+        raise L.T2Error("upsample_type %r is not implemented on the H100 path" % hp.upsample_type)
     cfg.upsample_type = _UPSAMPLE_TYPES.get(hp.upsample_type, 0)
     scales = list(hp.upsample_scales)
     cfg.n_upsample = len(scales)
@@ -136,7 +136,7 @@ def nn_upsample(hp, c, T):
 
 
 class WaveNet(object):
-    """B200 WaveNet (train path). Parameters live in ONE flat fp32 buffer in TensorFlow variable layouts."""
+    """H100 WaveNet (train path). Parameters live in ONE flat fp32 buffer in TensorFlow variable layouts."""
 
     def __init__(self, hparams, B, T, device="cuda", c_pre_upsampled=False, dropout=None, training=True, precision="bf16"):
         """precision: 'bf16' (training / benchmark path: bf16 operands and stored activations, fp32 accumulate) or 'fp32-class'
@@ -398,7 +398,7 @@ class WaveNet(object):
 
 
 class WaveNetSynthesizer(object):
-    """Fast-WaveNet autoregressive generation on the B200 (wavenet_vocoder/synthesizer.py + WaveNet.incremental)."""
+    """Fast-WaveNet autoregressive generation on the H100 (wavenet_vocoder/synthesizer.py + WaveNet.incremental)."""
 
     def __init__(self, hparams, B, T, cluster_size=8, device="cuda"):
         self.hp = hparams

@@ -4,7 +4,7 @@ through the C-ABI vs the fp32 CPU oracle.
 1. the CBHG engine alone on a GIVEN mel tensor (both sides see identical inputs): linear outputs, linear loss, regulariser, every
    weight gradient and the gradient handed back to the Tacotron graph (d loss / d mel_outputs);
 2. the whole Tacotron training step with the head attached: the extra gradient path through mel_outputs into postnet / decoder.
-Tolerances follow the bf16-operand figures of tests/test_tacotron_gpu.py (<= 2x measured, profiles/r02_measured_parity_v3.jsonl)."""
+Tolerances follow the bf16-operand figures of tests/test_tacotron_gpu.py (<= 2x the values measured on an H100)."""
 import ctypes
 
 import pytest

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM engine vs a plain PyTorch fp32 reference of the same contraction (bf16-rounded inputs)."""
+"""wgmma GEMM engine vs a plain PyTorch fp32 reference of the same contraction (bf16-rounded inputs)."""
 import ctypes
 
 import pytest

@@ -6,8 +6,8 @@ paths (dropout / zoneout masks rebuilt from the library's counter hash and injec
   Cfg-3'  Tacotron full widths (512 / 1024 / 512), B = 32, T_in = 160, T_out = 200, conv dropout 0.5, prenet dropout 0.5,
           zoneout 0.1 all ON with the same masks on both sides
 
-Tolerances are <= 2x the errors measured on B200 (profiles/r02_measured_parity.jsonl: logits max 1.8e-3 / mean 2.8e-4, CE error 8e-6,
-MoL NLL error 6e-5, alignments 3e-4, decoder-output L1 8e-4, stop logits 2.4e-3, mel-L1 on the post-net output 2.8e-2); the product
+Tolerances are <= 2x the errors measured on an H100 (logits max 1.8e-3 / mean 2.8e-4, CE error 8e-6,
+MoL NLL error 7e-5, alignments 3e-4, decoder-output L1 8e-4, stop logits 2.4e-3, mel-L1 on the post-net output 2.8e-2); the product
 runs bf16 GEMM operands / bf16-stored activations with fp32 accumulation here, the oracle fp32 end to end. The north-star 1e-3 figures
 are met by the losses in this mode and by logits / mel-L1 in the fp32-class mode (tests/test_precision_modes_gpu.py)."""
 import math

@@ -1,7 +1,7 @@
 """The two arithmetic modes of the CUDA path against the fp32 oracle (VERDICT r1 item 2, SURVEY §7 step 6 "parity in fp32 first, then
 bf16 mode"). The reference computes in fp32 throughout; the product's training / benchmark mode uses bf16 tensor-core operands and
 bf16-stored activations (fp32 accumulate). The 'fp32-class' mode carries every activation and weight as a bf16 hi + lo pair through the
-SAME tcgen05 kernels (three products per contraction), forward + loss only:
+SAME wgmma kernels (three products per contraction), forward + loss only:
 
   WaveNet fp32-class   logits max abs err <= 1e-4 (measured 6e-6), loss (CE / MoL NLL) abs err <= 1e-4   -> north-star 1e-3 met
   WaveNet bf16         logits max abs err <= 5e-3, loss abs err <= 1e-3 (measured: 1.7e-3 / 3e-5 at the 24-layer Cfg-2 shape)

@@ -1,5 +1,5 @@
 """CUDA Tacotron (through the C-ABI) vs the fp32 CPU oracle, dropout / zoneout off (rates are hparams), same seeded
-inputs. Tolerances (bf16 GEMM operands, fp32 accumulate / state; <= 2x the values measured on B200, profiles/r02_measured_parity.jsonl):
+inputs. Tolerances (bf16 GEMM operands, fp32 accumulate / state; <= 2x the values measured on an H100):
 losses <= 2e-3 absolute + 1e-3 relative, alignments max abs err <= 6e-4, decoder-output L1 <= 1.6e-3, stop logits <= 5e-3, mel outputs
 mean abs err <= 4e-2 (measured 2.5e-2: five batch-normalised postnet layers each add ~0.2 % of a unit-variance activation in bf16 storage
 - tools/taco_layer_diag.py; 6e-4 in the fp32-class mode, tests/test_precision_modes_gpu.py).

@@ -4,14 +4,14 @@ Tolerances: the product path computes its GEMMs with bf16 operands / fp32 accumu
   loss            |cuda - oracle| <= 1e-4 (CE; measured <= 3.4e-5), 6e-4 (MoL; measured 2.6e-4), 3e-3 (Gaussian log-density)
                   - north-star: NLL / CE parity within 1e-3
   logits          max abs err <= 8e-3, mean abs err <= 1.5e-3      (bf16 operand rounding through the stack; measured max 1.4e-3 with
-                  mu-law input, 3.7e-3 with raw input; <= 2x measured, profiles/r02_measured_parity.jsonl). The fp32-class mode
+                  mu-law input, 3.7e-3 with raw input; <= 2x measured on an H100). The fp32-class mode
                   (tests/test_precision_modes_gpu.py) reaches 6e-6.
   gradients       per tensor  ||g_cuda - g_ref|| / ||g_ref|| <= 5e-2 against the oracle run with bf16 STORAGE
                   EMULATION (oracle.wavenet.step_sim: same fp32 math, tensors rounded to bf16 where the CUDA path
                   stores bf16) and <= 1e-1 against the plain fp32 oracle. The second bound is loose on purpose: at
                   random init the gradient is a random-walk sum over positions, so the ~0.5 % of ReLU / gate units whose
                   sign flips under bf16 rounding move it by several percent (the fp32 oracle and its own bf16-emulated
-                  twin differ by ~8 % on CPU). Measured on B200: 0.5-3.7 % vs the emulation, 2-5.6 % vs fp32; a real
+                  twin differ by ~8 % on CPU). Measured on an H100: 1.3-4.3 % vs the emulation, 2.4-5.4 % vs fp32; a real
                   backward bug shows up as >= 50 %.
 """
 import math

@@ -1,4 +1,4 @@
-"""Config 5 (BASELINE.json): Fast-WaveNet autoregressive synthesis real-time factor on one B200.
+"""Config 5 (BASELINE.json): Fast-WaveNet autoregressive synthesis real-time factor on one H100.
 RTF = wall time / audio duration (T / 22050 s); < 1 is faster than real time. Paper widths, 1 s of audio."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Config 1 (BASELINE.json): fused STFT + 80-band mel on 1 s clips of 22.05 kHz audio, batch of 4096 clips on one B200.
+"""Config 1 (BASELINE.json): fused STFT + 80-band mel on 1 s clips of 22.05 kHz audio, batch of 4096 clips on one H100.
 Reports clip-seconds/s, achieved algorithmic HBM GB/s (114 120 B per clip-second, SURVEY.md §8d) against
 MEASURED_PEAKS.json, and the numpy oracle on the host cores (bounded sample)."""
 import json, os, sys, time

@@ -5,7 +5,7 @@ Semantics kept from the reference's wavenet_vocoder/feeder.py: deterministic spl
 of at most max_time_steps (rounded DOWN to a multiple of hop_size) starting at a random frame (:368-387); audio length ==
 frames * hop asserted (:400-401); conditioning mels clipped to the Tacotron output range, padded with its minimum and mapped to
 [0, 1] (:319-340); inputs padded with zeros. What differs by design: mu-law inputs stay INDICES ([B, T] int32, the one-hot float
-[B, 256, T] of :295-306 is never materialised: the first 1x1 convolution is a row gather on the B200 path); tensors are pinned
+[B, 256, T] of :295-306 is never materialised: the first 1x1 convolution is a row gather on the H100 path); tensors are pinned
 torch tensors; T is additionally right-padded to a whole hop multiple per batch (it already is, by construction)."""
 import os
 import queue
