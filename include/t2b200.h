@@ -33,7 +33,8 @@ extern "C" {
 const char* t2_last_error(void);
 int t2_abi_version(void);
 /* sizeof() of a POD struct of this header by name ("t2_wn_config_t", "t2_wn_sizes_t", "t2_taco_config_t", "t2_cbhg_config_t",
- * "t2_audio_config_t"), -1 for an unknown name: a binding asserts that its mirror of the struct matches the library it loaded */
+ * "t2_audio_config_t", "t2_dbg_act_t", "t2_dbg_gemm_t", "t2_dbg_wgrad_tile_t"), -1 for an unknown name: a binding asserts that its
+ * mirror of the struct matches the library it loaded */
 int t2_struct_size(const char* name);
 /* kernels launched (or captured) by this library so far in this process */
 long long t2_launch_count(void);
@@ -50,6 +51,58 @@ int t2_dbg_set_timing_buffer(long long* d_buf);
 /* weight-gradient GEMM: out[m,n] = scale * sum_{b,t} a[b,t+shift_a,m] * bm[b,t,n]  (fp32 [Ca,Cb]); synchronises. */
 int t2_dbg_wgrad(const void* d_a, int Ca, const void* d_bm, int Cb, int B, int T, int shift_a, float scale,
                  float* d_out, void* stream);
+
+/* The whole engine surface, for tests of every fused epilogue (tests/test_gemm_epilogues_gpu.py). One A operand: channels-last
+ * bf16 [L][B][T][ld], the first C channels addressable (ld % 8 == 0, 16-byte aligned). */
+typedef struct {
+  const void* ptr;
+  int C, T, B, L, ld;
+} t2_dbg_act_t;
+/* one K segment: nkb 64-wide K blocks of map `map` starting at channel k0, rows shifted by `shift`, looped over layers
+ * [layer0, layer0 + nlayers) (outer); segments consume consecutive K blocks of the packed weight */
+typedef struct {
+  int map, shift, k0, nkb, layer0, nlayers;
+} t2_dbg_seg_t;
+/* act_gemm: D[b, t, n] = sum over segments s, layers l, k of A_map(s)[layer0 + l, b, t + shift, k0 + k] * W[w_layer, n, w_k0 + K offset],
+ * rows outside [0, T) of item b read as zero, then epilogue `epi` (EPI_* of tacotron-2_b200/csrc/t2_gemm_types.h) with BN output columns
+ * per tile and the raw epilogue arguments ptr / f / i / seed documented next to each epilogue in t2_gemm.cuh. ksplit > 1 splits
+ * the reduction over that many CTAs per tile (EPI_TOUT with mode 2 only). cluster: 0 = library default, else 1, 2, 4 or 8 CTAs that
+ * share each weight tile by TMA multicast; cluster_used returns the size actually launched. */
+typedef struct {
+  t2_dbg_act_t a[4];
+  int na;
+  t2_dbg_seg_t seg[16];
+  int nseg;
+  const void* w;             /* packed bf16 weights [wL][wN][wK], K contiguous */
+  int wN, wK, wL, w_layer, w_k0;
+  int T, B, n_tiles, ksplit, epi, BN;
+  int cluster;               /* in */
+  int cluster_used;          /* out */
+  void* ptr[12];
+  float f[6];
+  int i[12];
+  unsigned long long seed;
+} t2_dbg_gemm_t;
+int t2_dbg_act_gemm(t2_dbg_gemm_t* call, void* stream);
+/* One tile of the weight-gradient GEMM: out[out_off + m * ldc + n] (=, +=, atomic +=: accumulate 0 / 1 / 2) scale / max(*div, 1e-20)
+ * * sum over b, t of A_{a_map}[a_layer, b, t + a_shift, a_ch0 + m] * A_{b_map}[b_layer, b, t + b_shift, b_ch0 + n], for m < m_valid (<= 128),
+ * n < n_valid (<= 256); div is a nullable device scalar. */
+typedef struct {
+  int a_map, a_ch0, a_shift, a_layer;
+  int b_map, b_ch0, b_shift, b_layer;
+  long long out_off;
+  int ldc, m_valid, n_valid;
+  float scale;
+  int accumulate;
+  const float* div;
+} t2_dbg_wgrad_tile_t;
+/* runs the host tile table `tiles` over up to 6 maps into the fp32 buffer d_out; synchronises */
+int t2_dbg_wgrad_tiles(const t2_dbg_act_t* maps, int nmaps, const t2_dbg_wgrad_tile_t* tiles, int ntiles, float* d_out, int T, int B,
+                       void* stream);
+/* The fixed-point column sums behind the multi-block gradients: adds d_addends[r * ncols + c] (r < nrows) into column c with the same
+ * atomics the GEMM epilogues use, then converts the totals as the gradient finalisation does: d_out[c] = value of the total (0 for an
+ * empty total). Synchronises. */
+int t2_dbg_fx_colsum(const float* d_addends, int nrows, int ncols, float* d_out, void* stream);
 
 
 /* ---- WaveNet vocoder: teacher-forced training path ---------------------------------------------------------

@@ -1,6 +1,7 @@
 // t2_api.cu — error plumbing of the C-ABI plus the engine-level entry points used by the unit tests.
 #include <stdarg.h>
 #include <stdio.h>
+#include <stddef.h>
 #include <string.h>
 
 #include <vector>
@@ -75,6 +76,89 @@ extern "C" int t2_dbg_wgrad(const void* a, int Ca, const void* bm, int Cb, int B
   return rc;
 }
 
+// the test structs of the header are the engine's own types: the hooks below reinterpret them without copying field by field
+#define T2_SAME_FIELD(A, B, f) static_assert(offsetof(A, f) == offsetof(B, f), #A " / " #B ": field " #f)
+static_assert(sizeof(t2_dbg_act_t) == sizeof(t2::ActT), "t2_dbg_act_t / ActT");
+T2_SAME_FIELD(t2_dbg_act_t, t2::ActT, ptr); T2_SAME_FIELD(t2_dbg_act_t, t2::ActT, C); T2_SAME_FIELD(t2_dbg_act_t, t2::ActT, ld);
+static_assert(sizeof(t2_dbg_seg_t) == sizeof(t2::Seg), "t2_dbg_seg_t / Seg");
+T2_SAME_FIELD(t2_dbg_seg_t, t2::Seg, map); T2_SAME_FIELD(t2_dbg_seg_t, t2::Seg, nlayers);
+static_assert(sizeof(t2_dbg_wgrad_tile_t) == sizeof(t2::WgradTile), "t2_dbg_wgrad_tile_t / WgradTile");
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, a_map); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, a_ch0);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, a_shift); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, a_layer);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, b_map); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, b_ch0);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, b_shift); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, b_layer);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, out_off); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, ldc);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, m_valid); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, n_valid);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, scale); T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, accumulate);
+T2_SAME_FIELD(t2_dbg_wgrad_tile_t, t2::WgradTile, div);
+#undef T2_SAME_FIELD
+
+extern "C" int t2_dbg_act_gemm(t2_dbg_gemm_t* call, void* stream) {
+  using namespace t2;
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "null call");
+  T2_REQUIRE(call->na >= 1 && call->na <= 4 && call->nseg >= 1 && call->nseg <= kMaxSeg, T2_ERR_INVALID_ARG,
+             "bad map/segment count (%d, %d)", call->na, call->nseg);
+  ActGemmCall c;
+  memset(&c, 0, sizeof(c));
+  memcpy(c.a, call->a, sizeof(c.a));
+  c.na = call->na;
+  memcpy(c.seg, call->seg, sizeof(c.seg));
+  c.nseg = call->nseg;
+  c.w = call->w; c.wN = call->wN; c.wK = call->wK; c.wL = call->wL; c.w_layer = call->w_layer; c.w_k0 = call->w_k0;
+  c.T = call->T; c.B = call->B; c.n_tiles = call->n_tiles; c.ksplit = call->ksplit; c.cluster = call->cluster;
+  memcpy(c.epi.ptr, call->ptr, sizeof(c.epi.ptr));
+  memcpy(c.epi.f, call->f, sizeof(c.epi.f));
+  memcpy(c.epi.i, call->i, sizeof(c.epi.i));
+  c.epi.seed = call->seed;
+  call->cluster_used = 0;
+  return launch_act_gemm(call->epi, call->BN, c, static_cast<cudaStream_t>(stream), &call->cluster_used);
+}
+
+extern "C" int t2_dbg_wgrad_tiles(const t2_dbg_act_t* maps, int nmaps, const t2_dbg_wgrad_tile_t* tiles, int ntiles, float* d_out, int T,
+                                  int B, void* stream) {
+  using namespace t2;
+  T2_REQUIRE(maps && tiles && nmaps >= 1 && nmaps <= 6 && ntiles >= 1, T2_ERR_INVALID_ARG, "wgrad_tiles: bad map/tile arguments");
+  for (int i = 0; i < ntiles; ++i)
+    T2_REQUIRE(tiles[i].a_map >= 0 && tiles[i].a_map < nmaps && tiles[i].b_map >= 0 && tiles[i].b_map < nmaps &&
+               tiles[i].m_valid >= 1 && tiles[i].m_valid <= 128 && tiles[i].n_valid >= 1 && tiles[i].n_valid <= 256 &&
+               tiles[i].accumulate >= 0 && tiles[i].accumulate <= 2,
+               T2_ERR_INVALID_ARG, "wgrad_tiles: bad tile %d", i);
+  WgradTile* dt = nullptr;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  T2_CHECK_CUDA(cudaMallocAsync(&dt, ntiles * sizeof(WgradTile), st));
+  const cudaError_t e = cudaMemcpyAsync(dt, tiles, ntiles * sizeof(WgradTile), cudaMemcpyHostToDevice, st);
+  int rc = e == cudaSuccess ? launch_wgrad(reinterpret_cast<const ActT*>(maps), nmaps, dt, ntiles, d_out, T, B, st)
+                            : t2_set_error(T2_ERR_CUDA, "wgrad_tiles: tile table upload failed: %s", cudaGetErrorString(e));
+  cudaStreamSynchronize(st);  // debug entry: the tile table is a temporary
+  cudaFreeAsync(dt, st);
+  return rc;
+}
+
+// each addend goes through fx_add (one thread per addend, so same-column atomics contend as in the epilogues)
+__global__ void fx_colsum_kernel(const float* __restrict__ v, long long n, int ncols, long long* acc) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < n) t2::fx_add(acc + i % ncols, v[i]);
+}
+extern "C" int t2_dbg_fx_colsum(const float* d_addends, int nrows, int ncols, float* d_out, void* stream) {
+  T2_REQUIRE(d_addends && d_out && nrows >= 0 && ncols >= 1, T2_ERR_INVALID_ARG, "fx_colsum: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  long long* acc = nullptr;
+  T2_CHECK_CUDA(cudaMallocAsync(&acc, size_t(ncols) * sizeof(long long), st));
+  const long long n = (long long)nrows * ncols;
+  cudaError_t e = cudaMemsetAsync(acc, 0, size_t(ncols) * sizeof(long long), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_out, 0, size_t(ncols) * sizeof(float), st);
+  if (e == cudaSuccess && n > 0) {
+    fx_colsum_kernel<<<unsigned((n + 255) / 256), 256, 0, st>>>(d_addends, n, ncols, acc);
+    t2_count_launch();
+    e = cudaGetLastError();
+  }
+  int rc = e == cudaSuccess ? t2::launch_fx_finalize(acc, d_out, ncols, st)
+                            : t2_set_error(T2_ERR_CUDA, "fx_colsum: %s", cudaGetErrorString(e));
+  cudaStreamSynchronize(st);  // debug entry: the accumulators are a temporary
+  cudaFreeAsync(acc, st);
+  return rc;
+}
+
 // debug: when non-NULL every act_gemm CTA writes stamps to d_buf[(launch offset + cta) * 16 + slot]: slots 0-6 clock64() at entry,
 // setup done, first stage landed, MMAs issued, accumulator ready, epilogue done, teardown; 8-10 %globaltimer (ns) at entry, after the
 // programmatic-dependent-launch wait, at exit; 11 = SM id. Each launch advances the offset by its CTA count.
@@ -108,5 +192,8 @@ extern "C" int t2_struct_size(const char* name) {
   if (!strcmp(name, "t2_taco_config_t")) return int(sizeof(t2_taco_config_t));
   if (!strcmp(name, "t2_cbhg_config_t")) return int(sizeof(t2_cbhg_config_t));
   if (!strcmp(name, "t2_audio_config_t")) return int(sizeof(t2_audio_config_t));
+  if (!strcmp(name, "t2_dbg_act_t")) return int(sizeof(t2_dbg_act_t));
+  if (!strcmp(name, "t2_dbg_gemm_t")) return int(sizeof(t2_dbg_gemm_t));
+  if (!strcmp(name, "t2_dbg_wgrad_tile_t")) return int(sizeof(t2_dbg_wgrad_tile_t));
   return -1;
 }

@@ -126,15 +126,51 @@ __device__ __host__ __forceinline__ bool hash_keep16(uint32_t hs, uint64_t idx, 
 }
 
 // Order-independent accumulation of float contributions from many threads / blocks: each addend becomes a 64-bit fixed-point
-// integer (resolution 2^-40, range +-2^23) and integer atomics sum them, so the total does not depend on the order in which
-// the contributions arrive (float atomics would make every run round differently). fx_value converts a total back.
-__device__ __forceinline__ long long fx_of(float v) {
-  return llrintf(fminf(fmaxf(v * 1099511627776.f, -9.2e18f), 9.2e18f));
+// integer (resolution 2^-40) and integer atomics sum them, so the total does not depend on the order in which the contributions
+// arrive (float atomics would make every run round differently). fx_value converts a total back.
+// Valid totals stay inside +-2^62 (+-2^22 = 4.19e6 in value), a quarter of the int64 range: adding one in-range addend to an in-range
+// total cannot wrap, so every fx_add can check the total it produced. A non-finite or out-of-range addend, or a total that leaves the
+// range, POISONS the accumulator (kFxPoison); an fx_add that finds it poisoned re-poisons it after its own add, so the poison sticks
+// whatever the order of the adds. fx_value turns a poisoned total into NaN: a NaN / Inf gradient stays non-finite, and an overflowing
+// sum never wraps into a finite value of either sign. (A sum whose partial sums leave the range but whose total returns into it may
+// come out poisoned in some orders and not in others: only gradients beyond 4e6 are affected.)
+constexpr long long kFxPoison = -0x7fffffffffffffffll - 1;   // INT64_MIN
+constexpr long long kFxRange = 1ll << 62;
+__device__ __forceinline__ bool fx_in_range(long long a) { return a > -kFxRange && a < kFxRange; }
+// fx_add in two halves: fx_issue starts the atomic add, fx_check looks at the total it returned. A thread that adds several values
+// issues them all before it checks any, so that their round trips overlap instead of queueing one behind the other.
+struct FxAdd {
+  unsigned long long* d;
+  long long a, old;
+};
+__device__ __forceinline__ FxAdd fx_issue(long long* dst, float v) {
+  FxAdd x{reinterpret_cast<unsigned long long*>(dst), 0, 0};
+  if (!(fabsf(v) < 4194304.f)) {   // NaN, +-Inf, |v| >= 2^22
+    x.old = kFxPoison;
+  } else {
+    x.a = llrintf(v * 1099511627776.f);
+    x.old = static_cast<long long>(atomicAdd(x.d, static_cast<unsigned long long>(x.a)));
+  }
+  return x;
 }
-__device__ __forceinline__ void fx_add(long long* dst, float v) {
-  atomicAdd(reinterpret_cast<unsigned long long*>(dst), static_cast<unsigned long long>(fx_of(v)));
+// a fixed-point TOTAL (a block's partial sum, itself built with fx_add) merged into dst: a poisoned or out-of-range total poisons dst
+__device__ __forceinline__ FxAdd fx_issue_total(long long* dst, long long v) {
+  FxAdd x{reinterpret_cast<unsigned long long*>(dst), 0, kFxPoison};
+  if (fx_in_range(v)) {
+    x.a = v;
+    x.old = static_cast<long long>(atomicAdd(x.d, static_cast<unsigned long long>(v)));
+  }
+  return x;
 }
-__device__ __forceinline__ float fx_value(long long a) { return float(double(a) * (1.0 / 1099511627776.0)); }
+__device__ __forceinline__ void fx_check(const FxAdd& x) {
+  if (!fx_in_range(x.old) || !fx_in_range(x.old + x.a)) atomicExch(x.d, static_cast<unsigned long long>(kFxPoison));
+}
+__device__ __forceinline__ void fx_add(long long* dst, float v) { fx_check(fx_issue(dst, v)); }
+__device__ __forceinline__ float fx_value(long long a) {
+  return fx_in_range(a) ? float(double(a) * (1.0 / 1099511627776.0)) : __int_as_float(0x7fffffff);
+}
+// host launcher of the kernel that adds the fixed-point totals acc[0, n) to the fp32 gradients out[0, n) (t2_wavenet.cu)
+int launch_fx_finalize(const long long* acc, float* out, long long n, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------
 // mbarrier

@@ -103,8 +103,8 @@ int cluster_pref() {
   }
   return v;
 }
-static int pick_cluster(int BN, const dim3& grid) {
-  int cs = cluster_pref();
+static int pick_cluster(int BN, const dim3& grid, int request) {
+  int cs = request ? request : cluster_pref();
   if (BN < 128 || grid.z > 1) return 1;                 // the swapped recurrence GEMMs (BN = 32) and split-K keep single CTAs
   while (cs > 1 && (grid.x % cs != 0 || (BN / cs) % 8 != 0)) cs >>= 1;
   return cs;
@@ -137,14 +137,40 @@ static int launch_one(const GemmArgs& g, dim3 grid, int cs, cudaStream_t stream)
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
+  if (cs > 1) {   // a cluster size the device cannot co-schedule is refused here, not at launch
+    static int max_clusters[4] = {-1, -1, -1, -1};
+    int& mc = max_clusters[cs == 2 ? 1 : cs == 4 ? 2 : 3];
+    if (mc < 0) T2_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&mc, act_gemm_kernel<EPI, BN>, &cfg));
+    T2_REQUIRE(mc > 0, T2_ERR_UNSUPPORTED_SHAPE, "act_gemm: clusters of %d CTAs cannot be scheduled on this device", cs);
+  }
   T2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, act_gemm_kernel<EPI, BN>, g));
   t2_count_launch();
   return T2_OK;
 }
 
-int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) {
+int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used) {
+  // argument checks first: they touch neither the device nor the driver
   T2_REQUIRE(c.na >= 1 && c.na <= 4 && c.nseg >= 1 && c.nseg <= kMaxSeg, T2_ERR_INVALID_ARG,
              "act_gemm: bad map/segment count (%d, %d)", c.na, c.nseg);
+  T2_REQUIRE(c.cluster == 0 || c.cluster == 1 || c.cluster == 2 || c.cluster == 4 || c.cluster == 8, T2_ERR_INVALID_ARG,
+             "act_gemm: cluster size must be 0 (default), 1, 2, 4 or 8 (got %d)", c.cluster);
+  int ktot = 0;
+  for (int s = 0; s < c.nseg; ++s) {
+    T2_REQUIRE(c.seg[s].map >= 0 && c.seg[s].map < c.na && c.seg[s].nkb > 0 && c.seg[s].nlayers > 0,
+               T2_ERR_INVALID_ARG, "act_gemm: bad segment %d", s);
+    ktot += c.seg[s].nkb * c.seg[s].nlayers * kBK;
+  }
+  T2_REQUIRE(c.w_k0 + ktot <= ((c.wK + kBK - 1) / kBK) * kBK, T2_ERR_INVALID_ARG,
+             "act_gemm: segments cover K=%d but packed weight has K=%d", ktot, c.wK);
+  if (c.ksplit > 1) {
+    T2_REQUIRE(epi == EPI_TOUT && c.ksplit * kBK <= ktot, T2_ERR_INVALID_ARG,
+               "act_gemm: split-K needs an atomically accumulating epilogue and at least one k-block per slice");
+    // the CTAs of one output tile add their partial sums into the same elements: only the atomic mode (2) is race-free
+    const bool use0 = c.epi.ptr[0] && c.epi.i[0] > 0, use1 = c.epi.ptr[1] && c.epi.i[3] > c.epi.i[0];
+    T2_REQUIRE((!use0 || c.epi.i[2] == 2) && (!use1 || c.epi.i[5] == 2), T2_ERR_INVALID_ARG,
+               "act_gemm: split-K needs atomic accumulation (mode 2) into every destination in use (modes %d, %d)", c.epi.i[2],
+               c.epi.i[5]);
+  }
   GemmArgs g;
   memset(&g, 0, sizeof(g));
   for (int i = 0; i < 4; ++i) {
@@ -152,19 +178,11 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) 
     if (rc) return rc;
   }
   dim3 grid((c.T + kBM - 1) / kBM * c.B, c.n_tiles, c.ksplit > 1 ? c.ksplit : 1);
-  const int cs = pick_cluster(BN, grid);
+  const int cs = pick_cluster(BN, grid, c.cluster);
   // weight-tile rows one TMA box fetches: 1/cs of the tile per CTA of a multicast cluster
   int rc = encode_wt_map(&g.bmap, c.w, c.wN, c.wK, c.wL, BN / cs);
   if (rc) return rc;
-  int ktot = 0;
-  for (int s = 0; s < c.nseg; ++s) {
-    g.seg[s] = c.seg[s];
-    T2_REQUIRE(c.seg[s].map >= 0 && c.seg[s].map < c.na && c.seg[s].nkb > 0 && c.seg[s].nlayers > 0,
-               T2_ERR_INVALID_ARG, "act_gemm: bad segment %d", s);
-    ktot += c.seg[s].nkb * c.seg[s].nlayers * kBK;
-  }
-  T2_REQUIRE(c.w_k0 + ktot <= ((c.wK + kBK - 1) / kBK) * kBK, T2_ERR_INVALID_ARG,
-             "act_gemm: segments cover K=%d but packed weight has K=%d", ktot, c.wK);
+  for (int s = 0; s < c.nseg; ++s) g.seg[s] = c.seg[s];
   g.nseg = c.nseg;
   g.T = c.T;
   g.tiles_per_b = (c.T + kBM - 1) / kBM;
@@ -186,10 +204,7 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream) 
         if (rc) return rc;
       }
   }
-  if (c.ksplit > 1) {
-    T2_REQUIRE(epi == EPI_TOUT && c.ksplit * kBK <= ktot, T2_ERR_INVALID_ARG,
-               "act_gemm: split-K needs an atomically accumulating epilogue and at least one k-block per slice");
-  }
+  if (cluster_used) *cluster_used = cs;
 #define T2_CASE(E, N) \
   if (epi == E && BN == N) return launch_one<E, N>(g, grid, cs, stream);
   T2_CASE(EPI_GATE, 256)

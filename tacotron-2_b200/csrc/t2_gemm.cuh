@@ -826,12 +826,16 @@ struct Epilogue<EPI_GATE_BWD, BN> {
       if (e.ptr[3]) {
         const float ca = warp_colsum32(a, c.lane), cb2 = warp_colsum32(s, c.lane);
         const int col = cb + cq * 32 + colsum32_col(c.lane);
-        fx_add(static_cast<long long*>(e.ptr[3]) + col, ca);
-        fx_add(static_cast<long long*>(e.ptr[3]) + Gh + col, cb2);
+        const FxAdd x0 = fx_issue(static_cast<long long*>(e.ptr[3]) + col, ca);
+        const FxAdd x1 = fx_issue(static_cast<long long*>(e.ptr[3]) + Gh + col, cb2);
         if (e.ptr[4]) {
-          fx_add(static_cast<long long*>(e.ptr[4]) + col, ca);
-          fx_add(static_cast<long long*>(e.ptr[4]) + Gh + col, cb2);
+          const FxAdd x2 = fx_issue(static_cast<long long*>(e.ptr[4]) + col, ca);
+          const FxAdd x3 = fx_issue(static_cast<long long*>(e.ptr[4]) + Gh + col, cb2);
+          fx_check(x2);
+          fx_check(x3);
         }
+        fx_check(x0);
+        fx_check(x1);
       }
     }
   }

@@ -28,6 +28,7 @@ struct ActGemmCall {
   int T, B;
   int n_tiles;     // grid.y
   int ksplit;      // grid.z: CTAs sharing one output tile over slices of K (0/1 = off; epilogue must accumulate atomically)
+  int cluster;     // requested weight-multicast cluster size along M: 0 = T2_CLUSTER / default, else 1, 2, 4 or 8
   EpiArgs epi;
 };
 
@@ -46,7 +47,8 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
-int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream);
+// *cluster_used (nullable) receives the cluster size the kernel was launched with
+int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used = nullptr);
 int launch_wgrad(const ActT* maps, int nmaps, const WgradTile* tiles_dev, int ntiles, float* out,
                  int T, int B, cudaStream_t stream);
 

@@ -478,9 +478,16 @@ __global__ void first_conv_bwd_kernel(const void* __restrict__ xin, int scalar_i
       acc += static_cast<const float*>(xin)[p0 + i] * __bfloat162float(dx0[(p0 + i) * R + r]);
     fx_add(dW + r, acc);
   } else {
-    for (int i = 0; i < 64 && p0 + i < npos; ++i) {
-      const int idx = static_cast<const int*>(xin)[p0 + i];
-      fx_add(dW + (long long)idx * R + r, __bfloat162float(dx0[(p0 + i) * R + r]));
+    const int n = npos - p0 < 64 ? int(npos - p0) : 64;
+    for (int i0 = 0; i0 < n; i0 += 8) {
+      FxAdd x[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (i0 + i < n)
+          x[i] = fx_issue(dW + (long long)static_cast<const int*>(xin)[p0 + i0 + i] * R + r, __bfloat162float(dx0[(p0 + i0 + i) * R + r]));
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (i0 + i < n) fx_check(x[i]);
     }
   }
 }
@@ -510,11 +517,19 @@ __global__ void colsum_kernel(const uint8_t* __restrict__ ws, long long* __restr
       a0 += bf16lo(u); a1 += bf16hi(u);
     }
     a0 *= sc; a1 *= sc;
-    fx_add(grads + j.dst_off + c, a0);
-    if (c + 1 < j.C) fx_add(grads + j.dst_off + c + 1, a1);
-    if (j.dst2_off >= 0) {
-      fx_add(grads + j.dst2_off + c, a0);
-      if (c + 1 < j.C) fx_add(grads + j.dst2_off + c + 1, a1);
+    const bool two = c + 1 < j.C, dup = j.dst2_off >= 0;
+    FxAdd x[4];
+    x[0] = fx_issue(grads + j.dst_off + c, a0);
+    if (two) x[1] = fx_issue(grads + j.dst_off + c + 1, a1);
+    if (dup) {
+      x[2] = fx_issue(grads + j.dst2_off + c, a0);
+      if (two) x[3] = fx_issue(grads + j.dst2_off + c + 1, a1);
+    }
+    fx_check(x[0]);
+    if (two) fx_check(x[1]);
+    if (dup) {
+      fx_check(x[2]);
+      if (two) fx_check(x[3]);
     }
   }
 }
@@ -620,17 +635,21 @@ __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const fl
       }
     }
   }
+  FxAdd x[10];
 #pragma unroll
   for (int i = 0; i < 9; ++i)
-    if (i < ntap && r[i] != 0.f) fx_add(&acc[i * s + k], r[i]);
-  if (r[9] != 0.f) fx_add(&acc[ntap * s + k], r[9]);
+    if (i < ntap && r[i] != 0.f) x[i] = fx_issue(&acc[i * s + k], r[i]);
+  if (r[9] != 0.f) x[9] = fx_issue(&acc[ntap * s + k], r[9]);
+#pragma unroll
+  for (int i = 0; i < 9; ++i)
+    if (i < ntap && r[i] != 0.f) fx_check(x[i]);
+  if (r[9] != 0.f) fx_check(x[9]);
   __syncthreads();
   for (int i = threadIdx.x; i < (ntap + 1) * s; i += blockDim.x) {
-    const unsigned long long v = static_cast<unsigned long long>(acc[i]);
+    const long long v = acc[i];
     if (v == 0) continue;
-    if (i < ntap * s) atomicAdd(reinterpret_cast<unsigned long long*>(dK + i), v);
-    else if (type == 0) atomicAdd(reinterpret_cast<unsigned long long*>(dbias + (i - ntap * s)), v);
-    else atomicAdd(reinterpret_cast<unsigned long long*>(dbias), v);
+    // checked merge: two poisoned block totals must not cancel, in-range totals must not wrap
+    fx_check(fx_issue_total(i < ntap * s ? dK + i : type == 0 ? dbias + (i - ntap * s) : dbias, v));
   }
 }
 __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const float* __restrict__ dout, int cl,
@@ -807,6 +826,14 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
 inline dim3 grid1d(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
 
 }  // namespace
+
+int launch_fx_finalize(const long long* acc, float* out, long long n, cudaStream_t st) {
+  if (n <= 0) return T2_OK;
+  fx_finalize_kernel<<<unsigned((n + 255) / 256), 256, 0, st>>>(acc, out, n);
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
 }  // namespace t2
 
 using namespace t2;
@@ -1066,11 +1093,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
       T2_CHECK_CUDA(cudaEventRecord(side->join, side->s));
       T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
     }
-    fx_finalize_kernel<<<grid1d(lo.n_params), 256, 0, st>>>(reinterpret_cast<const long long*>(static_cast<uint8_t*>(d_workspace) + lo.w_gfx),
-                                                           d_grads, lo.n_params);
-    t2_count_launch();
-    T2_CHECK_CUDA(cudaGetLastError());
-    return T2_OK;
+    return launch_fx_finalize(reinterpret_cast<const long long*>(static_cast<uint8_t*>(d_workspace) + lo.w_gfx), d_grads, lo.n_params, st);
   }
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
@@ -1208,9 +1231,8 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
   }
   if (phase == -1) {   // (phased: once the side stream has joined, in phase 100)
-    fx_finalize_kernel<<<grid1d(lo.n_params), 256, 0, st>>>(gfx, d_grads, lo.n_params);
-    t2_count_launch();
-    T2_CHECK_CUDA(cudaGetLastError());
+    const int rc = launch_fx_finalize(gfx, d_grads, lo.n_params, st);
+    if (rc) return rc;
   }
   return T2_OK;
 }

@@ -43,3 +43,31 @@ def ptr(t):
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+# ---- mirrors of the engine-level test structs of include/t2b200.h (t2_dbg_act_gemm / t2_dbg_wgrad_tiles) ----
+class DbgAct(ctypes.Structure):
+    _fields_ = [("ptr", ctypes.c_void_p), ("C", ctypes.c_int), ("T", ctypes.c_int), ("B", ctypes.c_int), ("L", ctypes.c_int),
+                ("ld", ctypes.c_int)]
+
+
+class DbgSeg(ctypes.Structure):
+    _fields_ = [("map", ctypes.c_int), ("shift", ctypes.c_int), ("k0", ctypes.c_int), ("nkb", ctypes.c_int),
+                ("layer0", ctypes.c_int), ("nlayers", ctypes.c_int)]
+
+
+class DbgGemm(ctypes.Structure):
+    _fields_ = [("a", DbgAct * 4), ("na", ctypes.c_int),
+                ("seg", DbgSeg * 16), ("nseg", ctypes.c_int),
+                ("w", ctypes.c_void_p), ("wN", ctypes.c_int), ("wK", ctypes.c_int), ("wL", ctypes.c_int),
+                ("w_layer", ctypes.c_int), ("w_k0", ctypes.c_int),
+                ("T", ctypes.c_int), ("B", ctypes.c_int), ("n_tiles", ctypes.c_int), ("ksplit", ctypes.c_int),
+                ("epi", ctypes.c_int), ("BN", ctypes.c_int), ("cluster", ctypes.c_int), ("cluster_used", ctypes.c_int),
+                ("ptr", ctypes.c_void_p * 12), ("f", ctypes.c_float * 6), ("i", ctypes.c_int * 12), ("seed", ctypes.c_ulonglong)]
+
+
+class DbgWgradTile(ctypes.Structure):
+    _fields_ = [("a_map", ctypes.c_int), ("a_ch0", ctypes.c_int), ("a_shift", ctypes.c_int), ("a_layer", ctypes.c_int),
+                ("b_map", ctypes.c_int), ("b_ch0", ctypes.c_int), ("b_shift", ctypes.c_int), ("b_layer", ctypes.c_int),
+                ("out_off", ctypes.c_longlong), ("ldc", ctypes.c_int), ("m_valid", ctypes.c_int), ("n_valid", ctypes.c_int),
+                ("scale", ctypes.c_float), ("accumulate", ctypes.c_int), ("div", ctypes.c_void_p)]

@@ -156,7 +156,63 @@ def test_ctypes_struct_mirrors_match_the_library():
     lib = t2.lib.load()
     lib.t2_struct_size.argtypes = [ctypes.c_char_p]
     pairs = {"t2_wn_config_t": t2.wavenet.WnConfig, "t2_wn_sizes_t": t2.wavenet.WnSizes, "t2_taco_config_t": t2.tacotron.TacoConfig,
-             "t2_cbhg_config_t": t2.tacotron.CbhgConfig, "t2_audio_config_t": t2.audio.AudioConfig}
+             "t2_cbhg_config_t": t2.tacotron.CbhgConfig, "t2_audio_config_t": t2.audio.AudioConfig,
+             "t2_dbg_act_t": t2.lib.DbgAct, "t2_dbg_gemm_t": t2.lib.DbgGemm, "t2_dbg_wgrad_tile_t": t2.lib.DbgWgradTile}
     for name, mirror in pairs.items():
         assert lib.t2_struct_size(name.encode()) == ctypes.sizeof(mirror), name
     assert lib.t2_struct_size(b"nope") == -1
+
+
+def test_split_k_rejects_non_atomic_output_modes():
+    """Split-K makes several CTAs add partial sums into the same output elements, so every destination in use must take mode 2
+    (atomic add). The check runs before any driver call. Nothing is launched: the rejected calls stop at the split-K check, and the
+    calls that pass it have a null weight pointer, which the weight tensor-map encoding refuses before any launch (on a host without a
+    driver the activation map encoding already fails). The fake pointers are never dereferenced."""
+    from t2_import import t2
+    lib = t2.lib.load()
+    EPI_TOUT = 9
+    fake = 1 << 20                                     # 16-byte aligned, never touched
+
+    def call(ksplit, mode0, mode1, dst1=True, rows0=64, rows1=128, epi=EPI_TOUT, w=fake):
+        c = t2.lib.DbgGemm()
+        c.a[0] = t2.lib.DbgAct(fake, 512, 128, 1, 1, 512)
+        c.na = 1
+        c.seg[0] = t2.lib.DbgSeg(0, 0, 0, 8, 0, 1)
+        c.nseg = 1
+        c.w, c.wN, c.wK, c.wL = w, 32, 512, 1
+        c.T, c.B, c.n_tiles, c.ksplit, c.epi, c.BN = 128, 1, 1, ksplit, epi, 32
+        c.ptr[0], c.ptr[1] = fake, (fake if dst1 else None)
+        c.i[0], c.i[1], c.i[2], c.i[3], c.i[4], c.i[5], c.i[6] = rows0, 32, mode0, rows1, 32, mode1, 32
+        return lib.t2_dbg_act_gemm(ctypes.byref(c), None)
+
+    for m0, m1 in [(0, 2), (1, 2), (2, 0), (2, 1), (0, 0), (1, 1)]:
+        rc = call(4, m0, m1)
+        assert rc == -1, (m0, m1, rc)
+        assert b"split-K" in lib.t2_last_error(), lib.t2_last_error()
+    # accepted by the split-K check (an unused destination's mode is not checked), then refused for the null weight pointer
+    for kw in (dict(dst1=False), dict(rows1=64), {}):
+        mode1 = 2 if not kw else 0
+        rc = call(4, 2, mode1, w=None, **kw)
+        assert rc != 0 and b"split-K" not in lib.t2_last_error(), (kw, rc, lib.t2_last_error())
+    assert call(4, 2, 2, epi=2) == -1 and b"split-K" in lib.t2_last_error()           # split-K with a non-accumulating epilogue
+    assert call(16, 2, 2) == -1 and b"split-K" in lib.t2_last_error()                  # fewer k-blocks (8) than slices
+
+
+def test_act_gemm_rejects_bad_cluster_and_segments():
+    """argument checks of the engine hook that need no device"""
+    from t2_import import t2
+    lib = t2.lib.load()
+    fake = 1 << 20
+    c = t2.lib.DbgGemm()
+    c.a[0] = t2.lib.DbgAct(fake, 64, 128, 1, 1, 64)
+    c.na, c.nseg = 1, 1
+    c.seg[0] = t2.lib.DbgSeg(0, 0, 0, 1, 0, 1)
+    c.w, c.wN, c.wK, c.wL = fake, 128, 64, 1
+    c.T, c.B, c.n_tiles, c.epi, c.BN = 128, 1, 1, 2, 128
+    c.cluster = 3
+    assert lib.t2_dbg_act_gemm(ctypes.byref(c), None) == -1 and b"cluster" in lib.t2_last_error()
+    c.cluster = 0
+    c.seg[0] = t2.lib.DbgSeg(1, 0, 0, 1, 0, 1)                 # map 1 of 1
+    assert lib.t2_dbg_act_gemm(ctypes.byref(c), None) == -1 and b"segment" in lib.t2_last_error()
+    c.seg[0] = t2.lib.DbgSeg(0, 0, 0, 2, 0, 1)                 # 2 k-blocks, weight has 1
+    assert lib.t2_dbg_act_gemm(ctypes.byref(c), None) == -1 and b"packed weight" in lib.t2_last_error()

@@ -185,3 +185,32 @@ def test_dropout_statistics_and_determinism():
     torch.cuda.synchronize()
     kept2 = model.workspace_tensor("xd", (hp.layers, B, T, 128)).float() != 0
     assert (kept2 != kept).float().mean().item() > 0.2   # a different seed draws different masks
+
+
+@pytest.mark.parametrize("upsample_type", ["SubPixel", "2D"])
+def test_nan_loss_gives_non_finite_block_summed_gradients(upsample_type):
+    """A NaN in the output-layer bias makes the loss and every upstream gradient NaN, except where a ReLU mask selects an exact zero
+    (a unit dead at every position gets a zero gradient, as from the reference's ReluGrad). The gradients that many blocks add up as
+    fixed point (biases, first conv, upsampling net) must follow the same rule: a NaN never becomes a finite non-zero number, and two
+    NaN block totals of the upsampling backward must not cancel. Both upsampling nets are run with an even scale."""
+    hp = _hp(input_type="mulaw-quantize", quantize_channels=256, out_channels=256, upsample_type=upsample_type)
+    B, T = 2, 256
+    params = ow.init_params(hp, seed=3, random_bias=True)
+    params["final_convolution_2/bias"][5] = float("nan")
+    x, c, y, lengths, xd, yd = _inputs(hp, B, T, 3)
+    model = t2.wavenet.WaveNet(hp, B, T)
+    model.load_params(params)
+    model.forward(xd.cuda(), c.cuda(), yd.cuda(), lengths.int().cuda())
+    model.backward()
+    torch.cuda.synchronize()
+    assert not math.isfinite(model.loss_value())
+    grads = model.export_grads()
+    finite = {name: int(torch.isfinite(g).sum()) for name, g in grads.items()}
+    finite_nonzero = {name: int((torch.isfinite(g) & (g != 0)).sum()) for name, g in grads.items()}
+    record("wavenet_nan_loss_%s" % upsample_type, finite_elements=sum(finite.values()), finite_nonzero=sum(finite_nonzero.values()))
+    bad = {name: n for name, n in finite_nonzero.items() if n}
+    assert not bad, "finite non-zero gradient elements under a NaN loss: %s" % bad
+    up = [n for n in grads if n.startswith("local_conditioning_upsampling")]
+    assert len(up) == 4
+    for name in up:
+        assert finite[name] == 0, "%s: %d of %d elements finite" % (name, finite[name], grads[name].numel())
