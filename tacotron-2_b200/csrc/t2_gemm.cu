@@ -93,7 +93,9 @@ bool pdl_enabled() {
   return v != 0;
 }
 
-// cluster size along M for the weight-tile multicast (T2_CLUSTER in the environment; default 1 = off)
+// cluster size along M for the weight-tile multicast (T2_CLUSTER in the environment, for A/B measurements; default 1 = off).
+// Multicast stays off by default: with the 4-stage ring, clusters of 2 and 4 made every WaveNet GEMM shape slower on an H100
+// (DESIGN §4).
 int cluster_pref() {
   static int v = -1;
   if (v < 0) {

@@ -88,22 +88,18 @@ __device__ __forceinline__ void load_split32(const __nv_bfloat16* src_hi, const 
 
 // ------------------------------------------------------------------------------------------------
 // Epilogue staging: a thread owns one accumulator ROW, but global memory wants a warp to touch one
-// row's contiguous bytes. Every epilogue therefore moves 32-row x 128-column bf16 tiles through a per-warp
-// shared-memory tile (the pipeline stages are free once the last MMA has committed): rows are written / read by
-// their owning lane, global traffic is issued with 16 lanes covering one 256-byte row segment.
+// row's contiguous bytes. Every epilogue therefore moves 32-row x 128-column bf16 tiles through shared-memory tiles of its
+// row quarter: rows are written / read by their owning lane, global traffic is issued with 16 lanes covering one 256-byte row.
+// A staged tile is two 64-column boxes of 32 rows x 128 bytes in the 128-byte swizzle (16-byte chunk index XOR row % 8) the
+// output tensor maps are encoded with, so one elected thread per row quarter can hand a finished tile to the TMA engine
+// (EPI_GATE / EPI_RES / EPI_GATE_BWD / EPI_DX) instead of 4 warps copying it out through registers.
+// Each quarter has three tiles (EpiCtx::tile). Tile 2 is dedicated shared memory: it is the only one an epilogue's prefetch()
+// may fill while the mainloop runs. Tiles 0 and 1 are the tail of the pipeline ring, past the fp32 accumulator tile, and exist
+// only in run(). The TMA-store epilogues rotate the three: a tile is rewritten two stores after its own (see tile_store).
 // ------------------------------------------------------------------------------------------------
-constexpr int kTilePitch = 256 + 16;              // bytes per staged row: 128 bf16 + 16 B pad (bank spread)
-constexpr int kTileBytes = 32 * kTilePitch;       // 8704
-constexpr int kEpiTilesPerWarp = 2;          // dedicated staging (not aliased with the pipeline stages)
-// TMA-store staging (EPI_GATE / EPI_RES / EPI_GATE_BWD / EPI_DX): a staged 32-row x 128-column bf16 tile is two 64-column boxes of
-// 32 rows x 128 bytes in the 128-byte swizzle (16-byte chunk index XOR row % 8) the output tensor maps are encoded with, so one
-// elected thread per row quarter hands a finished tile to the TMA engine instead of 4 warps copying it out through registers.
-// Three tiles per quarter rotate: a tile is rewritten two stores after its own (see tile_store).
 constexpr int kSBoxBytes = 32 * 128;
 constexpr int kSTileBytes = 2 * kSBoxBytes;
 constexpr int kSTiles = 3;
-constexpr int kEpiWarpBytes = kSTiles * kSTileBytes;     // 24 KB per row quarter (also covers the 2 x 8704-byte pitch-272 tiles)
-static_assert(kEpiWarpBytes >= kEpiTilesPerWarp * kTileBytes && kEpiWarpBytes % 1024 == 0, "staging size / swizzle-atom alignment");
 
 constexpr int kActEpiWarps = 16;                               // 4 row quarters x 4 column groups
 constexpr int kActGemmThreads = 32 * kActEpiWarps + 32;        // + producer warp
@@ -117,37 +113,16 @@ struct EpiCtx {
   size_t row0;             // b*T + (first time step of this warp)
   int nrows;               // valid rows among this warp's 32
   AccRow trow;             // this thread's row of the accumulator tile, column 0
-  uint8_t* wbuf;           // kEpiWarpBytes of shared memory shared by the 4 warps of this row quarter
-  uint8_t* smem_all;       // start of the (free after the mainloop) pipeline shared memory, CTA-wide scratch
+  uint8_t* stg;            // staging tile 0 of this row quarter; tile k is at stg + k * 4 * kSTileBytes (see tile())
+  uint8_t* smem_all;       // CTA-wide scratch that is free after the mainloop (the pipeline ring past the accumulator tile)
   int m_tile;              // index of this CTA's 128-row tile
   const CUtensorMap* omap; // output tensor maps (GemmArgs::omap) of the TMA-store epilogues
   int tq;                  // first time step of this row quarter (row coordinate of its stores)
   mutable int sk;          // stores issued so far by this quarter (tile rotation)
+  // staging tile k (0..2) of this row quarter; only tile 2 may be used by prefetch()
+  __device__ __forceinline__ uint8_t* tile(int k) const { return stg + k * (4 * kSTileBytes); }
 };
 
-__device__ __forceinline__ void stage_put(uint8_t* tile, int lane, int cq, const float (&v)[32]) {
-  uint4* d = reinterpret_cast<uint4*>(tile + lane * kTilePitch + cq * 64);
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 u;
-    u.x = pack_bf16x2(v[q * 8 + 0], v[q * 8 + 1]);
-    u.y = pack_bf16x2(v[q * 8 + 2], v[q * 8 + 3]);
-    u.z = pack_bf16x2(v[q * 8 + 4], v[q * 8 + 5]);
-    u.w = pack_bf16x2(v[q * 8 + 6], v[q * 8 + 7]);
-    d[q] = u;
-  }
-}
-__device__ __forceinline__ void stage_get(const uint8_t* tile, int lane, int cq, float (&v)[32]) {
-  const uint4* s = reinterpret_cast<const uint4*>(tile + lane * kTilePitch + cq * 64);
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const uint4 u = s[q];
-    v[q * 8 + 0] = bf16lo(u.x); v[q * 8 + 1] = bf16hi(u.x);
-    v[q * 8 + 2] = bf16lo(u.y); v[q * 8 + 3] = bf16hi(u.y);
-    v[q * 8 + 4] = bf16lo(u.z); v[q * 8 + 5] = bf16hi(u.z);
-    v[q * 8 + 6] = bf16lo(u.w); v[q * 8 + 7] = bf16hi(u.w);
-  }
-}
 __device__ __forceinline__ void quarter_sync(int id) {
   asm volatile("bar.sync %0, 128;\n" ::"r"(id) : "memory");
 }
@@ -159,10 +134,14 @@ __device__ __forceinline__ void load_f32x32(const float* p, float (&v)[32]) {
     v[q * 4] = f.x; v[q * 4 + 1] = f.y; v[q * 4 + 2] = f.z; v[q * 4 + 3] = f.w;
   }
 }
+// ---- swizzled staging tiles ----------------------------------------------------------------------
+__device__ __forceinline__ uint8_t* sw_addr(uint8_t* tile, int row, int chunk) {   // chunk: 16-byte column chunk 0..15 of the 128 columns
+  return tile + (chunk >> 3) * kSBoxBytes + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
+}
 // smem tile -> global rows g + r*ld (elements), 128 columns each; rows >= nrows are skipped.
 // NW warps cooperate (each moves 32/NW rows); with NW == 4 the quarter barrier orders it after every warp's puts.
 template <int NW>
-__device__ __forceinline__ void tile_flush(const uint8_t* tile, __nv_bfloat16* g, size_t ld, int nrows, const EpiCtx& c) {
+__device__ __forceinline__ void tile_flush(uint8_t* tile, __nv_bfloat16* g, size_t ld, int nrows, const EpiCtx& c) {
   if (NW == 4) quarter_sync(c.qbar); else __syncwarp();
   const int ch = c.lane & 15, rh = c.lane >> 4;
   const int it0 = NW == 4 ? c.cg * 4 : 0;
@@ -170,28 +149,9 @@ __device__ __forceinline__ void tile_flush(const uint8_t* tile, __nv_bfloat16* g
   for (int i = 0; i < 16 / NW; ++i) {
     const int r = (it0 + i) * 2 + rh;
     if (r < nrows)
-      *reinterpret_cast<uint4*>(g + size_t(r) * ld + ch * 8) = *reinterpret_cast<const uint4*>(tile + r * kTilePitch + ch * 16);
+      *reinterpret_cast<uint4*>(g + size_t(r) * ld + ch * 8) = *reinterpret_cast<const uint4*>(sw_addr(tile, r, ch));
   }
   if (NW == 4) quarter_sync(c.qbar); else __syncwarp();
-}
-// global rows -> smem tile (rows >= nrows are zero-filled)
-template <int NW>
-__device__ __forceinline__ void tile_fill(uint8_t* tile, const __nv_bfloat16* g, size_t ld, int nrows, const EpiCtx& c) {
-  const int ch = c.lane & 15, rh = c.lane >> 4;
-  const int it0 = NW == 4 ? c.cg * 4 : 0;
-#pragma unroll
-  for (int i = 0; i < 16 / NW; ++i) {
-    const int r = (it0 + i) * 2 + rh;
-    uint4 u = make_uint4(0, 0, 0, 0);
-    if (r < nrows) u = __ldg(reinterpret_cast<const uint4*>(g + size_t(r) * ld + ch * 8));
-    *reinterpret_cast<uint4*>(tile + r * kTilePitch + ch * 16) = u;
-  }
-  if (NW == 4) quarter_sync(c.qbar); else __syncwarp();
-}
-
-// ---- swizzled staging + TMA store ----------------------------------------------------------------
-__device__ __forceinline__ uint8_t* sw_addr(uint8_t* tile, int row, int chunk) {   // chunk: 16-byte column chunk 0..15 of the 128 columns
-  return tile + (chunk >> 3) * kSBoxBytes + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
 }
 __device__ __forceinline__ void stage_put_sw(uint8_t* tile, int lane, int cq, const float (&v)[32]) {
 #pragma unroll
@@ -347,19 +307,19 @@ struct Epilogue<EPI_GATE, 256> {
       }
       // three stores per call through the rotating tiles: tanh stash, z, sigmoid stash (omap 0 / 2 / 1)
       if (ta_o) {
-        uint8_t* t = c.wbuf + (c.sk % kSTiles) * kSTileBytes;
+        uint8_t* t = c.tile(c.sk % kSTiles);
         stage_put_sw(t, c.lane, cq, a);
         tile_store(t, c.omap + 0, cb, c);
       }
 #pragma unroll
       for (int j = 0; j < 32; ++j) a[j] *= g[j];
       {
-        uint8_t* t = c.wbuf + (c.sk % kSTiles) * kSTileBytes;
+        uint8_t* t = c.tile(c.sk % kSTiles);
         stage_put_sw(t, c.lane, cq, a);
         tile_store(t, c.omap + 2, cb, c);
       }
       if (ta_o) {
-        uint8_t* t = c.wbuf + (c.sk % kSTiles) * kSTileBytes;
+        uint8_t* t = c.tile(c.sk % kSTiles);
         stage_put_sw(t, c.lane, cq, g);
         tile_store(t, c.omap + 1, cb, c);
       }
@@ -373,13 +333,10 @@ struct Epilogue<EPI_GATE, 256> {
 // replayed CUDA graph draw fresh masks);  f0 res_scale, f1 dropout p;  i1 = layer
 template <int BN>
 struct Epilogue<EPI_RES, BN> {
-  // the x tiles (residual input) do not depend on this kernel's MMAs: load them while the mainloop runs
+  // the x tile (residual input) of column group 0 does not depend on this kernel's MMAs: load it while the mainloop runs
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     if (e.i[11]) return;   // split-bf16 mode reads x directly in run()
-    const __nv_bfloat16* x_in = static_cast<const __nv_bfloat16*>(e.ptr[0]);
-#pragma unroll
-    for (int gq = 0; gq < BN / 128; ++gq)
-      tile_fill_sw(c.wbuf + gq * kSTileBytes, x_in + c.row0 * BN + gq * 128, BN, c.nrows, c);
+    tile_fill_sw(c.tile(2), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN, BN, c.nrows, c);
   }
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int R = BN;
@@ -409,12 +366,13 @@ struct Epilogue<EPI_RES, BN> {
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
     const uint32_t hs = hash_seed(seed, uint32_t(e.i[1]));
     const size_t row = (size_t(c.b) * c.T + c.t) * R;
+    if (BN == 256) tile_fill_sw(c.tile(1), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN + 128, BN, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
-      // tiles: x of group 0 / 1 arrives in tile 0 / 1 and is replaced in place by x_out; the dropped copies go to tile 2 (group 0)
-      // and tile 0 (group 1): store order T0, T2, T1, T0 - never a tile of the two preceding stores (tile_store)
-      uint8_t* tile = c.wbuf + gq * kSTileBytes;
-      uint8_t* tile_d = c.wbuf + (gq == 0 ? 2 : 0) * kSTileBytes;
+      // tiles: x of group 0 / 1 arrives in tile 2 / 1 and is replaced in place by x_out; the dropped copies go to tile 0 (group 0)
+      // and tile 2 (group 1): store order T2, T0, T1, T2 - never a tile of the two preceding stores (tile_store)
+      uint8_t* tile = c.tile(gq == 0 ? 2 : 1);
+      uint8_t* tile_d = c.tile(gq == 0 ? 0 : 2);
       const int cq = c.cg;
       const int j0 = gq * 128 + cq * 32;
       float acc[32], x[32], bv[32];
@@ -451,7 +409,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
     const float* bias = static_cast<const float*>(e.ptr[1]);
     float* of = static_cast<float*>(e.ptr[2]);
     const size_t row = (size_t(c.b) * c.T + c.t) * ldo;
-    uint8_t* t_o = c.wbuf;
+    uint8_t* t_o = c.tile(0);
     const float pdrop = e.f[1];
     const float keep_inv = 1.f / (1.f - pdrop);
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
@@ -507,7 +465,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
           if (pdrop > 0.f) v = (hash_uniform32(hs, row + c0 + j) >= pdrop) ? v * keep_inv : 0.f;
           acc[j] = v;
         }
-        if (ob && full) stage_put(t_o, c.lane, cq, acc);
+        if (ob && full) stage_put_sw(t_o, c.lane, cq, acc);
         if (c.valid && c0 < nvalid) {
           if (of) {
             if (c0 + 32 <= nvalid) store_f32x32(of + row + c0, acc);
@@ -565,8 +523,8 @@ struct Epilogue<EPI_CE, 256> {
     float cnt = (loss != 0.f) ? 1.f : 0.f;
     if (dl) {
       const float inv = 1.f / se;
-      uint8_t* t_hi = c.wbuf;
-      uint8_t* t_lo = c.wbuf + kTileBytes;
+      uint8_t* t_hi = c.tile(0);
+      uint8_t* t_lo = c.tile(1);
 #pragma unroll 1
       for (int gq = 0; gq < 2; ++gq) {
 #pragma unroll 1
@@ -582,8 +540,8 @@ struct Epilogue<EPI_CE, 256> {
             v[j] = hi;
             lo[j] = d - hi;
           }
-          stage_put(t_hi, c.lane, cq, v);
-          stage_put(t_lo, c.lane, cq, lo);
+          stage_put_sw(t_hi, c.lane, cq, v);
+          stage_put_sw(t_lo, c.lane, cq, lo);
         }
         tile_flush<1>(t_hi, dl + c.row0 * ld + gq * 128, ld, c.nrows, c);
         tile_flush<1>(t_lo, dl + c.row0 * ld + 256 + gq * 128, ld, c.nrows, c);
@@ -751,29 +709,30 @@ struct Epilogue<EPI_MOL, 32> {
 //      3 int64 fixed-point [ldo] column sums of `out` (fx_add; nullable: bias gradient);  f0 const scale; i0 = ldo
 template <int BN>
 struct Epilogue<EPI_SCALE_RELUMASK, BN> {
+  // h of column group 0 is loaded while the mainloop runs, that of group 1 (BN = 256) after it
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     const int ldo = e.i[0];
     const __nv_bfloat16* h = static_cast<const __nv_bfloat16*>(e.ptr[1]);
-#pragma unroll
-    for (int gq = 0; gq < BN / 128; ++gq)
-      tile_fill<4>(c.wbuf + gq * kTileBytes, h + c.row0 * ldo + size_t(c.n_tile) * BN + gq * 128, ldo, c.nrows, c);
+    tile_fill_sw(c.tile(2), h + c.row0 * ldo + size_t(c.n_tile) * BN, ldo, c.nrows, c);
   }
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int ldo = e.i[0];
     __nv_bfloat16* out = static_cast<__nv_bfloat16*>(e.ptr[0]);
     float s = e.f[0];
     if (e.ptr[2]) s /= fmaxf(__ldg(static_cast<const float*>(e.ptr[2])), 1e-20f);
+    if (BN == 256)
+      tile_fill_sw(c.tile(1), static_cast<const __nv_bfloat16*>(e.ptr[1]) + c.row0 * ldo + size_t(c.n_tile) * BN + 128, ldo, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
       const size_t off = c.row0 * ldo + size_t(c.n_tile) * BN + gq * 128;
-      uint8_t* tile = c.wbuf + gq * kTileBytes;
+      uint8_t* tile = c.tile(gq == 0 ? 2 : 1);
       const int cq = c.cg;
       float acc[32], hv[32];
       acc_ld32f(c.trow + gq * 128 + cq * 32, acc);
-      stage_get(tile, c.lane, cq, hv);
+      stage_get_sw(tile, c.lane, cq, hv);
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = hv[j] > 0.f ? acc[j] * s : 0.f;
-      stage_put(tile, c.lane, cq, acc);
+      stage_put_sw(tile, c.lane, cq, acc);
       tile_flush<4>(tile, out + off, ldo, c.nrows, c);
       if (e.ptr[3]) {
         const float cs = warp_colsum32(acc, c.lane);
@@ -787,24 +746,24 @@ struct Epilogue<EPI_SCALE_RELUMASK, BN> {
 // gate-bias gradients (column sums of dg, fx_add; nullable — dilated-conv bias and cin-conv bias get the same sum); i0 = Gh
 template <int BN>
 struct Epilogue<EPI_GATE_BWD, BN> {
+  // ta of column group 0 is loaded while the mainloop runs; sb of group 0 and both inputs of group 1 after it
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     const int Gh = e.i[0];
-    const int cb = c.n_tile * BN;
-    tile_fill_sw(c.wbuf, static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * Gh + cb, Gh, c.nrows, c);
-    tile_fill_sw(c.wbuf + kSTileBytes, static_cast<const __nv_bfloat16*>(e.ptr[1]) + c.row0 * Gh + cb, Gh, c.nrows, c);
+    tile_fill_sw(c.tile(2), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * Gh + c.n_tile * BN, Gh, c.nrows, c);
   }
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int Gh = e.i[0];
     const __nv_bfloat16* ta = static_cast<const __nv_bfloat16*>(e.ptr[0]);
     const __nv_bfloat16* sb = static_cast<const __nv_bfloat16*>(e.ptr[1]);
-    uint8_t* t0 = c.wbuf;
-    uint8_t* t1 = c.wbuf + kSTileBytes;
+    uint8_t* t0 = c.tile(2);
+    uint8_t* t1 = c.tile(1);
+    tile_fill_sw(t1, sb + c.row0 * Gh + c.n_tile * BN, Gh, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
       const int cb = c.n_tile * BN + gq * 128;
       const int cq = c.cg;
       float dz[32], a[32], s[32];
-      if (gq > 0) {   // group 0 was prefetched during the mainloop; the tiles of group 0's stores must be released first
+      if (gq > 0) {   // the tiles of group 0's stores must be released before group 1's inputs overwrite them
         tile_guard(c);
         tile_fill_sw(t0, ta + c.row0 * Gh + cb, Gh, c.nrows, c);
         tile_fill_sw(t1, sb + c.row0 * Gh + cb, Gh, c.nrows, c);
@@ -849,10 +808,7 @@ template <int BN>
 struct Epilogue<EPI_DX, BN> {
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     const __nv_bfloat16* dxo = static_cast<const __nv_bfloat16*>(e.ptr[0]);
-    if (!dxo) return;
-#pragma unroll
-    for (int gq = 0; gq < BN / 128; ++gq)
-      tile_fill_sw(c.wbuf + gq * kSTileBytes, dxo + c.row0 * BN + gq * 128, BN, c.nrows, c);
+    if (dxo) tile_fill_sw(c.tile(2), dxo + c.row0 * BN, BN, c.nrows, c);   // column group 0; group 1 (BN = 256) is loaded in run()
   }
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int R = BN;
@@ -862,9 +818,10 @@ struct Epilogue<EPI_DX, BN> {
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
     const uint32_t hs = hash_seed(seed, uint32_t(e.i[1]));
     const size_t row = (size_t(c.b) * c.T + c.t) * R;
+    if (BN == 256 && dxo) tile_fill_sw(c.tile(1), dxo + c.row0 * BN + 128, BN, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
-      uint8_t* tile = c.wbuf + gq * kSTileBytes;
+      uint8_t* tile = c.tile(gq == 0 ? 2 : 1);
       const int cq = c.cg;
       const int j0 = gq * 128 + cq * 32;
       float acc[32], g[32];
@@ -1015,13 +972,17 @@ struct ActGemmCfg {
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kAccBytes = kBM * BN * 4;
-  static constexpr int kStagingBytes = 4 * kEpiWarpBytes;      // 4 row quarters x 3 store tiles, never aliased with the stages
-  static constexpr int kPipeBudget = 232448 - kStagingBytes - 1024 /*align*/ - 256 /*barriers*/;
-  // as many stages as fit next to the store staging (2 at BN = 256, 4 at 128, 6 for the narrow swapped GEMMs of the recurrences)
+  static constexpr int kEpiBytes = 4 * kSTileBytes;        // staging tile 2 of the 4 row quarters: the only bytes outside the ring
+  static constexpr int kTailBytes = 8 * kSTileBytes;       // staging tiles 0 and 1: the ring's last bytes, after the mainloop
+  static constexpr int kPipeBudget = 232448 - kEpiBytes - 1024 /*align*/ - 256 /*barriers*/;
+  // as many stages as fit (4 at BN = 256, 6 at 128 and for the narrow swapped GEMMs of the recurrences, capped at 6)
   static constexpr int kStages = kPipeBudget / kStageBytes > 6 ? 6 : kPipeBudget / kStageBytes;
-  static constexpr int kPipeBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : kAccBytes;
-  static constexpr int kSmemBytes = kPipeBytes + kStagingBytes + 1024 + 256;
-  static_assert(kStages >= 2 && kPipeBytes <= kPipeBudget, "shared memory budget");
+  // after the mainloop the ring holds the fp32 accumulator tile at its start and staging tiles 0 and 1 at its end
+  static constexpr int kPipeBytes =
+      kStages * kStageBytes > kAccBytes + kTailBytes ? kStages * kStageBytes : kAccBytes + kTailBytes;
+  static constexpr int kSmemBytes = kPipeBytes + kEpiBytes + 1024 + 256;
+  static_assert(kStages >= 2 && kPipeBytes <= kPipeBudget && kSmemBytes <= 232448, "shared memory budget");
+  static_assert(kPipeBytes % 1024 == 0, "staging tiles must be aligned to the 1024-byte swizzle atom");
 };
 
 template <int EPI, int BN>
@@ -1031,8 +992,9 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* acc_s = reinterpret_cast<float*>(smem);
-  uint8_t* staging = smem + Cfg::kPipeBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::kStagingBytes);
+  // staging tiles, tile-major over the row quarters: tiles 0 and 1 end the ring, the dedicated tile 2 follows it
+  uint8_t* staging = smem + Cfg::kPipeBytes - Cfg::kTailBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
   uint64_t* empty_bar = full_bar + Cfg::kStages;
 
   const int warp = threadIdx.x >> 5;
@@ -1111,8 +1073,8 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
     c.valid = c.t < g.T;
     c.row0 = size_t(b) * g.T + tw;
     c.nrows = g.T - tw < 0 ? 0 : (g.T - tw > 32 ? 32 : g.T - tw);
-    c.wbuf = staging + q * kEpiWarpBytes;
-    c.smem_all = staging;
+    c.stg = staging + q * kSTileBytes;
+    c.smem_all = smem + Cfg::kAccBytes;
     c.m_tile = m_tile;
     c.omap = g.omap; c.tq = tw; c.sk = 0;
     c.n_tile = blockIdx.y;
