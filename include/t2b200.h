@@ -33,7 +33,7 @@ extern "C" {
 const char* t2_last_error(void);
 int t2_abi_version(void);
 /* sizeof() of a POD struct of this header by name ("t2_wn_config_t", "t2_wn_sizes_t", "t2_taco_config_t", "t2_cbhg_config_t",
- * "t2_audio_config_t", "t2_dbg_act_t", "t2_dbg_gemm_t", "t2_dbg_wgrad_tile_t"), -1 for an unknown name: a binding asserts that its
+ * "t2_audio_config_t", "t2_dbg_act_t", "t2_dbg_gemm_t", "t2_dbg_wgrad_tile_t", "t2_dbg_kernel_t"), -1 for an unknown name: a binding asserts that its
  * mirror of the struct matches the library it loaded */
 int t2_struct_size(const char* name);
 /* kernels launched (or captured) by this library so far in this process */
@@ -103,6 +103,59 @@ int t2_dbg_wgrad_tiles(const t2_dbg_act_t* maps, int nmaps, const t2_dbg_wgrad_t
  * atomics the GEMM epilogues use, then converts the totals as the gradient finalisation does: d_out[c] = value of the total (0 for an
  * empty total). Synchronises. */
 int t2_dbg_fx_colsum(const float* d_addends, int nrows, int ncols, float* d_out, void* stream);
+
+/* One launch of a Tacotron / CBHG engine kernel on caller buffers, with the grid, block and shared-memory size of the product path
+ * (tests/test_taco_kernels_gpu.py). `kernel` selects the kernel; p / i / f carry its pointer, integer and float arguments in the order
+ * documented next to each T2_DBG_* id; seed / step feed the dropout hash. Every argument is checked before any driver call; no
+ * temporaries are allocated. Does not synchronise. */
+typedef struct {
+  int kernel;
+  void* p[16];
+  long long i[16];
+  float f[4];
+  unsigned long long seed;
+  const unsigned long long* step;   /* nullable device int64 added to seed */
+} t2_dbg_kernel_t;
+/* t2_dbg_taco_kernel ids:
+ * ATT_FWD  att_prep_kernel + att_fwd_kernel, one decoder step. p: h2out bf16 [B][ld_h2] (query source, first D used), WqT bf16 [A][D],
+ *          K fp32 [KA][F], bK [F], Wl [F][A], ba [A], U fp32 [(KA+1)][A] (out: merged filter bank), v [A], keys fp32 [B][Ti][A],
+ *          values bf16 [B][Ti][C2], lens int32 [B], cum fp32 [B][Ti] (in/out), alpha fp32 [B][Ti] (out), ctx_a bf16 (nullable),
+ *          ctx_b bf16. i: B, Ti, D, A, KA, F, C2, ld_h2, ld_a, ld_b.
+ * BN_FWD   bn_stats_kernel + bn_apply_kernel (conv-block batch norm). p: y (bf16, or fp32 when i[3]), x bf16 [rows][C] (split: [rows][2C]),
+ *          stats fp32 [4C], gamma, beta, moving mean, moving variance. i: rows, C, training, y_fp32, stream, split. f: dropout p.
+ * BN_BWD   bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: dout bf16, y bf16, stats fp32 [6C] (mean / rstd at [2C, 4C); [4C, 6C) receives
+ *          the backward sums), gamma, dpre bf16 (out), dgamma, dbeta (accumulated). i: rows, C, act, stream. f: dropout p. */
+#define T2_DBG_TACO_ATT_FWD 1
+#define T2_DBG_TACO_BN_FWD 2
+#define T2_DBG_TACO_BN_BWD 3
+/* CELL_BWD    lstm_cell_bwd_kernel, one step t. p: dh_ext fp32 [B][ld_ext] (cleared when zero_ext), dhs, dcs fp32 [B][H] (in/out), gst bf16
+ *             [B][4H] gate stash (i | j | f | o), tst bf16 [B][H] tanh(c) stash, c_prev fp32 [B][H], dg_a bf16 [B][ld_a] (out), dg_b
+ *             (nullable), lens int32 [B] (nullable). i: ld_ext, zero_ext, ld_a, ld_b, t, B, H, stream. f: zoneout rate.
+ * ATT_FINISH  att_finish_kernel + att_finish2_kernel. p: acc fp32 [B][(KA+2)][A], K [KA][F], bK [F], Wl [F][A], grads fp32 (accumulated
+ *             at the offsets), scratch fp32 [(KA+2)][A]. i: B, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba.
+ * DVALUES     dvalues_ctx_kernel. p: alpha fp32 [To][B][Ti], dctx bf16 [To][B][C2], lens int32 [B], dvalues fp32 [B][Ti][C2] (in/out).
+ *             i: B, Ti, To, C2. */
+#define T2_DBG_TACO_CELL_BWD 4
+#define T2_DBG_TACO_ATT_FINISH 5
+#define T2_DBG_TACO_DVALUES 6
+int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
+/* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
+ * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):
+ * BN_FWD       bn_stats_k (training) + bn_apply_k. p: y, xb bf16 (nullable), xf fp32 [rows][C] (nullable), add fp32 [rows][C] (nullable),
+ *              stats, gamma, beta, mm, mv. i: rows, C, ld, c0, Ct, training, y_fp32, stat_threads (128 or 256).
+ * BN_BWD       bn_bwd_stats_k + bn_bwd_apply_k. p: g, y (both bf16, or both fp32 when i[9]), stats, bsum, gamma, dpre bf16, dgamma, dbeta.
+ *              i: rows, C, ldg, ld, c0, Ct, ldd, act, stat_threads, fp32.
+ * POOL_FWD     maxpool_fwd_k. p: x bf16 [N][C], out. i: N (= B T rows), T, C.
+ * POOL_BWD     maxpool_bwd_k. p: x, dout, dx. i: N, T, C.
+ * HIGHWAY_FWD  highway_fwd_k. p: pre fp32 [N][2HU], bh, bt, h fp32 [N][HU], hf fp32, hb bf16, HT bf16 [N][2HU] (nullable). i: N, HU.
+ * HIGHWAY_BWD  highway_bwd_k. p: dh fp32, HT bf16, h fp32, dHT bf16 [N][2HU], dcarry fp32. i: N, HU. */
+#define T2_DBG_CBHG_BN_FWD 1
+#define T2_DBG_CBHG_BN_BWD 2
+#define T2_DBG_CBHG_POOL_FWD 3
+#define T2_DBG_CBHG_POOL_BWD 4
+#define T2_DBG_CBHG_HIGHWAY_FWD 5
+#define T2_DBG_CBHG_HIGHWAY_BWD 6
+int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream);
 
 
 /* ---- WaveNet vocoder: teacher-forced training path ---------------------------------------------------------

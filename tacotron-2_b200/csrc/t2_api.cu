@@ -195,5 +195,6 @@ extern "C" int t2_struct_size(const char* name) {
   if (!strcmp(name, "t2_dbg_act_t")) return int(sizeof(t2_dbg_act_t));
   if (!strcmp(name, "t2_dbg_gemm_t")) return int(sizeof(t2_dbg_gemm_t));
   if (!strcmp(name, "t2_dbg_wgrad_tile_t")) return int(sizeof(t2_dbg_wgrad_tile_t));
+  if (!strcmp(name, "t2_dbg_kernel_t")) return int(sizeof(t2_dbg_kernel_t));
   return -1;
 }

@@ -252,13 +252,16 @@ __device__ __forceinline__ float ldv(const float* p, long long i) { return p[i];
 // Batch-norm kernels work on a COLUMN SLICE [c0, c0 + C) of row-pitch-ld matrices (the conv bank keeps its K layers side by side in
 // one [N][K*CC] matrix but every layer owns its own gamma / beta / moving tensors); the statistics buffer has four sections of Ct
 // floats: sum | sum of squares | mean | rstd, indexed by the absolute column.
+// The sums are shifted by the column's first row (y - y[0]), which keeps the variance free of the E[y^2] - mean^2 cancellation
+// when |mean| >> std.
 template <typename TY>
 __global__ void bn_stats_k(const TY* __restrict__ y, int ld, int c0, float* __restrict__ stats, int Ct, long long rows, int C) {
   const long long per = (rows + gridDim.x - 1) / gridDim.x;
   const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float pv = ldv(y, c0 + c);
     float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) { const float v = ldv(y, r * ld + c0 + c); s += v; q += v * v; }
+    for (long long r = r0; r < r1; ++r) { const float v = ldv(y, r * ld + c0 + c) - pv; s += v; q += v * v; }
     atomicAdd(stats + c0 + c, s); atomicAdd(stats + Ct + c0 + c, q);
   }
 }
@@ -275,8 +278,9 @@ __global__ void bn_apply_k(const TY* __restrict__ y, int ld, int c0, bf16* __res
   const long long r = e / C;
   float mean, rstd;
   if (training) {
-    mean = stats[c0 + c] / float(rows);
-    const float var = fmaxf(stats[Ct + c0 + c] / float(rows) - mean * mean, 0.f);
+    const float d = stats[c0 + c] / float(rows);
+    mean = ldv(y, c0 + c) + d;
+    const float var = fmaxf(stats[Ct + c0 + c] / float(rows) - d * d, 0.f);
     rstd = rsqrtf(var + 1e-3f);
     if (e < C) {
       stats[2 * Ct + c0 + c] = mean; stats[3 * Ct + c0 + c] = rstd;
@@ -378,6 +382,32 @@ __global__ void highway_bwd_k(const float* __restrict__ dh, const bf16* __restri
   dHT[r * 2 * HU + c] = __float2bfloat16(Hh > 0.f ? g * Tt : 0.f);
   dHT[r * 2 * HU + HU + c] = __float2bfloat16(g * (Hh - h[e]) * Tt * (1.f - Tt));
   dcarry[e] = g * (1.f - Tt);
+}
+// launch helpers shared by the engine and t2_dbg_cbhg_kernel; the callers zero the statistics / backward sums first
+template <typename TY>
+void bn_fwd_launch(const TY* y, int ld, int c0, bf16* xb, float* xf, const float* add, float* stats, int Ct, const float* gamma, const float* beta,
+                   float* mm, float* mv, long long rows, int C, int training, int stat_threads, cudaStream_t st) {
+  if (training) { bn_stats_k<TY><<<64, stat_threads, 0, st>>>(y, ld, c0, stats, Ct, rows, C); t2_count_launch(); }
+  bn_apply_k<TY><<<g1(rows * C), 256, 0, st>>>(y, ld, c0, xb, xf, add, stats, Ct, gamma, beta, mm, mv, rows, C, training); t2_count_launch();
+}
+template <typename T>
+void bn_bwd_launch(const T* g, int ldg, const T* y, int ld, int c0, const float* stats, int Ct, float* bsum, const float* gamma, bf16* dpre, int ldd,
+                   float* dgamma, float* dbeta, long long rows, int C, int act, int stat_threads, cudaStream_t st) {
+  bn_bwd_stats_k<T, T><<<64, stat_threads, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, rows, C); t2_count_launch();
+  bn_bwd_apply_k<T, T><<<g1(rows * C), 256, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, gamma, dpre, ldd, dgamma, dbeta, rows, C, act);
+  t2_count_launch();
+}
+void maxpool_fwd(const bf16* x, bf16* out, long long N, int T, int C, cudaStream_t st) {
+  maxpool_fwd_k<<<g1(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
+}
+void maxpool_bwd(const bf16* x, const bf16* dout, bf16* dx, long long N, int T, int C, cudaStream_t st) {
+  maxpool_bwd_k<<<g1(N * C), 256, 0, st>>>(x, dout, dx, N, T, C); t2_count_launch();
+}
+void highway_fwd(const float* pre, const float* bh, const float* bt, const float* h, float* hf, bf16* hb, bf16* HT, long long N, int HU, cudaStream_t st) {
+  highway_fwd_k<<<g1(N * HU), 256, 0, st>>>(pre, bh, bt, h, hf, hb, HT, N, HU); t2_count_launch();
+}
+void highway_bwd(const float* dh, const bf16* HT, const float* h, bf16* dHT, float* dcarry, long long N, int HU, cudaStream_t st) {
+  highway_bwd_k<<<g1(N * HU), 256, 0, st>>>(dh, HT, h, dHT, dcarry, N, HU); t2_count_launch();
 }
 // out fp32 += a (fp32) ; optional bf16 copy
 __global__ void add_k(float* __restrict__ acc, const float* __restrict__ a, bf16* __restrict__ outb, long long n) {
@@ -839,34 +869,27 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
     const int c0 = (k - 1) * lo.CC;
     rc = conv_fwd(s, L, x0, M, Y + c0, nullptr, KC);
     if (rc) return rc;
-    if (training) { bn_stats_k<bf16><<<64, 128, 0, st>>>(Y, KC, c0, stb, KC, N, lo.CC); t2_count_launch(); }
-    bn_apply_k<bf16><<<g1(N * lo.CC), 256, 0, st>>>(Y, KC, c0, Xb, nullptr, nullptr, stb, KC, d_params + L.p_g, d_params + L.p_be, d_params + L.p_mm,
-                                                    d_params + L.p_mv, N, lo.CC, training); t2_count_launch();
+    bn_fwd_launch<bf16>(Y, KC, c0, Xb, nullptr, nullptr, stb, KC, d_params + L.p_g, d_params + L.p_be, d_params + L.p_mm, d_params + L.p_mv, N, lo.CC,
+                        training, 128, st);
   }
   bf16* P = W<bf16>(s, lo.w_P);
-  maxpool_fwd_k<<<g1(N * KC), 256, 0, st>>>(Xb, P, N, T, KC); t2_count_launch();
+  maxpool_fwd(Xb, P, N, T, KC, st);
   // ---- projections ----
   bf16* Y1 = W<bf16>(s, lo.w_Y1); bf16* X1 = W<bf16>(s, lo.w_X1); float* st1 = W<float>(s, lo.w_st1);
   rc = conv_fwd(s, lo.proj1, P, KC, Y1, nullptr, PJc);
   if (rc) return rc;
-  if (training) {
-    T2_CHECK_CUDA(cudaMemsetAsync(st1, 0, 2LL * PJc * sizeof(float), st));
-    bn_stats_k<bf16><<<64, 256, 0, st>>>(Y1, PJc, 0, st1, PJc, N, PJc); t2_count_launch();
-  }
-  bn_apply_k<bf16><<<g1(N * PJc), 256, 0, st>>>(Y1, PJc, 0, X1, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p_g, d_params + lo.proj1.p_be,
-                                                d_params + lo.proj1.p_mm, d_params + lo.proj1.p_mv, N, PJc, training); t2_count_launch();
+  if (training) T2_CHECK_CUDA(cudaMemsetAsync(st1, 0, 2LL * PJc * sizeof(float), st));
+  bn_fwd_launch<bf16>(Y1, PJc, 0, X1, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p_g, d_params + lo.proj1.p_be, d_params + lo.proj1.p_mm,
+                      d_params + lo.proj1.p_mv, N, PJc, training, 256, st);
   float* Y2 = W<float>(s, lo.w_Y2); float* st2 = W<float>(s, lo.w_st2);
   rc = conv_fwd(s, lo.proj2, X1, PJc, nullptr, Y2, M);
   if (rc) return rc;
-  if (training) {
-    T2_CHECK_CUDA(cudaMemsetAsync(st2, 0, 2LL * M * sizeof(float), st));
-    bn_stats_k<float><<<64, 128, 0, st>>>(Y2, M, 0, st2, M, N, M); t2_count_launch();
-  }
+  if (training) T2_CHECK_CUDA(cudaMemsetAsync(st2, 0, 2LL * M * sizeof(float), st));
   // highway input = BN(proj2) + mel_outputs (modules.py:59); the fp32 sum goes through w_dhin (free until the backward pass)
   float* hin_f = W<float>(s, lo.w_dhin);
   bf16* hin = W<bf16>(s, lo.w_hin);
-  bn_apply_k<float><<<g1(N * M), 256, 0, st>>>(Y2, M, 0, nullptr, hin_f, d_mel, st2, M, d_params + lo.proj2.p_g, d_params + lo.proj2.p_be,
-                                               d_params + lo.proj2.p_mm, d_params + lo.proj2.p_mv, N, M, training); t2_count_launch();
+  bn_fwd_launch<float>(Y2, M, 0, nullptr, hin_f, d_mel, st2, M, d_params + lo.proj2.p_g, d_params + lo.proj2.p_be, d_params + lo.proj2.p_mm,
+                       d_params + lo.proj2.p_mv, N, M, training, 128, st);
   f32_to_bf16_k<<<g1(N * M), 256, 0, st>>>(hin_f, hin, N * M); t2_count_launch();
   // ---- dense to the highway width, highway layers ----
   rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]), HU, HU, st);
@@ -875,8 +898,8 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   for (int i = 0; i < lo.NH; ++i) {
     rc = gemm(W<bf16>(s, lo.w_hb[i]), HU, HU, 0, T, B, s.pk + lo.k_hw[i], 2 * HU, HU, 1, nullptr, 256, nullptr, 0, nullptr, pre, 2 * HU, 2 * HU, st);
     if (rc) return rc;
-    highway_fwd_k<<<g1(N * HU), 256, 0, st>>>(pre, d_params + lo.p_hb[i][0], d_params + lo.p_hb[i][1], W<float>(s, lo.w_hf[i]), W<float>(s, lo.w_hf[i + 1]),
-                                              W<bf16>(s, lo.w_hb[i + 1]), training ? W<bf16>(s, lo.w_HT[i]) : nullptr, N, HU); t2_count_launch();
+    highway_fwd(pre, d_params + lo.p_hb[i][0], d_params + lo.p_hb[i][1], W<float>(s, lo.w_hf[i]), W<float>(s, lo.w_hf[i + 1]), W<bf16>(s, lo.w_hb[i + 1]),
+                training ? W<bf16>(s, lo.w_HT[i]) : nullptr, N, HU, st);
   }
   // ---- bidirectional GRU ----
   const int XPW = 6 * RU;
@@ -973,7 +996,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   bf16* dHT = W<bf16>(s, lo.w_dHT);
   float* dcar = W<float>(s, lo.w_XP);        // [N][HU] fp32 scratch (the forward input projections are no longer needed)
   for (int i = lo.NH - 1; i >= 0; --i) {
-    highway_bwd_k<<<g1(N * HU), 256, 0, st>>>(dh, W<bf16>(s, lo.w_HT[i]), W<float>(s, lo.w_hf[i]), dHT, dcar, N, HU); t2_count_launch();
+    highway_bwd(dh, W<bf16>(s, lo.w_HT[i]), W<float>(s, lo.w_hf[i]), dHT, dcar, N, HU, st);
     rc = gemm(dHT, 2 * HU, 2 * HU, 0, T, B, s.pk + lo.k_hwT[i], HU, 2 * HU, 1, nullptr, 128, nullptr, 0, nullptr, dh, HU, HU, st);
     if (rc) return rc;
     add_k<<<g1(N * HU), 256, 0, st>>>(dh, dcar, i == 0 ? W<bf16>(s, lo.w_dhb) : nullptr, N * HU); t2_count_launch();
@@ -992,9 +1015,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   float* bsum = W<float>(s, lo.w_bsum);
   bf16* dY2b = W<bf16>(s, lo.w_dY2b);
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2LL * KC * sizeof(float), st));
-  bn_bwd_stats_k<float, float><<<64, 128, 0, st>>>(dhin, M, W<float>(s, lo.w_Y2), M, 0, W<float>(s, lo.w_st2), M, bsum, N, M); t2_count_launch();
-  bn_bwd_apply_k<float, float><<<g1(N * M), 256, 0, st>>>(dhin, M, W<float>(s, lo.w_Y2), M, 0, W<float>(s, lo.w_st2), M, bsum, d_params + lo.proj2.p_g, dY2b, 128,
-                                                          d_grads + lo.proj2.p_g, d_grads + lo.proj2.p_be, N, M, 0); t2_count_launch();
+  bn_bwd_launch<float>(dhin, M, W<float>(s, lo.w_Y2), M, 0, W<float>(s, lo.w_st2), M, bsum, d_params + lo.proj2.p_g, dY2b, 128, d_grads + lo.proj2.p_g,
+                       d_grads + lo.proj2.p_be, N, M, 0, 128, st);
   int sh[16];
   bf16* d2 = W<bf16>(s, lo.w_d2);
   for (int j = 0; j < lo.PK; ++j) sh[j] = -conv_shift(lo.PK, j);
@@ -1005,9 +1027,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   // ---- proj1 (ReLU, BN) ----
   bf16* d1 = W<bf16>(s, lo.w_d1);
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2LL * KC * sizeof(float), st));
-  bn_bwd_stats_k<bf16, bf16><<<64, 256, 0, st>>>(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, N, PJc); t2_count_launch();
-  bn_bwd_apply_k<bf16, bf16><<<g1(N * PJc), 256, 0, st>>>(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, d_params + lo.proj1.p_g, d1, PJc,
-                                                          d_grads + lo.proj1.p_g, d_grads + lo.proj1.p_be, N, PJc, 1); t2_count_launch();
+  bn_bwd_launch<bf16>(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, d_params + lo.proj1.p_g, d1, PJc, d_grads + lo.proj1.p_g,
+                      d_grads + lo.proj1.p_be, N, PJc, 1, 256, st);
   bf16* dP = W<bf16>(s, lo.w_dP);
   rc = gemm(d1, PJc, PJc, 0, T, B, s.pk + lo.proj1.k_wT, KC, lo.PK * lo.proj1.coutp, lo.PK, sh, 256, nullptr, 0, dP, nullptr, KC, KC, st);
   if (rc) return rc;
@@ -1015,15 +1036,14 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   colsum_k<bf16><<<64, 256, 0, st>>>(d1, N, PJc, PJc, d_grads + lo.proj1.p_b); t2_count_launch();
   // ---- max-pool, conv bank ----
   bf16* dbank = W<bf16>(s, lo.w_dbank);
-  maxpool_bwd_k<<<g1(N * KC), 256, 0, st>>>(W<bf16>(s, lo.w_Xb), dP, dbank, N, T, KC); t2_count_launch();
+  maxpool_bwd(W<bf16>(s, lo.w_Xb), dP, dbank, N, T, KC, st);
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2LL * KC * sizeof(float), st));
   bf16* dpre = dP;                              // pre-activation gradients of the bank reuse the (consumed) dP buffer
   for (int k = 1; k <= lo.K; ++k) {
     const CConv& L = lo.bank[k - 1];
     const int c0 = (k - 1) * lo.CC;
-    bn_bwd_stats_k<bf16, bf16><<<64, 128, 0, st>>>(dbank, KC, W<bf16>(s, lo.w_Y), KC, c0, W<float>(s, lo.w_stb), KC, bsum, N, lo.CC); t2_count_launch();
-    bn_bwd_apply_k<bf16, bf16><<<g1(N * lo.CC), 256, 0, st>>>(dbank, KC, W<bf16>(s, lo.w_Y), KC, c0, W<float>(s, lo.w_stb), KC, bsum, d_params + L.p_g, dpre, KC,
-                                                              d_grads + L.p_g, d_grads + L.p_be, N, lo.CC, 1); t2_count_launch();
+    bn_bwd_launch<bf16>(dbank, KC, W<bf16>(s, lo.w_Y), KC, c0, W<float>(s, lo.w_stb), KC, bsum, d_params + L.p_g, dpre, KC, d_grads + L.p_g,
+                        d_grads + L.p_be, N, lo.CC, 1, 128, st);
     colsum_k<bf16><<<64, 128, 0, st>>>(dpre + c0, N, lo.CC, KC, d_grads + L.p_b); t2_count_launch();
   }
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_x0), M, T, B), make_act(dpre, KC, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
@@ -1059,5 +1079,70 @@ extern "C" int t2_cbhg_workspace_tensor(const t2_cbhg_config_t* cfg, void* d_wor
   T2_REQUIRE(off >= 0, T2_ERR_INVALID_ARG, "cbhg_workspace_tensor: unknown tensor '%s'", name);
   *ptr = ws + off;
   if (count) *count = cnt;
+  return T2_OK;
+}
+
+// test hook: one production kernel on caller buffers (include/t2b200.h, T2_DBG_CBHG_*)
+extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel: null call");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  void* const* p = call->p;
+  const long long* i = call->i;
+  switch (call->kernel) {
+    case T2_DBG_CBHG_BN_FWD: {
+      const long long rows = i[0];
+      const int C = int(i[1]), ld = int(i[2]), c0 = int(i[3]), Ct = int(i[4]), thr = int(i[7]);
+      T2_REQUIRE(rows >= 1 && C >= 1 && c0 >= 0 && c0 + C <= ld && c0 + C <= Ct && (thr == 128 || thr == 256) && p[0] && (p[1] || p[2]) && p[4] &&
+                     p[5] && p[6] && p[7] && p[8],
+                 T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_FWD: bad arguments");
+      if (i[6])
+        bn_fwd_launch<float>(static_cast<const float*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+                             static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
+                             static_cast<float*>(p[8]), rows, C, int(i[5]), thr, st);
+      else
+        bn_fwd_launch<bf16>(static_cast<const bf16*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+                            static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
+                            static_cast<float*>(p[8]), rows, C, int(i[5]), thr, st);
+      break;
+    }
+    case T2_DBG_CBHG_BN_BWD: {
+      const long long rows = i[0];
+      const int C = int(i[1]), ldg = int(i[2]), ld = int(i[3]), c0 = int(i[4]), Ct = int(i[5]), ldd = int(i[6]), act = int(i[7]), thr = int(i[8]);
+      T2_REQUIRE(rows >= 1 && C >= 1 && c0 >= 0 && c0 + C <= ld && c0 + C <= ldg && c0 + C <= ldd && c0 + C <= Ct && (act == 0 || act == 1) &&
+                     (thr == 128 || thr == 256) && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && p[7],
+                 T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_BWD: bad arguments");
+      if (i[9])
+        bn_bwd_launch<float>(static_cast<const float*>(p[0]), ldg, static_cast<const float*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
+                             static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
+                             static_cast<float*>(p[7]), rows, C, act, thr, st);
+      else
+        bn_bwd_launch<bf16>(static_cast<const bf16*>(p[0]), ldg, static_cast<const bf16*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
+                            static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
+                            static_cast<float*>(p[7]), rows, C, act, thr, st);
+      break;
+    }
+    case T2_DBG_CBHG_POOL_FWD:
+    case T2_DBG_CBHG_POOL_BWD: {
+      const bool fwd = call->kernel == T2_DBG_CBHG_POOL_FWD;
+      T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && i[0] % i[1] == 0 && i[2] >= 1 && p[0] && p[1] && (fwd || p[2]), T2_ERR_INVALID_ARG,
+                 "dbg_cbhg_kernel POOL: bad arguments");
+      if (fwd) maxpool_fwd(static_cast<const bf16*>(p[0]), static_cast<bf16*>(p[1]), i[0], int(i[1]), int(i[2]), st);
+      else maxpool_bwd(static_cast<const bf16*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<bf16*>(p[2]), i[0], int(i[1]), int(i[2]), st);
+      break;
+    }
+    case T2_DBG_CBHG_HIGHWAY_FWD:
+      T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5], T2_ERR_INVALID_ARG, "dbg_cbhg_kernel HIGHWAY_FWD: bad arguments");
+      highway_fwd(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]), static_cast<const float*>(p[3]),
+                  static_cast<float*>(p[4]), static_cast<bf16*>(p[5]), static_cast<bf16*>(p[6]), i[0], int(i[1]), st);
+      break;
+    case T2_DBG_CBHG_HIGHWAY_BWD:
+      T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && p[0] && p[1] && p[2] && p[3] && p[4], T2_ERR_INVALID_ARG, "dbg_cbhg_kernel HIGHWAY_BWD: bad arguments");
+      highway_bwd(static_cast<const float*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<const float*>(p[2]), static_cast<bf16*>(p[3]),
+                  static_cast<float*>(p[4]), i[0], int(i[1]), st);
+      break;
+    default:
+      return t2_set_error(T2_ERR_INVALID_ARG, "dbg_cbhg_kernel: unknown kernel id %d", call->kernel);
+  }
+  T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }

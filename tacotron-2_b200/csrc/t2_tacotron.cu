@@ -40,7 +40,7 @@ struct ConvL {   // one conv + BN block
   long long k_w, k_wT;     // packed forward [cout][k*cinp], packed dgrad [cinp][k*cout]
   int cinp;                // cin rounded up to 64
   long long w_y, w_x;      // workspace: y (post-activation, pre-BN) bf16 [B][T][cout], x = block output bf16
-  long long w_stats;       // fp32 [4][cout]: sum / sumsq (fwd) then mean / rstd ; [2][cout] bwd sums
+  long long w_stats;       // fp32 [4][cout]: sums of (y - y[0]) / (y - y[0])^2 (fwd) then mean / rstd ; [2][cout] bwd sums
   int stream;              // dropout hash stream
 };
 
@@ -358,7 +358,9 @@ __global__ void embed_bwd_kernel(const int* __restrict__ idx, const bf16* __rest
   atomicAdd(dtable + (long long)idx[e / E] * E + e % E, __bfloat162float(dx[e]));
 }
 
-// per-channel sum / sum of squares of y [rows][C] (bf16) -> stats[0..C), stats[C..2C)
+// per-channel shifted sums of y [rows][C]: stats[0..C) = sum (y - y[0]), stats[C..2C) = sum (y - y[0])^2. Subtracting the
+// channel's first row (a sample of the channel) keeps E[d^2] - E[d]^2 free of the cancellation that E[y^2] - mean^2 suffers
+// when |mean| >> std.
 __device__ __forceinline__ float ld_act(const bf16* p, long long i) { return __bfloat162float(p[i]); }
 __device__ __forceinline__ float ld_act(const float* p, long long i) { return p[i]; }
 template <typename TY>
@@ -366,8 +368,9 @@ __global__ void bn_stats_kernel(const TY* __restrict__ y, float* __restrict__ st
   const long long per = (rows + gridDim.x - 1) / gridDim.x;
   const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float pv = ld_act(y, c);
     float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) { const float v = ld_act(y, r * C + c); s += v; q += v * v; }
+    for (long long r = r0; r < r1; ++r) { const float v = ld_act(y, r * C + c) - pv; s += v; q += v * v; }
     atomicAdd(stats + c, s); atomicAdd(stats + C + c, q);
   }
 }
@@ -381,8 +384,9 @@ __global__ void bn_apply_kernel(const TY* __restrict__ y, bf16* __restrict__ x, 
   const int c = int(e % C);
   float mean, rstd;
   if (training) {
-    mean = stats[c] / float(rows);
-    const float var = fmaxf(stats[C + c] / float(rows) - mean * mean, 0.f);
+    const float d = stats[c] / float(rows);
+    mean = ld_act(y, c) + d;
+    const float var = fmaxf(stats[C + c] / float(rows) - d * d, 0.f);
     rstd = rsqrtf(var + 1e-3f);
     if (e < C) {
       stats[2 * C + c] = mean; stats[3 * C + c] = rstd;
@@ -436,6 +440,30 @@ __global__ void bn_bwd_apply_kernel(const bf16* __restrict__ dout, const bf16* _
   else if (act == 2) dy *= (1.f - yv * yv);
   dpre[e] = __float2bfloat16(dy);
   if (e < C) { dgamma[c] += bsum[C + c]; dbeta[c] += bsum[c]; }
+}
+// conv-block batch norm, forward: stats [4C] (training: shifted sums, then mean / rstd; inference reads the moving statistics)
+template <typename TY>
+int bn_fwd(const TY* y, bf16* x, float* stats, const float* gamma, const float* beta, float* mm, float* mv, long long rows, int C, int training,
+           float p, unsigned long long seed, const unsigned long long* step, int stream, int split, cudaStream_t st) {
+  if (training) {
+    T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * C * sizeof(float), st));
+    bn_stats_kernel<TY><<<64, 256, 0, st>>>(y, stats, rows, C); t2_count_launch();
+  }
+  bn_apply_kernel<TY><<<g1(rows * C), 256, 0, st>>>(y, x, stats, gamma, beta, mm, mv, rows, C, training, p, seed, step, stream, split);
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+// backward: stats [6C] as left by bn_fwd, the backward sums go to stats[4C..6C); dgamma / dbeta accumulate
+int bn_bwd(const bf16* dout, const bf16* y, float* stats, const float* gamma, bf16* dpre, float* dgamma, float* dbeta, long long rows, int C, int act,
+           float p, unsigned long long seed, const unsigned long long* step, int stream, cudaStream_t st) {
+  float* bsum = stats + 4 * C;
+  T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2 * C * sizeof(float), st));
+  bn_bwd_stats_kernel<<<64, 256, 0, st>>>(dout, y, stats, bsum, rows, C, p, seed, step, stream); t2_count_launch();
+  bn_bwd_apply_kernel<<<g1(rows * C), 256, 0, st>>>(dout, y, stats, bsum, gamma, dpre, dgamma, dbeta, rows, C, act, p, seed, step, stream);
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
 }
 
 // column sums of a bf16 [rows][ld] matrix (first C columns) into fp32 dst (+=), scaled
@@ -662,11 +690,12 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
   }
   __syncthreads();
   ATT_STAMP(4);
-  // context = alpha . values: 8 row groups x (C2/8) column chunks of 8 channels
+  // context = alpha . values: 8 row groups x (C2/8) column chunks of 8 channels; one work item per thread up to C2 = 512,
+  // strided over the CTA beyond that so that every row group of part[] is written
   {
     const int nch = a.C2 >> 3;                 // uint4 chunks per row
-    const int rg = tid / nch, ch = tid % nch;  // kAttThreads >= 8 * nch for C2 <= 512
-    if (rg < 8) {
+    for (int w = tid; w < 8 * nch; w += kAttThreads) {
+      const int rg = w / nch, ch = w % nch;
       float acc[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = 0.f;
@@ -693,6 +722,18 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
     a.ctx_b[(long long)b * a.ld_b + c] = r16;
   }
   ATT_STAMP(6);
+}
+// once per forward: the merged location filter bank U (from the conv kernel K [KA][F], its bias bK, the dense Wl [F][A] and the
+// attention bias) and the kernel's shared-memory opt-in
+int att_fwd_setup(const float* K, const float* bK, const float* Wl, const float* ba, float* U, int KA, int F, int A, size_t smem, cudaStream_t st) {
+  att_prep_kernel<<<g1((KA + 1) * A), 256, 0, st>>>(K, bK, Wl, ba, U, KA, F, A); t2_count_launch();
+  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+int launch_att_fwd(const AttArgs& a, size_t smem, cudaStream_t st) {
+  T2_CHECK_CUDA(launch_pdl(att_fwd_kernel, dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
+  return T2_OK;
 }
 
 // ---- output heads / losses ---------------------------------------------------------------------------------------
@@ -849,23 +890,13 @@ int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, long long
   if (rc) return rc;
   float* stats = reinterpret_cast<float*>(s.ws + L.w_stats);
   const long long rows = (long long)lo.B * T;
-  if (training) {
-    T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * L.cout * sizeof(float), s.st));
-    if (split) bn_stats_kernel<float><<<64, 256, 0, s.st>>>(yf, stats, rows, L.cout);
-    else bn_stats_kernel<bf16><<<64, 256, 0, s.st>>>(y, stats, rows, L.cout);
-    t2_count_launch();
-  }
   float* pp = const_cast<float*>(s.params);
+  bf16* x = reinterpret_cast<bf16*>(s.ws + L.w_x);
   if (split)
-    bn_apply_kernel<float><<<g1(rows * L.cout), 256, 0, s.st>>>(yf, reinterpret_cast<bf16*>(s.ws + L.w_x), stats, s.params + L.p_gamma, s.params + L.p_beta,
-                                                         pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed, s.d_step, L.stream, 1);
-  else
-    bn_apply_kernel<bf16><<<g1(rows * L.cout), 256, 0, s.st>>>(y, reinterpret_cast<bf16*>(s.ws + L.w_x), stats, s.params + L.p_gamma, s.params + L.p_beta,
-                                                       pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed, s.d_step,
-                                                       L.stream, 0);
-  t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
+    return bn_fwd(yf, x, stats, s.params + L.p_gamma, s.params + L.p_beta, pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed,
+                  s.d_step, L.stream, 1, s.st);
+  return bn_fwd(y, x, stats, s.params + L.p_gamma, s.params + L.p_beta, pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed,
+                s.d_step, L.stream, 0, s.st);
 }
 
 
@@ -1059,6 +1090,20 @@ inline size_t att_bwd_smem(int Ti, int KA, int A, int D, int C2) {
   const int Tip = (Ti + 3) & ~3;
   return sizeof(float) * (size_t)((KA + 1) * (A + kAttPad) + att_cumlen(Ti, KA) + A + 4 * Tip + D + C2 + 2 * A +
                                   att_erows(Ti, KA) * (A + kAttPad) + 32) + 64;
+}
+constexpr size_t kSmemOptin = 232448;   // per-block shared-memory opt-in limit of sm_90
+// Training runs att_bwd_kernel, whose [T_in + KA - 1][A + 8] fp32 dE tile lives in shared memory: refuse (before any launch) a
+// T_in it cannot hold. The forward-only paths (inference, GTA) are not limited by it.
+int check_att_bwd_fits(const TL& lo) {
+  const int C2 = 2 * lo.H;
+  const size_t need = att_bwd_smem(lo.Ti, lo.KA, lo.A, lo.D, C2);
+  if (need <= kSmemOptin) return T2_OK;
+  int tmax = lo.Ti;
+  while (tmax > 1 && att_bwd_smem(tmax, lo.KA, lo.A, lo.D, C2) > kSmemOptin) --tmax;
+  return t2_set_error(T2_ERR_UNSUPPORTED_SHAPE,
+                      "training: T_in = %d needs %zu B of shared memory in the attention backward, over the %zu B per-block limit; "
+                      "T_in <= %d at these attention widths",
+                      lo.Ti, need, kSmemOptin, tmax);
 }
 __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   extern __shared__ __align__(16) float sm[];
@@ -1329,22 +1374,34 @@ __global__ void dvalues_ctx_kernel(const float* __restrict__ alpha, const bf16* 
     dvalues[((long long)b * Ti + j) * C2 + c] = live ? acc : 0.f;
   }
 }
+// launch helpers shared by the backward pass and t2_dbg_taco_kernel
+int launch_cell_bwd(const CellBwd& c, cudaStream_t st) {
+  T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)c.B * c.H)), dim3(256), 0, st, c)); t2_count_launch();
+  return T2_OK;
+}
+// scratch: [(KA+2)][A] fp32 for the batch-reduced accumulators
+void launch_att_finish(const float* acc, const float* K, const float* bK, const float* Wl, float* grads, int B, int KA, int F, int A, long long o_k,
+                       long long o_bk, long long o_wl, long long o_v, long long o_ba, float* scratch, cudaStream_t st) {
+  att_finish_kernel<<<g1((long long)(KA + 2) * A), 256, 0, st>>>(acc, K, bK, Wl, grads, B, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba, scratch); t2_count_launch();
+  att_finish2_kernel<<<g1(KA * F + F * A + F + A), 256, 0, st>>>(scratch, K, bK, Wl, grads, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba); t2_count_launch();
+}
+void launch_dvalues_ctx(const float* alpha, const bf16* dctx, const int* lens, float* dvalues, int B, int Ti, int To, int C2, cudaStream_t st) {
+  dvalues_ctx_kernel<<<dim3(Ti, B), 256, 0, st>>>(alpha, dctx, lens, dvalues, B, Ti, To, C2); t2_count_launch();
+}
 
 int conv_block_bwd(const StepCtx& s, const ConvL& L, const void* x_in, long long T, const bf16* dout, bf16* dpre, bf16* dx, float* grads,
                    const WgradTile* tiles, int ntiles) {
   const TL& lo = *s.lo;
   const long long rows = (long long)lo.B * T;
   float* stats = reinterpret_cast<float*>(s.ws + L.w_stats);
-  float* bsum = stats + 4 * L.cout;
   const bf16* y = reinterpret_cast<const bf16*>(s.ws + L.w_y);
-  T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2 * L.cout * sizeof(float), s.st));
-  bn_bwd_stats_kernel<<<64, 256, 0, s.st>>>(dout, y, stats, bsum, rows, L.cout, lo.c.dropout_rate, s.seed, s.d_step, L.stream); t2_count_launch();
-  bn_bwd_apply_kernel<<<g1(rows * L.cout), 256, 0, s.st>>>(dout, y, stats, bsum, s.params + L.p_gamma, dpre, grads + L.p_gamma, grads + L.p_beta, rows,
-                                                           L.cout, L.act, lo.c.dropout_rate, s.seed, s.d_step, L.stream); t2_count_launch();
+  int rc = bn_bwd(dout, y, stats, s.params + L.p_gamma, dpre, grads + L.p_gamma, grads + L.p_beta, rows, L.cout, L.act, lo.c.dropout_rate, s.seed,
+                  s.d_step, L.stream, s.st);
+  if (rc) return rc;
   colsum_bf16_kernel<<<64, 256, 0, s.st>>>(dpre, rows, L.cout, L.cout, grads + L.p_b, 1.f); t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   ActT maps[2] = {make_act(x_in, L.cin, int(T), lo.B), make_act(dpre, L.cout, int(T), lo.B)};
-  int rc = launch_wgrad(maps, 2, tiles, ntiles, grads, int(T), lo.B, s.st);
+  rc = launch_wgrad(maps, 2, tiles, ntiles, grads, int(T), lo.B, s.st);
   if (rc) return rc;
   if (dx) {
     int shifts[8];
@@ -1501,12 +1558,8 @@ static int decoder_reset(const StepCtx& s, DecBufs& d) {
   T2_CHECK_CUDA(cudaMemsetAsync(d.c1, 0, (size_t)B * D * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.c2, 0, (size_t)B * D * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.cum, 0, (size_t)B * Ti * 4, st));
-  att_prep_kernel<<<g1((lo.KA + 1) * lo.A), 256, 0, st>>>(d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_params + lo.p_ba, d.attU,
-                                                       lo.KA, lo.F, lo.A); t2_count_launch();
   d.att_smem = att_fwd_smem(Ti, lo.KA, lo.A, D, 2 * H);
-  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(d.att_smem)));
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
+  return att_fwd_setup(d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_params + lo.p_ba, d.attU, lo.KA, lo.F, lo.A, d.att_smem, st);
 }
 // decoder step t: LSTM-1 (prenet part of its gates precomputed in pre1[t]), LSTM-2, attention (Architecture_wrappers.py:169-213)
 static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_lengths, int t) {
@@ -1536,8 +1589,7 @@ static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_l
   a.alpha = reinterpret_cast<float*>(ws + lo.w_alpha) + (long long)t * B * Ti;
   a.ctx_a = S1n; a.ld_a = K1r; a.ctx_b = PIt + D; a.ld_b = PIK;
   a.B = B; a.Ti = Ti; a.D = D; a.A = lo.A; a.KA = lo.KA; a.C2 = 2 * H;
-  T2_CHECK_CUDA(launch_pdl(att_fwd_kernel, dim3(B), dim3(kAttThreads), d.att_smem, st, a)); t2_count_launch();
-  return T2_OK;
+  return launch_att_fwd(a, d.att_smem, st);
 }
 
 // forward + losses. d_inputs int32 [B][T_in]; d_input_lengths int32 [B]; d_mel_targets fp32 [B][T_out][M];
@@ -1548,6 +1600,7 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   TL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
+  if (training) { rc = check_att_bwd_fits(lo); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
@@ -1750,6 +1803,7 @@ extern "C" int t2_taco_workspace_tensor(const t2_taco_config_t* cfg, void* d_wor
       {"memory", lo.w_memory, B * Ti * 2 * lo.H, 2}, {"keys", lo.w_keys, B * Ti * lo.A, 4}, {"alignments", lo.w_alpha, To * B * Ti, 4},
       {"decoder_output", lo.w_decf, B * To * lo.M, 4}, {"mel_outputs", lo.w_mel, B * To * lo.M, 4}, {"stop_logits", lo.w_stop, B * To, 4},
       {"projection_rows", lo.w_projo, To * B * 128, 4}, {"enc_conv_out", lo.enc.back().w_x, B * Ti * lo.C, 2}, {"prenet", lo.w_pn2, To * B * lo.P2, 2}, {"proj_in", lo.w_PI, To * B * (lo.D + 2 * lo.H), 2},
+      {"attention_filter_bank", lo.w_attU, (lo.KA + 1) * lo.A, 4},   // merged location filters U [KA][A] + offset row u0
   };
   for (const E& e : table)
     if (strcmp(e.n, name) == 0) { *ptr = ws + e.off; *count = e.cnt; *elem_bytes = e.eb; return T2_OK; }
@@ -1798,6 +1852,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
   T2_REQUIRE(!lo.c.split_bf16, T2_ERR_INVALID_ARG, "split_bf16 (fp32-class conv stacks) mode has no backward pass");
+  rc = check_att_bwd_fits(lo);
+  if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
@@ -1902,14 +1958,14 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     c2.c_prev = reinterpret_cast<const float*>(ws + lo.w_c2) + (long long)t * B * D;
     c2.dg_a = dg2 + (long long)t * B * 4 * D; c2.ld_a = 4 * D; c2.dg_b = nullptr; c2.ld_b = 0; c2.lens = nullptr; c2.t = t; c2.B = B; c2.H = D; c2.stream = 55;
     c2.zone = lo.c.zoneout_rate; c2.seed = seed; c2.step = d_step;
-    T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)B * D)), dim3(256), 0, st, c2)); t2_count_launch();
+    rc = launch_cell_bwd(c2, st); if (rc) return rc;
     rc = lstm_bwd_gemm(s, pk + lo.k_l2T, K2, 4 * D, c2.dg_a, B, dh1ext, D, D, 2, dhs2, D, 2, ks_dec);   // dh1ext: zeroed by its consumer
     if (rc) return rc;
     CellBwd c1 = c2;
     c1.dh_ext = dh1ext; c1.zero_ext = 1; c1.dhs = dhs1; c1.dcs = dcs1;
     c1.gst = reinterpret_cast<const bf16*>(ws + lo.w_g1) + (long long)t * B * 4 * D; c1.tst = reinterpret_cast<const bf16*>(ws + lo.w_t1) + (long long)t * B * D;
     c1.c_prev = reinterpret_cast<const float*>(ws + lo.w_c1) + (long long)t * B * D; c1.dg_a = dg1 + (long long)t * B * 4 * D; c1.stream = 54;
-    T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)B * D)), dim3(256), 0, st, c1)); t2_count_launch();
+    rc = launch_cell_bwd(c1, st); if (rc) return rc;
     rc = lstm_bwd_gemm(s, pk + lo.k_l1rT, K1r, 4 * D, c1.dg_a, B, dctxl, 2 * H, 2 * H, 2, dhs1, D, 2, ks_dec);  // dctxl: zeroed by att_bwd
     if (rc) return rc;
   }
@@ -1944,11 +2000,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   }
   {
     float* scratch = reinterpret_cast<float*>(ws + lo.w_attU) + (lo.KA + 1) * A;   // [(KA+2)][A] reduced accumulators
-    att_finish_kernel<<<g1(nacc), 256, 0, st>>>(attacc, d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_grads, B, lo.KA, lo.F, A,
-                                                lo.p_lck, lo.p_lcb, lo.p_lfl, lo.p_v, lo.p_ba, scratch); t2_count_launch();
-    att_finish2_kernel<<<g1(lo.KA * lo.F + lo.F * A + lo.F + A), 256, 0, st>>>(scratch, d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl,
-                                                                             d_grads, lo.KA, lo.F, A, lo.p_lck, lo.p_lcb, lo.p_lfl, lo.p_v,
-                                                                             lo.p_ba); t2_count_launch();
+    launch_att_finish(attacc, d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_grads, B, lo.KA, lo.F, A, lo.p_lck, lo.p_lcb, lo.p_lfl,
+                      lo.p_v, lo.p_ba, scratch, st);
   }
   // ---- attention memory: keys / values ----
   bf16* dkeysb = reinterpret_cast<bf16*>(ws + lo.w_dkeysb);
@@ -1961,8 +2014,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     ActT maps[2] = {make_act(ws + lo.w_values, 2 * H, Ti, B), make_act(dkeysb, A, Ti, B)};
     rc = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, Ti, B, st); if (rc) return rc; ++li;
   }
-  dvalues_ctx_kernel<<<dim3(Ti, B), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_alpha), dctx_all, d_input_lengths, dvalues, B, Ti, To, 2 * H);
-  t2_count_launch();
+  launch_dvalues_ctx(reinterpret_cast<float*>(ws + lo.w_alpha), dctx_all, d_input_lengths, dvalues, B, Ti, To, 2 * H, st);
   // ---- encoder BiLSTM, backward through time ----
   const void* x3 = ws + lo.enc.back().w_x;
   TacoSide* side = taco_side();
@@ -1988,7 +2040,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
       c.c_prev = reinterpret_cast<const float*>(ws + lo.w_encc[d]) + (long long)sidx * B * H;
       c.dg_a = dgall + (long long)sidx * B * 4 * H; c.ld_a = 4 * H; c.dg_b = dpre + (long long)t * 4 * H; c.ld_b = (long long)Ti * 4 * H;
       c.lens = d_input_lengths; c.t = t; c.B = B; c.H = H; c.stream = 52 + d; c.zone = lo.c.zoneout_rate; c.seed = seed; c.step = d_step;
-      T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)B * H)), dim3(256), 0, sx, c)); t2_count_launch();
+      rc = launch_cell_bwd(c, sx); if (rc) return rc;
       rc = lstm_bwd_gemm(sc, pk + lo.k_encWrT[d], H, 4 * H, c.dg_a, B, edh, H, H, 2, nullptr, 0, 0, ks_enc);
       if (rc) return rc;
     }
@@ -2036,4 +2088,98 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
+}
+
+// test hook: one production kernel on caller buffers (include/t2b200.h, T2_DBG_TACO_*)
+extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_taco_kernel: null call");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  void* const* p = call->p;
+  const long long* i = call->i;
+  auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  switch (call->kernel) {
+    case T2_DBG_TACO_ATT_FWD: {
+      const int B = int(i[0]), Ti = int(i[1]), D = int(i[2]), A = int(i[3]), KA = int(i[4]), F = int(i[5]), C2 = int(i[6]);
+      for (int k = 0; k < 15; ++k)
+        T2_REQUIRE(k == 13 || p[k] != nullptr, T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FWD: null pointer argument %d", k);
+      T2_REQUIRE(B >= 1 && B <= 256 && Ti >= 1 && Ti <= 1024 && D >= 32 && D % 32 == 0 && A % 64 == 0 && A >= 64 && A <= 128 && KA >= 1 &&
+                     KA % 2 == 1 && KA <= 31 && F >= 1 && F <= 32 && C2 >= 64 && C2 % 64 == 0,
+                 T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_FWD: unsupported shape");
+      T2_REQUIRE(i[7] >= D && i[8] >= C2 && i[9] >= C2 && aligned16(p[1]) && aligned16(p[9]) && (reinterpret_cast<uintptr_t>(p[8]) & 7) == 0 &&
+                     (reinterpret_cast<uintptr_t>(p[7]) & 7) == 0,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FWD: bad pitch or alignment");
+      const size_t smem = att_fwd_smem(Ti, KA, A, D, C2);
+      T2_REQUIRE(smem <= kSmemOptin, T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_FWD: %zu B of shared memory", smem);
+      AttArgs a;
+      a.h2out = static_cast<const bf16*>(p[0]); a.ld_h2 = int(i[7]); a.WqT = static_cast<const bf16*>(p[1]);
+      a.U = static_cast<float*>(p[6]); a.v = static_cast<const float*>(p[7]);
+      a.keys = static_cast<const float*>(p[8]); a.values = static_cast<const bf16*>(p[9]); a.lens = static_cast<const int*>(p[10]);
+      a.cum = static_cast<float*>(p[11]); a.alpha = static_cast<float*>(p[12]);
+      a.ctx_a = static_cast<bf16*>(p[13]); a.ld_a = int(i[8]); a.ctx_b = static_cast<bf16*>(p[14]); a.ld_b = int(i[9]);
+      a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2;
+      int rc = att_fwd_setup(static_cast<const float*>(p[2]), static_cast<const float*>(p[3]), static_cast<const float*>(p[4]),
+                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, st);
+      return rc ? rc : launch_att_fwd(a, smem, st);
+    }
+    case T2_DBG_TACO_BN_FWD: {
+      const long long rows = i[0];
+      const int C = int(i[1]);
+      T2_REQUIRE(rows >= 1 && C >= 1 && C <= 4096 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && (i[2] == 0 || i[2] == 1) &&
+                     (i[3] == 0 || i[3] == 1) && (i[5] == 0 || i[5] == 1) && i[4] >= 0 && call->f[0] >= 0.f && call->f[0] < 1.f,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel BN_FWD: bad arguments");
+      if (i[3])
+        return bn_fwd(static_cast<const float*>(p[0]), static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+                      static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
+                      call->step, int(i[4]), int(i[5]), st);
+      return bn_fwd(static_cast<const bf16*>(p[0]), static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+                    static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
+                    call->step, int(i[4]), int(i[5]), st);
+    }
+    case T2_DBG_TACO_BN_BWD: {
+      const long long rows = i[0];
+      const int C = int(i[1]);
+      T2_REQUIRE(rows >= 1 && C >= 1 && C <= 4096 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && i[2] >= 0 && i[2] <= 2 &&
+                     i[3] >= 0 && call->f[0] >= 0.f && call->f[0] < 1.f,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel BN_BWD: bad arguments");
+      return bn_bwd(static_cast<const bf16*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+                    static_cast<bf16*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
+                    call->step, int(i[3]), st);
+    }
+    case T2_DBG_TACO_CELL_BWD: {
+      CellBwd c;
+      c.dh_ext = static_cast<float*>(p[0]); c.ld_ext = i[0]; c.zero_ext = int(i[1]);
+      c.dhs = static_cast<float*>(p[1]); c.dcs = static_cast<float*>(p[2]);
+      c.gst = static_cast<const bf16*>(p[3]); c.tst = static_cast<const bf16*>(p[4]); c.c_prev = static_cast<const float*>(p[5]);
+      c.dg_a = static_cast<bf16*>(p[6]); c.ld_a = i[2]; c.dg_b = static_cast<bf16*>(p[7]); c.ld_b = i[3];
+      c.lens = static_cast<const int*>(p[8]); c.t = int(i[4]); c.B = int(i[5]); c.H = int(i[6]); c.stream = int(i[7]);
+      c.zone = call->f[0]; c.seed = call->seed; c.step = call->step;
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && c.B >= 1 && c.H >= 1 && c.t >= 0 && c.ld_ext >= c.H &&
+                     c.ld_a >= 4 * c.H && (!c.dg_b || c.ld_b >= 4 * c.H) && (c.zero_ext == 0 || c.zero_ext == 1) && c.stream >= 0 &&
+                     c.zone >= 0.f && c.zone < 1.f,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel CELL_BWD: bad arguments");
+      return launch_cell_bwd(c, st);
+    }
+    case T2_DBG_TACO_ATT_FINISH: {
+      const int B = int(i[0]), KA = int(i[1]), F = int(i[2]), A = int(i[3]);
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && B >= 1 && KA >= 1 && KA <= 31 && F >= 1 && F <= 32 && A >= 1 && A <= 128 &&
+                     i[4] >= 0 && i[5] >= 0 && i[6] >= 0 && i[7] >= 0 && i[8] >= 0,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FINISH: bad arguments");
+      launch_att_finish(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
+                        static_cast<const float*>(p[3]), static_cast<float*>(p[4]), B, KA, F, A, i[4], i[5], i[6], i[7], i[8],
+                        static_cast<float*>(p[5]), st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
+    }
+    case T2_DBG_TACO_DVALUES: {
+      const int B = int(i[0]), Ti = int(i[1]), To = int(i[2]), C2 = int(i[3]);
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && B >= 1 && B <= 65535 && Ti >= 1 && To >= 1 && C2 >= 1, T2_ERR_INVALID_ARG,
+                 "dbg_taco_kernel DVALUES: bad arguments");
+      launch_dvalues_ctx(static_cast<const float*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<const int*>(p[2]), static_cast<float*>(p[3]),
+                         B, Ti, To, C2, st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
+    }
+    default:
+      return t2_set_error(T2_ERR_INVALID_ARG, "dbg_taco_kernel: unknown kernel id %d", call->kernel);
+  }
 }

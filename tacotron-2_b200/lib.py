@@ -71,3 +71,9 @@ class DbgWgradTile(ctypes.Structure):
                 ("b_map", ctypes.c_int), ("b_ch0", ctypes.c_int), ("b_shift", ctypes.c_int), ("b_layer", ctypes.c_int),
                 ("out_off", ctypes.c_longlong), ("ldc", ctypes.c_int), ("m_valid", ctypes.c_int), ("n_valid", ctypes.c_int),
                 ("scale", ctypes.c_float), ("accumulate", ctypes.c_int), ("div", ctypes.c_void_p)]
+
+
+class DbgKernel(ctypes.Structure):
+    """t2_dbg_kernel_t: one Tacotron / CBHG kernel launch for t2_dbg_taco_kernel / t2_dbg_cbhg_kernel"""
+    _fields_ = [("kernel", ctypes.c_int), ("p", ctypes.c_void_p * 16), ("i", ctypes.c_longlong * 16), ("f", ctypes.c_float * 4),
+                ("seed", ctypes.c_ulonglong), ("step", ctypes.c_void_p)]

@@ -157,7 +157,8 @@ def test_ctypes_struct_mirrors_match_the_library():
     lib.t2_struct_size.argtypes = [ctypes.c_char_p]
     pairs = {"t2_wn_config_t": t2.wavenet.WnConfig, "t2_wn_sizes_t": t2.wavenet.WnSizes, "t2_taco_config_t": t2.tacotron.TacoConfig,
              "t2_cbhg_config_t": t2.tacotron.CbhgConfig, "t2_audio_config_t": t2.audio.AudioConfig,
-             "t2_dbg_act_t": t2.lib.DbgAct, "t2_dbg_gemm_t": t2.lib.DbgGemm, "t2_dbg_wgrad_tile_t": t2.lib.DbgWgradTile}
+             "t2_dbg_act_t": t2.lib.DbgAct, "t2_dbg_gemm_t": t2.lib.DbgGemm, "t2_dbg_wgrad_tile_t": t2.lib.DbgWgradTile,
+             "t2_dbg_kernel_t": t2.lib.DbgKernel}
     for name, mirror in pairs.items():
         assert lib.t2_struct_size(name.encode()) == ctypes.sizeof(mirror), name
     assert lib.t2_struct_size(b"nope") == -1
@@ -216,3 +217,25 @@ def test_act_gemm_rejects_bad_cluster_and_segments():
     assert lib.t2_dbg_act_gemm(ctypes.byref(c), None) == -1 and b"segment" in lib.t2_last_error()
     c.seg[0] = t2.lib.DbgSeg(0, 0, 0, 2, 0, 1)                 # 2 k-blocks, weight has 1
     assert lib.t2_dbg_act_gemm(ctypes.byref(c), None) == -1 and b"packed weight" in lib.t2_last_error()
+
+
+def test_training_rejects_t_in_past_the_attention_backward_limit():
+    """The attention backward keeps a [T_in + KA - 1][A + 8] fp32 tile in shared memory, which at attention_dim 128 / kernel 31 holds
+    T_in <= 336 within the 232,448 B per-block limit. A training forward or backward past that returns T2_ERR_UNSUPPORTED_SHAPE with a
+    message naming the limit, before any driver call: the null buffers here are never touched. Only refused shapes are passed, so
+    nothing can be launched."""
+    from hparams import hparams
+    from t2_import import t2
+    lib = t2.lib.load()
+    hp = hparams.copy()
+    hp.set_hparam("predict_linear", False)
+    null = ctypes.c_void_p(0)
+    for T_in in (337, 1024):
+        cfg = t2.tacotron.make_config(hp, 2, T_in, 8)
+        assert (cfg.attention_dim, cfg.attention_kernel) == (128, 31)
+        rcs = [lib.t2_taco_forward(ctypes.byref(cfg), null, null, null, null, null, null, null, null, 1, ctypes.c_ulonglong(0), null, null),
+               lib.t2_taco_backward(ctypes.byref(cfg), null, null, null, null, null, null, null, null, ctypes.c_ulonglong(0), null, null)]
+        for rc in rcs:
+            assert rc == -2, (T_in, rc, lib.t2_last_error())
+            msg = lib.t2_last_error()
+            assert b"T_in <= 336" in msg and b"232448" in msg, msg

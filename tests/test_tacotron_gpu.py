@@ -77,6 +77,22 @@ def test_forward_matches_oracle(B, T_in, T_out):
         assert abs(los[k] - parts[k].item()) < 2e-3 + 1e-3 * abs(parts[k].item()), k
 
 
+def test_forward_matches_oracle_at_384_encoder_units():
+    """2 * encoder_lstm_units = 768 > 512: the attention context needs more work items than the attention CTA has threads"""
+    B, T_in, T_out = 3, 40, 24
+    hp = _hp(encoder_lstm_units=384)
+    model, params, ref, parts, _ = _run_forward(hp, B, T_in, T_out, 37)
+    al = model.workspace_tensor("alignments", (T_out, B, T_in)).float().cpu().transpose(0, 1)
+    err_al = (al - ref["alignments"]).abs().max().item()
+    dec = model.workspace_tensor("decoder_output", (B, T_out, hp.num_mels)).cpu()
+    e_dec = (dec - ref["decoder_output"]).abs()
+    los = model.losses()
+    record("tacotron_fwd_H384_B%d_Tin%d_Tout%d" % (B, T_in, T_out), align_max_err=err_al, dec_l1=e_dec.mean().item())
+    assert err_al < 6e-4 and e_dec.mean().item() < 1.6e-3                 # the same tolerances as test_forward_matches_oracle
+    for k in ("before", "after", "stop", "reg"):
+        assert abs(los[k] - parts[k].item()) < 2e-3 + 1e-3 * abs(parts[k].item()), k
+
+
 @pytest.mark.parametrize("B,T_in,T_out", [(3, 40, 24), (8, 60, 64)])
 def test_backward_matches_oracle(B, T_in, T_out):
     hp = _hp()
