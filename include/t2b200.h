@@ -182,6 +182,8 @@ typedef struct {
   int split_bf16;            /* 1 = "fp32-class" forward: activations and weights travel as bf16 hi + lo pairs (3 tensor-core products per
                               * contraction, fp32 accumulate; ~2^-17 relative operand error instead of 2^-9). Forward / loss only, dropout 0:
                               * the parity mode that shows the bf16-mode deviation from the reference's fp32 graph is storage rounding. */
+  int gin_channels;          /* global (speaker) conditioning: width of the speaker embedding (wavenet.py:151-158), 0 = off */
+  int n_speakers;            /* rows of gc_embedding (>= 1 when gin_channels > 0) */
 } t2_wn_config_t;
 
 typedef struct {
@@ -231,6 +233,11 @@ int t2_wn_time_kernel(const t2_wn_config_t* cfg, const float* d_params, const vo
  * element count and element size */
 int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspace, const char* name, void** ptr,
                            long long* count, int* elem_bytes);
+/* gin_channels > 0: the speaker ids (device int32 [B]) of the next forwards, copied into the workspace, so a replayed CUDA graph
+ * uses the ids set last. NULL = no speaker term (the reference skips it when g is None, modules.py:504); t2_wn_init starts there.
+ * Every layer then adds b_gin + W_gin^T gc_embedding[id_b] to item b's gate pre-activations. An id outside [0, n_speakers) reads
+ * nothing: it makes that item's gate biases, and so its gate activations, NaN. */
+int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* d_speaker_ids, void* stream);
 
 
 /* ---- WaveNet vocoder: Fast-WaveNet autoregressive synthesis ---------------------------------------------------
@@ -250,6 +257,10 @@ int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, const float* 
                       void* d_workspace, const float* d_c, const void* d_initial, const void* d_test_inputs,
                       const float* d_u_a, const float* d_u_b, unsigned long long seed, void* d_out_samples,
                       float* d_out_raw, void* stream);
+/* gin_channels > 0: per-item gate biases of the following t2_wn_ar_generate calls from the speaker ids (device int32 [B]; NULL = no
+ * speaker term) and the masters. Call after t2_wn_ar_pack, which resets them to no speaker term. Items of one cluster may differ. */
+int t2_wn_ar_set_speakers(const t2_wn_config_t* cfg, int cluster_size, const float* d_params, const void* d_packed_ar,
+                          void* d_workspace, const int* d_speaker_ids, void* stream);
 
 
 /* ---- Tacotron-2 mel predictor: training graph (teacher forcing, outputs_per_step = 1, predict_linear = False) ----

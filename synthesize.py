@@ -54,7 +54,8 @@ def main():
     parser.add_argument("--mode", default="eval", help="mode of run: can be one of %s" % accepted_modes)
     parser.add_argument("--GTA", default="True", help="Ground truth aligned synthesis, defaults to True, only considered in synthesis mode")
     parser.add_argument("--text_list", default="", help="Text file contains list of texts to be synthesized. Valid if mode=eval")
-    parser.add_argument("--speaker_id", default=None, help="(global conditioning is out of scope on the H100 path)")
+    parser.add_argument("--speaker_id", default=None,
+                        help="Comma-separated speaker ids, one per mel file of --mels_dir (WaveNet with gin_channels > 0).")
     args = parser.parse_args()
     accepted_models = ["Tacotron", "WaveNet", "Tacotron-2"]
     if args.model not in accepted_models:

@@ -565,7 +565,10 @@ def wavenet_tf_name(name, upsample_type="SubPixel"):
     their convs inside `variable_scope('ResidualConv1DGLU_<l>')` (modules.py:482) with layer names
     `residual_block_<role>_conv_ResidualConv1DGLU_<l>` (modules.py:412-450); first / last convs are named at wavenet.py:109-149;
     the upsampling layers `<Type>_layer_<i>` at wavenet.py:176-192. The saver of the reference stores the EMA shadow next to each
-    variable as `<name>/ExponentialMovingAverage` (wavenet_vocoder/train.py:75-83)."""
+    variable as `<name>/ExponentialMovingAverage` (wavenet_vocoder/train.py:75-83). The speaker embedding is created outside the
+    `inference` scope (modules.py:12-21): `WaveNet_model/gc_embedding`."""
+    if name == "gc_embedding":
+        return "WaveNet_model/gc_embedding"
     P = "WaveNet_model/inference/"
     head, _, leaf = name.rpartition("/")
     parts = head.split("/")
@@ -582,6 +585,8 @@ def engine_name(tf_name):
     """inverse of tacotron_tf_name / wavenet_tf_name for a variable name WITHOUT slot suffix; None when the name is not a model
     variable of either graph (optimizer scalars, `global_step`, unrelated scopes). Outer scopes in front of `inference/` are ignored."""
     import re
+    if tf_name == "WaveNet_model/gc_embedding" or tf_name.endswith("/WaveNet_model/gc_embedding"):
+        return "gc_embedding"
     if "/inference/" not in tf_name:
         return None
     outer, tail = tf_name.split("/inference/", 1)

@@ -268,13 +268,14 @@ struct EpiHasPrefetch { static constexpr bool value = EPI == EPI_RES || EPI == E
 
 // tanh/sigmoid gate of ResidualConv1DGLU (wavenet_vocoder/models/modules.py:494-510).
 // tile columns [0,128) = 'a' (tanh) channels cb..cb+127, [128,256) = 'b' (sigmoid) channels.
-// ptr: 0 ta_out, 1 sb_out, 2 z_out (bf16 [pos, Gh]), 3 bias fp32 [2*Gh];  i0 = Gh
+// ptr: 0 ta_out, 1 sb_out, 2 z_out (bf16 [pos, Gh]), 3 bias fp32 [2*Gh];  i0 = Gh, i2 = bias stride per batch item (0: one bias
+// for every item; 2*Gh: per-item gate biases of the speaker conditioning - every M tile lies within one item)
 template <>
 struct Epilogue<EPI_GATE, 256> {
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int Gh = e.i[0];
     const int cb = c.n_tile * 128;
-    const float* bias = static_cast<const float*>(e.ptr[3]);
+    const float* bias = static_cast<const float*>(e.ptr[3]) + size_t(c.b) * e.i[2];
     __nv_bfloat16* ta_o = static_cast<__nv_bfloat16*>(e.ptr[0]);
     __nv_bfloat16* sb_o = static_cast<__nv_bfloat16*>(e.ptr[1]);
     __nv_bfloat16* z_o = static_cast<__nv_bfloat16*>(e.ptr[2]);
@@ -743,7 +744,8 @@ struct Epilogue<EPI_SCALE_RELUMASK, BN> {
 };
 
 // backward of the gate: dz -> (da, db).  ptr: 0 ta, 1 sb (bf16 [pos,Gh]), 2 dg out (bf16 [pos,2Gh]), 3 / 4 int64 fixed-point [2Gh]
-// gate-bias gradients (column sums of dg, fx_add; nullable — dilated-conv bias and cin-conv bias get the same sum); i0 = Gh
+// gate-bias gradients (column sums of dg, fx_add; nullable — dilated-conv bias and cin-conv bias get the same sum); i0 = Gh,
+// i1 = stride of ptr 3 per batch item (0: one sum over all items; 2*Gh: per-item sums for the speaker conditioning)
 template <int BN>
 struct Epilogue<EPI_GATE_BWD, BN> {
   // ta of column group 0 is loaded while the mainloop runs; sb of group 0 and both inputs of group 1 after it
@@ -785,8 +787,9 @@ struct Epilogue<EPI_GATE_BWD, BN> {
       if (e.ptr[3]) {
         const float ca = warp_colsum32(a, c.lane), cb2 = warp_colsum32(s, c.lane);
         const int col = cb + cq * 32 + colsum32_col(c.lane);
-        const FxAdd x0 = fx_issue(static_cast<long long*>(e.ptr[3]) + col, ca);
-        const FxAdd x1 = fx_issue(static_cast<long long*>(e.ptr[3]) + Gh + col, cb2);
+        long long* sum = static_cast<long long*>(e.ptr[3]) + size_t(c.b) * e.i[1];
+        const FxAdd x0 = fx_issue(sum + col, ca);
+        const FxAdd x1 = fx_issue(sum + Gh + col, cb2);
         if (e.ptr[4]) {
           const FxAdd x2 = fx_issue(static_cast<long long*>(e.ptr[4]) + col, ca);
           const FxAdd x3 = fx_issue(static_cast<long long*>(e.ptr[4]) + Gh + col, cb2);

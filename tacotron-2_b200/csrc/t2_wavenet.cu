@@ -9,6 +9,7 @@
 //   gate : [x(t-2d) | x(t-d) | x(t) | c(t)] (K = 3R + 128) x Wg -> tanh*sigmoid epilogue -> z (+ stashes)
 //   out  : z (K = G/2) x Wo -> (o + b + x) * sqrt(.5) epilogue -> x_next
 // the skip 1x1 of ALL layers is deferred into one K = L*G/2 GEMM (skips never round-trip through HBM).
+// Global (speaker) conditioning (gin_channels > 0) enters the gate GEMM's epilogue as a per-item bias, not as a GEMM operand.
 #include <stdlib.h>
 #include <math.h>
 #include <stdio.h>
@@ -61,6 +62,7 @@ struct Layout {
   bool split;   // split-bf16 forward (t2_wn_config_t.split_bf16)
   int xm;       // channel multiplier of the stored activations: 2 in split mode (hi | lo), else 1
   bool scalar_in, mol, gauss;   // mol: scalar-input head (mixture of logistics, or a single Gaussian when gauss)
+  int Gi, NS;   // global (speaker) conditioning: embedding width (0 = off) and rows of gc_embedding
   float res_scale;
   std::vector<float> skip_scale;
   // params
@@ -68,12 +70,18 @@ struct Layout {
   long long n_params;
   long long p_in_k, p_in_b, p_f1_k, p_f1_b, p_f2_k, p_f2_b;
   std::vector<long long> p_dil_k, p_dil_b, p_c_k, p_c_b, p_s_k, p_s_b, p_o_k, p_o_b, p_up_k, p_up_b;
+  std::vector<long long> p_g_k, p_g_b;   // residual_block_gin_conv of each layer (Gi > 0)
+  long long p_emb;                       // gc_embedding [NS][Gi] (Gi > 0)
+  long long layer_stride;                // parameter elements per residual layer (every layer has the same tensors)
   // packed (byte offsets)
   long long k_Wg, k_Wo, k_Ws, k_Wf1, k_Wf2, k_WozT, k_WdT, k_WcT, k_Wf1T, k_Wf2T, k_bias_g, k_bias_skip;
   long long packed_bytes;
   // workspace (byte offsets)
   long long w_cup, w_x, w_xd, w_ta, w_sb, w_z, w_h1, w_h2, w_dlog, w_dh2, w_dskip, w_dxin, w_dg, w_dcup;
   long long w_skipsum;
+  long long w_spk;      // Gi > 0: int32 [1 + B]: speaker term on / off, then the ids (t2_wn_set_speakers)
+  long long w_gbias;    // Gi > 0: fp32 [L][B][G] per-item gate biases: bias_g + (b_gin + W_gin^T emb[id_b])
+  long long w_gsum;     // Gi > 0: int64 fixed-point [L][B][G] per-item column sums of d gate pre-activation
   long long w_gfx;      // int64 fixed-point accumulators of the gradients summed by many blocks (t2_common.cuh fx_add)
   long long w_upgrad[2], w_scalars, w_tiles_main, w_tiles_head, w_packjobs, w_colsum, w_tables;
   std::vector<long long> w_upout;
@@ -126,6 +134,9 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     T2_REQUIRE(lo.O == 256 && lo.Q == 256, T2_ERR_UNSUPPORTED_SHAPE, "mulaw-quantize needs out_channels == quantize_channels == 256");
   }
   T2_REQUIRE(lo.B >= 1 && lo.T >= 1, T2_ERR_INVALID_ARG, "bad B/T");
+  lo.Gi = cfg->gin_channels; lo.NS = cfg->n_speakers;
+  T2_REQUIRE(lo.Gi >= 0 && (lo.Gi == 0 || lo.NS >= 1), T2_ERR_INVALID_ARG,
+             "gin_channels must be >= 0, and n_speakers >= 1 when gin_channels > 0 (got %d / %d)", lo.Gi, lo.NS);
   lo.Kg = 3 * lo.R + (lo.C > 0 ? 128 : 0);
   lo.ldo = lo.mol ? 64 : 512;   // row pitch of dlog (bf16): MoL 32 values (+pad so a 64-wide TMA box fits); CE hi|lo pair
   lo.Op = lo.mol ? 64 : 512;    // K of Wf2T (CE: [Wf2^T | Wf2^T] against the hi|lo split of dlog)
@@ -160,6 +171,10 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
       lo.p_c_k.push_back(add_param(lo, s + "residual_block_cin_conv/kernel", {1, lo.C, lo.G}));
       lo.p_c_b.push_back(add_param(lo, s + "residual_block_cin_conv/bias", {lo.G}));
     }
+    if (lo.Gi > 0) {
+      lo.p_g_k.push_back(add_param(lo, s + "residual_block_gin_conv/kernel", {1, lo.Gi, lo.G}));
+      lo.p_g_b.push_back(add_param(lo, s + "residual_block_gin_conv/bias", {lo.G}));
+    }
     lo.p_s_k.push_back(add_param(lo, s + "residual_block_skip_conv/kernel", {1, lo.Gh, lo.S}));
     lo.p_s_b.push_back(add_param(lo, s + "residual_block_skip_conv/bias", {lo.S}));
     lo.p_o_k.push_back(add_param(lo, s + "residual_block_out_conv/kernel", {1, lo.Gh, lo.R}));
@@ -169,6 +184,8 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.p_f1_b = add_param(lo, "final_convolution_1/bias", {lo.S});
   lo.p_f2_k = add_param(lo, "final_convolution_2/kernel", {1, lo.S, lo.O});
   lo.p_f2_b = add_param(lo, "final_convolution_2/bias", {lo.O});
+  lo.p_emb = lo.Gi > 0 ? add_param(lo, "gc_embedding", {lo.NS, lo.Gi}) : -1;   // outside the residual stack (modules.py:12-21)
+  lo.layer_stride = lo.L > 1 ? lo.p_dil_k[1] - lo.p_dil_k[0] : 0;
   for (size_t i = 0; i < lo.up_w.size(); ++i) {
     char p[64];
     snprintf(p, sizeof(p), "local_conditioning_upsampling_%d/", int(i) + 1);
@@ -336,6 +353,12 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.w_packjobs = takeb((long long)lo.n_packjobs * sizeof(PackJob));
   lo.w_colsum = takeb((long long)lo.n_colsum * sizeof(ColsumJob));
   lo.w_tables = takeb((long long)lo.L * (3 * sizeof(long long) + sizeof(float)));
+  lo.w_spk = lo.w_gbias = lo.w_gsum = -1;
+  if (lo.Gi > 0) {
+    lo.w_spk = takeb((1LL + lo.B) * 4);
+    lo.w_gbias = takeb(L * lo.B * lo.G * 4);
+    lo.w_gsum = takeb(L * lo.B * lo.G * 8);
+  }
   lo.workspace_bytes = o;
   return T2_OK;
 }
@@ -416,6 +439,117 @@ __global__ void derived_bias_kernel(DerivedArgs a) {
     float v = 0.f;
     for (int l = 0; l < a.L; ++l) v += a.scales[l] * a.params[a.offs[3 * l + 2] + i];
     a.bias_skip[i] = v;
+  }
+}
+
+// ---- global (speaker) conditioning (modules.py:10-21,426-433,503-508; wavenet.py:669-678) ----------------------------------
+// The speaker term is constant along time, so per layer l and item b it is a gate bias:
+//   out[l][b][g] = bias[l][g] + (b_gin[l][g] + sum_k W_gin[l][k][g] * emb[id_b][k])
+// kept as its own sum added onto the shared bias, so that zero gin weights give exactly the shared bias. Gate channels are in
+// natural order (tanh half, then sigmoid half) like bias_g; the gate epilogue applies the tile permutation.
+struct GinArgs {
+  const float* params;
+  const float* bias;          // shared gate bias of layer l at bias + l * bias_ld
+  long long bias_ld;
+  const int* on;              // device flag (nullable = on): 0 = no speaker term
+  const int* ids;             // [B] (nullable = no speaker term)
+  float* out;                 // out + l * out_l + b * out_b + g
+  long long out_l, out_b;
+  long long p_k, p_b, p_stride, p_emb;   // W_gin / b_gin of layer l at params + p_k / p_b + l * p_stride
+  int L, B, G, Gi, NS;
+};
+__global__ void gin_bias_kernel(GinArgs a) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= (long long)a.L * a.B * a.G) return;
+  const int g = int(i % a.G), b = int((i / a.G) % a.B), l = int(i / ((long long)a.G * a.B));
+  float v = a.bias[l * a.bias_ld + g];
+  if (a.ids && (!a.on || *a.on)) {
+    const int id = a.ids[b];
+    float s = __int_as_float(0x7fffffff);   // an id outside [0, NS) reads nothing and makes the item's gate activations NaN
+    if (id >= 0 && id < a.NS) {
+      const float* W = a.params + a.p_k + l * a.p_stride + g;
+      const float* e = a.params + a.p_emb + (long long)id * a.Gi;
+      s = a.params[a.p_b + l * a.p_stride + g];
+      for (int k = 0; k < a.Gi; ++k) s += W[(long long)k * a.G] * e[k];
+    }
+    v += s;
+  }
+  a.out[l * a.out_l + b * a.out_b + g] = v;
+}
+// workspace speaker state: spk[0] = 1 if ids are given, spk[1 + b] = id of item b
+__global__ void set_speakers_kernel(int* __restrict__ spk, const int* __restrict__ ids, int B) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) spk[0] = ids != nullptr;
+  if (ids && i < B) spk[1 + i] = ids[i];
+}
+// Gradients of the speaker term from the per-item fixed-point column sums S[l][b][g] of d gate pre-activation, one thread per
+// (l, g): the gate biases get sum_b S (an integer sum, exact: the same total the shared accumulator would hold), and
+// dW_gin[l][k][g] = sum_b emb[id_b][k] * S[l][b][g] in the order of b.
+struct GinGradArgs {
+  const float* params;
+  const int* spk;             // workspace speaker state (see set_speakers_kernel)
+  const long long* S;         // [L][B][G]
+  long long* gfx;             // fixed-point gradient accumulators (bias gradients)
+  float* grads;
+  const long long* offs;      // [3L]: dil_b, c_b (or -1), ... (w_tables)
+  long long p_k, p_b, p_stride, p_emb;
+  int L, B, G, Gi, NS;
+};
+__global__ void gin_wgrad_kernel(GinGradArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.L * a.G) return;
+  const int l = i / a.G, g = i % a.G;
+  const long long* S = a.S + (long long)l * a.B * a.G + g;
+  long long tot = 0;
+  bool poison = false;
+  for (int b = 0; b < a.B; ++b) {
+    const long long s = S[(long long)b * a.G];
+    if (!fx_in_range(s)) poison = true;
+    else if (!fx_in_range(tot += s)) poison = true;
+  }
+  if (poison) tot = kFxPoison;
+  a.gfx[a.offs[3 * l] + g] = tot;
+  if (a.offs[3 * l + 1] >= 0) a.gfx[a.offs[3 * l + 1] + g] = tot;
+  if (!a.spk[0]) return;      // no speaker term: its parameters get no gradient
+  a.gfx[a.p_b + l * a.p_stride + g] = tot;
+  float* dW = a.grads + a.p_k + l * a.p_stride + g;
+  for (int k = 0; k < a.Gi; ++k) {
+    float acc = 0.f;
+    for (int b = 0; b < a.B; ++b) {
+      const int id = a.spk[1 + b];
+      const float e = (id >= 0 && id < a.NS) ? a.params[a.p_emb + (long long)id * a.Gi + k] : __int_as_float(0x7fffffff);
+      acc += e * fx_value(S[(long long)b * a.G]);
+    }
+    dW[(long long)k * a.G] = acc;
+  }
+}
+// d gc_embedding[s][k] = sum over items b with id_b == s (in the order of b) of sum_{l,g} W_gin[l][k][g] * S[l][b][g]; one block
+// per (speaker, k), a fixed-shape tree per item: no float atomics. Rows no item uses stay exactly 0 (the gradient buffer is cleared).
+constexpr int kGinThreads = 256;
+__global__ void __launch_bounds__(kGinThreads) gin_demb_kernel(GinGradArgs a) {
+  __shared__ float red[kGinThreads];
+  if (!a.spk[0]) return;
+  const int s = blockIdx.x, k = blockIdx.y, tid = threadIdx.x;
+  {
+    float acc = 0.f;
+    for (int b = 0; b < a.B; ++b) {
+      if (a.spk[1 + b] != s) continue;
+      float part = 0.f;
+      for (int l = 0; l < a.L; ++l) {
+        const float* W = a.params + a.p_k + l * a.p_stride + (long long)k * a.G;
+        const long long* S = a.S + ((long long)l * a.B + b) * a.G;
+        for (int g = tid; g < a.G; g += kGinThreads) part += W[g] * fx_value(S[g]);
+      }
+      red[tid] = part;
+      __syncthreads();
+      for (int h = kGinThreads / 2; h > 0; h >>= 1) {
+        if (tid < h) red[tid] += red[tid + h];
+        __syncthreads();
+      }
+      if (tid == 0) acc += red[0];
+      __syncthreads();
+    }
+    if (tid == 0) a.grads[a.p_emb + (long long)s * a.Gi + k] = acc;
   }
 }
 
@@ -745,6 +879,10 @@ ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int
   g.epi.ptr[2] = reinterpret_cast<bf16*>(ws + lo.w_z) + lofs * lo.xm;
   g.epi.i[11] = lo.split ? 1 : 0;
   g.epi.ptr[3] = const_cast<float*>(reinterpret_cast<const float*>(pk + lo.k_bias_g) + (long long)l * lo.G);
+  if (lo.Gi > 0) {   // per-item gate biases (gin_bias_kernel): item b's row at + b * G
+    g.epi.ptr[3] = reinterpret_cast<float*>(ws + lo.w_gbias) + (long long)l * lo.B * lo.G;
+    g.epi.i[2] = lo.G;
+  }
   g.epi.i[0] = lo.Gh;
   return g;
 }
@@ -796,6 +934,11 @@ ActGemmCall make_dz_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
   g.epi.ptr[2] = reinterpret_cast<bf16*>(ws + lo.w_dg) + (long long)l * BT * lo.G;
   g.epi.ptr[3] = grads ? grads + lo.p_dil_b[l] : nullptr;
   g.epi.ptr[4] = (grads && lo.C > 0) ? grads + lo.p_c_b[l] : nullptr;
+  if (grads && lo.Gi > 0) {   // per-item sums S[l][b][:], turned into the bias and speaker gradients by gin_wgrad_kernel
+    g.epi.ptr[3] = reinterpret_cast<long long*>(ws + lo.w_gsum) + (long long)l * lo.B * lo.G;
+    g.epi.ptr[4] = nullptr;
+    g.epi.i[1] = lo.G;
+  }
   g.epi.i[0] = lo.Gh;
   return g;
 }
@@ -824,6 +967,15 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
 }
 
 inline dim3 grid1d(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
+
+GinArgs gin_args(const Layout& lo, const float* params) {
+  GinArgs a;
+  memset(&a, 0, sizeof(a));
+  a.params = params;
+  a.p_k = lo.p_g_k[0]; a.p_b = lo.p_g_b[0]; a.p_stride = lo.layer_stride; a.p_emb = lo.p_emb;
+  a.L = lo.L; a.B = lo.B; a.G = lo.G; a.Gi = lo.Gi; a.NS = lo.NS;
+  return a;
+}
 
 }  // namespace
 
@@ -933,6 +1085,15 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
 
   T2_REQUIRE(!lo.split || (!save_for_backward && !cfg->c_pre_upsampled), T2_ERR_INVALID_ARG,
              "split_bf16 (fp32-class) mode is forward / loss only (save_for_backward = 0) and needs the upsampling net");
+  if (lo.Gi > 0) {   // 0. per-item gate biases from the speaker ids last set (t2_wn_set_speakers)
+    GinArgs a = gin_args(lo, d_params);
+    const int* spk = reinterpret_cast<const int*>(ws + lo.w_spk);
+    a.bias = reinterpret_cast<const float*>(pk + lo.k_bias_g); a.bias_ld = lo.G;
+    a.on = spk; a.ids = spk + 1;
+    a.out = reinterpret_cast<float*>(ws + lo.w_gbias); a.out_l = (long long)lo.B * lo.G; a.out_b = lo.G;
+    gin_bias_kernel<<<grid1d((long long)lo.L * lo.B * lo.G), 256, 0, st>>>(a); t2_count_launch();
+    T2_CHECK_CUDA(cudaGetLastError());
+  }
   // 1. conditioning -> c_up (bf16 channels-last)
   bf16* c_up = reinterpret_cast<bf16*>(ws + lo.w_cup);
   if (lo.split) T2_CHECK_CUDA(cudaMemsetAsync(c_up, 0, (size_t)BT * 256 * 2, st));     // the channel padding of both halves must read as zero
@@ -1103,6 +1264,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   T2_CHECK_CUDA(cudaMemsetAsync(d_grads, 0, lo.n_params * sizeof(float), st));
   T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_skipsum, 0, lo.S * sizeof(long long), st));
   T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_gfx, 0, lo.n_params * sizeof(long long), st));
+  if (lo.Gi > 0) T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_gsum, 0, (size_t)lo.L * lo.B * lo.G * sizeof(long long), st));
   long long* gfx = reinterpret_cast<long long*>(ws + lo.w_gfx);
   bf16* h1 = reinterpret_cast<bf16*>(ws + lo.w_h1);
   bf16* h2 = reinterpret_cast<bf16*>(ws + lo.w_h2);
@@ -1172,6 +1334,17 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     rc = launch_act_gemm(EPI_DX, lo.R, gx, st);
     if (rc) return rc;
   }
+  if (lo.Gi > 0) {   // gate-bias and speaker-term gradients from the per-item sums of the gate backward
+    GinGradArgs a;
+    a.params = d_params; a.spk = reinterpret_cast<const int*>(ws + lo.w_spk);
+    a.S = reinterpret_cast<const long long*>(ws + lo.w_gsum); a.gfx = gfx; a.grads = d_grads;
+    a.offs = reinterpret_cast<const long long*>(ws + lo.w_tables);
+    a.p_k = lo.p_g_k[0]; a.p_b = lo.p_g_b[0]; a.p_stride = lo.layer_stride; a.p_emb = lo.p_emb;
+    a.L = lo.L; a.B = lo.B; a.G = lo.G; a.Gi = lo.Gi; a.NS = lo.NS;
+    gin_wgrad_kernel<<<grid1d((long long)lo.L * lo.G), 256, 0, st>>>(a); t2_count_launch();
+    gin_demb_kernel<<<dim3(lo.NS, lo.Gi), kGinThreads, 0, st>>>(a); t2_count_launch();
+    T2_CHECK_CUDA(cudaGetLastError());
+  }
   // From here on two independent tails: (A) the batched weight-gradient GEMM of the stack (fills the machine), (B) the
   // conditioning path (K = L*G data-gradient GEMM, transposes, upsampling-net backward) + first-conv gradient: latency-bound
   // small kernels. (B) continues on the side stream (fork/join through events, capturable into the caller's CUDA graph).
@@ -1234,6 +1407,18 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     const int rc = launch_fx_finalize(gfx, d_grads, lo.n_params, st);
     if (rc) return rc;
   }
+  return T2_OK;
+}
+
+extern "C" int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* d_speaker_ids, void* stream) {
+  Layout lo;
+  int rc = build_layout(cfg, lo);
+  if (rc) return rc;
+  T2_REQUIRE(lo.Gi > 0, T2_ERR_INVALID_ARG, "speaker ids need gin_channels > 0");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  set_speakers_kernel<<<grid1d(lo.B), 256, 0, st>>>(reinterpret_cast<int*>(static_cast<uint8_t*>(d_workspace) + lo.w_spk), d_speaker_ids, lo.B);
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
 
@@ -1343,6 +1528,7 @@ struct ArLayout {
   long long packed_bytes;
   long long ring_slots_total;      // sum over layers of slots
   long long workspace_bytes, w_cup, w_upout_base, w_ring, w_ringoff;
+  long long w_gbias;               // Gi > 0: fp32 [B][L][G] per-item gate biases (t2_wn_ar_set_speakers), else -1
   std::vector<int> ring_slots, ring_off;
 };
 
@@ -1376,6 +1562,7 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
   for (size_t i = 0; i < lo.up_w.size(); ++i) takeb((long long)lo.B * lo.C * lo.up_w[i] * 4);
   a.w_ring = takeb((long long)lo.B * off * lo.R * 4);
   a.w_ringoff = takeb(2LL * lo.L * 4);
+  a.w_gbias = lo.Gi > 0 ? takeb((long long)lo.B * lo.L * lo.G * 4) : -1;
   a.workspace_bytes = o;
   return T2_OK;
 }
@@ -1446,6 +1633,7 @@ __global__ void ar_pack_kernel(ArPackArgs a) {
 struct ArArgs {
   const bf16* w;            // slice-major weights
   const float* bias;
+  const float* gbias;       // nullable: per-item gate biases [B][L][G] replacing the shared gate rows of `bias` (speaker conditioning)
   const float* in_k;        // input_convolution kernel fp32 [cin][R]
   const float* in_b;
   const bf16* c_up;         // [B][T][C]
@@ -1652,8 +1840,14 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
       const float* bg = bsl + l * nbs;
       for (int i = tid; i < ni * a.ZC; i += kArThreads) {
         const int it = i / a.ZC, j = i % a.ZC;
-        const float av = loc[it * 2 * a.ZC + j] + bg[j];
-        const float bv = loc[it * 2 * a.ZC + a.ZC + j] + bg[a.ZC + j];
+        float ba = bg[j], bb = bg[a.ZC + j];
+        if (a.gbias) {
+          const float* gb = a.gbias + ((long long)(item0 + it) * a.L + l) * a.G + rank * a.ZC + j;
+          ba = __ldg(gb);
+          bb = __ldg(gb + a.Gh);
+        }
+        const float av = loc[it * 2 * a.ZC + j] + ba;
+        const float bv = loc[it * 2 * a.ZC + a.ZC + j] + bb;
         zsl[it * a.ZC + j] = tanhf_(av) * sigmoidf_(bv);      // local slice; the cluster PULLS it after the barrier
       }
       AR_STAMP(4);
@@ -1858,9 +2052,32 @@ extern "C" int t2_wn_ar_pack(const t2_wn_config_t* cfg, int cluster_size, const 
   for (int l = 0; l < lo.L; ++l) { rt[l] = a.ring_off[l]; rt[lo.L + l] = a.ring_slots[l]; }
   rt[2 * lo.L] = int(a.ring_slots_total);
   T2_CHECK_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(d_workspace) + a.w_ringoff, rt.data(), rt.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (lo.Gi > 0) {   // per-item gate biases start without a speaker term
+    rc = t2_wn_ar_set_speakers(cfg, cluster_size, d_params, d_packed_ar, d_workspace, nullptr, stream);
+    if (rc) return rc;
+  }
   T2_CHECK_CUDA(cudaStreamSynchronize(st));
   cudaFreeAsync(d_offs, st);
   cudaFreeAsync(d_scale, st);
+  return T2_OK;
+}
+
+extern "C" int t2_wn_ar_set_speakers(const t2_wn_config_t* cfg, int cluster_size, const float* d_params, const void* d_packed_ar,
+                                     void* d_workspace, const int* d_speaker_ids, void* stream) {
+  Layout lo;
+  int rc = build_layout(cfg, lo);
+  if (rc) return rc;
+  ArLayout al;
+  rc = build_ar_layout(lo, cluster_size, al);
+  if (rc) return rc;
+  T2_REQUIRE(lo.Gi > 0, T2_ERR_INVALID_ARG, "speaker ids need gin_channels > 0");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  GinArgs a = gin_args(lo, d_params);
+  a.bias = reinterpret_cast<const float*>(static_cast<const uint8_t*>(d_packed_ar) + al.o_bias); a.bias_ld = lo.G + lo.R;
+  a.on = nullptr; a.ids = d_speaker_ids;
+  a.out = reinterpret_cast<float*>(static_cast<uint8_t*>(d_workspace) + al.w_gbias); a.out_l = lo.G; a.out_b = (long long)lo.L * lo.G;
+  gin_bias_kernel<<<grid1d((long long)lo.L * lo.B * lo.G), 256, 0, st>>>(a); t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
 
@@ -1905,6 +2122,7 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
   memset(&a, 0, sizeof(a));
   a.w = reinterpret_cast<const bf16*>(pk);
   a.bias = reinterpret_cast<const float*>(pk + al.o_bias);
+  a.gbias = lo.Gi > 0 ? reinterpret_cast<const float*>(ws + al.w_gbias) : nullptr;
   a.in_k = d_params + lo.p_in_k; a.in_b = d_params + lo.p_in_b;
   a.c_up = c_up;
   a.ring = reinterpret_cast<float*>(ws + al.w_ring);

@@ -25,6 +25,16 @@ def glorot_uniform(shape, gen):
     return (torch.rand(shape, generator=gen, dtype=torch.float32) * 2.0 - 1.0) * limit
 
 
+def truncated_normal(shape, std, gen):
+    """tf.truncated_normal_initializer: normal draws, redrawn while beyond two standard deviations"""
+    x = torch.randn(shape, generator=gen, dtype=torch.float32)
+    while True:
+        bad = x.abs() > 2.0
+        if not bad.any():
+            return x * std
+        x[bad] = torch.randn(int(bad.sum()), generator=gen, dtype=torch.float32)
+
+
 def nn_upsample_kernel(shape, scale, n_layers, nn_scaler, subpixel):
     """shape: TF kernel shape [freq_kernel, time_kernel, 1, filters]. One centre tap (SubPixel, odd time kernel) or a row
     of 1/overlap taps (ConvTranspose2D) on the middle frequency row, scaled by NN_scaler ** (1 / n_layers)."""
@@ -50,6 +60,8 @@ def wavenet_variables(hp, tensors, seed=None):
     for name, _, shape in tensors:
         if name.endswith("bias"):
             out[name] = torch.zeros(shape)
+        elif name == "gc_embedding":                 # truncated normal, std 0.1 (modules.py:10-21)
+            out[name] = truncated_normal(shape, 0.1, gen)
         elif name.startswith("local_conditioning_upsampling") and hp.NN_init:
             i = int(name.split("/")[0].rsplit("_", 1)[-1]) - 1
             out[name] = nn_upsample_kernel(shape, hp.upsample_scales[i], n_up, hp.NN_scaler, hp.upsample_type == "SubPixel")

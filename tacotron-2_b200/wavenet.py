@@ -23,6 +23,7 @@ class WnConfig(ctypes.Structure):
         ("freq_axis_kernel_size", ctypes.c_int), ("dropout", ctypes.c_float), ("log_scale_min", ctypes.c_float),
         ("B", ctypes.c_int), ("T", ctypes.c_int), ("Tc", ctypes.c_int), ("c_pre_upsampled", ctypes.c_int),
         ("log_scale_min_gauss", ctypes.c_float), ("cdf_loss", ctypes.c_int), ("split_bf16", ctypes.c_int),
+        ("gin_channels", ctypes.c_int), ("n_speakers", ctypes.c_int),
     ]
 
 
@@ -43,7 +44,10 @@ def unsupported_hparams(hp):
             bad.append("%s=%r (%s)" % (name, getattr(hp, name), why))
     need("wavenet_weight_normalization", lambda v: not v, "weight normalisation with data-dependent init: modules.py:44-177")
     need("use_bias", lambda v: bool(v), "bias-free convolutions")
-    need("gin_channels", lambda v: v is None or v <= 0, "global (speaker) conditioning: wavenet.py:151-158,669-678")
+    if (getattr(hp, "gin_channels", None) or 0) > 0:        # global (speaker) conditioning through gc_embedding
+        need("use_speaker_embedding", lambda v: bool(v),
+             "speaker ids fed straight into the gin convolution without an embedding: wavenet.py:151-158")
+        need("n_speakers", lambda v: v is not None and v >= 1, "gin_channels > 0 needs n_speakers >= 1")
     need("kernel_size", lambda v: v == 3, "kernel_size 3")
     need("upsample_type", lambda v: v in _UPSAMPLE_TYPES or v == "NearestNeighbor", "Resize / 1D upsamplers: modules.py:657-733")
     need("upsample_activation", lambda v: v in ("Relu", "relu", "RELU"), "LeakyRelu / linear upsampling activations: wavenet.py:190-201")
@@ -84,6 +88,8 @@ def make_config(hp, B, T, c_pre_upsampled=False, dropout=None, precision="bf16")
     if precision not in ("bf16", "fp32-class"):
         raise L.T2Error("precision must be 'bf16' or 'fp32-class'")
     cfg.split_bf16 = int(precision == "fp32-class")
+    if (getattr(hp, "gin_channels", None) or 0) > 0:
+        cfg.gin_channels, cfg.n_speakers = hp.gin_channels, hp.n_speakers
     cfg.B, cfg.T = B, T
     hop = 1
     for s in scales:
@@ -123,6 +129,18 @@ def grad_buckets(tensors, n_layers, n_params, n_groups):
     groups = [(bounds[g], bounds[g + 1]) for g in range(n_groups)]
     rest = [(0, first(0)), (stack_end, n_params)]
     return groups, [r for r in rest if r[1] > r[0]]
+
+
+def speaker_ids(speakers, B, n_speakers):
+    """speaker ids ([B, 1] or [B] ints, tensor or sequence) -> int32 [B] on the host; raises ValueError on a bad shape or an id outside
+    [0, n_speakers), before anything reaches the device"""
+    ids = torch.as_tensor(speakers).detach().cpu().reshape(-1)
+    if ids.numel() != B or ids.is_floating_point() or ids.is_complex():
+        raise ValueError("speaker ids must be %d integers ([B] or [B, 1]), got %s %s" % (B, tuple(torch.as_tensor(speakers).shape), ids.dtype))
+    bad = [int(v) for v in ids.tolist() if not 0 <= int(v) < n_speakers]
+    if bad:
+        raise ValueError("speaker id(s) %s outside [0, n_speakers=%d)" % (bad, n_speakers))
+    return ids.to(torch.int32)
 
 
 def nn_upsample(hp, c, T):
@@ -173,6 +191,7 @@ class WaveNet(object):
         self.global_step = 0
         self.seed = int(hparams.wavenet_random_seed)
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device)  # added to the dropout seed on device
+        self._spk = torch.zeros(B, dtype=torch.int32, device=self.device) if self.cfg.gin_channels > 0 else None
         self._graph = None
         with torch.cuda.device(self.device):
             L.check(self.lib.t2_wn_init(ctypes.byref(self.cfg), L.ptr(self.packed), L.ptr(self.workspace),
@@ -211,9 +230,23 @@ class WaveNet(object):
                                             L.ptr(self.workspace), L.stream_ptr()))
         self._packed_dirty = False
 
+    def set_speakers(self, speakers):
+        """gin_channels > 0: speaker ids ([B] or [B, 1] ints) of the following forwards, or None for no speaker term (the reference
+        skips it when g is None). The ids are validated here and copied into the workspace, so a captured step uses the ids set last."""
+        if self._spk is None:
+            raise L.T2Error("speaker ids need gin_channels > 0")
+        if speakers is None:
+            L.check(self.lib.t2_wn_set_speakers(ctypes.byref(self.cfg), L.ptr(self.workspace), None, L.stream_ptr()))
+            return
+        self._spk.copy_(speaker_ids(speakers, self.cfg.B, self.cfg.n_speakers))
+        L.check(self.lib.t2_wn_set_speakers(ctypes.byref(self.cfg), L.ptr(self.workspace), L.ptr(self._spk), L.stream_ptr()))
+
     # ---- compute -----------------------------------------------------------------------------------------
-    def forward(self, x, c, targets, lengths, logits=None, save_for_backward=True, seed=None):
-        """x: int32 [B,T] (mulaw-quantize) or fp32 [B,T]; c: fp32 [B,cin,Tc]; returns loss_buf (sum, normaliser)."""
+    def forward(self, x, c, targets, lengths, logits=None, save_for_backward=True, seed=None, speakers=None):
+        """x: int32 [B,T] (mulaw-quantize) or fp32 [B,T]; c: fp32 [B,cin,Tc]; speakers: ids [B] / [B, 1] (gin_channels > 0; None keeps
+        the ids of the last set_speakers, initially none); returns loss_buf (sum, normaliser)."""
+        if speakers is not None:
+            self.set_speakers(speakers)
         if self._packed_dirty:
             self.pack()
         if self.hp.upsample_type == "NearestNeighbor" and c is not None and c.dim() == 3 and c.shape[1] == self.cfg.cin_channels and c.shape[2] != self.cfg.T:
@@ -294,9 +327,11 @@ class WaveNet(object):
         self._fwd_bwd_launches = self.lib.t2_launch_count() - n0
         return self._graph
 
-    def train_step(self, x=None, c=None, targets=None, lengths=None, world_size=1, process_group=None):
+    def train_step(self, x=None, c=None, targets=None, lengths=None, world_size=1, process_group=None, speakers=None):
         """One optimisation step: forward + loss + backward (+ gradient all-reduce) + clip + Adam + EMA.
-        With a captured graph, non-None arguments are copied into the static buffers first."""
+        With a captured graph, non-None arguments are copied into the static buffers first. speakers: as in forward."""
+        if speakers is not None:
+            self.set_speakers(speakers)
         if self._graph is not None and getattr(self, "_graphs", None):
             import torch.distributed as dist
             for dst, src in zip(self._static, (x, c, targets, lengths)):
@@ -414,6 +449,7 @@ class WaveNetSynthesizer(object):
         L.check(self.lib.t2_wn_ar_sizes(ctypes.byref(self.cfg), self.cs, ctypes.byref(pb), ctypes.byref(wb)))
         self.packed = torch.empty(pb.value, dtype=torch.uint8, device=self.device)
         self.workspace = torch.zeros(wb.value, dtype=torch.uint8, device=self.device)
+        self._spk = torch.zeros(B, dtype=torch.int32, device=self.device) if self.cfg.gin_channels > 0 else None
         self.tensors = []
         name = ctypes.create_string_buffer(160)
         off, nd, shp = ctypes.c_longlong(), ctypes.c_int(), (ctypes.c_int * 4)()
@@ -433,9 +469,18 @@ class WaveNetSynthesizer(object):
         from . import init
         self.load_params(init.wavenet_variables(self.hp, self.tensors, seed))
 
-    def generate(self, c, initial, test_inputs=None, u_a=None, u_b=None, seed=0, return_raw=False):
-        """c: fp32 [B,cin,Tc]; initial: int32/fp32 [B]. Returns samples [B,T] (and raw outputs [B,T,out])."""
+    def generate(self, c, initial, test_inputs=None, u_a=None, u_b=None, seed=0, return_raw=False, speakers=None):
+        """c: fp32 [B,cin,Tc]; initial: int32/fp32 [B]; speakers: ids [B] / [B, 1] (gin_channels > 0; None = no speaker term).
+        Returns samples [B,T] (and raw outputs [B,T,out])."""
         B, T = self.cfg.B, self.cfg.T
+        if speakers is not None and self._spk is None:
+            raise L.T2Error("speaker ids need gin_channels > 0")
+        if self._spk is not None:
+            if speakers is not None:
+                self._spk.copy_(speaker_ids(speakers, B, self.cfg.n_speakers))
+            L.check(self.lib.t2_wn_ar_set_speakers(ctypes.byref(self.cfg), self.cs, L.ptr(self.params), L.ptr(self.packed),
+                                                   L.ptr(self.workspace), None if speakers is None else L.ptr(self._spk),
+                                                   L.stream_ptr()))
         if self.hp.upsample_type == "NearestNeighbor" and c is not None and c.dim() == 3 and c.shape[1] == self.cfg.cin_channels and c.shape[2] != T:
             c = nn_upsample(self.hp, c, T)
         scalar = self.cfg.input_type != 2

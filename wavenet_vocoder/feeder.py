@@ -66,7 +66,15 @@ class Feeder(object):
             raise RuntimeError("Linear spectrogram files selected instead of GTA mels, did you specify the wrong metadata?")
         x = np.load(os.path.join(self._base_dir, meta[0]))
         c = np.load(os.path.join(self._base_dir, mel_file)) if self.local_condition else None
+        if self._global_condition():      # speaker id column (feeder.py:184-189)
+            g = meta[3]
+            if g == "<no_g>":
+                raise RuntimeError("Please redo the wavenet preprocessing (or GTA synthesis) to assign global condition features!")
+            return x, c, int(g), len(x)
         return x, c, len(x)
+
+    def _global_condition(self):
+        return (getattr(self._hparams, "gin_channels", None) or 0) > 0
 
     def _next_example(self):
         if self._train_offset >= len(self._train_meta):
@@ -94,7 +102,7 @@ class Feeder(object):
 
     def prepare_batch(self, batch):
         hp = self._hparams
-        items = [self._crop(x, c) for x, c, _ in batch]
+        items = [self._crop(e[0], e[1]) for e in batch]     # examples are (x, c, len), or (x, c, speaker id, len) with gin
         lengths = np.asarray([len(x) for x, _ in items], dtype=np.int32)
         T = int(lengths.max())
         quant = is_mulaw_quantize(hp.input_type)
@@ -108,7 +116,10 @@ class Feeder(object):
         if hp.normalize_for_wavenet:
             c = _interp(c, (lo, hi)).astype(np.float32)
         # inputs == targets (the loss shifts by one sample, wavenet.py:488); y keeps the reference's trailing axis
-        return {"inputs": x, "targets": x[:, :, None], "input_lengths": lengths, "local_condition_features": np.ascontiguousarray(c)}
+        out = {"inputs": x, "targets": x[:, :, None], "input_lengths": lengths, "local_condition_features": np.ascontiguousarray(c)}
+        if self._global_condition():
+            out["global_condition_features"] = np.asarray([[e[2]] for e in batch], dtype=np.int32)   # [B, 1] (feeder.py:94-95)
+        return out
 
     def train_group(self):
         n = self._hparams.wavenet_batch_size

@@ -71,10 +71,11 @@ class WaveNet(object):
     def initialize(self, y, c, g, input_lengths, x=None, synthesis_length=None, test_inputs=None, split_infos=None):
         """wavenet.py:218. Training: x = inputs ([B, T] mu-law indices, one-hot float [B, Q, T], or raw [B, 1, T] / [B, T]),
         y = targets ([B, T] or [B, T, 1]), c = local conditioning [B, cin, Tc], input_lengths [B]. Synthesis (x is None and
-        y is None): c + synthesis_length (+ test_inputs for teacher-forced debugging)."""
+        y is None): c + synthesis_length (+ test_inputs for teacher-forced debugging). g: speaker ids [B, 1] or [B] (gin_channels > 0),
+        or None for no speaker term."""
         hp = self._hparams
-        if g is not None:
-            raise NotImplementedError("global conditioning (gin_channels > 0) is out of scope (SURVEY.md §8)")
+        if g is not None and not self.global_conditioning_enabled():
+            raise ValueError("speaker ids given but gin_channels = %r (global conditioning is off)" % hp.gin_channels)
         self.is_training = x is not None
         self.is_evaluating = not self.is_training and y is not None
         scalar = is_scalar_input(hp.input_type)
@@ -109,6 +110,8 @@ class WaveNet(object):
             ldo = 256 if is_mulaw_quantize(hp.input_type) else 32
             self._logits = torch.empty(B, T, ldo, device=xin.device) if getattr(hp, "keep_logits", False) else None
             eng.training = self.is_training
+            if self.global_conditioning_enabled():
+                eng.set_speakers(g)
             eng.step_dev.add_(1)
             eng.forward(xin, c.float().contiguous(), tin, input_lengths.int().contiguous(), logits=self._logits,
                         save_for_backward=self.is_training)
@@ -151,7 +154,7 @@ class WaveNet(object):
             initial = torch.zeros(B, dtype=torch.float32 if scalar else torch.int32, device=c.device)
             if not scalar:
                 initial.fill_((hp.quantize_channels - 1) // 2)                      # mulaw_quantize(0) (wavenet.py:341-348)
-            out = syn.generate(c.float().contiguous(), initial, test_inputs=test_inputs)
+            out = syn.generate(c.float().contiguous(), initial, test_inputs=test_inputs, speakers=g)
             # wavenet.py:450-456: the published y_hat is the decoded waveform in [-1, 1]
             if is_mulaw_quantize(hp.input_type):
                 out = t2.audio.inv_mulaw_quantize(out.contiguous())

@@ -34,7 +34,8 @@ class Synthesizer(object):
         if maxlen == 0:             # every mel is empty (an untrained Tacotron can fire its stop token on the first frame)
             wavs = np.zeros((len(mel_spectrograms), 0), dtype=np.float32)
         else:
-            self.model.initialize(None, torch.from_numpy(c).cuda(), None, None)   # c: [batch, frames, num_mels] (wavenet.py:408-427)
+            g = None if speaker_ids is None else torch.tensor([[int(s)] for s in speaker_ids], dtype=torch.int32)   # [batch, 1]
+            self.model.initialize(None, torch.from_numpy(c).cuda(), g, None)   # c: [batch, frames, num_mels] (wavenet.py:408-427)
             wavs = self.model.tower_y_hat[0].cpu().numpy()
         names = []
         for w, n, b in zip(wavs, audio_lengths, basenames):

@@ -19,10 +19,11 @@ log = infolog.log
 def _run_model(model, b, training):
     x = b["inputs"]
     y = b["targets"]
+    g = b.get("global_condition_features")      # speaker ids [B, 1] when gin_channels > 0
     if training:
-        model.initialize(y, b["local_condition_features"], None, b["input_lengths"], x=x)
+        model.initialize(y, b["local_condition_features"], g, b["input_lengths"], x=x)
     else:
-        model.initialize(y, b["local_condition_features"], None, b["input_lengths"])
+        model.initialize(y, b["local_condition_features"], g, b["input_lengths"])
     return model.add_loss()
 
 
