@@ -285,6 +285,14 @@ typedef struct {
                               * (sum / count_nonzero of the mask), stop-token loss = weighted sigmoid CE over the same frames divided by the
                               * number of NON-ZERO masked terms; the lengths come from t2_taco_set_target_lengths */
   float cross_entropy_pos_weight;  /* pos_weight of tf.nn.weighted_cross_entropy_with_logits (masked stop-token loss only) */
+  float teacher_forcing_ratio;     /* tacotron_teacher_forcing_ratio in [0, 1] ('constant' mode, helpers.py:115-128) of t2_taco_forward /
+                              * t2_taco_backward; anything else is T2_ERR_INVALID_ARG. 1 = full teacher forcing: the prenet, the LSTM-1 input
+                              * projection and the frame / stop projections run batched over all T_out steps. < 1: at the end of decoder step t
+                              * ONE draw u_t (hash stream 40, element t) decides for the whole batch: u_t < ratio feeds step t + 1 the target
+                              * frame t, otherwise the raw (bias added, un-clipped) frame it just predicted, and the backward pass
+                              * differentiates through the fed-back frames. That path runs the prenet, the input projection and the
+                              * projections once per step. Workspace "teacher_forced" int32 [T_out] holds the choices of the last forward
+                              * (element t = 1: step t + 1 consumed the target). Free-running synthesis ignores the field. */
 } t2_taco_config_t;
 
 int t2_taco_sizes(const t2_taco_config_t* cfg, long long* n_params, long long* packed_bytes, long long* workspace_bytes,
@@ -336,7 +344,9 @@ int t2_taco_infer_finish(const t2_taco_config_t* cfg, float* d_params, const voi
  * t2_taco_forward / t2_wn_forward plus the device step counter). Element kept / updated iff d_out[i] >= rate.
  * Tacotron stream ids: encoder conv dropout 10+i, prenet 20 / 21, postnet conv dropout 30+i (element = linear index of
  * the layer output), zoneout (c, h) = 2*s, 2*s+1 with s = 52 / 53 (encoder fw / bw), 54 / 55 (decoder LSTM 1 / 2) and
- * element = (t*B + b)*H + unit. Replaces tf.layers.dropout / tf.nn.dropout draws of tacotron/models/modules.py:133-134,249,389. */
+ * element = (t*B + b)*H + unit; the teacher-forcing draw (teacher_forcing_ratio < 1) is stream 40, element = decoder step t.
+ * Replaces tf.layers.dropout / tf.nn.dropout draws of tacotron/models/modules.py:133-134,249,389 and the tf.random_uniform([])
+ * of tacotron/models/helpers.py:121. */
 int t2_rng_uniform_f32(unsigned long long seed, unsigned int stream_id, long long first_index, long long n, float* d_out,
                        void* stream);
 int t2_dbg_att_stamps(long long* d_buf);

@@ -401,7 +401,9 @@ struct Epilogue<EPI_RES, BN> {
 
 // out = dropout(act(acc + bias)).  ptr: 0 out bf16 [pos, ldo] (nullable), 1 bias fp32 (nullable), 2 out fp32
 // [pos, ldo] (nullable), 7 device u64 seed offset (nullable);  i0 = ldo, i1 = act (0 none, 1 relu, 2 tanh),
-// i2 = n_valid columns, i3 = dropout hash stream;  f1 = dropout rate (0 = off; mask = hash(seed, stream, pos*ldo + col))
+// i2 = n_valid columns, i3 = dropout hash stream, i4 = position offset of the dropout hash;  f1 = dropout rate (0 = off;
+// mask = hash(seed, stream, (i4 + pos)*ldo + col)): a launch over rows [i4, i4 + T*B) of a larger matrix draws the same mask as
+// one launch over the whole matrix
 template <int BN>
 struct Epilogue<EPI_BIAS_ACT, BN> {
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
@@ -410,6 +412,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
     const float* bias = static_cast<const float*>(e.ptr[1]);
     float* of = static_cast<float*>(e.ptr[2]);
     const size_t row = (size_t(c.b) * c.T + c.t) * ldo;
+    const size_t hrow = row + size_t(e.i[4]) * ldo;
     uint8_t* t_o = c.tile(0);
     const float pdrop = e.f[1];
     const float keep_inv = 1.f / (1.f - pdrop);
@@ -463,7 +466,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
           if (bias && c0 + j < nvalid) v += __ldg(bias + c0 + j);
           if (act == 1) v = fmaxf(v, 0.f);
           else if (act == 2) v = tanhf_(v);
-          if (pdrop > 0.f) v = (hash_uniform32(hs, row + c0 + j) >= pdrop) ? v * keep_inv : 0.f;
+          if (pdrop > 0.f) v = (hash_uniform32(hs, hrow + c0 + j) >= pdrop) ? v * keep_inv : 0.f;
           acc[j] = v;
         }
         if (ob && full) stage_put_sw(t_o, c.lane, cq, acc);

@@ -64,6 +64,7 @@ struct TL {  // layout
   long long w_dctxl, w_dctx_all, w_dq_all, w_dcum, w_cumrun, w_dkeys, w_dvalues, w_attacc, w_dpn2, w_dpn1;
   long long w_dencpre[2], w_dx3, w_encdh[2], w_encdc[2], w_encdg, w_demb, w_tiles, w_packjobs, w_regtab;
   long long w_ddecf, w_encdgall[2], w_dkeysb, w_dz, w_attU;
+  long long w_tfsel, w_dfb;   // teacher_forcing_ratio < 1: per-step choices int32 [To], d(fed-back frame) fp32 [B][M]
   std::vector<int> tile_off, tile_cnt;  // per wgrad launch (fixed order, see build_tiles)
   long long workspace_bytes;
   int n_packjobs, n_reg;
@@ -99,6 +100,8 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
   T2_REQUIRE(lo.M % 8 == 0 && lo.M + 1 <= 128 && lo.Ti <= 1024, T2_ERR_UNSUPPORTED_SHAPE, "num_mels / T_in");
   T2_REQUIRE(cfg->enc_conv_layers >= 1 && cfg->enc_conv_layers <= 8 && cfg->postnet_layers >= 1 && cfg->postnet_layers <= 8,
              T2_ERR_INVALID_ARG, "layer counts");
+  T2_REQUIRE(cfg->teacher_forcing_ratio >= 0.f && cfg->teacher_forcing_ratio <= 1.f, T2_ERR_INVALID_ARG,
+             "teacher_forcing_ratio %g outside [0, 1]", double(cfg->teacher_forcing_ratio));
   // ---- parameters (order == oracle/tacotron.py:param_shapes) ----
   lo.n_params = 0; lo.params.clear(); lo.enc.clear(); lo.post.clear();
   lo.p_emb = addp(lo, "inputs_embedding", {lo.NS, lo.E});
@@ -282,6 +285,8 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
   for (auto& p : lo.params) lo.n_reg += p.reg ? 1 : 0;
   lo.w_regtab = takeb((long long)lo.n_reg * 2 * sizeof(long long));
   lo.w_zero = takeb(B * 4096 * 4);
+  lo.w_tfsel = takeb(To * 4);
+  lo.w_dfb = takeb(B * lo.M * 4);
   lo.workspace_bytes = o;
   if (jobs_out) jobs_out->swap(jobs);
   return T2_OK;
@@ -810,6 +815,27 @@ __global__ void proj_bias_kernel(float* p, const float* fb, const float* sb, lon
   const int m = int(e % (M + 1));
   p[(e / (M + 1)) * 128 + m] += m < M ? fb[m] : sb[0];
 }
+constexpr uint32_t kTfStream = 40;   // hash stream of the per-step teacher-forcing draw (include/t2b200.h)
+// projo[t] += bias; next decoder input = the raw (un-clipped) frame just predicted (helpers.py:56). With tgt (TacoTrainingHelper at a
+// teacher-forcing ratio < 1, helpers.py:115-128): ONE draw u_t for the whole batch (stream kTfStream, element t, under seed + *step);
+// u_t < ratio feeds the target frame tgt[b][t] instead, and choice[t] records which of the two step t + 1 consumed.
+__global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __restrict__ fb, const float* __restrict__ sb, bf16* __restrict__ next_in,
+                                          int B, int M, const float* __restrict__ tgt, int To, int t, float ratio, unsigned long long seed,
+                                          const unsigned long long* __restrict__ step, int* __restrict__ choice) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= B * (M + 1)) return;
+  bool forced = false;
+  if (tgt) {
+    forced = hash_uniform32(hash_seed(seed + (step ? *step : 0ull), kTfStream), (unsigned long long)t) < ratio;
+    if (e == 0) choice[t] = forced ? 1 : 0;
+  }
+  const int m = e % (M + 1), b = e / (M + 1);
+  const float v = p[b * 128 + m] + (m < M ? fb[m] : sb[0]);
+  p[b * 128 + m] = v;
+  if (m < M && next_in) next_in[b * M + m] = __float2bfloat16(forced ? tgt[((long long)b * To + t) * M + m] : v);
+}
 // normalisers -> s[5] (mel terms), s[6] (stop term); out (nullable) = the four normalised loss terms
 __global__ void loss_norm_kernel(float* s, float* out, float n_mel, float n_stop, float regw, const int* tlen, int B, int To, int M) {
   if (tlen) {
@@ -825,10 +851,11 @@ __global__ void loss_norm_kernel(float* s, float* out, float n_mel, float n_stop
 // generic helper: 1x1 / k-tap conv GEMM through the engine
 // split != 0 ("fp32-class" conv stacks): the input rows are [hi | lo], each half `C` channels zero-padded to Cp = ceil(C / 64) * 64; per
 // tap one segment over both halves against [W_hi | W_hi] and one over the hi half against [W_lo] (wK = 3 * ntaps * Cp); a bf16 output is
-// written as [hi(ldo) | lo(ldo)]
+// written as [hi(ldo) | lo(ldo)]. hash_row0: position offset of the dropout mask (a launch over the rows of one decoder step draws
+// the elements of those rows in the batched [T_out * B] launch)
 int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, int wK, int ntaps, const int* shifts, int BN, float* bias,
               int act, void* out_bf16, float* out_f32, int ldo, int nvalid, float pdrop, int stream_id, unsigned long long seed,
-              const unsigned long long* d_step, cudaStream_t st, int split = 0) {
+              const unsigned long long* d_step, cudaStream_t st, int split = 0, int hash_row0 = 0) {
   ActGemmCall g;
   memset(&g, 0, sizeof(g));
   const int nkb = (C + kBK - 1) / kBK;
@@ -850,7 +877,8 @@ int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, i
   g.w = w; g.wN = N; g.wK = wK; g.wL = 1;
   g.T = int(T); g.B = Bn; g.n_tiles = (nvalid + BN - 1) / BN;
   g.epi.ptr[0] = out_bf16; g.epi.ptr[1] = bias; g.epi.ptr[2] = out_f32; g.epi.ptr[7] = const_cast<unsigned long long*>(d_step);
-  g.epi.i[0] = ldo; g.epi.i[1] = act; g.epi.i[2] = nvalid; g.epi.i[3] = stream_id; g.epi.f[1] = pdrop; g.epi.seed = seed;
+  g.epi.i[0] = ldo; g.epi.i[1] = act; g.epi.i[2] = nvalid; g.epi.i[3] = stream_id; g.epi.i[4] = hash_row0; g.epi.f[1] = pdrop;
+  g.epi.seed = seed;
   return launch_act_gemm(EPI_BIAS_ACT, BN, g, st);
 }
 
@@ -970,12 +998,15 @@ __global__ void loss_seed_kernel(const float* __restrict__ dec_f, const float* _
   }
   dmel[e] = __float2bfloat16(g);
 }
-// ddec_tm[t][b][0..M) = (ddec_direct + ddec_post)[b][t][:] * [decoder clip inactive] ; col M = d BCE / d stop logit
+// ddec_tm[t][b][0..M) = (ddec_direct + ddec_post)[b][t][:] * [decoder clip inactive] ; col M = d BCE / d stop logit; steps [t0, t1).
+// fb (teacher_forcing_ratio < 1, one step): + fb[b][:] = d(loss)/d(input frame of step t + 1) when that step consumed the frame step t
+// predicted (choice[t] == 0). The fed-back frame is the raw projection output, so this term does not pass the clip mask.
 __global__ void ddec_tm_kernel(const float* __restrict__ ddec, const bf16* __restrict__ dpost, const float* __restrict__ projo,
                                const float* __restrict__ stop_tgt, bf16* __restrict__ out, int B, int To, int M, int clip, float lo, float hi,
-                               const int* __restrict__ tlen, float pos_w, const float* __restrict__ scal) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)To * B * 128) return;
+                               const int* __restrict__ tlen, float pos_w, const float* __restrict__ scal, int t0, int t1,
+                               const float* __restrict__ fb, const int* __restrict__ choice) {
+  const long long e = (long long)t0 * B * 128 + blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= (long long)t1 * B * 128) return;
   const int m = int(e % 128), b = int((e / 128) % B), t = int(e / (128LL * B));
   float g = 0.f;
   if (m < M) {
@@ -983,6 +1014,7 @@ __global__ void ddec_tm_kernel(const float* __restrict__ ddec, const bf16* __res
     g = ddec[o] + __bfloat162float(dpost[o]);
     const float raw = projo[((long long)t * B + b) * 128 + m];
     if (clip && (raw < lo || raw > hi)) g = 0.f;
+    if (fb && !choice[t]) g += fb[(long long)b * M + m];
   } else if (m == M) {
     const float x = projo[((long long)t * B + b) * 128 + M];
     const float z = stop_tgt[(long long)b * To + t];
@@ -1612,38 +1644,66 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   rc = encoder_fwd(s, d_inputs, d_input_lengths, training);
   if (rc) return rc;
   const void* x = nullptr;
-  // ---- decoder: everything that does not depend on the recurrence is batched over time (teacher forcing) ----
   bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
   decin_kernel<<<g1((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M); t2_count_launch();
   const long long TB = (long long)To * B;
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
-  rc = conv_gemm(decin, lo.M, TB, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, pn1, nullptr, lo.P1,
-                 lo.P1, lo.c.dropout_rate, 20, seed, d_step, st);
-  if (rc) return rc;
-  rc = conv_gemm(pn1, lo.P1, TB, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, pn2, nullptr, lo.P2,
-                 lo.P2, lo.c.dropout_rate, 21, seed, d_step, st);
-  if (rc) return rc;
   float* pre1 = reinterpret_cast<float*>(ws + lo.w_pre1);
-  rc = conv_gemm(pn2, lo.P2, TB, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr, pre1, 4 * D, 4 * D, 0.f, 0, 0,
-                 nullptr, st);
-  if (rc) return rc;
+  float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
   const int PIK = D + 2 * H;
   DecBufs db;
-  rc = decoder_reset(s, db);
-  if (rc) return rc;
-  bf16* PI = db.PI;
-  for (int t = 0; t < To; ++t) { rc = decoder_step(s, db, d_input_lengths, t); if (rc) return rc; }
-  T2_CHECK_CUDA(cudaGetLastError());
-  // frame + stop projections for all steps at once
-  float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
-  {
-    // bias vector [M frames | 1 stop] lives in two parameter tensors: add them in the finishing kernel instead
-    rc = conv_gemm(PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st);
+  if (lo.c.teacher_forcing_ratio >= 1.f) {
+    // ---- decoder: everything that does not depend on the recurrence is batched over time (teacher forcing) ----
+    rc = conv_gemm(decin, lo.M, TB, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, pn1, nullptr, lo.P1,
+                   lo.P1, lo.c.dropout_rate, 20, seed, d_step, st);
     if (rc) return rc;
+    rc = conv_gemm(pn1, lo.P1, TB, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, pn2, nullptr, lo.P2,
+                   lo.P2, lo.c.dropout_rate, 21, seed, d_step, st);
+    if (rc) return rc;
+    rc = conv_gemm(pn2, lo.P2, TB, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr, pre1, 4 * D, 4 * D, 0.f, 0, 0,
+                   nullptr, st);
+    if (rc) return rc;
+    rc = decoder_reset(s, db);
+    if (rc) return rc;
+    for (int t = 0; t < To; ++t) { rc = decoder_step(s, db, d_input_lengths, t); if (rc) return rc; }
+    T2_CHECK_CUDA(cudaGetLastError());
+    // frame + stop projections for all steps at once
+    // bias vector [M frames | 1 stop] lives in two parameter tensors: add them in the finishing kernel instead
+    rc = conv_gemm(db.PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st);
+    if (rc) return rc;
+    // add the projection biases in place (tiny), then clip / losses
+    proj_bias_kernel<<<g1(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
+  } else {
+    // ---- decoder at a teacher-forcing ratio < 1: step t + 1's input is known only once step t has drawn and projected, so the
+    // prenet, the LSTM-1 input projection and the projections run per step (the loop of t2_taco_infer_steps). The prenet masks are the
+    // elements the batched launches draw (hash row offset t * B), so a step that takes the target repeats the batched arithmetic. ----
+    rc = decoder_reset(s, db);
+    if (rc) return rc;
+    int* choice = reinterpret_cast<int*>(ws + lo.w_tfsel);
+    for (int t = 0; t < To; ++t) {
+      rc = conv_gemm(decin + (long long)t * B * lo.M, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b,
+                     1, pn1 + (long long)t * B * lo.P1, nullptr, lo.P1, lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, 0, t * B);
+      if (rc) return rc;
+      rc = conv_gemm(pn1 + (long long)t * B * lo.P1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128,
+                     d_params + lo.p_p2b, 1, pn2 + (long long)t * B * lo.P2, nullptr, lo.P2, lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, 0, t * B);
+      if (rc) return rc;
+      rc = conv_gemm(pn2 + (long long)t * B * lo.P2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
+                     pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st);
+      if (rc) return rc;
+      rc = decoder_step(s, db, d_input_lengths, t);
+      if (rc) return rc;
+      float* pt = projo + (long long)t * B * 128;
+      rc = conv_gemm(db.PI + (long long)t * B * PIK, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
+                     lo.M + 1, 0.f, 0, 0, nullptr, st);
+      if (rc) return rc;
+      T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(g1((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
+                               d_params + lo.p_sb, t + 1 < To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M, d_mel_targets, To, t,
+                               lo.c.teacher_forcing_ratio, seed, d_step, choice));
+      t2_count_launch();
+    }
+    T2_CHECK_CUDA(cudaGetLastError());
   }
-  // add the projection biases in place (tiny), then clip / losses
-  proj_bias_kernel<<<g1(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
   bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
   float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
@@ -1669,19 +1729,6 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
 // ======================================================================================================
 // free-running synthesis (TacoTestHelper, helpers.py:6-59; tacotron.py:150-200 with is_training = False)
 // ======================================================================================================
-// projo[t] += bias; next decoder input = the raw (un-clipped) frame just predicted (helpers.py:56)
-__global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __restrict__ fb, const float* __restrict__ sb, bf16* __restrict__ next_in,
-                                          int B, int M) {
-  pdl_wait();
-  pdl_launch_dependents();
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= B * (M + 1)) return;
-  const int m = e % (M + 1), b = e / (M + 1);
-  const float v = p[b * 128 + m] + (m < M ? fb[m] : sb[0]);
-  p[b * 128 + m] = v;
-  if (m < M && next_in) next_in[b * M + m] = __float2bfloat16(v);
-}
-
 // encoder + zero decoder state + go frame. inputs int32 [B][T_in], lengths int32 [B].
 extern "C" int t2_taco_infer_begin(const t2_taco_config_t* cfg, float* d_params, const void* d_packed, void* d_workspace, const int* d_inputs,
                                    const int* d_input_lengths, void* stream) {
@@ -1747,7 +1794,8 @@ extern "C" int t2_taco_infer_steps(const t2_taco_config_t* cfg, float* d_params,
                    0.f, 0, 0, nullptr, st);
     if (rc) return rc;
     T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(g1((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
-                             d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M));
+                             d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M,
+                             (const float*)nullptr, lo.To, t, 0.f, 0ull, (const unsigned long long*)nullptr, (int*)nullptr));
     t2_count_launch();
   }
   T2_CHECK_CUDA(cudaGetLastError());
@@ -1804,6 +1852,7 @@ extern "C" int t2_taco_workspace_tensor(const t2_taco_config_t* cfg, void* d_wor
       {"decoder_output", lo.w_decf, B * To * lo.M, 4}, {"mel_outputs", lo.w_mel, B * To * lo.M, 4}, {"stop_logits", lo.w_stop, B * To, 4},
       {"projection_rows", lo.w_projo, To * B * 128, 4}, {"enc_conv_out", lo.enc.back().w_x, B * Ti * lo.C, 2}, {"prenet", lo.w_pn2, To * B * lo.P2, 2}, {"proj_in", lo.w_PI, To * B * (lo.D + 2 * lo.H), 2},
       {"attention_filter_bank", lo.w_attU, (lo.KA + 1) * lo.A, 4},   // merged location filters U [KA][A] + offset row u0
+      {"teacher_forced", lo.w_tfsel, To, 4},   // int32 per-step choices of the last forward at teacher_forcing_ratio < 1
   };
   for (const E& e : table)
     if (strcmp(e.n, name) == 0) { *ptr = ws + e.off; *count = e.cnt; *elem_bytes = e.eb; return T2_OK; }
@@ -1890,7 +1939,13 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     rc = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, To, B, st); if (rc) return rc; ++li;
     colsum_bf16_kernel<<<64, 256, 0, st>>>(dmel, BTo, M, 128, d_grads + lo.p_ppb, 1.f); t2_count_launch();
   }
-  bf16* ddec_post = reinterpret_cast<bf16*>(ws + lo.w_dz);
+  // teacher_forcing_ratio < 1: the frame projection's gradient of step t waits for step t + 1's prenet backward inside the loop below,
+  // which writes the prenet gradients into w_dz step by step; the decoder-output gradient then goes to dY0 (the first postnet block's
+  // output gradient is dead once its batch-norm backward has run)
+  const bool per_step = lo.c.teacher_forcing_ratio < 1.f;
+  T2_REQUIRE(!per_step || (To > Ti ? To : Ti) * (long long)(lo.PC > lo.C ? lo.PC : lo.C) >= (long long)To * M, T2_ERR_UNSUPPORTED_SHAPE,
+             "teacher_forcing_ratio < 1 needs postnet_channels or enc_conv_channels >= num_mels");
+  bf16* ddec_post = per_step ? dY0 : reinterpret_cast<bf16*>(ws + lo.w_dz);
   for (int i = int(lo.post.size()) - 1; i >= 0; --i) {
     const void* xin = i > 0 ? (const void*)(ws + lo.post[i - 1].w_x) : (const void*)dec_bm;
     rc = conv_block_bwd(s, lo.post[i], xin, To, dY0, dY1, i > 0 ? dY0 : ddec_post, d_grads, TILES(li), NT(li));
@@ -1900,19 +1955,24 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   // ---- projections ----
   bf16* ddec_tm = reinterpret_cast<bf16*>(ws + lo.w_ddec_tm);
   float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
-  ddec_tm_kernel<<<g1(TB * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c, hi_c, tlen,
-                                               lo.c.cross_entropy_pos_weight, scal);
-  t2_count_launch();
   float* dPI = reinterpret_cast<float*>(ws + lo.w_dPI);
-  rc = conv_gemm(ddec_tm, 128, TB, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dPI, PIK, PIK, 0.f, 0, 0,
-                 nullptr, st);
-  if (rc) return rc;
   bf16* PI = reinterpret_cast<bf16*>(ws + lo.w_PI);
-  {
+  auto proj_wgrad = [&]() -> int {
     ActT maps[2] = {make_act(PI, PIK, int(TB), 1), make_act(ddec_tm, 128, int(TB), 1)};
-    rc = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, int(TB), 1, st); if (rc) return rc; ++li;
+    int r = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, int(TB), 1, st); if (r) return r; ++li;
     colsum_bf16_kernel<<<64, 256, 0, st>>>(ddec_tm, TB, M, 128, d_grads + lo.p_fb, 1.f); t2_count_launch();
     colsum_bf16_kernel<<<64, 256, 0, st>>>(ddec_tm + M, TB, 1, 128, d_grads + lo.p_sb, 1.f); t2_count_launch();
+    return T2_OK;
+  };
+  if (!per_step) {
+    ddec_tm_kernel<<<g1(TB * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c, hi_c, tlen,
+                                                 lo.c.cross_entropy_pos_weight, scal, 0, To, nullptr, nullptr);
+    t2_count_launch();
+    rc = conv_gemm(ddec_tm, 128, TB, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dPI, PIK, PIK, 0.f, 0, 0,
+                   nullptr, st);
+    if (rc) return rc;
+    rc = proj_wgrad();
+    if (rc) return rc;
   }
   // ---- decoder: backward through time ----
   float* dh1ext = reinterpret_cast<float*>(ws + lo.w_dh1ext);
@@ -1942,7 +2002,25 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   const size_t ab_smem = att_bwd_smem(Ti, lo.KA, A, D, 2 * H);
   const float* attU = reinterpret_cast<const float*>(ws + lo.w_attU);
   T2_CHECK_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ab_smem)));
+  bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
+  bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
+  bf16* dpn2 = reinterpret_cast<bf16*>(ws + lo.w_dpn2);
+  bf16* dpn1 = reinterpret_cast<bf16*>(ws + lo.w_dpn1);
+  bf16* dz2 = reinterpret_cast<bf16*>(ws + lo.w_dz);
+  float* dfb = reinterpret_cast<float*>(ws + lo.w_dfb);
+  const int* choice = reinterpret_cast<const int*>(ws + lo.w_tfsel);
   for (int t = To - 1; t >= 0; --t) {
+    if (per_step) {
+      // loss gradient of step t's projection outputs + (when step t + 1 consumed step t's frame) the gradient of step t + 1's input,
+      // left in dfb by the previous iteration; then dPI_t through the frame / stop projections
+      ddec_tm_kernel<<<g1((long long)B * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c,
+                                                            hi_c, tlen, lo.c.cross_entropy_pos_weight, scal, t, t + 1,
+                                                            t + 1 < To ? dfb : nullptr, choice);
+      t2_count_launch();
+      rc = conv_gemm(ddec_tm + (long long)t * B * 128, 128, B, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0,
+                     nullptr, dPI + (long long)t * B * PIK, PIK, PIK, 0.f, 0, 0, nullptr, st);
+      if (rc) return rc;
+    }
     AttBwd a;
     a.h2out = PI + (long long)t * B * PIK; a.ld_h2 = PIK; a.WqT = reinterpret_cast<const bf16*>(pk + lo.k_qT); a.Wq = d_params + lo.p_qry;
     a.U = attU; a.v = d_params + lo.p_v;
@@ -1968,11 +2046,29 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     rc = launch_cell_bwd(c1, st); if (rc) return rc;
     rc = lstm_bwd_gemm(s, pk + lo.k_l1rT, K1r, 4 * D, c1.dg_a, B, dctxl, 2 * H, 2 * H, 2, dhs1, D, 2, ks_dec);  // dctxl: zeroed by att_bwd
     if (rc) return rc;
+    if (per_step) {
+      // the input part of LSTM-1's gate gradient back through the input projection and both prenet layers (ReLU + dropout), into the
+      // [T_out * B] buffers of the batched path; for t >= 1 on to d(input frame of step t) = dfb
+      const long long r2 = (long long)t * B * lo.P2, r1 = (long long)t * B * lo.P1;
+      rc = conv_gemm(c1.dg_a, 4 * D, B, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2 + r2, nullptr,
+                     lo.P2, lo.P2, 0.f, 0, 0, nullptr, st);
+      if (rc) return rc;
+      relu_drop_bwd_kernel<<<g1((long long)B * lo.P2), 256, 0, st>>>(dpn2 + r2, pn2 + r2, dz2 + r2, (long long)B * lo.P2, lo.c.dropout_rate);
+      t2_count_launch();
+      rc = conv_gemm(dz2 + r2, lo.P2, B, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1 + r1, nullptr,
+                     lo.P1, lo.P1, 0.f, 0, 0, nullptr, st);
+      if (rc) return rc;
+      relu_drop_bwd_kernel<<<g1((long long)B * lo.P1), 256, 0, st>>>(dpn1 + r1, pn1 + r1, dpn1 + r1, (long long)B * lo.P1, lo.c.dropout_rate);
+      t2_count_launch();
+      if (t >= 1) {
+        rc = conv_gemm(dpn1 + r1, lo.P1, B, 1, pk + lo.k_p1T, M, lo.P1, 1, nullptr, 128, nullptr, 0, nullptr, dfb, M, M, 0.f, 0, 0, nullptr, st);
+        if (rc) return rc;
+      }
+    }
   }
   T2_CHECK_CUDA(cudaGetLastError());
+  if (per_step) { rc = proj_wgrad(); if (rc) return rc; }
   // ---- recurrent / prenet weight gradients: one wgrad GEMM over all steps ----
-  bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
-  bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
   {
     ActT maps[5] = {make_act(ws + lo.w_S2, K2, int(TB), 1), make_act(dg2, 4 * D, int(TB), 1), make_act(ws + lo.w_S1, K1r, int(TB), 1),
                     make_act(dg1, 4 * D, int(TB), 1), make_act(pn2, lo.P2, int(TB), 1)};
@@ -1980,17 +2076,16 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     colsum_bf16_kernel<<<64, 256, 0, st>>>(dg2, TB, 4 * D, 4 * D, d_grads + lo.p_l2b, 1.f); t2_count_launch();
     colsum_bf16_kernel<<<64, 256, 0, st>>>(dg1, TB, 4 * D, 4 * D, d_grads + lo.p_l1b, 1.f); t2_count_launch();
   }
-  bf16* dpn2 = reinterpret_cast<bf16*>(ws + lo.w_dpn2);
-  bf16* dpn1 = reinterpret_cast<bf16*>(ws + lo.w_dpn1);
-  bf16* dz2 = reinterpret_cast<bf16*>(ws + lo.w_dz);
-  rc = conv_gemm(dg1, 4 * D, TB, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2, nullptr, lo.P2, lo.P2, 0.f, 0,
-                 0, nullptr, st);
-  if (rc) return rc;
-  relu_drop_bwd_kernel<<<g1(TB * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, TB * lo.P2, lo.c.dropout_rate); t2_count_launch();
-  rc = conv_gemm(dz2, lo.P2, TB, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1, nullptr, lo.P1, lo.P1, 0.f, 0, 0,
-                 nullptr, st);
-  if (rc) return rc;
-  relu_drop_bwd_kernel<<<g1(TB * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, TB * lo.P1, lo.c.dropout_rate); t2_count_launch();
+  if (!per_step) {   // prenet data gradients over all steps (the per-step path wrote them inside the loop)
+    rc = conv_gemm(dg1, 4 * D, TB, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2, nullptr, lo.P2, lo.P2, 0.f,
+                   0, 0, nullptr, st);
+    if (rc) return rc;
+    relu_drop_bwd_kernel<<<g1(TB * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, TB * lo.P2, lo.c.dropout_rate); t2_count_launch();
+    rc = conv_gemm(dz2, lo.P2, TB, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1, nullptr, lo.P1, lo.P1, 0.f, 0,
+                   0, nullptr, st);
+    if (rc) return rc;
+    relu_drop_bwd_kernel<<<g1(TB * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, TB * lo.P1, lo.c.dropout_rate); t2_count_launch();
+  }
   {
     ActT maps[6] = {make_act(pn1, lo.P1, int(TB), 1), make_act(dz2, lo.P2, int(TB), 1), make_act(ws + lo.w_decin, M, int(TB), 1),
                     make_act(dpn1, lo.P1, int(TB), 1), make_act(PI, PIK, int(TB), 1), make_act(dq_all, A, int(TB), 1)};

@@ -16,7 +16,8 @@ class TacoConfig(ctypes.Structure):
         "enc_conv_channels", "encoder_lstm_units", "attention_dim", "attention_filters", "attention_kernel", "prenet1",
         "prenet2", "decoder_lstm_units", "postnet_layers", "postnet_kernel", "postnet_channels", "clip_outputs")] + [
         (n, ctypes.c_float) for n in ("dropout_rate", "zoneout_rate", "reg_weight", "max_abs_value", "lower_bound_decay")] + [
-        ("split_bf16", ctypes.c_int), ("mask_decoder", ctypes.c_int), ("cross_entropy_pos_weight", ctypes.c_float)]
+        ("split_bf16", ctypes.c_int), ("mask_decoder", ctypes.c_int), ("cross_entropy_pos_weight", ctypes.c_float),
+        ("teacher_forcing_ratio", ctypes.c_float)]
 
 
 class CbhgConfig(ctypes.Structure):
@@ -68,7 +69,7 @@ def unsupported_hparams(hp):
     need("batch_norm_position", lambda v: v == "after", "batch norm before the activation: modules.py:386-389")
     need("mask_encoder", lambda v: bool(v), "un-masked encoder memory")
     need("tacotron_teacher_forcing_mode", lambda v: v == "constant", "scheduled teacher forcing: helpers.py:135-169")
-    need("tacotron_teacher_forcing_ratio", lambda v: float(v) == 1.0, "per-step teacher-forcing draw: helpers.py:121-124")
+    need("tacotron_teacher_forcing_ratio", lambda v: 0.0 <= float(v) <= 1.0, "teacher-forcing ratio outside [0, 1]: helpers.py:121-124")
     need("synthesis_constraint", lambda v: not v, "attention window / monotonic constraint at synthesis: attention.py:201-214")
     need("tacotron_natural_eval", lambda v: not v, "evaluation that feeds the model its own predictions: helpers.py:97-100")
     if not getattr(hp, "mask_decoder", False):
@@ -76,7 +77,8 @@ def unsupported_hparams(hp):
     return bad
 
 
-def make_config(hp, B, T_in, T_out, precision="bf16"):
+def make_config(hp, B, T_in, T_out, precision="bf16", teacher_forcing_ratio=None):
+    """teacher_forcing_ratio: None = hparams.tacotron_teacher_forcing_ratio ('constant' mode); GTA passes 1 (helpers.py:101-102)"""
     if precision not in ("bf16", "fp32-class"):
         raise L.T2Error("precision must be 'bf16' or 'fp32-class'")
     bad = unsupported_hparams(hp)
@@ -100,18 +102,24 @@ def make_config(hp, B, T_in, T_out, precision="bf16"):
     c.split_bf16 = int(precision == "fp32-class")
     c.mask_decoder = int(bool(hp.mask_decoder))
     c.cross_entropy_pos_weight = float(hp.cross_entropy_pos_weight)
+    ratio = float(getattr(hp, "tacotron_teacher_forcing_ratio", 1.0) if teacher_forcing_ratio is None else teacher_forcing_ratio)
+    if not 0.0 <= ratio <= 1.0:
+        raise L.T2Error("teacher_forcing_ratio %r outside [0, 1]" % (ratio,))
+    c.teacher_forcing_ratio = ratio
     return c
 
 
 class Tacotron(object):
-    def __init__(self, hparams, B, T_in, T_out, device="cuda", precision="bf16"):
+    def __init__(self, hparams, B, T_in, T_out, device="cuda", precision="bf16", teacher_forcing_ratio=None):
         """precision 'fp32-class': the convolution stacks (encoder convs, postnet) run on bf16 hi + lo operand pairs with fp32
-        pre-batch-norm activations; forward / losses only (include/t2b200.h, t2_taco_config_t.split_bf16)."""
+        pre-batch-norm activations; forward / losses only (include/t2b200.h, t2_taco_config_t.split_bf16).
+        teacher_forcing_ratio (default hparams.tacotron_teacher_forcing_ratio): below 1, every decoder step of forward() draws whether
+        the next step consumes the target frame or the frame just predicted, and backward() differentiates through the fed-back frames."""
         self.hp = hparams
         self.lib = L.load()
         self.device = torch.device(device)
         self.precision = precision
-        self.cfg = make_config(hparams, B, T_in, T_out, precision)
+        self.cfg = make_config(hparams, B, T_in, T_out, precision, teacher_forcing_ratio)
         n, pb, wb, nt = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_int()
         L.check(self.lib.t2_taco_sizes(ctypes.byref(self.cfg), ctypes.byref(n), ctypes.byref(pb), ctypes.byref(wb), ctypes.byref(nt)))
         self.n_taco = n.value
@@ -398,6 +406,11 @@ class Tacotron(object):
         L.check(self.lib.t2_rng_uniform_f32(ctypes.c_ulonglong(seed), ctypes.c_uint(stream_id), ctypes.c_longlong(first_index),
                                             ctypes.c_longlong(n), L.ptr(out), L.stream_ptr()))
         return out
+
+    def teacher_forcing_choices(self):
+        """bool [T_out] of the last forward at a teacher-forcing ratio < 1: element t is True when step t + 1 consumed the target
+        frame t, False when it consumed the frame step t predicted (the draw of element t, hash stream 40, is below the ratio)"""
+        return self.workspace_tensor("teacher_forced").view(torch.int32) != 0
 
     def losses(self):
         b, a, s, r = self.loss_buf.tolist()

@@ -1,8 +1,8 @@
 """Python surface of the reference's Tacotron class (tacotron/models/tacotron.py) on top of libt2b200.
 
 As in wavenet_vocoder/models/wavenet.py of this repo, the TF1 graph-building calls execute eagerly:
-`initialize(...)` runs the encoder / decoder / postnet (teacher-forced for training, evaluation and GTA, free-running
-otherwise), `add_loss()` publishes the four loss terms, `add_optimizer(global_step)` runs BPTT (+ NCCL mean over ranks)
+`initialize(...)` runs the encoder / decoder / postnet (TacoTrainingHelper for training, evaluation and GTA: teacher-forced at
+hparams.tacotron_teacher_forcing_ratio, always at ratio 1 for GTA; free-running otherwise), `add_loss()` publishes the four loss terms, `add_optimizer(global_step)` runs BPTT (+ NCCL mean over ranks)
 + clip_by_global_norm + Adam. Attribute names read by tacotron/train.py and tacotron/synthesizer.py are kept
 (`tower_mel_outputs`, `tower_alignments`, `tower_stop_token_prediction`, `tower_decoder_output`, `loss`,
 `before_loss`, `after_loss`, `stop_token_loss`, `regularization_loss`, `learning_rate`, `gradients`). One process per
@@ -21,14 +21,20 @@ from t2_import import t2
 _MAX_ENGINES = 4
 
 
+def engine_teacher_forcing_ratio(hparams, gta):
+    """Teacher-forcing ratio of the engine behind a teacher-forced graph (helpers.py:86-108): GTA always feeds the targets; training
+    and evaluation use hparams.tacotron_teacher_forcing_ratio ('constant' mode; tacotron_natural_eval stays rejected by make_config)."""
+    return 1.0 if gta else float(hparams.tacotron_teacher_forcing_ratio)
+
+
 class Tacotron(object):
     def __init__(self, hparams):
         self._hparams = hparams
         self._engines = collections.OrderedDict()
         self._pending = None
 
-    def _engine(self, B, T_in, T_out):
-        key = (B, T_in, T_out)
+    def _engine(self, B, T_in, T_out, teacher_forcing_ratio=1.0):
+        key = (B, T_in, T_out, float(teacher_forcing_ratio))
         if key in self._engines:
             self._engines.move_to_end(key)
             return self._engines[key]
@@ -36,7 +42,7 @@ class Tacotron(object):
         while len(self._engines) >= _MAX_ENGINES:                      # evict BEFORE allocating the new workspace
             _, old = self._engines.popitem(last=False)
             old.workspace = old.packed = None
-        eng = t2.tacotron.Tacotron(self._hparams, B, T_in, T_out)
+        eng = t2.tacotron.Tacotron(self._hparams, B, T_in, T_out, teacher_forcing_ratio=teacher_forcing_ratio)
         if donor is not None:
             eng.params, eng.m, eng.v, eng.grads, eng.global_step = donor.params, donor.m, donor.v, donor.grads, donor.global_step
         elif self._pending is not None:
@@ -78,9 +84,9 @@ class Tacotron(object):
         self.is_training, self.is_evaluating, self.gta = is_training, is_evaluating, gta
         B, T_in = inputs.shape
         ids, lens = inputs.int().contiguous(), input_lengths.int().contiguous()
-        if is_training or is_evaluating or gta:                     # TacoTrainingHelper (teacher forcing ratio 1)
+        if is_training or is_evaluating or gta:                     # TacoTrainingHelper
             T_out = mel_targets.shape[1]
-            eng = self._engine(B, T_in, T_out)
+            eng = self._engine(B, T_in, T_out, engine_teacher_forcing_ratio(hp, gta))
             if global_step is not None:
                 eng.global_step = int(global_step)
             stop = stop_token_targets if stop_token_targets is not None else torch.zeros(B, T_out, device=inputs.device)
