@@ -169,7 +169,8 @@ typedef struct {
   int quantize_channels;     /* 256 or 65536 */
   int input_type;            /* 0 'raw', 1 'mulaw', 2 'mulaw-quantize' */
   int legacy, residual_legacy;
-  int upsample_type;         /* 0 'SubPixel', 1 '2D' (ConvTranspose2D) */
+  int upsample_type;         /* 0 'SubPixel', 1 '2D' (ConvTranspose2D), 2 '1D' (ConvTranspose1D: kernel = stride = s over time, mixes the
+                              * cin channels; kernel [1][s][C][C] = [kh][kw][out][in], bias [C]; freq_axis_kernel_size is not read) */
   int n_upsample;
   int upsample_scales[4];
   int freq_axis_kernel_size;
@@ -184,6 +185,8 @@ typedef struct {
                               * the parity mode that shows the bf16-mode deviation from the reference's fp32 graph is storage rounding. */
   int gin_channels;          /* global (speaker) conditioning: width of the speaker embedding (wavenet.py:151-158), 0 = off */
   int n_speakers;            /* rows of gc_embedding (>= 1 when gin_channels > 0) */
+  int upsample_activation;   /* after each learnable upsampling layer (wavenet.py:197-203): 0 ReLU, 1 LeakyReLU max(alpha x, x), 2 none */
+  float leaky_alpha;         /* LeakyReLU slope, in [0, 1] (checked whatever the activation; 0 in a zeroed struct) */
 } t2_wn_config_t;
 
 typedef struct {
@@ -238,6 +241,20 @@ int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspace, const c
  * Every layer then adds b_gin + W_gin^T gc_embedding[id_b] to item b's gate pre-activations. An id outside [0, n_speakers) reads
  * nothing: it makes that item's gate biases, and so its gate activations, NaN. */
 int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* d_speaker_ids, void* stream);
+/* One launch of a conditioning-upsampler kernel of the WaveNet engine on caller buffers (t2_dbg_kernel_t above), with the product's grid,
+ * block and shared memory. Every argument is checked before any driver call. Layouts: in fp32 [B][C][W], layer output fp32 [B][C][W*s];
+ * K / bias as the layer's parameters (upsample_type 0: [3][3][1][s] / [s]; 1: [3][s][1][1] / [1]; 2: [1][s][C][C] / [C]). Common i:
+ * B, C (1..128), W, s, type (0 SubPixel, 1 2D, 2 1D), act (0 ReLU, 1 LeakyReLU, 2 none); f[0]: LeakyReLU alpha in [0, 1].
+ * UP_FWD        p: in, K, bias, out fp32 [B][C][W*s] (post-activation), c_up bf16 (nullable: channels-last [B][W*s][C], or the split
+ *               rows [B][W*s][256] = hi | lo when i[6] = 1). i[6]: split.
+ * UP_BWD_PARAM  p: in, out (post-activation), dout fp32 [B][C][W*s] (d loss / d out), dK fp32, dbias fp32 (both out), acc int64 [nK + nb]
+ *               (scratch: the fixed-point totals, nK / nb = elements of K / bias). dK and dbias are overwritten with the totals converted
+ *               as the engine's gradient finalisation does. Synchronises nothing.
+ * UP_BWD_INPUT  p: out, dout, K, din fp32 [B][C][W] (out). */
+#define T2_DBG_WN_UP_FWD 1
+#define T2_DBG_WN_UP_BWD_PARAM 2
+#define T2_DBG_WN_UP_BWD_INPUT 3
+int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream);
 
 
 /* ---- WaveNet vocoder: Fast-WaveNet autoregressive synthesis ---------------------------------------------------

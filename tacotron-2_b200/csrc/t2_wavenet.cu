@@ -15,6 +15,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -137,6 +138,12 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.Gi = cfg->gin_channels; lo.NS = cfg->n_speakers;
   T2_REQUIRE(lo.Gi >= 0 && (lo.Gi == 0 || lo.NS >= 1), T2_ERR_INVALID_ARG,
              "gin_channels must be >= 0, and n_speakers >= 1 when gin_channels > 0 (got %d / %d)", lo.Gi, lo.NS);
+  T2_REQUIRE(cfg->upsample_type >= 0 && cfg->upsample_type <= 2, T2_ERR_INVALID_ARG,
+             "upsample_type must be 0 (SubPixel), 1 (2D) or 2 (1D), got %d", cfg->upsample_type);
+  T2_REQUIRE(cfg->upsample_activation >= 0 && cfg->upsample_activation <= 2, T2_ERR_INVALID_ARG,
+             "upsample_activation must be 0 (ReLU), 1 (LeakyReLU) or 2 (none), got %d", cfg->upsample_activation);
+  T2_REQUIRE(cfg->leaky_alpha >= 0.f && cfg->leaky_alpha <= 1.f, T2_ERR_INVALID_ARG, "leaky_alpha must be in [0, 1], got %g",
+             double(cfg->leaky_alpha));
   lo.Kg = 3 * lo.R + (lo.C > 0 ? 128 : 0);
   lo.ldo = lo.mol ? 64 : 512;   // row pitch of dlog (bf16): MoL 32 values (+pad so a 64-wide TMA box fits); CE hi|lo pair
   lo.Op = lo.mol ? 64 : 512;    // K of Wf2T (CE: [Wf2^T | Wf2^T] against the hi|lo split of dlog)
@@ -150,7 +157,10 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.up_w.clear();
   if (lo.C > 0 && !cfg->c_pre_upsampled) {
     T2_REQUIRE(cfg->n_upsample >= 1 && cfg->n_upsample <= 4, T2_ERR_INVALID_ARG, "n_upsample out of range");
-    T2_REQUIRE(cfg->freq_axis_kernel_size == 3, T2_ERR_UNSUPPORTED_SHAPE, "freq_axis_kernel_size must be 3");
+    T2_REQUIRE(cfg->upsample_type == 2 || cfg->freq_axis_kernel_size == 3, T2_ERR_UNSUPPORTED_SHAPE,
+               "freq_axis_kernel_size must be 3");   // ConvTranspose1D has no frequency axis
+    for (int i = 0; i < cfg->n_upsample; ++i)
+      T2_REQUIRE(cfg->upsample_scales[i] >= 1, T2_ERR_INVALID_ARG, "upsample_scales[%d] = %d < 1", i, cfg->upsample_scales[i]);
     int w = lo.Tc;
     for (int i = 0; i < cfg->n_upsample; ++i) { w *= cfg->upsample_scales[i]; lo.up_w.push_back(w); }
     T2_REQUIRE(w == lo.T, T2_ERR_INVALID_ARG, "Tc * prod(upsample_scales) = %d != T = %d", w, lo.T);
@@ -194,6 +204,9 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     if (cfg->upsample_type == 0) {
       lo.p_up_k.push_back(add_param(lo, s + "kernel", {3, 3, 1, sc}));
       lo.p_up_b.push_back(add_param(lo, s + "bias", {sc}));
+    } else if (cfg->upsample_type == 2) {
+      lo.p_up_k.push_back(add_param(lo, s + "kernel", {1, sc, lo.C, lo.C}));
+      lo.p_up_b.push_back(add_param(lo, s + "bias", {lo.C}));
     } else {
       lo.p_up_k.push_back(add_param(lo, s + "kernel", {3, sc, 1, 1}));
       lo.p_up_b.push_back(add_param(lo, s + "bias", {1}));
@@ -668,10 +681,20 @@ __global__ void colsum_kernel(const uint8_t* __restrict__ ws, long long* __restr
   }
 }
 
-// ---- conditioning upsampling net (modules.py:539-654 SubPixel, :736-770 ConvTranspose2D) + ReLU -------------
-// in [B][H][W] fp32 -> out [B][H][W*s] fp32 (post-ReLU); optional bf16 channels-last copy [B][W*s][H]
+// ---- conditioning upsampling net (modules.py:539-654 SubPixel, :697-733 ConvTranspose1D, :736-770 ConvTranspose2D) + activation ----
+// activation after each layer (wavenet.py:197-203): 0 ReLU, 1 LeakyReLU max(alpha x, x) (tf.nn.leaky_relu), 2 none
+__device__ __forceinline__ float up_act(float x, int act, float alpha) {
+  return act == 0 ? fmaxf(x, 0.f) : act == 1 ? fmaxf(alpha * x, x) : x;
+}
+// d pre-activation from the stored post-activation output o and d out: ReLU 0 where o <= 0; LeakyReLU alpha there (the gradient of
+// tf.nn.leaky_relu for 0 <= alpha <= 1: o <= 0 exactly where x <= 0, up to alpha = 0 where both are 0); none: unchanged
+__device__ __forceinline__ float up_dact(float o, float g, int act, float alpha) {
+  return act == 2 || o > 0.f ? g : act == 1 ? alpha * g : 0.f;
+}
+// in [B][H][W] fp32 -> out [B][H][W*s] fp32 (post-activation); optional bf16 channels-last copy [B][W*s][H]
 __global__ void upsample_fwd_kernel(const float* __restrict__ in, const float* __restrict__ K, const float* __restrict__ bias,
-                                    float* __restrict__ out, bf16* __restrict__ out_cl, int B, int H, int W, int s, int type, int split = 0) {
+                                    float* __restrict__ out, bf16* __restrict__ out_cl, int B, int H, int W, int s, int type, int act,
+                                    float alpha, int split) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   const long long n = (long long)B * H * W * s;
   if (e >= n) return;
@@ -704,7 +727,7 @@ __global__ void upsample_fwd_kernel(const float* __restrict__ in, const float* _
       acc += K[q * s + k] * ib[hh * W + w];
     }
   }
-  acc = fmaxf(acc, 0.f);
+  acc = up_act(acc, act, alpha);
   out[e] = acc;
   if (out_cl && split) {   // rows are [hi(H) zero-padded to 128 | lo(H) zero-padded to 128]
     const bf16 hi = __float2bfloat16(acc);
@@ -727,11 +750,12 @@ __global__ void cl_to_chw_kernel(const float* __restrict__ in, float* __restrict
     if (t < T && c < C) out[((long long)b * C + c) * T + t] = tile[threadIdx.x][r];
   }
 }
-// d_pre = d_out * (out > 0); accumulates dK [ntap][s] and dbias. The launch uses gridDim.x * blockDim.x % s == 0, so a
+// d_pre = d_out * act'(out); accumulates dK [ntap][s] and dbias. The launch uses gridDim.x * blockDim.x % s == 0, so a
 // thread always meets the same sub-pixel phase k = e % s: it sums its taps in registers, the block merges through a
 // small shared-memory table (10 atomics per thread, once) and issues one global atomic per table entry.
 __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const float* __restrict__ out, const float* __restrict__ dout,
-                                          long long* __restrict__ dK, long long* __restrict__ dbias, int B, int H, int W, int s, int type) {
+                                          long long* __restrict__ dK, long long* __restrict__ dbias, int B, int H, int W, int s, int type,
+                                          int act, float alpha) {
   __shared__ long long acc[10 * 32];
   const int ntap = type == 0 ? 9 : 3;
   for (int i = threadIdx.x; i < (ntap + 1) * s; i += blockDim.x) acc[i] = 0;
@@ -744,8 +768,9 @@ __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const fl
 #pragma unroll
   for (int i = 0; i < 10; ++i) r[i] = 0.f;
   for (long long e = e0; e < n; e += (long long)gridDim.x * blockDim.x) {
-    if (out[e] <= 0.f) continue;
-    const float g = dout[e];
+    const float o = out[e];
+    if (act == 0 && o <= 0.f) continue;   // ReLU: nothing to add (only here may elements be skipped)
+    const float g = up_dact(o, dout[e], act, alpha);
     const int xo = int(e % Wo), h = int((e / Wo) % H), b = int(e / ((long long)Wo * H));
     const int w = xo / s;
     r[9] += g;
@@ -787,7 +812,8 @@ __global__ void upsample_bwd_param_kernel(const float* __restrict__ in, const fl
   }
 }
 __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const float* __restrict__ dout, int cl,
-                                          const float* __restrict__ K, float* __restrict__ din, int B, int H, int W, int s, int type) {
+                                          const float* __restrict__ K, float* __restrict__ din, int B, int H, int W, int s, int type,
+                                          int act, float alpha) {
   // 4 lanes per input pixel, each walking every 4th sub-pixel phase k; partial sums meet through two shuffles
   const long long e4 = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   const long long n = (long long)B * H * W;
@@ -800,8 +826,8 @@ __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const f
   float acc = 0.f;
   auto dpre = [&](int hh, int xo) -> float {
     const float o = out[((long long)b * H + hh) * Wo + xo];
-    if (o <= 0.f) return 0.f;
-    return cl ? dout[((long long)b * Wo + xo) * H + hh] : dout[((long long)b * H + hh) * Wo + xo];
+    if (act == 0 && o <= 0.f) return 0.f;
+    return up_dact(o, cl ? dout[((long long)b * Wo + xo) * H + hh] : dout[((long long)b * H + hh) * Wo + xo], act, alpha);
   };
   if (type == 0) {
     for (int dh = 0; dh < 3; ++dh) {
@@ -823,6 +849,213 @@ __global__ void upsample_bwd_input_kernel(const float* __restrict__ out, const f
   acc += __shfl_xor_sync(0xffffffffu, acc, 1);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
   if (live && part == 0) din[e] = acc;
+}
+
+// ---- ConvTranspose1D (modules.py:697-733): kernel = stride = s along time, 'same' padding, so the windows never overlap:
+//   out[b][co][w*s + j] = act(bias[co] + sum_ci K[j][co][ci] in[b][ci][w])      K = TF [1][s][C(out)][C(in)]
+// Per tap j a [B*W, C] x [C, C] product in fp32 (C = 80 does not fill the 64-wide K blocks of the bf16 tensor-core engine, and the
+// upsampler is fp32 throughout). Blocks of 32 time positions x 8 rows of threads; a thread owns the channels ty + 8k (k < 16, C <= 128).
+// Every output is one thread's sum in a fixed order: no atomics, the same bits on every run.
+constexpr int kUp1Tw = 32, kUp1Rows = 8, kUp1MaxK = 16;
+inline size_t up1d_smem(int C) { return sizeof(float) * (size_t(C) * C + size_t(C) * kUp1Tw); }
+// grid (ceil(W / 32), B, taps per block group): the block stages its 32 input frames once and loops over taps j = z, z + gridDim.z, ...
+__global__ void __launch_bounds__(kUp1Tw * kUp1Rows) up1d_fwd_kernel(const float* __restrict__ in, const float* __restrict__ K,
+                                                                    const float* __restrict__ bias, float* __restrict__ out,
+                                                                    bf16* __restrict__ out_cl, int C, int W, int s, int act, float alpha,
+                                                                    int split) {
+  extern __shared__ float sm[];
+  float* ks = sm;                              // [C][C]: K[j][co][ci]
+  float* xs = sm + C * C;                      // [C][32]: in[b][ci][w0 + t]
+  const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * kUp1Tw + tx;
+  const int w0 = blockIdx.x * kUp1Tw, b = blockIdx.y;
+  const int nw = min(kUp1Tw, W - w0);
+  const long long Wo = (long long)W * s;
+  for (int e = tid; e < C * kUp1Tw; e += kUp1Tw * kUp1Rows) {
+    const int ci = e / kUp1Tw, t = e % kUp1Tw;
+    xs[e] = t < nw ? in[((long long)b * C + ci) * W + w0 + t] : 0.f;
+  }
+  for (int j = blockIdx.z; j < s; j += gridDim.z) {
+    __syncthreads();                           // xs staged / the previous tap's ks reads are done
+    const float* Kj = K + (long long)j * C * C;
+    for (int e = tid; e < C * C; e += kUp1Tw * kUp1Rows) ks[e] = Kj[e];
+    __syncthreads();
+    float acc[kUp1MaxK];
+#pragma unroll
+    for (int k = 0; k < kUp1MaxK; ++k) acc[k] = 0.f;
+    if ((C & 3) == 0) {                        // float4 rows of K; the same sequential order over ci as the scalar loop
+      for (int ci = 0; ci < C; ci += 4) {
+        const float x0 = xs[ci * kUp1Tw + tx], x1 = xs[(ci + 1) * kUp1Tw + tx], x2 = xs[(ci + 2) * kUp1Tw + tx], x3 = xs[(ci + 3) * kUp1Tw + tx];
+#pragma unroll
+        for (int k = 0; k < kUp1MaxK; ++k) {
+          const int co = ty + kUp1Rows * k;
+          if (co < C) {
+            const float4 kv = *reinterpret_cast<const float4*>(ks + co * C + ci);
+            acc[k] = fmaf(kv.x, x0, acc[k]); acc[k] = fmaf(kv.y, x1, acc[k]); acc[k] = fmaf(kv.z, x2, acc[k]); acc[k] = fmaf(kv.w, x3, acc[k]);
+          }
+        }
+      }
+    } else {
+      for (int ci = 0; ci < C; ++ci) {
+        const float x = xs[ci * kUp1Tw + tx];
+#pragma unroll
+        for (int k = 0; k < kUp1MaxK; ++k) {
+          const int co = ty + kUp1Rows * k;
+          if (co < C) acc[k] = fmaf(ks[co * C + ci], x, acc[k]);
+        }
+      }
+    }
+    if (tx < nw) {
+      const long long xo = (long long)(w0 + tx) * s + j;
+#pragma unroll
+      for (int k = 0; k < kUp1MaxK; ++k) {
+        const int co = ty + kUp1Rows * k;
+        if (co >= C) continue;
+        const float v = up_act(bias[co] + acc[k], act, alpha);
+        out[((long long)b * C + co) * Wo + xo] = v;
+        if (out_cl && split) {   // rows are [hi(C) zero-padded to 128 | lo(C) zero-padded to 128]
+          const bf16 hi = __float2bfloat16(v);
+          bf16* row = out_cl + ((long long)b * Wo + xo) * 256;
+          row[co] = hi;
+          row[128 + co] = __float2bfloat16(v - __bfloat162float(hi));
+        } else if (out_cl) out_cl[((long long)b * Wo + xo) * C + co] = __float2bfloat16(v);
+      }
+    }
+  }
+}
+// din[b][ci][w] = sum_j sum_co K[j][co][ci] dpre[b][co][w*s + j]; grid (ceil(W / 32), B). Per tap the block stages K[j] transposed
+// ([ci][co]) and the 32 positions' dpre; a thread sums its channels ci = ty + 8k over j, then co, in order.
+__global__ void __launch_bounds__(kUp1Tw * kUp1Rows) up1d_bwd_input_kernel(const float* __restrict__ out, const float* __restrict__ dout,
+                                                                          const float* __restrict__ K, float* __restrict__ din, int C, int W,
+                                                                          int s, int act, float alpha) {
+  extern __shared__ float sm[];
+  float* kt = sm;                              // [C][C]: K[j][co][ci] at kt[ci * C + co]
+  float* gs = sm + C * C;                      // [C][32]: dpre[b][co][(w0 + t) * s + j]
+  const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * kUp1Tw + tx;
+  const int w0 = blockIdx.x * kUp1Tw, b = blockIdx.y;
+  const int nw = min(kUp1Tw, W - w0);
+  const long long Wo = (long long)W * s;
+  float acc[kUp1MaxK];
+#pragma unroll
+  for (int k = 0; k < kUp1MaxK; ++k) acc[k] = 0.f;
+  for (int j = 0; j < s; ++j) {
+    __syncthreads();
+    const float* Kj = K + (long long)j * C * C;
+    for (int e = tid; e < C * C; e += kUp1Tw * kUp1Rows) kt[e] = Kj[(e % C) * C + e / C];   // conflict-free stores; K[j] sits in L1
+    for (int e = tid; e < C * kUp1Tw; e += kUp1Tw * kUp1Rows) {
+      const int co = e / kUp1Tw, t = e % kUp1Tw;
+      float g = 0.f;
+      if (t < nw) {
+        const long long i = ((long long)b * C + co) * Wo + (long long)(w0 + t) * s + j;
+        g = up_dact(out[i], dout[i], act, alpha);
+      }
+      gs[e] = g;
+    }
+    __syncthreads();
+    if ((C & 3) == 0) {
+      for (int co = 0; co < C; co += 4) {
+        const float g0 = gs[co * kUp1Tw + tx], g1 = gs[(co + 1) * kUp1Tw + tx], g2 = gs[(co + 2) * kUp1Tw + tx], g3 = gs[(co + 3) * kUp1Tw + tx];
+#pragma unroll
+        for (int k = 0; k < kUp1MaxK; ++k) {
+          const int ci = ty + kUp1Rows * k;
+          if (ci < C) {
+            const float4 kv = *reinterpret_cast<const float4*>(kt + ci * C + co);
+            acc[k] = fmaf(kv.x, g0, acc[k]); acc[k] = fmaf(kv.y, g1, acc[k]); acc[k] = fmaf(kv.z, g2, acc[k]); acc[k] = fmaf(kv.w, g3, acc[k]);
+          }
+        }
+      }
+    } else {
+      for (int co = 0; co < C; ++co) {
+        const float g = gs[co * kUp1Tw + tx];
+#pragma unroll
+        for (int k = 0; k < kUp1MaxK; ++k) {
+          const int ci = ty + kUp1Rows * k;
+          if (ci < C) acc[k] = fmaf(kt[ci * C + co], g, acc[k]);
+        }
+      }
+    }
+  }
+  if (tx < nw) {
+#pragma unroll
+    for (int k = 0; k < kUp1MaxK; ++k) {
+      const int ci = ty + kUp1Rows * k;
+      if (ci < C) din[((long long)b * C + ci) * W + w0 + tx] = acc[k];
+    }
+  }
+}
+// dK[j][co][ci] = sum_{b,w} dpre[b][co][w*s + j] in[b][ci][w], dbias[co] = sum dpre[b][co][:]. grid (s, G): block (j, y) sums the
+// 32-position chunks y, y + G, ... of the flattened (b, w) range in registers (a thread owns ci = tx + 32m, co = ty + 8k) and adds
+// its partial tile to the fixed-point accumulators; G depends on the shape only, so every run rounds the same partial sums.
+constexpr int kUp1MaxM = 4;
+inline size_t up1d_param_smem(int C) { return sizeof(float) * 2 * kUp1Tw * size_t(C + 1); }
+__global__ void __launch_bounds__(kUp1Tw * kUp1Rows) up1d_bwd_param_kernel(const float* __restrict__ in, const float* __restrict__ out,
+                                                                          const float* __restrict__ dout, long long* __restrict__ dK,
+                                                                          long long* __restrict__ dbias, int B, int C, int W, int s, int act,
+                                                                          float alpha) {
+  extern __shared__ float sm[];
+  const int ld = C + 1;
+  float* xs = sm;                              // [32][C + 1]: in[b][ci][w] of position t of the chunk
+  float* gs = sm + kUp1Tw * ld;                // [32][C + 1]: dpre[b][co][w*s + j]
+  const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * kUp1Tw + tx;
+  const int j = blockIdx.x;
+  const long long npos = (long long)B * W, Wo = (long long)W * s;
+  const long long nchunk = (npos + kUp1Tw - 1) / kUp1Tw;
+  float acc[kUp1MaxM][kUp1MaxK];
+#pragma unroll
+  for (int m = 0; m < kUp1MaxM; ++m)
+#pragma unroll
+    for (int k = 0; k < kUp1MaxK; ++k) acc[m][k] = 0.f;
+  float bsum = 0.f;                            // thread tid < C: column tid of gs
+  for (long long ch = blockIdx.y; ch < nchunk; ch += gridDim.y) {
+    __syncthreads();
+    for (int e = tid; e < C * kUp1Tw; e += kUp1Tw * kUp1Rows) {
+      const int c = e / kUp1Tw, t = e % kUp1Tw;
+      const long long p = ch * kUp1Tw + t;
+      float x = 0.f, g = 0.f;
+      if (p < npos) {
+        const long long b = p / W, w = p % W;
+        x = in[(b * C + c) * W + w];
+        const long long i = (b * C + c) * Wo + w * s + j;
+        g = up_dact(out[i], dout[i], act, alpha);
+      }
+      xs[t * ld + c] = x;
+      gs[t * ld + c] = g;
+    }
+    __syncthreads();
+    if (tid < C)
+      for (int t = 0; t < kUp1Tw; ++t) bsum += gs[t * ld + tid];
+    for (int t = 0; t < kUp1Tw; ++t) {
+      float x[kUp1MaxM];
+#pragma unroll
+      for (int m = 0; m < kUp1MaxM; ++m) x[m] = tx + kUp1Tw * m < C ? xs[t * ld + tx + kUp1Tw * m] : 0.f;
+#pragma unroll
+      for (int k = 0; k < kUp1MaxK; ++k) {
+        const int co = ty + kUp1Rows * k;
+        if (co < C) {
+          const float g = gs[t * ld + co];
+#pragma unroll
+          for (int m = 0; m < kUp1MaxM; ++m) acc[m][k] = fmaf(g, x[m], acc[m][k]);
+        }
+      }
+    }
+  }
+  long long* dKj = dK + (long long)j * C * C;
+#pragma unroll
+  for (int k = 0; k < kUp1MaxK; ++k) {
+    const int co = ty + kUp1Rows * k;
+    if (co >= C) continue;
+    FxAdd xa[kUp1MaxM];
+#pragma unroll
+    for (int m = 0; m < kUp1MaxM; ++m) {
+      const int ci = tx + kUp1Tw * m;
+      if (ci < C && acc[m][k] != 0.f) xa[m] = fx_issue(dKj + (long long)co * C + ci, acc[m][k]);
+    }
+#pragma unroll
+    for (int m = 0; m < kUp1MaxM; ++m) {
+      const int ci = tx + kUp1Tw * m;
+      if (ci < C && acc[m][k] != 0.f) fx_check(xa[m]);
+    }
+  }
+  if (tid < C && bsum != 0.f) fx_add(dbias + tid, bsum);
 }
 // skip-conv bias gradients: db_s[l] = skip_scale[l] * column sums of dskip (table layout: offs[3l+2] = skip bias offset)
 __global__ void skip_bias_kernel(const long long* __restrict__ skipsum, float* __restrict__ grads, const long long* __restrict__ offs,
@@ -968,6 +1201,58 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
 
 inline dim3 grid1d(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
 
+// One layer of the conditioning upsampler (type 0 SubPixel, 1 ConvTranspose2D, 2 ConvTranspose1D; in [B][C][W], out [B][C][W*s]):
+// the launches of the training forward / backward, AR synthesis and t2_dbg_wn_kernel.
+int up1d_smem_limit(const void* fn, size_t smem) {
+  if (smem > 48 * 1024) T2_CHECK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  return T2_OK;
+}
+int launch_upsample_fwd(const float* in, const float* K, const float* bias, float* out, bf16* c_up, int B, int C, int W, int s, int type,
+                        int act, float alpha, int split, cudaStream_t st) {
+  if (type == 2) {
+    const size_t smem = up1d_smem(C);
+    const int rc = up1d_smem_limit(reinterpret_cast<const void*>(up1d_fwd_kernel), smem);
+    if (rc) return rc;
+    const long long wt = (W + kUp1Tw - 1) / kUp1Tw;
+    const int jz = int(std::max(1LL, std::min<long long>(s, (264 + wt * B - 1) / (wt * B))));   // taps split over blocks: >= ~2 per SM
+    up1d_fwd_kernel<<<dim3(unsigned(wt), B, jz), dim3(kUp1Tw, kUp1Rows), smem, st>>>(in, K, bias, out, c_up, C, W, s, act, alpha, split);
+  } else {
+    upsample_fwd_kernel<<<grid1d((long long)B * C * W * s), 256, 0, st>>>(in, K, bias, out, c_up, B, C, W, s, type, act, alpha, split);
+  }
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+// dK / dbias: int64 fixed-point accumulators (fx_add), turned into gradients by the finalisation
+int launch_upsample_bwd_param(const float* in, const float* out, const float* dout, long long* dK, long long* dbias, int B, int C, int W,
+                              int s, int type, int act, float alpha, cudaStream_t st) {
+  if (type == 2) {
+    const long long nchunk = ((long long)B * W + kUp1Tw - 1) / kUp1Tw;
+    const int G = int(std::min<long long>(nchunk, (264 + s - 1) / s));
+    up1d_bwd_param_kernel<<<dim3(s, G), dim3(kUp1Tw, kUp1Rows), up1d_param_smem(C), st>>>(in, out, dout, dK, dbias, B, C, W, s, act, alpha);
+  } else {
+    T2_REQUIRE(s <= 32, T2_ERR_UNSUPPORTED_SHAPE, "upsample scale %d > 32, the limit of the SubPixel / 2D weight-gradient kernel", s);
+    upsample_bwd_param_kernel<<<s * ((296 + s - 1) / s), 256, 0, st>>>(in, out, dout, dK, dbias, B, C, W, s, type, act, alpha);
+  }
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+int launch_upsample_bwd_input(const float* out, const float* dout, const float* K, float* din, int B, int C, int W, int s, int type, int act,
+                              float alpha, cudaStream_t st) {
+  if (type == 2) {
+    const size_t smem = up1d_smem(C);
+    const int rc = up1d_smem_limit(reinterpret_cast<const void*>(up1d_bwd_input_kernel), smem);
+    if (rc) return rc;
+    up1d_bwd_input_kernel<<<dim3((W + kUp1Tw - 1) / kUp1Tw, B), dim3(kUp1Tw, kUp1Rows), smem, st>>>(out, dout, K, din, C, W, s, act, alpha);
+  } else {
+    upsample_bwd_input_kernel<<<grid1d(4LL * B * C * W), 256, 0, st>>>(out, dout, 0, K, din, B, C, W, s, type, act, alpha);
+  }
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+
 GinArgs gin_args(const Layout& lo, const float* params) {
   GinArgs a;
   memset(&a, 0, sizeof(a));
@@ -1108,9 +1393,9 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
         const int s = cfg->upsample_scales[i];
         float* out = reinterpret_cast<float*>(ws + lo.w_upout[i]);
         const bool last = i + 1 == lo.up_w.size();
-        upsample_fwd_kernel<<<grid1d((long long)lo.B * lo.C * W * s), 256, 0, st>>>(
-            in, d_params + lo.p_up_k[i], d_params + lo.p_up_b[i], out, last ? c_up : nullptr, lo.B, lo.C, W, s, cfg->upsample_type,
-            lo.split ? 1 : 0); t2_count_launch();
+        rc = launch_upsample_fwd(in, d_params + lo.p_up_k[i], d_params + lo.p_up_b[i], out, last ? c_up : nullptr, lo.B, lo.C, W, s,
+                                 cfg->upsample_type, cfg->upsample_activation, cfg->leaky_alpha, lo.split ? 1 : 0, st);
+        if (rc) return rc;
         in = out;
         W *= s;
       }
@@ -1384,19 +1669,19 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     for (int i = int(lo.up_w.size()) - 1; i >= 0; --i) {
       const int s = cfg->upsample_scales[i];
       const int W = lo.up_w[i] / s;
-      T2_REQUIRE(s <= 32, T2_ERR_UNSUPPORTED_SHAPE, "upsample scale > 32");
       const float* layer_in = i == 0 ? d_c : reinterpret_cast<const float*>(ws + lo.w_upout[i - 1]);
       const float* out = reinterpret_cast<const float*>(ws + lo.w_upout[i]);
-      upsample_bwd_param_kernel<<<s * ((296 + s - 1) / s), 256, 0, sb>>>(layer_in, out, dout, gfx + lo.p_up_k[i], gfx + lo.p_up_b[i], lo.B, lo.C, W, s,
-                                                     cfg->upsample_type); t2_count_launch();
+      rc = launch_upsample_bwd_param(layer_in, out, dout, gfx + lo.p_up_k[i], gfx + lo.p_up_b[i], lo.B, lo.C, W, s, cfg->upsample_type,
+                                     cfg->upsample_activation, cfg->leaky_alpha, sb);
+      if (rc) return rc;
       if (i > 0) {
         float* din = reinterpret_cast<float*>(ws + lo.w_upgrad[pp]);
-        upsample_bwd_input_kernel<<<grid1d(4LL * lo.B * lo.C * W), 256, 0, sb>>>(out, dout, 0, d_params + lo.p_up_k[i], din, lo.B, lo.C, W, s,
-                                                                                    cfg->upsample_type); t2_count_launch();
+        rc = launch_upsample_bwd_input(out, dout, d_params + lo.p_up_k[i], din, lo.B, lo.C, W, s, cfg->upsample_type, cfg->upsample_activation,
+                                       cfg->leaky_alpha, sb);
+        if (rc) return rc;
         dout = din;
         pp ^= 1;
       }
-      T2_CHECK_CUDA(cudaGetLastError());
     }
   }
   if (side && phase == -1) {
@@ -1443,6 +1728,48 @@ extern "C" int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspa
       return T2_OK;
     }
   return t2_set_error(T2_ERR_INVALID_ARG, "unknown workspace tensor '%s'", name);
+}
+
+// test hook: one conditioning-upsampler launch on caller buffers (include/t2b200.h, T2_DBG_WN_*)
+extern "C" int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream) {
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_wn_kernel: null call");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  void* const* p = call->p;
+  const long long* i = call->i;
+  const long long B = i[0], C = i[1], W = i[2], s = i[3], type = i[4], act = i[5];
+  const float alpha = call->f[0];
+  T2_REQUIRE(B >= 1 && B <= 65535 && C >= 1 && C <= 128 && W >= 1 && s >= 1 && W * s <= (1LL << 28) && B * C * W * s <= (1LL << 31) &&
+                 type >= 0 && type <= 2 && act >= 0 && act <= 2 && alpha >= 0.f && alpha <= 1.f,
+             T2_ERR_INVALID_ARG, "dbg_wn_kernel: bad shape, type, activation or alpha");
+  const int b = int(B), c = int(C), w = int(W), sc = int(s), ty = int(type), ac = int(act);
+  switch (call->kernel) {
+    case T2_DBG_WN_UP_FWD:
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && (i[6] == 0 || i[6] == 1), T2_ERR_INVALID_ARG, "dbg_wn_kernel UP_FWD: bad arguments");
+      return launch_upsample_fwd(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
+                                 static_cast<float*>(p[3]), static_cast<bf16*>(p[4]), b, c, w, sc, ty, ac, alpha, int(i[6]), st);
+    case T2_DBG_WN_UP_BWD_PARAM: {
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[5], T2_ERR_INVALID_ARG, "dbg_wn_kernel UP_BWD_PARAM: null pointer argument");
+      T2_REQUIRE(ty == 2 || sc <= 32, T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel UP_BWD_PARAM: upsample scale %d > 32 (SubPixel / 2D)", sc);
+      const long long nK = ty == 0 ? 9LL * sc : ty == 1 ? 3LL * sc : s * C * C, nb = ty == 0 ? sc : ty == 1 ? 1 : C;
+      long long* acc = static_cast<long long*>(p[5]);
+      float* dK = static_cast<float*>(p[3]);
+      float* db = static_cast<float*>(p[4]);
+      T2_CHECK_CUDA(cudaMemsetAsync(acc, 0, size_t(nK + nb) * sizeof(long long), st));
+      int rc = launch_upsample_bwd_param(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
+                                         acc, acc + nK, b, c, w, sc, ty, ac, alpha, st);
+      if (rc) return rc;
+      T2_CHECK_CUDA(cudaMemsetAsync(dK, 0, size_t(nK) * sizeof(float), st));
+      T2_CHECK_CUDA(cudaMemsetAsync(db, 0, size_t(nb) * sizeof(float), st));
+      rc = launch_fx_finalize(acc, dK, nK, st);
+      return rc ? rc : launch_fx_finalize(acc + nK, db, nb, st);
+    }
+    case T2_DBG_WN_UP_BWD_INPUT:
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3], T2_ERR_INVALID_ARG, "dbg_wn_kernel UP_BWD_INPUT: null pointer argument");
+      return launch_upsample_bwd_input(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
+                                       static_cast<float*>(p[3]), b, c, w, sc, ty, ac, alpha, st);
+    default:
+      return t2_set_error(T2_ERR_INVALID_ARG, "dbg_wn_kernel: unknown kernel id %d", call->kernel);
+  }
 }
 
 // Times `reps` back-to-back launches of one per-layer GEMM of the residual stack with CUDA events on the launching
@@ -2110,9 +2437,9 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
       float* out = reinterpret_cast<float*>(ws + o);
       o = align_up(o + (long long)lo.B * lo.C * lo.up_w[i] * 4, 256);
       const bool last = i + 1 == lo.up_w.size();
-      upsample_fwd_kernel<<<grid1d((long long)lo.B * lo.C * W * s), 256, 0, st>>>(
-          in, d_params + lo.p_up_k[i], d_params + lo.p_up_b[i], out, last ? c_up : nullptr, lo.B, lo.C, W, s, cfg->upsample_type);
-      t2_count_launch();
+      rc = launch_upsample_fwd(in, d_params + lo.p_up_k[i], d_params + lo.p_up_b[i], out, last ? c_up : nullptr, lo.B, lo.C, W, s,
+                               cfg->upsample_type, cfg->upsample_activation, cfg->leaky_alpha, 0, st);
+      if (rc) return rc;
       in = out;
       W *= s;
     }

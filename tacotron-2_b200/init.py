@@ -1,7 +1,7 @@
 """Fresh-variable initialisers for the flat parameter buffers (what `tf.global_variables_initializer()` does for the
 reference graphs): glorot-uniform kernels (TF1 `get_variable` / `tf.layers` default), zero biases, batch-norm
 gamma = 1 / beta = 0 / moving_mean = 0 / moving_variance = 1, and the nearest-neighbour "checkerboard free" kernels of the
-WaveNet conditioning upsamplers when `hparams.NN_init` (wavenet_vocoder/models/modules.py:642-654, :761-770).
+WaveNet conditioning upsamplers when `hparams.NN_init` (wavenet_vocoder/models/modules.py:642-654, :724-733, :761-770).
 Host-side plumbing only; the values are uploaded once into the C-ABI's parameter buffer."""
 import math
 
@@ -52,6 +52,14 @@ def nn_upsample_kernel(shape, scale, n_layers, nn_scaler, subpixel):
     return k[:, :, None, None].expand(*shape).contiguous()
 
 
+def nn_convtranspose1d_kernel(shape, n_layers, nn_scaler):
+    """ConvTranspose1D._init_kernel (modules.py:724-733): shape [1, s, C, C] ([kh, kw, out, in]); every tap is the identity over the
+    channels, scaled by NN_scaler ** (1 / n_layers). (Kernel size equals the stride, so the reference's 1 / overlap factor is 1.)"""
+    _, s, c_out, c_in = shape
+    eye = torch.eye(c_out, c_in, dtype=torch.float32) * nn_scaler ** (1.0 / n_layers)
+    return eye.expand(1, s, c_out, c_in).contiguous()
+
+
 def wavenet_variables(hp, tensors, seed=None):
     """tensors: [(name, offset, shape)] from t2_wn_param_info. Returns {name: tensor}."""
     gen = torch.Generator().manual_seed(int(hp.wavenet_random_seed if seed is None else seed))
@@ -64,7 +72,10 @@ def wavenet_variables(hp, tensors, seed=None):
             out[name] = truncated_normal(shape, 0.1, gen)
         elif name.startswith("local_conditioning_upsampling") and hp.NN_init:
             i = int(name.split("/")[0].rsplit("_", 1)[-1]) - 1
-            out[name] = nn_upsample_kernel(shape, hp.upsample_scales[i], n_up, hp.NN_scaler, hp.upsample_type == "SubPixel")
+            if hp.upsample_type == "1D":
+                out[name] = nn_convtranspose1d_kernel(shape, n_up, hp.NN_scaler)
+            else:
+                out[name] = nn_upsample_kernel(shape, hp.upsample_scales[i], n_up, hp.NN_scaler, hp.upsample_type == "SubPixel")
         else:
             out[name] = glorot_uniform(shape, gen)
     return out

@@ -24,6 +24,7 @@ class WnConfig(ctypes.Structure):
         ("B", ctypes.c_int), ("T", ctypes.c_int), ("Tc", ctypes.c_int), ("c_pre_upsampled", ctypes.c_int),
         ("log_scale_min_gauss", ctypes.c_float), ("cdf_loss", ctypes.c_int), ("split_bf16", ctypes.c_int),
         ("gin_channels", ctypes.c_int), ("n_speakers", ctypes.c_int),
+        ("upsample_activation", ctypes.c_int), ("leaky_alpha", ctypes.c_float),
     ]
 
 
@@ -33,7 +34,17 @@ class WnSizes(ctypes.Structure):
 
 
 _INPUT_TYPES = {"raw": 0, "mulaw": 1, "mulaw-quantize": 2}
-_UPSAMPLE_TYPES = {"SubPixel": 0, "2D": 1}
+_UPSAMPLE_TYPES = {"SubPixel": 0, "2D": 1, "1D": 2}
+# activation after each learnable upsampling layer (wavenet.py:197-203); None = linear
+_UPSAMPLE_ACTIVATIONS = {"Relu": 0, "relu": 0, "RELU": 0, "LeakyRelu": 1, None: 2}
+
+
+def _leaky_alpha_ok(v):
+    try:
+        a = float(v)
+    except (TypeError, ValueError):
+        return False
+    return 0.0 <= a <= 1.0          # NaN fails both comparisons
 
 
 def unsupported_hparams(hp):
@@ -49,9 +60,12 @@ def unsupported_hparams(hp):
              "speaker ids fed straight into the gin convolution without an embedding: wavenet.py:151-158")
         need("n_speakers", lambda v: v is not None and v >= 1, "gin_channels > 0 needs n_speakers >= 1")
     need("kernel_size", lambda v: v == 3, "kernel_size 3")
-    need("upsample_type", lambda v: v in _UPSAMPLE_TYPES or v == "NearestNeighbor", "Resize / 1D upsamplers: modules.py:657-733")
-    need("upsample_activation", lambda v: v in ("Relu", "relu", "RELU"), "LeakyRelu / linear upsampling activations: wavenet.py:190-201")
-    need("freq_axis_kernel_size", lambda v: v == 3, "freq_axis_kernel_size 3")
+    need("upsample_type", lambda v: v in _UPSAMPLE_TYPES or v == "NearestNeighbor", "Resize upsampler: modules.py:657-693")
+    need("upsample_activation", lambda v: v in _UPSAMPLE_ACTIVATIONS, "Relu | LeakyRelu | None: wavenet.py:197-203")
+    if getattr(hp, "upsample_activation", None) == "LeakyRelu":
+        need("leaky_alpha", _leaky_alpha_ok, "LeakyRelu slope in [0, 1] (max(alpha * x, x) is leaky_relu only there)")
+    if getattr(hp, "upsample_type", None) != "1D":             # ConvTranspose1D has no frequency axis (modules.py:697-733)
+        need("freq_axis_kernel_size", lambda v: v == 3, "freq_axis_kernel_size 3")
     need("input_type", lambda v: v in _INPUT_TYPES, "raw | mulaw | mulaw-quantize")
     need("wavenet_synth_debug", lambda v: not v, "teacher-forced synthesis debugging from wavenet_debug_wavs: synthesizer.py:54-57,85-97")
     need("wavenet_natural_eval", lambda v: not v, "free-running evaluation: wavenet.py:386 (evaluation here is teacher forced)")
@@ -76,6 +90,9 @@ def make_config(hp, B, T, c_pre_upsampled=False, dropout=None, precision="bf16")
     elif hp.upsample_type not in _UPSAMPLE_TYPES:
         raise L.T2Error("upsample_type %r is not implemented on the H100 path" % hp.upsample_type)
     cfg.upsample_type = _UPSAMPLE_TYPES.get(hp.upsample_type, 0)
+    act = getattr(hp, "upsample_activation", "Relu")
+    cfg.upsample_activation = _UPSAMPLE_ACTIVATIONS[act]
+    cfg.leaky_alpha = float(hp.leaky_alpha) if act == "LeakyRelu" else 0.0
     scales = list(hp.upsample_scales)
     cfg.n_upsample = len(scales)
     for i, s in enumerate(scales):
