@@ -119,8 +119,9 @@ typedef struct {
 /* t2_dbg_taco_kernel ids:
  * ATT_FWD  att_prep_kernel + att_fwd_kernel, one decoder step. p: h2out bf16 [B][ld_h2] (query source, first D used), WqT bf16 [A][D],
  *          K fp32 [KA][F], bK [F], Wl [F][A], ba [A], U fp32 [(KA+1)][A] (out: merged filter bank), v [A], keys fp32 [B][Ti][A],
- *          values bf16 [B][Ti][C2], lens int32 [B], cum fp32 [B][Ti] (in/out), alpha fp32 [B][Ti] (out), ctx_a bf16 (nullable),
- *          ctx_b bf16. i: B, Ti, D, A, KA, F, C2, ld_h2, ld_a, ld_b.
+ *          values bf16 [B][Ti][C2], lens int32 [B], cum fp32 [B][Ti] (in/out: the attention state), alpha fp32 [B][Ti] (out), ctx_a
+ *          bf16 (nullable), ctx_b bf16. i: B, Ti, D, A, KA, F, C2, ld_h2, ld_a, ld_b, unmasked, noncumulative (the two
+ *          t2_taco_config_t flags; 0 = masked scores and cum + alpha as the new state, 1 = all T_in scores and alpha as the new state).
  * BN_FWD   bn_stats_kernel + bn_apply_kernel (conv-block batch norm). p: y (bf16, or fp32 when i[3]), x bf16 [rows][C] (split: [rows][2C]),
  *          stats fp32 [4C], gamma, beta, moving mean, moving variance. i: rows, C, training, y_fp32, stream, split. f: dropout p.
  * BN_BWD   bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: dout bf16, y bf16, stats fp32 [6C] (mean / rstd at [2C, 4C); [4C, 6C) receives
@@ -134,10 +135,19 @@ typedef struct {
  * ATT_FINISH  att_finish_kernel + att_finish2_kernel. p: acc fp32 [B][(KA+2)][A], K [KA][F], bK [F], Wl [F][A], grads fp32 (accumulated
  *             at the offsets), scratch fp32 [(KA+2)][A]. i: B, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba.
  * DVALUES     dvalues_ctx_kernel. p: alpha fp32 [To][B][Ti], dctx bf16 [To][B][C2], lens int32 [B], dvalues fp32 [B][Ti][C2] (in/out).
- *             i: B, Ti, To, C2. */
+ *             i: B, Ti, To, C2.
+ * ATT_BWD     att_bwd_kernel, one decoder step (the training backward's grid, block and shared memory). p: h2out bf16 [B][ld_h2] (query
+ *             source, first D used), WqT bf16 [A][D], U fp32 [(KA+1)][A] (merged filter bank, row KA = u0, as ATT_FWD leaves it), v [A],
+ *             keys fp32 [B][Ti][A], values bf16 [B][Ti][C2], lens int32 [B], alpha fp32 [B][Ti] (this step), state: cumulative = cum_t
+ *             fp32 [B][Ti] (in; out: cum_{t-1} = cum_t - alpha), non-cumulative = alpha_{t-1} fp32 [B][Ti] (read; nullable = zeros, step
+ *             0), dstate fp32 [B][Ti] (in: d loss / d state_t; out: d loss / d state_{t-1}), dPI fp32 [B][ld_dPI] (cols [0, D): d h2out,
+ *             [D, D + C2): d context), dctxl fp32 [B][C2] (added to the context gradient, then cleared), dh2ext fp32 [B][D] (out),
+ *             dsave bf16 [B][C2] dctx followed by [B][A] dq (out), dkeys fp32 [B][Ti][A] (accumulated), acc fp32 [B][(KA+2)][A]
+ *             (accumulated: dU rows 0..KA-1, du0, dv). i: B, Ti, D, A, KA, C2, ld_h2, ld_dPI, unmasked, noncumulative. */
 #define T2_DBG_TACO_CELL_BWD 4
 #define T2_DBG_TACO_ATT_FINISH 5
 #define T2_DBG_TACO_DVALUES 6
+#define T2_DBG_TACO_ATT_BWD 7
 int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 /* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
  * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):
@@ -302,6 +312,14 @@ typedef struct {
                               * (sum / count_nonzero of the mask), stop-token loss = weighted sigmoid CE over the same frames divided by the
                               * number of NON-ZERO masked terms; the lengths come from t2_taco_set_target_lengths */
   float cross_entropy_pos_weight;  /* pos_weight of tf.nn.weighted_cross_entropy_with_logits (masked stop-token loss only) */
+  int unmasked_encoder;      /* 1 = mask_encoder False (tacotron/models/attention.py:140-151, tacotron.py:135): the attention energies and
+                              * the softmax cover all T_in positions of every row, not only the first input_lengths[b]. The encoder outputs
+                              * (values, keys) past a length are zero either way (dynamic BiLSTM, modules.py:207-217), but their energies
+                              * are not, so the results depend on the padded T_in. 0 = masked (the reference default). Other values are
+                              * T2_ERR_INVALID_ARG. Applies to training, evaluation, GTA and synthesis. */
+  int noncumulative_weights; /* 1 = cumulative_weights False (attention.py:220-224): the attention state after a step is that step's
+                              * alignments, not their running sum. 0 = cumulative (the reference default); other values are
+                              * T2_ERR_INVALID_ARG. Applies everywhere the attention runs. */
   float teacher_forcing_ratio;     /* tacotron_teacher_forcing_ratio in [0, 1] ('constant' mode, helpers.py:115-128) of t2_taco_forward /
                               * t2_taco_backward; anything else is T2_ERR_INVALID_ARG. 1 = full teacher forcing: the prenet, the LSTM-1 input
                               * projection and the frame / stop projections run batched over all T_out steps. < 1: at the end of decoder step t

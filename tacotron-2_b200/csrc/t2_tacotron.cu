@@ -102,6 +102,10 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
              T2_ERR_INVALID_ARG, "layer counts");
   T2_REQUIRE(cfg->teacher_forcing_ratio >= 0.f && cfg->teacher_forcing_ratio <= 1.f, T2_ERR_INVALID_ARG,
              "teacher_forcing_ratio %g outside [0, 1]", double(cfg->teacher_forcing_ratio));
+  T2_REQUIRE(cfg->unmasked_encoder == 0 || cfg->unmasked_encoder == 1, T2_ERR_INVALID_ARG, "unmasked_encoder %d is not 0 or 1",
+             cfg->unmasked_encoder);
+  T2_REQUIRE(cfg->noncumulative_weights == 0 || cfg->noncumulative_weights == 1, T2_ERR_INVALID_ARG, "noncumulative_weights %d is not 0 or 1",
+             cfg->noncumulative_weights);
   // ---- parameters (order == oracle/tacotron.py:param_shapes) ----
   lo.n_params = 0; lo.params.clear(); lo.enc.clear(); lo.post.clear();
   lo.p_emb = addp(lo, "inputs_embedding", {lo.NS, lo.E});
@@ -527,6 +531,7 @@ struct AttArgs {
   bf16* ctx_a; int ld_a;                    // context -> S1_all[t+1][b][0:C2]
   bf16* ctx_b; int ld_b;                    // context -> PI_all[t][b][D:]
   int B, Ti, D, A, KA, C2;
+  int unmasked, noncumulative;              // t2_taco_config_t flags: pick the att_fwd_kernel instantiation (host side only)
 };
 // q[a] = sum_k h[k] WqT[a][k]: one warp per output row (two rows in flight), lanes stride the row in 16-byte pieces so
 // that every load instruction reads 512 contiguous bytes (the 4-threads-per-output form touched 32 sectors per load)
@@ -610,6 +615,10 @@ __device__ __forceinline__ void loc_tile(const float* __restrict__ Us, int AP, c
 inline size_t att_fwd_smem(int Ti, int KA, int A, int D, int C2) {
   return sizeof(float) * (size_t)((KA + 1) * (A + kAttPad) + att_cumlen(Ti, KA) + A + ((Ti + 3) & ~3) + D + 8 * C2 + 32) + 64;
 }
+// kMasked: the scores of positions past lens[b] are -inf (mask_encoder); otherwise the energies and the softmax cover all T_in
+// positions. The context sum stays bounded by lens[b] either way: the values rows past it are zero. kCumulative: the state after
+// the step is cum + alpha (cumulative_weights); otherwise alpha itself.
+template <bool kMasked, bool kCumulative>
 __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
   extern __shared__ __align__(16) float sm[];
   pdl_wait();
@@ -638,17 +647,18 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
   __syncthreads();
   ATT_STAMP(2);
   const int len = a.lens[b];
+  const int el = kMasked ? len : Ti;    // positions that get an energy
   {
     // energies: units of 16 memory rows x 64 channels; e[j] += sum over the unit's channels of v tanh(keys + q + pl)
     const int g = lane >> 2, t = lane & 3;
-    const int n_nh = A >> 6, n_units = ((len + 15) >> 4) * n_nh;
+    const int n_nh = A >> 6, n_units = ((el + 15) >> 4) * n_nh;
     for (int u = warp; u < n_units; u += NW) {
       const int j0 = (u / n_nh) * 16, n0 = (u % n_nh) * 64;
       float acc[8][4];
       loc_tile(Us, AP, cum, a.KA, j0, n0, acc);
       const int r0 = j0 + g, r1 = r0 + 8;
-      const float* k0p = a.keys + ((long long)b * Ti + (r0 < len ? r0 : 0)) * A + n0 + 2 * t;
-      const float* k1p = a.keys + ((long long)b * Ti + (r1 < len ? r1 : 0)) * A + n0 + 2 * t;
+      const float* k0p = a.keys + ((long long)b * Ti + (r0 < el ? r0 : 0)) * A + n0 + 2 * t;
+      const float* k1p = a.keys + ((long long)b * Ti + (r1 < el ? r1 : 0)) * A + n0 + 2 * t;
       float2 ky0[8], ky1[8];
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) { ky0[nt] = __ldg(reinterpret_cast<const float2*>(k0p + nt * 8)); ky1[nt] = __ldg(reinterpret_cast<const float2*>(k1p + nt * 8)); }
@@ -664,15 +674,15 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
       e0 += __shfl_xor_sync(0xffffffffu, e0, 1); e0 += __shfl_xor_sync(0xffffffffu, e0, 2);
       e1 += __shfl_xor_sync(0xffffffffu, e1, 1); e1 += __shfl_xor_sync(0xffffffffu, e1, 2);
       if (t == 0) {
-        if (r0 < len) atomicAdd(&e[r0], e0);
-        if (r1 < len) atomicAdd(&e[r1], e1);
+        if (r0 < el) atomicAdd(&e[r0], e0);
+        if (r1 < el) atomicAdd(&e[r1], e1);
       }
     }
   }
   __syncthreads();
   ATT_STAMP(3);
   float mx = -INFINITY;
-  for (int j = tid; j < len; j += kAttThreads) mx = fmaxf(mx, e[j]);
+  for (int j = tid; j < el; j += kAttThreads) mx = fmaxf(mx, e[j]);
   mx = warp_max(mx);
   if (lane == 0) red[warp] = mx;
   __syncthreads();
@@ -680,7 +690,7 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
   for (int w = 1; w < kAttThreads / 32; ++w) mx = fmaxf(mx, red[w]);
   __syncthreads();
   float s = 0.f;
-  for (int j = tid; j < Ti; j += kAttThreads) { const float p = j < len ? __expf(e[j] - mx) : 0.f; e[j] = p; s += p; }
+  for (int j = tid; j < Ti; j += kAttThreads) { const float p = j < el ? __expf(e[j] - mx) : 0.f; e[j] = p; s += p; }
   s = warp_sum(s);
   if (lane == 0) red[warp] = s;
   __syncthreads();
@@ -691,7 +701,7 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
     const float al = e[j] * inv;
     e[j] = al;
     a.alpha[(long long)b * Ti + j] = al;
-    a.cum[(long long)b * Ti + j] = cum[j + half] + al;
+    a.cum[(long long)b * Ti + j] = kCumulative ? cum[j + half] + al : al;
   }
   __syncthreads();
   ATT_STAMP(4);
@@ -730,14 +740,20 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
 }
 // once per forward: the merged location filter bank U (from the conv kernel K [KA][F], its bias bK, the dense Wl [F][A] and the
 // attention bias) and the kernel's shared-memory opt-in
-int att_fwd_setup(const float* K, const float* bK, const float* Wl, const float* ba, float* U, int KA, int F, int A, size_t smem, cudaStream_t st) {
+using AttFwdFn = void (*)(AttArgs);
+AttFwdFn att_fwd_fn(int unmasked, int noncumulative) {
+  return unmasked ? (noncumulative ? att_fwd_kernel<false, false> : att_fwd_kernel<false, true>)
+                  : (noncumulative ? att_fwd_kernel<true, false> : att_fwd_kernel<true, true>);
+}
+int att_fwd_setup(const float* K, const float* bK, const float* Wl, const float* ba, float* U, int KA, int F, int A, size_t smem, int unmasked,
+                  int noncumulative, cudaStream_t st) {
   att_prep_kernel<<<g1((KA + 1) * A), 256, 0, st>>>(K, bK, Wl, ba, U, KA, F, A); t2_count_launch();
-  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_fn(unmasked, noncumulative), cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
 int launch_att_fwd(const AttArgs& a, size_t smem, cudaStream_t st) {
-  T2_CHECK_CUDA(launch_pdl(att_fwd_kernel, dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
+  T2_CHECK_CUDA(launch_pdl(att_fwd_fn(a.unmasked, a.noncumulative), dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
   return T2_OK;
 }
 
@@ -1107,8 +1123,9 @@ struct AttBwd {
   const float* U; const float* v;
   const float* keys; const bf16* values; const int* lens;
   const float* alpha;      // [B][Ti] of this step
-  float* cumrun;           // [B][Ti]: cum_t on entry, cum_{t-1} on exit
-  float* dcum;             // [B][Ti] running grad wrt cum_t (in) / cum_{t-1} (out)
+  float* cumrun;           // cumulative: [B][Ti] cum_t on entry, cum_{t-1} on exit
+  const float* alpha_prev; // non-cumulative: [B][Ti] alpha_{t-1} = the state the step read (nullptr at t = 0: zeros)
+  float* dcum;             // [B][Ti] running grad wrt state_t (in) / state_{t-1} (out)
   const float* dPI; int ld_dPI;   // dPI_all[t]: [B][PIK] fp32
   float* dctxl;            // [B][C2] grad wrt ctx_t from LSTM-1 of step t+1 (read, then cleared for the split-K accumulation)
   float* dh2ext;           // [B][D] out: grad wrt the un-zoned LSTM-2 output of this step
@@ -1117,6 +1134,7 @@ struct AttBwd {
   float* dkeys;            // [B][Ti][A] accumulated
   float* acc;              // per item: dU [(KA+1)][A] (row KA = d u0) | dv [A]
   int B, Ti, D, A, KA, C2;
+  int unmasked, noncumulative;   // pick the att_bwd_kernel instantiation (host side only)
 };
 inline size_t att_bwd_smem(int Ti, int KA, int A, int D, int C2) {
   const int Tip = (Ti + 3) & ~3;
@@ -1137,6 +1155,10 @@ int check_att_bwd_fits(const TL& lo) {
                       "T_in <= %d at these attention widths",
                       lo.Ti, need, kSmemOptin, tmax);
 }
+// kMasked / kCumulative as in att_fwd_kernel. Un-masked, d alpha_j past lens[b] is d state_j alone (the values rows there are zero)
+// and every energy gets a gradient. Non-cumulative, state_{t-1} is alpha_{t-1}, and d state_{t-1} is the location-path term only:
+// alpha_t does not carry state_{t-1} forward.
+template <bool kMasked, bool kCumulative>
 __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   extern __shared__ __align__(16) float sm[];
   pdl_wait();
@@ -1160,6 +1182,7 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   float* dE = dv + A;                     // [RE][AP]: position j lives in row j + half; everything else stays zero
   float* red = dE + RE * AP;              // [32]
   const int len = a.lens[b];
+  const int el = kMasked ? len : Ti;      // positions with an energy
   for (int i = tid; i < (a.KA + 1) * A; i += kAttThreads) Us[(i / A) * AP + (i % A)] = a.U[i];
   for (int i = tid; i < cumlen; i += kAttThreads) {
     const int j = i - half;
@@ -1167,8 +1190,12 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
     if (j >= 0 && j < Ti) {
       const float aj = a.alpha[(long long)b * Ti + j];
       al[j] = aj;
-      cp = a.cumrun[(long long)b * Ti + j] - aj;
-      a.cumrun[(long long)b * Ti + j] = cp;
+      if (kCumulative) {
+        cp = a.cumrun[(long long)b * Ti + j] - aj;
+        a.cumrun[(long long)b * Ti + j] = cp;
+      } else if (a.alpha_prev) {
+        cp = a.alpha_prev[(long long)b * Ti + j];
+      }
       dcs[j] = a.dcum[(long long)b * Ti + j];
       dca[j] = 0.f;
     }
@@ -1214,7 +1241,14 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
         }
       }
     }
-    for (int j = len + tid; j < Ti; j += kAttThreads) de[j] = 0.f;
+    if (kMasked) {
+      for (int j = len + tid; j < Ti; j += kAttThreads) de[j] = 0.f;
+    } else {
+      float tail = 0.f;      // past the length dctx . values[j] = 0: d alpha[j] = dcum[j]
+      for (int j = len + tid; j < Ti; j += kAttThreads) { const float da = dcs[j]; de[j] = da; tail += al[j] * da; }
+      tail = warp_sum(tail);
+      if (lane == 0) part += tail;
+    }
   }
   if (lane == 0) red[warp] = part;
   __syncthreads();
@@ -1222,17 +1256,17 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   float dot = 0.f;
   for (int w = 0; w < NW; ++w) dot += red[w];
   __syncthreads();
-  for (int j = tid; j < Ti; j += kAttThreads) de[j] = j < len ? al[j] * (de[j] - dot) : 0.f;
+  for (int j = tid; j < Ti; j += kAttThreads) de[j] = j < el ? al[j] * (de[j] - dot) : 0.f;
   __syncthreads();
   // energies backward: units of 16 rows x 64 channels (pl recomputed on the tensor cores, see loc_tile)
   {
-    const int n_nh = A >> 6, n_units = ((len + 15) >> 4) * n_nh;
+    const int n_nh = A >> 6, n_units = ((el + 15) >> 4) * n_nh;
     for (int u = warp; u < n_units; u += NW) {
       const int j0 = (u / n_nh) * 16, n0 = (u % n_nh) * 64;
       float acc[8][4];
       loc_tile(Us, AP, cum, a.KA, j0, n0, acc);
       const int r0 = j0 + g, r1 = r0 + 8;
-      const bool ok0 = r0 < len, ok1 = r1 < len;
+      const bool ok0 = r0 < el, ok1 = r1 < el;
       const long long kr0 = ((long long)b * Ti + (ok0 ? r0 : 0)) * A + n0 + 2 * t, kr1 = ((long long)b * Ti + (ok1 ? r1 : 0)) * A + n0 + 2 * t;
       float2 ky0[8], ky1[8];
 #pragma unroll
@@ -1280,7 +1314,7 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   // dU[k][c] += sum_j cum_{t-1}[j + k - half] dE[j][c] = (T^T dE)[k][c]: M = 32 taps (2 m-tiles), N = A (one n-tile per
   // warp pass), K = memory rows
   {
-    const int nks = (len + 7) >> 3;
+    const int nks = (el + 7) >> 3;
     for (int nt = warp; nt < (A >> 3); nt += NW) {
       float acc[2][4];
 #pragma unroll
@@ -1306,12 +1340,12 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
     }
   }
   ATT_STAMP(21);
-  // dcum_{t-1}[i] = dcum_t[i] + sum_k P[i - k + 2*half][k] with P = dE U^T ([RE rows] x [32 taps], K = A): one m-tile of
-  // dE rows per warp pass, the anti-diagonal sums go through shared-memory atomics
+  // dcum_{t-1}[i] = dcum_t[i] (cumulative only) + sum_k P[i - k + 2*half][k] with P = dE U^T ([RE rows] x [32 taps], K = A): one
+  // m-tile of dE rows per warp pass, the anti-diagonal sums go through shared-memory atomics
   {
     for (int mt = warp; mt < (RE >> 4); mt += NW) {
       const int r0 = mt * 16 + g, r1 = r0 + 8;
-      if (mt * 16 >= len + 2 * half) continue;     // rows past the last written position are zero (warp-uniform)
+      if (mt * 16 >= el + 2 * half) continue;      // rows past the last written position are zero (warp-uniform)
       float acc[4][4];
 #pragma unroll
       for (int n = 0; n < 4; ++n) acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.f;
@@ -1339,7 +1373,7 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
     }
   }
   __syncthreads();
-  for (int i = tid; i < Ti; i += kAttThreads) a.dcum[(long long)b * Ti + i] = dcs[i] + dca[i];
+  for (int i = tid; i < Ti; i += kAttThreads) a.dcum[(long long)b * Ti + i] = kCumulative ? dcs[i] + dca[i] : dca[i];
   ATT_STAMP(22);
   // dh2ext = dPI[:, 0:D] + dq . Wq^T   (bf16 [A][D] copy of the query weights: coalesced along D)
   for (int k2 = tid; k2 < (a.D >> 1); k2 += kAttThreads) {
@@ -1407,6 +1441,19 @@ __global__ void dvalues_ctx_kernel(const float* __restrict__ alpha, const bf16* 
   }
 }
 // launch helpers shared by the backward pass and t2_dbg_taco_kernel
+using AttBwdFn = void (*)(AttBwd);
+AttBwdFn att_bwd_fn(int unmasked, int noncumulative) {
+  return unmasked ? (noncumulative ? att_bwd_kernel<false, false> : att_bwd_kernel<false, true>)
+                  : (noncumulative ? att_bwd_kernel<true, false> : att_bwd_kernel<true, true>);
+}
+int att_bwd_setup(size_t smem, int unmasked, int noncumulative) {
+  T2_CHECK_CUDA(cudaFuncSetAttribute(att_bwd_fn(unmasked, noncumulative), cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  return T2_OK;
+}
+int launch_att_bwd(const AttBwd& a, size_t smem, cudaStream_t st) {
+  T2_CHECK_CUDA(launch_pdl(att_bwd_fn(a.unmasked, a.noncumulative), dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
+  return T2_OK;
+}
 int launch_cell_bwd(const CellBwd& c, cudaStream_t st) {
   T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)c.B * c.H)), dim3(256), 0, st, c)); t2_count_launch();
   return T2_OK;
@@ -1591,7 +1638,8 @@ static int decoder_reset(const StepCtx& s, DecBufs& d) {
   T2_CHECK_CUDA(cudaMemsetAsync(d.c2, 0, (size_t)B * D * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.cum, 0, (size_t)B * Ti * 4, st));
   d.att_smem = att_fwd_smem(Ti, lo.KA, lo.A, D, 2 * H);
-  return att_fwd_setup(d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_params + lo.p_ba, d.attU, lo.KA, lo.F, lo.A, d.att_smem, st);
+  return att_fwd_setup(d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_params + lo.p_ba, d.attU, lo.KA, lo.F, lo.A, d.att_smem,
+                       lo.c.unmasked_encoder, lo.c.noncumulative_weights, st);
 }
 // decoder step t: LSTM-1 (prenet part of its gates precomputed in pre1[t]), LSTM-2, attention (Architecture_wrappers.py:169-213)
 static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_lengths, int t) {
@@ -1621,6 +1669,7 @@ static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_l
   a.alpha = reinterpret_cast<float*>(ws + lo.w_alpha) + (long long)t * B * Ti;
   a.ctx_a = S1n; a.ld_a = K1r; a.ctx_b = PIt + D; a.ld_b = PIK;
   a.B = B; a.Ti = Ti; a.D = D; a.A = lo.A; a.KA = lo.KA; a.C2 = 2 * H;
+  a.unmasked = lo.c.unmasked_encoder; a.noncumulative = lo.c.noncumulative_weights;
   return launch_att_fwd(a, d.att_smem, st);
 }
 
@@ -1994,14 +2043,18 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   T2_CHECK_CUDA(cudaMemsetAsync(dcum, 0, (size_t)B * Ti * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(dkeys, 0, (size_t)B * Ti * A * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(attacc, 0, (size_t)B * nacc * 4, st));
-  T2_CHECK_CUDA(cudaMemcpyAsync(cumrun, ws + lo.w_cum, (size_t)B * Ti * 4, cudaMemcpyDeviceToDevice, st));
+  const int unmasked = lo.c.unmasked_encoder, noncum = lo.c.noncumulative_weights;
+  // cumulative state: rebuilt step by step from the final cum_{T_out} (cum_{t-1} = cum_t - alpha_t); non-cumulative: read from the
+  // stored alignments of the previous step
+  if (!noncum) T2_CHECK_CUDA(cudaMemcpyAsync(cumrun, ws + lo.w_cum, (size_t)B * Ti * 4, cudaMemcpyDeviceToDevice, st));
   bf16* dg1 = reinterpret_cast<bf16*>(ws + lo.w_dg1);
   bf16* dg2 = reinterpret_cast<bf16*>(ws + lo.w_dg2);
   bf16* dctx_all = reinterpret_cast<bf16*>(ws + lo.w_dctx_all);
   bf16* dq_all = reinterpret_cast<bf16*>(ws + lo.w_dq_all);
   const size_t ab_smem = att_bwd_smem(Ti, lo.KA, A, D, 2 * H);
   const float* attU = reinterpret_cast<const float*>(ws + lo.w_attU);
-  T2_CHECK_CUDA(cudaFuncSetAttribute(att_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(ab_smem)));
+  rc = att_bwd_setup(ab_smem, unmasked, noncum);
+  if (rc) return rc;
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
   bf16* dpn2 = reinterpret_cast<bf16*>(ws + lo.w_dpn2);
@@ -2026,10 +2079,11 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     a.U = attU; a.v = d_params + lo.p_v;
     a.keys = reinterpret_cast<const float*>(ws + lo.w_keys); a.values = reinterpret_cast<const bf16*>(ws + lo.w_values); a.lens = d_input_lengths;
     a.alpha = reinterpret_cast<const float*>(ws + lo.w_alpha) + (long long)t * B * Ti; a.cumrun = cumrun; a.dcum = dcum;
+    a.alpha_prev = t > 0 ? a.alpha - (long long)B * Ti : nullptr;
     a.dPI = dPI + (long long)t * B * PIK; a.ld_dPI = PIK; a.dctxl = dctxl; a.dh2ext = dh2ext;
     a.dctx_save = dctx_all + (long long)t * B * 2 * H; a.dq_save = dq_all + (long long)t * B * A; a.dkeys = dkeys; a.acc = attacc;
-    a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = lo.KA; a.C2 = 2 * H;
-    T2_CHECK_CUDA(launch_pdl(att_bwd_kernel, dim3(B), dim3(kAttThreads), ab_smem, st, a)); t2_count_launch();
+    a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = lo.KA; a.C2 = 2 * H; a.unmasked = unmasked; a.noncumulative = noncum;
+    rc = launch_att_bwd(a, ab_smem, st); if (rc) return rc;
     CellBwd c2;
     c2.dh_ext = dh2ext; c2.zero_ext = 0; c2.ld_ext = D; c2.dhs = dhs2; c2.dcs = dcs2;
     c2.gst = reinterpret_cast<const bf16*>(ws + lo.w_g2) + (long long)t * B * 4 * D; c2.tst = reinterpret_cast<const bf16*>(ws + lo.w_t2) + (long long)t * B * D;
@@ -2203,6 +2257,8 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_REQUIRE(i[7] >= D && i[8] >= C2 && i[9] >= C2 && aligned16(p[1]) && aligned16(p[9]) && (reinterpret_cast<uintptr_t>(p[8]) & 7) == 0 &&
                      (reinterpret_cast<uintptr_t>(p[7]) & 7) == 0,
                  T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FWD: bad pitch or alignment");
+      T2_REQUIRE((i[10] == 0 || i[10] == 1) && (i[11] == 0 || i[11] == 1), T2_ERR_INVALID_ARG,
+                 "dbg_taco_kernel ATT_FWD: unmasked / noncumulative must be 0 or 1");
       const size_t smem = att_fwd_smem(Ti, KA, A, D, C2);
       T2_REQUIRE(smem <= kSmemOptin, T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_FWD: %zu B of shared memory", smem);
       AttArgs a;
@@ -2211,10 +2267,42 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       a.keys = static_cast<const float*>(p[8]); a.values = static_cast<const bf16*>(p[9]); a.lens = static_cast<const int*>(p[10]);
       a.cum = static_cast<float*>(p[11]); a.alpha = static_cast<float*>(p[12]);
       a.ctx_a = static_cast<bf16*>(p[13]); a.ld_a = int(i[8]); a.ctx_b = static_cast<bf16*>(p[14]); a.ld_b = int(i[9]);
-      a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2;
+      a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2; a.unmasked = int(i[10]); a.noncumulative = int(i[11]);
       int rc = att_fwd_setup(static_cast<const float*>(p[2]), static_cast<const float*>(p[3]), static_cast<const float*>(p[4]),
-                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, st);
+                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, a.unmasked, a.noncumulative, st);
       return rc ? rc : launch_att_fwd(a, smem, st);
+    }
+    case T2_DBG_TACO_ATT_BWD: {
+      const int B = int(i[0]), Ti = int(i[1]), D = int(i[2]), A = int(i[3]), KA = int(i[4]), C2 = int(i[5]);
+      const int unmasked = int(i[8]), noncum = int(i[9]);
+      for (int k = 0; k < 16; ++k)
+        T2_REQUIRE(k == 8 || p[k] != nullptr, T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_BWD: null pointer argument %d", k);
+      T2_REQUIRE((i[8] == 0 || i[8] == 1) && (i[9] == 0 || i[9] == 1), T2_ERR_INVALID_ARG,
+                 "dbg_taco_kernel ATT_BWD: unmasked / noncumulative must be 0 or 1");
+      T2_REQUIRE(noncum || p[8] != nullptr, T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_BWD: the cumulative state needs cumrun (p[8])");
+      T2_REQUIRE(B >= 1 && B <= 256 && Ti >= 1 && Ti <= 1024 && D >= 32 && D % 32 == 0 && A % 64 == 0 && A >= 64 && A <= 128 && KA >= 1 &&
+                     KA % 2 == 1 && KA <= 31 && C2 >= 64 && C2 % 64 == 0,
+                 T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_BWD: unsupported shape");
+      auto aligned8 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; };
+      T2_REQUIRE(i[6] >= D && i[7] >= D + C2 && i[7] % 2 == 0 && aligned16(p[1]) && aligned16(p[5]) && aligned8(p[3]) && aligned8(p[4]) &&
+                     aligned8(p[10]) && aligned8(p[12]) && aligned8(p[14]) && aligned8(p[15]),
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_BWD: bad pitch or alignment");
+      const size_t smem = att_bwd_smem(Ti, KA, A, D, C2);
+      T2_REQUIRE(smem <= kSmemOptin, T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_BWD: %zu B of shared memory", smem);
+      AttBwd a;
+      a.h2out = static_cast<const bf16*>(p[0]); a.ld_h2 = int(i[6]); a.WqT = static_cast<const bf16*>(p[1]); a.Wq = nullptr;
+      a.U = static_cast<const float*>(p[2]); a.v = static_cast<const float*>(p[3]);
+      a.keys = static_cast<const float*>(p[4]); a.values = static_cast<const bf16*>(p[5]); a.lens = static_cast<const int*>(p[6]);
+      a.alpha = static_cast<const float*>(p[7]);
+      a.cumrun = noncum ? nullptr : static_cast<float*>(p[8]);
+      a.alpha_prev = noncum ? static_cast<const float*>(p[8]) : nullptr;
+      a.dcum = static_cast<float*>(p[9]); a.dPI = static_cast<const float*>(p[10]); a.ld_dPI = int(i[7]);
+      a.dctxl = static_cast<float*>(p[11]); a.dh2ext = static_cast<float*>(p[12]);
+      a.dctx_save = static_cast<bf16*>(p[13]); a.dq_save = static_cast<bf16*>(p[13]) + (long long)B * C2;
+      a.dkeys = static_cast<float*>(p[14]); a.acc = static_cast<float*>(p[15]);
+      a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2; a.unmasked = unmasked; a.noncumulative = noncum;
+      int rc = att_bwd_setup(smem, unmasked, noncum);
+      return rc ? rc : launch_att_bwd(a, smem, st);
     }
     case T2_DBG_TACO_BN_FWD: {
       const long long rows = i[0];

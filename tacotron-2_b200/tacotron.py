@@ -17,7 +17,7 @@ class TacoConfig(ctypes.Structure):
         "prenet2", "decoder_lstm_units", "postnet_layers", "postnet_kernel", "postnet_channels", "clip_outputs")] + [
         (n, ctypes.c_float) for n in ("dropout_rate", "zoneout_rate", "reg_weight", "max_abs_value", "lower_bound_decay")] + [
         ("split_bf16", ctypes.c_int), ("mask_decoder", ctypes.c_int), ("cross_entropy_pos_weight", ctypes.c_float),
-        ("teacher_forcing_ratio", ctypes.c_float)]
+        ("unmasked_encoder", ctypes.c_int), ("noncumulative_weights", ctypes.c_int), ("teacher_forcing_ratio", ctypes.c_float)]
 
 
 class CbhgConfig(ctypes.Structure):
@@ -65,9 +65,7 @@ def unsupported_hparams(hp):
     need("prenet_layers", lambda v: len(v) == 2, "2 prenet layers")
     need("decoder_layers", lambda v: v == 2, "2 decoder LSTM layers")
     need("smoothing", lambda v: not v, "smoothing normalisation instead of softmax: attention.py:72-92")
-    need("cumulative_weights", lambda v: bool(v), "non-cumulative location features: attention.py:220-224")
     need("batch_norm_position", lambda v: v == "after", "batch norm before the activation: modules.py:386-389")
-    need("mask_encoder", lambda v: bool(v), "un-masked encoder memory")
     need("tacotron_teacher_forcing_mode", lambda v: v == "constant", "scheduled teacher forcing: helpers.py:135-169")
     need("tacotron_teacher_forcing_ratio", lambda v: 0.0 <= float(v) <= 1.0, "teacher-forcing ratio outside [0, 1]: helpers.py:121-124")
     need("synthesis_constraint", lambda v: not v, "attention window / monotonic constraint at synthesis: attention.py:201-214")
@@ -102,6 +100,8 @@ def make_config(hp, B, T_in, T_out, precision="bf16", teacher_forcing_ratio=None
     c.split_bf16 = int(precision == "fp32-class")
     c.mask_decoder = int(bool(hp.mask_decoder))
     c.cross_entropy_pos_weight = float(hp.cross_entropy_pos_weight)
+    c.unmasked_encoder = int(not getattr(hp, "mask_encoder", True))               # attention.py:140-151
+    c.noncumulative_weights = int(not getattr(hp, "cumulative_weights", True))    # attention.py:220-224
     ratio = float(getattr(hp, "tacotron_teacher_forcing_ratio", 1.0) if teacher_forcing_ratio is None else teacher_forcing_ratio)
     if not 0.0 <= ratio <= 1.0:
         raise L.T2Error("teacher_forcing_ratio %r outside [0, 1]" % (ratio,))
