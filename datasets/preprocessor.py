@@ -1,4 +1,4 @@
-"""Dataset preprocessing on the H100 front-end: wav -> (mu-law / raw audio, mel [frames, 80], linear [frames, 1025]) .npy files + the
+"""Dataset preprocessing on the H100 front-end: wav -> (mu-law / raw audio, mel [frames, 80], linear [frames, n_fft/2+1]) .npy files + the
 metadata rows `audio|mel|linear|time_steps|mel_frames|text` (reference datasets/preprocessor.py:12-165). Same step order: load,
 optional silence trim, pre-emphasis, separate rescale of the plain and pre-emphasised signals, mu-law + silence clipping when the
 WaveNet input is quantised, spectrograms from the PRE-EMPHASISED signal, right zero-padding so that len(audio) == frames * hop.

@@ -407,7 +407,7 @@ typedef struct {
   int highwaynet_layers;     /* cbhg_highwaynet_layers (4) */
   int highway_units;         /* cbhg_highway_units (128) */
   int rnn_units;             /* cbhg_rnn_units (128): GRU units per direction */
-  int num_freq;              /* 1025 */
+  int num_freq;              /* n_fft/2 + 1: 1025 at n_fft = 2048 */
   int n_priority_freq;       /* int(2000 / (sample_rate / 2) * num_freq): bins carrying the second half of the L1 weight */
   int clip_outputs, mask_decoder;
   float max_abs_value, lower_bound_decay, reg_weight;
@@ -453,6 +453,8 @@ typedef struct {
   int symmetric_mels, allow_clipping_in_normalization, signal_normalization;
 } t2_audio_config_t;
 
+/* n_fft: 512, 1024, 2048 or 4096 (else T2_ERR_UNSUPPORTED_SHAPE); 2 <= win_size <= n_fft; num_mels <= 128; fmax <= sample_rate / 2.
+ * Spectra have bins = n_fft/2 + 1 rows (257, 513, 1025 or 2049). */
 int t2_stft_mel_plan_bytes(const t2_audio_config_t* cfg, long long* bytes);
 /* builds twiddles, the periodic Hann window and the sparse Slaney mel filterbank (librosa.filters.mel restated in
  * fp64 on the host) into d_plan; synchronises the stream */
@@ -470,7 +472,7 @@ int t2_stft_mel_f32(const t2_audio_config_t* cfg, const void* d_plan, const floa
 int t2_mel_basis_f64(const t2_audio_config_t* cfg, double* h_basis);
 /* Griffin-Lim phase reconstruction on the GPU: replaces datasets/audio.py:151-161 (_griffin_lim: librosa istft / stft iterations)
  * and :163-176 (the TF-graph variant). d_mag: fp32 [B][frames][n_fft/2+1] magnitudes (already raised to hparams.power);
- * d_phase_io: optional float2 [B][frames][bins] unit phases (in: initial phases, out: final) - NULL draws exp(2 pi i u) from the
+ * d_phase_io: optional float2 [B][frames][n_fft/2+1] unit phases (in: initial phases, out: final) - NULL draws exp(2 pi i u) from the
  * counter hash under `seed` (the reference draws np.random.rand); iters = hparams.griffin_lim_iters re-estimation rounds (iters + 1
  * inverse transforms); d_wav: fp32 [B][hop * (frames - 1)] (librosa.istft length, centre-trimmed). Workspace: t2_griffin_lim_bytes. */
 int t2_griffin_lim_bytes(const t2_audio_config_t* cfg, int B, int frames, long long* bytes);

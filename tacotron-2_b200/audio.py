@@ -20,8 +20,11 @@ def make_config(hp):
     hop = hp.hop_size
     if hop is None:
         hop = int(hp.frame_shift_ms / 1000 * hp.sample_rate)
+    win = hp.win_size
+    if win is None:  # librosa.stft(win_length=None): the window spans the whole frame (reference hparams.py:81)
+        win = hp.n_fft
     c = AudioConfig()
-    c.sample_rate, c.n_fft, c.hop_size, c.win_size, c.num_mels = hp.sample_rate, hp.n_fft, hop, hp.win_size, hp.num_mels
+    c.sample_rate, c.n_fft, c.hop_size, c.win_size, c.num_mels = hp.sample_rate, hp.n_fft, hop, win, hp.num_mels
     c.fmin, c.fmax, c.magnitude_power = hp.fmin, hp.fmax, hp.magnitude_power
     c.min_level_db, c.ref_level_db, c.max_abs_value = hp.min_level_db, hp.ref_level_db, hp.max_abs_value
     c.symmetric_mels = int(hp.symmetric_mels)

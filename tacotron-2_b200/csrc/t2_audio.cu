@@ -10,6 +10,8 @@
 // normalised — one HBM read of the samples, one HBM write of num_mels floats per frame, nothing in between.
 // The FFT runs in fp64: the reference's spectra come from a double-precision FFT (numpy) and the dB floor sits
 // ~100 dB under the spectral peak, which fp32 butterflies cannot resolve to the 1e-3 parity tolerance.
+// n_fft is 512, 1024, 2048 or 4096 (the reference's advice, hparams.py:52: the first power of two above win_size,
+// i.e. 8, 16, 22.05-24 and 44.1-48 kHz audio); the FFT kernels are instantiated once per complex length N = n_fft / 2.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -22,10 +24,10 @@
 namespace t2 {
 namespace {
 
-constexpr int kNfft = 2048;
-constexpr int kN = kNfft / 2;      // complex FFT length
-constexpr int kBins = kN + 1;      // 1025
+constexpr int kV1Nfft = 2048;     // the v1 kernel (T2_STFT_V1=1) is sized for this n_fft only
 constexpr int kMaxMels = 128;
+
+bool nfft_supported(int n_fft) { return n_fft == 512 || n_fft == 1024 || n_fft == 2048 || n_fft == 4096; }
 
 struct Plan {
   // byte offsets inside the device plan buffer
@@ -66,7 +68,8 @@ void mel_basis(const t2_audio_config_t& c, std::vector<double>& W) {
 
 int make_plan(const t2_audio_config_t* c, Plan& p, std::vector<double>* basis_out) {
   T2_REQUIRE(c != nullptr, T2_ERR_INVALID_ARG, "null audio config");
-  T2_REQUIRE(c->n_fft == kNfft, T2_ERR_UNSUPPORTED_SHAPE, "n_fft must be %d (got %d)", kNfft, c->n_fft);
+  T2_REQUIRE(nfft_supported(c->n_fft), T2_ERR_UNSUPPORTED_SHAPE,
+             "n_fft must be 512, 1024, 2048 or 4096 (got %d): the first power of two above win_size (hparams.py:52)", c->n_fft);
   T2_REQUIRE(c->win_size >= 2 && c->win_size <= c->n_fft && c->hop_size >= 1, T2_ERR_INVALID_ARG, "bad win/hop");
   T2_REQUIRE(c->num_mels >= 1 && c->num_mels <= kMaxMels, T2_ERR_UNSUPPORTED_SHAPE, "num_mels out of range");
   T2_REQUIRE(c->fmax <= c->sample_rate / 2 && c->fmin >= 0, T2_ERR_INVALID_ARG, "bad fmin/fmax");
@@ -74,9 +77,10 @@ int make_plan(const t2_audio_config_t* c, Plan& p, std::vector<double>* basis_ou
   mel_basis(*c, W);
   int nnz = 0;
   for (double w : W) nnz += w != 0.0;
+  const int N = c->n_fft / 2;
   long long o = 0;
-  p.o_tw = o; o = al(o + kN * 16);
-  p.o_tw2 = o; o = al(o + (kN / 2 + 1) * 16);
+  p.o_tw = o; o = al(o + N * 16);
+  p.o_tw2 = o; o = al(o + (N / 2 + 1) * 16);
   p.o_win = o; o = al(o + c->win_size * 8);
   p.o_fstart = o; o = al(o + c->num_mels * 4);
   p.o_fcount = o; o = al(o + c->num_mels * 4);
@@ -92,8 +96,8 @@ struct StftArgs {
   const float* wav;       // [B][n_samples]
   float* mel;             // [B][frames][nm] or [B][nm][frames]
   float* lin;             // nullable, [B][frames][bins] or [B][bins][frames]
-  const double2* tw;      // W_1024^k
-  const double2* tw2;     // W_2048^k, k = 0..512
+  const double2* tw;      // W_N^k, k = 0..N-1 (N = n_fft / 2)
+  const double2* tw2;     // W_n_fft^k, k = 0..N/2
   const double* win;      // periodic Hann, win_size
   const int* fstart; const int* fcount; const int* foff; const double* fw;
   int B, n_samples, frames, hop, win_size, nm, time_major;
@@ -118,6 +122,7 @@ __device__ __forceinline__ float finish(const StftArgs& a, double v) {
 }
 
 __global__ void __launch_bounds__(256) stft_mel_kernel(StftArgs a) {
+  constexpr int kNfft = kV1Nfft, kN = kNfft / 2, kBins = kN + 1;
   __shared__ double2 buf0[kN];
   __shared__ double2 buf1[kN];
   __shared__ double pw[kBins + 7];
@@ -220,20 +225,33 @@ __global__ void __launch_bounds__(256) stft_mel_kernel(StftArgs a) {
   }
 }
 
-// ---- v2: register-radix FFT, 4 frames per CTA ------------------------------------------------------------------------------
-// 64 threads own one frame (16 complex points each); 1024 = 16 x 16 x 4 Stockham passes with the radix-16 butterflies held in
-// registers, so a frame crosses shared memory three times instead of ten (5 radix-4 passes x read + write) and never needs a
-// CTA-wide barrier: the two warps of a frame meet on their own named barrier. The first pass reads the windowed samples
-// straight from global memory (no staging pass). Shared-memory rows are padded by one element per 16 (17 j + r) so that the
-// transposing stores of the radix-16 passes are conflict-free for 16-byte elements. Post-FFT arithmetic is the v1 arithmetic.
-constexpr int kFramesPerCta = 4;
-constexpr int kFrameThreads = 64;
-constexpr int kPadN = kN + kN / 16;                 // padded complex buffer
-constexpr int kPwN = kBins + 7;
-constexpr int kV2SmemBytes = kFramesPerCta * (kPadN * 16 + kPwN * 8);
+// ---- v2: register-radix FFT, 4096 / N frames per CTA ------------------------------------------------------------------------
+// N / 16 threads own one frame (16 complex points each); N = 16 x 16 x R Stockham passes (R = N / 256 = 1, 2, 4 or 8) with the
+// radix-16 butterflies held in registers, so a frame crosses shared memory at most three times (n_fft = 2048: instead of ten,
+// 5 radix-4 passes x read + write) and never needs a CTA-wide barrier: the threads of a frame meet on their own named barrier,
+// or on a half-warp __syncwarp when a frame is 16 threads. The first pass reads the windowed samples straight from global memory
+// (no staging pass). Shared-memory rows are padded by one element per 16 (17 j + r) so that the transposing stores of the
+// radix-16 passes are conflict-free for 16-byte elements. Post-FFT arithmetic is the v1 arithmetic. The CTA is 256 threads for
+// every N and a frame's shared memory grows with N, so every size keeps ~102.5 KB per CTA and 2 CTAs per SM.
+constexpr int kCtaThreads = 256;
+template <int N>
+struct FftShape {
+  static_assert(N == 256 || N == 512 || N == 1024 || N == 2048, "complex FFT length N = n_fft / 2");
+  static constexpr int kFrameThreads = N / 16;
+  static constexpr int kFramesPerCta = kCtaThreads / kFrameThreads;
+  static constexpr int kPadN = N + N / 16;                    // padded complex buffer
+  static constexpr int kPwN = N + 8;                          // N + 1 power-spectrum bins, padded
+  static constexpr int kSmemBytes = kFramesPerCta * (kPadN * 16 + kPwN * 8);
+};
+static_assert(FftShape<1024>::kSmemBytes == 102656, "n_fft = 2048 keeps its shared-memory footprint");
 
 __device__ __forceinline__ int padi(int i) { return i + (i >> 4); }
-__device__ __forceinline__ void frame_sync(int slot) { asm volatile("bar.sync %0, 64;" ::"r"(slot + 1) : "memory"); }
+// the T threads of frame `slot` meet; T >= 32: named barrier slot + 1 (at most 8 frames per CTA), T = 16: half a warp
+template <int T>
+__device__ __forceinline__ void frame_sync(int slot) {
+  if constexpr (T >= 32) asm volatile("bar.sync %0, %1;" ::"r"(slot + 1), "n"(T) : "memory");
+  else __syncwarp(((1u << T) - 1) << (T * (slot & (32 / T - 1))));
+}
 __device__ __forceinline__ double2 cadd(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ double2 csub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
 // forward DFT-4 in place: (a, b, c, d) -> (X0, X1, X2, X3)
@@ -268,67 +286,92 @@ __device__ __forceinline__ void dft16(double2* v) {
     for (int j = i + 1; j < 4; ++j) { const double2 t = v[4 * i + j]; v[4 * i + j] = v[4 * j + i]; v[4 * j + i] = t; }
 }
 
-// The three Stockham passes of the 1024-point forward FFT of one frame. In: v[r] = z[j + 64 r] (thread j of the frame's 64). Out: the
-// transform in natural order in `buf` (padded index padi(k)), visible to all 64 threads of the frame.
-__device__ __forceinline__ void fft1024_passes(double2 (&v)[16], double2* buf, const double2* __restrict__ tw, int slot, int j) {
+// forward DFT-8 of v[0..7] (natural order in and out) as 2 x 4: X[k] = E[k] + W8^k O[k], X[k + 4] = E[k] - W8^k O[k]
+__device__ __forceinline__ void dft8(double2* v) {
+  constexpr double h = 0.70710678118654752440;
+  dft4(v[0], v[2], v[4], v[6]);                                   // E[k] at v[2 k]
+  dft4(v[1], v[3], v[5], v[7]);                                   // O[k] at v[2 k + 1]
+  const double2 o[4] = {v[1], cmul(v[3], make_double2(h, -h)), make_double2(v[5].y, -v[5].x), cmul(v[7], make_double2(-h, -h))};
+  const double2 e[4] = {v[0], v[2], v[4], v[6]};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { v[k] = cadd(e[k], o[k]); v[k + 4] = csub(e[k], o[k]); }
+}
+// forward DFT-R of v[0..R-1] in place, natural order in and out
+template <int R>
+__device__ __forceinline__ void dft_small(double2* v) {
+  if constexpr (R == 2) { const double2 t = v[1]; v[1] = csub(v[0], t); v[0] = cadd(v[0], t); }
+  else if constexpr (R == 4) dft4(v[0], v[1], v[2], v[3]);
+  else dft8(v);
+}
+
+// The Stockham passes of the N-point forward FFT of one frame (T = N / 16 threads). In: v[r] = z[j + T r] (thread j of the
+// frame's T). Out: the transform in natural order in `buf` (padded index padi(k)), visible to all T threads of the frame.
+template <int N>
+__device__ __forceinline__ void fft_passes(double2 (&v)[16], double2* buf, const double2* __restrict__ tw, int slot, int j) {
+    constexpr int T = N / 16, R = N / 256;
     dft16(v);
 #pragma unroll
     for (int r = 0; r < 16; ++r) buf[17 * j + r] = v[r];          // padi(16 j + r)
-    frame_sync(slot);
-    // pass 2 (radix 16, Ns = 16): twiddle W_256^(r k) = W_1024^(4 r k)
+    frame_sync<T>(slot);
+    // pass 2 (radix 16, Ns = 16): twiddle W_256^(r k) = W_N^(R r k)
     {
       const int k = j & 15;
 #pragma unroll
-      for (int r = 0; r < 16; ++r) v[r] = buf[padi(j + 64 * r)];
+      for (int r = 0; r < 16; ++r) v[r] = buf[padi(j + T * r)];
 #pragma unroll
-      for (int r = 1; r < 16; ++r) v[r] = cmul(v[r], __ldg(tw + 4 * r * k));
+      for (int r = 1; r < 16; ++r) v[r] = cmul(v[r], __ldg(tw + R * r * k));
       dft16(v);
-      frame_sync(slot);
+      frame_sync<T>(slot);
       const int base = (j - k) * 16 + k;
 #pragma unroll
       for (int r = 0; r < 16; ++r) buf[padi(base + 16 * r)] = v[r];
     }
-    frame_sync(slot);
-    // pass 3 (radix 4, Ns = 256): four butterflies per thread, output in natural order
+    frame_sync<T>(slot);
+    if constexpr (R > 1) {
+      // pass 3 (radix R, Ns = 256): 16 / R butterflies per thread, output in natural order
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int jj = j + 64 * u;
-      v[4 * u] = buf[padi(jj)];
+      for (int u = 0; u < 16 / R; ++u) {
+        const int jj = j + T * u;
+        v[R * u] = buf[padi(jj)];
 #pragma unroll
-      for (int r = 1; r < 4; ++r) v[4 * u + r] = cmul(buf[padi(jj + 256 * r)], __ldg(tw + r * jj));
-      dft4(v[4 * u], v[4 * u + 1], v[4 * u + 2], v[4 * u + 3]);
+        for (int r = 1; r < R; ++r) v[R * u + r] = cmul(buf[padi(jj + 256 * r)], __ldg(tw + r * jj));
+        dft_small<R>(v + R * u);
+      }
+      frame_sync<T>(slot);
+#pragma unroll
+      for (int u = 0; u < 16 / R; ++u)
+#pragma unroll
+        for (int r = 0; r < R; ++r) buf[padi(j + T * u + 256 * r)] = v[R * u + r];
+      frame_sync<T>(slot);
     }
-    frame_sync(slot);
-#pragma unroll
-    for (int u = 0; u < 4; ++u)
-#pragma unroll
-      for (int r = 0; r < 4; ++r) buf[padi(j + 64 * u + 256 * r)] = v[4 * u + r];
-    frame_sync(slot);
 }
 
-__global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) stft_mel_kernel_v2(StftArgs a) {
+template <int N>
+__global__ void __launch_bounds__(kCtaThreads, 2) stft_mel_kernel_v2(StftArgs a) {
+  using S = FftShape<N>;
+  constexpr int T = S::kFrameThreads, F = S::kFramesPerCta;
   extern __shared__ __align__(16) uint8_t smem_v2[];
-  const int slot = threadIdx.x / kFrameThreads;
-  const int j = threadIdx.x % kFrameThreads;
-  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * kPadN;
-  double* pw = reinterpret_cast<double*>(smem_v2 + kFramesPerCta * kPadN * 16) + slot * kPwN;
+  const int slot = threadIdx.x / T;
+  const int j = threadIdx.x % T;
+  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * S::kPadN;
+  double* pw = reinterpret_cast<double*>(smem_v2 + F * S::kPadN * 16) + slot * S::kPwN;
   const long long total = (long long)a.B * a.frames;
-  const int lpad = (kNfft - a.win_size) / 2;
-  for (long long fr = (long long)blockIdx.x * kFramesPerCta + slot; fr < total; fr += (long long)gridDim.x * kFramesPerCta) {
+  const int lpad = (2 * N - a.win_size) / 2;
+  for (long long fr = (long long)blockIdx.x * F + slot; fr < total; fr += (long long)gridDim.x * F) {
     const int b = int(fr / a.frames), f = int(fr % a.frames);
     const float* w = a.wav + (long long)b * a.n_samples;
     double2 v[16];
-    // pass 1 (radix 16, Ns = 1): v[r] = z[j + 64 r], z[n] = x[2n] + i x[2n+1] (windowed, centred, zero padded)
+    // pass 1 (radix 16, Ns = 1): v[r] = z[j + T r], z[n] = x[2n] + i x[2n+1] (windowed, centred, zero padded)
 #pragma unroll
     for (int r = 0; r < 16; ++r) {
-      const int q0 = 2 * (j + 64 * r);
+      const int q0 = 2 * (j + T * r);
       double c[2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int q = q0 + hh, wi = q - lpad;
         double s = 0.0;
         if (wi >= 0 && wi < a.win_size) {
-          const long long si = (long long)f * a.hop - kNfft / 2 + q;
+          const long long si = (long long)f * a.hop - N + q;
           if (si >= 0 && si < a.n_samples) {
             double x = double(__ldg(w + si));
             if (a.preemph != 0.f) x -= double(a.preemph) * (si > 0 ? double(__ldg(w + si - 1)) : 0.0);
@@ -339,16 +382,16 @@ __global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) stft_mel_ker
       }
       v[r] = make_double2(c[0], c[1]);
     }
-    fft1024_passes(v, buf, a.tw, slot, j);
+    fft_passes<N>(v, buf, a.tw, slot, j);
     // untangle to the real-FFT bins and take |X|^p (v1 arithmetic)
-    for (int k = j; k <= kN; k += kFrameThreads) {
-      const double2 zk = buf[padi(k & (kN - 1))];
-      const double2 zn = buf[padi((kN - k) & (kN - 1))];
+    for (int k = j; k <= N; k += T) {
+      const double2 zk = buf[padi(k & (N - 1))];
+      const double2 zn = buf[padi((N - k) & (N - 1))];
       const double2 e = make_double2(0.5 * (zk.x + zn.x), 0.5 * (zk.y - zn.y));
       const double2 o = make_double2(0.5 * (zk.y + zn.y), -0.5 * (zk.x - zn.x));
-      const int kk = k <= kN / 2 ? k : kN - k;
+      const int kk = k <= N / 2 ? k : N - k;
       double2 t2w = __ldg(a.tw2 + kk);
-      if (k > kN / 2) t2w = make_double2(-t2w.x, t2w.y);
+      if (k > N / 2) t2w = make_double2(-t2w.x, t2w.y);
       const double2 ow = cmul(o, t2w);
       const float ref = float(e.x + ow.x), imf = float(e.y + ow.y);
       const double mag2 = double(ref) * double(ref) + double(imf) * double(imf);
@@ -362,16 +405,16 @@ __global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) stft_mel_ker
       pw[k] = val;
       if (a.lin) {
         const float r = finish(a, val);
-        if (a.time_major) a.lin[((long long)b * a.frames + f) * kBins + k] = r;
-        else a.lin[((long long)b * kBins + k) * a.frames + f] = r;
+        if (a.time_major) a.lin[((long long)b * a.frames + f) * (N + 1) + k] = r;
+        else a.lin[((long long)b * (N + 1) + k) * a.frames + f] = r;
       }
     }
-    frame_sync(slot);
+    frame_sync<T>(slot);
     // sparse mel filterbank: one thread per filter (the long high-frequency filters pair up with the short low ones)
-    for (int m = j; m < a.nm; m += kFrameThreads) {
+    for (int m = j; m < a.nm; m += T) {
       const int s = __ldg(a.fstart + m), n = __ldg(a.fcount + m);
       const double* fw = a.fw + __ldg(a.foff + m);
-      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;   // four independent chains: the longest filter spans ~70 bins
+      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;   // four independent chains: the longest filter spans ~70 bins at n_fft = 2048
       int i = 0;
       for (; i + 4 <= n; i += 4) {
         a0 += __ldg(fw + i) * pw[s + i];
@@ -385,7 +428,7 @@ __global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) stft_mel_ker
       if (a.time_major) a.mel[((long long)b * a.frames + f) * a.nm + m] = r;
       else a.mel[((long long)b * a.nm + m) * a.frames + f] = r;
     }
-    frame_sync(slot);
+    frame_sync<T>(slot);
   }
 }
 
@@ -402,52 +445,55 @@ struct GlArgs {
   float* fr;              // [B][frames][win] windowed time-domain frames
   float* y;               // [B][n_out]
   const double2* tw; const double2* tw2; const double* win;
-  int B, frames, hop, win_size, n_out;
+  int B, frames, hop, win_size, n_out, n_fft;
 };
-__global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) gl_istft_kernel(GlArgs a) {
+template <int N>
+__global__ void __launch_bounds__(kCtaThreads, 2) gl_istft_kernel(GlArgs a) {
+  using Sh = FftShape<N>;
+  constexpr int T = Sh::kFrameThreads, F = Sh::kFramesPerCta;
   extern __shared__ __align__(16) uint8_t smem_v2[];
-  const int slot = threadIdx.x / kFrameThreads, j = threadIdx.x % kFrameThreads;
-  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * kPadN;
+  const int slot = threadIdx.x / T, j = threadIdx.x % T;
+  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * Sh::kPadN;
   const long long total = (long long)a.B * a.frames;
-  const int lpad = (kNfft - a.win_size) / 2;
-  for (long long fr = (long long)blockIdx.x * kFramesPerCta + slot; fr < total; fr += (long long)gridDim.x * kFramesPerCta) {
-    const float* S = a.mag + fr * kBins;
-    const float2* ph = a.phase + fr * kBins;
+  const int lpad = (2 * N - a.win_size) / 2;
+  for (long long fr = (long long)blockIdx.x * F + slot; fr < total; fr += (long long)gridDim.x * F) {
+    const float* S = a.mag + fr * (N + 1);
+    const float2* ph = a.phase + fr * (N + 1);
     double2 v[16];
 #pragma unroll
     for (int r = 0; r < 16; ++r) {
-      const int k = j + 64 * r;                     // Z[k] = E[k] + i O[k], E / O from X[k] and conj(X[N/2 - k])
-      const float sk = S[k], sn = S[kN - k];
-      const float2 pk = ph[k], pn = ph[kN - k];
+      const int k = j + T * r;                      // Z[k] = E[k] + i O[k], E / O from X[k] and conj(X[N - k])
+      const float sk = S[k], sn = S[N - k];
+      const float2 pk = ph[k], pn = ph[N - k];
       double2 xk = make_double2(double(sk) * pk.x, double(sk) * pk.y);
-      double2 xn = make_double2(double(sn) * pn.x, -double(sn) * pn.y);           // conj(X[N/2 - k])
+      double2 xn = make_double2(double(sn) * pn.x, -double(sn) * pn.y);           // conj(X[N - k])
       if (k == 0) { xk.y = 0.0; xn.y = 0.0; }       // a real inverse transform ignores the imaginary parts of the DC / Nyquist bins (np.fft.irfft)
       const double2 e = make_double2(0.5 * (xk.x + xn.x), 0.5 * (xk.y + xn.y));
       const double2 d = make_double2(0.5 * (xk.x - xn.x), 0.5 * (xk.y - xn.y));
-      const int kk = k <= kN / 2 ? k : kN - k;
-      double2 w = __ldg(a.tw2 + kk);                // W_2048^kk = exp(-2 pi i kk / 2048); needed: exp(+2 pi i k / 2048)
-      w = k <= kN / 2 ? make_double2(w.x, -w.y) : make_double2(-w.x, -w.y);       // k > N/4: exp(+i pi (N/2 - kk) / (N/2)) = -conj(exp(+..kk))
+      const int kk = k <= N / 2 ? k : N - k;
+      double2 w = __ldg(a.tw2 + kk);                // W_n_fft^kk = exp(-2 pi i kk / n_fft); needed: exp(+2 pi i k / n_fft)
+      w = k <= N / 2 ? make_double2(w.x, -w.y) : make_double2(-w.x, -w.y);         // k > n_fft/4: exp(+i pi (N - kk) / N) = -conj(exp(+..kk))
       const double2 o = cmul(d, w);
       const double2 z = make_double2(e.x - o.y, e.y + o.x);                       // E + i O
-      v[r] = make_double2(z.x, -z.y);               // conj: the inverse transform is conj(FFT(conj(Z))) / (N/2)
+      v[r] = make_double2(z.x, -z.y);               // conj: the inverse transform is conj(FFT(conj(Z))) / N
     }
-    fft1024_passes(v, buf, a.tw, slot, j);
+    fft_passes<N>(v, buf, a.tw, slot, j);
     float* out = a.fr + fr * a.win_size;
-    for (int wi = j; wi < a.win_size; wi += kFrameThreads) {
-      const int q = wi + lpad;                      // sample q of the n_fft frame = (q even ? Re : Im) z[q / 2], z = conj(W) / (N/2)
+    for (int wi = j; wi < a.win_size; wi += T) {
+      const int q = wi + lpad;                      // sample q of the n_fft frame = (q even ? Re : Im) z[q / 2], z = conj(W) / N
       const double2 wv = buf[padi(q >> 1)];
-      const double x = ((q & 1) ? -wv.y : wv.x) * (1.0 / kN);
+      const double x = ((q & 1) ? -wv.y : wv.x) * (1.0 / N);
       out[wi] = float(x * __ldg(a.win + wi));
     }
-    frame_sync(slot);
+    frame_sync<T>(slot);
   }
 }
 __global__ void gl_ola_kernel(GlArgs a) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= (long long)a.B * a.n_out) return;
   const int b = int(e / a.n_out), n = int(e % a.n_out);
-  const int lpad = (kNfft - a.win_size) / 2;
-  const int p = n + kNfft / 2 - lpad;               // position relative to the window support of frame 0
+  const int lpad = (a.n_fft - a.win_size) / 2;
+  const int p = n + a.n_fft / 2 - lpad;             // position relative to the window support of frame 0
   int k1 = p / a.hop;
   if (k1 > a.frames - 1) k1 = a.frames - 1;
   float acc = 0.f, wss = 0.f;
@@ -460,48 +506,51 @@ __global__ void gl_ola_kernel(GlArgs a) {
   }
   a.y[e] = wss > 1.17549435e-38f ? acc / wss : acc;
 }
-__global__ void __launch_bounds__(kFramesPerCta * kFrameThreads, 2) gl_stft_kernel(GlArgs a) {
+template <int N>
+__global__ void __launch_bounds__(kCtaThreads, 2) gl_stft_kernel(GlArgs a) {
+  using Sh = FftShape<N>;
+  constexpr int T = Sh::kFrameThreads, F = Sh::kFramesPerCta;
   extern __shared__ __align__(16) uint8_t smem_v2[];
-  const int slot = threadIdx.x / kFrameThreads, j = threadIdx.x % kFrameThreads;
-  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * kPadN;
+  const int slot = threadIdx.x / T, j = threadIdx.x % T;
+  double2* buf = reinterpret_cast<double2*>(smem_v2) + slot * Sh::kPadN;
   const long long total = (long long)a.B * a.frames;
-  const int lpad = (kNfft - a.win_size) / 2;
-  for (long long fr = (long long)blockIdx.x * kFramesPerCta + slot; fr < total; fr += (long long)gridDim.x * kFramesPerCta) {
+  const int lpad = (2 * N - a.win_size) / 2;
+  for (long long fr = (long long)blockIdx.x * F + slot; fr < total; fr += (long long)gridDim.x * F) {
     const int b = int(fr / a.frames), f = int(fr % a.frames);
     const float* w = a.y + (long long)b * a.n_out;
     double2 v[16];
 #pragma unroll
     for (int r = 0; r < 16; ++r) {
-      const int q0 = 2 * (j + 64 * r);
+      const int q0 = 2 * (j + T * r);
       double c[2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int q = q0 + hh, wi = q - lpad;
         double sv = 0.0;
         if (wi >= 0 && wi < a.win_size) {
-          const long long si = (long long)f * a.hop - kNfft / 2 + q;
+          const long long si = (long long)f * a.hop - N + q;
           if (si >= 0 && si < a.n_out) sv = double(__ldg(w + si)) * __ldg(a.win + wi);
         }
         c[hh] = sv;
       }
       v[r] = make_double2(c[0], c[1]);
     }
-    fft1024_passes(v, buf, a.tw, slot, j);
-    float2* ph = a.phase + fr * kBins;
-    for (int k = j; k <= kN; k += kFrameThreads) {
-      const double2 zk = buf[padi(k & (kN - 1))];
-      const double2 zn = buf[padi((kN - k) & (kN - 1))];
+    fft_passes<N>(v, buf, a.tw, slot, j);
+    float2* ph = a.phase + fr * (N + 1);
+    for (int k = j; k <= N; k += T) {
+      const double2 zk = buf[padi(k & (N - 1))];
+      const double2 zn = buf[padi((N - k) & (N - 1))];
       const double2 e = make_double2(0.5 * (zk.x + zn.x), 0.5 * (zk.y - zn.y));
       const double2 o = make_double2(0.5 * (zk.y + zn.y), -0.5 * (zk.x - zn.x));
-      const int kk = k <= kN / 2 ? k : kN - k;
+      const int kk = k <= N / 2 ? k : N - k;
       double2 t2w = __ldg(a.tw2 + kk);
-      if (k > kN / 2) t2w = make_double2(-t2w.x, t2w.y);
+      if (k > N / 2) t2w = make_double2(-t2w.x, t2w.y);
       const double2 ow = cmul(o, t2w);
       const float re = float(e.x + ow.x), im = float(e.y + ow.y);   // complex64 like librosa's STFT matrix
       const float m = sqrtf(re * re + im * im);
       ph[k] = m > 0.f ? make_float2(re / m, im / m) : make_float2(1.f, 0.f);      // np.angle(0) = 0
     }
-    frame_sync(slot);
+    frame_sync<T>(slot);
   }
 }
 // initial phases exp(2 pi i u), u from the counter hash (the reference draws np.random.rand)
@@ -558,6 +607,45 @@ __global__ void inv_mulaw_quantize_kernel(const int* __restrict__ q, float* __re
 
 inline unsigned nblk(long long n) { return (unsigned)((n + 255) / 256); }
 
+// grid of the frame-parallel kernels: 2 resident CTAs per SM (~102.5 KB smem, 256 threads, <= 128 registers each)
+template <int N>
+unsigned frame_grid(long long frames, int sms) {
+  const long long groups = (frames + FftShape<N>::kFramesPerCta - 1) / FftShape<N>::kFramesPerCta, cap = (long long)sms * 2;
+  return (unsigned)(groups < cap ? groups : cap);
+}
+
+template <int N>
+int launch_stft_mel(const StftArgs& a, int sms, cudaStream_t st) {
+  constexpr int smem = FftShape<N>::kSmemBytes;
+  static bool configured = false;
+  if (!configured) {
+    T2_CHECK_CUDA(cudaFuncSetAttribute(stft_mel_kernel_v2<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = true;
+  }
+  stft_mel_kernel_v2<N><<<frame_grid<N>((long long)a.B * a.frames, sms), kCtaThreads, smem, st>>>(a); t2_count_launch();
+  return T2_OK;
+}
+
+template <int N>
+int launch_griffin_lim(const GlArgs& a, int iters, bool init_phase, unsigned long long seed, int sms, cudaStream_t st) {
+  constexpr int smem = FftShape<N>::kSmemBytes;
+  static bool configured = false;
+  if (!configured) {
+    T2_CHECK_CUDA(cudaFuncSetAttribute(gl_istft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    T2_CHECK_CUDA(cudaFuncSetAttribute(gl_stft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = true;
+  }
+  const long long total = (long long)a.B * a.frames, ny = (long long)a.B * a.n_out;
+  const unsigned grid = frame_grid<N>(total, sms);
+  if (init_phase) { gl_init_phase_kernel<<<nblk(total * (N + 1)), 256, 0, st>>>(a.phase, total * (N + 1), seed); t2_count_launch(); }
+  for (int it = 0; it <= iters; ++it) {
+    gl_istft_kernel<N><<<grid, kCtaThreads, smem, st>>>(a); t2_count_launch();
+    gl_ola_kernel<<<nblk(ny), 256, 0, st>>>(a); t2_count_launch();
+    if (it < iters) { gl_stft_kernel<N><<<grid, kCtaThreads, smem, st>>>(a); t2_count_launch(); }
+  }
+  return T2_OK;
+}
+
 }  // namespace
 }  // namespace t2
 
@@ -577,10 +665,11 @@ extern "C" int t2_stft_mel_plan_init(const t2_audio_config_t* cfg, void* d_plan,
   int rc = make_plan(cfg, p, &W);
   if (rc) return rc;
   std::vector<uint8_t> h(p.bytes, 0);
+  const int n_fft = cfg->n_fft, N = n_fft / 2;
   double* tw = reinterpret_cast<double*>(h.data() + p.o_tw);
-  for (int k = 0; k < kN; ++k) { tw[2 * k] = cos(-2.0 * M_PI * k / kN); tw[2 * k + 1] = sin(-2.0 * M_PI * k / kN); }
+  for (int k = 0; k < N; ++k) { tw[2 * k] = cos(-2.0 * M_PI * k / N); tw[2 * k + 1] = sin(-2.0 * M_PI * k / N); }
   double* tw2 = reinterpret_cast<double*>(h.data() + p.o_tw2);
-  for (int k = 0; k <= kN / 2; ++k) { tw2[2 * k] = cos(-2.0 * M_PI * k / kNfft); tw2[2 * k + 1] = sin(-2.0 * M_PI * k / kNfft); }
+  for (int k = 0; k <= N / 2; ++k) { tw2[2 * k] = cos(-2.0 * M_PI * k / n_fft); tw2[2 * k + 1] = sin(-2.0 * M_PI * k / n_fft); }
   double* win = reinterpret_cast<double*>(h.data() + p.o_win);
   for (int n = 0; n < cfg->win_size; ++n) win[n] = 0.5 - 0.5 * cos(2.0 * M_PI * n / cfg->win_size);  // periodic Hann
   int* fstart = reinterpret_cast<int*>(h.data() + p.o_fstart);
@@ -638,22 +727,23 @@ extern "C" int t2_stft_mel_f32(const t2_audio_config_t* cfg, const void* d_plan,
   int dev = 0, sms = 148;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   static int use_v1 = -1;
   if (use_v1 < 0) { const char* e = getenv("T2_STFT_V1"); use_v1 = (e && e[0] == '1') ? 1 : 0; }
   if (use_v1) {
+    T2_REQUIRE(cfg->n_fft == kV1Nfft, T2_ERR_UNSUPPORTED_SHAPE, "T2_STFT_V1=1: the v1 kernel runs n_fft = %d only (got %d)", kV1Nfft, cfg->n_fft);
     const long long cap = (long long)sms * 4;  // 4 resident CTAs per SM (41 KB smem, 256 threads each)
     const unsigned grid = (unsigned)(total < cap ? total : cap);
-    stft_mel_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(a); t2_count_launch();
+    stft_mel_kernel<<<grid, 256, 0, st>>>(a); t2_count_launch();
   } else {
-    static bool configured = false;
-    if (!configured) {
-      T2_CHECK_CUDA(cudaFuncSetAttribute(stft_mel_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, kV2SmemBytes));
-      configured = true;
+    switch (cfg->n_fft) {
+      case 512: rc = launch_stft_mel<256>(a, sms, st); break;
+      case 1024: rc = launch_stft_mel<512>(a, sms, st); break;
+      case 2048: rc = launch_stft_mel<1024>(a, sms, st); break;
+      case 4096: rc = launch_stft_mel<2048>(a, sms, st); break;
+      default: rc = t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "stft_mel: no kernel for n_fft %d", cfg->n_fft);
     }
-    const long long groups = (total + kFramesPerCta - 1) / kFramesPerCta;
-    const long long cap = (long long)sms * 2;  // 2 resident CTAs per SM (102 KB smem, 256 threads, <= 128 registers each)
-    const unsigned grid = (unsigned)(groups < cap ? groups : cap);
-    stft_mel_kernel_v2<<<grid, kFramesPerCta * kFrameThreads, kV2SmemBytes, static_cast<cudaStream_t>(stream)>>>(a); t2_count_launch();
+    if (rc) return rc;
   }
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -671,7 +761,7 @@ extern "C" int t2_mel_basis_f64(const t2_audio_config_t* cfg, double* h_basis) {
 
 extern "C" int t2_griffin_lim_bytes(const t2_audio_config_t* cfg, int B, int frames, long long* bytes) {
   T2_REQUIRE(cfg && bytes && B >= 1 && frames >= 2, T2_ERR_INVALID_ARG, "griffin_lim_bytes: bad arguments");
-  *bytes = al((long long)B * frames * kBins * 8) + al((long long)B * frames * cfg->win_size * 4);
+  *bytes = al((long long)B * frames * (cfg->n_fft / 2 + 1) * 8) + al((long long)B * frames * cfg->win_size * 4);
   return T2_OK;
 }
 
@@ -688,31 +778,25 @@ extern "C" int t2_griffin_lim_f32(const t2_audio_config_t* cfg, const void* d_pl
   memset(&a, 0, sizeof(a));
   a.mag = d_mag;
   a.phase = d_phase_io ? reinterpret_cast<float2*>(d_phase_io) : reinterpret_cast<float2*>(ws);
-  a.fr = reinterpret_cast<float*>(ws + al((long long)B * frames * kBins * 8));
+  a.fr = reinterpret_cast<float*>(ws + al((long long)B * frames * (cfg->n_fft / 2 + 1) * 8));
   a.y = d_wav;
   a.tw = reinterpret_cast<const double2*>(pl + p.o_tw);
   a.tw2 = reinterpret_cast<const double2*>(pl + p.o_tw2);
   a.win = reinterpret_cast<const double*>(pl + p.o_win);
   a.B = B; a.frames = frames; a.hop = cfg->hop_size; a.win_size = cfg->win_size; a.n_out = cfg->hop_size * (frames - 1);
-  static bool configured = false;
-  if (!configured) {
-    T2_CHECK_CUDA(cudaFuncSetAttribute(gl_istft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kV2SmemBytes));
-    T2_CHECK_CUDA(cudaFuncSetAttribute(gl_stft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kV2SmemBytes));
-    configured = true;
-  }
-  const long long total = (long long)B * frames;
+  a.n_fft = cfg->n_fft;
   int dev = 0, sms = 148;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long groups = (total + kFramesPerCta - 1) / kFramesPerCta, cap = (long long)sms * 2;
-  const unsigned grid = (unsigned)(groups < cap ? groups : cap);
-  const long long ny = (long long)B * a.n_out;
-  if (!d_phase_io) { gl_init_phase_kernel<<<nblk(total * kBins), 256, 0, st>>>(a.phase, total * kBins, seed); t2_count_launch(); }
-  for (int it = 0; it <= iters; ++it) {
-    gl_istft_kernel<<<grid, kFramesPerCta * kFrameThreads, kV2SmemBytes, st>>>(a); t2_count_launch();
-    gl_ola_kernel<<<nblk(ny), 256, 0, st>>>(a); t2_count_launch();
-    if (it < iters) { gl_stft_kernel<<<grid, kFramesPerCta * kFrameThreads, kV2SmemBytes, st>>>(a); t2_count_launch(); }
+  const bool init_phase = d_phase_io == nullptr;
+  switch (cfg->n_fft) {
+    case 512: rc = launch_griffin_lim<256>(a, iters, init_phase, seed, sms, st); break;
+    case 1024: rc = launch_griffin_lim<512>(a, iters, init_phase, seed, sms, st); break;
+    case 2048: rc = launch_griffin_lim<1024>(a, iters, init_phase, seed, sms, st); break;
+    case 4096: rc = launch_griffin_lim<2048>(a, iters, init_phase, seed, sms, st); break;
+    default: rc = t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "griffin_lim: no kernel for n_fft %d", cfg->n_fft);
   }
+  if (rc) return rc;
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
