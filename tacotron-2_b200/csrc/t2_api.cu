@@ -53,19 +53,11 @@ extern "C" int t2_dbg_wgrad(const void* a, int Ca, const void* bm, int Cb, int B
                             float scale, float* out, void* stream) {
   using namespace t2;
   ActT maps[2] = {make_act(a, Ca, T, B), make_act(bm, Cb, T, B)};
+  WgradTile proto;
+  memset(&proto, 0, sizeof(proto));
+  proto.a_map = 0; proto.a_shift = shift_a; proto.b_map = 1; proto.scale = scale;
   std::vector<WgradTile> tiles;
-  for (int m0 = 0; m0 < Ca; m0 += 128)
-    for (int n0 = 0; n0 < Cb; n0 += 256) {
-      WgradTile t;
-      memset(&t, 0, sizeof(t));
-      t.a_map = 0; t.a_ch0 = m0; t.a_shift = shift_a; t.a_layer = 0;
-      t.b_map = 1; t.b_ch0 = n0; t.b_shift = 0; t.b_layer = 0;
-      t.out_off = (long long)m0 * Cb + n0; t.ldc = Cb;
-      t.m_valid = Ca - m0 < 128 ? Ca - m0 : 128;
-      t.n_valid = Cb - n0 < 256 ? Cb - n0 : 256;
-      t.scale = scale; t.accumulate = 0; t.div = nullptr;
-      tiles.push_back(t);
-    }
+  append_wgrad_tiles(tiles, proto, 0, Ca, 0, Cb, 0, Cb);
   WgradTile* dt = nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   T2_CHECK_CUDA(cudaMallocAsync(&dt, tiles.size() * sizeof(WgradTile), st));

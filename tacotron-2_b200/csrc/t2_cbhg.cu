@@ -27,31 +27,28 @@
 #include "../../include/t2b200.h"
 #include "t2_common.cuh"
 #include "t2_gemm.h"
+#include "t2_params.h"
 
 namespace t2 {
 namespace {
 
 typedef __nv_bfloat16 bf16;
-inline long long al256(long long v) { return (v + 255) / 256 * 256; }
-inline dim3 g1(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
 constexpr int kMaxBank = 16, kMaxHw = 8;
 constexpr int kGruItems = 4;          // batch items per CTA of the recurrent kernels
 constexpr int kGruThreads = 256;
 
-struct CPT { std::string name; long long off; int ndim; int shape[4]; bool trainable, reg; };
 struct CConv {
   int cin, cout, k, act;               // act: 1 relu, 0 none
   long long p_k, p_b, p_g, p_be, p_mm, p_mv;
   int cinp, coutp;                     // channels rounded up to 64 (K slots of the packed operands)
   long long k_w, k_wT;                 // packed forward [cout][k * cinp], packed dgrad [cin rows][k * coutp]
 };
-struct PJ { long long src_off; int K, N; long long dst_off; int dst_ld, transpose, col0; };
 
 struct CL {
   t2_cbhg_config_t c;
   int B, T, M, K, CC, KC, PJc, PK, NH, HU, RU, NF, NFP, NFR;
   long long N;
-  std::vector<CPT> params;
+  std::vector<Param> params;
   long long n_params;
   std::vector<CConv> bank;
   CConv proj1, proj2;
@@ -68,21 +65,7 @@ struct CL {
   int n_jobs, n_reg;
 };
 
-long long addp(CL& lo, const std::string& name, std::initializer_list<int> shape, bool trainable = true) {
-  CPT p; p.name = name; p.off = lo.n_params; p.ndim = int(shape.size());
-  long long n = 1; int i = 0;
-  for (int s : shape) { p.shape[i++] = s; n *= s; }
-  for (; i < 4; ++i) p.shape[i] = 1;
-  p.trainable = trainable;
-  // tacotron.py:343-345: no 'bias', 'Bias', '_projection', 'inputs_embedding', 'RNN', 'LSTM' in the variable name
-  p.reg = trainable && name.find("bias") == std::string::npos && name.find("_projection") == std::string::npos &&
-          name.find("RNN") == std::string::npos;
-  lo.n_params += (n + 3) / 4 * 4;
-  lo.params.push_back(p);
-  return p.off;
-}
-
-int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PJ>* jobs_out) {
+int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   T2_REQUIRE(cfg != nullptr, T2_ERR_INVALID_ARG, "null CBHG config");
   lo.c = *cfg;
   lo.B = cfg->B; lo.T = cfg->T; lo.M = cfg->num_mels; lo.K = cfg->kernels; lo.CC = cfg->conv_channels; lo.KC = lo.K * lo.CC;
@@ -102,9 +85,9 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PJ>* jobs_out) {
   lo.n_params = 0; lo.params.clear(); lo.bank.clear();
   const std::string P = "CBHG_postnet/";
   auto conv_params = [&](CConv& L, const std::string& pre) {
-    L.p_k = addp(lo, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = addp(lo, pre + "bias", {L.cout});
-    L.p_g = addp(lo, pre + "gamma", {L.cout}); L.p_be = addp(lo, pre + "beta", {L.cout});
-    L.p_mm = addp(lo, pre + "moving_mean", {L.cout}, false); L.p_mv = addp(lo, pre + "moving_variance", {L.cout}, false);
+    L.p_k = add_param(lo.params, lo.n_params, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = add_param(lo.params, lo.n_params, pre + "bias", {L.cout});
+    L.p_g = add_param(lo.params, lo.n_params, pre + "gamma", {L.cout}); L.p_be = add_param(lo.params, lo.n_params, pre + "beta", {L.cout});
+    L.p_mm = add_param(lo.params, lo.n_params, pre + "moving_mean", {L.cout}, false); L.p_mv = add_param(lo.params, lo.n_params, pre + "moving_variance", {L.cout}, false);
     L.cinp = (L.cin + 63) / 64 * 64; L.coutp = (L.cout + 63) / 64 * 64;
   };
   for (int k = 1; k <= lo.K; ++k) {
@@ -116,35 +99,31 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PJ>* jobs_out) {
   lo.proj2.cin = lo.PJc; lo.proj2.cout = lo.M; lo.proj2.k = lo.PK; lo.proj2.act = 0; conv_params(lo.proj2, P + "proj2/");
   lo.has_dense = lo.M != lo.HU;
   T2_REQUIRE(lo.has_dense, T2_ERR_UNSUPPORTED_SHAPE, "CBHG: num_mels == highway_units (no dense layer) is not implemented");
-  lo.p_dk = addp(lo, P + "dense/kernel", {lo.M, lo.HU}); lo.p_db = addp(lo, P + "dense/bias", {lo.HU});
+  lo.p_dk = add_param(lo.params, lo.n_params, P + "dense/kernel", {lo.M, lo.HU}); lo.p_db = add_param(lo.params, lo.n_params, P + "dense/bias", {lo.HU});
   for (int i = 0; i < lo.NH; ++i) {
     char b[64];
     for (int j = 0; j < 2; ++j) {
       snprintf(b, sizeof(b), "highwaynet_%d/%s/", i + 1, j == 0 ? "H" : "T");
-      lo.p_hk[i][j] = addp(lo, P + b + "kernel", {lo.HU, lo.HU}); lo.p_hb[i][j] = addp(lo, P + b + "bias", {lo.HU});
+      lo.p_hk[i][j] = add_param(lo.params, lo.n_params, P + b + "kernel", {lo.HU, lo.HU}); lo.p_hb[i][j] = add_param(lo.params, lo.n_params, P + b + "bias", {lo.HU});
     }
   }
   const char* dn[2] = {"forward_RNN/", "backward_RNN/"};
   for (int d = 0; d < 2; ++d) {
-    lo.p_gk[d] = addp(lo, P + dn[d] + "gates/kernel", {lo.HU + lo.RU, 2 * lo.RU}); lo.p_gb[d] = addp(lo, P + dn[d] + "gates/bias", {2 * lo.RU});
-    lo.p_ck[d] = addp(lo, P + dn[d] + "candidate/kernel", {lo.HU + lo.RU, lo.RU}); lo.p_cb[d] = addp(lo, P + dn[d] + "candidate/bias", {lo.RU});
+    lo.p_gk[d] = add_param(lo.params, lo.n_params, P + dn[d] + "gates/kernel", {lo.HU + lo.RU, 2 * lo.RU}); lo.p_gb[d] = add_param(lo.params, lo.n_params, P + dn[d] + "gates/bias", {2 * lo.RU});
+    lo.p_ck[d] = add_param(lo.params, lo.n_params, P + dn[d] + "candidate/kernel", {lo.HU + lo.RU, lo.RU}); lo.p_cb[d] = add_param(lo.params, lo.n_params, P + dn[d] + "candidate/bias", {lo.RU});
   }
-  lo.p_lk = addp(lo, "cbhg_linear_specs_projection/kernel", {2 * lo.RU, lo.NF}); lo.p_lb = addp(lo, "cbhg_linear_specs_projection/bias", {lo.NF});
+  lo.p_lk = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/kernel", {2 * lo.RU, lo.NF}); lo.p_lb = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/bias", {lo.NF});
 
   // ---- packed operands ----
-  std::vector<PJ> jobs;
-  long long o = 0;
-  auto takeb = [&](long long bytes) { long long r = o; o = al256(o + bytes); return r; };
-  auto pj = [&](long long src, int K, int N, long long dst_bytes, int ld, int tr, int col0) {
-    PJ j; j.src_off = src; j.K = K; j.N = N; j.dst_off = dst_bytes / 2; j.dst_ld = ld; j.transpose = tr; j.col0 = col0; jobs.push_back(j);
-  };
+  std::vector<PackJob> jobs;
+  Arena pk;
   auto conv_pack = [&](CConv& L, bool with_t) {
     const int rows_f = (L.cout + 127) / 128 * 128, rows_t = (L.cin + 127) / 128 * 128;
-    L.k_w = takeb(2LL * rows_f * L.k * L.cinp);
-    L.k_wT = with_t ? takeb(2LL * rows_t * L.k * L.coutp) : 0;
+    L.k_w = pk.take(2LL * rows_f * L.k * L.cinp);
+    L.k_wT = with_t ? pk.take(2LL * rows_t * L.k * L.coutp) : 0;
     for (int j = 0; j < L.k; ++j) {
-      pj(L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
-      if (with_t) pj(L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
+      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
+      if (with_t) add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
     }
   };
   for (auto& L : lo.bank) conv_pack(L, false);
@@ -158,73 +137,73 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PJ>* jobs_out) {
   }
   T2_REQUIRE(lo.n_grp <= 3, T2_ERR_UNSUPPORTED_SHAPE, "CBHG: conv bank too large for three data-gradient groups");
   for (int g = 0; g < lo.n_grp; ++g) {
-    lo.k_bankT[g] = takeb(2LL * 128 * lo.grp_taps[g] * lo.CC);
+    lo.k_bankT[g] = pk.take(2LL * 128 * lo.grp_taps[g] * lo.CC);
     int slot = 0;
     for (int l = lo.grp_first[g]; l < lo.grp_first[g + 1]; ++l)
       for (int j = 0; j < lo.bank[l].k; ++j, ++slot)
-        pj(lo.bank[l].p_k + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
+        add_pack(jobs, lo.bank[l].p_k + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
   }
   const int Mp = 128;
-  lo.k_dense = takeb(2LL * lo.HU * Mp); pj(lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0);
-  lo.k_denseT = takeb(2LL * 128 * lo.HU); pj(lo.p_dk, lo.M, lo.HU, lo.k_denseT, lo.HU, 0, 0);
+  lo.k_dense = pk.take(2LL * lo.HU * Mp); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0);
+  lo.k_denseT = pk.take(2LL * 128 * lo.HU); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_denseT, lo.HU, 0, 0);
   for (int i = 0; i < lo.NH; ++i) {
-    lo.k_hw[i] = takeb(2LL * 2 * lo.HU * lo.HU);             // rows [H units | T units][K = HU]
-    pj(lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 1, 0);
-    { PJ j; j.src_off = lo.p_hk[i][1]; j.K = lo.HU; j.N = lo.HU; j.dst_off = lo.k_hw[i] / 2 + (long long)lo.HU * lo.HU; j.dst_ld = lo.HU; j.transpose = 1; j.col0 = 0; jobs.push_back(j); }
-    lo.k_hwT[i] = takeb(2LL * lo.HU * 2 * lo.HU);            // [HU in][H units | T units]
-    pj(lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, 0);
-    pj(lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, lo.HU);
+    lo.k_hw[i] = pk.take(2LL * 2 * lo.HU * lo.HU);             // rows [H units | T units][K = HU]
+    add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 1, 0);
+    add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * lo.HU, lo.HU, 1, 0);
+    lo.k_hwT[i] = pk.take(2LL * lo.HU * 2 * lo.HU);            // [HU in][H units | T units]
+    add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, 0);
+    add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, lo.HU);
   }
   // GRU input projections: output columns [fw gates 2RU | fw cand RU | bw gates 2RU | bw cand RU], K = HU (the first HU kernel rows)
   const int XPW = 6 * lo.RU;
-  lo.k_gx = takeb(2LL * XPW * lo.HU);
-  lo.k_gxT = takeb(2LL * lo.HU * XPW);
+  lo.k_gx = pk.take(2LL * XPW * lo.HU);
+  lo.k_gxT = pk.take(2LL * lo.HU * XPW);
   for (int d = 0; d < 2; ++d) {
-    { PJ j; j.src_off = lo.p_gk[d]; j.K = lo.HU; j.N = 2 * lo.RU; j.dst_off = lo.k_gx / 2 + (long long)(d * 3 * lo.RU) * lo.HU; j.dst_ld = lo.HU; j.transpose = 1; j.col0 = 0; jobs.push_back(j); }
-    { PJ j; j.src_off = lo.p_ck[d]; j.K = lo.HU; j.N = lo.RU; j.dst_off = lo.k_gx / 2 + (long long)(d * 3 * lo.RU + 2 * lo.RU) * lo.HU; j.dst_ld = lo.HU; j.transpose = 1; j.col0 = 0; jobs.push_back(j); }
-    pj(lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU);
-    pj(lo.p_ck[d], lo.HU, lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU + 2 * lo.RU);
+    add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * lo.HU, lo.HU, 1, 0);
+    add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * lo.HU, lo.HU, 1, 0);
+    add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU);
+    add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU + 2 * lo.RU);
   }
-  lo.k_lin = takeb(2LL * lo.NFR * 2 * lo.RU); pj(lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 1, 0);
+  lo.k_lin = pk.take(2LL * lo.NFR * 2 * lo.RU); add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 1, 0);
   const int NFK = (lo.NF + 63) / 64 * 64;
-  lo.k_linT = takeb(2LL * 2 * lo.RU * NFK); pj(lo.p_lk, 2 * lo.RU, lo.NF, lo.k_linT, NFK, 0, 0);
-  lo.packed_bytes = o;
+  lo.k_linT = pk.take(2LL * 2 * lo.RU * NFK); add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_linT, NFK, 0, 0);
+  lo.packed_bytes = pk.used;
   lo.n_jobs = int(jobs.size());
 
   // ---- workspace ----
-  o = 0;
+  Arena ws;
   const long long N = lo.N;
-  lo.w_x0 = takeb(N * lo.M * 2);
-  lo.w_Y = takeb(N * lo.KC * 2); lo.w_Xb = takeb(N * lo.KC * 2); lo.w_P = takeb(N * lo.KC * 2); lo.w_stb = takeb(8LL * lo.KC * 4);
-  lo.w_Y1 = takeb(N * lo.PJc * 2); lo.w_X1 = takeb(N * lo.PJc * 2); lo.w_st1 = takeb(8LL * lo.PJc * 4);
-  lo.w_Y2 = takeb(N * lo.M * 4); lo.w_st2 = takeb(8LL * 128 * 4);
-  lo.w_hin = takeb(N * lo.M * 2);
-  for (int i = 0; i <= lo.NH; ++i) { lo.w_hf[i] = takeb(N * lo.HU * 4); lo.w_hb[i] = takeb(N * lo.HU * 2); }
-  for (int i = 0; i < lo.NH; ++i) lo.w_HT[i] = takeb(N * 2 * lo.HU * 2);
-  lo.w_XP = takeb(N * XPW * 4);
-  lo.w_out = takeb(N * 2 * lo.RU * 2);
-  for (int d = 0; d < 2; ++d) { lo.w_gr[d] = takeb(N * lo.RU * 2); lo.w_gu[d] = takeb(N * lo.RU * 2); lo.w_gc[d] = takeb(N * lo.RU * 2); lo.w_grh[d] = takeb(N * lo.RU * 2); }
-  lo.w_lin = takeb(N * lo.NFP * 4);            // fp32 [N][NFP]: padded pitch (the epilogue stores whole float4s)
-  lo.w_scal = takeb(64 * 4);
-  lo.w_tlen = takeb(lo.B * 4);
+  lo.w_x0 = ws.take(N * lo.M * 2);
+  lo.w_Y = ws.take(N * lo.KC * 2); lo.w_Xb = ws.take(N * lo.KC * 2); lo.w_P = ws.take(N * lo.KC * 2); lo.w_stb = ws.take(8LL * lo.KC * 4);
+  lo.w_Y1 = ws.take(N * lo.PJc * 2); lo.w_X1 = ws.take(N * lo.PJc * 2); lo.w_st1 = ws.take(8LL * lo.PJc * 4);
+  lo.w_Y2 = ws.take(N * lo.M * 4); lo.w_st2 = ws.take(8LL * 128 * 4);
+  lo.w_hin = ws.take(N * lo.M * 2);
+  for (int i = 0; i <= lo.NH; ++i) { lo.w_hf[i] = ws.take(N * lo.HU * 4); lo.w_hb[i] = ws.take(N * lo.HU * 2); }
+  for (int i = 0; i < lo.NH; ++i) lo.w_HT[i] = ws.take(N * 2 * lo.HU * 2);
+  lo.w_XP = ws.take(N * XPW * 4);
+  lo.w_out = ws.take(N * 2 * lo.RU * 2);
+  for (int d = 0; d < 2; ++d) { lo.w_gr[d] = ws.take(N * lo.RU * 2); lo.w_gu[d] = ws.take(N * lo.RU * 2); lo.w_gc[d] = ws.take(N * lo.RU * 2); lo.w_grh[d] = ws.take(N * lo.RU * 2); }
+  lo.w_lin = ws.take(N * lo.NFP * 4);            // fp32 [N][NFP]: padded pitch (the epilogue stores whole float4s)
+  lo.w_scal = ws.take(64 * 4);
+  lo.w_tlen = ws.take(lo.B * 4);
   // backward
-  lo.w_dlin = takeb(N * lo.NFP * 2);
-  lo.w_dout = takeb(N * 2 * lo.RU * 4);
-  lo.w_dXP = takeb(N * XPW * 2);
-  lo.w_dh = takeb(N * lo.HU * 4); lo.w_dhb = takeb(N * lo.HU * 2);
-  lo.w_dHT = takeb(N * 2 * lo.HU * 2);
-  lo.w_dhin = takeb(N * lo.M * 4);
-  lo.w_dY2b = takeb(N * 128 * 2);
-  lo.w_d1 = takeb(N * lo.PJc * 2); lo.w_d2 = takeb(N * lo.PJc * 2);
-  lo.w_dP = takeb(N * lo.KC * 2); lo.w_dbank = takeb(N * lo.KC * 2);
-  for (int i = 0; i < 3; ++i) lo.w_dx0[i] = takeb(N * 128 * 4);
-  lo.w_bsum = takeb(2LL * lo.KC * 4);
-  lo.w_tiles = takeb(4096 * sizeof(WgradTile));
-  lo.w_jobs = takeb((long long)jobs.size() * sizeof(PJ));
+  lo.w_dlin = ws.take(N * lo.NFP * 2);
+  lo.w_dout = ws.take(N * 2 * lo.RU * 4);
+  lo.w_dXP = ws.take(N * XPW * 2);
+  lo.w_dh = ws.take(N * lo.HU * 4); lo.w_dhb = ws.take(N * lo.HU * 2);
+  lo.w_dHT = ws.take(N * 2 * lo.HU * 2);
+  lo.w_dhin = ws.take(N * lo.M * 4);
+  lo.w_dY2b = ws.take(N * 128 * 2);
+  lo.w_d1 = ws.take(N * lo.PJc * 2); lo.w_d2 = ws.take(N * lo.PJc * 2);
+  lo.w_dP = ws.take(N * lo.KC * 2); lo.w_dbank = ws.take(N * lo.KC * 2);
+  for (int i = 0; i < 3; ++i) lo.w_dx0[i] = ws.take(N * 128 * 4);
+  lo.w_bsum = ws.take(2LL * lo.KC * 4);
+  lo.w_tiles = ws.take(4096 * sizeof(WgradTile));
+  lo.w_jobs = ws.take((long long)jobs.size() * sizeof(PackJob));
   lo.n_reg = 0;
   for (auto& p : lo.params) lo.n_reg += p.reg ? 1 : 0;
-  lo.w_regtab = takeb((long long)lo.n_reg * 2 * sizeof(long long));
-  lo.workspace_bytes = o;
+  lo.w_regtab = ws.take((long long)lo.n_reg * 2 * sizeof(long long));
+  lo.workspace_bytes = ws.used;
   if (jobs_out) jobs_out->swap(jobs);
   return T2_OK;
 }
@@ -232,21 +211,6 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PJ>* jobs_out) {
 // ------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------
-// fp32 [K][N] (TensorFlow [in][out]) -> bf16; transpose: dst[n][col0 + k] (K-major rows per output), else dst[k][col0 + n]
-__global__ void cpack_kernel(const float* __restrict__ params, bf16* __restrict__ packed, const PJ* __restrict__ jobs) {
-  const PJ j = jobs[blockIdx.y];
-  const long long n_el = (long long)j.K * j.N;
-  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n_el; e += (long long)gridDim.x * blockDim.x) {
-    const int k = int(e / j.N), n = int(e % j.N);
-    const bf16 v = __float2bfloat16(params[j.src_off + e]);
-    if (j.transpose) packed[j.dst_off + (long long)n * j.dst_ld + j.col0 + k] = v;
-    else packed[j.dst_off + (long long)k * j.dst_ld + j.col0 + n] = v;
-  }
-}
-__global__ void f32_to_bf16_k(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < n) out[e] = __float2bfloat16(in[e]);
-}
 __device__ __forceinline__ float ldv(const bf16* p, long long i) { return __bfloat162float(p[i]); }
 __device__ __forceinline__ float ldv(const float* p, long long i) { return p[i]; }
 // Batch-norm kernels work on a COLUMN SLICE [c0, c0 + C) of row-pitch-ld matrices (the conv bank keeps its K layers side by side in
@@ -388,26 +352,26 @@ template <typename TY>
 void bn_fwd_launch(const TY* y, int ld, int c0, bf16* xb, float* xf, const float* add, float* stats, int Ct, const float* gamma, const float* beta,
                    float* mm, float* mv, long long rows, int C, int training, int stat_threads, cudaStream_t st) {
   if (training) { bn_stats_k<TY><<<64, stat_threads, 0, st>>>(y, ld, c0, stats, Ct, rows, C); t2_count_launch(); }
-  bn_apply_k<TY><<<g1(rows * C), 256, 0, st>>>(y, ld, c0, xb, xf, add, stats, Ct, gamma, beta, mm, mv, rows, C, training); t2_count_launch();
+  bn_apply_k<TY><<<grid1d(rows * C), 256, 0, st>>>(y, ld, c0, xb, xf, add, stats, Ct, gamma, beta, mm, mv, rows, C, training); t2_count_launch();
 }
 template <typename T>
 void bn_bwd_launch(const T* g, int ldg, const T* y, int ld, int c0, const float* stats, int Ct, float* bsum, const float* gamma, bf16* dpre, int ldd,
                    float* dgamma, float* dbeta, long long rows, int C, int act, int stat_threads, cudaStream_t st) {
   bn_bwd_stats_k<T, T><<<64, stat_threads, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, rows, C); t2_count_launch();
-  bn_bwd_apply_k<T, T><<<g1(rows * C), 256, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, gamma, dpre, ldd, dgamma, dbeta, rows, C, act);
+  bn_bwd_apply_k<T, T><<<grid1d(rows * C), 256, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, gamma, dpre, ldd, dgamma, dbeta, rows, C, act);
   t2_count_launch();
 }
 void maxpool_fwd(const bf16* x, bf16* out, long long N, int T, int C, cudaStream_t st) {
-  maxpool_fwd_k<<<g1(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
+  maxpool_fwd_k<<<grid1d(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
 }
 void maxpool_bwd(const bf16* x, const bf16* dout, bf16* dx, long long N, int T, int C, cudaStream_t st) {
-  maxpool_bwd_k<<<g1(N * C), 256, 0, st>>>(x, dout, dx, N, T, C); t2_count_launch();
+  maxpool_bwd_k<<<grid1d(N * C), 256, 0, st>>>(x, dout, dx, N, T, C); t2_count_launch();
 }
 void highway_fwd(const float* pre, const float* bh, const float* bt, const float* h, float* hf, bf16* hb, bf16* HT, long long N, int HU, cudaStream_t st) {
-  highway_fwd_k<<<g1(N * HU), 256, 0, st>>>(pre, bh, bt, h, hf, hb, HT, N, HU); t2_count_launch();
+  highway_fwd_k<<<grid1d(N * HU), 256, 0, st>>>(pre, bh, bt, h, hf, hb, HT, N, HU); t2_count_launch();
 }
 void highway_bwd(const float* dh, const bf16* HT, const float* h, bf16* dHT, float* dcarry, long long N, int HU, cudaStream_t st) {
-  highway_bwd_k<<<g1(N * HU), 256, 0, st>>>(dh, HT, h, dHT, dcarry, N, HU); t2_count_launch();
+  highway_bwd_k<<<grid1d(N * HU), 256, 0, st>>>(dh, HT, h, dHT, dcarry, N, HU); t2_count_launch();
 }
 // out fp32 += a (fp32) ; optional bf16 copy
 __global__ void add_k(float* __restrict__ acc, const float* __restrict__ a, bf16* __restrict__ outb, long long n) {
@@ -448,17 +412,6 @@ __global__ void lin_finish_k(float* __restrict__ lin, const float* __restrict__ 
   }
   l_all = warp_sum(l_all); l_low = warp_sum(l_low);
   if ((threadIdx.x & 31) == 0 && tgt) { atomicAdd(scal + 0, l_all); atomicAdd(scal + 1, l_low); }
-}
-__global__ void reg_loss_k(const float* __restrict__ params, const long long* __restrict__ tab, int n, float* __restrict__ scal) {
-  const long long off = tab[2 * blockIdx.y], cnt = tab[2 * blockIdx.y + 1];
-  float s = 0.f;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) { const float v = params[off + i]; s += v * v; }
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) atomicAdd(scal + 2, 0.5f * s);
-}
-__global__ void reg_grad_k(const float* __restrict__ params, float* __restrict__ grads, const long long* __restrict__ tab, float w) {
-  const long long off = tab[2 * blockIdx.y], cnt = tab[2 * blockIdx.y + 1];
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < cnt; i += (long long)gridDim.x * blockDim.x) grads[off + i] += w * params[off + i];
 }
 // normalisers of the two L1 means: plain = (N NF, N n_prio); masked (MaskedLinearLoss) = sum(mask) for BOTH terms
 __global__ void lin_norm_k(float* __restrict__ scal, const int* __restrict__ tlen, int B, int T, int NF, int n_prio) {
@@ -701,42 +654,36 @@ int gemm(const void* a, int C, int ld, int k0, long long T, int Bn, const void* 
   return launch_act_gemm(EPI_BIAS_ACT, BN, g, st);
 }
 
-void wg_tile(std::vector<WgradTile>& v, int am, int ach, int ash, int bm, int bch, long long off, int ldc, int mv, int nv) {
-  WgradTile t; memset(&t, 0, sizeof(t));
-  t.a_map = am; t.a_ch0 = ach; t.a_shift = ash; t.b_map = bm; t.b_ch0 = bch; t.out_off = off; t.ldc = ldc;
-  t.m_valid = mv; t.n_valid = nv; t.scale = 1.f; t.accumulate = 0; t.div = nullptr;
-  v.push_back(t);
-}
-void wg_dense(std::vector<WgradTile>& v, int am, int a0, int Ca, int bm, int b0, int Cb, long long off, int ldc, int shift = 0) {
-  for (int m0 = 0; m0 < Ca; m0 += 128)
-    for (int n0 = 0; n0 < Cb; n0 += 256)
-      wg_tile(v, am, a0 + m0, shift, bm, b0 + n0, off + (long long)m0 * ldc + n0, ldc, Ca - m0 < 128 ? Ca - m0 : 128, Cb - n0 < 256 ? Cb - n0 : 256);
-}
 inline int conv_shift(int k, int j) { return j - (k - 1) / 2; }
 // wgrad launches, in the order t2_cbhg_backward issues them
 enum { WG_LIN = 0, WG_GRU = 1, WG_HW0 = 2 /* NH launches, last highway layer first */ };
 void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
   L.clear();
+  auto dense = [](int am, int bm, int shift = 0) {   // a plain weight gradient: maps, A time shift, scale 1
+    WgradTile t; memset(&t, 0, sizeof(t));
+    t.a_map = am; t.a_shift = shift; t.b_map = bm; t.scale = 1.f;
+    return t;
+  };
   const int RU = lo.RU, HU = lo.HU;
-  { std::vector<WgradTile> w; wg_dense(w, 0, 0, 2 * RU, 1, 0, lo.NF, lo.p_lk, lo.NF); L.push_back(w); }      // maps: 0 rnn out, 1 dlin
+  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense(0, 1), 0, 2 * RU, 0, lo.NF, lo.p_lk, lo.NF); L.push_back(w); }      // maps: 0 rnn out, 1 dlin
   { std::vector<WgradTile> w;     // maps: 0 h_last (bf16 [N][HU]), 1 dXP, 2 rnn out, 3 rh fw, 4 rh bw
     for (int d = 0; d < 2; ++d) {
-      wg_dense(w, 0, 0, HU, 1, d * 3 * RU, 2 * RU, lo.p_gk[d], 2 * RU);                                       // input rows of the gates kernel
-      wg_dense(w, 0, 0, HU, 1, d * 3 * RU + 2 * RU, RU, lo.p_ck[d], RU);                                      // input rows of the candidate kernel
-      wg_dense(w, 2, d * RU, RU, 1, d * 3 * RU, 2 * RU, lo.p_gk[d] + (long long)HU * 2 * RU, 2 * RU, d == 0 ? -1 : 1);   // h_prev x d gates
-      wg_dense(w, 3 + d, 0, RU, 1, d * 3 * RU + 2 * RU, RU, lo.p_ck[d] + (long long)HU * RU, RU);             // (r h_prev) x d cand
+      append_wgrad_tiles(w, dense(0, 1), 0, HU, d * 3 * RU, 2 * RU, lo.p_gk[d], 2 * RU);                                       // input rows of the gates kernel
+      append_wgrad_tiles(w, dense(0, 1), 0, HU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d], RU);                                      // input rows of the candidate kernel
+      append_wgrad_tiles(w, dense(2, 1, d == 0 ? -1 : 1), d * RU, RU, d * 3 * RU, 2 * RU, lo.p_gk[d] + (long long)HU * 2 * RU, 2 * RU);   // h_prev x d gates
+      append_wgrad_tiles(w, dense(3 + d, 1), 0, RU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d] + (long long)HU * RU, RU);             // (r h_prev) x d cand
     }
     L.push_back(w); }
   for (int i = lo.NH - 1; i >= 0; --i) {   // maps: 0 h_i (bf16), 1 dHT
     std::vector<WgradTile> w;
-    wg_dense(w, 0, 0, HU, 1, 0, HU, lo.p_hk[i][0], HU);
-    wg_dense(w, 0, 0, HU, 1, HU, HU, lo.p_hk[i][1], HU);
+    append_wgrad_tiles(w, dense(0, 1), 0, HU, 0, HU, lo.p_hk[i][0], HU);
+    append_wgrad_tiles(w, dense(0, 1), 0, HU, HU, HU, lo.p_hk[i][1], HU);
     L.push_back(w);
   }
-  { std::vector<WgradTile> w; wg_dense(w, 0, 0, lo.M, 1, 0, HU, lo.p_dk, HU); L.push_back(w); }               // dense: hin x dh0
+  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense(0, 1), 0, lo.M, 0, HU, lo.p_dk, HU); L.push_back(w); }               // dense: hin x dh0
   auto conv = [&](const CConv& c, int a_ch0, int b_ch0) {
     std::vector<WgradTile> w;
-    for (int j = 0; j < c.k; ++j) wg_dense(w, 0, a_ch0, c.cin, 1, b_ch0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout, conv_shift(c.k, j));
+    for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w, dense(0, 1, conv_shift(c.k, j)), a_ch0, c.cin, b_ch0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
     L.push_back(w);
   };
   conv(lo.proj2, 0, 0);     // maps: 0 X1, 1 dY2b
@@ -744,7 +691,7 @@ void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
   { std::vector<WgradTile> w;  // bank: maps 0 x0, 1 dbank (channel block k-1)
     for (int k = 1; k <= lo.K; ++k) {
       const CConv& c = lo.bank[k - 1];
-      for (int j = 0; j < c.k; ++j) wg_dense(w, 0, 0, c.cin, 1, (k - 1) * lo.CC, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout, conv_shift(c.k, j));
+      for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w, dense(0, 1, conv_shift(c.k, j)), 0, c.cin, (k - 1) * lo.CC, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
     }
     L.push_back(w); }
 }
@@ -772,19 +719,12 @@ extern "C" int t2_cbhg_param_info(const t2_cbhg_config_t* cfg, int i, char* name
   CL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
-  T2_REQUIRE(i >= 0 && i < int(lo.params.size()) && name && cap > 0, T2_ERR_INVALID_ARG, "cbhg_param_info: bad index");
-  const CPT& p = lo.params[i];
-  snprintf(name, cap, "%s", p.name.c_str());
-  if (offset) *offset = p.off;
-  if (ndim) *ndim = p.ndim;
-  if (shape4) for (int k = 0; k < 4; ++k) shape4[k] = p.shape[k];
-  if (trainable) *trainable = p.trainable ? 1 : 0;
-  return T2_OK;
+  return param_info(lo.params, i, name, cap, offset, ndim, shape4, trainable);
 }
 
 extern "C" int t2_cbhg_init(const t2_cbhg_config_t* cfg, void* d_packed, void* d_workspace, void* stream) {
   CL lo;
-  std::vector<PJ> jobs;
+  std::vector<PackJob> jobs;
   int rc = build(cfg, lo, &jobs);
   if (rc) return rc;
   T2_REQUIRE(d_packed && d_workspace, T2_ERR_INVALID_ARG, "cbhg_init: null buffers");
@@ -792,17 +732,15 @@ extern "C" int t2_cbhg_init(const t2_cbhg_config_t* cfg, void* d_packed, void* d
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   T2_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, lo.packed_bytes, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d_workspace, 0, lo.workspace_bytes, st));
-  T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_jobs, jobs.data(), jobs.size() * sizeof(PJ), cudaMemcpyHostToDevice, st));
+  T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_jobs, jobs.data(), jobs.size() * sizeof(PackJob), cudaMemcpyHostToDevice, st));
   std::vector<std::vector<WgradTile>> wl;
   build_tiles(lo, wl);
   std::vector<WgradTile> all;
   for (auto& w : wl) all.insert(all.end(), w.begin(), w.end());
   T2_REQUIRE(all.size() <= 4096, T2_ERR_UNSUPPORTED_SHAPE, "cbhg: too many wgrad tiles (%d)", int(all.size()));
   T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_tiles, all.data(), all.size() * sizeof(WgradTile), cudaMemcpyHostToDevice, st));
-  std::vector<long long> tab;
-  for (auto& p : lo.params)
-    if (p.reg) { long long n = 1; for (int k = 0; k < p.ndim; ++k) n *= p.shape[k]; tab.push_back(p.off); tab.push_back(n); }
-  if (!tab.empty()) T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_regtab, tab.data(), tab.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  rc = upload_reg_table(lo.params, ws + lo.w_regtab, st);
+  if (rc) return rc;
   T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem())));
   T2_CHECK_CUDA(cudaFuncSetAttribute(gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_bwd_smem())));
   T2_CHECK_CUDA(cudaStreamSynchronize(st));
@@ -813,12 +751,8 @@ extern "C" int t2_cbhg_pack_weights(const t2_cbhg_config_t* cfg, const float* d_
   CL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cpack_kernel<<<dim3(32, lo.n_jobs), 256, 0, st>>>(d_params, static_cast<bf16*>(d_packed),
-                                                    reinterpret_cast<const PJ*>(static_cast<uint8_t*>(d_workspace) + lo.w_jobs));
-  t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
+  return launch_pack(d_params, d_packed, reinterpret_cast<const PackJob*>(static_cast<uint8_t*>(d_workspace) + lo.w_jobs), lo.n_jobs, 32, 32,
+                     static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int t2_cbhg_set_target_lengths(const t2_cbhg_config_t* cfg, void* d_workspace, const int* d_target_lengths, void* stream) {
@@ -858,7 +792,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   float* scal = W<float>(s, lo.w_scal);
   T2_CHECK_CUDA(cudaMemsetAsync(scal, 0, 16 * sizeof(float), st));
   bf16* x0 = W<bf16>(s, lo.w_x0);
-  f32_to_bf16_k<<<g1(N * M), 256, 0, st>>>(d_mel, x0, N * M); t2_count_launch();
+  launch_f32_to_bf16(d_mel, x0, N * M, st);
   // ---- conv bank (each layer writes its 128-column slice) + per-layer batch norm ----
   bf16* Y = W<bf16>(s, lo.w_Y);
   bf16* Xb = W<bf16>(s, lo.w_Xb);
@@ -890,7 +824,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   bf16* hin = W<bf16>(s, lo.w_hin);
   bn_fwd_launch<float>(Y2, M, 0, nullptr, hin_f, d_mel, st2, M, d_params + lo.proj2.p_g, d_params + lo.proj2.p_be, d_params + lo.proj2.p_mm,
                        d_params + lo.proj2.p_mv, N, M, training, 128, st);
-  f32_to_bf16_k<<<g1(N * M), 256, 0, st>>>(hin_f, hin, N * M); t2_count_launch();
+  launch_f32_to_bf16(hin_f, hin, N * M, st);
   // ---- dense to the highway width, highway layers ----
   rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]), HU, HU, st);
   if (rc) return rc;
@@ -925,10 +859,10 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   const int* tlen = lo.c.mask_decoder ? W<int>(s, lo.w_tlen) : nullptr;
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
   lin_norm_k<<<1, 1, 0, st>>>(scal, tlen, B, T, lo.NF, lo.c.n_priority_freq); t2_count_launch();
-  lin_finish_k<<<g1(N * lo.NFP), 256, 0, st>>>(lin, d_linear_targets, (training && d_linear_targets) ? W<bf16>(s, lo.w_dlin) : nullptr, scal, N, T, lo.NF,
+  lin_finish_k<<<grid1d(N * lo.NFP), 256, 0, st>>>(lin, d_linear_targets, (training && d_linear_targets) ? W<bf16>(s, lo.w_dlin) : nullptr, scal, N, T, lo.NF,
                                                lo.NFP, lo.c.n_priority_freq, lo.c.clip_outputs, lo_c, hi_c, tlen); t2_count_launch();
   if (d_loss) {
-    if (lo.n_reg > 0) { reg_loss_k<<<dim3(8, lo.n_reg), 256, 0, st>>>(d_params, W<long long>(s, lo.w_regtab), lo.n_reg, scal); t2_count_launch(); }
+    launch_reg_loss(d_params, W<long long>(s, lo.w_regtab), lo.n_reg, scal + 2, st);
     loss_out_k<<<1, 1, 0, st>>>(scal, d_loss, lo.c.reg_weight); t2_count_launch();
   }
   T2_CHECK_CUDA(cudaGetLastError());
@@ -999,7 +933,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     highway_bwd(dh, W<bf16>(s, lo.w_HT[i]), W<float>(s, lo.w_hf[i]), dHT, dcar, N, HU, st);
     rc = gemm(dHT, 2 * HU, 2 * HU, 0, T, B, s.pk + lo.k_hwT[i], HU, 2 * HU, 1, nullptr, 128, nullptr, 0, nullptr, dh, HU, HU, st);
     if (rc) return rc;
-    add_k<<<g1(N * HU), 256, 0, st>>>(dh, dcar, i == 0 ? W<bf16>(s, lo.w_dhb) : nullptr, N * HU); t2_count_launch();
+    add_k<<<grid1d(N * HU), 256, 0, st>>>(dh, dcar, i == 0 ? W<bf16>(s, lo.w_dhb) : nullptr, N * HU); t2_count_launch();
     { ActT maps[2] = {make_act(W<bf16>(s, lo.w_hb[i]), HU, T, B), make_act(dHT, 2 * HU, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
     colsum_k<bf16><<<64, 128, 0, st>>>(dHT, N, HU, 2 * HU, d_grads + lo.p_hb[i][0]); t2_count_launch();
     colsum_k<bf16><<<64, 128, 0, st>>>(dHT + HU, N, HU, 2 * HU, d_grads + lo.p_hb[i][1]); t2_count_launch();
@@ -1056,10 +990,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     rc = gemm(dpre, lo.CC, KC, 0, T, B, s.pk + lo.k_bankT[g], 128, n * lo.CC, n, shifts, 128, nullptr, 0, nullptr, dx, 128, M, st, k0s, KC);
     if (rc) return rc;
   }
-  dmel_k<<<g1(N * M), 256, 0, st>>>(W<float>(s, lo.w_dx0[0]), W<float>(s, lo.w_dx0[1]), W<float>(s, lo.w_dx0[2]), dhin, d_mel_grad, N, M); t2_count_launch();
-  if (lo.n_reg > 0 && lo.c.reg_weight != 0.f) {
-    reg_grad_k<<<dim3(8, lo.n_reg), 256, 0, st>>>(d_params, d_grads, W<long long>(s, lo.w_regtab), lo.c.reg_weight); t2_count_launch();
-  }
+  dmel_k<<<grid1d(N * M), 256, 0, st>>>(W<float>(s, lo.w_dx0[0]), W<float>(s, lo.w_dx0[1]), W<float>(s, lo.w_dx0[2]), dhin, d_mel_grad, N, M); t2_count_launch();
+  if (lo.c.reg_weight != 0.f) launch_reg_grad(d_params, d_grads, W<long long>(s, lo.w_regtab), lo.n_reg, lo.c.reg_weight, st);
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }

@@ -258,4 +258,20 @@ int launch_wgrad(const ActT* maps, int nmaps, const WgradTile* tiles_dev, int nt
   return T2_OK;
 }
 
+void append_wgrad_tiles(std::vector<WgradTile>& v, const WgradTile& proto, int a_ch0, int Ca, int b_ch0, int Cb, long long out_off,
+                        int ldc) {
+  for (int m0 = 0; m0 < Ca; m0 += kWgBM)
+    for (int n0 = 0; n0 < Cb; n0 += kWgBN) {
+      WgradTile t;
+      memset(&t, 0, sizeof(t));
+      t.a_map = proto.a_map; t.a_ch0 = a_ch0 + m0; t.a_shift = proto.a_shift; t.a_layer = proto.a_layer;
+      t.b_map = proto.b_map; t.b_ch0 = b_ch0 + n0; t.b_shift = proto.b_shift; t.b_layer = proto.b_layer;
+      t.out_off = out_off + (long long)m0 * ldc + n0; t.ldc = ldc;
+      t.m_valid = Ca - m0 < kWgBM ? Ca - m0 : kWgBM;
+      t.n_valid = Cb - n0 < kWgBN ? Cb - n0 : kWgBN;
+      t.scale = proto.scale; t.accumulate = proto.accumulate; t.div = proto.div;
+      v.push_back(t);
+    }
+}
+
 }  // namespace t2

@@ -1153,6 +1153,7 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
 //   Warps 0..7 = two consumer warpgroups (warpgroup w: output rows [64 w, +64), i.e. A channel block w, all N columns),
 //   warp 8 = TMA producer. The accumulators go from registers straight to the fp32 output.
 // ------------------------------------------------------------------------------------------------
+constexpr int kWgBM = 128;      // output rows per tile: one 64-row block per consumer warpgroup
 constexpr int kWgBN = 256;      // up to 256 output columns per tile: the A block pair is reused for twice the MMA work
 constexpr int kWgStages = 4;
 constexpr int kWgStageBytes = 6 * (kBK * 128);  // A: 2 blocks of [64 pos x 128 B] (16 KB), B: up to 4 blocks (32 KB)

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <string.h>
 
+#include <vector>
+
 #include "t2_gemm_types.h"
 
 namespace t2 {
@@ -51,5 +53,9 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used = nullptr);
 int launch_wgrad(const ActT* maps, int nmaps, const WgradTile* tiles_dev, int ntiles, float* out,
                  int T, int B, cudaStream_t stream);
+// appends the tiles of the dense [Ca x Cb] weight gradient out[out_off + m * ldc + n] of A channels [a_ch0, a_ch0 + Ca) and B channels
+// [b_ch0, b_ch0 + Cb), row blocks outer; proto gives the maps, shifts, layers, scale, accumulate and div of every tile
+void append_wgrad_tiles(std::vector<WgradTile>& v, const WgradTile& proto, int a_ch0, int Ca, int b_ch0, int Cb, long long out_off,
+                        int ldc);
 
 }  // namespace t2

@@ -24,15 +24,12 @@
 #include "../../include/t2b200.h"
 #include "t2_common.cuh"
 #include "t2_gemm.h"
+#include "t2_params.h"
 
 namespace t2 {
 namespace {
 
 typedef __nv_bfloat16 bf16;
-inline long long al256(long long v) { return (v + 255) / 256 * 256; }
-inline dim3 g1(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
-
-struct PT { std::string name; long long off; int ndim; int shape[4]; bool trainable, reg; };
 
 struct ConvL {   // one conv + BN block
   int cin, cout, k, act;   // act: 1 relu, 2 tanh, 0 none
@@ -47,7 +44,7 @@ struct ConvL {   // one conv + BN block
 struct TL {  // layout
   t2_taco_config_t c;
   int B, Ti, To, E, C, H, D, A, F, KA, P1, P2, M, PC, NS;
-  std::vector<PT> params;
+  std::vector<Param> params;
   long long n_params;
   long long p_emb, p_elk[2], p_elb[2], p_mem, p_qry, p_lck, p_lcb, p_lfl, p_v, p_ba, p_p1k, p_p1b, p_p2k, p_p2b;
   long long p_l1k, p_l1b, p_l2k, p_l2b, p_fk, p_fb, p_sk, p_sb, p_ppk, p_ppb;
@@ -70,22 +67,7 @@ struct TL {  // layout
   int n_packjobs, n_reg;
 };
 
-struct PJ { long long src_off; int K, N; long long dst_off; int dst_ld, transpose, col0; float scale; int perm_h; int part; };   // part 2: bf16(w - bf16(w))
-
-long long addp(TL& lo, const std::string& name, std::initializer_list<int> shape, bool trainable = true) {
-  PT p; p.name = name; p.off = lo.n_params; p.ndim = int(shape.size());
-  long long n = 1; int i = 0;
-  for (int s : shape) { p.shape[i++] = s; n *= s; }
-  for (; i < 4; ++i) p.shape[i] = 1;
-  p.trainable = trainable;
-  p.reg = trainable && name.find("bias") == std::string::npos && name.find("_projection") == std::string::npos &&
-          name.find("inputs_embedding") == std::string::npos && name.find("LSTM") == std::string::npos;
-  lo.n_params += (n + 3) / 4 * 4;
-  lo.params.push_back(p);
-  return p.off;
-}
-
-int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
+int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   T2_REQUIRE(cfg != nullptr, T2_ERR_INVALID_ARG, "null config");
   lo.c = *cfg;
   lo.B = cfg->B; lo.Ti = cfg->T_in; lo.To = cfg->T_out; lo.E = cfg->embedding_dim; lo.C = cfg->enc_conv_channels;
@@ -108,11 +90,11 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
              cfg->noncumulative_weights);
   // ---- parameters (order == oracle/tacotron.py:param_shapes) ----
   lo.n_params = 0; lo.params.clear(); lo.enc.clear(); lo.post.clear();
-  lo.p_emb = addp(lo, "inputs_embedding", {lo.NS, lo.E});
+  lo.p_emb = add_param(lo.params, lo.n_params, "inputs_embedding", {lo.NS, lo.E});
   auto conv_params = [&](ConvL& L, const std::string& pre) {
-    L.p_k = addp(lo, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = addp(lo, pre + "bias", {L.cout});
-    L.p_gamma = addp(lo, pre + "gamma", {L.cout}); L.p_beta = addp(lo, pre + "beta", {L.cout});
-    L.p_mm = addp(lo, pre + "moving_mean", {L.cout}, false); L.p_mv = addp(lo, pre + "moving_variance", {L.cout}, false);
+    L.p_k = add_param(lo.params, lo.n_params, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = add_param(lo.params, lo.n_params, pre + "bias", {L.cout});
+    L.p_gamma = add_param(lo.params, lo.n_params, pre + "gamma", {L.cout}); L.p_beta = add_param(lo.params, lo.n_params, pre + "beta", {L.cout});
+    L.p_mm = add_param(lo.params, lo.n_params, pre + "moving_mean", {L.cout}, false); L.p_mv = add_param(lo.params, lo.n_params, pre + "moving_variance", {L.cout}, false);
   };
   int cin = lo.E;
   for (int i = 0; i < cfg->enc_conv_layers; ++i) {
@@ -122,176 +104,163 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
   }
   const char* dn[2] = {"fw", "bw"};
   for (int d = 0; d < 2; ++d) {
-    lo.p_elk[d] = addp(lo, std::string("encoder_LSTM/") + dn[d] + "/kernel", {lo.C + lo.H, 4 * lo.H});
-    lo.p_elb[d] = addp(lo, std::string("encoder_LSTM/") + dn[d] + "/bias", {4 * lo.H});
+    lo.p_elk[d] = add_param(lo.params, lo.n_params, std::string("encoder_LSTM/") + dn[d] + "/kernel", {lo.C + lo.H, 4 * lo.H});
+    lo.p_elb[d] = add_param(lo.params, lo.n_params, std::string("encoder_LSTM/") + dn[d] + "/bias", {4 * lo.H});
   }
-  lo.p_mem = addp(lo, "attention/memory_layer/kernel", {2 * lo.H, lo.A});
-  lo.p_qry = addp(lo, "attention/query_layer/kernel", {lo.D, lo.A});
-  lo.p_lck = addp(lo, "attention/location_features_convolution/kernel", {lo.KA, 1, lo.F});
-  lo.p_lcb = addp(lo, "attention/location_features_convolution/bias", {lo.F});
-  lo.p_lfl = addp(lo, "attention/location_features_layer/kernel", {lo.F, lo.A});
-  lo.p_v = addp(lo, "attention/attention_variable_projection", {lo.A});
-  lo.p_ba = addp(lo, "attention/attention_bias", {lo.A});
-  lo.p_p1k = addp(lo, "decoder_prenet/dense_1/kernel", {lo.M, lo.P1}); lo.p_p1b = addp(lo, "decoder_prenet/dense_1/bias", {lo.P1});
-  lo.p_p2k = addp(lo, "decoder_prenet/dense_2/kernel", {lo.P1, lo.P2}); lo.p_p2b = addp(lo, "decoder_prenet/dense_2/bias", {lo.P2});
+  lo.p_mem = add_param(lo.params, lo.n_params, "attention/memory_layer/kernel", {2 * lo.H, lo.A});
+  lo.p_qry = add_param(lo.params, lo.n_params, "attention/query_layer/kernel", {lo.D, lo.A});
+  lo.p_lck = add_param(lo.params, lo.n_params, "attention/location_features_convolution/kernel", {lo.KA, 1, lo.F});
+  lo.p_lcb = add_param(lo.params, lo.n_params, "attention/location_features_convolution/bias", {lo.F});
+  lo.p_lfl = add_param(lo.params, lo.n_params, "attention/location_features_layer/kernel", {lo.F, lo.A});
+  lo.p_v = add_param(lo.params, lo.n_params, "attention/attention_variable_projection", {lo.A});
+  lo.p_ba = add_param(lo.params, lo.n_params, "attention/attention_bias", {lo.A});
+  lo.p_p1k = add_param(lo.params, lo.n_params, "decoder_prenet/dense_1/kernel", {lo.M, lo.P1}); lo.p_p1b = add_param(lo.params, lo.n_params, "decoder_prenet/dense_1/bias", {lo.P1});
+  lo.p_p2k = add_param(lo.params, lo.n_params, "decoder_prenet/dense_2/kernel", {lo.P1, lo.P2}); lo.p_p2b = add_param(lo.params, lo.n_params, "decoder_prenet/dense_2/bias", {lo.P2});
   const int K1 = lo.P2 + 2 * lo.H + lo.D, K2 = 2 * lo.D;
-  lo.p_l1k = addp(lo, "decoder_LSTM/cell_1/kernel", {K1, 4 * lo.D}); lo.p_l1b = addp(lo, "decoder_LSTM/cell_1/bias", {4 * lo.D});
-  lo.p_l2k = addp(lo, "decoder_LSTM/cell_2/kernel", {K2, 4 * lo.D}); lo.p_l2b = addp(lo, "decoder_LSTM/cell_2/bias", {4 * lo.D});
+  lo.p_l1k = add_param(lo.params, lo.n_params, "decoder_LSTM/cell_1/kernel", {K1, 4 * lo.D}); lo.p_l1b = add_param(lo.params, lo.n_params, "decoder_LSTM/cell_1/bias", {4 * lo.D});
+  lo.p_l2k = add_param(lo.params, lo.n_params, "decoder_LSTM/cell_2/kernel", {K2, 4 * lo.D}); lo.p_l2b = add_param(lo.params, lo.n_params, "decoder_LSTM/cell_2/bias", {4 * lo.D});
   const int PIK = lo.D + 2 * lo.H;
-  lo.p_fk = addp(lo, "linear_transform_projection/kernel", {PIK, lo.M}); lo.p_fb = addp(lo, "linear_transform_projection/bias", {lo.M});
-  lo.p_sk = addp(lo, "stop_token_projection/kernel", {PIK, 1}); lo.p_sb = addp(lo, "stop_token_projection/bias", {1});
+  lo.p_fk = add_param(lo.params, lo.n_params, "linear_transform_projection/kernel", {PIK, lo.M}); lo.p_fb = add_param(lo.params, lo.n_params, "linear_transform_projection/bias", {lo.M});
+  lo.p_sk = add_param(lo.params, lo.n_params, "stop_token_projection/kernel", {PIK, 1}); lo.p_sb = add_param(lo.params, lo.n_params, "stop_token_projection/bias", {1});
   cin = lo.M;
   for (int i = 0; i < cfg->postnet_layers; ++i) {
     ConvL L; L.cin = cin; L.cout = lo.PC; L.k = cfg->postnet_kernel; L.act = (i + 1 < cfg->postnet_layers) ? 2 : 0; L.stream = 30 + i;
     char b[64]; snprintf(b, sizeof(b), "postnet_convolutions/conv_layer_%d/", i + 1);
     conv_params(L, b); lo.post.push_back(L); cin = lo.PC;
   }
-  lo.p_ppk = addp(lo, "postnet_projection/kernel", {lo.PC, lo.M}); lo.p_ppb = addp(lo, "postnet_projection/bias", {lo.M});
+  lo.p_ppk = add_param(lo.params, lo.n_params, "postnet_projection/kernel", {lo.PC, lo.M}); lo.p_ppb = add_param(lo.params, lo.n_params, "postnet_projection/bias", {lo.M});
 
   // ---- packed operands + pack jobs ----
-  std::vector<PJ> jobs;
-  long long o = 0;
-  auto takeb = [&](long long bytes) { long long r = o; o = al256(o + bytes); return r; };
-  auto pj = [&](long long src, int K, int N, long long dst_bytes, int ld, int tr, int col0, int perm = 0) {
-    PJ j; j.src_off = src; j.K = K; j.N = N; j.dst_off = dst_bytes / 2; j.dst_ld = ld; j.transpose = tr; j.col0 = col0; j.scale = 1.f;
-    j.perm_h = perm; j.part = 0; jobs.push_back(j);
-  };
+  std::vector<PackJob> jobs;
+  Arena pk;
   const bool split = cfg->split_bf16 != 0;
-  // split-bf16 operand: the K slot [col, col + slot) of the plain layout becomes [W_hi | W_hi | W_lo]
-  auto pj3 = [&](long long src, int K, int N, long long dst_bytes, int ld, int col, int slot) {
-    pj(src, K, N, dst_bytes, ld, 1, col);
-    pj(src, K, N, dst_bytes, ld, 1, col + slot);
-    pj(src, K, N, dst_bytes, ld, 1, col + 2 * slot);
-    jobs.back().part = 2;
-  };
   auto conv_pack = [&](ConvL& L) {
     L.cinp = (L.cin + 63) / 64 * 64;
-    L.k_w = takeb(2LL * L.cout * L.k * L.cinp * (split ? 3 : 1));
-    L.k_wT = takeb(2LL * L.cinp * L.k * L.cout);
+    L.k_w = pk.take(2LL * L.cout * L.k * L.cinp * (split ? 3 : 1));
+    L.k_wT = pk.take(2LL * L.cinp * L.k * L.cout);
     for (int j = 0; j < L.k; ++j) {
-      if (split) pj3(L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp, L.cinp);
+      if (split) add_pack_split(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp, 3 * j * L.cinp + 2 * L.cinp, L.cinp);
       else
-      pj(L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd: [cout][tap j | cin]
-      pj(L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.cout, 0, j * L.cout);     // dgrad: [cin][tap j | cout]
+      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd: [cout][tap j | cin]
+      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.cout, 0, j * L.cout);     // dgrad: [cin][tap j | cout]
     }
   };
   for (auto& L : lo.enc) conv_pack(L);
   for (auto& L : lo.post) conv_pack(L);
   for (int d = 0; d < 2; ++d) {
-    lo.k_encWx[d] = takeb(2LL * 4 * lo.H * lo.C * (split ? 3 : 1));            // [4H][C]  input projection (natural gate order)
-    if (split) pj3(lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], 3 * lo.C, 0, lo.C);
-    else pj(lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], lo.C, 1, 0);
-    lo.k_encWr[d] = takeb(2LL * 4 * lo.H * lo.H);            // [4H perm][H] recurrent, rows permuted for EPI_LSTM
-    pj(lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 1, 0, lo.H);
-    lo.k_encWrT[d] = takeb(2LL * lo.H * 4 * lo.H);           // [H][4H] for the backward step
-    pj(lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWrT[d], 4 * lo.H, 0, 0);
+    lo.k_encWx[d] = pk.take(2LL * 4 * lo.H * lo.C * (split ? 3 : 1));            // [4H][C]  input projection (natural gate order)
+    if (split) add_pack_split(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], 3 * lo.C, 0, 2 * lo.C, lo.C);
+    else add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], lo.C, 1, 0);
+    lo.k_encWr[d] = pk.take(2LL * 4 * lo.H * lo.H);            // [4H perm][H] recurrent, rows permuted for EPI_LSTM
+    add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 1, 0, 1.f, lo.H);
+    lo.k_encWrT[d] = pk.take(2LL * lo.H * 4 * lo.H);           // [H][4H] for the backward step
+    add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWrT[d], 4 * lo.H, 0, 0);
   }
-  lo.k_encWxT = takeb(2LL * lo.C * 8 * lo.H);                // [C][fw 4H | bw 4H]
-  for (int d = 0; d < 2; ++d) pj(lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWxT, 8 * lo.H, 0, d * 4 * lo.H);
-  lo.k_mem = takeb(2LL * lo.A * 2 * lo.H); pj(lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 1, 0);
-  lo.k_memT = takeb(2LL * 2 * lo.H * lo.A); pj(lo.p_mem, 2 * lo.H, lo.A, lo.k_memT, lo.A, 0, 0);
+  lo.k_encWxT = pk.take(2LL * lo.C * 8 * lo.H);                // [C][fw 4H | bw 4H]
+  for (int d = 0; d < 2; ++d) add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWxT, 8 * lo.H, 0, d * 4 * lo.H);
+  lo.k_mem = pk.take(2LL * lo.A * 2 * lo.H); add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 1, 0);
+  lo.k_memT = pk.take(2LL * 2 * lo.H * lo.A); add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_memT, lo.A, 0, 0);
   const int Mp = 128;  // mel channels padded for TMA boxes
-  lo.k_p1 = takeb(2LL * lo.P1 * Mp); pj(lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mp, 1, 0);
-  lo.k_p1T = takeb(2LL * lo.M * lo.P1); pj(lo.p_p1k, lo.M, lo.P1, lo.k_p1T, lo.P1, 0, 0);
-  lo.k_p2 = takeb(2LL * lo.P2 * lo.P1); pj(lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 1, 0);
-  lo.k_p2T = takeb(2LL * lo.P1 * lo.P2); pj(lo.p_p2k, lo.P1, lo.P2, lo.k_p2T, lo.P2, 0, 0);
-  lo.k_l1x = takeb(2LL * 4 * lo.D * lo.P2); pj(lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 1, 0);
-  lo.k_l1xT = takeb(2LL * lo.P2 * 4 * lo.D); pj(lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1xT, 4 * lo.D, 0, 0);
+  lo.k_p1 = pk.take(2LL * lo.P1 * Mp); add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mp, 1, 0);
+  lo.k_p1T = pk.take(2LL * lo.M * lo.P1); add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1T, lo.P1, 0, 0);
+  lo.k_p2 = pk.take(2LL * lo.P2 * lo.P1); add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 1, 0);
+  lo.k_p2T = pk.take(2LL * lo.P1 * lo.P2); add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2T, lo.P2, 0, 0);
+  lo.k_l1x = pk.take(2LL * 4 * lo.D * lo.P2); add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 1, 0);
+  lo.k_l1xT = pk.take(2LL * lo.P2 * 4 * lo.D); add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1xT, 4 * lo.D, 0, 0);
   const int K1r = 2 * lo.H + lo.D;
-  lo.k_l1r = takeb(2LL * 4 * lo.D * K1r); pj(lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 1, 0, lo.D);
-  lo.k_l1rT = takeb(2LL * K1r * 4 * lo.D); pj(lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1rT, 4 * lo.D, 0, 0);
-  lo.k_l2 = takeb(2LL * 4 * lo.D * K2); pj(lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 1, 0, lo.D);
-  lo.k_l2T = takeb(2LL * K2 * 4 * lo.D); pj(lo.p_l2k, K2, 4 * lo.D, lo.k_l2T, 4 * lo.D, 0, 0);
-  lo.k_proj = takeb(2LL * 128 * PIK);                         // rows 0..M-1 frame projection, row M stop projection
-  pj(lo.p_fk, PIK, lo.M, lo.k_proj, PIK, 1, 0);
-  { PJ j; j.src_off = lo.p_sk; j.K = PIK; j.N = 1; j.dst_off = lo.k_proj / 2 + (long long)lo.M * PIK; j.dst_ld = PIK; j.transpose = 1; j.col0 = 0;
-    j.scale = 1.f; j.perm_h = 0; j.part = 0; jobs.push_back(j); }
-  lo.k_projT = takeb(2LL * PIK * 128);                        // [PIK][128]: cols 0..M-1 Wf, col M Ws
-  pj(lo.p_fk, PIK, lo.M, lo.k_projT, 128, 0, 0);
-  pj(lo.p_sk, PIK, 1, lo.k_projT, 128, 0, lo.M);
-  lo.k_pp = takeb(2LL * 128 * lo.PC * (split ? 3 : 1));
-  if (split) pj3(lo.p_ppk, lo.PC, lo.M, lo.k_pp, 3 * lo.PC, 0, lo.PC);
-  else pj(lo.p_ppk, lo.PC, lo.M, lo.k_pp, lo.PC, 1, 0);
-  lo.k_ppT = takeb(2LL * lo.PC * 128); pj(lo.p_ppk, lo.PC, lo.M, lo.k_ppT, 128, 0, 0);
-  lo.k_qT = takeb(2LL * lo.A * lo.D); pj(lo.p_qry, lo.D, lo.A, lo.k_qT, lo.D, 1, 0);   // [A][D] for the attention kernel
-  lo.packed_bytes = o;
+  lo.k_l1r = pk.take(2LL * 4 * lo.D * K1r); add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 1, 0, 1.f, lo.D);
+  lo.k_l1rT = pk.take(2LL * K1r * 4 * lo.D); add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1rT, 4 * lo.D, 0, 0);
+  lo.k_l2 = pk.take(2LL * 4 * lo.D * K2); add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 1, 0, 1.f, lo.D);
+  lo.k_l2T = pk.take(2LL * K2 * 4 * lo.D); add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2T, 4 * lo.D, 0, 0);
+  lo.k_proj = pk.take(2LL * 128 * PIK);                         // rows 0..M-1 frame projection, row M stop projection
+  add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_proj, PIK, 1, 0);
+  add_pack(jobs, lo.p_sk, PIK, 1, lo.k_proj + 2LL * lo.M * PIK, PIK, 1, 0);
+  lo.k_projT = pk.take(2LL * PIK * 128);                        // [PIK][128]: cols 0..M-1 Wf, col M Ws
+  add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_projT, 128, 0, 0);
+  add_pack(jobs, lo.p_sk, PIK, 1, lo.k_projT, 128, 0, lo.M);
+  lo.k_pp = pk.take(2LL * 128 * lo.PC * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, 3 * lo.PC, 0, 2 * lo.PC, lo.PC);
+  else add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, lo.PC, 1, 0);
+  lo.k_ppT = pk.take(2LL * lo.PC * 128); add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_ppT, 128, 0, 0);
+  lo.k_qT = pk.take(2LL * lo.A * lo.D); add_pack(jobs, lo.p_qry, lo.D, lo.A, lo.k_qT, lo.D, 1, 0);   // [A][D] for the attention kernel
+  lo.packed_bytes = pk.used;
   lo.n_packjobs = int(jobs.size());
 
   // ---- workspace ----
-  o = 0;
+  Arena ws;
   const long long B = lo.B, Ti = lo.Ti, To = lo.To;
   const long long xm = split ? 2 : 1;       // split-bf16: stored conv-stack activations are [hi | lo]; pre-batch-norm activations fp32
-  lo.w_emb = takeb(B * Ti * lo.E * 2 * xm);
+  lo.w_emb = ws.take(B * Ti * lo.E * 2 * xm);
   auto conv_ws = [&](ConvL& L, long long T) {
-    L.w_y = takeb(B * T * L.cout * (split ? 4 : 2)); L.w_x = takeb(B * T * L.cout * 2 * xm); L.w_stats = takeb(8LL * L.cout * 4);
+    L.w_y = ws.take(B * T * L.cout * (split ? 4 : 2)); L.w_x = ws.take(B * T * L.cout * 2 * xm); L.w_stats = ws.take(8LL * L.cout * 4);
   };
   for (auto& L : lo.enc) conv_ws(L, Ti);
   for (int d = 0; d < 2; ++d) {
-    lo.w_encpre[d] = takeb(B * Ti * 4 * lo.H * 4);
-    lo.w_ench[d] = takeb((Ti + 1) * B * lo.H * 2);      // h_state history, slot s = state after s processed steps
-    lo.w_encc[d] = takeb((Ti + 1) * B * lo.H * 4);
-    lo.w_encg[d] = takeb(Ti * B * 4 * lo.H * 2);
-    lo.w_enct[d] = takeb(Ti * B * lo.H * 2);
+    lo.w_encpre[d] = ws.take(B * Ti * 4 * lo.H * 4);
+    lo.w_ench[d] = ws.take((Ti + 1) * B * lo.H * 2);      // h_state history, slot s = state after s processed steps
+    lo.w_encc[d] = ws.take((Ti + 1) * B * lo.H * 4);
+    lo.w_encg[d] = ws.take(Ti * B * 4 * lo.H * 2);
+    lo.w_enct[d] = ws.take(Ti * B * lo.H * 2);
   }
-  lo.w_memory = takeb(B * Ti * 2 * lo.H * 2);
-  lo.w_values = takeb(B * Ti * 2 * lo.H * 2);
-  lo.w_keys = takeb(B * Ti * lo.A * 4);
-  lo.w_decin = takeb(B * To * lo.M * 2);                  // time-major [To][B][M]
-  lo.w_pn1 = takeb(To * B * lo.P1 * 2);
-  lo.w_pn2 = takeb(To * B * lo.P2 * 2);
-  lo.w_pre1 = takeb(To * B * 4 * lo.D * 4);
-  lo.w_S1 = takeb((To + 1) * B * K1r * 2);
-  lo.w_S2 = takeb((To + 1) * B * K2 * 2);
-  lo.w_PI = takeb(To * B * PIK * 2);
-  lo.w_c1 = takeb((To + 1) * B * lo.D * 4); lo.w_c2 = takeb((To + 1) * B * lo.D * 4);
-  lo.w_g1 = takeb(To * B * 4 * lo.D * 2); lo.w_g2 = takeb(To * B * 4 * lo.D * 2);
-  lo.w_t1 = takeb(To * B * lo.D * 2); lo.w_t2 = takeb(To * B * lo.D * 2);
-  lo.w_cum = takeb(B * Ti * 4);
-  lo.w_alpha = takeb(To * B * Ti * 4);
-  lo.w_projo = takeb(To * B * 128 * 4);
-  lo.w_decbm = takeb(split ? B * To * 256 * 2 : B * To * lo.M * 2);     /* split: [hi(M) padded to 128 | lo(M) padded to 128] */ lo.w_decf = takeb(B * To * lo.M * 4); lo.w_stop = takeb(B * To * 4);
+  lo.w_memory = ws.take(B * Ti * 2 * lo.H * 2);
+  lo.w_values = ws.take(B * Ti * 2 * lo.H * 2);
+  lo.w_keys = ws.take(B * Ti * lo.A * 4);
+  lo.w_decin = ws.take(B * To * lo.M * 2);                  // time-major [To][B][M]
+  lo.w_pn1 = ws.take(To * B * lo.P1 * 2);
+  lo.w_pn2 = ws.take(To * B * lo.P2 * 2);
+  lo.w_pre1 = ws.take(To * B * 4 * lo.D * 4);
+  lo.w_S1 = ws.take((To + 1) * B * K1r * 2);
+  lo.w_S2 = ws.take((To + 1) * B * K2 * 2);
+  lo.w_PI = ws.take(To * B * PIK * 2);
+  lo.w_c1 = ws.take((To + 1) * B * lo.D * 4); lo.w_c2 = ws.take((To + 1) * B * lo.D * 4);
+  lo.w_g1 = ws.take(To * B * 4 * lo.D * 2); lo.w_g2 = ws.take(To * B * 4 * lo.D * 2);
+  lo.w_t1 = ws.take(To * B * lo.D * 2); lo.w_t2 = ws.take(To * B * lo.D * 2);
+  lo.w_cum = ws.take(B * Ti * 4);
+  lo.w_alpha = ws.take(To * B * Ti * 4);
+  lo.w_projo = ws.take(To * B * 128 * 4);
+  lo.w_decbm = ws.take(split ? B * To * 256 * 2 : B * To * lo.M * 2);     /* split: [hi(M) padded to 128 | lo(M) padded to 128] */ lo.w_decf = ws.take(B * To * lo.M * 4); lo.w_stop = ws.take(B * To * 4);
   for (auto& L : lo.post) conv_ws(L, To);
-  lo.w_tlen = takeb(B * 4);
-  lo.w_resid = takeb(B * To * 128 * 4); lo.w_mel = takeb(B * To * lo.M * 4);
-  lo.w_scal = takeb(64 * 4);
+  lo.w_tlen = ws.take(B * 4);
+  lo.w_resid = ws.take(B * To * 128 * 4); lo.w_mel = ws.take(B * To * lo.M * 4);
+  lo.w_scal = ws.take(64 * 4);
   // backward
-  lo.w_dmel = takeb(B * To * 128 * 2);                    // bf16 [B][To][128] (cols >= M zero)
-  lo.w_dY = takeb(2 * B * (To > Ti ? To : Ti) * (lo.PC > lo.C ? lo.PC : lo.C) * 2);   // ping-pong activation grads bf16
-  lo.w_ddec_tm = takeb(To * B * 128 * 2);
-  lo.w_dPI = takeb(To * B * PIK * 4);
-  lo.w_dh1ext = takeb(B * lo.D * 4); lo.w_dh2ext = takeb(B * lo.D * 4);
-  lo.w_dhs1 = takeb(B * lo.D * 4); lo.w_dhs2 = takeb(B * lo.D * 4); lo.w_dcs1 = takeb(B * lo.D * 4); lo.w_dcs2 = takeb(B * lo.D * 4);
-  lo.w_dg1 = takeb(To * B * 4 * lo.D * 2); lo.w_dg2 = takeb(To * B * 4 * lo.D * 2);
+  lo.w_dmel = ws.take(B * To * 128 * 2);                    // bf16 [B][To][128] (cols >= M zero)
+  lo.w_dY = ws.take(2 * B * (To > Ti ? To : Ti) * (lo.PC > lo.C ? lo.PC : lo.C) * 2);   // ping-pong activation grads bf16
+  lo.w_ddec_tm = ws.take(To * B * 128 * 2);
+  lo.w_dPI = ws.take(To * B * PIK * 4);
+  lo.w_dh1ext = ws.take(B * lo.D * 4); lo.w_dh2ext = ws.take(B * lo.D * 4);
+  lo.w_dhs1 = ws.take(B * lo.D * 4); lo.w_dhs2 = ws.take(B * lo.D * 4); lo.w_dcs1 = ws.take(B * lo.D * 4); lo.w_dcs2 = ws.take(B * lo.D * 4);
+  lo.w_dg1 = ws.take(To * B * 4 * lo.D * 2); lo.w_dg2 = ws.take(To * B * 4 * lo.D * 2);
   lo.w_dgstep = 0;
-  lo.w_dctxl = takeb(B * 2 * lo.H * 4);
-  lo.w_dctx_all = takeb(To * B * 2 * lo.H * 2);
-  lo.w_dq_all = takeb(To * B * lo.A * 2);
-  lo.w_dcum = takeb(B * Ti * 4); lo.w_cumrun = takeb(B * Ti * 4);
-  lo.w_dkeys = takeb(B * Ti * lo.A * 4);
-  lo.w_dvalues = takeb(B * Ti * 2 * lo.H * 4);
-  lo.w_attacc = takeb(B * (lo.KA + 2) * lo.A * 4);
-  lo.w_attU = takeb((2 * lo.KA + 4) * lo.A * 4);
-  lo.w_dpn2 = takeb(To * B * lo.P2 * 2); lo.w_dpn1 = takeb(To * B * lo.P1 * 2);
+  lo.w_dctxl = ws.take(B * 2 * lo.H * 4);
+  lo.w_dctx_all = ws.take(To * B * 2 * lo.H * 2);
+  lo.w_dq_all = ws.take(To * B * lo.A * 2);
+  lo.w_dcum = ws.take(B * Ti * 4); lo.w_cumrun = ws.take(B * Ti * 4);
+  lo.w_dkeys = ws.take(B * Ti * lo.A * 4);
+  lo.w_dvalues = ws.take(B * Ti * 2 * lo.H * 4);
+  lo.w_attacc = ws.take(B * (lo.KA + 2) * lo.A * 4);
+  lo.w_attU = ws.take((2 * lo.KA + 4) * lo.A * 4);
+  lo.w_dpn2 = ws.take(To * B * lo.P2 * 2); lo.w_dpn1 = ws.take(To * B * lo.P1 * 2);
   for (int d = 0; d < 2; ++d) {
-    lo.w_dencpre[d] = takeb(B * Ti * 4 * lo.H * 2);       // bf16 gate grads [B][Ti][4H] (batch-major, = dpre)
-    lo.w_encdh[d] = takeb(B * lo.H * 4); lo.w_encdc[d] = takeb(B * lo.H * 4);
+    lo.w_dencpre[d] = ws.take(B * Ti * 4 * lo.H * 2);       // bf16 gate grads [B][Ti][4H] (batch-major, = dpre)
+    lo.w_encdh[d] = ws.take(B * lo.H * 4); lo.w_encdc[d] = ws.take(B * lo.H * 4);
   }
-  lo.w_encdg = takeb(B * 4 * lo.H * 2);
-  lo.w_ddecf = takeb(B * To * lo.M * 4);
-  for (int d = 0; d < 2; ++d) lo.w_encdgall[d] = takeb(Ti * B * 4 * lo.H * 2);
-  lo.w_dkeysb = takeb(B * Ti * lo.A * 2);
-  lo.w_dz = takeb(To * B * (lo.P1 > lo.P2 ? lo.P1 : lo.P2) * 2);
-  lo.w_dx3 = takeb(B * Ti * lo.C * 2);
-  lo.w_demb = takeb(B * Ti * lo.E * 2);
-  lo.w_tiles = takeb(16384 * sizeof(WgradTile));
-  lo.w_packjobs = takeb((long long)jobs.size() * sizeof(PJ));
+  lo.w_encdg = ws.take(B * 4 * lo.H * 2);
+  lo.w_ddecf = ws.take(B * To * lo.M * 4);
+  for (int d = 0; d < 2; ++d) lo.w_encdgall[d] = ws.take(Ti * B * 4 * lo.H * 2);
+  lo.w_dkeysb = ws.take(B * Ti * lo.A * 2);
+  lo.w_dz = ws.take(To * B * (lo.P1 > lo.P2 ? lo.P1 : lo.P2) * 2);
+  lo.w_dx3 = ws.take(B * Ti * lo.C * 2);
+  lo.w_demb = ws.take(B * Ti * lo.E * 2);
+  lo.w_tiles = ws.take(16384 * sizeof(WgradTile));
+  lo.w_packjobs = ws.take((long long)jobs.size() * sizeof(PackJob));
   lo.n_reg = 0;
   for (auto& p : lo.params) lo.n_reg += p.reg ? 1 : 0;
-  lo.w_regtab = takeb((long long)lo.n_reg * 2 * sizeof(long long));
-  lo.w_zero = takeb(B * 4096 * 4);
-  lo.w_tfsel = takeb(To * 4);
-  lo.w_dfb = takeb(B * lo.M * 4);
-  lo.workspace_bytes = o;
+  lo.w_regtab = ws.take((long long)lo.n_reg * 2 * sizeof(long long));
+  lo.w_zero = ws.take(B * 4096 * 4);
+  lo.w_tfsel = ws.take(To * 4);
+  lo.w_dfb = ws.take(B * lo.M * 4);
+  lo.workspace_bytes = ws.used;
   if (jobs_out) jobs_out->swap(jobs);
   return T2_OK;
 }
@@ -299,58 +268,6 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PJ>* jobs_out) {
 // ------------------------------------------------------------------------------------------------------
 // kernels
 // ------------------------------------------------------------------------------------------------------
-__global__ void tpack_kernel(const float* __restrict__ params, bf16* __restrict__ packed, const PJ* __restrict__ jobs) {
-  // 64x64 tiles through shared memory: float2 reads along the source's fast axis (N), bf16x2 writes along the destination's
-  // fast axis (K for the transposing jobs); scalar fallbacks when an offset / leading dimension is odd
-  __shared__ float tile[64][65];
-  const PJ j = jobs[blockIdx.y];
-  const int tiles_n = (j.N + 63) / 64, tiles_k = (j.K + 63) / 64;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  const bool vec_src = ((j.N | int(j.src_off)) & 1) == 0;
-  const bool vec_dst = ((j.dst_ld | j.col0 | int(j.dst_off)) & 1) == 0;
-  for (int ti = blockIdx.x; ti < tiles_n * tiles_k; ti += gridDim.x) {
-    const int k0 = (ti / tiles_n) * 64, n0 = (ti % tiles_n) * 64;
-    for (int r = ty; r < 64; r += 8) {
-      const int k = k0 + r, n = n0 + 2 * tx;
-      float a = 0.f, b = 0.f;
-      if (k < j.K) {
-        const float* src = params + j.src_off + (long long)k * j.N + n;
-        if (vec_src && n + 1 < j.N) { const float2 v = *reinterpret_cast<const float2*>(src); a = v.x; b = v.y; }
-        else { if (n < j.N) a = src[0]; if (n + 1 < j.N) b = src[1]; }
-      }
-      a *= j.scale; b *= j.scale;
-      if (j.part == 2) { a -= __bfloat162float(__float2bfloat16(a)); b -= __bfloat162float(__float2bfloat16(b)); }
-      tile[r][2 * tx] = a; tile[r][2 * tx + 1] = b;
-    }
-    __syncthreads();
-    if (j.transpose) {
-      for (int r = ty; r < 64; r += 8) {
-        const int n = n0 + r, k = k0 + 2 * tx;
-        if (n < j.N && k < j.K) {
-          int row = n;
-          if (j.perm_h > 0) {  // gate-major column n = g*H + u  ->  EPI_LSTM row (u/32)*128 + g*32 + u%32
-            const int g = n / j.perm_h, u = n % j.perm_h;
-            row = (u / 32) * 128 + g * 32 + (u % 32);
-          }
-          bf16* dst = packed + j.dst_off + (long long)row * j.dst_ld + j.col0 + k;
-          if (vec_dst && k + 1 < j.K) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(tile[2 * tx][r], tile[2 * tx + 1][r]);
-          else { dst[0] = __float2bfloat16(tile[2 * tx][r]); if (k + 1 < j.K) dst[1] = __float2bfloat16(tile[2 * tx + 1][r]); }
-        }
-      }
-    } else {
-      for (int r = ty; r < 64; r += 8) {
-        const int k = k0 + r, n = n0 + 2 * tx;
-        if (n < j.N && k < j.K) {
-          bf16* dst = packed + j.dst_off + (long long)k * j.dst_ld + j.col0 + n;
-          if (vec_dst && n + 1 < j.N) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(tile[r][2 * tx], tile[r][2 * tx + 1]);
-          else { dst[0] = __float2bfloat16(tile[r][2 * tx]); if (n + 1 < j.N) dst[1] = __float2bfloat16(tile[r][2 * tx + 1]); }
-        }
-      }
-    }
-    __syncthreads();
-  }
-}
-
 __global__ void embed_fwd_kernel(const int* __restrict__ idx, const float* __restrict__ table, bf16* __restrict__ out, long long npos, int E,
                                  int split) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -458,7 +375,7 @@ int bn_fwd(const TY* y, bf16* x, float* stats, const float* gamma, const float* 
     T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * C * sizeof(float), st));
     bn_stats_kernel<TY><<<64, 256, 0, st>>>(y, stats, rows, C); t2_count_launch();
   }
-  bn_apply_kernel<TY><<<g1(rows * C), 256, 0, st>>>(y, x, stats, gamma, beta, mm, mv, rows, C, training, p, seed, step, stream, split);
+  bn_apply_kernel<TY><<<grid1d(rows * C), 256, 0, st>>>(y, x, stats, gamma, beta, mm, mv, rows, C, training, p, seed, step, stream, split);
   t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -469,7 +386,7 @@ int bn_bwd(const bf16* dout, const bf16* y, float* stats, const float* gamma, bf
   float* bsum = stats + 4 * C;
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2 * C * sizeof(float), st));
   bn_bwd_stats_kernel<<<64, 256, 0, st>>>(dout, y, stats, bsum, rows, C, p, seed, step, stream); t2_count_launch();
-  bn_bwd_apply_kernel<<<g1(rows * C), 256, 0, st>>>(dout, y, stats, bsum, gamma, dpre, dgamma, dbeta, rows, C, act, p, seed, step, stream);
+  bn_bwd_apply_kernel<<<grid1d(rows * C), 256, 0, st>>>(dout, y, stats, bsum, gamma, dpre, dgamma, dbeta, rows, C, act, p, seed, step, stream);
   t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -747,7 +664,7 @@ AttFwdFn att_fwd_fn(int unmasked, int noncumulative) {
 }
 int att_fwd_setup(const float* K, const float* bK, const float* Wl, const float* ba, float* U, int KA, int F, int A, size_t smem, int unmasked,
                   int noncumulative, cudaStream_t st) {
-  att_prep_kernel<<<g1((KA + 1) * A), 256, 0, st>>>(K, bK, Wl, ba, U, KA, F, A); t2_count_launch();
+  att_prep_kernel<<<grid1d((KA + 1) * A), 256, 0, st>>>(K, bK, Wl, ba, U, KA, F, A); t2_count_launch();
   T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_fn(unmasked, noncumulative), cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -815,16 +732,6 @@ __global__ void mel_finish_kernel(const float* __restrict__ dec_f, const float* 
   l = warp_sum(l);
   if ((threadIdx.x & 31) == 0 && l != 0.f) atomicAdd(scal + 1, l);
 }
-__global__ void reg_loss_kernel(const float* __restrict__ params, const long long* __restrict__ tab, int n, float* __restrict__ scal) {
-  const long long off = tab[2 * blockIdx.y], len = tab[2 * blockIdx.y + 1];
-  float s = 0.f;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < len; i += (long long)gridDim.x * blockDim.x) {
-    const float v = params[off + i]; s += v * v;
-  }
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0 && s != 0.f) atomicAdd(scal + 3, 0.5f * s);
-}
-
 __global__ void proj_bias_kernel(float* p, const float* fb, const float* sb, long long rows, int M) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= rows * (M + 1)) return;
@@ -949,46 +856,39 @@ int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, long long
 // ======================================================================================================
 // fixed-order list of weight-gradient GEMM launches; tiles live in the workspace (uploaded by t2_taco_init)
 struct WgL { std::vector<WgradTile> tiles; };
-void wg_tile(std::vector<WgradTile>& v, int am, int ach, int ash, int bm, int bch, long long off, int ldc, int mv, int nv, float scale = 1.f) {
-  WgradTile t; memset(&t, 0, sizeof(t));
-  t.a_map = am; t.a_ch0 = ach; t.a_shift = ash; t.b_map = bm; t.b_ch0 = bch; t.out_off = off; t.ldc = ldc;
-  t.m_valid = mv; t.n_valid = nv; t.scale = scale; t.accumulate = 0; t.div = nullptr;
-  v.push_back(t);
-}
-// dense [Ca x Cb] gradient of a 1x1 map: A channels [a0, a0+Ca), B channels [b0, b0+Cb)
-void wg_dense(std::vector<WgradTile>& v, int am, int a0, int Ca, int bm, int b0, int Cb, long long off, int ldc, int shift = 0) {
-  for (int m0 = 0; m0 < Ca; m0 += 128)
-    for (int n0 = 0; n0 < Cb; n0 += 256)   // wgrad_gemm_kernel tiles: 128 x (up to) 256
-      wg_tile(v, am, a0 + m0, shift, bm, b0 + n0, off + (long long)m0 * ldc + n0, ldc, Ca - m0 < 128 ? Ca - m0 : 128, Cb - n0 < 256 ? Cb - n0 : 256);
-}
 enum { WG_PP = 0, WG_POST0 = 1 /* .. +postnet layers */ };
 void build_tiles(const TL& lo, std::vector<WgL>& L) {
   L.clear();
+  auto dense = [](int am, int bm, int shift = 0) {   // a plain weight gradient: maps, A time shift, scale 1
+    WgradTile t; memset(&t, 0, sizeof(t));
+    t.a_map = am; t.a_shift = shift; t.b_map = bm; t.scale = 1.f;
+    return t;
+  };
   const int H = lo.H, D = lo.D, K1r = 2 * H + D, K2 = 2 * D, PIK = D + 2 * H;
   auto conv = [&](const ConvL& c) {
     WgL w;
-    for (int j = 0; j < c.k; ++j) wg_dense(w.tiles, 0, 0, c.cin, 1, 0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout, j - (c.k - 1) / 2);
+    for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w.tiles, dense(0, 1, j - (c.k - 1) / 2), 0, c.cin, 0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
     L.push_back(w);
   };
-  { WgL w; wg_dense(w.tiles, 0, 0, lo.PC, 1, 0, lo.M, lo.p_ppk, lo.M); L.push_back(w); }            // 0: postnet projection
+  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, lo.PC, 0, lo.M, lo.p_ppk, lo.M); L.push_back(w); }            // 0: postnet projection
   for (int i = int(lo.post.size()) - 1; i >= 0; --i) conv(lo.post[i]);                                // 1..: postnet convs (reverse)
-  { WgL w; wg_dense(w.tiles, 0, 0, PIK, 1, 0, lo.M, lo.p_fk, lo.M); wg_dense(w.tiles, 0, 0, PIK, 1, lo.M, 1, lo.p_sk, 1); L.push_back(w); }  // proj
+  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, PIK, 0, lo.M, lo.p_fk, lo.M); append_wgrad_tiles(w.tiles, dense(0, 1), 0, PIK, lo.M, 1, lo.p_sk, 1); L.push_back(w); }  // proj
   { WgL w;                                                                                               // decoder LSTMs + prenet-to-LSTM
-    wg_dense(w.tiles, 0, 0, K2, 1, 0, 4 * D, lo.p_l2k, 4 * D);                                          // maps: 0 S2, 1 dg2, 2 S1, 3 dg1, 4 pn2
-    wg_dense(w.tiles, 2, 0, K1r, 3, 0, 4 * D, lo.p_l1k + (long long)lo.P2 * 4 * D, 4 * D);
-    wg_dense(w.tiles, 4, 0, lo.P2, 3, 0, 4 * D, lo.p_l1k, 4 * D);
+    append_wgrad_tiles(w.tiles, dense(0, 1), 0, K2, 0, 4 * D, lo.p_l2k, 4 * D);                                          // maps: 0 S2, 1 dg2, 2 S1, 3 dg1, 4 pn2
+    append_wgrad_tiles(w.tiles, dense(2, 3), 0, K1r, 0, 4 * D, lo.p_l1k + (long long)lo.P2 * 4 * D, 4 * D);
+    append_wgrad_tiles(w.tiles, dense(4, 3), 0, lo.P2, 0, 4 * D, lo.p_l1k, 4 * D);
     L.push_back(w); }
   { WgL w;                                                                                               // prenet + query layer
-    wg_dense(w.tiles, 0, 0, lo.P1, 1, 0, lo.P2, lo.p_p2k, lo.P2);                                       // maps: 0 pn1, 1 dz2, 2 decin, 3 dz1, 4 PI, 5 dq_all
-    wg_dense(w.tiles, 2, 0, lo.M, 3, 0, lo.P1, lo.p_p1k, lo.P1);
-    wg_dense(w.tiles, 4, 0, D, 5, 0, lo.A, lo.p_qry, lo.A);
+    append_wgrad_tiles(w.tiles, dense(0, 1), 0, lo.P1, 0, lo.P2, lo.p_p2k, lo.P2);                                       // maps: 0 pn1, 1 dz2, 2 decin, 3 dz1, 4 PI, 5 dq_all
+    append_wgrad_tiles(w.tiles, dense(2, 3), 0, lo.M, 0, lo.P1, lo.p_p1k, lo.P1);
+    append_wgrad_tiles(w.tiles, dense(4, 5), 0, D, 0, lo.A, lo.p_qry, lo.A);
     L.push_back(w); }
-  { WgL w; wg_dense(w.tiles, 0, 0, 2 * H, 1, 0, lo.A, lo.p_mem, lo.A); L.push_back(w); }               // memory layer: values x dkeys
+  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, 2 * H, 0, lo.A, lo.p_mem, lo.A); L.push_back(w); }               // memory layer: values x dkeys
   for (int d = 0; d < 2; ++d) {                                                                          // encoder LSTM d
     WgL w;  // maps: 0 h history (time-major), 1 gate grads time-major, 2 x3 (batch-major), 3 gate grads batch-major
-    wg_dense(w.tiles, 0, 0, H, 1, 0, 4 * H, lo.p_elk[d] + (long long)lo.C * 4 * H, 4 * H);
+    append_wgrad_tiles(w.tiles, dense(0, 1), 0, H, 0, 4 * H, lo.p_elk[d] + (long long)lo.C * 4 * H, 4 * H);
     L.push_back(w);
-    WgL w2; wg_dense(w2.tiles, 0, 0, lo.C, 1, 0, 4 * H, lo.p_elk[d], 4 * H); L.push_back(w2);
+    WgL w2; append_wgrad_tiles(w2.tiles, dense(0, 1), 0, lo.C, 0, 4 * H, lo.p_elk[d], 4 * H); L.push_back(w2);
   }
   for (int i = int(lo.enc.size()) - 1; i >= 0; --i) conv(lo.enc[i]);
 }
@@ -1043,15 +943,6 @@ __global__ void ddec_tm_kernel(const float* __restrict__ ddec, const bf16* __res
 __global__ void relu_drop_bwd_kernel(const bf16* __restrict__ d, const bf16* __restrict__ y, bf16* __restrict__ dz, long long n, float p) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e < n) dz[e] = __float2bfloat16(__bfloat162float(y[e]) > 0.f ? __bfloat162float(d[e]) / (1.f - p) : 0.f);
-}
-__global__ void f32_to_bf16_k(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < n) out[e] = __float2bfloat16(in[e]);
-}
-__global__ void reg_grad_kernel(const float* __restrict__ params, float* __restrict__ grads, const long long* __restrict__ tab, float w) {
-  const long long off = tab[2 * blockIdx.y], len = tab[2 * blockIdx.y + 1];
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < len; i += (long long)gridDim.x * blockDim.x)
-    grads[off + i] += w * params[off + i];
 }
 
 // backward of one LSTM cell + zoneout (see EPI_LSTM): produces the pre-activation gate gradients and the state grads
@@ -1455,14 +1346,14 @@ int launch_att_bwd(const AttBwd& a, size_t smem, cudaStream_t st) {
   return T2_OK;
 }
 int launch_cell_bwd(const CellBwd& c, cudaStream_t st) {
-  T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(g1((long long)c.B * c.H)), dim3(256), 0, st, c)); t2_count_launch();
+  T2_CHECK_CUDA(launch_pdl(lstm_cell_bwd_kernel, dim3(grid1d((long long)c.B * c.H)), dim3(256), 0, st, c)); t2_count_launch();
   return T2_OK;
 }
 // scratch: [(KA+2)][A] fp32 for the batch-reduced accumulators
 void launch_att_finish(const float* acc, const float* K, const float* bK, const float* Wl, float* grads, int B, int KA, int F, int A, long long o_k,
                        long long o_bk, long long o_wl, long long o_v, long long o_ba, float* scratch, cudaStream_t st) {
-  att_finish_kernel<<<g1((long long)(KA + 2) * A), 256, 0, st>>>(acc, K, bK, Wl, grads, B, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba, scratch); t2_count_launch();
-  att_finish2_kernel<<<g1(KA * F + F * A + F + A), 256, 0, st>>>(scratch, K, bK, Wl, grads, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba); t2_count_launch();
+  att_finish_kernel<<<grid1d((long long)(KA + 2) * A), 256, 0, st>>>(acc, K, bK, Wl, grads, B, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba, scratch); t2_count_launch();
+  att_finish2_kernel<<<grid1d(KA * F + F * A + F + A), 256, 0, st>>>(scratch, K, bK, Wl, grads, KA, F, A, o_k, o_bk, o_wl, o_v, o_ba); t2_count_launch();
 }
 void launch_dvalues_ctx(const float* alpha, const bf16* dctx, const int* lens, float* dvalues, int B, int Ti, int To, int C2, cudaStream_t st) {
   dvalues_ctx_kernel<<<dim3(Ti, B), 256, 0, st>>>(alpha, dctx, lens, dvalues, B, Ti, To, C2); t2_count_launch();
@@ -1502,7 +1393,10 @@ extern "C" int t2_taco_sizes(const t2_taco_config_t* cfg, long long* n_params, l
   TL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
-  *n_params = lo.n_params; *packed_bytes = lo.packed_bytes; *workspace_bytes = lo.workspace_bytes; *n_tensors = int(lo.params.size());
+  if (n_params) *n_params = lo.n_params;
+  if (packed_bytes) *packed_bytes = lo.packed_bytes;
+  if (workspace_bytes) *workspace_bytes = lo.workspace_bytes;
+  if (n_tensors) *n_tensors = int(lo.params.size());
   return T2_OK;
 }
 
@@ -1511,28 +1405,21 @@ extern "C" int t2_taco_param_info(const t2_taco_config_t* cfg, int i, char* name
   TL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
-  T2_REQUIRE(i >= 0 && i < int(lo.params.size()), T2_ERR_INVALID_ARG, "tensor index out of range");
-  const PT& p = lo.params[i];
-  snprintf(name, cap, "%s", p.name.c_str());
-  *offset = p.off; *ndim = p.ndim; *trainable = p.trainable ? 1 : 0;
-  for (int k = 0; k < 4; ++k) shape4[k] = p.shape[k];
-  return T2_OK;
+  return param_info(lo.params, i, name, cap, offset, ndim, shape4, trainable);
 }
 
 extern "C" int t2_taco_init(const t2_taco_config_t* cfg, void* d_packed, void* d_workspace, void* stream) {
   TL lo;
-  std::vector<PJ> jobs;
+  std::vector<PackJob> jobs;
   int rc = build(cfg, lo, &jobs);
   if (rc) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   T2_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, lo.packed_bytes, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d_workspace, 0, lo.workspace_bytes, st));
-  T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_packjobs, jobs.data(), jobs.size() * sizeof(PJ), cudaMemcpyHostToDevice, st));
-  std::vector<long long> reg;
-  for (auto& p : lo.params)
-    if (p.reg) { long long n = 1; for (int k = 0; k < p.ndim; ++k) n *= p.shape[k]; reg.push_back(p.off); reg.push_back(n); }
-  T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_regtab, reg.data(), reg.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
+  T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_packjobs, jobs.data(), jobs.size() * sizeof(PackJob), cudaMemcpyHostToDevice, st));
+  rc = upload_reg_table(lo.params, ws + lo.w_regtab, st);
+  if (rc) return rc;
   std::vector<WgL> wl;
   build_tiles(lo, wl);
   std::vector<WgradTile> all;
@@ -1547,42 +1434,23 @@ extern "C" int t2_taco_pack_weights(const t2_taco_config_t* cfg, const float* d_
   TL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  tpack_kernel<<<dim3(32, lo.n_packjobs), dim3(32, 8), 0, st>>>(d_params, static_cast<bf16*>(d_packed),
-                                                        reinterpret_cast<const PJ*>(static_cast<uint8_t*>(d_workspace) + lo.w_packjobs));
-  t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
-}
-
-// The two directions of the encoder BiLSTM are independent chains of small launches (8-16 CTAs each): the backward
-// direction runs on a side stream (fork / join through events; capturable; T2_SIDE_STREAM=0 keeps one stream).
-struct TacoSide { cudaStream_t s; cudaEvent_t fork, join; };
-static TacoSide* taco_side() {
-  static TacoSide ss;
-  static int state = 0;   // 0 unknown, 1 ready, -1 disabled
-  if (state == 0) {
-    const char* e = getenv("T2_SIDE_STREAM");
-    if (e && e[0] == '0') state = -1;
-    else if (cudaStreamCreateWithFlags(&ss.s, cudaStreamNonBlocking) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ss.fork, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ss.join, cudaEventDisableTiming) == cudaSuccess) state = 1;
-    else state = -1;
-  }
-  return state == 1 ? &ss : nullptr;
+  return launch_pack(d_params, d_packed, reinterpret_cast<const PackJob*>(static_cast<uint8_t*>(d_workspace) + lo.w_packjobs), lo.n_packjobs,
+                     32, 32, static_cast<cudaStream_t>(stream));
 }
 
 // ---- encoder: embedding -> conv blocks -> BiLSTM -> masked values -> attention keys (tacotron.py:113-131) ----
+// The two directions of the encoder BiLSTM are independent chains of small launches (8-16 CTAs each): the backward
+// direction runs on the side stream (fork / join through events; capturable).
 static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input_lengths, int training) {
   const TL& lo = *s.lo;
   uint8_t* ws = s.ws; const uint8_t* pk = s.pk; const float* d_params = s.params; cudaStream_t st = s.st;
   const int B = lo.B, Ti = lo.Ti, H = lo.H;
   int rc;
   bf16* emb = reinterpret_cast<bf16*>(ws + lo.w_emb);
-  embed_fwd_kernel<<<g1((long long)B * Ti * lo.E), 256, 0, st>>>(d_inputs, d_params + lo.p_emb, emb, (long long)B * Ti, lo.E, lo.c.split_bf16); t2_count_launch();
+  embed_fwd_kernel<<<grid1d((long long)B * Ti * lo.E), 256, 0, st>>>(d_inputs, d_params + lo.p_emb, emb, (long long)B * Ti, lo.E, lo.c.split_bf16); t2_count_launch();
   const void* x = emb;
   for (auto& L : lo.enc) { rc = conv_block_fwd(s, L, x, Ti, training); if (rc) return rc; x = ws + L.w_x; }
-  TacoSide* side = taco_side();
+  SideStream* side = side_stream();
   if (side) {
     T2_CHECK_CUDA(cudaEventRecord(side->fork, st));
     T2_CHECK_CUDA(cudaStreamWaitEvent(side->s, side->fork, 0));
@@ -1614,7 +1482,7 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
     T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
   }
   bf16* values = reinterpret_cast<bf16*>(ws + lo.w_values);
-  mask_values_kernel<<<g1((long long)B * Ti * 2 * H), 256, 0, st>>>(reinterpret_cast<bf16*>(ws + lo.w_memory), d_input_lengths, values, B, Ti, 2 * H);
+  mask_values_kernel<<<grid1d((long long)B * Ti * 2 * H), 256, 0, st>>>(reinterpret_cast<bf16*>(ws + lo.w_memory), d_input_lengths, values, B, Ti, 2 * H);
   t2_count_launch();
   float* keys = reinterpret_cast<float*>(ws + lo.w_keys);
   return conv_gemm(values, 2 * H, Ti, B, pk + lo.k_mem, lo.A, 2 * H, 1, nullptr, 128, nullptr, 0, nullptr, keys, lo.A, lo.A, 0.f, 0, 0, nullptr, st);
@@ -1694,7 +1562,7 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   if (rc) return rc;
   const void* x = nullptr;
   bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
-  decin_kernel<<<g1((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M); t2_count_launch();
+  decin_kernel<<<grid1d((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M); t2_count_launch();
   const long long TB = (long long)To * B;
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
@@ -1722,7 +1590,7 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
     rc = conv_gemm(db.PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st);
     if (rc) return rc;
     // add the projection biases in place (tiny), then clip / losses
-    proj_bias_kernel<<<g1(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
+    proj_bias_kernel<<<grid1d(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
   } else {
     // ---- decoder at a teacher-forcing ratio < 1: step t + 1's input is known only once step t has drawn and projected, so the
     // prenet, the LSTM-1 input projection and the projections run per step (the loop of t2_taco_infer_steps). The prenet masks are the
@@ -1746,7 +1614,7 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
       rc = conv_gemm(db.PI + (long long)t * B * PIK, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
                      lo.M + 1, 0.f, 0, 0, nullptr, st);
       if (rc) return rc;
-      T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(g1((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
+      T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
                                d_params + lo.p_sb, t + 1 < To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M, d_mel_targets, To, t,
                                lo.c.teacher_forcing_ratio, seed, d_step, choice));
       t2_count_launch();
@@ -1756,7 +1624,7 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
   bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
   float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
-  dec_finish_kernel<<<g1((long long)B * To * (lo.M + 1)), 256, 0, st>>>(projo, d_mel_targets, d_stop_targets, dec_bm, dec_f,
+  dec_finish_kernel<<<grid1d((long long)B * To * (lo.M + 1)), 256, 0, st>>>(projo, d_mel_targets, d_stop_targets, dec_bm, dec_f,
                                                                         reinterpret_cast<float*>(ws + lo.w_stop), scal, B, To, lo.M,
                                                                         lo.c.clip_outputs, lo_c, hi_c, lo.c.split_bf16, tlen, lo.c.cross_entropy_pos_weight); t2_count_launch();
   // ---- postnet ----
@@ -1766,9 +1634,9 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   rc = conv_gemm(x, lo.PC, To, B, pk + lo.k_pp, lo.M, lo.PC * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, d_params + lo.p_ppb, 0, nullptr, resid, 128, lo.M,
                  0.f, 0, 0, nullptr, st, lo.c.split_bf16);
   if (rc) return rc;
-  mel_finish_kernel<<<g1((long long)B * To * lo.M), 256, 0, st>>>(dec_f, resid, d_mel_targets, reinterpret_cast<float*>(ws + lo.w_mel), scal,
+  mel_finish_kernel<<<grid1d((long long)B * To * lo.M), 256, 0, st>>>(dec_f, resid, d_mel_targets, reinterpret_cast<float*>(ws + lo.w_mel), scal,
                                                                   (long long)B * To, lo.M, lo.c.clip_outputs, lo_c, hi_c, tlen, To); t2_count_launch();
-  reg_loss_kernel<<<dim3(8, lo.n_reg), 256, 0, st>>>(d_params, reinterpret_cast<const long long*>(ws + lo.w_regtab), lo.n_reg, scal); t2_count_launch();
+  launch_reg_loss(d_params, reinterpret_cast<const long long*>(ws + lo.w_regtab), lo.n_reg, scal + 3, st);
   T2_CHECK_CUDA(cudaGetLastError());
   loss_norm_kernel<<<1, 1, 0, st>>>(scal, d_loss, float((long long)B * To * lo.M), float((long long)B * To), lo.c.reg_weight, tlen, B, To, lo.M);
   t2_count_launch();
@@ -1842,7 +1710,7 @@ extern "C" int t2_taco_infer_steps(const t2_taco_config_t* cfg, float* d_params,
     rc = conv_gemm(db.PI + (long long)t * B * PIK, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128, lo.M + 1,
                    0.f, 0, 0, nullptr, st);
     if (rc) return rc;
-    T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(g1((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
+    T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
                              d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M,
                              (const float*)nullptr, lo.To, t, 0.f, 0ull, (const unsigned long long*)nullptr, (int*)nullptr));
     t2_count_launch();
@@ -1867,7 +1735,7 @@ extern "C" int t2_taco_infer_finish(const t2_taco_config_t* cfg, float* d_params
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
   bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
   float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
-  dec_finish_kernel<<<g1((long long)B * T_used * (lo.M + 1)), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_projo), nullptr, nullptr, dec_bm, dec_f,
+  dec_finish_kernel<<<grid1d((long long)B * T_used * (lo.M + 1)), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_projo), nullptr, nullptr, dec_bm, dec_f,
                                                                             reinterpret_cast<float*>(ws + lo.w_stop), scal, B, T_used, lo.M,
                                                                             lo.c.clip_outputs, lo_c, hi_c, lo.c.split_bf16, nullptr, 1.f); t2_count_launch();
   const void* x = dec_bm;
@@ -1876,7 +1744,7 @@ extern "C" int t2_taco_infer_finish(const t2_taco_config_t* cfg, float* d_params
   rc = conv_gemm(x, lo.PC, T_used, B, pk + lo.k_pp, lo.M, lo.PC * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, d_params + lo.p_ppb, 0, nullptr, resid, 128, lo.M,
                  0.f, 0, 0, nullptr, st, lo.c.split_bf16);
   if (rc) return rc;
-  mel_finish_kernel<<<g1((long long)B * T_used * lo.M), 256, 0, st>>>(dec_f, resid, nullptr, reinterpret_cast<float*>(ws + lo.w_mel), scal,
+  mel_finish_kernel<<<grid1d((long long)B * T_used * lo.M), 256, 0, st>>>(dec_f, resid, nullptr, reinterpret_cast<float*>(ws + lo.w_mel), scal,
                                                                       (long long)B * T_used, lo.M, lo.c.clip_outputs, lo_c, hi_c, nullptr, T_used); t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -1977,7 +1845,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   const int* tlen = lo.c.mask_decoder ? reinterpret_cast<const int*>(ws + lo.w_tlen) : nullptr;
   const float* scal = reinterpret_cast<const float*>(ws + lo.w_scal);      // [5], [6]: the loss normalisers of the forward pass
   // ---- loss seeds + postnet ----
-  loss_seed_kernel<<<g1(BTo * 128), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_decf), reinterpret_cast<float*>(ws + lo.w_resid),
+  loss_seed_kernel<<<grid1d(BTo * 128), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_decf), reinterpret_cast<float*>(ws + lo.w_resid),
                                                   reinterpret_cast<float*>(ws + lo.w_mel), d_mel_targets, dmel, ddecf, BTo, M, lo.c.clip_outputs,
                                                   lo_c, hi_c, tlen, To, scal, d_mel_outputs_grad); t2_count_launch();
   rc = conv_gemm(dmel, 128, To, B, pk + lo.k_ppT, lo.PC, 128, 1, nullptr, lo.PC % 256 == 0 ? 256 : 128, nullptr, 0, dY0, nullptr, lo.PC, lo.PC, 0.f, 0, 0,
@@ -2014,7 +1882,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     return T2_OK;
   };
   if (!per_step) {
-    ddec_tm_kernel<<<g1(TB * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c, hi_c, tlen,
+    ddec_tm_kernel<<<grid1d(TB * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c, hi_c, tlen,
                                                  lo.c.cross_entropy_pos_weight, scal, 0, To, nullptr, nullptr);
     t2_count_launch();
     rc = conv_gemm(ddec_tm, 128, TB, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dPI, PIK, PIK, 0.f, 0, 0,
@@ -2066,7 +1934,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     if (per_step) {
       // loss gradient of step t's projection outputs + (when step t + 1 consumed step t's frame) the gradient of step t + 1's input,
       // left in dfb by the previous iteration; then dPI_t through the frame / stop projections
-      ddec_tm_kernel<<<g1((long long)B * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c,
+      ddec_tm_kernel<<<grid1d((long long)B * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c,
                                                             hi_c, tlen, lo.c.cross_entropy_pos_weight, scal, t, t + 1,
                                                             t + 1 < To ? dfb : nullptr, choice);
       t2_count_launch();
@@ -2107,12 +1975,12 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
       rc = conv_gemm(c1.dg_a, 4 * D, B, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2 + r2, nullptr,
                      lo.P2, lo.P2, 0.f, 0, 0, nullptr, st);
       if (rc) return rc;
-      relu_drop_bwd_kernel<<<g1((long long)B * lo.P2), 256, 0, st>>>(dpn2 + r2, pn2 + r2, dz2 + r2, (long long)B * lo.P2, lo.c.dropout_rate);
+      relu_drop_bwd_kernel<<<grid1d((long long)B * lo.P2), 256, 0, st>>>(dpn2 + r2, pn2 + r2, dz2 + r2, (long long)B * lo.P2, lo.c.dropout_rate);
       t2_count_launch();
       rc = conv_gemm(dz2 + r2, lo.P2, B, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1 + r1, nullptr,
                      lo.P1, lo.P1, 0.f, 0, 0, nullptr, st);
       if (rc) return rc;
-      relu_drop_bwd_kernel<<<g1((long long)B * lo.P1), 256, 0, st>>>(dpn1 + r1, pn1 + r1, dpn1 + r1, (long long)B * lo.P1, lo.c.dropout_rate);
+      relu_drop_bwd_kernel<<<grid1d((long long)B * lo.P1), 256, 0, st>>>(dpn1 + r1, pn1 + r1, dpn1 + r1, (long long)B * lo.P1, lo.c.dropout_rate);
       t2_count_launch();
       if (t >= 1) {
         rc = conv_gemm(dpn1 + r1, lo.P1, B, 1, pk + lo.k_p1T, M, lo.P1, 1, nullptr, 128, nullptr, 0, nullptr, dfb, M, M, 0.f, 0, 0, nullptr, st);
@@ -2134,11 +2002,11 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     rc = conv_gemm(dg1, 4 * D, TB, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2, nullptr, lo.P2, lo.P2, 0.f,
                    0, 0, nullptr, st);
     if (rc) return rc;
-    relu_drop_bwd_kernel<<<g1(TB * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, TB * lo.P2, lo.c.dropout_rate); t2_count_launch();
+    relu_drop_bwd_kernel<<<grid1d(TB * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, TB * lo.P2, lo.c.dropout_rate); t2_count_launch();
     rc = conv_gemm(dz2, lo.P2, TB, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1, nullptr, lo.P1, lo.P1, 0.f, 0,
                    0, nullptr, st);
     if (rc) return rc;
-    relu_drop_bwd_kernel<<<g1(TB * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, TB * lo.P1, lo.c.dropout_rate); t2_count_launch();
+    relu_drop_bwd_kernel<<<grid1d(TB * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, TB * lo.P1, lo.c.dropout_rate); t2_count_launch();
   }
   {
     ActT maps[6] = {make_act(pn1, lo.P1, int(TB), 1), make_act(dz2, lo.P2, int(TB), 1), make_act(ws + lo.w_decin, M, int(TB), 1),
@@ -2154,7 +2022,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   }
   // ---- attention memory: keys / values ----
   bf16* dkeysb = reinterpret_cast<bf16*>(ws + lo.w_dkeysb);
-  f32_to_bf16_k<<<g1((long long)B * Ti * A), 256, 0, st>>>(dkeys, dkeysb, (long long)B * Ti * A); t2_count_launch();
+  launch_f32_to_bf16(dkeys, dkeysb, (long long)B * Ti * A, st);
   float* dvalues = reinterpret_cast<float*>(ws + lo.w_dvalues);
   rc = conv_gemm(dkeysb, A, Ti, B, pk + lo.k_memT, 2 * H, A, 1, nullptr, (2 * H) % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dvalues, 2 * H, 2 * H, 0.f, 0, 0,
                  nullptr, st);
@@ -2166,7 +2034,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   launch_dvalues_ctx(reinterpret_cast<float*>(ws + lo.w_alpha), dctx_all, d_input_lengths, dvalues, B, Ti, To, 2 * H, st);
   // ---- encoder BiLSTM, backward through time ----
   const void* x3 = ws + lo.enc.back().w_x;
-  TacoSide* side = taco_side();
+  SideStream* side = side_stream();
   if (side) {
     T2_CHECK_CUDA(cudaEventRecord(side->fork, st));
     T2_CHECK_CUDA(cudaStreamWaitEvent(side->s, side->fork, 0));
@@ -2230,11 +2098,10 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
       ++li;
       dout = dx;
     }
-    embed_bwd_kernel<<<g1((long long)B * Ti * lo.E), 256, 0, st>>>(d_inputs, demb, d_grads + lo.p_emb, (long long)B * Ti, lo.E); t2_count_launch();
+    embed_bwd_kernel<<<grid1d((long long)B * Ti * lo.E), 256, 0, st>>>(d_inputs, demb, d_grads + lo.p_emb, (long long)B * Ti, lo.E); t2_count_launch();
   }
   // ---- L2 regulariser (tacotron.py:343-345) ----
-  reg_grad_kernel<<<dim3(8, lo.n_reg), 256, 0, st>>>(d_params, d_grads, reinterpret_cast<const long long*>(ws + lo.w_regtab), lo.c.reg_weight);
-  t2_count_launch();
+  launch_reg_grad(d_params, d_grads, reinterpret_cast<const long long*>(ws + lo.w_regtab), lo.n_reg, lo.c.reg_weight, st);
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }

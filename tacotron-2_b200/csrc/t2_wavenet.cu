@@ -22,23 +22,13 @@
 #include "../../include/t2b200.h"
 #include "t2_common.cuh"
 #include "t2_gemm.h"
+#include "t2_params.h"
 
 namespace t2 {
 namespace {
 
 typedef __nv_bfloat16 bf16;
 
-struct PackJob {
-  long long src_off;  // fp32 element offset in params ([K][N] row-major == TF [in][out])
-  int K, N;
-  long long dst_off;  // bf16 element offset in packed
-  int dst_ld;
-  int transpose;      // 1: dst[rowmap(n)][col0 + k] ; 0: dst[k][col0 + n]
-  int col0;
-  float scale;
-  int perm_gh;        // >0: gate row permutation with this G/2
-  int part;           // 0 / 1: bf16(w) ; 2: bf16(w - bf16(w)), the low half of the split-bf16 operand
-};
 struct ColsumJob {
   long long src_off;  // byte offset in workspace of a bf16 [rows][ld] matrix
   long long rows;
@@ -46,15 +36,6 @@ struct ColsumJob {
   long long dst_off, dst2_off;  // fp32 element offsets in grads (dst2 < 0: none)
   float scale;
   int div_scalar;     // index into ws scalars to divide by (or -1)
-};
-
-inline long long align_up(long long v, long long a) { return (v + a - 1) / a * a; }
-
-struct ParamT {
-  std::string name;
-  long long off;
-  int ndim;
-  int shape[4];
 };
 
 struct Layout {
@@ -67,7 +48,7 @@ struct Layout {
   float res_scale;
   std::vector<float> skip_scale;
   // params
-  std::vector<ParamT> params;
+  std::vector<Param> params;
   long long n_params;
   long long p_in_k, p_in_b, p_f1_k, p_f1_b, p_f2_k, p_f2_b;
   std::vector<long long> p_dil_k, p_dil_b, p_c_k, p_c_b, p_s_k, p_s_b, p_o_k, p_o_b, p_up_k, p_up_b;
@@ -95,20 +76,6 @@ struct Layout {
   std::vector<int> tile_start;   // [L + 1]: first entry of tiles_main that belongs to layer l (the table is layer-major)
   int dil(int l) const { return 1 << (l % (L / c.stacks)); }
 };
-
-long long add_param(Layout& lo, const std::string& name, std::initializer_list<int> shape) {
-  ParamT p;
-  p.name = name;
-  p.off = lo.n_params;
-  p.ndim = int(shape.size());
-  long long n = 1;
-  int i = 0;
-  for (int s : shape) { p.shape[i++] = s; n *= s; }
-  for (; i < 4; ++i) p.shape[i] = 1;
-  lo.n_params += align_up(n, 4);  // keep every tensor 16-byte aligned inside the flat buffer
-  lo.params.push_back(p);
-  return p.off;
-}
 
 int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   T2_REQUIRE(cfg != nullptr, T2_ERR_INVALID_ARG, "null config");
@@ -169,32 +136,32 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.n_params = 0;
   lo.params.clear();
   const int cin = lo.scalar_in ? 1 : lo.Q;
-  lo.p_in_k = add_param(lo, "input_convolution/kernel", {1, cin, lo.R});
-  lo.p_in_b = add_param(lo, "input_convolution/bias", {lo.R});
+  lo.p_in_k = add_param(lo.params, lo.n_params, "input_convolution/kernel", {1, cin, lo.R});
+  lo.p_in_b = add_param(lo.params, lo.n_params, "input_convolution/bias", {lo.R});
   for (int l = 0; l < lo.L; ++l) {
     char p[64];
     snprintf(p, sizeof(p), "ResidualConv1DGLU_%d/", l);
     std::string s(p);
-    lo.p_dil_k.push_back(add_param(lo, s + "residual_block_causal_conv/kernel", {3, lo.R, lo.G}));
-    lo.p_dil_b.push_back(add_param(lo, s + "residual_block_causal_conv/bias", {lo.G}));
+    lo.p_dil_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_causal_conv/kernel", {3, lo.R, lo.G}));
+    lo.p_dil_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_causal_conv/bias", {lo.G}));
     if (lo.C > 0) {
-      lo.p_c_k.push_back(add_param(lo, s + "residual_block_cin_conv/kernel", {1, lo.C, lo.G}));
-      lo.p_c_b.push_back(add_param(lo, s + "residual_block_cin_conv/bias", {lo.G}));
+      lo.p_c_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_cin_conv/kernel", {1, lo.C, lo.G}));
+      lo.p_c_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_cin_conv/bias", {lo.G}));
     }
     if (lo.Gi > 0) {
-      lo.p_g_k.push_back(add_param(lo, s + "residual_block_gin_conv/kernel", {1, lo.Gi, lo.G}));
-      lo.p_g_b.push_back(add_param(lo, s + "residual_block_gin_conv/bias", {lo.G}));
+      lo.p_g_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_gin_conv/kernel", {1, lo.Gi, lo.G}));
+      lo.p_g_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_gin_conv/bias", {lo.G}));
     }
-    lo.p_s_k.push_back(add_param(lo, s + "residual_block_skip_conv/kernel", {1, lo.Gh, lo.S}));
-    lo.p_s_b.push_back(add_param(lo, s + "residual_block_skip_conv/bias", {lo.S}));
-    lo.p_o_k.push_back(add_param(lo, s + "residual_block_out_conv/kernel", {1, lo.Gh, lo.R}));
-    lo.p_o_b.push_back(add_param(lo, s + "residual_block_out_conv/bias", {lo.R}));
+    lo.p_s_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_skip_conv/kernel", {1, lo.Gh, lo.S}));
+    lo.p_s_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_skip_conv/bias", {lo.S}));
+    lo.p_o_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_out_conv/kernel", {1, lo.Gh, lo.R}));
+    lo.p_o_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_out_conv/bias", {lo.R}));
   }
-  lo.p_f1_k = add_param(lo, "final_convolution_1/kernel", {1, lo.S, lo.S});
-  lo.p_f1_b = add_param(lo, "final_convolution_1/bias", {lo.S});
-  lo.p_f2_k = add_param(lo, "final_convolution_2/kernel", {1, lo.S, lo.O});
-  lo.p_f2_b = add_param(lo, "final_convolution_2/bias", {lo.O});
-  lo.p_emb = lo.Gi > 0 ? add_param(lo, "gc_embedding", {lo.NS, lo.Gi}) : -1;   // outside the residual stack (modules.py:12-21)
+  lo.p_f1_k = add_param(lo.params, lo.n_params, "final_convolution_1/kernel", {1, lo.S, lo.S});
+  lo.p_f1_b = add_param(lo.params, lo.n_params, "final_convolution_1/bias", {lo.S});
+  lo.p_f2_k = add_param(lo.params, lo.n_params, "final_convolution_2/kernel", {1, lo.S, lo.O});
+  lo.p_f2_b = add_param(lo.params, lo.n_params, "final_convolution_2/bias", {lo.O});
+  lo.p_emb = lo.Gi > 0 ? add_param(lo.params, lo.n_params, "gc_embedding", {lo.NS, lo.Gi}) : -1;   // outside the residual stack (modules.py:12-21)
   lo.layer_stride = lo.L > 1 ? lo.p_dil_k[1] - lo.p_dil_k[0] : 0;
   for (size_t i = 0; i < lo.up_w.size(); ++i) {
     char p[64];
@@ -202,149 +169,125 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     std::string s(p);
     const int sc = cfg->upsample_scales[i];
     if (cfg->upsample_type == 0) {
-      lo.p_up_k.push_back(add_param(lo, s + "kernel", {3, 3, 1, sc}));
-      lo.p_up_b.push_back(add_param(lo, s + "bias", {sc}));
+      lo.p_up_k.push_back(add_param(lo.params, lo.n_params, s + "kernel", {3, 3, 1, sc}));
+      lo.p_up_b.push_back(add_param(lo.params, lo.n_params, s + "bias", {sc}));
     } else if (cfg->upsample_type == 2) {
-      lo.p_up_k.push_back(add_param(lo, s + "kernel", {1, sc, lo.C, lo.C}));
-      lo.p_up_b.push_back(add_param(lo, s + "bias", {lo.C}));
+      lo.p_up_k.push_back(add_param(lo.params, lo.n_params, s + "kernel", {1, sc, lo.C, lo.C}));
+      lo.p_up_b.push_back(add_param(lo.params, lo.n_params, s + "bias", {lo.C}));
     } else {
-      lo.p_up_k.push_back(add_param(lo, s + "kernel", {3, sc, 1, 1}));
-      lo.p_up_b.push_back(add_param(lo, s + "bias", {1}));
+      lo.p_up_k.push_back(add_param(lo.params, lo.n_params, s + "kernel", {3, sc, 1, 1}));
+      lo.p_up_b.push_back(add_param(lo.params, lo.n_params, s + "bias", {1}));
     }
   }
   // ---- packed ----
-  long long o = 0;
-  auto takeb = [&](long long bytes) { long long r = o; o = align_up(o + bytes, 256); return r; };
+  Arena pk;
   const long long L = lo.L;
   const long long km = lo.split ? 3 : 1;   // split-bf16: every forward K segment becomes [W_hi | W_hi | W_lo]
-  lo.k_Wg = takeb(L * lo.G * lo.Kg * km * 2);
-  lo.k_Wo = takeb(L * lo.R * lo.Gh * km * 2);
-  lo.k_Ws = takeb((long long)lo.S * L * lo.Gh * km * 2);
-  lo.k_Wf1 = takeb((long long)lo.S * lo.S * km * 2);
-  lo.k_Wf2 = takeb((long long)(lo.O < 32 ? 32 : lo.O) * lo.S * km * 2);
-  lo.k_WozT = takeb(L * lo.Gh * (lo.R + lo.S) * 2);
-  lo.k_WdT = takeb(L * lo.R * 3 * lo.G * 2);
-  lo.k_WcT = takeb((long long)(lo.C > 0 ? lo.C : 8) * L * lo.G * 2);
-  lo.k_Wf1T = takeb((long long)lo.S * lo.S * 2);
-  lo.k_Wf2T = takeb((long long)lo.S * lo.Op * 2);
-  lo.k_bias_g = takeb(L * lo.G * 4);
-  lo.k_bias_skip = takeb(lo.S * 4);
-  lo.packed_bytes = o;
+  lo.k_Wg = pk.take(L * lo.G * lo.Kg * km * 2);
+  lo.k_Wo = pk.take(L * lo.R * lo.Gh * km * 2);
+  lo.k_Ws = pk.take((long long)lo.S * L * lo.Gh * km * 2);
+  lo.k_Wf1 = pk.take((long long)lo.S * lo.S * km * 2);
+  lo.k_Wf2 = pk.take((long long)(lo.O < 32 ? 32 : lo.O) * lo.S * km * 2);
+  lo.k_WozT = pk.take(L * lo.Gh * (lo.R + lo.S) * 2);
+  lo.k_WdT = pk.take(L * lo.R * 3 * lo.G * 2);
+  lo.k_WcT = pk.take((long long)(lo.C > 0 ? lo.C : 8) * L * lo.G * 2);
+  lo.k_Wf1T = pk.take((long long)lo.S * lo.S * 2);
+  lo.k_Wf2T = pk.take((long long)lo.S * lo.Op * 2);
+  lo.k_bias_g = pk.take(L * lo.G * 4);
+  lo.k_bias_skip = pk.take(lo.S * 4);
+  lo.packed_bytes = pk.used;
   // ---- workspace ----
-  o = 0;
+  Arena ws;
   const long long BT = (long long)lo.B * lo.T;
-  lo.w_cup = takeb(BT * (lo.split ? 256 : (lo.C > 0 ? lo.C : 8)) * 2);     // split: [hi(C) pad 128 | lo(C) pad 128]
+  lo.w_cup = ws.take(BT * (lo.split ? 256 : (lo.C > 0 ? lo.C : 8)) * 2);     // split: [hi(C) pad 128 | lo(C) pad 128]
   lo.w_upout.clear();
-  for (size_t i = 0; i < lo.up_w.size(); ++i) lo.w_upout.push_back(takeb((long long)lo.B * lo.C * lo.up_w[i] * 4));
-  lo.w_upgrad[0] = takeb(BT * (lo.C > 0 ? lo.C : 8) * 4);
-  lo.w_upgrad[1] = takeb(BT * (lo.C > 0 ? lo.C : 8) * 4);
-  lo.w_x = takeb(L * BT * lo.R * 2 * lo.xm);
-  lo.w_xd = cfg->dropout > 0.f ? takeb(L * BT * lo.R * 2) : lo.w_x;
-  lo.w_ta = takeb(L * BT * lo.Gh * 2);
-  lo.w_sb = takeb(L * BT * lo.Gh * 2);
-  lo.w_z = takeb(L * BT * lo.Gh * 2 * lo.xm);
-  lo.w_h1 = takeb(BT * lo.S * 2 * lo.xm);
-  lo.w_h2 = takeb(BT * lo.S * 2 * lo.xm);
-  lo.w_dlog = takeb(BT * lo.ldo * 2);
-  lo.w_dh2 = takeb(BT * lo.S * 2);
-  lo.w_dskip = takeb(BT * lo.S * 2);
-  lo.w_dxin = takeb(L * BT * lo.R * 2);
-  lo.w_dg = takeb(L * BT * lo.G * 2);
-  lo.w_dcup = takeb(BT * (lo.C > 0 ? lo.C : 8) * 4);
-  lo.w_scalars = takeb(64 * 4);
-  lo.w_skipsum = takeb(lo.S * 8);
-  lo.w_gfx = takeb(lo.n_params * 8);
+  for (size_t i = 0; i < lo.up_w.size(); ++i) lo.w_upout.push_back(ws.take((long long)lo.B * lo.C * lo.up_w[i] * 4));
+  lo.w_upgrad[0] = ws.take(BT * (lo.C > 0 ? lo.C : 8) * 4);
+  lo.w_upgrad[1] = ws.take(BT * (lo.C > 0 ? lo.C : 8) * 4);
+  lo.w_x = ws.take(L * BT * lo.R * 2 * lo.xm);
+  lo.w_xd = cfg->dropout > 0.f ? ws.take(L * BT * lo.R * 2) : lo.w_x;
+  lo.w_ta = ws.take(L * BT * lo.Gh * 2);
+  lo.w_sb = ws.take(L * BT * lo.Gh * 2);
+  lo.w_z = ws.take(L * BT * lo.Gh * 2 * lo.xm);
+  lo.w_h1 = ws.take(BT * lo.S * 2 * lo.xm);
+  lo.w_h2 = ws.take(BT * lo.S * 2 * lo.xm);
+  lo.w_dlog = ws.take(BT * lo.ldo * 2);
+  lo.w_dh2 = ws.take(BT * lo.S * 2);
+  lo.w_dskip = ws.take(BT * lo.S * 2);
+  lo.w_dxin = ws.take(L * BT * lo.R * 2);
+  lo.w_dg = ws.take(L * BT * lo.G * 2);
+  lo.w_dcup = ws.take(BT * (lo.C > 0 ? lo.C : 8) * 4);
+  lo.w_scalars = ws.take(64 * 4);
+  lo.w_skipsum = ws.take(lo.S * 8);
+  lo.w_gfx = ws.take(lo.n_params * 8);
 
   // ---- pack jobs ----
   lo.packjobs.clear();
-  auto pj = [&](long long src, int K, int N, long long dst_bytes, int ld, int transpose, int col0, float scale, int perm) {
-    PackJob j; j.src_off = src; j.K = K; j.N = N; j.dst_off = dst_bytes / 2; j.dst_ld = ld; j.transpose = transpose;
-    j.col0 = col0; j.scale = scale; j.perm_gh = perm; j.part = 0; lo.packjobs.push_back(j);
-  };
-  // split-bf16 forward operand: the K range [col0, col0 + slot) of the plain layout becomes [W_hi | W_hi | W_lo], slot columns each
-  auto pj3 = [&](long long src, int K, int N, long long dst_bytes, int ld, int col_hi, int col_lo, int slot, float scale, int perm) {
-    pj(src, K, N, dst_bytes, ld, 1, col_hi, scale, perm);
-    pj(src, K, N, dst_bytes, ld, 1, col_hi + slot, scale, perm);
-    pj(src, K, N, dst_bytes, ld, 1, col_lo, scale, perm);
-    lo.packjobs.back().part = 2;
-  };
+  std::vector<PackJob>& pj = lo.packjobs;
   for (int l = 0; l < lo.L; ++l) {
     const long long wg = lo.k_Wg + (long long)l * lo.G * lo.Kg * km * 2;
     if (lo.split) {
       const int R = lo.R, Gh = lo.Gh;
-      for (int j = 0; j < 3; ++j) pj3(lo.p_dil_k[l] + (long long)j * R * lo.G, R, lo.G, wg, 3 * lo.Kg, j * 3 * R, j * 3 * R + 2 * R, R, 1.f, Gh);
-      if (lo.C > 0) pj3(lo.p_c_k[l], lo.C, lo.G, wg, 3 * lo.Kg, 9 * R, 9 * R + 256, 128, 1.f, Gh);
-      pj3(lo.p_o_k[l], Gh, R, lo.k_Wo + (long long)l * R * Gh * 3 * 2, 3 * Gh, 0, 2 * Gh, Gh, 1.f, 0);
+      for (int j = 0; j < 3; ++j) add_pack_split(pj, lo.p_dil_k[l] + (long long)j * R * lo.G, R, lo.G, wg, 3 * lo.Kg, j * 3 * R, j * 3 * R + 2 * R, R, 1.f, Gh);
+      if (lo.C > 0) add_pack_split(pj, lo.p_c_k[l], lo.C, lo.G, wg, 3 * lo.Kg, 9 * R, 9 * R + 256, 128, 1.f, Gh);
+      add_pack_split(pj, lo.p_o_k[l], Gh, R, lo.k_Wo + (long long)l * R * Gh * 3 * 2, 3 * Gh, 0, 2 * Gh, Gh);
       // skip GEMM: K runs over [all layers: hi | hi] then [all layers: lo]
-      pj3(lo.p_s_k[l], Gh, lo.S, lo.k_Ws, 3 * lo.L * Gh, l * 2 * Gh, 2 * lo.L * Gh + l * Gh, Gh, lo.skip_scale[l], 0);
+      add_pack_split(pj, lo.p_s_k[l], Gh, lo.S, lo.k_Ws, 3 * lo.L * Gh, l * 2 * Gh, 2 * lo.L * Gh + l * Gh, Gh, lo.skip_scale[l]);
     } else {
-    for (int j = 0; j < 3; ++j) pj(lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, 1, j * lo.R, 1.f, lo.Gh);
-    if (lo.C > 0) pj(lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, 1, 3 * lo.R, 1.f, lo.Gh);
-    pj(lo.p_o_k[l], lo.Gh, lo.R, lo.k_Wo + (long long)l * lo.R * lo.Gh * 2, lo.Gh, 1, 0, 1.f, 0);
-    pj(lo.p_s_k[l], lo.Gh, lo.S, lo.k_Ws, lo.L * lo.Gh, 1, l * lo.Gh, lo.skip_scale[l], 0);
+    for (int j = 0; j < 3; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, 1, j * lo.R, 1.f, lo.Gh);
+    if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, 1, 3 * lo.R, 1.f, lo.Gh);
+    add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, lo.k_Wo + (long long)l * lo.R * lo.Gh * 2, lo.Gh, 1, 0);
+    add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, lo.k_Ws, lo.L * lo.Gh, 1, l * lo.Gh, lo.skip_scale[l]);
     }
     const long long woz = lo.k_WozT + (long long)l * lo.Gh * (lo.R + lo.S) * 2;
-    pj(lo.p_o_k[l], lo.Gh, lo.R, woz, lo.R + lo.S, 0, 0, lo.res_scale, 0);
-    pj(lo.p_s_k[l], lo.Gh, lo.S, woz, lo.R + lo.S, 0, lo.R, lo.skip_scale[l], 0);
+    add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, woz, lo.R + lo.S, 0, 0, lo.res_scale);
+    add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, woz, lo.R + lo.S, 0, lo.R, lo.skip_scale[l]);
     const long long wd = lo.k_WdT + (long long)l * lo.R * 3 * lo.G * 2;
-    for (int j = 0; j < 3; ++j) pj(lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wd, 3 * lo.G, 0, j * lo.G, 1.f, 0);
-    if (lo.C > 0) pj(lo.p_c_k[l], lo.C, lo.G, lo.k_WcT, lo.L * lo.G, 0, l * lo.G, 1.f, 0);
+    for (int j = 0; j < 3; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wd, 3 * lo.G, 0, j * lo.G);
+    if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, lo.k_WcT, lo.L * lo.G, 0, l * lo.G);
   }
   if (lo.split) {
-    pj3(lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, 3 * lo.S, 0, 2 * lo.S, lo.S, 1.f, 0);
-    pj3(lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, 3 * lo.S, 0, 2 * lo.S, lo.S, 1.f, 0);
+    add_pack_split(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, 3 * lo.S, 0, 2 * lo.S, lo.S);
+    add_pack_split(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, 3 * lo.S, 0, 2 * lo.S, lo.S);
   } else {
-    pj(lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, lo.S, 1, 0, 1.f, 0);
-    pj(lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, lo.S, 1, 0, 1.f, 0);
+    add_pack(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, lo.S, 1, 0);
+    add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, lo.S, 1, 0);
   }
-  pj(lo.p_f1_k, lo.S, lo.S, lo.k_Wf1T, lo.S, 0, 0, 1.f, 0);
-  pj(lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 0, 1.f, 0);
-  if (!lo.mol) pj(lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 256, 1.f, 0);
+  add_pack(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1T, lo.S, 0, 0);
+  add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 0);
+  if (!lo.mol) add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 256);
   lo.n_packjobs = int(lo.packjobs.size());
 
   // ---- wgrad tiles ----
   // main maps: 0 xd_all, 1 dg_all, 2 c_up, 3 z_all, 4 dxin_all, 5 dskip
   lo.tiles_main.clear();
-  auto wt = [&](std::vector<WgradTile>& v, int am, int ach, int ash, int al, int bm, int bch, int bl, long long off,
-                int ldc, int mv, int nv, float scale, const float* div) {
+  auto proto = [](int am, int ash, int al, int bm, int bl, float scale) {
     WgradTile t; memset(&t, 0, sizeof(t));
-    t.a_map = am; t.a_ch0 = ach; t.a_shift = ash; t.a_layer = al; t.b_map = bm; t.b_ch0 = bch; t.b_shift = 0; t.b_layer = bl;
-    t.out_off = off; t.ldc = ldc; t.m_valid = mv; t.n_valid = nv; t.scale = scale; t.accumulate = 0; t.div = div;
-    v.push_back(t);
+    t.a_map = am; t.a_shift = ash; t.a_layer = al; t.b_map = bm; t.b_layer = bl; t.scale = scale;
+    return t;
   };
-  const int WN = 256;   // output columns per weight-gradient tile (wgrad_gemm_kernel: kWgBN)
-  auto nmin = [&](int rem) { return rem < WN ? rem : WN; };
   lo.tile_start.assign(lo.L + 1, 0);
   for (int l = 0; l < lo.L; ++l) {
     const int d = lo.dil(l);
     lo.tile_start[l] = int(lo.tiles_main.size());
     for (int j = 0; j < 3; ++j)
-      for (int m0 = 0; m0 < lo.R; m0 += 128)
-        for (int n0 = 0; n0 < lo.G; n0 += WN)
-          wt(lo.tiles_main, 0, m0, -(2 - j) * d, l, 1, n0, l, lo.p_dil_k[l] + (long long)j * lo.R * lo.G + (long long)m0 * lo.G + n0,
-             lo.G, 128, nmin(lo.G - n0), 1.f, nullptr);
-    if (lo.C > 0)
-      for (int n0 = 0; n0 < lo.G; n0 += WN)
-        wt(lo.tiles_main, 2, 0, 0, 0, 1, n0, l, lo.p_c_k[l] + n0, lo.G, lo.C, nmin(lo.G - n0), 1.f, nullptr);
-    for (int m0 = 0; m0 < lo.Gh; m0 += 128) {
+      append_wgrad_tiles(lo.tiles_main, proto(0, -(2 - j) * d, l, 1, l, 1.f), 0, lo.R, 0, lo.G, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.G);
+    if (lo.C > 0) append_wgrad_tiles(lo.tiles_main, proto(2, 0, 0, 1, l, 1.f), 0, lo.C, 0, lo.G, lo.p_c_k[l], lo.G);
+    for (int m0 = 0; m0 < lo.Gh; m0 += 128) {   // out and skip tiles of one row block side by side
       if (l < lo.L - 1)
-        for (int n0 = 0; n0 < lo.R; n0 += WN)
-          wt(lo.tiles_main, 3, m0, 0, l, 4, n0, l + 1, lo.p_o_k[l] + (long long)m0 * lo.R + n0, lo.R, 128, nmin(lo.R - n0), lo.res_scale, nullptr);
-      for (int n0 = 0; n0 < lo.S; n0 += WN)
-        wt(lo.tiles_main, 3, m0, 0, l, 5, n0, 0, lo.p_s_k[l] + (long long)m0 * lo.S + n0, lo.S, 128, nmin(lo.S - n0), lo.skip_scale[l], nullptr);
+        append_wgrad_tiles(lo.tiles_main, proto(3, 0, l, 4, l + 1, lo.res_scale), m0, 128, 0, lo.R, lo.p_o_k[l] + (long long)m0 * lo.R, lo.R);
+      append_wgrad_tiles(lo.tiles_main, proto(3, 0, l, 5, 0, lo.skip_scale[l]), m0, 128, 0, lo.S, lo.p_s_k[l] + (long long)m0 * lo.S, lo.S);
     }
   }
   // head maps: 0 h1, 1 dh2, 2 h2, 3 dlog
   lo.tiles_head.clear();
+  WgradTile f2 = proto(2, 0, 0, 3, 0, 1.f);
+  f2.accumulate = 2;                                   // CE: hi and lo halves of dlog both accumulate (atomics)
+  f2.div = reinterpret_cast<const float*>(1);          // patched to scalars[1] at init
   for (int m0 = 0; m0 < lo.S; m0 += 128) {
-    for (int n0 = 0; n0 < lo.S; n0 += WN)
-      wt(lo.tiles_head, 0, m0, 0, 0, 1, n0, 0, lo.p_f1_k + (long long)m0 * lo.S + n0, lo.S, 128, nmin(lo.S - n0), 1.f, nullptr);
-    for (int n0 = 0; n0 < lo.O; n0 += WN)
-      for (int part = 0; part < (lo.mol ? 1 : 2); ++part) {  // CE: hi and lo halves of dlog both accumulate (atomics)
-        wt(lo.tiles_head, 2, m0, 0, 0, 3, part * 256 + n0, 0, lo.p_f2_k + (long long)m0 * lo.O + n0, lo.O, 128,
-           nmin(lo.O - n0), 1.f, reinterpret_cast<const float*>(1) /* patched to scalars[1] at init */);
-        lo.tiles_head.back().accumulate = 2;
-      }
+    append_wgrad_tiles(lo.tiles_head, proto(0, 0, 0, 1, 0, 1.f), m0, 128, 0, lo.S, lo.p_f1_k + (long long)m0 * lo.S, lo.S);
+    for (int part = 0; part < (lo.mol ? 1 : 2); ++part)   // O <= 256: one column block per part
+      append_wgrad_tiles(lo.tiles_head, f2, m0, 128, part * 256, lo.O, lo.p_f2_k + (long long)m0 * lo.O, lo.O);
   }
   lo.n_tiles_main = int(lo.tiles_main.size());
   lo.tile_start[lo.L] = lo.n_tiles_main;
@@ -361,76 +304,24 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   if (!lo.mol) cs(lo.w_dlog + 256 * 2, BT, lo.O, lo.ldo, lo.p_f2_b, -1, 1.f, 1);
   lo.n_colsum = int(lo.colsums.size());
 
-  lo.w_tiles_main = takeb((long long)lo.n_tiles_main * sizeof(WgradTile));
-  lo.w_tiles_head = takeb((long long)lo.n_tiles_head * sizeof(WgradTile));
-  lo.w_packjobs = takeb((long long)lo.n_packjobs * sizeof(PackJob));
-  lo.w_colsum = takeb((long long)lo.n_colsum * sizeof(ColsumJob));
-  lo.w_tables = takeb((long long)lo.L * (3 * sizeof(long long) + sizeof(float)));
+  lo.w_tiles_main = ws.take((long long)lo.n_tiles_main * sizeof(WgradTile));
+  lo.w_tiles_head = ws.take((long long)lo.n_tiles_head * sizeof(WgradTile));
+  lo.w_packjobs = ws.take((long long)lo.n_packjobs * sizeof(PackJob));
+  lo.w_colsum = ws.take((long long)lo.n_colsum * sizeof(ColsumJob));
+  lo.w_tables = ws.take((long long)lo.L * (3 * sizeof(long long) + sizeof(float)));
   lo.w_spk = lo.w_gbias = lo.w_gsum = -1;
   if (lo.Gi > 0) {
-    lo.w_spk = takeb((1LL + lo.B) * 4);
-    lo.w_gbias = takeb(L * lo.B * lo.G * 4);
-    lo.w_gsum = takeb(L * lo.B * lo.G * 8);
+    lo.w_spk = ws.take((1LL + lo.B) * 4);
+    lo.w_gbias = ws.take(L * lo.B * lo.G * 4);
+    lo.w_gsum = ws.take(L * lo.B * lo.G * 8);
   }
-  lo.workspace_bytes = o;
+  lo.workspace_bytes = ws.used;
   return T2_OK;
 }
 
 // ------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------
-__global__ void pack_kernel(const float* __restrict__ params, bf16* __restrict__ packed, const PackJob* __restrict__ jobs) {
-  // 64x64 tiles through shared memory: float2 reads along the source's fast axis (N), bf16x2 writes along the
-  // destination's fast axis (K for the transposing jobs). All offsets / leading dimensions in the job table are even.
-  __shared__ float tile[64][65];
-  const PackJob j = jobs[blockIdx.y];
-  const int tiles_n = (j.N + 63) / 64, tiles_k = (j.K + 63) / 64;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  const bool vec_src = ((j.N | int(j.src_off)) & 1) == 0;
-  const bool vec_dst = ((j.dst_ld | j.col0 | int(j.dst_off)) & 1) == 0;
-  for (int ti = blockIdx.x; ti < tiles_n * tiles_k; ti += gridDim.x) {
-    const int k0 = (ti / tiles_n) * 64, n0 = (ti % tiles_n) * 64;
-    for (int r = ty; r < 64; r += 8) {
-      const int k = k0 + r, n = n0 + 2 * tx;
-      float a = 0.f, b = 0.f;
-      if (k < j.K) {
-        const float* src = params + j.src_off + (long long)k * j.N + n;
-        if (vec_src && n + 1 < j.N) { const float2 v = *reinterpret_cast<const float2*>(src); a = v.x; b = v.y; }
-        else { if (n < j.N) a = src[0]; if (n + 1 < j.N) b = src[1]; }
-      }
-      a *= j.scale; b *= j.scale;
-      if (j.part == 2) { a -= __bfloat162float(__float2bfloat16(a)); b -= __bfloat162float(__float2bfloat16(b)); }
-      tile[r][2 * tx] = a; tile[r][2 * tx + 1] = b;
-    }
-    __syncthreads();
-    if (j.transpose) {
-      for (int r = ty; r < 64; r += 8) {
-        const int n = n0 + r, k = k0 + 2 * tx;
-        if (n < j.N && k < j.K) {
-          int row = n;
-          if (j.perm_gh > 0) {
-            const int half = n / j.perm_gh, idx = n % j.perm_gh;
-            row = (idx / 128) * 256 + half * 128 + (idx % 128);
-          }
-          bf16* dst = packed + j.dst_off + (long long)row * j.dst_ld + j.col0 + k;
-          if (vec_dst && k + 1 < j.K) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(tile[2 * tx][r], tile[2 * tx + 1][r]);
-          else { dst[0] = __float2bfloat16(tile[2 * tx][r]); if (k + 1 < j.K) dst[1] = __float2bfloat16(tile[2 * tx + 1][r]); }
-        }
-      }
-    } else {
-      for (int r = ty; r < 64; r += 8) {
-        const int k = k0 + r, n = n0 + 2 * tx;
-        if (n < j.N && k < j.K) {
-          bf16* dst = packed + j.dst_off + (long long)k * j.dst_ld + j.col0 + n;
-          if (vec_dst && n + 1 < j.N) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(tile[r][2 * tx], tile[r][2 * tx + 1]);
-          else { dst[0] = __float2bfloat16(tile[r][2 * tx]); if (n + 1 < j.N) dst[1] = __float2bfloat16(tile[r][2 * tx + 1]); }
-        }
-      }
-    }
-    __syncthreads();
-  }
-}
-
 // bias_g[l][g] = b_dil + b_cin ; bias_skip[s] = sum_l scale_l * b_skip_l[s]
 struct DerivedArgs {
   const float* params;
@@ -1070,10 +961,6 @@ __global__ void fx_finalize_kernel(const long long* __restrict__ acc, float* __r
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e < n && acc[e] != 0) grads[e] += fx_value(acc[e]);
 }
-__global__ void f32_to_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < n) out[e] = __float2bfloat16(in[e]);
-}
 
 // the per-layer gate GEMM: [x(t-2d) | x(t-d) | x(t) | c(t)] x Wg with the tanh*sigmoid epilogue
 ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l, bool save) {
@@ -1199,8 +1086,6 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
   return g;
 }
 
-inline dim3 grid1d(long long n, int block = 256) { return dim3((unsigned)((n + block - 1) / block)); }
-
 // One layer of the conditioning upsampler (type 0 SubPixel, 1 ConvTranspose2D, 2 ConvTranspose1D; in [B][C][W], out [B][C][W*s]):
 // the launches of the training forward / backward, AR synthesis and t2_dbg_wn_kernel.
 int up1d_smem_limit(const void* fn, size_t smem) {
@@ -1295,13 +1180,7 @@ extern "C" int t2_wn_param_info(const t2_wn_config_t* cfg, int i, char* name, in
   Layout lo;
   int rc = build_layout(cfg, lo);
   if (rc) return rc;
-  T2_REQUIRE(i >= 0 && i < int(lo.params.size()), T2_ERR_INVALID_ARG, "tensor index %d out of range", i);
-  const ParamT& p = lo.params[i];
-  snprintf(name, name_cap, "%s", p.name.c_str());
-  *offset = p.off;
-  *ndim = p.ndim;
-  for (int k = 0; k < 4; ++k) shape4[k] = p.shape[k];
-  return T2_OK;
+  return param_info(lo.params, i, name, name_cap, offset, ndim, shape4, nullptr);
 }
 
 extern "C" int t2_wn_init(const t2_wn_config_t* cfg, void* d_packed, void* d_workspace, void* stream) {
@@ -1340,9 +1219,8 @@ extern "C" int t2_wn_pack_weights(const t2_wn_config_t* cfg, const float* d_para
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   uint8_t* pk = static_cast<uint8_t*>(d_packed);
-  pack_kernel<<<dim3(16, lo.n_packjobs), dim3(32, 8), 0, st>>>(d_params, reinterpret_cast<bf16*>(pk),
-                                                       reinterpret_cast<const PackJob*>(ws + lo.w_packjobs)); t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
+  rc = launch_pack(d_params, pk, reinterpret_cast<const PackJob*>(ws + lo.w_packjobs), lo.n_packjobs, 128, 16, st);
+  if (rc) return rc;
   long long* d_offs = reinterpret_cast<long long*>(ws + lo.w_tables);
   float* d_scales = reinterpret_cast<float*>(ws + lo.w_tables + 3 * lo.L * sizeof(long long));
   DerivedArgs a;
@@ -1385,7 +1263,7 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   if (lo.C > 0) {
     T2_REQUIRE(d_c != nullptr, T2_ERR_INVALID_ARG, "local conditioning enabled but d_c is NULL");
     if (cfg->c_pre_upsampled) {
-      f32_to_bf16_kernel<<<grid1d(BT * lo.C), 256, 0, st>>>(d_c, c_up, BT * lo.C); t2_count_launch();
+      launch_f32_to_bf16(d_c, c_up, BT * lo.C, st);
     } else {
       const float* in = d_c;
       int W = lo.Tc;
@@ -1481,24 +1359,6 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   }
   if (d_loss) T2_CHECK_CUDA(cudaMemcpyAsync(d_loss, scalars, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return T2_OK;
-}
-
-// side stream + fork/join events for the independent tail of the backward pass (created once per process; T2_SIDE_STREAM=0
-// in the environment keeps everything on the caller's stream)
-struct SideStream { cudaStream_t s; cudaEvent_t fork, fork2, join; };
-static SideStream* side_stream() {
-  static SideStream ss;
-  static int state = 0;   // 0 unknown, 1 ready, -1 disabled
-  if (state == 0) {
-    const char* e = getenv("T2_SIDE_STREAM");
-    if (e && e[0] == '0') state = -1;
-    else if (cudaStreamCreateWithFlags(&ss.s, cudaStreamNonBlocking) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ss.fork, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ss.fork2, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&ss.join, cudaEventDisableTiming) == cudaSuccess) state = 1;
-    else state = -1;
-  }
-  return state == 1 ? &ss : nullptr;
 }
 
 extern "C" int t2_wn_backward(const t2_wn_config_t* cfg, const float* d_params, const void* d_packed,
@@ -1881,16 +1741,15 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
     off += s;
   }
   a.ring_slots_total = off;
-  long long o = 0;
-  auto takeb = [&](long long bytes) { long long r = o; o = align_up(o + bytes, 256); return r; };
+  Arena ws;
   const long long BT = (long long)lo.B * lo.T;
-  a.w_cup = takeb(BT * (lo.C > 0 ? lo.C : 8) * 2);
-  a.w_upout_base = o;
-  for (size_t i = 0; i < lo.up_w.size(); ++i) takeb((long long)lo.B * lo.C * lo.up_w[i] * 4);
-  a.w_ring = takeb((long long)lo.B * off * lo.R * 4);
-  a.w_ringoff = takeb(2LL * lo.L * 4);
-  a.w_gbias = lo.Gi > 0 ? takeb((long long)lo.B * lo.L * lo.G * 4) : -1;
-  a.workspace_bytes = o;
+  a.w_cup = ws.take(BT * (lo.C > 0 ? lo.C : 8) * 2);
+  a.w_upout_base = ws.used;
+  for (size_t i = 0; i < lo.up_w.size(); ++i) ws.take((long long)lo.B * lo.C * lo.up_w[i] * 4);
+  a.w_ring = ws.take((long long)lo.B * off * lo.R * 4);
+  a.w_ringoff = ws.take(2LL * lo.L * 4);
+  a.w_gbias = lo.Gi > 0 ? ws.take((long long)lo.B * lo.L * lo.G * 4) : -1;
+  a.workspace_bytes = ws.used;
   return T2_OK;
 }
 
@@ -2427,7 +2286,7 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
   // conditioning -> c_up (bf16 channels-last), same kernels as the training path
   bf16* c_up = reinterpret_cast<bf16*>(ws + al.w_cup);
   if (cfg->c_pre_upsampled) {
-    f32_to_bf16_kernel<<<grid1d(BT * lo.C), 256, 0, st>>>(d_c, c_up, BT * lo.C); t2_count_launch();
+    launch_f32_to_bf16(d_c, c_up, BT * lo.C, st);
   } else {
     const float* in = d_c;
     int W = lo.Tc;

@@ -40,6 +40,20 @@ def ptr(t):
     return ctypes.c_void_p(t.data_ptr())
 
 
+def param_table(info, cfg, n_tensors, trainable=True, base=0):
+    """[(name, offset, shape, trainable)] of an engine's flat parameter buffer from its t2_*_param_info function (host-only: no CUDA
+    device needed). trainable=False for an info function without the trainable out-parameter (WaveNet): [(name, offset, shape)].
+    base is added to every offset."""
+    name = ctypes.create_string_buffer(160)
+    off, nd, shp, tr = ctypes.c_longlong(), ctypes.c_int(), (ctypes.c_int * 4)(), ctypes.c_int()
+    out = []
+    for i in range(n_tensors):
+        check(info(ctypes.byref(cfg), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp, *((ctypes.byref(tr),) if trainable else ())))
+        t = (name.value.decode(), base + off.value, tuple(shp[k] for k in range(nd.value)))
+        out.append(t + (bool(tr.value),) if trainable else t)
+    return out
+
+
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)

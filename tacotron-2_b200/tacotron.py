@@ -123,6 +123,7 @@ class Tacotron(object):
         n, pb, wb, nt = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_int()
         L.check(self.lib.t2_taco_sizes(ctypes.byref(self.cfg), ctypes.byref(n), ctypes.byref(pb), ctypes.byref(wb), ctypes.byref(nt)))
         self.n_taco = n.value
+        self.tensors = L.param_table(self.lib.t2_taco_param_info, self.cfg, nt.value)
         self.cbhg = None
         n_cb = 0
         if getattr(hparams, "predict_linear", False):       # CBHG + linear head: a second engine chained on mel_outputs (include/t2b200.h)
@@ -136,23 +137,13 @@ class Tacotron(object):
             self.cb_workspace = torch.empty(cwb.value, dtype=torch.uint8, device=self.device)
             self.cb_loss = torch.zeros(2, dtype=torch.float32, device=self.device)
             self.cb_dmel = torch.zeros(B * T_out * hparams.num_mels, dtype=torch.float32, device=self.device)
-            self._cb_ntensors = cnt.value
+            self.tensors += L.param_table(self.lib.t2_cbhg_param_info, self.cbhg, cnt.value, base=self.n_taco)
         self.n_params = n.value + n_cb
         self.params = torch.zeros(self.n_params, dtype=torch.float32, device=self.device)
         self.packed = torch.empty(pb.value, dtype=torch.uint8, device=self.device)
         self.workspace = torch.empty(wb.value, dtype=torch.uint8, device=self.device)
         self.loss_buf = torch.zeros(4, dtype=torch.float32, device=self.device)
         self.grads = self.m = self.v = None
-        self.tensors = []
-        name = ctypes.create_string_buffer(160)
-        off, nd, shp, tr = ctypes.c_longlong(), ctypes.c_int(), (ctypes.c_int * 4)(), ctypes.c_int()
-        for i in range(nt.value):
-            L.check(self.lib.t2_taco_param_info(ctypes.byref(self.cfg), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp, ctypes.byref(tr)))
-            self.tensors.append((name.value.decode(), off.value, tuple(shp[k] for k in range(nd.value)), bool(tr.value)))
-        if self.cbhg is not None:
-            for i in range(self._cb_ntensors):
-                L.check(self.lib.t2_cbhg_param_info(ctypes.byref(self.cbhg), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp, ctypes.byref(tr)))
-                self.tensors.append((name.value.decode(), self.n_taco + off.value, tuple(shp[k] for k in range(nd.value)), bool(tr.value)))
         self.offsets = torch.tensor([t[1] for t in self.tensors] + [self.n_params], dtype=torch.int64, device=self.device)
         self.opt_scratch = torch.zeros(len(self.tensors) + 2, dtype=torch.float32, device=self.device)
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device)

@@ -126,13 +126,7 @@ def param_table(cfg):
     lib = L.load()
     sz = WnSizes()
     L.check(lib.t2_wn_sizes(ctypes.byref(cfg), ctypes.byref(sz)))
-    name = ctypes.create_string_buffer(160)
-    off, nd, shp = ctypes.c_longlong(), ctypes.c_int(), (ctypes.c_int * 4)()
-    out = []
-    for i in range(sz.n_tensors):
-        L.check(lib.t2_wn_param_info(ctypes.byref(cfg), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp))
-        out.append((name.value.decode(), off.value, tuple(shp[k] for k in range(nd.value))))
-    return out, sz.n_params
+    return L.param_table(lib.t2_wn_param_info, cfg, sz.n_tensors, trainable=False), sz.n_params
 
 
 def grad_buckets(tensors, n_layers, n_params, n_groups):
@@ -193,15 +187,7 @@ class WaveNet(object):
         self.workspace = torch.empty(sz.workspace_bytes, dtype=torch.uint8, device=self.device)
         self.loss_buf = torch.zeros(2, dtype=torch.float32, device=self.device)
         self.grads = self.m = self.v = self.ema = None
-        self.tensors = []  # (name, offset, shape)
-        name = ctypes.create_string_buffer(160)
-        off = ctypes.c_longlong()
-        nd = ctypes.c_int()
-        shp = (ctypes.c_int * 4)()
-        for i in range(sz.n_tensors):
-            L.check(self.lib.t2_wn_param_info(ctypes.byref(self.cfg), i, name, 160, ctypes.byref(off),
-                                              ctypes.byref(nd), shp))
-            self.tensors.append((name.value.decode(), off.value, tuple(shp[k] for k in range(nd.value))))
+        self.tensors = L.param_table(self.lib.t2_wn_param_info, self.cfg, sz.n_tensors, trainable=False)  # (name, offset, shape)
         offs = [t[1] for t in self.tensors] + [sz.n_params]
         self.offsets = torch.tensor(offs, dtype=torch.int64, device=self.device)
         self.opt_scratch = torch.zeros(sz.n_tensors + 2, dtype=torch.float32, device=self.device)
@@ -467,12 +453,7 @@ class WaveNetSynthesizer(object):
         self.packed = torch.empty(pb.value, dtype=torch.uint8, device=self.device)
         self.workspace = torch.zeros(wb.value, dtype=torch.uint8, device=self.device)
         self._spk = torch.zeros(B, dtype=torch.int32, device=self.device) if self.cfg.gin_channels > 0 else None
-        self.tensors = []
-        name = ctypes.create_string_buffer(160)
-        off, nd, shp = ctypes.c_longlong(), ctypes.c_int(), (ctypes.c_int * 4)()
-        for i in range(sz.n_tensors):
-            L.check(self.lib.t2_wn_param_info(ctypes.byref(self.cfg), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp))
-            self.tensors.append((name.value.decode(), off.value, tuple(shp[k] for k in range(nd.value))))
+        self.tensors = L.param_table(self.lib.t2_wn_param_info, self.cfg, sz.n_tensors, trainable=False)
 
     def load_params(self, params):
         flat = torch.zeros(self.n_params, dtype=torch.float32)

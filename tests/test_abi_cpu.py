@@ -66,6 +66,13 @@ def test_layout_queries_match_the_oracle_parameter_tables():
         t2.lib.check(lib.t2_taco_param_info(ctypes.byref(tc), i, name, 160, ctypes.byref(off), ctypes.byref(nd), shp, ctypes.byref(tr)))
         got.append((name.value.decode(), tuple(shp[k] for k in range(nd.value)), bool(tr.value)))
     assert got == [(k, tuple(v), ot.is_trainable(k)) for k, v in ot.param_shapes(hp2).items()]
+    hp3 = hparams.copy()
+    hp3.set_hparam("predict_linear", True)
+    cc = t2.tacotron.make_cbhg_config(hp3, 4, 80, 0.0)
+    t2.lib.check(lib.t2_cbhg_sizes(ctypes.byref(cc), None, None, None, ctypes.byref(nt)))
+    got = [(k, shape, trainable) for k, _, shape, trainable in t2.lib.param_table(lib.t2_cbhg_param_info, cc, nt.value)]
+    cbhg = list(ot.param_shapes(hp3).items())[len(ot.param_shapes(hp2)):]
+    assert len(cbhg) > 0 and got == [(k, tuple(v), ot.is_trainable(k)) for k, v in cbhg]
 
 
 def test_product_path_has_no_oracle_import():
