@@ -242,6 +242,16 @@ int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_params, cons
  * Synchronises. */
 int t2_wn_time_kernel(const t2_wn_config_t* cfg, const float* d_params, const void* d_packed, void* d_workspace,
                       int which, int layer, int reps, float* ms_per_launch, void* stream);
+/* The forward gate / out GEMMs of every residual layer can run as ONE persistent launch, and so can the backward dz / dx GEMMs:
+ * tiles wait for the neighbour tiles they read instead of for whole launches. By default (mode 0) they do where a layer's gate
+ * GEMM is at most two waves of CTAs; mode 1 makes the following calls launch them per layer (the reference the chains are compared
+ * with bit for bit), mode 2 always uses the chains. */
+int t2_dbg_wn_per_layer(int mode);
+/* The work tickets of a persistent chain (dir 0 forward, 1 backward), in the order CTAs take them: 8 ints per ticket
+ * {kind (0 gate / dz, 1 out / dx), layer, M tile over all items, N tile, first and last counter waited for, count awaited,
+ * counter completed}, counter of (kind, layer, M tile m) = (kind * layers + layer) * M tiles + m. out == NULL: count only.
+ * Host only. Returns the ticket count. */
+int t2_dbg_wn_chain(const t2_wn_config_t* cfg, int dir, int* out, int cap);
 /* debug / test access to workspace tensors by name ("x", "z", "c_up", "h1", "dg", ...): returns device pointer,
  * element count and element size */
 int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspace, const char* name, void** ptr,

@@ -150,7 +150,7 @@ static int launch_one(const GemmArgs& g, dim3 grid, int cs, cudaStream_t stream)
   return T2_OK;
 }
 
-int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used) {
+int make_gemm_args(int epi, int BN, const ActGemmCall& c, GemmArgs& g, dim3& grid, int& cs) {
   // argument checks first: they touch neither the device nor the driver
   T2_REQUIRE(c.na >= 1 && c.na <= 4 && c.nseg >= 1 && c.nseg <= kMaxSeg, T2_ERR_INVALID_ARG,
              "act_gemm: bad map/segment count (%d, %d)", c.na, c.nseg);
@@ -173,14 +173,13 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, 
                "act_gemm: split-K needs atomic accumulation (mode 2) into every destination in use (modes %d, %d)", c.epi.i[2],
                c.epi.i[5]);
   }
-  GemmArgs g;
   memset(&g, 0, sizeof(g));
   for (int i = 0; i < 4; ++i) {
     int rc = encode_act_map(&g.amap[i], c.a[i < c.na ? i : 0], kBM);
     if (rc) return rc;
   }
-  dim3 grid((c.T + kBM - 1) / kBM * c.B, c.n_tiles, c.ksplit > 1 ? c.ksplit : 1);
-  const int cs = pick_cluster(BN, grid, c.cluster);
+  grid = dim3((c.T + kBM - 1) / kBM * c.B, c.n_tiles, c.ksplit > 1 ? c.ksplit : 1);
+  cs = pick_cluster(BN, grid, c.cluster);
   // weight-tile rows one TMA box fetches: 1/cs of the tile per CTA of a multicast cluster
   int rc = encode_wt_map(&g.bmap, c.w, c.wN, c.wK, c.wL, BN / cs);
   if (rc) return rc;
@@ -206,6 +205,21 @@ int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, 
         if (rc) return rc;
       }
   }
+  return T2_OK;
+}
+
+long long* take_timing_slice(long long n_slots) {
+  long long* p = g_timing_buffer;
+  if (p) g_timing_buffer = p + n_slots;
+  return p;
+}
+
+int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used) {
+  GemmArgs g;
+  dim3 grid;
+  int cs = 1;
+  const int rc = make_gemm_args(epi, BN, c, g, grid, cs);
+  if (rc) return rc;
   if (cluster_used) *cluster_used = cs;
 #define T2_CASE(E, N) \
   if (epi == E && BN == N) return launch_one<E, N>(g, grid, cs, stream);
@@ -272,6 +286,145 @@ void append_wgrad_tiles(std::vector<WgradTile>& v, const WgradTile& proto, int a
       t.scale = proto.scale; t.accumulate = proto.accumulate; t.div = proto.div;
       v.push_back(t);
     }
+}
+
+// ------------------------------------------------------------------------------------------------------
+// Persistent layer chains: the gate/out GEMMs of every forward layer (or the dz/dx GEMMs of every backward layer) as ONE launch.
+// Each CTA takes tickets (ChainTicket; t2_wavenet.cu build_chain) from a global counter in launch order and runs the same tile body as act_gemm_kernel on
+// the GemmArgs of that (kind, layer), so every tile computes exactly what its per-layer launch computes. A ticket waits only for
+// the neighbour tiles it reads, not for the whole previous GEMM. Progress does not rely on co-residency: a CTA holds one ticket
+// at a time and waits only for tickets handed out before its own, all held by running CTAs, so the lowest unfinished ticket can
+// always run.
+// ------------------------------------------------------------------------------------------------------
+constexpr long long kChainTimeoutNs = 1000000000LL;
+
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// orders generic-proxy accesses (the counters) with async-proxy (TMA) accesses of global memory
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// the stage barriers of ActGemmCfg<BN> (full: 1 arrival, empty: one per consumer warp), as act_gemm_kernel sets them up
+template <int BN>
+__device__ __forceinline__ void chain_init_barriers(uint8_t* smem) {
+  using Cfg = ActGemmCfg<BN>;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
+  for (int i = 0; i < Cfg::kStages; ++i) {
+    mbar_init(&full_bar[i], 1);
+    mbar_init(&full_bar[Cfg::kStages + i], kActEpiWarps);
+  }
+  fence_barrier_init();
+}
+// the previous ticket's barriers are invalidated before their memory is initialised again (the two GEMMs of a chain may place
+// them differently: 4 stages at BN 256, 6 at BN 128)
+template <int BN>
+__device__ __forceinline__ void chain_inval_barriers(uint8_t* smem) {
+  using Cfg = ActGemmCfg<BN>;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
+  for (int i = 0; i < 2 * Cfg::kStages; ++i)
+    asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[i])) : "memory");
+}
+
+// FWD: kind 0 = EPI_GATE (BN 256), kind 1 = EPI_RES (BN1 = R); backward: kind 0 = EPI_GATE_BWD (BN0), kind 1 = EPI_DX (BN1 = R)
+template <bool FWD, int BN0, int BN1>
+__global__ void __launch_bounds__(kActGemmThreads, 1) wn_chain_kernel(const __grid_constant__ ChainArgs a) {
+  constexpr int E0 = FWD ? EPI_GATE : EPI_GATE_BWD, E1 = FWD ? EPI_RES : EPI_DX;
+  using C0 = ActGemmCfg<BN0>;
+  using C1 = ActGemmCfg<BN1>;
+  static_assert(C0::kPipeBytes == C1::kPipeBytes && C0::kEpiBytes == C1::kEpiBytes && C0::kSmemBytes == C1::kSmemBytes,
+                "both GEMMs of a chain share one shared-memory plan");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  __shared__ EpiArgs s_epi;    // the ticket's epilogue arguments with the per-call values filled in
+  __shared__ int s_ticket;
+  int* done = a.ctr + 16;
+  int* stop = a.ctr + 1;       // set once a wait of this launch timed out: the remaining tickets are skipped
+  int prev_kind = -1;          // thread 0: the kind whose barriers are initialised
+  for (;;) {
+    if (threadIdx.x == 0) {
+      int t = atomicAdd(a.ctr, 1);
+      if (t < a.n_tix && *reinterpret_cast<volatile int*>(stop) == 0) {
+        long long* dbg = a.dbg ? a.dbg + size_t(t) * kDbgSlots : nullptr;
+        const long long t_start = globaltimer_ns();
+        if (dbg) { dbg[0] = t_start; dbg[3] = smid(); }
+        const ChainTicket k = a.tix[t];
+        for (int i = k.dep_lo; i <= k.dep_hi && t < a.n_tix; ++i)
+          while (ld_acquire_gpu(done + i) < k.dep_target) {
+            if (globaltimer_ns() - t_start > kChainTimeoutNs) {
+              if (atomicExch(stop, 1) == 0) atomicAdd(a.err, 1);   // one count per failed launch, read by the host
+              t = a.n_tix;
+              break;
+            }
+            __nanosleep(32);
+          }
+        fence_proxy_async_global();
+        if (dbg) dbg[1] = globaltimer_ns();
+        EpiArgs e = a.args[k.kind * a.L + k.layer].epi;
+        if (FWD && k.kind == 0 && !a.save) { e.ptr[0] = nullptr; e.ptr[1] = nullptr; }
+        if (FWD && k.kind == 1) e.ptr[3] = const_cast<float*>(a.params) + reinterpret_cast<uintptr_t>(e.ptr[3]);
+        if (k.kind == 1) { e.seed = a.seed; e.ptr[7] = const_cast<unsigned long long*>(a.d_step); }
+        s_epi = e;
+        if (prev_kind == 0) chain_inval_barriers<BN0>(smem);
+        else if (prev_kind == 1) chain_inval_barriers<BN1>(smem);
+        if (k.kind == 0) chain_init_barriers<BN0>(smem);
+        else chain_init_barriers<BN1>(smem);
+        prev_kind = k.kind;
+      } else {
+        t = a.n_tix;
+      }
+      s_ticket = t;
+    }
+    __syncthreads();
+    const int t = s_ticket;
+    if (t >= a.n_tix) break;
+    const ChainTicket k = a.tix[t];
+    const GemmArgs& g = a.args[k.kind * a.L + k.layer];
+    int all_kb = 0;
+    for (int s = 0; s < g.nseg; ++s) all_kb += g.seg[s].nkb * g.seg[s].nlayers;
+    // The producer's TMA loads follow the acquire (global), and they overwrite ring bytes the previous ticket's epilogue wrote
+    // through the generic proxy (accumulator and staging tiles), observed through the CTA barrier above (shared). Both fences are
+    // issued by the one thread that issues the loads: the same fence in all 544 threads cost 0.07 ms per Cfg-2 step.
+    if ((threadIdx.x >> 5) == kActEpiWarps) {
+      fence_proxy_async_global();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    if (k.kind == 0) act_gemm_tile<E0, BN0, true>(g, s_epi, smem, k.m, k.n, 0, all_kb, 1, 0, 1, nullptr);
+    else act_gemm_tile<E1, BN1, true>(g, s_epi, smem, k.m, k.n, 0, all_kb, 1, 0, 1, nullptr);
+    // the tile's TMA stores are complete in the threads that issued them: publish them to the tiles that wait for this one
+    fence_proxy_async_global();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      red_release_gpu_add(done + k.done, 1);
+      if (a.dbg) a.dbg[size_t(t) * kDbgSlots + 2] = globaltimer_ns();
+    }
+  }
+}
+
+template <bool FWD, int BN0, int BN1>
+int launch_chain_kernel(const ChainArgs& a, int grid, cudaStream_t st) {
+  static bool configured = false;
+  if (!configured) {
+    T2_CHECK_CUDA(cudaFuncSetAttribute(wn_chain_kernel<FWD, BN0, BN1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       ActGemmCfg<BN0>::kSmemBytes));
+    configured = true;
+  }
+  wn_chain_kernel<FWD, BN0, BN1><<<grid, kActGemmThreads, ActGemmCfg<BN0>::kSmemBytes, st>>>(a);
+  t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+
+
+int launch_wn_chain(bool fwd, int bn0, int bn1, const ChainArgs& a, int grid, cudaStream_t st) {
+  if (fwd && bn0 == 256) return bn1 == 256 ? launch_chain_kernel<true, 256, 256>(a, grid, st) : launch_chain_kernel<true, 256, 128>(a, grid, st);
+  if (!fwd && bn0 == 256) return bn1 == 256 ? launch_chain_kernel<false, 256, 256>(a, grid, st) : launch_chain_kernel<false, 256, 128>(a, grid, st);
+  if (!fwd && bn0 == 128) return bn1 == 256 ? launch_chain_kernel<false, 128, 256>(a, grid, st) : launch_chain_kernel<false, 128, 128>(a, grid, st);
+  return t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "layer chain: no kernel for %s with BN %d / %d", fwd ? "forward" : "backward", bn0, bn1);
 }
 
 }  // namespace t2

@@ -174,15 +174,32 @@ __device__ __forceinline__ void stage_get_sw(uint8_t* tile, int lane, int cq, fl
     v[q * 8 + 6] = bf16lo(u.w); v[q * 8 + 7] = bf16hi(u.w);
   }
 }
-// global rows -> swizzled tile (rows >= nrows are zero-filled); the 4 warps of the quarter cooperate, then meet on its barrier
+// global rows -> swizzled tile (rows >= nrows are zero-filled); the 4 warps of the quarter cooperate, then meet on its barrier.
+// kCoherent: the rows were written earlier in the same grid by another CTA (the persistent layer chains), so they are read through
+// the coherent path instead of the read-only one
+template <bool kCoherent = false>
 __device__ __forceinline__ void tile_fill_sw(uint8_t* tile, const __nv_bfloat16* g, size_t ld, int nrows, const EpiCtx& c) {
   const int ch = c.lane & 15, rh = c.lane >> 4;
+  if constexpr (kCoherent) {
+    uint4 u[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int r = (c.cg * 4 + i) * 2 + rh;
-    uint4 u = make_uint4(0, 0, 0, 0);
-    if (r < nrows) u = __ldg(reinterpret_cast<const uint4*>(g + size_t(r) * ld + ch * 8));
-    *reinterpret_cast<uint4*>(sw_addr(tile, r, ch)) = u;
+    for (int i = 0; i < 4; ++i) {   // all four loads in flight before the first store
+      const int r = (c.cg * 4 + i) * 2 + rh;
+      u[i] = make_uint4(0, 0, 0, 0);
+      if (r < nrows)
+        asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];"
+                     : "=r"(u[i].x), "=r"(u[i].y), "=r"(u[i].z), "=r"(u[i].w) : "l"(g + size_t(r) * ld + ch * 8));
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(sw_addr(tile, (c.cg * 4 + i) * 2 + rh, ch)) = u[i];
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int r = (c.cg * 4 + i) * 2 + rh;
+      uint4 u = make_uint4(0, 0, 0, 0);
+      if (r < nrows) u = __ldg(reinterpret_cast<const uint4*>(g + size_t(r) * ld + ch * 8));
+      *reinterpret_cast<uint4*>(sw_addr(tile, r, ch)) = u;
+    }
   }
   quarter_sync(c.qbar);
 }
@@ -334,11 +351,14 @@ struct Epilogue<EPI_GATE, 256> {
 // replayed CUDA graph draw fresh masks);  f0 res_scale, f1 dropout p;  i1 = layer
 template <int BN>
 struct Epilogue<EPI_RES, BN> {
-  // the x tile (residual input) of column group 0 does not depend on this kernel's MMAs: load it while the mainloop runs
+  // the x tile (residual input) of column group 0 does not depend on this kernel's MMAs: load it while the mainloop runs.
+  // kCoherent: x was written by another CTA of the same grid (persistent layer chain)
+  template <bool kCoherent = false>
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     if (e.i[11]) return;   // split-bf16 mode reads x directly in run()
-    tile_fill_sw(c.tile(2), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN, BN, c.nrows, c);
+    tile_fill_sw<kCoherent>(c.tile(2), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN, BN, c.nrows, c);
   }
+  template <bool kCoherent = false>
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int R = BN;
     __nv_bfloat16* x_out = static_cast<__nv_bfloat16*>(e.ptr[1]);
@@ -367,7 +387,7 @@ struct Epilogue<EPI_RES, BN> {
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
     const uint32_t hs = hash_seed(seed, uint32_t(e.i[1]));
     const size_t row = (size_t(c.b) * c.T + c.t) * R;
-    if (BN == 256) tile_fill_sw(c.tile(1), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN + 128, BN, c.nrows, c);
+    if (BN == 256) tile_fill_sw<kCoherent>(c.tile(1), static_cast<const __nv_bfloat16*>(e.ptr[0]) + c.row0 * BN + 128, BN, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
       // tiles: x of group 0 / 1 arrives in tile 2 / 1 and is replaced in place by x_out; the dropped copies go to tile 0 (group 0)
@@ -812,10 +832,13 @@ struct Epilogue<EPI_GATE_BWD, BN> {
 // f0 res_scale, f1 dropout p, f2 bias-gradient scale; i1 = layer
 template <int BN>
 struct Epilogue<EPI_DX, BN> {
+  // kCoherent: dxo was written by another CTA of the same grid (persistent layer chain)
+  template <bool kCoherent = false>
   static __device__ __forceinline__ void prefetch(const EpiArgs& e, const EpiCtx& c) {
     const __nv_bfloat16* dxo = static_cast<const __nv_bfloat16*>(e.ptr[0]);
-    if (dxo) tile_fill_sw(c.tile(2), dxo + c.row0 * BN, BN, c.nrows, c);   // column group 0; group 1 (BN = 256) is loaded in run()
+    if (dxo) tile_fill_sw<kCoherent>(c.tile(2), dxo + c.row0 * BN, BN, c.nrows, c);   // column group 0; group 1 (BN = 256) is loaded in run()
   }
+  template <bool kCoherent = false>
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
     const int R = BN;
     const __nv_bfloat16* dxo = static_cast<const __nv_bfloat16*>(e.ptr[0]);
@@ -824,7 +847,7 @@ struct Epilogue<EPI_DX, BN> {
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
     const uint32_t hs = hash_seed(seed, uint32_t(e.i[1]));
     const size_t row = (size_t(c.b) * c.T + c.t) * R;
-    if (BN == 256 && dxo) tile_fill_sw(c.tile(1), dxo + c.row0 * BN + 128, BN, c.nrows, c);
+    if (BN == 256 && dxo) tile_fill_sw<kCoherent>(c.tile(1), dxo + c.row0 * BN + 128, BN, c.nrows, c);
 #pragma unroll 1
     for (int gq = 0; gq < BN / 128; ++gq) {
       uint8_t* tile = c.tile(gq == 0 ? 2 : 1);
@@ -990,6 +1013,138 @@ struct ActGemmCfg {
   static_assert(kStages >= 2 && kPipeBytes <= kPipeBudget && kSmemBytes <= 232448, "shared memory budget");
   static_assert(kPipeBytes % 1024 == 0, "staging tiles must be aligned to the 1024-byte swizzle atom");
 };
+
+// One (m_tile, n_tile) output tile of `g`, exactly as one CTA of act_gemm_kernel computes it, for the tickets of the persistent WaveNet
+// layer chains. act_gemm_kernel keeps its own copy of these lines: calling this function from it gives the same PTX up to where the
+// tile-index arithmetic is placed, but ptxas then allocates its 96 registers differently and the per-layer gate GEMM spills more
+// (72 instead of 24 stack bytes) and runs 3.6 % slower on an H100. Keep the two in step: TMA producer loop, wgmma mainloop over k-blocks [kb_lo, kb_hi), the fp32 accumulator
+// tile, the fused epilogue (on `epi`) and the drain of its TMA stores. The caller has initialised the stage barriers of
+// ActGemmCfg<BN> (full: 1 arrival, empty: kActEpiWarps * cs) behind a CTA barrier and has made the tile's inputs visible; the
+// tile ends with every store's global writes complete in the threads that issued them (no CTA barrier at its end).
+// `smem` is the 1024-byte aligned base of the dynamic shared memory; cs / crank / cmask describe the multicast cluster.
+// kChain: the tile is a ticket of a persistent layer chain, whose epilogue inputs may come from other CTAs of the same grid
+template <int EPI, int BN, bool kChain = false>
+__device__ __forceinline__ void act_gemm_tile(const GemmArgs& g, const EpiArgs& epi, uint8_t* smem, int m_tile, int n_tile,
+                                              int kb_lo, int kb_hi, uint32_t cs, uint32_t crank, uint16_t cmask, long long* dbg) {
+  using Cfg = ActGemmCfg<BN>;
+  constexpr int WN = BN / 2;          // columns per consumer warpgroup
+  float* acc_s = reinterpret_cast<float*>(smem);
+  // staging tiles, tile-major over the row quarters: tiles 0 and 1 end the ring, the dedicated tile 2 follows it
+  uint8_t* staging = smem + Cfg::kPipeBytes - Cfg::kTailBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
+  const int warp = threadIdx.x >> 5;
+  const int b = m_tile / g.tiles_per_b;
+  const int t0 = (m_tile - b * g.tiles_per_b) * kBM;
+  const int total_kb = kb_hi - kb_lo;
+
+  if (warp == kActEpiWarps) {
+    if (elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      int kb_global = 0;
+      for (int s = 0; s < g.nseg; ++s) {
+        const Seg sg = g.seg[s];
+        for (int l = 0; l < sg.nlayers; ++l) {
+          for (int kb = 0; kb < sg.nkb; ++kb, ++kb_global) {
+            if (kb_global < kb_lo || kb_global >= kb_hi) continue;
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+            uint8_t* sa = smem + stage * Cfg::kStageBytes;
+            uint8_t* sb = sa + Cfg::kABytes;
+            tma_load_4d(sa, &g.amap[sg.map], &full_bar[stage], sg.k0 + kb * kBK, t0 + sg.shift, b, sg.layer0 + l);
+            if (cs == 1) {
+              tma_load_3d(sb, &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK, n_tile * BN, g.b_layer);
+            } else {
+              const int rows = BN / int(cs);     // this CTA's slice of the weight tile (whole 8-row swizzle atoms: 1024-byte aligned)
+              tma_load_3d_mc(sb + crank * rows * (kBK * 2), &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK,
+                             n_tile * BN + int(crank) * rows, g.b_layer, cmask);
+            }
+            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+  } else {
+    const int q = warp & 3;  // row quarter of this warp in the epilogue
+    const int lane = threadIdx.x & 31;
+    EpiCtx c;
+    c.lane = lane;
+    c.cg = warp >> 2;
+    c.qbar = 1 + q;
+    c.b = b; c.T = g.T;
+    const int tw = t0 + q * 32;          // first time step of this warp
+    c.t = tw + c.lane;
+    c.valid = c.t < g.T;
+    c.row0 = size_t(b) * g.T + tw;
+    c.nrows = g.T - tw < 0 ? 0 : (g.T - tw > 32 ? 32 : g.T - tw);
+    c.stg = staging + q * kSTileBytes;
+    c.smem_all = smem + Cfg::kAccBytes;
+    c.m_tile = m_tile;
+    c.omap = g.omap; c.tq = tw; c.sk = 0;
+    c.n_tile = n_tile;
+    constexpr bool kCoh = EPI == EPI_RES || EPI == EPI_DX;   // the epilogues that take a template read-path flag
+    if constexpr (kCoh) Epilogue<EPI, BN>::template prefetch<kChain>(epi, c);
+    else if constexpr (EpiHasPrefetch<EPI>::value) Epilogue<EPI, BN>::prefetch(epi, c);
+
+    // ---- mainloop: this warpgroup's 64 x WN quarter of the tile
+    const int wg = warp >> 2, mh = wg >> 1, nh = wg & 1;
+    float d[WN / 2];
+#pragma unroll
+    for (int i = 0; i < WN / 2; ++i) d[i] = 0.f;
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < total_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      __syncwarp();                    // wgmma is warp-aligned: reconverge after the spin-wait
+      if (dbg && kb == 0 && threadIdx.x == 0) dbg[2] = clock64();
+      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + uint32_t(mh * 64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes) + uint32_t(nh * WN * 128);
+      const uint64_t adesc = make_gdesc_sw128(sa, 16, 1024);
+      const uint64_t bdesc = make_gdesc_sw128(sb, 16, 1024);
+      wgmma_fence();
+      wgmma_fence_regs(d);
+#pragma unroll
+      for (int k = 0; k < kBK / 16; ++k)
+        // advancing K by 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr>>4) field
+        Wgmma<WN, 0, 0>::mma(d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), (kb > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_fence_regs(d);
+      // the previous k-block's MMAs have finished reading their stage: hand it back to the producer(s)
+      wgmma_wait<1>();
+      if (kb > 0 && lane == 0) {
+        if (cs == 1) mbar_arrive(&empty_bar[prev]);
+        else for (uint32_t r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+    if (dbg && threadIdx.x == 0) dbg[3] = clock64();
+    // every warpgroup's MMAs are done with the stages: the accumulator tile may overwrite them
+    asm volatile("bar.sync 6, 512;\n" ::: "memory");
+    {
+      const int r0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < WN / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = r0 + 8 * i, col = nh * WN + 8 * j + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc_s + r * BN + ((((col >> 2) ^ (r & 7)) << 2) | (col & 3))) =
+              make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+        }
+    }
+    asm volatile("bar.sync 6, 512;\n" ::: "memory");
+    const int row = q * 32 + lane;
+    c.trow = AccRow{acc_s + row * BN, 0, row & 7};
+    if (dbg && threadIdx.x == 0) dbg[4] = clock64();
+    if constexpr (kCoh) Epilogue<EPI, BN>::template run<kChain>(epi, c);
+    else Epilogue<EPI, BN>::run(epi, c);
+    if (dbg && threadIdx.x == 0) dbg[5] = clock64();
+    tile_store_drain(c);
+  }
+}
 
 template <int EPI, int BN>
 __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __grid_constant__ GemmArgs g) {

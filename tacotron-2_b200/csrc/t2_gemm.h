@@ -36,6 +36,7 @@ struct ActGemmCall {
 
 void set_timing_buffer(long long* p);
 bool pdl_enabled();
+int cluster_pref();   // weight-multicast cluster size of the act_gemm launches (T2_CLUSTER; 1 = off)
 // launch any kernel with the programmatic-dependent-launch attribute (the kernel must call pdl_wait() before it touches
 // global memory; see t2_common.cuh)
 template <typename... KArgs, typename... Args>
@@ -51,6 +52,13 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 // *cluster_used (nullable) receives the cluster size the kernel was launched with
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used = nullptr);
+// the checked kernel arguments (tensor maps encoded), grid and cluster size launch_act_gemm launches `c` with
+int make_gemm_args(int epi, int BN, const ActGemmCall& c, GemmArgs& g, dim3& grid, int& cs);
+// one persistent layer chain (wn_chain_kernel): kind 0 / 1 tiles are EPI_GATE (BN 256) / EPI_RES (BN bn1) when fwd, else
+// EPI_GATE_BWD (BN bn0) / EPI_DX (BN bn1); `grid` CTAs take the tickets
+int launch_wn_chain(bool fwd, int bn0, int bn1, const ChainArgs& a, int grid, cudaStream_t st);
+// the next n_slots int64 stamps of the timing buffer (t2_dbg_set_timing_buffer), or nullptr when it is off
+long long* take_timing_slice(long long n_slots);
 int launch_wgrad(const ActT* maps, int nmaps, const WgradTile* tiles_dev, int ntiles, float* out,
                  int T, int B, cudaStream_t stream);
 // appends the tiles of the dense [Ca x Cb] weight gradient out[out_off + m * ldc + n] of A channels [a_ch0, a_ch0 + Ca) and B channels

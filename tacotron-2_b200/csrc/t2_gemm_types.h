@@ -72,4 +72,28 @@ struct WgradArgs {
   int T, B;
 };
 
+// One work item of a persistent layer chain (wn_chain_kernel, t2_gemm.cu; built by build_chain, t2_wavenet.cu): output tile (m, n) of the kind-th GEMM of `layer` (forward: 0 gate,
+// 1 out; backward: 0 dz, 1 dx). It may start once the completion counters [dep_lo, dep_hi] have all reached dep_target (dep_hi <
+// dep_lo: no dependency inside the kernel) and adds 1 to counter `done` when its stores are complete. Counter of (kind, layer, M
+// tile m) = (kind * L + layer) * MT + m, with MT = B * ceil(T / 128) M tiles over all batch items.
+struct ChainTicket {
+  int kind, layer, m, n;
+  int dep_lo, dep_hi, dep_target;
+  int done;
+};
+
+struct ChainArgs {
+  const GemmArgs* args;        // [2][L]: kind-major
+  const ChainTicket* tix;
+  int n_tix, L;
+  int* ctr;                    // [0] ticket counter, [1] stop flag; completion counters from ctr + 16
+  int* err;                    // += 1 when a dependency wait of the launch times out (its remaining tickets are then skipped)
+  long long* dbg;              // optional: kDbgSlots stamps per ticket (start, dependencies met, end, SM)
+  // per-call values the workspace table leaves out (it depends only on the configuration, workspace and packed weights)
+  const float* params;         // forward out GEMM: its bias is params + (offset the table stores in epi.ptr[3])
+  const unsigned long long* d_step;
+  unsigned long long seed;
+  int save;                    // forward: write the tanh / sigmoid stashes
+};
+
 }  // namespace t2

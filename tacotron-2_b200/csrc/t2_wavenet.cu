@@ -16,6 +16,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -74,8 +75,60 @@ struct Layout {
   std::vector<ColsumJob> colsums;
   std::vector<WgradTile> tiles_main, tiles_head;
   std::vector<int> tile_start;   // [L + 1]: first entry of tiles_main that belongs to layer l (the table is layer-major)
+  // persistent layer chains, [0] forward, [1] backward: tickets in launch order, and per direction a workspace block of
+  // 16 ints (ticket counter first) + 2 * L * MT completion counters, the tickets and the GemmArgs table ([kind][layer])
+  int MT;
+  int n_chain[2];   // ticket counts (the tickets themselves are built by build_chain only where a chain is launched or queried)
+  long long w_chain_ctr[2], w_chain_tix[2], w_chain_args[2], w_chain_err;
   int dil(int l) const { return 1 << (l % (L / c.stacks)); }
 };
+
+// The tickets of both chains, in the order of the per-layer launches they replace: forward, per layer the gate tiles (M fastest, then
+// N), then the out tiles (none after the last layer); backward, from the top layer down, the dz tiles then the dx tiles. A ticket
+// waits only for the tiles whose outputs its GEMM reads (its A operand through the dilated taps, and its epilogue inputs), all of
+// them earlier in the order and inside its batch item (the taps' rows before 0 / past T are zero-filled, not read):
+//   gate(l, m) <- out(l-1, m-k..m)   rows [t0 - 2d, t0 + 128) of xd_l, k = ceil(2d / 128)   (out(l-1, m) also wrote x_l for out(l, m))
+//   out(l, m)  <- gate(l, m, every n)   z_l rows [t0, t0 + 128)
+//   dz(l, m)   <- dx(l+1, m)         dxin_{l+1} rows [t0, t0 + 128)   (and the dx epilogue's residual input of the same rows)
+//   dx(l, m)   <- dz(l, m..m+k, every n)   dg_l rows [t0, t0 + 128 + 2d)
+// Every buffer a chain writes is per layer and read only by later tickets, so no ticket overwrites what an earlier one still reads.
+// dir 0: forward, 1: backward.
+void build_chain(const Layout& lo, int dir, std::vector<ChainTicket>& v) {
+  const int tpb = (lo.T + kBM - 1) / kBM;
+  auto idx = [&](int kind, int l, int m) { return (kind * lo.L + l) * lo.MT + m; };
+  const int ng = lo.G / 256;                                       // N tiles of the gate GEMM (BN = 256)
+  const int nz = lo.Gh / (lo.Gh >= 256 ? 256 : 128);               // N tiles of the dz GEMM
+  v.clear();
+  v.reserve(lo.n_chain[dir]);
+  if (dir == 0) {
+    for (int l = 0; l < lo.L; ++l) {
+      const int k = (2 * lo.dil(l) + kBM - 1) / kBM;
+      for (int n = 0; n < ng; ++n)
+        for (int m = 0; m < lo.MT; ++m) {
+          const int m0 = m / tpb * tpb;                            // first M tile of this batch item
+          ChainTicket t{0, l, m, n, 0, -1, 0, idx(0, l, m)};
+          if (l > 0) { t.dep_lo = idx(1, l - 1, std::max(m0, m - k)); t.dep_hi = idx(1, l - 1, m); t.dep_target = 1; }
+          v.push_back(t);
+        }
+      if (l + 1 < lo.L)
+        for (int m = 0; m < lo.MT; ++m) v.push_back(ChainTicket{1, l, m, 0, idx(0, l, m), idx(0, l, m), ng, idx(1, l, m)});
+    }
+    return;
+  }
+  for (int l = lo.L - 1; l >= 0; --l) {
+    const int k = (2 * lo.dil(l) + kBM - 1) / kBM;
+    for (int n = 0; n < nz; ++n)
+      for (int m = 0; m < lo.MT; ++m) {
+        ChainTicket t{0, l, m, n, 0, -1, 0, idx(0, l, m)};
+        if (l + 1 < lo.L) { t.dep_lo = t.dep_hi = idx(1, l + 1, m); t.dep_target = 1; }
+        v.push_back(t);
+      }
+    for (int m = 0; m < lo.MT; ++m) {
+      const int m1 = m / tpb * tpb + tpb - 1;                      // last M tile of this batch item
+      v.push_back(ChainTicket{1, l, m, 0, idx(0, l, m), idx(0, l, std::min(m1, m + k)), nz, idx(1, l, m)});
+    }
+  }
+}
 
 int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   T2_REQUIRE(cfg != nullptr, T2_ERR_INVALID_ARG, "null config");
@@ -309,6 +362,15 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.w_packjobs = ws.take((long long)lo.n_packjobs * sizeof(PackJob));
   lo.w_colsum = ws.take((long long)lo.n_colsum * sizeof(ColsumJob));
   lo.w_tables = ws.take((long long)lo.L * (3 * sizeof(long long) + sizeof(float)));
+  lo.MT = lo.B * ((lo.T + kBM - 1) / kBM);
+  lo.n_chain[0] = lo.L * (lo.G / 256) * lo.MT + (lo.L - 1) * lo.MT;
+  lo.n_chain[1] = lo.L * (lo.Gh / (lo.Gh >= 256 ? 256 : 128)) * lo.MT + lo.L * lo.MT;
+  for (int dir = 0; dir < 2; ++dir) {   // a few MB at most, against the GBs of activations: kept whether the chains run or not
+    lo.w_chain_ctr[dir] = ws.take((16 + 2LL * lo.L * lo.MT) * 4);
+    lo.w_chain_tix[dir] = ws.take((long long)lo.n_chain[dir] * sizeof(ChainTicket));
+    lo.w_chain_args[dir] = ws.take(2LL * lo.L * sizeof(GemmArgs));   // 256-byte aligned: tensor maps in global memory need 64
+  }
+  lo.w_chain_err = ws.take(4);
   lo.w_spk = lo.w_gbias = lo.w_gsum = -1;
   if (lo.Gi > 0) {
     lo.w_spk = ws.take((1LL + lo.B) * 4);
@@ -1086,6 +1148,126 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
   return g;
 }
 
+// ------------------------------------------------------------------------------------------------------
+// Persistent layer chains (wn_chain_kernel in t2_gemm.cu): the tickets come from build_chain, the per-(kind, layer) GemmArgs from
+// the same make_*_call as the per-layer launches.
+// ------------------------------------------------------------------------------------------------------
+// uploaded chain tables per (workspace, direction): the table depends only on the configuration, the workspace and the packed
+// weights, so it is written once and stays valid for eager calls and CUDA-graph replays alike (t2_wn_init forgets it)
+struct ChainTable {
+  const void* key;         // device address of the table (workspace + direction)
+  const void* packed;
+  t2_wn_config_t cfg;
+};
+struct ChainCache {
+  std::mutex mu;
+  std::vector<ChainTable> entries;
+};
+ChainCache& chain_cache() {
+  static ChainCache c;
+  return c;
+}
+void chain_cache_forget(const void* ws, long long bytes) {
+  ChainCache& c = chain_cache();
+  std::lock_guard<std::mutex> lk(c.mu);
+  const uint8_t* lo = static_cast<const uint8_t*>(ws);
+  c.entries.erase(std::remove_if(c.entries.begin(), c.entries.end(),
+                                 [&](const ChainTable& e) {
+                                   const uint8_t* k = static_cast<const uint8_t*>(e.key);
+                                   return k >= lo && k < lo + bytes;
+                                 }),
+                  c.entries.end());
+}
+
+int g_chain_mode = 0;   // t2_dbg_wn_per_layer: 0 automatic, 1 per-layer launches (the bit-exact reference), 2 persistent chains
+
+// SM count of the current device (cached per device)
+int device_sms() {
+  static int sms[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (sms[dev] == 0 && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
+  return sms[dev];
+}
+
+// dir 0: the forward gate / out GEMMs of every layer; dir 1: the backward dz / dx GEMMs. `free_sms` SMs are left to concurrent work.
+int launch_chain(const Layout& lo, int dir, uint8_t* ws, const uint8_t* pk, const float* params, int save, unsigned long long seed,
+                 const unsigned long long* d_step, int free_sms, cudaStream_t st) {
+  const int bn_z = lo.Gh >= 256 ? 256 : 128;
+  const void* key = ws + lo.w_chain_tix[dir];
+  ChainCache& cache = chain_cache();
+  std::lock_guard<std::mutex> lk(cache.mu);
+  auto it = std::find_if(cache.entries.begin(), cache.entries.end(), [&](const ChainTable& e) { return e.key == key; });
+  if (it == cache.entries.end() || it->packed != pk || memcmp(&it->cfg, &lo.c, sizeof(lo.c)) != 0) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    T2_CHECK_CUDA(cudaStreamIsCapturing(st, &cap));
+    T2_REQUIRE(cap == cudaStreamCaptureStatusNone, T2_ERR_INVALID_ARG,
+               "the WaveNet layer-chain table of this workspace is not written yet: run one forward / backward before capturing a graph");
+    // the table: the tickets, then the GemmArgs [kind][layer] of the per-layer launches (per-call values left out, see ChainArgs)
+    std::vector<ChainTicket> tix;
+    build_chain(lo, dir, tix);
+    std::vector<GemmArgs> args(2 * lo.L);
+    memset(args.data(), 0, args.size() * sizeof(GemmArgs));
+    long long* gfx = reinterpret_cast<long long*>(ws + lo.w_gfx);
+    for (int l = 0; l < lo.L; ++l) {
+      ActGemmCall c0, c1;
+      int e0, e1, b0, b1;
+      const bool has1 = dir == 1 || l + 1 < lo.L;                     // no out GEMM after the top layer
+      if (dir == 0) {
+        c0 = make_gate_call(lo, ws, pk, l, true); e0 = EPI_GATE; b0 = 256;
+        if (has1) {
+          c1 = make_out_call(lo, ws, pk, nullptr, l, lo.c.dropout, 0, nullptr);
+          c1.epi.ptr[3] = reinterpret_cast<void*>(uintptr_t(lo.p_o_b[l]));   // bias offset in params, resolved by the kernel
+        }
+        e1 = EPI_RES; b1 = lo.R;
+      } else {
+        c0 = make_dz_call(lo, ws, pk, l, gfx); e0 = EPI_GATE_BWD; b0 = bn_z;
+        c1 = make_dx_call(lo, ws, pk, l, lo.c.dropout, 0, nullptr, gfx); e1 = EPI_DX; b1 = lo.R;
+      }
+      c0.cluster = c1.cluster = 1;
+      dim3 grid;
+      int cs = 1;
+      int rc = make_gemm_args(e0, b0, c0, args[l], grid, cs);
+      if (rc) return rc;
+      args[l].dbg = nullptr;
+      if (has1) {
+        rc = make_gemm_args(e1, b1, c1, args[lo.L + l], grid, cs);
+        if (rc) return rc;
+        args[lo.L + l].dbg = nullptr;
+      }
+    }
+    T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_chain_tix[dir], tix.data(), tix.size() * sizeof(ChainTicket), cudaMemcpyHostToDevice, st));
+    T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_chain_args[dir], args.data(), args.size() * sizeof(GemmArgs), cudaMemcpyHostToDevice, st));
+    T2_CHECK_CUDA(cudaStreamSynchronize(st));
+    const ChainTable e{key, pk, lo.c};
+    if (it == cache.entries.end()) cache.entries.push_back(e);
+    else *it = e;
+  }
+  ChainArgs a;
+  a.args = reinterpret_cast<const GemmArgs*>(ws + lo.w_chain_args[dir]);
+  a.tix = reinterpret_cast<const ChainTicket*>(ws + lo.w_chain_tix[dir]);
+  a.n_tix = lo.n_chain[dir]; a.L = lo.L;
+  a.ctr = reinterpret_cast<int*>(ws + lo.w_chain_ctr[dir]);
+  a.err = reinterpret_cast<int*>(ws + lo.w_chain_err);
+  a.dbg = take_timing_slice((long long)lo.n_chain[dir] * kDbgSlots);
+  a.params = params; a.d_step = d_step; a.seed = seed; a.save = save;
+  T2_CHECK_CUDA(cudaMemsetAsync(a.ctr, 0, (16 + 2LL * lo.L * lo.MT) * 4, st));
+  int grid = device_sms() - free_sms;
+  if (grid > a.n_tix) grid = a.n_tix;
+  if (grid < 1) grid = 1;
+  return launch_wn_chain(dir == 0, dir == 0 ? 256 : bn_z, lo.R, a, grid, st);
+}
+
+// the persistent chains run unless the per-layer reference is asked for, or the launch needs what they do not support (split-bf16
+// forward, weight multicast clusters). Automatically they run where a layer's gate GEMM is at most two waves of CTAs: there the
+// grid-wide drains between launches are a large part of every GEMM. Layers of many waves lose less to the drains than the chains'
+// per-tile overheads cost them (wavenet_mol, 1008 M tiles per layer, ran 1.3 % slower on an H100 80GB HBM3 at 700 W).
+bool use_chain(const Layout& lo) {
+  if (lo.split || cluster_pref() != 1 || g_chain_mode == 1) return false;
+  if (g_chain_mode == 2) return true;
+  return (long long)lo.MT * (lo.G / 256) <= 2LL * device_sms();
+}
+
 // One layer of the conditioning upsampler (type 0 SubPixel, 1 ConvTranspose2D, 2 ConvTranspose1D; in [B][C][W], out [B][C][W*s]):
 // the launches of the training forward / backward, AR synthesis and t2_dbg_wn_kernel.
 int up1d_smem_limit(const void* fn, size_t smem) {
@@ -1191,6 +1373,7 @@ extern "C" int t2_wn_init(const t2_wn_config_t* cfg, void* d_packed, void* d_wor
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   T2_CHECK_CUDA(cudaMemsetAsync(d_packed, 0, lo.packed_bytes, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d_workspace, 0, lo.workspace_bytes, st));
+  chain_cache_forget(d_workspace, lo.workspace_bytes);   // the chain tables were just cleared with the rest of the workspace
   float* scalars = reinterpret_cast<float*>(ws + lo.w_scalars);
   for (auto& t : lo.tiles_head)
     if (t.div != nullptr) t.div = scalars + 1;
@@ -1289,14 +1472,19 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   // 3. residual stack
   bf16* z_all = reinterpret_cast<bf16*>(ws + lo.w_z);
   const ActT a_z = make_act(z_all, lo.Gh * lo.xm, lo.T, lo.B, lo.L);
-  for (int l = 0; l < lo.L; ++l) {
-    ActGemmCall g = make_gate_call(lo, ws, pk, l, save_for_backward != 0);
-    rc = launch_act_gemm(EPI_GATE, 256, g, st);
+  if (use_chain(lo)) {
+    rc = launch_chain(lo, 0, ws, pk, d_params, save_for_backward != 0, seed, d_step, 0, st);
     if (rc) return rc;
-    if (l + 1 < lo.L) {
-      ActGemmCall o = make_out_call(lo, ws, pk, d_params, l, p, seed, d_step);
-      rc = launch_act_gemm(EPI_RES, lo.R, o, st);
+  } else {
+    for (int l = 0; l < lo.L; ++l) {
+      ActGemmCall g = make_gate_call(lo, ws, pk, l, save_for_backward != 0);
+      rc = launch_act_gemm(EPI_GATE, 256, g, st);
       if (rc) return rc;
+      if (l + 1 < lo.L) {
+        ActGemmCall o = make_out_call(lo, ws, pk, d_params, l, p, seed, d_step);
+        rc = launch_act_gemm(EPI_RES, lo.R, o, st);
+        if (rc) return rc;
+      }
     }
   }
   // 4. all skip 1x1s as one K = L*Gh GEMM, + ReLU
@@ -1471,13 +1659,19 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   const ActT a_dskip = make_act(dskip, lo.S, lo.T, lo.B, 1);
   const ActT a_dg = make_act(dg, lo.G, lo.T, lo.B, lo.L);
   const int bn_z = lo.Gh >= 256 ? 256 : 128;
-  for (int l = lo.L - 1; l >= 0; --l) {
-    ActGemmCall gz = make_dz_call(lo, ws, pk, l, gfx);
-    rc = launch_act_gemm(EPI_GATE_BWD, bn_z, gz, st);
+  if (use_chain(lo)) {
+    // the head weight-gradient tiles on the side stream keep their SMs (they used to run on the SMs the 120-tile launches left idle)
+    rc = launch_chain(lo, 1, ws, pk, d_params, 1, seed, d_step, side ? lo.n_tiles_head : 0, st);
     if (rc) return rc;
-    ActGemmCall gx = make_dx_call(lo, ws, pk, l, p, seed, d_step, gfx);
-    rc = launch_act_gemm(EPI_DX, lo.R, gx, st);
-    if (rc) return rc;
+  } else {
+    for (int l = lo.L - 1; l >= 0; --l) {
+      ActGemmCall gz = make_dz_call(lo, ws, pk, l, gfx);
+      rc = launch_act_gemm(EPI_GATE_BWD, bn_z, gz, st);
+      if (rc) return rc;
+      ActGemmCall gx = make_dx_call(lo, ws, pk, l, p, seed, d_step, gfx);
+      rc = launch_act_gemm(EPI_DX, lo.R, gx, st);
+      if (rc) return rc;
+    }
   }
   if (lo.Gi > 0) {   // gate-bias and speaker-term gradients from the per-item sums of the gate backward
     GinGradArgs a;
@@ -1555,6 +1749,31 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   return T2_OK;
 }
 
+extern "C" int t2_dbg_wn_per_layer(int mode) {
+  T2_REQUIRE(mode >= 0 && mode <= 2, T2_ERR_INVALID_ARG, "dbg_wn_per_layer: mode must be 0, 1 or 2 (got %d)", mode);
+  g_chain_mode = mode;
+  return T2_OK;
+}
+
+extern "C" int t2_dbg_wn_chain(const t2_wn_config_t* cfg, int dir, int* out, int cap) {
+  Layout lo;
+  int rc = build_layout(cfg, lo);
+  if (rc) return rc;
+  T2_REQUIRE(dir == 0 || dir == 1, T2_ERR_INVALID_ARG, "dbg_wn_chain: dir must be 0 (forward) or 1 (backward), got %d", dir);
+  std::vector<ChainTicket> v;
+  build_chain(lo, dir, v);
+  T2_REQUIRE(int(v.size()) == lo.n_chain[dir], T2_ERR_INVALID_ARG, "dbg_wn_chain: %d tickets built, %d reserved", int(v.size()),
+             lo.n_chain[dir]);
+  T2_REQUIRE(out == nullptr || cap >= int(v.size()), T2_ERR_INVALID_ARG, "dbg_wn_chain: %d tickets do not fit in %d", int(v.size()), cap);
+  if (out)
+    for (size_t i = 0; i < v.size(); ++i) {
+      const ChainTicket& t = v[i];
+      const int row[8] = {t.kind, t.layer, t.m, t.n, t.dep_lo, t.dep_hi, t.dep_target, t.done};
+      memcpy(out + 8 * i, row, sizeof(row));
+    }
+  return int(v.size());
+}
+
 extern "C" int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* d_speaker_ids, void* stream) {
   Layout lo;
   int rc = build_layout(cfg, lo);
@@ -1581,6 +1800,7 @@ extern "C" int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspa
       {"h1", lo.w_h1, BT * lo.S, 2},          {"h2", lo.w_h2, BT * lo.S, 2},         {"dlog", lo.w_dlog, BT * lo.ldo, 2},
       {"dh2", lo.w_dh2, BT * lo.S, 2},        {"dskip", lo.w_dskip, BT * lo.S, 2},   {"dxin", lo.w_dxin, lo.L * BT * lo.R, 2},
       {"dg", lo.w_dg, lo.L * BT * lo.G, 2},   {"dc_up", lo.w_dcup, BT * lo.C, 4},    {"scalars", lo.w_scalars, 16, 4},
+      {"chain_err", lo.w_chain_err, 1, 4},
   };
   for (const E& e : table)
     if (strcmp(e.n, name) == 0) {

@@ -432,7 +432,17 @@ class WaveNet(object):
 
     def loss_value(self):
         s, n = self.loss_buf.tolist()
+        if self.chain_errors():
+            raise RuntimeError("a persistent layer-chain launch timed out waiting for a tile and skipped the rest of its work")
         return s / max(n, 1e-20)
+
+    def chain_errors(self):
+        """Launches of the persistent layer chains (t2_wn_forward / backward) whose dependency waits timed out since t2_wn_init."""
+        p, n, eb = ctypes.c_void_p(), ctypes.c_longlong(), ctypes.c_int()
+        L.check(self.lib.t2_wn_workspace_tensor(ctypes.byref(self.cfg), L.ptr(self.workspace), b"chain_err", ctypes.byref(p),
+                                                ctypes.byref(n), ctypes.byref(eb)))
+        off = p.value - self.workspace.data_ptr()
+        return int(self.workspace[off:off + 4].view(torch.int32).item())
 
 
 class WaveNetSynthesizer(object):
