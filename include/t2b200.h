@@ -122,7 +122,7 @@ typedef struct {
  *          values bf16 [B][Ti][C2], lens int32 [B], cum fp32 [B][Ti] (in/out: the attention state), alpha fp32 [B][Ti] (out), ctx_a
  *          bf16 (nullable), ctx_b bf16. i: B, Ti, D, A, KA, F, C2, ld_h2, ld_a, ld_b, unmasked, noncumulative (the two
  *          t2_taco_config_t flags; 0 = masked scores and cum + alpha as the new state, 1 = all T_in scores and alpha as the new state).
- * BN_FWD   bn_stats_kernel + bn_apply_kernel (conv-block batch norm). p: y (bf16, or fp32 when i[3]), x bf16 [rows][C] (split: [rows][2C]),
+ * BN_FWD   bn_stats_kernel (training) + bn_apply_kernel (conv-block batch norm). p: y (bf16, or fp32 when i[3]), x bf16 [rows][C] (split: [rows][2C]),
  *          stats fp32 [4C], gamma, beta, moving mean, moving variance. i: rows, C, training, y_fp32, stream, split. f: dropout p.
  * BN_BWD   bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: dout bf16, y bf16, stats fp32 [6C] (mean / rstd at [2C, 4C); [4C, 6C) receives
  *          the backward sums), gamma, dpre bf16 (out), dgamma, dbeta (accumulated). i: rows, C, act, stream. f: dropout p. */
@@ -151,9 +151,9 @@ typedef struct {
 int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 /* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
  * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):
- * BN_FWD       bn_stats_k (training) + bn_apply_k. p: y, xb bf16 (nullable), xf fp32 [rows][C] (nullable), add fp32 [rows][C] (nullable),
+ * BN_FWD       bn_stats_kernel (training) + bn_apply_kernel. p: y, xb bf16 (nullable), xf fp32 [rows][C] (nullable), add fp32 [rows][C] (nullable),
  *              stats, gamma, beta, mm, mv. i: rows, C, ld, c0, Ct, training, y_fp32, stat_threads (128 or 256).
- * BN_BWD       bn_bwd_stats_k + bn_bwd_apply_k. p: g, y (both bf16, or both fp32 when i[9]), stats, bsum, gamma, dpre bf16, dgamma, dbeta.
+ * BN_BWD       bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: g, y (both bf16, or both fp32 when i[9]), stats, bsum, gamma, dpre bf16, dgamma, dbeta.
  *              i: rows, C, ldg, ld, c0, Ct, ldd, act, stat_threads, fp32.
  * POOL_FWD     maxpool_fwd_k. p: x bf16 [N][C], out. i: N (= B T rows), T, C.
  * POOL_BWD     maxpool_bwd_k. p: x, dout, dx. i: N, T, C.

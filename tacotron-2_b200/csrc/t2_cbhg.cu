@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/t2b200.h"
+#include "t2_batchnorm.h"
 #include "t2_common.cuh"
 #include "t2_gemm.h"
 #include "t2_params.h"
@@ -39,7 +40,7 @@ constexpr int kGruThreads = 256;
 
 struct CConv {
   int cin, cout, k, act;               // act: 1 relu, 0 none
-  long long p_k, p_b, p_g, p_be, p_mm, p_mv;
+  ConvBnParams p;
   int cinp, coutp;                     // channels rounded up to 64 (K slots of the packed operands)
   long long k_w, k_wT;                 // packed forward [cout][k * cinp], packed dgrad [cin rows][k * coutp]
 };
@@ -85,9 +86,7 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   lo.n_params = 0; lo.params.clear(); lo.bank.clear();
   const std::string P = "CBHG_postnet/";
   auto conv_params = [&](CConv& L, const std::string& pre) {
-    L.p_k = add_param(lo.params, lo.n_params, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = add_param(lo.params, lo.n_params, pre + "bias", {L.cout});
-    L.p_g = add_param(lo.params, lo.n_params, pre + "gamma", {L.cout}); L.p_be = add_param(lo.params, lo.n_params, pre + "beta", {L.cout});
-    L.p_mm = add_param(lo.params, lo.n_params, pre + "moving_mean", {L.cout}, false); L.p_mv = add_param(lo.params, lo.n_params, pre + "moving_variance", {L.cout}, false);
+    L.p = add_conv_bn_params(lo.params, lo.n_params, pre, L.k, L.cin, L.cout);
     L.cinp = (L.cin + 63) / 64 * 64; L.coutp = (L.cout + 63) / 64 * 64;
   };
   for (int k = 1; k <= lo.K; ++k) {
@@ -122,8 +121,8 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
     L.k_w = pk.take(2LL * rows_f * L.k * L.cinp);
     L.k_wT = with_t ? pk.take(2LL * rows_t * L.k * L.coutp) : 0;
     for (int j = 0; j < L.k; ++j) {
-      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
-      if (with_t) add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
+      add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
+      if (with_t) add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
     }
   };
   for (auto& L : lo.bank) conv_pack(L, false);
@@ -141,7 +140,7 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
     int slot = 0;
     for (int l = lo.grp_first[g]; l < lo.grp_first[g + 1]; ++l)
       for (int j = 0; j < lo.bank[l].k; ++j, ++slot)
-        add_pack(jobs, lo.bank[l].p_k + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
+        add_pack(jobs, lo.bank[l].p.kernel + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
   }
   const int Mp = 128;
   lo.k_dense = pk.take(2LL * lo.HU * Mp); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0);
@@ -211,95 +210,6 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
 // ------------------------------------------------------------------------------------------------------
 // small kernels
 // ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float ldv(const bf16* p, long long i) { return __bfloat162float(p[i]); }
-__device__ __forceinline__ float ldv(const float* p, long long i) { return p[i]; }
-// Batch-norm kernels work on a COLUMN SLICE [c0, c0 + C) of row-pitch-ld matrices (the conv bank keeps its K layers side by side in
-// one [N][K*CC] matrix but every layer owns its own gamma / beta / moving tensors); the statistics buffer has four sections of Ct
-// floats: sum | sum of squares | mean | rstd, indexed by the absolute column.
-// The sums are shifted by the column's first row (y - y[0]), which keeps the variance free of the E[y^2] - mean^2 cancellation
-// when |mean| >> std.
-template <typename TY>
-__global__ void bn_stats_k(const TY* __restrict__ y, int ld, int c0, float* __restrict__ stats, int Ct, long long rows, int C) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float pv = ldv(y, c0 + c);
-    float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) { const float v = ldv(y, r * ld + c0 + c) - pv; s += v; q += v * v; }
-    atomicAdd(stats + c0 + c, s); atomicAdd(stats + Ct + c0 + c, q);
-  }
-}
-// batch norm (tf.layers.batch_normalization: eps 1e-3, biased batch variance, momentum 0.99): x = (y - mean) rstd gamma + beta.
-// Writes mean / rstd into the statistics buffer and updates the moving statistics in training mode.
-// Outputs: bf16 xb (same pitch / slice as y) and / or fp32 xf (dense [rows][C], + add).
-template <typename TY>
-__global__ void bn_apply_k(const TY* __restrict__ y, int ld, int c0, bf16* __restrict__ xb, float* __restrict__ xf, const float* __restrict__ add,
-                           float* __restrict__ stats, int Ct, const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ mm,
-                           float* __restrict__ mv, long long rows, int C, int training) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= rows * C) return;
-  const int c = int(e % C);
-  const long long r = e / C;
-  float mean, rstd;
-  if (training) {
-    const float d = stats[c0 + c] / float(rows);
-    mean = ldv(y, c0 + c) + d;
-    const float var = fmaxf(stats[Ct + c0 + c] / float(rows) - d * d, 0.f);
-    rstd = rsqrtf(var + 1e-3f);
-    if (e < C) {
-      stats[2 * Ct + c0 + c] = mean; stats[3 * Ct + c0 + c] = rstd;
-      mm[c] = 0.99f * mm[c] + 0.01f * mean; mv[c] = 0.99f * mv[c] + 0.01f * var;
-    }
-  } else { mean = mm[c]; rstd = rsqrtf(mv[c] + 1e-3f); }
-  float v = (ldv(y, r * ld + c0 + c) - mean) * rstd * gamma[c] + beta[c];
-  if (add) v += add[e];
-  if (xb) xb[r * ld + c0 + c] = __float2bfloat16(v);
-  if (xf) xf[e] = v;
-}
-// backward sums: bsum[c0 + c] = sum g, bsum[Ct + c0 + c] = sum g * xhat   (g: pitch ldg, same column slice)
-template <typename TG, typename TY>
-__global__ void bn_bwd_stats_k(const TG* __restrict__ g, int ldg, const TY* __restrict__ y, int ld, int c0, const float* __restrict__ stats, int Ct,
-                               float* __restrict__ bsum, long long rows, int C) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float mean = stats[2 * Ct + c0 + c], rstd = stats[3 * Ct + c0 + c];
-    float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) {
-      const float gv = ldv(g, r * ldg + c0 + c);
-      s += gv; q += gv * (ldv(y, r * ld + c0 + c) - mean) * rstd;
-    }
-    atomicAdd(bsum + c0 + c, s); atomicAdd(bsum + Ct + c0 + c, q);
-  }
-}
-// d(pre-activation) = act'(y) gamma rstd (g - mean(g) - xhat mean(g xhat)) -> dpre (bf16, pitch ldd, same column slice)
-template <typename TG, typename TY>
-__global__ void bn_bwd_apply_k(const TG* __restrict__ g, int ldg, const TY* __restrict__ y, int ld, int c0, const float* __restrict__ stats, int Ct,
-                               const float* __restrict__ bsum, const float* __restrict__ gamma, bf16* __restrict__ dpre, int ldd,
-                               float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows, int C, int act) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= rows * C) return;
-  const int c = int(e % C);
-  const long long r = e / C;
-  const float mean = stats[2 * Ct + c0 + c], rstd = stats[3 * Ct + c0 + c];
-  const float yv = ldv(y, r * ld + c0 + c);
-  const float xhat = (yv - mean) * rstd;
-  float dy = gamma[c] * rstd * (ldv(g, r * ldg + c0 + c) - bsum[c0 + c] / float(rows) - xhat * bsum[Ct + c0 + c] / float(rows));
-  if (act == 1) dy = yv > 0.f ? dy : 0.f;
-  dpre[r * ldd + c0 + c] = __float2bfloat16(dy);
-  if (e < C) { dgamma[c] += bsum[Ct + c0 + c]; dbeta[c] += bsum[c0 + c]; }
-}
-// column sums of [rows][ld] (first C columns) added to dst
-template <typename TS>
-__global__ void colsum_k(const TS* __restrict__ src, long long rows, int C, int ld, float* __restrict__ dst) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    float s = 0.f;
-    for (long long r = r0; r < r1; ++r) s += ldv(src, r * ld + c);
-    atomicAdd(dst + c, s);
-  }
-}
 // tf.layers.max_pooling1d(pool 2, stride 1, 'same'): out[t] = max(x[t], x[t + 1]) (last step: x[t])
 __global__ void maxpool_fwd_k(const bf16* __restrict__ x, bf16* __restrict__ out, long long N, int T, int C) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -346,20 +256,6 @@ __global__ void highway_bwd_k(const float* __restrict__ dh, const bf16* __restri
   dHT[r * 2 * HU + c] = __float2bfloat16(Hh > 0.f ? g * Tt : 0.f);
   dHT[r * 2 * HU + HU + c] = __float2bfloat16(g * (Hh - h[e]) * Tt * (1.f - Tt));
   dcarry[e] = g * (1.f - Tt);
-}
-// launch helpers shared by the engine and t2_dbg_cbhg_kernel; the callers zero the statistics / backward sums first
-template <typename TY>
-void bn_fwd_launch(const TY* y, int ld, int c0, bf16* xb, float* xf, const float* add, float* stats, int Ct, const float* gamma, const float* beta,
-                   float* mm, float* mv, long long rows, int C, int training, int stat_threads, cudaStream_t st) {
-  if (training) { bn_stats_k<TY><<<64, stat_threads, 0, st>>>(y, ld, c0, stats, Ct, rows, C); t2_count_launch(); }
-  bn_apply_k<TY><<<grid1d(rows * C), 256, 0, st>>>(y, ld, c0, xb, xf, add, stats, Ct, gamma, beta, mm, mv, rows, C, training); t2_count_launch();
-}
-template <typename T>
-void bn_bwd_launch(const T* g, int ldg, const T* y, int ld, int c0, const float* stats, int Ct, float* bsum, const float* gamma, bf16* dpre, int ldd,
-                   float* dgamma, float* dbeta, long long rows, int C, int act, int stat_threads, cudaStream_t st) {
-  bn_bwd_stats_k<T, T><<<64, stat_threads, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, rows, C); t2_count_launch();
-  bn_bwd_apply_k<T, T><<<grid1d(rows * C), 256, 0, st>>>(g, ldg, y, ld, c0, stats, Ct, bsum, gamma, dpre, ldd, dgamma, dbeta, rows, C, act);
-  t2_count_launch();
 }
 void maxpool_fwd(const bf16* x, bf16* out, long long N, int T, int C, cudaStream_t st) {
   maxpool_fwd_k<<<grid1d(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
@@ -654,45 +550,32 @@ int gemm(const void* a, int C, int ld, int k0, long long T, int Bn, const void* 
   return launch_act_gemm(EPI_BIAS_ACT, BN, g, st);
 }
 
-inline int conv_shift(int k, int j) { return j - (k - 1) / 2; }
 // wgrad launches, in the order t2_cbhg_backward issues them
 enum { WG_LIN = 0, WG_GRU = 1, WG_HW0 = 2 /* NH launches, last highway layer first */ };
 void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
   L.clear();
-  auto dense = [](int am, int bm, int shift = 0) {   // a plain weight gradient: maps, A time shift, scale 1
-    WgradTile t; memset(&t, 0, sizeof(t));
-    t.a_map = am; t.a_shift = shift; t.b_map = bm; t.scale = 1.f;
-    return t;
-  };
   const int RU = lo.RU, HU = lo.HU;
-  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense(0, 1), 0, 2 * RU, 0, lo.NF, lo.p_lk, lo.NF); L.push_back(w); }      // maps: 0 rnn out, 1 dlin
+  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense_proto(0, 1), 0, 2 * RU, 0, lo.NF, lo.p_lk, lo.NF); L.push_back(w); }      // maps: 0 rnn out, 1 dlin
   { std::vector<WgradTile> w;     // maps: 0 h_last (bf16 [N][HU]), 1 dXP, 2 rnn out, 3 rh fw, 4 rh bw
     for (int d = 0; d < 2; ++d) {
-      append_wgrad_tiles(w, dense(0, 1), 0, HU, d * 3 * RU, 2 * RU, lo.p_gk[d], 2 * RU);                                       // input rows of the gates kernel
-      append_wgrad_tiles(w, dense(0, 1), 0, HU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d], RU);                                      // input rows of the candidate kernel
-      append_wgrad_tiles(w, dense(2, 1, d == 0 ? -1 : 1), d * RU, RU, d * 3 * RU, 2 * RU, lo.p_gk[d] + (long long)HU * 2 * RU, 2 * RU);   // h_prev x d gates
-      append_wgrad_tiles(w, dense(3 + d, 1), 0, RU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d] + (long long)HU * RU, RU);             // (r h_prev) x d cand
+      append_wgrad_tiles(w, dense_proto(0, 1), 0, HU, d * 3 * RU, 2 * RU, lo.p_gk[d], 2 * RU);                                       // input rows of the gates kernel
+      append_wgrad_tiles(w, dense_proto(0, 1), 0, HU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d], RU);                                      // input rows of the candidate kernel
+      append_wgrad_tiles(w, dense_proto(2, 1, d == 0 ? -1 : 1), d * RU, RU, d * 3 * RU, 2 * RU, lo.p_gk[d] + (long long)HU * 2 * RU, 2 * RU);   // h_prev x d gates
+      append_wgrad_tiles(w, dense_proto(3 + d, 1), 0, RU, d * 3 * RU + 2 * RU, RU, lo.p_ck[d] + (long long)HU * RU, RU);             // (r h_prev) x d cand
     }
     L.push_back(w); }
   for (int i = lo.NH - 1; i >= 0; --i) {   // maps: 0 h_i (bf16), 1 dHT
     std::vector<WgradTile> w;
-    append_wgrad_tiles(w, dense(0, 1), 0, HU, 0, HU, lo.p_hk[i][0], HU);
-    append_wgrad_tiles(w, dense(0, 1), 0, HU, HU, HU, lo.p_hk[i][1], HU);
+    append_wgrad_tiles(w, dense_proto(0, 1), 0, HU, 0, HU, lo.p_hk[i][0], HU);
+    append_wgrad_tiles(w, dense_proto(0, 1), 0, HU, HU, HU, lo.p_hk[i][1], HU);
     L.push_back(w);
   }
-  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense(0, 1), 0, lo.M, 0, HU, lo.p_dk, HU); L.push_back(w); }               // dense: hin x dh0
-  auto conv = [&](const CConv& c, int a_ch0, int b_ch0) {
-    std::vector<WgradTile> w;
-    for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w, dense(0, 1, conv_shift(c.k, j)), a_ch0, c.cin, b_ch0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
-    L.push_back(w);
-  };
-  conv(lo.proj2, 0, 0);     // maps: 0 X1, 1 dY2b
-  conv(lo.proj1, 0, 0);     // maps: 0 P, 1 d1
+  { std::vector<WgradTile> w; append_wgrad_tiles(w, dense_proto(0, 1), 0, lo.M, 0, HU, lo.p_dk, HU); L.push_back(w); }               // dense: hin x dh0
+  for (const CConv* c : {&lo.proj2, &lo.proj1}) {   // maps: 0 X1, 1 dY2b / 0 P, 1 d1
+    std::vector<WgradTile> w; append_conv_wgrad_tiles(w, c->k, 0, c->cin, 0, c->cout, c->p.kernel); L.push_back(w);
+  }
   { std::vector<WgradTile> w;  // bank: maps 0 x0, 1 dbank (channel block k-1)
-    for (int k = 1; k <= lo.K; ++k) {
-      const CConv& c = lo.bank[k - 1];
-      for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w, dense(0, 1, conv_shift(c.k, j)), 0, c.cin, (k - 1) * lo.CC, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
-    }
+    for (int k = 1; k <= lo.K; ++k) append_conv_wgrad_tiles(w, k, 0, lo.M, (k - 1) * lo.CC, lo.CC, lo.bank[k - 1].p.kernel);
     L.push_back(w); }
 }
 
@@ -772,9 +655,9 @@ template <typename T> T* W(const Ctx& s, long long off) { return reinterpret_cas
 // conv (+ bias, activation) into `y` (bf16 [N][ldo] column slice or fp32), batch-norm statistics are taken by the caller
 int conv_fwd(const Ctx& s, const CConv& L, const void* x, int ld_x, bf16* y_b, float* y_f, int ldo) {
   int shifts[16];
-  for (int j = 0; j < L.k; ++j) shifts[j] = conv_shift(L.k, j);
+  for (int j = 0; j < L.k; ++j) shifts[j] = conv_tap_shift(L.k, j);
   const int BN = L.cout % 256 == 0 ? 256 : 128;
-  return gemm(x, L.cin, ld_x, 0, s.lo->T, s.lo->B, s.pk + L.k_w, (L.cout + 127) / 128 * 128, L.k * L.cinp, L.k, shifts, BN, s.params + L.p_b, L.act, y_b, y_f,
+  return gemm(x, L.cin, ld_x, 0, s.lo->T, s.lo->B, s.pk + L.k_w, (L.cout + 127) / 128 * 128, L.k * L.cinp, L.k, shifts, BN, s.params + L.p.bias, L.act, y_b, y_f,
               ldo, L.cout, s.st);
 }
 }  // namespace
@@ -803,8 +686,8 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
     const int c0 = (k - 1) * lo.CC;
     rc = conv_fwd(s, L, x0, M, Y + c0, nullptr, KC);
     if (rc) return rc;
-    bn_fwd_launch<bf16>(Y, KC, c0, Xb, nullptr, nullptr, stb, KC, d_params + L.p_g, d_params + L.p_be, d_params + L.p_mm, d_params + L.p_mv, N, lo.CC,
-                        training, 128, st);
+    bn_fwd(Y, KC, c0, Xb, 0, nullptr, nullptr, stb, KC, d_params + L.p.gamma, d_params + L.p.beta, d_params + L.p.mm, d_params + L.p.mv, N, lo.CC,
+           training, BnDropout{}, 128, st);
   }
   bf16* P = W<bf16>(s, lo.w_P);
   maxpool_fwd(Xb, P, N, T, KC, st);
@@ -813,8 +696,8 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   rc = conv_fwd(s, lo.proj1, P, KC, Y1, nullptr, PJc);
   if (rc) return rc;
   if (training) T2_CHECK_CUDA(cudaMemsetAsync(st1, 0, 2LL * PJc * sizeof(float), st));
-  bn_fwd_launch<bf16>(Y1, PJc, 0, X1, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p_g, d_params + lo.proj1.p_be, d_params + lo.proj1.p_mm,
-                      d_params + lo.proj1.p_mv, N, PJc, training, 256, st);
+  bn_fwd(Y1, PJc, 0, X1, 0, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p.gamma, d_params + lo.proj1.p.beta, d_params + lo.proj1.p.mm,
+         d_params + lo.proj1.p.mv, N, PJc, training, BnDropout{}, 256, st);
   float* Y2 = W<float>(s, lo.w_Y2); float* st2 = W<float>(s, lo.w_st2);
   rc = conv_fwd(s, lo.proj2, X1, PJc, nullptr, Y2, M);
   if (rc) return rc;
@@ -822,8 +705,8 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   // highway input = BN(proj2) + mel_outputs (modules.py:59); the fp32 sum goes through w_dhin (free until the backward pass)
   float* hin_f = W<float>(s, lo.w_dhin);
   bf16* hin = W<bf16>(s, lo.w_hin);
-  bn_fwd_launch<float>(Y2, M, 0, nullptr, hin_f, d_mel, st2, M, d_params + lo.proj2.p_g, d_params + lo.proj2.p_be, d_params + lo.proj2.p_mm,
-                       d_params + lo.proj2.p_mv, N, M, training, 128, st);
+  bn_fwd(Y2, M, 0, nullptr, 0, hin_f, d_mel, st2, M, d_params + lo.proj2.p.gamma, d_params + lo.proj2.p.beta, d_params + lo.proj2.p.mm,
+         d_params + lo.proj2.p.mv, N, M, training, BnDropout{}, 128, st);
   launch_f32_to_bf16(hin_f, hin, N * M, st);
   // ---- dense to the highway width, highway layers ----
   rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]), HU, HU, st);
@@ -899,7 +782,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   rc = gemm(dlin, lo.NF, lo.NFP, 0, T, B, s.pk + lo.k_linT, 2 * RU, NFK, 1, nullptr, 256, nullptr, 0, nullptr, dout, 2 * RU, 2 * RU, st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(out, 2 * RU, T, B), make_act(dlin, lo.NF, T, B, 1, lo.NFP)}; rc = wgrad(maps, 2); if (rc) return rc; }
-  colsum_k<bf16><<<64, 256, 0, st>>>(dlin, N, lo.NF, lo.NFP, d_grads + lo.p_lb); t2_count_launch();
+  colsum(dlin, N, lo.NF, lo.NFP, d_grads + lo.p_lb, 256, st);
   // ---- GRU ----
   bf16* dXP = W<bf16>(s, lo.w_dXP);
   {
@@ -920,8 +803,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     rc = wgrad(maps, 5); if (rc) return rc;
   }
   for (int d = 0; d < 2; ++d) {
-    colsum_k<bf16><<<64, 256, 0, st>>>(dXP + d * 3 * RU, N, 2 * RU, XPW, d_grads + lo.p_gb[d]); t2_count_launch();
-    colsum_k<bf16><<<64, 128, 0, st>>>(dXP + d * 3 * RU + 2 * RU, N, RU, XPW, d_grads + lo.p_cb[d]); t2_count_launch();
+    colsum(dXP + d * 3 * RU, N, 2 * RU, XPW, d_grads + lo.p_gb[d], 256, st);
+    colsum(dXP + d * 3 * RU + 2 * RU, N, RU, XPW, d_grads + lo.p_cb[d], 128, st);
   }
   float* dh = W<float>(s, lo.w_dh);
   rc = gemm(dXP, XPW, XPW, 0, T, B, s.pk + lo.k_gxT, HU, XPW, 1, nullptr, 128, nullptr, 0, nullptr, dh, HU, HU, st);
@@ -935,8 +818,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     if (rc) return rc;
     add_k<<<grid1d(N * HU), 256, 0, st>>>(dh, dcar, i == 0 ? W<bf16>(s, lo.w_dhb) : nullptr, N * HU); t2_count_launch();
     { ActT maps[2] = {make_act(W<bf16>(s, lo.w_hb[i]), HU, T, B), make_act(dHT, 2 * HU, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
-    colsum_k<bf16><<<64, 128, 0, st>>>(dHT, N, HU, 2 * HU, d_grads + lo.p_hb[i][0]); t2_count_launch();
-    colsum_k<bf16><<<64, 128, 0, st>>>(dHT + HU, N, HU, 2 * HU, d_grads + lo.p_hb[i][1]); t2_count_launch();
+    colsum(dHT, N, HU, 2 * HU, d_grads + lo.p_hb[i][0], 128, st);
+    colsum(dHT + HU, N, HU, 2 * HU, d_grads + lo.p_hb[i][1], 128, st);
   }
   // ---- dense ----
   bf16* dhb = W<bf16>(s, lo.w_dhb);
@@ -944,30 +827,30 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   rc = gemm(dhb, HU, HU, 0, T, B, s.pk + lo.k_denseT, 128, HU, 1, nullptr, 128, nullptr, 0, nullptr, dhin, M, M, st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_hin), M, T, B), make_act(dhb, HU, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
-  colsum_k<bf16><<<64, 128, 0, st>>>(dhb, N, HU, HU, d_grads + lo.p_db); t2_count_launch();
+  colsum(dhb, N, HU, HU, d_grads + lo.p_db, 128, st);
   // ---- proj2 (BN, linear) ----
   float* bsum = W<float>(s, lo.w_bsum);
   bf16* dY2b = W<bf16>(s, lo.w_dY2b);
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2LL * KC * sizeof(float), st));
-  bn_bwd_launch<float>(dhin, M, W<float>(s, lo.w_Y2), M, 0, W<float>(s, lo.w_st2), M, bsum, d_params + lo.proj2.p_g, dY2b, 128, d_grads + lo.proj2.p_g,
-                       d_grads + lo.proj2.p_be, N, M, 0, 128, st);
+  bn_bwd(dhin, M, W<float>(s, lo.w_Y2), M, 0, W<float>(s, lo.w_st2), M, bsum, d_params + lo.proj2.p.gamma, dY2b, 128, d_grads + lo.proj2.p.gamma,
+         d_grads + lo.proj2.p.beta, N, M, 0, BnDropout{}, 128, st);
   int sh[16];
   bf16* d2 = W<bf16>(s, lo.w_d2);
-  for (int j = 0; j < lo.PK; ++j) sh[j] = -conv_shift(lo.PK, j);
+  for (int j = 0; j < lo.PK; ++j) sh[j] = -conv_tap_shift(lo.PK, j);
   rc = gemm(dY2b, lo.proj2.coutp, 128, 0, T, B, s.pk + lo.proj2.k_wT, (PJc + 127) / 128 * 128, lo.PK * lo.proj2.coutp, lo.PK, sh, 256, nullptr, 0, d2, nullptr, PJc, PJc, st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_X1), PJc, T, B), make_act(dY2b, M, T, B, 1, 128)}; rc = wgrad(maps, 2); if (rc) return rc; }
-  colsum_k<bf16><<<64, 128, 0, st>>>(dY2b, N, M, 128, d_grads + lo.proj2.p_b); t2_count_launch();
+  colsum(dY2b, N, M, 128, d_grads + lo.proj2.p.bias, 128, st);
   // ---- proj1 (ReLU, BN) ----
   bf16* d1 = W<bf16>(s, lo.w_d1);
   T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2LL * KC * sizeof(float), st));
-  bn_bwd_launch<bf16>(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, d_params + lo.proj1.p_g, d1, PJc, d_grads + lo.proj1.p_g,
-                      d_grads + lo.proj1.p_be, N, PJc, 1, 256, st);
+  bn_bwd(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, d_params + lo.proj1.p.gamma, d1, PJc, d_grads + lo.proj1.p.gamma,
+         d_grads + lo.proj1.p.beta, N, PJc, 1, BnDropout{}, 256, st);
   bf16* dP = W<bf16>(s, lo.w_dP);
   rc = gemm(d1, PJc, PJc, 0, T, B, s.pk + lo.proj1.k_wT, KC, lo.PK * lo.proj1.coutp, lo.PK, sh, 256, nullptr, 0, dP, nullptr, KC, KC, st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_P), KC, T, B), make_act(d1, PJc, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
-  colsum_k<bf16><<<64, 256, 0, st>>>(d1, N, PJc, PJc, d_grads + lo.proj1.p_b); t2_count_launch();
+  colsum(d1, N, PJc, PJc, d_grads + lo.proj1.p.bias, 256, st);
   // ---- max-pool, conv bank ----
   bf16* dbank = W<bf16>(s, lo.w_dbank);
   maxpool_bwd(W<bf16>(s, lo.w_Xb), dP, dbank, N, T, KC, st);
@@ -976,9 +859,9 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   for (int k = 1; k <= lo.K; ++k) {
     const CConv& L = lo.bank[k - 1];
     const int c0 = (k - 1) * lo.CC;
-    bn_bwd_launch<bf16>(dbank, KC, W<bf16>(s, lo.w_Y), KC, c0, W<float>(s, lo.w_stb), KC, bsum, d_params + L.p_g, dpre, KC, d_grads + L.p_g,
-                        d_grads + L.p_be, N, lo.CC, 1, 128, st);
-    colsum_k<bf16><<<64, 128, 0, st>>>(dpre + c0, N, lo.CC, KC, d_grads + L.p_b); t2_count_launch();
+    bn_bwd(dbank, KC, W<bf16>(s, lo.w_Y), KC, c0, W<float>(s, lo.w_stb), KC, bsum, d_params + L.p.gamma, dpre, KC, d_grads + L.p.gamma,
+           d_grads + L.p.beta, N, lo.CC, 1, BnDropout{}, 128, st);
+    colsum(dpre + c0, N, lo.CC, KC, d_grads + L.p.bias, 128, st);
   }
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_x0), M, T, B), make_act(dpre, KC, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
   for (int g = 0; g < 3; ++g) {
@@ -986,7 +869,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     if (g >= lo.n_grp) { T2_CHECK_CUDA(cudaMemsetAsync(dx, 0, N * 128 * sizeof(float), st)); continue; }
     int shifts[16], k0s[16], n = 0;
     for (int l = lo.grp_first[g]; l < lo.grp_first[g + 1]; ++l)
-      for (int j = 0; j < lo.bank[l].k; ++j, ++n) { shifts[n] = -conv_shift(lo.bank[l].k, j); k0s[n] = l * lo.CC; }
+      for (int j = 0; j < lo.bank[l].k; ++j, ++n) { shifts[n] = -conv_tap_shift(lo.bank[l].k, j); k0s[n] = l * lo.CC; }
     rc = gemm(dpre, lo.CC, KC, 0, T, B, s.pk + lo.k_bankT[g], 128, n * lo.CC, n, shifts, 128, nullptr, 0, nullptr, dx, 128, M, st, k0s, KC);
     if (rc) return rc;
   }
@@ -1028,13 +911,13 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
                      p[5] && p[6] && p[7] && p[8],
                  T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_FWD: bad arguments");
       if (i[6])
-        bn_fwd_launch<float>(static_cast<const float*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
-                             static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
-                             static_cast<float*>(p[8]), rows, C, int(i[5]), thr, st);
+        bn_fwd(static_cast<const float*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), 0, static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+               static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
+               static_cast<float*>(p[8]), rows, C, int(i[5]), BnDropout{}, thr, st);
       else
-        bn_fwd_launch<bf16>(static_cast<const bf16*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
-                            static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
-                            static_cast<float*>(p[8]), rows, C, int(i[5]), thr, st);
+        bn_fwd(static_cast<const bf16*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), 0, static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+               static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
+               static_cast<float*>(p[8]), rows, C, int(i[5]), BnDropout{}, thr, st);
       break;
     }
     case T2_DBG_CBHG_BN_BWD: {
@@ -1044,13 +927,13 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
                      (thr == 128 || thr == 256) && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && p[7],
                  T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_BWD: bad arguments");
       if (i[9])
-        bn_bwd_launch<float>(static_cast<const float*>(p[0]), ldg, static_cast<const float*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
-                             static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
-                             static_cast<float*>(p[7]), rows, C, act, thr, st);
+        bn_bwd(static_cast<const float*>(p[0]), ldg, static_cast<const float*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
+               static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
+               static_cast<float*>(p[7]), rows, C, act, BnDropout{}, thr, st);
       else
-        bn_bwd_launch<bf16>(static_cast<const bf16*>(p[0]), ldg, static_cast<const bf16*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
-                            static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
-                            static_cast<float*>(p[7]), rows, C, act, thr, st);
+        bn_bwd(static_cast<const bf16*>(p[0]), ldg, static_cast<const bf16*>(p[1]), ld, c0, static_cast<const float*>(p[2]), Ct,
+               static_cast<float*>(p[3]), static_cast<const float*>(p[4]), static_cast<bf16*>(p[5]), ldd, static_cast<float*>(p[6]),
+               static_cast<float*>(p[7]), rows, C, act, BnDropout{}, thr, st);
       break;
     }
     case T2_DBG_CBHG_POOL_FWD:

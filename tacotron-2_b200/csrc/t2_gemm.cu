@@ -288,6 +288,18 @@ void append_wgrad_tiles(std::vector<WgradTile>& v, const WgradTile& proto, int a
     }
 }
 
+WgradTile dense_proto(int am, int bm, int a_shift) {
+  WgradTile t;
+  memset(&t, 0, sizeof(t));
+  t.a_map = am; t.a_shift = a_shift; t.b_map = bm; t.scale = 1.f;
+  return t;
+}
+
+void append_conv_wgrad_tiles(std::vector<WgradTile>& v, int k, int a_ch0, int Ca, int b_ch0, int Cb, long long out_off) {
+  for (int j = 0; j < k; ++j)
+    append_wgrad_tiles(v, dense_proto(0, 1, conv_tap_shift(k, j)), a_ch0, Ca, b_ch0, Cb, out_off + (long long)j * Ca * Cb, Cb);
+}
+
 // ------------------------------------------------------------------------------------------------------
 // Persistent layer chains: the gate/out GEMMs of every forward layer (or the dz/dx GEMMs of every backward layer) as ONE launch.
 // Each CTA takes tickets (ChainTicket; t2_wavenet.cu build_chain) from a global counter in launch order and runs the same tile body as act_gemm_kernel on

@@ -65,5 +65,12 @@ int launch_wgrad(const ActT* maps, int nmaps, const WgradTile* tiles_dev, int nt
 // [b_ch0, b_ch0 + Cb), row blocks outer; proto gives the maps, shifts, layers, scale, accumulate and div of every tile
 void append_wgrad_tiles(std::vector<WgradTile>& v, const WgradTile& proto, int a_ch0, int Ca, int b_ch0, int Cb, long long out_off,
                         int ldc);
+// proto of a plain weight gradient: A map am shifted by a_shift time steps, B map bm, scale 1
+WgradTile dense_proto(int am, int bm, int a_shift = 0);
+// tap j of a k-tap 'same' convolution reads input row t + conv_tap_shift(k, j) (an even k pads the extra row on the right)
+inline int conv_tap_shift(int k, int j) { return j - (k - 1) / 2; }
+// the tiles of a conv kernel [k][Ca][Cb] at out_off: per tap, in tap order, the dense weight gradient of map 0 (input, A channels from
+// a_ch0, shifted by the tap) x map 1 (output gradient, B channels from b_ch0)
+void append_conv_wgrad_tiles(std::vector<WgradTile>& v, int k, int a_ch0, int Ca, int b_ch0, int Cb, long long out_off);
 
 }  // namespace t2

@@ -31,6 +31,17 @@ bool regularized(const std::string& name) {
   return true;
 }
 
+ConvBnParams add_conv_bn_params(std::vector<Param>& table, long long& n_params, const std::string& prefix, int k, int cin, int cout) {
+  ConvBnParams p;
+  p.kernel = add_param(table, n_params, prefix + "kernel", {k, cin, cout});
+  p.bias = add_param(table, n_params, prefix + "bias", {cout});
+  p.gamma = add_param(table, n_params, prefix + "gamma", {cout});
+  p.beta = add_param(table, n_params, prefix + "beta", {cout});
+  p.mm = add_param(table, n_params, prefix + "moving_mean", {cout}, false);
+  p.mv = add_param(table, n_params, prefix + "moving_variance", {cout}, false);
+  return p;
+}
+
 int param_info(const std::vector<Param>& table, int i, char* name, int cap, long long* offset, int* ndim, int* shape4, int* trainable) {
   T2_REQUIRE(i >= 0 && i < int(table.size()), T2_ERR_INVALID_ARG, "tensor index %d out of range", i);
   T2_REQUIRE(name && cap > 0, T2_ERR_INVALID_ARG, "param_info: null name buffer");

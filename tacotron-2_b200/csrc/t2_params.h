@@ -32,6 +32,10 @@ struct Param {
 long long add_param(std::vector<Param>& table, long long& n_params, const std::string& name, std::initializer_list<int> shape,
                     bool trainable = true);
 bool regularized(const std::string& name);
+// offsets of a convolution + batch-norm block's tensors
+struct ConvBnParams { long long kernel, bias, gamma, beta, mm, mv; };
+// prefix + kernel [k][cin][cout], bias, gamma, beta (trainable) and moving_mean, moving_variance [cout], in that order
+ConvBnParams add_conv_bn_params(std::vector<Param>& table, long long& n_params, const std::string& prefix, int k, int cin, int cout);
 // the out-parameters of the *_param_info C-ABI functions; offset, ndim, shape4 and trainable may be NULL
 int param_info(const std::vector<Param>& table, int i, char* name, int cap, long long* offset, int* ndim, int* shape4, int* trainable);
 

@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "../../include/t2b200.h"
+#include "t2_batchnorm.h"
 #include "t2_common.cuh"
 #include "t2_gemm.h"
 #include "t2_params.h"
@@ -33,7 +34,7 @@ typedef __nv_bfloat16 bf16;
 
 struct ConvL {   // one conv + BN block
   int cin, cout, k, act;   // act: 1 relu, 2 tanh, 0 none
-  long long p_k, p_b, p_gamma, p_beta, p_mm, p_mv;
+  ConvBnParams p;
   long long k_w, k_wT;     // packed forward [cout][k*cinp], packed dgrad [cinp][k*cout]
   int cinp;                // cin rounded up to 64
   long long w_y, w_x;      // workspace: y (post-activation, pre-BN) bf16 [B][T][cout], x = block output bf16
@@ -91,16 +92,11 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   // ---- parameters (order == oracle/tacotron.py:param_shapes) ----
   lo.n_params = 0; lo.params.clear(); lo.enc.clear(); lo.post.clear();
   lo.p_emb = add_param(lo.params, lo.n_params, "inputs_embedding", {lo.NS, lo.E});
-  auto conv_params = [&](ConvL& L, const std::string& pre) {
-    L.p_k = add_param(lo.params, lo.n_params, pre + "kernel", {L.k, L.cin, L.cout}); L.p_b = add_param(lo.params, lo.n_params, pre + "bias", {L.cout});
-    L.p_gamma = add_param(lo.params, lo.n_params, pre + "gamma", {L.cout}); L.p_beta = add_param(lo.params, lo.n_params, pre + "beta", {L.cout});
-    L.p_mm = add_param(lo.params, lo.n_params, pre + "moving_mean", {L.cout}, false); L.p_mv = add_param(lo.params, lo.n_params, pre + "moving_variance", {L.cout}, false);
-  };
   int cin = lo.E;
   for (int i = 0; i < cfg->enc_conv_layers; ++i) {
     ConvL L; L.cin = cin; L.cout = lo.C; L.k = cfg->enc_conv_kernel; L.act = 1; L.stream = 10 + i;
     char b[64]; snprintf(b, sizeof(b), "encoder_convolutions/conv_layer_%d/", i + 1);
-    conv_params(L, b); lo.enc.push_back(L); cin = lo.C;
+    L.p = add_conv_bn_params(lo.params, lo.n_params, b, L.k, L.cin, L.cout); lo.enc.push_back(L); cin = lo.C;
   }
   const char* dn[2] = {"fw", "bw"};
   for (int d = 0; d < 2; ++d) {
@@ -126,7 +122,7 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   for (int i = 0; i < cfg->postnet_layers; ++i) {
     ConvL L; L.cin = cin; L.cout = lo.PC; L.k = cfg->postnet_kernel; L.act = (i + 1 < cfg->postnet_layers) ? 2 : 0; L.stream = 30 + i;
     char b[64]; snprintf(b, sizeof(b), "postnet_convolutions/conv_layer_%d/", i + 1);
-    conv_params(L, b); lo.post.push_back(L); cin = lo.PC;
+    L.p = add_conv_bn_params(lo.params, lo.n_params, b, L.k, L.cin, L.cout); lo.post.push_back(L); cin = lo.PC;
   }
   lo.p_ppk = add_param(lo.params, lo.n_params, "postnet_projection/kernel", {lo.PC, lo.M}); lo.p_ppb = add_param(lo.params, lo.n_params, "postnet_projection/bias", {lo.M});
 
@@ -139,10 +135,10 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
     L.k_w = pk.take(2LL * L.cout * L.k * L.cinp * (split ? 3 : 1));
     L.k_wT = pk.take(2LL * L.cinp * L.k * L.cout);
     for (int j = 0; j < L.k; ++j) {
-      if (split) add_pack_split(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp, 3 * j * L.cinp + 2 * L.cinp, L.cinp);
+      if (split) add_pack_split(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp, 3 * j * L.cinp + 2 * L.cinp, L.cinp);
       else
-      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd: [cout][tap j | cin]
-      add_pack(jobs, L.p_k + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.cout, 0, j * L.cout);     // dgrad: [cin][tap j | cout]
+      add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd: [cout][tap j | cin]
+      add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.cout, 0, j * L.cout);     // dgrad: [cin][tap j | cout]
     }
   };
   for (auto& L : lo.enc) conv_pack(L);
@@ -282,125 +278,6 @@ __global__ void embed_bwd_kernel(const int* __restrict__ idx, const bf16* __rest
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= npos * E) return;
   atomicAdd(dtable + (long long)idx[e / E] * E + e % E, __bfloat162float(dx[e]));
-}
-
-// per-channel shifted sums of y [rows][C]: stats[0..C) = sum (y - y[0]), stats[C..2C) = sum (y - y[0])^2. Subtracting the
-// channel's first row (a sample of the channel) keeps E[d^2] - E[d]^2 free of the cancellation that E[y^2] - mean^2 suffers
-// when |mean| >> std.
-__device__ __forceinline__ float ld_act(const bf16* p, long long i) { return __bfloat162float(p[i]); }
-__device__ __forceinline__ float ld_act(const float* p, long long i) { return p[i]; }
-template <typename TY>
-__global__ void bn_stats_kernel(const TY* __restrict__ y, float* __restrict__ stats, long long rows, int C) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float pv = ld_act(y, c);
-    float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) { const float v = ld_act(y, r * C + c) - pv; s += v; q += v * v; }
-    atomicAdd(stats + c, s); atomicAdd(stats + C + c, q);
-  }
-}
-// x = dropout(((y - mean) * rstd) * gamma + beta); writes mean / rstd into stats[2C..4C), updates the moving stats
-template <typename TY>
-__global__ void bn_apply_kernel(const TY* __restrict__ y, bf16* __restrict__ x, float* __restrict__ stats, const float* __restrict__ gamma,
-                                const float* __restrict__ beta, float* __restrict__ mm, float* __restrict__ mv, long long rows, int C,
-                                int training, float p, unsigned long long seed, const unsigned long long* step, int stream, int split) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= rows * C) return;
-  const int c = int(e % C);
-  float mean, rstd;
-  if (training) {
-    const float d = stats[c] / float(rows);
-    mean = ld_act(y, c) + d;
-    const float var = fmaxf(stats[C + c] / float(rows) - d * d, 0.f);
-    rstd = rsqrtf(var + 1e-3f);
-    if (e < C) {
-      stats[2 * C + c] = mean; stats[3 * C + c] = rstd;
-      mm[c] = 0.99f * mm[c] + 0.01f * mean; mv[c] = 0.99f * mv[c] + 0.01f * var;
-    }
-  } else { mean = mm[c]; rstd = rsqrtf(mv[c] + 1e-3f); }
-  float v = (ld_act(y, e) - mean) * rstd * gamma[c] + beta[c];
-  if (training && p > 0.f) {
-    if (step) seed += *step;
-    v = hash_uniform32(hash_seed(seed, uint32_t(stream)), (unsigned long long)e) >= p ? v / (1.f - p) : 0.f;
-  }
-  if (!split) { x[e] = __float2bfloat16(v); return; }
-  const bf16 hi = __float2bfloat16(v);
-  bf16* row = x + (e / C) * 2 * C + c;             // rows [hi(C) | lo(C)]
-  row[0] = hi; row[C] = __float2bfloat16(v - __bfloat162float(hi));
-}
-// backward sums: sg[c] = sum g, sgx[c] = sum g * xhat   (g = dout * dropout mask)
-__global__ void bn_bwd_stats_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ y, const float* __restrict__ stats,
-                                    float* __restrict__ bsum, long long rows, int C, float p, unsigned long long seed,
-                                    const unsigned long long* step, int stream) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  if (step) seed += *step;
-  const uint32_t hs = hash_seed(seed, uint32_t(stream));
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float mean = stats[2 * C + c], rstd = stats[3 * C + c];
-    float s = 0.f, q = 0.f;
-    for (long long r = r0; r < r1; ++r) {
-      float g = __bfloat162float(dout[r * C + c]);
-      if (p > 0.f) g = hash_uniform32(hs, (unsigned long long)(r * C + c)) >= p ? g / (1.f - p) : 0.f;
-      s += g; q += g * (__bfloat162float(y[r * C + c]) - mean) * rstd;
-    }
-    atomicAdd(bsum + c, s); atomicAdd(bsum + C + c, q);
-  }
-}
-__global__ void bn_bwd_apply_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ y, const float* __restrict__ stats,
-                                    const float* __restrict__ bsum, const float* __restrict__ gamma, bf16* __restrict__ dpre,
-                                    float* __restrict__ dgamma, float* __restrict__ dbeta, long long rows, int C, int act, float p,
-                                    unsigned long long seed, const unsigned long long* step, int stream) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= rows * C) return;
-  const int c = int(e % C);
-  if (step) seed += *step;
-  const float mean = stats[2 * C + c], rstd = stats[3 * C + c];
-  float g = __bfloat162float(dout[e]);
-  if (p > 0.f) g = hash_uniform32(hash_seed(seed, uint32_t(stream)), (unsigned long long)e) >= p ? g / (1.f - p) : 0.f;
-  const float yv = __bfloat162float(y[e]);
-  const float xhat = (yv - mean) * rstd;
-  float dy = gamma[c] * rstd * (g - bsum[c] / float(rows) - xhat * bsum[C + c] / float(rows));
-  if (act == 1) dy = yv > 0.f ? dy : 0.f;
-  else if (act == 2) dy *= (1.f - yv * yv);
-  dpre[e] = __float2bfloat16(dy);
-  if (e < C) { dgamma[c] += bsum[C + c]; dbeta[c] += bsum[c]; }
-}
-// conv-block batch norm, forward: stats [4C] (training: shifted sums, then mean / rstd; inference reads the moving statistics)
-template <typename TY>
-int bn_fwd(const TY* y, bf16* x, float* stats, const float* gamma, const float* beta, float* mm, float* mv, long long rows, int C, int training,
-           float p, unsigned long long seed, const unsigned long long* step, int stream, int split, cudaStream_t st) {
-  if (training) {
-    T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * C * sizeof(float), st));
-    bn_stats_kernel<TY><<<64, 256, 0, st>>>(y, stats, rows, C); t2_count_launch();
-  }
-  bn_apply_kernel<TY><<<grid1d(rows * C), 256, 0, st>>>(y, x, stats, gamma, beta, mm, mv, rows, C, training, p, seed, step, stream, split);
-  t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
-}
-// backward: stats [6C] as left by bn_fwd, the backward sums go to stats[4C..6C); dgamma / dbeta accumulate
-int bn_bwd(const bf16* dout, const bf16* y, float* stats, const float* gamma, bf16* dpre, float* dgamma, float* dbeta, long long rows, int C, int act,
-           float p, unsigned long long seed, const unsigned long long* step, int stream, cudaStream_t st) {
-  float* bsum = stats + 4 * C;
-  T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2 * C * sizeof(float), st));
-  bn_bwd_stats_kernel<<<64, 256, 0, st>>>(dout, y, stats, bsum, rows, C, p, seed, step, stream); t2_count_launch();
-  bn_bwd_apply_kernel<<<grid1d(rows * C), 256, 0, st>>>(dout, y, stats, bsum, gamma, dpre, dgamma, dbeta, rows, C, act, p, seed, step, stream);
-  t2_count_launch();
-  T2_CHECK_CUDA(cudaGetLastError());
-  return T2_OK;
-}
-
-// column sums of a bf16 [rows][ld] matrix (first C columns) into fp32 dst (+=), scaled
-__global__ void colsum_bf16_kernel(const bf16* __restrict__ src, long long rows, int C, int ld, float* __restrict__ dst, float scale) {
-  const long long per = (rows + gridDim.x - 1) / gridDim.x;
-  const long long r0 = blockIdx.x * per, r1 = r0 + per < rows ? r0 + per : rows;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    float s = 0.f;
-    for (long long r = r0; r < r1; ++r) s += __bfloat162float(src[r * ld + c]);
-    atomicAdd(dst + c, s * scale);
-  }
 }
 
 // memory [B][Ti][2H] -> values = memory * mask (BahdanauAttention memory masking)
@@ -831,23 +708,28 @@ int lstm_step(const StepCtx& s, const void* wrec, int H, int K, const void* stat
 int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, long long T, int training) {
   const TL& lo = *s.lo;
   int shifts[8];
-  for (int j = 0; j < L.k; ++j) shifts[j] = j - (L.k - 1) / 2;
+  for (int j = 0; j < L.k; ++j) shifts[j] = conv_tap_shift(L.k, j);
   const int split = lo.c.split_bf16;
   bf16* y = reinterpret_cast<bf16*>(s.ws + L.w_y);
   float* yf = reinterpret_cast<float*>(s.ws + L.w_y);     // split mode keeps the pre-batch-norm activation in fp32
   int rc = conv_gemm(x_in, L.cin, T, lo.B, s.pk + L.k_w, L.cout, L.k * L.cinp * (split ? 3 : 1), L.k, shifts, L.cout % 256 == 0 ? 256 : 128,
-                     const_cast<float*>(s.params + L.p_b), L.act, split ? nullptr : y,
+                     const_cast<float*>(s.params + L.p.bias), L.act, split ? nullptr : y,
                      split ? yf : nullptr, L.cout, L.cout, 0.f, 0, 0, nullptr, s.st, split);
   if (rc) return rc;
   float* stats = reinterpret_cast<float*>(s.ws + L.w_stats);
   const long long rows = (long long)lo.B * T;
   float* pp = const_cast<float*>(s.params);
   bf16* x = reinterpret_cast<bf16*>(s.ws + L.w_x);
+  const BnDropout drop{lo.c.dropout_rate, s.seed, s.d_step, L.stream};
+  if (training) T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * L.cout * sizeof(float), s.st));
   if (split)
-    return bn_fwd(yf, x, stats, s.params + L.p_gamma, s.params + L.p_beta, pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed,
-                  s.d_step, L.stream, 1, s.st);
-  return bn_fwd(y, x, stats, s.params + L.p_gamma, s.params + L.p_beta, pp + L.p_mm, pp + L.p_mv, rows, L.cout, training, lo.c.dropout_rate, s.seed,
-                s.d_step, L.stream, 0, s.st);
+    bn_fwd(yf, L.cout, 0, x, 1, nullptr, nullptr, stats, L.cout, s.params + L.p.gamma, s.params + L.p.beta, pp + L.p.mm, pp + L.p.mv, rows, L.cout,
+           training, drop, 256, s.st);
+  else
+    bn_fwd(y, L.cout, 0, x, 0, nullptr, nullptr, stats, L.cout, s.params + L.p.gamma, s.params + L.p.beta, pp + L.p.mm, pp + L.p.mv, rows, L.cout,
+           training, drop, 256, s.st);
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
 }
 
 
@@ -859,36 +741,27 @@ struct WgL { std::vector<WgradTile> tiles; };
 enum { WG_PP = 0, WG_POST0 = 1 /* .. +postnet layers */ };
 void build_tiles(const TL& lo, std::vector<WgL>& L) {
   L.clear();
-  auto dense = [](int am, int bm, int shift = 0) {   // a plain weight gradient: maps, A time shift, scale 1
-    WgradTile t; memset(&t, 0, sizeof(t));
-    t.a_map = am; t.a_shift = shift; t.b_map = bm; t.scale = 1.f;
-    return t;
-  };
   const int H = lo.H, D = lo.D, K1r = 2 * H + D, K2 = 2 * D, PIK = D + 2 * H;
-  auto conv = [&](const ConvL& c) {
-    WgL w;
-    for (int j = 0; j < c.k; ++j) append_wgrad_tiles(w.tiles, dense(0, 1, j - (c.k - 1) / 2), 0, c.cin, 0, c.cout, c.p_k + (long long)j * c.cin * c.cout, c.cout);
-    L.push_back(w);
-  };
-  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, lo.PC, 0, lo.M, lo.p_ppk, lo.M); L.push_back(w); }            // 0: postnet projection
+  auto conv = [&](const ConvL& c) { WgL w; append_conv_wgrad_tiles(w.tiles, c.k, 0, c.cin, 0, c.cout, c.p.kernel); L.push_back(w); };
+  { WgL w; append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, lo.PC, 0, lo.M, lo.p_ppk, lo.M); L.push_back(w); }            // 0: postnet projection
   for (int i = int(lo.post.size()) - 1; i >= 0; --i) conv(lo.post[i]);                                // 1..: postnet convs (reverse)
-  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, PIK, 0, lo.M, lo.p_fk, lo.M); append_wgrad_tiles(w.tiles, dense(0, 1), 0, PIK, lo.M, 1, lo.p_sk, 1); L.push_back(w); }  // proj
+  { WgL w; append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, PIK, 0, lo.M, lo.p_fk, lo.M); append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, PIK, lo.M, 1, lo.p_sk, 1); L.push_back(w); }  // proj
   { WgL w;                                                                                               // decoder LSTMs + prenet-to-LSTM
-    append_wgrad_tiles(w.tiles, dense(0, 1), 0, K2, 0, 4 * D, lo.p_l2k, 4 * D);                                          // maps: 0 S2, 1 dg2, 2 S1, 3 dg1, 4 pn2
-    append_wgrad_tiles(w.tiles, dense(2, 3), 0, K1r, 0, 4 * D, lo.p_l1k + (long long)lo.P2 * 4 * D, 4 * D);
-    append_wgrad_tiles(w.tiles, dense(4, 3), 0, lo.P2, 0, 4 * D, lo.p_l1k, 4 * D);
+    append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, K2, 0, 4 * D, lo.p_l2k, 4 * D);                                          // maps: 0 S2, 1 dg2, 2 S1, 3 dg1, 4 pn2
+    append_wgrad_tiles(w.tiles, dense_proto(2, 3), 0, K1r, 0, 4 * D, lo.p_l1k + (long long)lo.P2 * 4 * D, 4 * D);
+    append_wgrad_tiles(w.tiles, dense_proto(4, 3), 0, lo.P2, 0, 4 * D, lo.p_l1k, 4 * D);
     L.push_back(w); }
   { WgL w;                                                                                               // prenet + query layer
-    append_wgrad_tiles(w.tiles, dense(0, 1), 0, lo.P1, 0, lo.P2, lo.p_p2k, lo.P2);                                       // maps: 0 pn1, 1 dz2, 2 decin, 3 dz1, 4 PI, 5 dq_all
-    append_wgrad_tiles(w.tiles, dense(2, 3), 0, lo.M, 0, lo.P1, lo.p_p1k, lo.P1);
-    append_wgrad_tiles(w.tiles, dense(4, 5), 0, D, 0, lo.A, lo.p_qry, lo.A);
+    append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, lo.P1, 0, lo.P2, lo.p_p2k, lo.P2);                                       // maps: 0 pn1, 1 dz2, 2 decin, 3 dz1, 4 PI, 5 dq_all
+    append_wgrad_tiles(w.tiles, dense_proto(2, 3), 0, lo.M, 0, lo.P1, lo.p_p1k, lo.P1);
+    append_wgrad_tiles(w.tiles, dense_proto(4, 5), 0, D, 0, lo.A, lo.p_qry, lo.A);
     L.push_back(w); }
-  { WgL w; append_wgrad_tiles(w.tiles, dense(0, 1), 0, 2 * H, 0, lo.A, lo.p_mem, lo.A); L.push_back(w); }               // memory layer: values x dkeys
+  { WgL w; append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, 2 * H, 0, lo.A, lo.p_mem, lo.A); L.push_back(w); }               // memory layer: values x dkeys
   for (int d = 0; d < 2; ++d) {                                                                          // encoder LSTM d
     WgL w;  // maps: 0 h history (time-major), 1 gate grads time-major, 2 x3 (batch-major), 3 gate grads batch-major
-    append_wgrad_tiles(w.tiles, dense(0, 1), 0, H, 0, 4 * H, lo.p_elk[d] + (long long)lo.C * 4 * H, 4 * H);
+    append_wgrad_tiles(w.tiles, dense_proto(0, 1), 0, H, 0, 4 * H, lo.p_elk[d] + (long long)lo.C * 4 * H, 4 * H);
     L.push_back(w);
-    WgL w2; append_wgrad_tiles(w2.tiles, dense(0, 1), 0, lo.C, 0, 4 * H, lo.p_elk[d], 4 * H); L.push_back(w2);
+    WgL w2; append_wgrad_tiles(w2.tiles, dense_proto(0, 1), 0, lo.C, 0, 4 * H, lo.p_elk[d], 4 * H); L.push_back(w2);
   }
   for (int i = int(lo.enc.size()) - 1; i >= 0; --i) conv(lo.enc[i]);
 }
@@ -1365,17 +1238,18 @@ int conv_block_bwd(const StepCtx& s, const ConvL& L, const void* x_in, long long
   const long long rows = (long long)lo.B * T;
   float* stats = reinterpret_cast<float*>(s.ws + L.w_stats);
   const bf16* y = reinterpret_cast<const bf16*>(s.ws + L.w_y);
-  int rc = bn_bwd(dout, y, stats, s.params + L.p_gamma, dpre, grads + L.p_gamma, grads + L.p_beta, rows, L.cout, L.act, lo.c.dropout_rate, s.seed,
-                  s.d_step, L.stream, s.st);
-  if (rc) return rc;
-  colsum_bf16_kernel<<<64, 256, 0, s.st>>>(dpre, rows, L.cout, L.cout, grads + L.p_b, 1.f); t2_count_launch();
+  float* bsum = stats + 4 * L.cout;
+  T2_CHECK_CUDA(cudaMemsetAsync(bsum, 0, 2 * L.cout * sizeof(float), s.st));
+  bn_bwd(dout, L.cout, y, L.cout, 0, stats, L.cout, bsum, s.params + L.p.gamma, dpre, L.cout, grads + L.p.gamma, grads + L.p.beta, rows, L.cout, L.act,
+         BnDropout{lo.c.dropout_rate, s.seed, s.d_step, L.stream}, 256, s.st);
+  colsum(dpre, rows, L.cout, L.cout, grads + L.p.bias, 256, s.st);
   T2_CHECK_CUDA(cudaGetLastError());
   ActT maps[2] = {make_act(x_in, L.cin, int(T), lo.B), make_act(dpre, L.cout, int(T), lo.B)};
-  rc = launch_wgrad(maps, 2, tiles, ntiles, grads, int(T), lo.B, s.st);
+  int rc = launch_wgrad(maps, 2, tiles, ntiles, grads, int(T), lo.B, s.st);
   if (rc) return rc;
   if (dx) {
     int shifts[8];
-    for (int j = 0; j < L.k; ++j) shifts[j] = (L.k - 1) / 2 - j;
+    for (int j = 0; j < L.k; ++j) shifts[j] = -conv_tap_shift(L.k, j);
     rc = conv_gemm(dpre, L.cout, T, lo.B, s.pk + L.k_wT, L.cin, L.k * L.cout, L.k, shifts, L.cin % 256 == 0 ? 256 : 128, nullptr, 0, dx, nullptr, L.cin,
                    L.cin, 0.f, 0, 0, nullptr, s.st);
     if (rc) return rc;
@@ -1854,7 +1728,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   {
     ActT maps[2] = {make_act(ws + lo.post.back().w_x, lo.PC, To, B), make_act(dmel, 128, To, B)};
     rc = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, To, B, st); if (rc) return rc; ++li;
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(dmel, BTo, M, 128, d_grads + lo.p_ppb, 1.f); t2_count_launch();
+    colsum(dmel, BTo, M, 128, d_grads + lo.p_ppb, 256, st);
   }
   // teacher_forcing_ratio < 1: the frame projection's gradient of step t waits for step t + 1's prenet backward inside the loop below,
   // which writes the prenet gradients into w_dz step by step; the decoder-output gradient then goes to dY0 (the first postnet block's
@@ -1877,8 +1751,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   auto proj_wgrad = [&]() -> int {
     ActT maps[2] = {make_act(PI, PIK, int(TB), 1), make_act(ddec_tm, 128, int(TB), 1)};
     int r = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, int(TB), 1, st); if (r) return r; ++li;
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(ddec_tm, TB, M, 128, d_grads + lo.p_fb, 1.f); t2_count_launch();
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(ddec_tm + M, TB, 1, 128, d_grads + lo.p_sb, 1.f); t2_count_launch();
+    colsum(ddec_tm, TB, M, 128, d_grads + lo.p_fb, 256, st);
+    colsum(ddec_tm + M, TB, 1, 128, d_grads + lo.p_sb, 256, st);
     return T2_OK;
   };
   if (!per_step) {
@@ -1995,8 +1869,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     ActT maps[5] = {make_act(ws + lo.w_S2, K2, int(TB), 1), make_act(dg2, 4 * D, int(TB), 1), make_act(ws + lo.w_S1, K1r, int(TB), 1),
                     make_act(dg1, 4 * D, int(TB), 1), make_act(pn2, lo.P2, int(TB), 1)};
     rc = launch_wgrad(maps, 5, TILES(li), NT(li), d_grads, int(TB), 1, st); if (rc) return rc; ++li;
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(dg2, TB, 4 * D, 4 * D, d_grads + lo.p_l2b, 1.f); t2_count_launch();
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(dg1, TB, 4 * D, 4 * D, d_grads + lo.p_l1b, 1.f); t2_count_launch();
+    colsum(dg2, TB, 4 * D, 4 * D, d_grads + lo.p_l2b, 256, st);
+    colsum(dg1, TB, 4 * D, 4 * D, d_grads + lo.p_l1b, 256, st);
   }
   if (!per_step) {   // prenet data gradients over all steps (the per-step path wrote them inside the loop)
     rc = conv_gemm(dg1, 4 * D, TB, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2, nullptr, lo.P2, lo.P2, 0.f,
@@ -2012,8 +1886,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     ActT maps[6] = {make_act(pn1, lo.P1, int(TB), 1), make_act(dz2, lo.P2, int(TB), 1), make_act(ws + lo.w_decin, M, int(TB), 1),
                     make_act(dpn1, lo.P1, int(TB), 1), make_act(PI, PIK, int(TB), 1), make_act(dq_all, A, int(TB), 1)};
     rc = launch_wgrad(maps, 6, TILES(li), NT(li), d_grads, int(TB), 1, st); if (rc) return rc; ++li;
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(dz2, TB, lo.P2, lo.P2, d_grads + lo.p_p2b, 1.f); t2_count_launch();
-    colsum_bf16_kernel<<<64, 256, 0, st>>>(dpn1, TB, lo.P1, lo.P1, d_grads + lo.p_p1b, 1.f); t2_count_launch();
+    colsum(dz2, TB, lo.P2, lo.P2, d_grads + lo.p_p2b, 256, st);
+    colsum(dpn1, TB, lo.P1, lo.P1, d_grads + lo.p_p1b, 256, st);
   }
   {
     float* scratch = reinterpret_cast<float*>(ws + lo.w_attU) + (lo.KA + 1) * A;   // [(KA+2)][A] reduced accumulators
@@ -2066,7 +1940,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
       rc = launch_wgrad(maps, 2, TILES(li), NT(li), d_grads, Ti * B, 1, sx); if (rc) return rc; ++li;
       ActT maps2[2] = {make_act(x3, lo.C, Ti, B), make_act(dpre, 4 * H, Ti, B)};
       rc = launch_wgrad(maps2, 2, TILES(li), NT(li), d_grads, Ti, B, sx); if (rc) return rc; ++li;
-      colsum_bf16_kernel<<<64, 256, 0, sx>>>(dpre, (long long)B * Ti, 4 * H, 4 * H, d_grads + lo.p_elb[d], 1.f); t2_count_launch();
+      colsum(dpre, (long long)B * Ti, 4 * H, 4 * H, d_grads + lo.p_elb[d], 256, sx);
     }
   }
   if (side) {
@@ -2177,13 +2051,17 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_REQUIRE(rows >= 1 && C >= 1 && C <= 4096 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && (i[2] == 0 || i[2] == 1) &&
                      (i[3] == 0 || i[3] == 1) && (i[5] == 0 || i[5] == 1) && i[4] >= 0 && call->f[0] >= 0.f && call->f[0] < 1.f,
                  T2_ERR_INVALID_ARG, "dbg_taco_kernel BN_FWD: bad arguments");
+      float* stats = static_cast<float*>(p[2]);
+      const BnDropout drop{call->f[0], call->seed, call->step, int(i[4])};
+      if (i[2]) T2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 2 * C * sizeof(float), st));
       if (i[3])
-        return bn_fwd(static_cast<const float*>(p[0]), static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
-                      static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
-                      call->step, int(i[4]), int(i[5]), st);
-      return bn_fwd(static_cast<const bf16*>(p[0]), static_cast<bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
-                    static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
-                    call->step, int(i[4]), int(i[5]), st);
+        bn_fwd(static_cast<const float*>(p[0]), C, 0, static_cast<bf16*>(p[1]), int(i[5]), nullptr, nullptr, stats, C, static_cast<const float*>(p[3]),
+               static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), drop, 256, st);
+      else
+        bn_fwd(static_cast<const bf16*>(p[0]), C, 0, static_cast<bf16*>(p[1]), int(i[5]), nullptr, nullptr, stats, C, static_cast<const float*>(p[3]),
+               static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), drop, 256, st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
     }
     case T2_DBG_TACO_BN_BWD: {
       const long long rows = i[0];
@@ -2191,9 +2069,13 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_REQUIRE(rows >= 1 && C >= 1 && C <= 4096 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[6] && i[2] >= 0 && i[2] <= 2 &&
                      i[3] >= 0 && call->f[0] >= 0.f && call->f[0] < 1.f,
                  T2_ERR_INVALID_ARG, "dbg_taco_kernel BN_BWD: bad arguments");
-      return bn_bwd(static_cast<const bf16*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
-                    static_cast<bf16*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]), call->f[0], call->seed,
-                    call->step, int(i[3]), st);
+      float* stats = static_cast<float*>(p[2]);
+      T2_CHECK_CUDA(cudaMemsetAsync(stats + 4 * C, 0, 2 * C * sizeof(float), st));
+      bn_bwd(static_cast<const bf16*>(p[0]), C, static_cast<const bf16*>(p[1]), C, 0, stats, C, stats + 4 * C, static_cast<const float*>(p[3]),
+             static_cast<bf16*>(p[4]), C, static_cast<float*>(p[5]), static_cast<float*>(p[6]), rows, C, int(i[2]),
+             BnDropout{call->f[0], call->seed, call->step, int(i[3])}, 256, st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
     }
     case T2_DBG_TACO_CELL_BWD: {
       CellBwd c;
