@@ -158,13 +158,22 @@ int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
  * POOL_FWD     maxpool_fwd_k. p: x bf16 [N][C], out. i: N (= B T rows), T, C.
  * POOL_BWD     maxpool_bwd_k. p: x, dout, dx. i: N, T, C.
  * HIGHWAY_FWD  highway_fwd_k. p: pre fp32 [N][2HU], bh, bt, h fp32 [N][HU], hf fp32, hb bf16, HT bf16 [N][2HU] (nullable). i: N, HU.
- * HIGHWAY_BWD  highway_bwd_k. p: dh fp32, HT bf16, h fp32, dHT bf16 [N][2HU], dcarry fp32. i: N, HU. */
+ * HIGHWAY_BWD  highway_bwd_k. p: dh fp32, HT bf16, h fp32, dHT bf16 [N][2HU], dcarry fp32. i: N, HU.
+ * GRU_FWD      gru_fwd_kernel, both directions over the whole padded sequence (rows b T + t, N = B T). p: params fp32 (flat; the kernel
+ *              reads the recurrent rows [HU, HU + RU) of the two kernels and the biases), XP fp32 [N][6RU] ([fw gates | fw cand | bw gates
+ *              | bw cand], no biases), out bf16 [N][2RU], then the stashes bf16 [N][RU] r, u, c, rh of fw, then of bw (all eight present,
+ *              or all null as in inference). i: B, T, HU, RU (= 128), then p_gk, p_ck, p_gb, p_cb of fw, then of bw (offsets into params).
+ * GRU_BWD      gru_bwd_kernel (BPTT of both directions). p: params, dout fp32 [N][2RU], out bf16 [N][2RU] (h_prev, as GRU_FWD writes it),
+ *              the stashes r, u, c of fw, then of bw, dXP bf16 [N][6RU] (out: [dr_pre | du_pre | dc_pre] per direction).
+ *              i: B, T, HU, RU (= 128), then p_gk, p_ck of fw, then of bw. */
 #define T2_DBG_CBHG_BN_FWD 1
 #define T2_DBG_CBHG_BN_BWD 2
 #define T2_DBG_CBHG_POOL_FWD 3
 #define T2_DBG_CBHG_POOL_BWD 4
 #define T2_DBG_CBHG_HIGHWAY_FWD 5
 #define T2_DBG_CBHG_HIGHWAY_BWD 6
+#define T2_DBG_CBHG_GRU_FWD 7
+#define T2_DBG_CBHG_GRU_BWD 8
 int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream);
 
 

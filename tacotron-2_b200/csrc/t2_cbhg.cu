@@ -582,6 +582,50 @@ void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
 size_t gru_fwd_smem() { return (64 * 256 + 64 * 128) * 4 + 3 * kGruItems * kRU * 4; }
 size_t gru_bwd_smem() { return (128 * 128 + 64 * 128) * 4 + (2 * kGruItems * kRU + kGruItems * 2 * kRU) * 4; }
 
+// launch helpers shared by t2_cbhg_forward / t2_cbhg_backward and t2_dbg_cbhg_kernel: one grid (B / 4 items x 2 directions), block and
+// shared-memory size. The checks run before any driver call.
+int gru_setup() {
+  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem())));
+  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_bwd_smem())));
+  return T2_OK;
+}
+int check_gru_shape(int B, int T, int HU, int RU, const char* what) {
+  T2_REQUIRE(B >= 1 && T >= 1 && HU >= 1, T2_ERR_UNSUPPORTED_SHAPE, "%s: B >= 1, T >= 1, HU >= 1 (B %d, T %d, HU %d)", what, B, T, HU);
+  T2_REQUIRE(RU == kRU, T2_ERR_UNSUPPORTED_SHAPE, "%s: RU must be %d (got %d)", what, kRU, RU);
+  return T2_OK;
+}
+int check_gru_fwd(const GruArgs& a) {
+  T2_REQUIRE(a.params && a.XP && a.out, T2_ERR_INVALID_ARG, "gru_fwd: null params / XP / out");
+  int n = 0;
+  for (int d = 0; d < 2; ++d) n += (a.r[d] != nullptr) + (a.u[d] != nullptr) + (a.c[d] != nullptr) + (a.rh[d] != nullptr);
+  T2_REQUIRE(n == 0 || n == 8, T2_ERR_INVALID_ARG, "gru_fwd: the r / u / c / rh stashes of both directions are all present or all null (%d of 8)", n);
+  for (int d = 0; d < 2; ++d)
+    T2_REQUIRE(a.p_gk[d] >= 0 && a.p_ck[d] >= 0 && a.p_gb[d] >= 0 && a.p_cb[d] >= 0, T2_ERR_INVALID_ARG, "gru_fwd: negative parameter offset");
+  return check_gru_shape(a.B, a.T, a.HU, a.RU, "gru_fwd");
+}
+int check_gru_bwd(const GruBwdArgs& a) {
+  T2_REQUIRE(a.params && a.dout && a.out && a.dXP, T2_ERR_INVALID_ARG, "gru_bwd: null params / dout / out / dXP");
+  for (int d = 0; d < 2; ++d) {
+    T2_REQUIRE(a.r[d] && a.u[d] && a.c[d], T2_ERR_INVALID_ARG, "gru_bwd: null stash of direction %d", d);
+    T2_REQUIRE(a.p_gk[d] >= 0 && a.p_ck[d] >= 0, T2_ERR_INVALID_ARG, "gru_bwd: negative parameter offset");
+  }
+  return check_gru_shape(a.B, a.T, a.HU, a.RU, "gru_bwd");
+}
+int launch_gru_fwd(const GruArgs& a, cudaStream_t st) {
+  int rc = check_gru_fwd(a);
+  if (rc) return rc;
+  gru_fwd_kernel<<<dim3((a.B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_fwd_smem(), st>>>(a); t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+int launch_gru_bwd(const GruBwdArgs& a, cudaStream_t st) {
+  int rc = check_gru_bwd(a);
+  if (rc) return rc;
+  gru_bwd_kernel<<<dim3((a.B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_bwd_smem(), st>>>(a); t2_count_launch();
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+
 }  // namespace
 }  // namespace t2
 
@@ -624,8 +668,8 @@ extern "C" int t2_cbhg_init(const t2_cbhg_config_t* cfg, void* d_packed, void* d
   T2_CHECK_CUDA(cudaMemcpyAsync(ws + lo.w_tiles, all.data(), all.size() * sizeof(WgradTile), cudaMemcpyHostToDevice, st));
   rc = upload_reg_table(lo.params, ws + lo.w_regtab, st);
   if (rc) return rc;
-  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem())));
-  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_bwd_smem())));
+  rc = gru_setup();
+  if (rc) return rc;
   T2_CHECK_CUDA(cudaStreamSynchronize(st));
   return T2_OK;
 }
@@ -732,8 +776,8 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
       if (training) { a.r[d] = W<bf16>(s, lo.w_gr[d]); a.u[d] = W<bf16>(s, lo.w_gu[d]); a.c[d] = W<bf16>(s, lo.w_gc[d]); a.rh[d] = W<bf16>(s, lo.w_grh[d]); }
     }
     a.XP = XP; a.out = W<bf16>(s, lo.w_out); a.B = B; a.T = T; a.HU = HU; a.RU = RU;
-    gru_fwd_kernel<<<dim3((B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_fwd_smem(), st>>>(a); t2_count_launch();
-    T2_CHECK_CUDA(cudaGetLastError());
+    rc = launch_gru_fwd(a, st);
+    if (rc) return rc;
   }
   // ---- linear projection, clip, loss ----
   float* lin = W<float>(s, lo.w_lin);
@@ -794,8 +838,8 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
       a.r[d] = W<bf16>(s, lo.w_gr[d]); a.u[d] = W<bf16>(s, lo.w_gu[d]); a.c[d] = W<bf16>(s, lo.w_gc[d]);
     }
     a.dout = dout; a.out = out; a.dXP = dXP; a.B = B; a.T = T; a.HU = HU; a.RU = RU;
-    gru_bwd_kernel<<<dim3((B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_bwd_smem(), st>>>(a); t2_count_launch();
-    T2_CHECK_CUDA(cudaGetLastError());
+    rc = launch_gru_bwd(a, st);
+    if (rc) return rc;
   }
   {
     ActT maps[5] = {make_act(W<bf16>(s, lo.w_hb[lo.NH]), HU, T, B), make_act(dXP, XPW, T, B), make_act(out, 2 * RU, T, B),
@@ -891,6 +935,24 @@ extern "C" int t2_cbhg_workspace_tensor(const t2_cbhg_config_t* cfg, void* d_wor
   else if (n == "rnn_outputs") { off = lo.w_out; cnt = lo.N * 2 * lo.RU; }     // bf16 [B][T][2 RU]
   else if (n == "highway_input") { off = lo.w_hin; cnt = lo.N * lo.M; }        // bf16 [B][T][M]
   else if (n == "bank_outputs") { off = lo.w_Xb; cnt = lo.N * lo.KC; }         // bf16 [B][T][K CC] (after batch norm)
+  else if (n == "gru_input") { off = lo.w_hb[lo.NH]; cnt = lo.N * lo.HU; }     // bf16 [B][T][HU]: the last highway output
+  // fp32 [B][T][6 RU] input projections [fw gates | fw cand | bw gates | bw cand] (no biases); valid between the forward and the
+  // backward pass only: the highway backward reuses the buffer
+  else if (n == "gru_xp") { off = lo.w_XP; cnt = lo.N * 6 * lo.RU; }
+  else if (n == "gru_dout") { off = lo.w_dout; cnt = lo.N * 2 * lo.RU; }       // fp32 [B][T][2 RU]: d loss / d rnn_outputs
+  else if (n == "gru_dxp") { off = lo.w_dXP; cnt = lo.N * 6 * lo.RU; }         // bf16 [B][T][6 RU]: [dr_pre | du_pre | dc_pre] per direction
+  else {
+    // training stashes, bf16 [B][T][RU]: gru_{r,u,c,rh}_{fw,bw} (reset gate, update gate, candidate, r * h_prev)
+    const char* dn[2] = {"fw", "bw"};
+    for (int d = 0; d < 2 && off < 0; ++d) {
+      const std::string sfx = std::string("_") + dn[d];
+      if (n == "gru_r" + sfx) off = lo.w_gr[d];
+      else if (n == "gru_u" + sfx) off = lo.w_gu[d];
+      else if (n == "gru_c" + sfx) off = lo.w_gc[d];
+      else if (n == "gru_rh" + sfx) off = lo.w_grh[d];
+    }
+    cnt = lo.N * lo.RU;
+  }
   T2_REQUIRE(off >= 0, T2_ERR_INVALID_ARG, "cbhg_workspace_tensor: unknown tensor '%s'", name);
   *ptr = ws + off;
   if (count) *count = cnt;
@@ -955,6 +1017,38 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
       highway_bwd(static_cast<const float*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<const float*>(p[2]), static_cast<bf16*>(p[3]),
                   static_cast<float*>(p[4]), i[0], int(i[1]), st);
       break;
+    case T2_DBG_CBHG_GRU_FWD: {
+      GruArgs a;
+      memset(&a, 0, sizeof(a));
+      a.params = static_cast<const float*>(p[0]); a.XP = static_cast<const float*>(p[1]); a.out = static_cast<bf16*>(p[2]);
+      for (int d = 0; d < 2; ++d) {
+        a.r[d] = static_cast<bf16*>(p[3 + 4 * d]); a.u[d] = static_cast<bf16*>(p[4 + 4 * d]);
+        a.c[d] = static_cast<bf16*>(p[5 + 4 * d]); a.rh[d] = static_cast<bf16*>(p[6 + 4 * d]);
+        a.p_gk[d] = i[4 + 4 * d]; a.p_ck[d] = i[5 + 4 * d]; a.p_gb[d] = i[6 + 4 * d]; a.p_cb[d] = i[7 + 4 * d];
+      }
+      for (int k = 0; k < 4; ++k)   // B, T, HU, RU: in int range before the narrowing below
+        T2_REQUIRE(i[k] >= 1 && i[k] <= (1 << 20), T2_ERR_UNSUPPORTED_SHAPE, "dbg_cbhg_kernel GRU_FWD: B, T, HU, RU must be in [1, 2^20] (i[%d] = %lld)", k, i[k]);
+      a.B = int(i[0]); a.T = int(i[1]); a.HU = int(i[2]); a.RU = int(i[3]);
+      int rc = check_gru_fwd(a);
+      if (!rc) rc = gru_setup();
+      return rc ? rc : launch_gru_fwd(a, st);
+    }
+    case T2_DBG_CBHG_GRU_BWD: {
+      GruBwdArgs a;
+      memset(&a, 0, sizeof(a));
+      a.params = static_cast<const float*>(p[0]); a.dout = static_cast<const float*>(p[1]); a.out = static_cast<const bf16*>(p[2]);
+      for (int d = 0; d < 2; ++d) {
+        a.r[d] = static_cast<const bf16*>(p[3 + 3 * d]); a.u[d] = static_cast<const bf16*>(p[4 + 3 * d]); a.c[d] = static_cast<const bf16*>(p[5 + 3 * d]);
+        a.p_gk[d] = i[4 + 2 * d]; a.p_ck[d] = i[5 + 2 * d];
+      }
+      a.dXP = static_cast<bf16*>(p[9]);
+      for (int k = 0; k < 4; ++k)   // B, T, HU, RU: in int range before the narrowing below
+        T2_REQUIRE(i[k] >= 1 && i[k] <= (1 << 20), T2_ERR_UNSUPPORTED_SHAPE, "dbg_cbhg_kernel GRU_BWD: B, T, HU, RU must be in [1, 2^20] (i[%d] = %lld)", k, i[k]);
+      a.B = int(i[0]); a.T = int(i[1]); a.HU = int(i[2]); a.RU = int(i[3]);
+      int rc = check_gru_bwd(a);
+      if (!rc) rc = gru_setup();
+      return rc ? rc : launch_gru_bwd(a, st);
+    }
     default:
       return t2_set_error(T2_ERR_INVALID_ARG, "dbg_cbhg_kernel: unknown kernel id %d", call->kernel);
   }

@@ -29,8 +29,9 @@ still be NaN (or exactly 0 where the kernel promises it), and NaN in the unread 
 
 COVERAGE maps every __global__ kernel of the two files and of the kernels they share (t2_params.cu, t2_batchnorm.cu) to the test here that
 launches it (the shared batch-norm kernels are launched by both the Tacotron and the CBHG batch-norm tests);
-EXEMPT names the existing end-to-end test that covers each plumbing kernel (packing, embedding, losses, column sums). att_bwd_kernel and the two GRU kernels are listed apart, in
-NOT_YET_ISOLATED: they are checked only end to end until their own hooks and tests exist.
+a COVERAGE value is either the name of a test here or `file::test` for a per-kernel test in another module (att_bwd_kernel:
+tests/test_attention_state_gpu.py; the two GRU kernels: tests/test_cbhg_gru_gpu.py). EXEMPT names the existing end-to-end test that covers
+each plumbing kernel (packing, embedding, losses, column sums).
 test_every_engine_and_shared_kernel_is_covered (CPU) fails for a kernel added without an entry."""
 import ctypes
 import math
@@ -64,7 +65,8 @@ COVERAGE = {
     "bn_bwd_stats_kernel": "test_taco_bn_bwd", "bn_bwd_apply_kernel": "test_taco_bn_bwd",
     "maxpool_fwd_k": "test_maxpool", "maxpool_bwd_k": "test_maxpool", "highway_fwd_k": "test_highway", "highway_bwd_k": "test_highway",
     "lstm_cell_bwd_kernel": "test_lstm_cell_bwd", "att_finish_kernel": "test_att_finish", "att_finish2_kernel": "test_att_finish",
-    "dvalues_ctx_kernel": "test_dvalues_ctx",
+    "dvalues_ctx_kernel": "test_dvalues_ctx", "att_bwd_kernel": "test_attention_state_gpu.py::test_att_bwd",
+    "gru_fwd_kernel": "test_cbhg_gru_gpu.py::test_gru_fwd", "gru_bwd_kernel": "test_cbhg_gru_gpu.py::test_gru_bwd",
 }
 _TACO_E2E = "test_tacotron_gpu.py::test_backward_matches_oracle"
 _CBHG_E2E = "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle"
@@ -80,9 +82,6 @@ EXEMPT = {
     "add_k": _CBHG_E2E, "lin_finish_k": _CBHG_E2E,
     "lin_norm_k": "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle", "loss_out_k": _CBHG_E2E, "dmel_k": _CBHG_E2E,
 }
-# Kernels whose per-kernel float64 tests are still to be written (hooks and tests for them are the next change); until then only the
-# end-to-end gradient tests named here see them. Nothing may be added to this list.
-NOT_YET_ISOLATED = {"att_bwd_kernel": _TACO_E2E, "gru_fwd_kernel": _CBHG_E2E, "gru_bwd_kernel": _CBHG_E2E}
 
 
 def test_every_engine_and_shared_kernel_is_covered():
@@ -93,15 +92,11 @@ def test_every_engine_and_shared_kernel_is_covered():
         src = open(os.path.join(ROOT, "tacotron-2_b200", "csrc", f)).read()
         names |= set(re.findall(r"__global__\s+void\s+(?:__launch_bounds__\([^)]*\)\s+)?(\w+)\s*\(", src))
     assert len(names) >= 39
-    missing = sorted(n for n in names if n not in COVERAGE and n not in EXEMPT and n not in NOT_YET_ISOLATED)
+    missing = sorted(n for n in names if n not in COVERAGE and n not in EXEMPT)
     assert not missing, "kernels without a test: %s" % missing
-    assert not set(COVERAGE) & set(EXEMPT) and not (set(COVERAGE) | set(EXEMPT)) & set(NOT_YET_ISOLATED)
-    assert sorted(NOT_YET_ISOLATED) == ["att_bwd_kernel", "gru_bwd_kernel", "gru_fwd_kernel"]
-    here = open(os.path.abspath(__file__)).read()
-    for k, t in COVERAGE.items():
-        assert re.search(r"^def %s\(" % t, here, re.M), (k, t)
-    for k, t in list(EXEMPT.items()) + list(NOT_YET_ISOLATED.items()):
-        f, name = t.split("::")
+    assert not set(COVERAGE) & set(EXEMPT)
+    for k, t in list(COVERAGE.items()) + list(EXEMPT.items()):
+        f, name = t.split("::") if "::" in t else (os.path.basename(__file__), t)
         assert re.search(r"^def %s\(" % name, open(os.path.join(ROOT, "tests", f)).read(), re.M), (k, t)
 
 
