@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define T2B200_ABI_VERSION 2
+#define T2B200_ABI_VERSION 3
 
 #define T2_OK 0
 #define T2_ERR_INVALID_ARG (-1)
@@ -270,8 +270,9 @@ int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspace, const c
  * Every layer then adds b_gin + W_gin^T gc_embedding[id_b] to item b's gate pre-activations. An id outside [0, n_speakers) reads
  * nothing: it makes that item's gate biases, and so its gate activations, NaN. */
 int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* d_speaker_ids, void* stream);
-/* One launch of a conditioning-upsampler kernel of the WaveNet engine on caller buffers (t2_dbg_kernel_t above), with the product's grid,
- * block and shared memory. Every argument is checked before any driver call. Layouts: in fp32 [B][C][W], layer output fp32 [B][C][W*s];
+/* One launch of a conditioning-upsampler kernel or of a small kernel of the WaveNet engine on caller buffers (t2_dbg_kernel_t above), with
+ * the product's grid, block and shared memory. Every argument is checked before any driver call; no temporaries are allocated. Upsampler
+ * layouts: in fp32 [B][C][W], layer output fp32 [B][C][W*s];
  * K / bias as the layer's parameters (upsample_type 0: [3][3][1][s] / [s]; 1: [3][s][1][1] / [1]; 2: [1][s][C][C] / [C]). Common i:
  * B, C (1..128), W, s, type (0 SubPixel, 1 2D, 2 1D), act (0 ReLU, 1 LeakyReLU, 2 none); f[0]: LeakyReLU alpha in [0, 1].
  * UP_FWD        p: in, K, bias, out fp32 [B][C][W*s] (post-activation), c_up bf16 (nullable: channels-last [B][W*s][C], or the split
@@ -283,6 +284,45 @@ int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, const int* 
 #define T2_DBG_WN_UP_FWD 1
 #define T2_DBG_WN_UP_BWD_PARAM 2
 #define T2_DBG_WN_UP_BWD_INPUT 3
+/* The small kernels of the WaveNet engine, one launch each with the engine's launcher (tests/test_wavenet_kernels_gpu.py); their ids
+ * start at 10, ids 4 to 9 are not assigned. p / i / f:
+ * FIRST_CONV      first_conv_kernel. p: xin (int32 [npos] one-hot indices in [0, Q): not checked, or fp32 [npos] samples), W fp32 ([Q][R],
+ *                 or [1][R] for scalar input), bias fp32 [R], x bf16 [npos][R] (out; split: [npos][2R] = hi | lo), xd bf16 [npos][R]
+ *                 (nullable: the dropout copy, kept with probability 1 - f[0], hash seed = seed + *step). i: npos, R (multiple of 8, <= 1024),
+ *                 scalar_in, split (no xd). f[0]: dropout p in [0, 1).
+ * FIRST_CONV_BWD  first_conv_bwd_kernel + the gradient finalisation. p: xin (as FIRST_CONV), dx0 bf16 [npos][R], acc int64 [Q][R] (scratch:
+ *                 cleared, then the fixed-point totals), dW fp32 [Q][R] (in/out: each non-zero total is added). i: npos, R (<= 1024),
+ *                 scalar_in, Q (1 for scalar input).
+ * COLSUM          colsum_kernel + the gradient finalisation. p: ws (base of the src_off byte offsets), acc int64 [n_acc] (scratch, as above),
+ *                 grads fp32 [n_acc] (in/out, as above), scalars fp32 [n_scalars] (nullable when n_scalars = 0), table (device scratch,
+ *                 64 bytes per job), jobs HOST int64 [njobs][7] {src_off (bytes, bf16 [rows][ld] source), rows, C, ld (both even),
+ *                 dst_off, dst2_off (-1: none), div_scalar (-1: none)}, scales HOST fp32 [njobs]. i: njobs, n_acc, ws bytes, n_scalars.
+ *                 Column c of a job adds scale / max(scalars[div_scalar], 1e-20) * sum_r src[r][c] to acc[dst_off + c] (and dst2_off + c).
+ * DERIVED_BIAS    derived_bias_kernel. p: params, bias_g fp32 [L][G] (out), bias_skip fp32 [S] (out), offs int64 [3L] device (per layer the
+ *                 offsets of b_dil, b_cin (-1: none), b_skip), scales fp32 [L] device. i: L, G, S.
+ * SKIP_BIAS       skip_bias_kernel. p: skipsum int64 [S] (fixed-point), grads fp32 (out: scales[l] * skipsum at offs[3l + 2]), offs, scales.
+ *                 i: L, S.
+ * FX_FINALIZE     fx_finalize_kernel. p: acc int64 [n], grads fp32 [n] (in/out: + the value of every non-zero total). i: n.
+ * CL_TO_CHW       cl_to_chw_kernel. p: in fp32 [B][T][C], out fp32 [B][C][T]. i: B, T, C.
+ * GIN_BIAS        gin_bias_kernel. p: params, bias fp32 (layer l at + l bias_ld), on int32 (nullable = on), ids int32 [B] (nullable = no
+ *                 speaker term), out fp32 (out: [l][b][g] at + l out_l + b out_b + g). i: L, B, G, Gi, NS, bias_ld, out_l, out_b, p_k, p_b,
+ *                 p_stride, p_emb (W_gin / b_gin of layer l at params + p_k / p_b + l p_stride, the embedding [NS][Gi] at p_emb).
+ * SET_SPEAKERS    set_speakers_kernel. p: spk int32 [1 + B] (out: on flag, then the ids), ids int32 [B] (nullable). i: B.
+ * GIN_WGRAD       gin_wgrad_kernel. p: params, spk int32 [1 + B], S int64 [L][B][G] (fixed-point per-item sums), gfx int64 (out: the
+ *                 integer totals at offs[3l], offs[3l + 1] and, with spk[0], p_b + l p_stride), grads fp32 (out with spk[0]: dW_gin), offs
+ *                 int64 [3L]. i: L, B, G, Gi, NS, p_k, p_b, p_stride, p_emb.
+ * GIN_DEMB        gin_demb_kernel. p, i: as GIN_WGRAD; writes the embedding gradient rows of the speakers some item uses (with spk[0]). */
+#define T2_DBG_WN_FIRST_CONV 10
+#define T2_DBG_WN_FIRST_CONV_BWD 11
+#define T2_DBG_WN_COLSUM 12
+#define T2_DBG_WN_DERIVED_BIAS 13
+#define T2_DBG_WN_SKIP_BIAS 14
+#define T2_DBG_WN_FX_FINALIZE 15
+#define T2_DBG_WN_CL_TO_CHW 16
+#define T2_DBG_WN_GIN_BIAS 17
+#define T2_DBG_WN_SET_SPEAKERS 18
+#define T2_DBG_WN_GIN_WGRAD 19
+#define T2_DBG_WN_GIN_DEMB 20
 int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream);
 
 
@@ -455,7 +495,13 @@ int t2_cbhg_workspace_tensor(const t2_cbhg_config_t* cfg, void* d_workspace, con
  * d_offsets: int64 [n_tensors + 1] element offsets of the tensors inside the flat buffers.
  * grad_scale multiplies every gradient first (1/world_size after an NCCL sum all-reduce).
  * max_norm <= 0 disables per-tensor norm clipping; max_value <= 0 disables value clipping;
- * global_norm_clip > 0 applies tf.clip_by_global_norm instead. d_ema may be NULL. d_scratch: fp32 [n_tensors+1]. */
+ * global_norm_clip > 0 applies tf.clip_by_global_norm instead. d_ema may be NULL.
+ * d_scratch: fp32 [2 n_tensors + ceil(n_total / 4096)]: the norms are summed in a fixed order without float
+ * atomics, so the same call on the same state gives bit-identical results (data-parallel replicas stay identical).
+ * Non-finite gradients: the clips propagate NaN, as tf.clip_by_norm / clip_by_global_norm / clip_by_value do. A NaN or Inf anywhere
+ * in a tensor (per-tensor clip) or in any tensor (global clip) makes the norm non-finite: NaN turns every clipped gradient of that
+ * tensor (of every tensor) into NaN, Inf scales every finite gradient to 0 and the Inf ones to NaN. Without a norm clip only the
+ * non-finite elements themselves go non-finite; the value clip keeps NaN as NaN and clamps +-Inf to +-max_value. */
 int t2_adam_step(float* d_params, const float* d_grads, float* d_m, float* d_v, float* d_ema,
                  const long long* d_offsets, int n_tensors, long long n_total, float lr, float beta1, float beta2,
                  float eps, int step, float grad_scale, float max_norm, float max_value, float global_norm_clip,

@@ -16,6 +16,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -490,7 +491,7 @@ __global__ void gin_wgrad_kernel(GinGradArgs a) {
   }
 }
 // d gc_embedding[s][k] = sum over items b with id_b == s (in the order of b) of sum_{l,g} W_gin[l][k][g] * S[l][b][g]; one block
-// per (speaker, k), a fixed-shape tree per item: no float atomics. Rows no item uses stay exactly 0 (the gradient buffer is cleared).
+// per (speaker, k), a fixed-shape tree per item: no float atomics. Rows no item uses get exactly 0.
 constexpr int kGinThreads = 256;
 __global__ void __launch_bounds__(kGinThreads) gin_demb_kernel(GinGradArgs a) {
   __shared__ float red[kGinThreads];
@@ -1329,6 +1330,39 @@ GinArgs gin_args(const Layout& lo, const float* params) {
   return a;
 }
 
+// Launches of the small kernels, shared by the engine and t2_dbg_wn_kernel (same grid and block). Each counts its launch.
+void launch_derived_bias(const DerivedArgs& a, cudaStream_t st) {
+  derived_bias_kernel<<<grid1d(std::max((long long)a.L * a.G, (long long)a.S)), 256, 0, st>>>(a); t2_count_launch();
+}
+void launch_gin_bias(const GinArgs& a, cudaStream_t st) {
+  gin_bias_kernel<<<grid1d((long long)a.L * a.B * a.G), 256, 0, st>>>(a); t2_count_launch();
+}
+void launch_set_speakers(int* spk, const int* ids, int B, cudaStream_t st) {
+  set_speakers_kernel<<<grid1d(B), 256, 0, st>>>(spk, ids, B); t2_count_launch();
+}
+void launch_gin_wgrad(const GinGradArgs& a, cudaStream_t st) {
+  gin_wgrad_kernel<<<grid1d((long long)a.L * a.G), 256, 0, st>>>(a); t2_count_launch();
+}
+void launch_gin_demb(const GinGradArgs& a, cudaStream_t st) {
+  gin_demb_kernel<<<dim3(a.NS, a.Gi), kGinThreads, 0, st>>>(a); t2_count_launch();
+}
+void launch_first_conv(const void* xin, int scalar_in, const float* W, const float* bias, bf16* x, bf16* xd, long long npos, int R,
+                       float p, unsigned long long seed, const unsigned long long* step, int split, cudaStream_t st) {
+  first_conv_kernel<<<grid1d(npos * (R / 8)), 256, 0, st>>>(xin, scalar_in, W, bias, x, xd, npos, R, p, seed, step, split); t2_count_launch();
+}
+void launch_first_conv_bwd(const void* xin, int scalar_in, const bf16* dx0, long long* dW, long long npos, int R, cudaStream_t st) {
+  first_conv_bwd_kernel<<<dim3((unsigned)((npos + 63) / 64)), R, 0, st>>>(xin, scalar_in, dx0, dW, npos, R); t2_count_launch();
+}
+void launch_colsum(const uint8_t* ws, long long* acc, const ColsumJob* jobs, int njobs, const float* scalars, cudaStream_t st) {
+  colsum_kernel<<<dim3(96, njobs), 256, 0, st>>>(ws, acc, jobs, scalars); t2_count_launch();
+}
+void launch_skip_bias(const long long* skipsum, float* grads, const long long* offs, const float* scales, int L, int S, cudaStream_t st) {
+  skip_bias_kernel<<<grid1d((long long)L * S), 256, 0, st>>>(skipsum, grads, offs, scales, L, S); t2_count_launch();
+}
+void launch_cl_to_chw(const float* in, float* out, int B, int T, int C, cudaStream_t st) {
+  cl_to_chw_kernel<<<dim3((T + 31) / 32, (C + 31) / 32, B), dim3(32, 8), 0, st>>>(in, out, T, C); t2_count_launch();
+}
+
 }  // namespace
 
 int launch_fx_finalize(const long long* acc, float* out, long long n, cudaStream_t st) {
@@ -1409,7 +1443,7 @@ extern "C" int t2_wn_pack_weights(const t2_wn_config_t* cfg, const float* d_para
   DerivedArgs a;
   a.params = d_params; a.bias_g = reinterpret_cast<float*>(pk + lo.k_bias_g); a.bias_skip = reinterpret_cast<float*>(pk + lo.k_bias_skip);
   a.offs = d_offs; a.scales = d_scales; a.L = lo.L; a.G = lo.G; a.S = lo.S;
-  derived_bias_kernel<<<grid1d((long long)lo.L * lo.G), 256, 0, st>>>(a); t2_count_launch();
+  launch_derived_bias(a, st);
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
@@ -1437,7 +1471,7 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
     a.bias = reinterpret_cast<const float*>(pk + lo.k_bias_g); a.bias_ld = lo.G;
     a.on = spk; a.ids = spk + 1;
     a.out = reinterpret_cast<float*>(ws + lo.w_gbias); a.out_l = (long long)lo.B * lo.G; a.out_b = lo.G;
-    gin_bias_kernel<<<grid1d((long long)lo.L * lo.B * lo.G), 256, 0, st>>>(a); t2_count_launch();
+    launch_gin_bias(a, st);
     T2_CHECK_CUDA(cudaGetLastError());
   }
   // 1. conditioning -> c_up (bf16 channels-last)
@@ -1466,8 +1500,8 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   // 2. first conv
   bf16* x_all = reinterpret_cast<bf16*>(ws + lo.w_x);
   bf16* xd_all = reinterpret_cast<bf16*>(ws + lo.w_xd);
-  first_conv_kernel<<<grid1d(BT * (lo.R / 8)), 256, 0, st>>>(d_x, lo.scalar_in ? 1 : 0, d_params + lo.p_in_k, d_params + lo.p_in_b,
-                                                       x_all, p > 0.f ? xd_all : x_all, BT, lo.R, p, seed, d_step, lo.split ? 1 : 0); t2_count_launch();
+  launch_first_conv(d_x, lo.scalar_in ? 1 : 0, d_params + lo.p_in_k, d_params + lo.p_in_b, x_all, p > 0.f ? xd_all : x_all, BT, lo.R, p, seed,
+                    d_step, lo.split ? 1 : 0, st);
   T2_CHECK_CUDA(cudaGetLastError());
   // 3. residual stack
   bf16* z_all = reinterpret_cast<bf16*>(ws + lo.w_z);
@@ -1633,9 +1667,8 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     rc = launch_act_gemm(EPI_SCALE_RELUMASK, lo.S, g, st);
     if (rc) return rc;
   }
-  skip_bias_kernel<<<grid1d((long long)lo.L * lo.S), 256, 0, st>>>(reinterpret_cast<const long long*>(ws + lo.w_skipsum), d_grads,
-      reinterpret_cast<const long long*>(ws + lo.w_tables), reinterpret_cast<const float*>(ws + lo.w_tables + 3 * lo.L * sizeof(long long)), lo.L, lo.S);
-  t2_count_launch();
+  launch_skip_bias(reinterpret_cast<const long long*>(ws + lo.w_skipsum), d_grads, reinterpret_cast<const long long*>(ws + lo.w_tables),
+                   reinterpret_cast<const float*>(ws + lo.w_tables + 3 * lo.L * sizeof(long long)), lo.L, lo.S, st);
   // The head's weight gradients (6 tiles with a 15360-long reduction: ~100 us on 6 SMs) and the bias column sums of dlog
   // depend only on the head backward above: they run on the side stream underneath the whole residual-stack chain below,
   // which leaves SMs idle (120 M tiles).
@@ -1651,7 +1684,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
                      make_act(dlog, lo.ldo, lo.T, lo.B)};
     rc = launch_wgrad(hmaps, 4, reinterpret_cast<const WgradTile*>(ws + lo.w_tiles_head), lo.n_tiles_head, d_grads, lo.T, lo.B, sb);
     if (rc) return rc;
-    colsum_kernel<<<dim3(96, lo.n_colsum), 256, 0, sb>>>(ws, gfx, reinterpret_cast<const ColsumJob*>(ws + lo.w_colsum), scalars); t2_count_launch();
+    launch_colsum(ws, gfx, reinterpret_cast<const ColsumJob*>(ws + lo.w_colsum), lo.n_colsum, scalars, sb);
     T2_CHECK_CUDA(cudaGetLastError());
   }
   // residual stack, top down
@@ -1680,8 +1713,8 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     a.offs = reinterpret_cast<const long long*>(ws + lo.w_tables);
     a.p_k = lo.p_g_k[0]; a.p_b = lo.p_g_b[0]; a.p_stride = lo.layer_stride; a.p_emb = lo.p_emb;
     a.L = lo.L; a.B = lo.B; a.G = lo.G; a.Gi = lo.Gi; a.NS = lo.NS;
-    gin_wgrad_kernel<<<grid1d((long long)lo.L * lo.G), 256, 0, st>>>(a); t2_count_launch();
-    gin_demb_kernel<<<dim3(lo.NS, lo.Gi), kGinThreads, 0, st>>>(a); t2_count_launch();
+    launch_gin_wgrad(a, st);
+    launch_gin_demb(a, st);
     T2_CHECK_CUDA(cudaGetLastError());
   }
   // From here on two independent tails: (A) the batched weight-gradient GEMM of the stack (fills the machine), (B) the
@@ -1700,7 +1733,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     if (rc) return rc;
   }
   // first conv
-  first_conv_bwd_kernel<<<dim3((unsigned)((BT + 63) / 64)), lo.R, 0, sb>>>(d_x, lo.scalar_in ? 1 : 0, dxin, gfx + lo.p_in_k, BT, lo.R); t2_count_launch();
+  launch_first_conv_bwd(d_x, lo.scalar_in ? 1 : 0, dxin, gfx + lo.p_in_k, BT, lo.R, sb);
   T2_CHECK_CUDA(cudaGetLastError());
   // conditioning path
   if (lo.C > 0 && !cfg->c_pre_upsampled) {
@@ -1717,7 +1750,7 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
     if (rc) return rc;
     // dc_up arrives channels-last from the GEMM: transpose once into [B][C][T]
     float* dchw = reinterpret_cast<float*>(ws + lo.w_upgrad[1]);
-    cl_to_chw_kernel<<<dim3((lo.T + 31) / 32, (lo.C + 31) / 32, lo.B), dim3(32, 8), 0, sb>>>(dcup, dchw, lo.T, lo.C); t2_count_launch();
+    launch_cl_to_chw(dcup, dchw, lo.B, lo.T, lo.C, sb);
     const float* dout = dchw;
     int pp = 0;
     for (int i = int(lo.up_w.size()) - 1; i >= 0; --i) {
@@ -1780,8 +1813,7 @@ extern "C" int t2_wn_set_speakers(const t2_wn_config_t* cfg, void* d_workspace, 
   if (rc) return rc;
   T2_REQUIRE(lo.Gi > 0, T2_ERR_INVALID_ARG, "speaker ids need gin_channels > 0");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  set_speakers_kernel<<<grid1d(lo.B), 256, 0, st>>>(reinterpret_cast<int*>(static_cast<uint8_t*>(d_workspace) + lo.w_spk), d_speaker_ids, lo.B);
-  t2_count_launch();
+  launch_set_speakers(reinterpret_cast<int*>(static_cast<uint8_t*>(d_workspace) + lo.w_spk), d_speaker_ids, lo.B, st);
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
@@ -1810,10 +1842,9 @@ extern "C" int t2_wn_workspace_tensor(const t2_wn_config_t* cfg, void* d_workspa
   return t2_set_error(T2_ERR_INVALID_ARG, "unknown workspace tensor '%s'", name);
 }
 
-// test hook: one conditioning-upsampler launch on caller buffers (include/t2b200.h, T2_DBG_WN_*)
-extern "C" int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream) {
-  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_wn_kernel: null call");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+// test hook: one launch of a conditioning-upsampler kernel or of a small kernel on caller buffers (include/t2b200.h, T2_DBG_WN_*)
+namespace {
+int dbg_wn_upsample(const t2_dbg_kernel_t* call, cudaStream_t st) {
   void* const* p = call->p;
   const long long* i = call->i;
   const long long B = i[0], C = i[1], W = i[2], s = i[3], type = i[4], act = i[5];
@@ -1843,13 +1874,158 @@ extern "C" int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream) {
       rc = launch_fx_finalize(acc, dK, nK, st);
       return rc ? rc : launch_fx_finalize(acc + nK, db, nb, st);
     }
-    case T2_DBG_WN_UP_BWD_INPUT:
+    default:  // T2_DBG_WN_UP_BWD_INPUT
       T2_REQUIRE(p[0] && p[1] && p[2] && p[3], T2_ERR_INVALID_ARG, "dbg_wn_kernel UP_BWD_INPUT: null pointer argument");
       return launch_upsample_bwd_input(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
                                        static_cast<float*>(p[3]), b, c, w, sc, ty, ac, alpha, st);
+  }
+}
+
+bool in_range(long long v, long long lo, long long hi) { return v >= lo && v <= hi; }
+
+// the speaker kernels' integer arguments i[0..11]: L, B, G, Gi, NS, then (per id) offsets; shapes in [1, 2^20] with L*B*G < 2^31
+int dbg_gin_shape(const long long* i, const char* what) {
+  for (int k = 0; k < 5; ++k)
+    T2_REQUIRE(in_range(i[k], 1, 1 << 20), T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel %s: L, B, G, Gi, NS must be in [1, 2^20] (i[%d] = %lld)",
+               what, k, i[k]);
+  T2_REQUIRE(i[0] * i[1] * i[2] < (1LL << 31) && i[3] <= 65535, T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel %s: L*B*G >= 2^31 or Gi > 65535",
+             what);
+  return T2_OK;
+}
+}  // namespace
+
+extern "C" int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream) {
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_wn_kernel: null call");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  void* const* p = call->p;
+  const long long* i = call->i;
+  switch (call->kernel) {
+    case T2_DBG_WN_UP_FWD:
+    case T2_DBG_WN_UP_BWD_PARAM:
+    case T2_DBG_WN_UP_BWD_INPUT:
+      return dbg_wn_upsample(call, st);
+    case T2_DBG_WN_FIRST_CONV: {
+      const long long npos = i[0], R = i[1];
+      const float pd = call->f[0];
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3], T2_ERR_INVALID_ARG, "dbg_wn_kernel FIRST_CONV: null pointer argument");
+      T2_REQUIRE(in_range(npos, 1, 1LL << 28) && in_range(R, 8, 1024) && R % 8 == 0, T2_ERR_UNSUPPORTED_SHAPE,
+                 "dbg_wn_kernel FIRST_CONV: npos must be in [1, 2^28], R a multiple of 8 in [8, 1024]");
+      T2_REQUIRE(in_range(i[2], 0, 1) && in_range(i[3], 0, 1) && (i[3] == 0 || p[4] == nullptr) && pd >= 0.f && pd < 1.f, T2_ERR_INVALID_ARG,
+                 "dbg_wn_kernel FIRST_CONV: scalar_in and split are 0 / 1, split has no dropout copy, dropout p in [0, 1)");
+      launch_first_conv(p[0], int(i[2]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]), static_cast<bf16*>(p[3]),
+                        static_cast<bf16*>(p[4]), npos, int(R), pd, call->seed, call->step, int(i[3]), st);
+      break;
+    }
+    case T2_DBG_WN_FIRST_CONV_BWD: {
+      const long long npos = i[0], R = i[1], Q = i[3];
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3], T2_ERR_INVALID_ARG, "dbg_wn_kernel FIRST_CONV_BWD: null pointer argument");
+      T2_REQUIRE(in_range(npos, 1, 1LL << 28) && in_range(R, 1, 1024) && in_range(i[2], 0, 1) && in_range(Q, 1, 1 << 20) &&
+                     (i[2] == 0 || Q == 1),
+                 T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel FIRST_CONV_BWD: npos in [1, 2^28], R in [1, 1024], scalar_in 0 / 1, Q in [1, 2^20] (1 for scalar input)");
+      long long* acc = static_cast<long long*>(p[2]);
+      T2_CHECK_CUDA(cudaMemsetAsync(acc, 0, size_t(Q * R) * sizeof(long long), st));
+      launch_first_conv_bwd(p[0], int(i[2]), static_cast<const bf16*>(p[1]), acc, npos, int(R), st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return launch_fx_finalize(acc, static_cast<float*>(p[3]), Q * R, st);
+    }
+    case T2_DBG_WN_COLSUM: {
+      const long long njobs = i[0], n_acc = i[1], ws_bytes = i[2], n_scalars = i[3];
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[4] && p[5] && p[6], T2_ERR_INVALID_ARG, "dbg_wn_kernel COLSUM: null pointer argument");
+      T2_REQUIRE(in_range(njobs, 1, 65535) && in_range(n_acc, 1, 1LL << 40) && ws_bytes >= 0 && in_range(n_scalars, 0, 1 << 20) &&
+                     (n_scalars == 0 || p[3]),
+                 T2_ERR_INVALID_ARG, "dbg_wn_kernel COLSUM: bad job count, accumulator count, workspace size or scalars");
+      static_assert(sizeof(ColsumJob) <= 64, "T2_DBG_WN_COLSUM documents 64 bytes of table per job");
+      const long long* ji = static_cast<const long long*>(p[5]);
+      const float* jf = static_cast<const float*>(p[6]);
+      std::vector<ColsumJob> jobs(static_cast<size_t>(njobs));
+      for (long long k = 0; k < njobs; ++k) {
+        const long long* r = ji + 7 * k;
+        ColsumJob& j = jobs[size_t(k)];
+        T2_REQUIRE(in_range(r[1], 1, 1LL << 31) && in_range(r[2], 2, 1 << 20) && r[2] % 2 == 0 && in_range(r[3], r[2], 1 << 20) && r[3] % 2 == 0,
+                   T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel COLSUM job %lld: rows in [1, 2^31], C and ld even with 2 <= C <= ld <= 2^20", k);
+        T2_REQUIRE(r[0] >= 0 && r[0] % 4 == 0 && r[0] + r[1] * r[3] * 2 <= ws_bytes && in_range(r[4], 0, n_acc - r[2]) &&
+                       (r[5] == -1 || in_range(r[5], 0, n_acc - r[2])) && in_range(r[6], -1, n_scalars - 1) && std::isfinite(jf[k]),
+                   T2_ERR_INVALID_ARG, "dbg_wn_kernel COLSUM job %lld: source outside the workspace, destination outside the accumulators, "
+                   "bad scalar index or non-finite scale", k);
+        j.src_off = r[0]; j.rows = r[1]; j.C = int(r[2]); j.ld = int(r[3]); j.dst_off = r[4]; j.dst2_off = r[5]; j.scale = jf[k];
+        j.div_scalar = int(r[6]);
+      }
+      long long* acc = static_cast<long long*>(p[1]);
+      ColsumJob* table = static_cast<ColsumJob*>(p[4]);
+      T2_CHECK_CUDA(cudaMemsetAsync(acc, 0, size_t(n_acc) * sizeof(long long), st));
+      // from pageable memory: returns once the table is staged, so it may go out of scope
+      T2_CHECK_CUDA(cudaMemcpyAsync(table, jobs.data(), jobs.size() * sizeof(ColsumJob), cudaMemcpyHostToDevice, st));
+      launch_colsum(static_cast<const uint8_t*>(p[0]), acc, table, int(njobs), static_cast<const float*>(p[3]), st);
+      T2_CHECK_CUDA(cudaGetLastError());
+      return launch_fx_finalize(acc, static_cast<float*>(p[2]), n_acc, st);
+    }
+    case T2_DBG_WN_DERIVED_BIAS: {
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4], T2_ERR_INVALID_ARG, "dbg_wn_kernel DERIVED_BIAS: null pointer argument");
+      T2_REQUIRE(in_range(i[0], 1, 1 << 20) && in_range(i[1], 1, 1 << 20) && in_range(i[2], 1, 1 << 20) && i[0] * i[1] < (1LL << 31),
+                 T2_ERR_UNSUPPORTED_SHAPE, "dbg_wn_kernel DERIVED_BIAS: L, G, S in [1, 2^20] with L*G < 2^31");
+      DerivedArgs a;
+      a.params = static_cast<const float*>(p[0]); a.bias_g = static_cast<float*>(p[1]); a.bias_skip = static_cast<float*>(p[2]);
+      a.offs = static_cast<const long long*>(p[3]); a.scales = static_cast<const float*>(p[4]);
+      a.L = int(i[0]); a.G = int(i[1]); a.S = int(i[2]);
+      launch_derived_bias(a, st);
+      break;
+    }
+    case T2_DBG_WN_SKIP_BIAS:
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3], T2_ERR_INVALID_ARG, "dbg_wn_kernel SKIP_BIAS: null pointer argument");
+      T2_REQUIRE(in_range(i[0], 1, 1 << 20) && in_range(i[1], 1, 1 << 20) && i[0] * i[1] < (1LL << 31), T2_ERR_UNSUPPORTED_SHAPE,
+                 "dbg_wn_kernel SKIP_BIAS: L, S in [1, 2^20] with L*S < 2^31");
+      launch_skip_bias(static_cast<const long long*>(p[0]), static_cast<float*>(p[1]), static_cast<const long long*>(p[2]),
+                       static_cast<const float*>(p[3]), int(i[0]), int(i[1]), st);
+      break;
+    case T2_DBG_WN_FX_FINALIZE:
+      T2_REQUIRE(p[0] && p[1] && in_range(i[0], 1, 1LL << 40), T2_ERR_INVALID_ARG, "dbg_wn_kernel FX_FINALIZE: null pointer or n outside [1, 2^40]");
+      return launch_fx_finalize(static_cast<const long long*>(p[0]), static_cast<float*>(p[1]), i[0], st);
+    case T2_DBG_WN_CL_TO_CHW:
+      T2_REQUIRE(p[0] && p[1], T2_ERR_INVALID_ARG, "dbg_wn_kernel CL_TO_CHW: null pointer argument");
+      T2_REQUIRE(in_range(i[0], 1, 65535) && in_range(i[1], 1, 1 << 26) && in_range(i[2], 1, 1 << 20), T2_ERR_UNSUPPORTED_SHAPE,
+                 "dbg_wn_kernel CL_TO_CHW: B in [1, 65535], T in [1, 2^26], C in [1, 2^20]");
+      launch_cl_to_chw(static_cast<const float*>(p[0]), static_cast<float*>(p[1]), int(i[0]), int(i[1]), int(i[2]), st);
+      break;
+    case T2_DBG_WN_GIN_BIAS: {
+      T2_REQUIRE(p[0] && p[1] && p[4], T2_ERR_INVALID_ARG, "dbg_wn_kernel GIN_BIAS: null pointer argument");
+      int rc = dbg_gin_shape(i, "GIN_BIAS");
+      if (rc) return rc;
+      for (int k = 5; k < 12; ++k)
+        T2_REQUIRE(in_range(i[k], 0, 1LL << 40), T2_ERR_INVALID_ARG, "dbg_wn_kernel GIN_BIAS: strides / offsets must be in [0, 2^40] (i[%d])", k);
+      GinArgs a;
+      a.params = static_cast<const float*>(p[0]); a.bias = static_cast<const float*>(p[1]); a.on = static_cast<const int*>(p[2]);
+      a.ids = static_cast<const int*>(p[3]); a.out = static_cast<float*>(p[4]);
+      a.L = int(i[0]); a.B = int(i[1]); a.G = int(i[2]); a.Gi = int(i[3]); a.NS = int(i[4]);
+      a.bias_ld = i[5]; a.out_l = i[6]; a.out_b = i[7]; a.p_k = i[8]; a.p_b = i[9]; a.p_stride = i[10]; a.p_emb = i[11];
+      launch_gin_bias(a, st);
+      break;
+    }
+    case T2_DBG_WN_SET_SPEAKERS:
+      T2_REQUIRE(p[0] && in_range(i[0], 1, 1 << 20), T2_ERR_INVALID_ARG, "dbg_wn_kernel SET_SPEAKERS: null spk or B outside [1, 2^20]");
+      launch_set_speakers(static_cast<int*>(p[0]), static_cast<const int*>(p[1]), int(i[0]), st);
+      break;
+    case T2_DBG_WN_GIN_WGRAD:
+    case T2_DBG_WN_GIN_DEMB: {
+      const char* what = call->kernel == T2_DBG_WN_GIN_WGRAD ? "GIN_WGRAD" : "GIN_DEMB";
+      T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[5], T2_ERR_INVALID_ARG, "dbg_wn_kernel %s: null pointer argument", what);
+      int rc = dbg_gin_shape(i, what);
+      if (rc) return rc;
+      for (int k = 5; k < 9; ++k)
+        T2_REQUIRE(in_range(i[k], 0, 1LL << 40), T2_ERR_INVALID_ARG, "dbg_wn_kernel %s: offsets must be in [0, 2^40] (i[%d])", what, k);
+      GinGradArgs a;
+      a.params = static_cast<const float*>(p[0]); a.spk = static_cast<const int*>(p[1]); a.S = static_cast<const long long*>(p[2]);
+      a.gfx = static_cast<long long*>(p[3]); a.grads = static_cast<float*>(p[4]); a.offs = static_cast<const long long*>(p[5]);
+      a.L = int(i[0]); a.B = int(i[1]); a.G = int(i[2]); a.Gi = int(i[3]); a.NS = int(i[4]);
+      a.p_k = i[5]; a.p_b = i[6]; a.p_stride = i[7]; a.p_emb = i[8];
+      if (call->kernel == T2_DBG_WN_GIN_WGRAD) launch_gin_wgrad(a, st);
+      else launch_gin_demb(a, st);
+      break;
+    }
     default:
       return t2_set_error(T2_ERR_INVALID_ARG, "dbg_wn_kernel: unknown kernel id %d", call->kernel);
   }
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
 }
 
 // Times `reps` back-to-back launches of one per-layer GEMM of the residual stack with CUDA events on the launching
@@ -2482,7 +2658,7 @@ extern "C" int t2_wn_ar_set_speakers(const t2_wn_config_t* cfg, int cluster_size
   a.bias = reinterpret_cast<const float*>(static_cast<const uint8_t*>(d_packed_ar) + al.o_bias); a.bias_ld = lo.G + lo.R;
   a.on = nullptr; a.ids = d_speaker_ids;
   a.out = reinterpret_cast<float*>(static_cast<uint8_t*>(d_workspace) + al.w_gbias); a.out_l = lo.G; a.out_b = (long long)lo.L * lo.G;
-  gin_bias_kernel<<<grid1d((long long)lo.L * lo.B * lo.G), 256, 0, st>>>(a); t2_count_launch();
+  launch_gin_bias(a, st);
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }

@@ -54,6 +54,12 @@ def param_table(info, cfg, n_tensors, trainable=True, base=0):
     return out
 
 
+def adam_scratch_floats(n_tensors, n_total):
+    """fp32 elements of t2_adam_step's d_scratch: per-tensor norms, the global norm and one partial per tensor segment of a 4096-element
+    chunk (include/t2b200.h)"""
+    return 2 * n_tensors + (n_total + 4095) // 4096
+
+
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)

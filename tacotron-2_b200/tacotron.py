@@ -145,7 +145,7 @@ class Tacotron(object):
         self.loss_buf = torch.zeros(4, dtype=torch.float32, device=self.device)
         self.grads = self.m = self.v = None
         self.offsets = torch.tensor([t[1] for t in self.tensors] + [self.n_params], dtype=torch.int64, device=self.device)
-        self.opt_scratch = torch.zeros(len(self.tensors) + 2, dtype=torch.float32, device=self.device)
+        self.opt_scratch = torch.zeros(L.adam_scratch_floats(len(self.tensors), self.n_params), dtype=torch.float32, device=self.device)
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.global_step = 0
         self.seed = int(hparams.tacotron_random_seed)

@@ -190,7 +190,7 @@ class WaveNet(object):
         self.tensors = L.param_table(self.lib.t2_wn_param_info, self.cfg, sz.n_tensors, trainable=False)  # (name, offset, shape)
         offs = [t[1] for t in self.tensors] + [sz.n_params]
         self.offsets = torch.tensor(offs, dtype=torch.int64, device=self.device)
-        self.opt_scratch = torch.zeros(sz.n_tensors + 2, dtype=torch.float32, device=self.device)
+        self.opt_scratch = torch.zeros(L.adam_scratch_floats(sz.n_tensors, sz.n_params), dtype=torch.float32, device=self.device)
         self.global_step = 0
         self.seed = int(hparams.wavenet_random_seed)
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=self.device)  # added to the dropout seed on device

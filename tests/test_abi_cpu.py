@@ -22,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert len(names) >= 30
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, missing
-    assert lib.t2_abi_version() == 2
+    assert lib.t2_abi_version() == 3
 
 
 def test_errors_are_return_codes_with_messages():
