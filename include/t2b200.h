@@ -364,9 +364,11 @@ typedef struct {
   float zoneout_rate;        /* tacotron_zoneout_rate */
   float reg_weight;          /* tacotron_reg_weight */
   float max_abs_value, lower_bound_decay;
-  int split_bf16;            /* 1 = "fp32-class" convolution stacks: the embedding, the encoder conv blocks + the BiLSTM input projection and
-                              * the postnet conv blocks + projection run on bf16 hi + lo operand pairs with fp32 pre-batch-norm activations
-                              * (forward / losses only). The recurrences (LSTMs, attention) keep bf16 operands / fp32 state. */
+  int split_bf16;            /* 1 = "fp32-class" forward: every contraction of the training / GTA forward and of free-running synthesis
+                              * (embedding, encoder conv blocks, encoder BiLSTM, memory layer, prenet, decoder LSTMs, attention query and
+                              * context, frame / stop projection, postnet) runs on bf16 hi + lo operand pairs (hi.hi + lo.hi + hi.lo, fp32
+                              * accumulate) and every stored activation / recurrent state is a hi + lo pair; pre-batch-norm activations and
+                              * cell states are fp32. Forward / losses / synthesis only (no backward); the LSTM sizes must be multiples of 64. */
   int mask_decoder;          /* 1 = masked losses (tacotron/models/modules.py:412-455): MSE terms over the frames t < targets_lengths[b]
                               * (sum / count_nonzero of the mask), stop-token loss = weighted sigmoid CE over the same frames divided by the
                               * number of NON-ZERO masked terms; the lengths come from t2_taco_set_target_lengths */
@@ -445,6 +447,9 @@ int t2_rng_uniform_f32(unsigned long long seed, unsigned int stream_id, long lon
                        void* stream);
 int t2_dbg_att_stamps(long long* d_buf);
 int t2_dbg_ar_stamps(long long* d_buf);    /* same for one layer pass of the AR synthesis kernel (16 int64) */
+/* debug / test access to workspace tensors by name. With split_bf16 = 1 the bf16 activation tensors double their rows: "memory"
+ * [B][T_in][hi(2H) | lo(2H)], "prenet" [T_out][B][hi(P2) | lo(P2)] and "proj_in" [T_out][B][hi(D + 2H) | lo(D + 2H)] (count is
+ * twice the bf16-mode count); the fp32 value of a channel is float(hi) + float(lo). "keys" stays fp32 [B][T_in][attention_dim]. */
 int t2_taco_workspace_tensor(const t2_taco_config_t* cfg, void* d_workspace, const char* name, void** ptr,
                              long long* count, int* elem_bytes);
 

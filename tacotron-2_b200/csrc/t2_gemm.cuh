@@ -438,7 +438,8 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
     const float keep_inv = 1.f / (1.f - pdrop);
     const unsigned long long seed = e.seed + (e.ptr[7] ? *static_cast<const unsigned long long*>(e.ptr[7]) : 0ull);
     const uint32_t hs = hash_seed(seed, uint32_t(e.i[3]));
-    if (e.i[11]) {   // split-bf16 mode: bf16 output rows are [hi(ldo) | lo(ldo)] (pitch 2 ldo); fp32 output unchanged; no dropout
+    if (e.i[11]) {   // split-bf16 mode: bf16 output rows are [hi(ldo) | lo(ldo)] (pitch 2 ldo); fp32 output unchanged; the dropout
+                     // mask is the bf16 path's draw (same element index), applied before the value is split
 #pragma unroll 1
       for (int gq = 0; gq < BN / 128; ++gq) {
         const int c0 = c.n_tile * BN + gq * 128 + c.cg * 32;
@@ -451,6 +452,7 @@ struct Epilogue<EPI_BIAS_ACT, BN> {
           if (bias && c0 + j < nvalid) v += __ldg(bias + c0 + j);
           if (act == 1) v = fmaxf(v, 0.f);
           else if (act == 2) v = tanhf_(v);
+          if (pdrop > 0.f) v = (hash_uniform32(hs, hrow + c0 + j) >= pdrop) ? v * keep_inv : 0.f;
           acc[j] = c0 + j < nvalid ? v : 0.f;
         }
         if (!c.valid) continue;
@@ -889,6 +891,9 @@ struct Epilogue<EPI_DX, BN> {
 //      8 tanh(c_new) stash bf16 [B][H] (nullable), 9 lengths int32 [B] (nullable), 10 device u64 seed offset
 // i0 = H, i1 = B, i3 = pre stride, i4/i5/i6 = row strides, i7 = time step, i8 = hash stream, i9 = training
 // f0 = zoneout rate
+// i11 != 0: split-bf16 mode, forward only (the stashes 7 / 8 are not written). h_prev / h_state rows are swapped-GEMM state operands
+// [hi | lo | hi]: lo at +i10, the second hi copy at +2 i10. h_out is written as hi at +0 and lo at +i2, plus a second hi copy at +2 i2
+// when i11 == 2 (h_out is the next GEMM's state operand) - with i11 == 1 it is a plain [hi | lo] activation row.
 template <>
 struct Epilogue<EPI_LSTM, 32> {
   static __device__ __forceinline__ void run(const EpiArgs& e, const EpiCtx& c) {
@@ -916,6 +921,7 @@ struct Epilogue<EPI_LSTM, 32> {
     const uint32_t hs_c = hash_seed(seed, uint32_t(e.i[8]) * 2u), hs_h = hash_seed(seed, uint32_t(e.i[8]) * 2u + 1u);
     const float z = e.f[0];
     const int t = e.i[7];
+    const int split = e.i[11];
     const int etid = (c.cg * 4 + q) * 32 + c.lane;
     const int u0 = c.m_tile * 32, b0 = c.n_tile * 32;
 #pragma unroll 1
@@ -932,7 +938,8 @@ struct Epilogue<EPI_LSTM, 32> {
       if (bias) { zi += bias[u]; zj += bias[H + u]; zf += bias[2 * H + u]; zo += bias[3 * H + u]; }
       float gi = sigmoidf_(zi), gj = tanhf_(zj), gf = sigmoidf_(zf + 1.f), go = sigmoidf_(zo);
       const float cp = c_prev[size_t(b) * H + u];
-      const float hp = __bfloat162float(h_prev[size_t(b) * e.i[4] + u]);
+      const __nv_bfloat16* hpp = h_prev + size_t(b) * e.i[4] + u;
+      const float hp = split ? __bfloat162float(hpp[0]) + __bfloat162float(hpp[e.i[10]]) : __bfloat162float(hpp[0]);
       const float cn = gf * cp + gi * gj;
       const float tc = tanhf_(cn);
       const float hn = go * tc;
@@ -949,6 +956,15 @@ struct Epilogue<EPI_LSTM, 32> {
       float tcs = tc;
       if (!live) { cs = cp; hsv = hp; ho = 0.f; gi = gj = gf = go = 0.f; tcs = 0.f; }
       c_out[size_t(b) * H + u] = cs;
+      if (split) {
+        const __nv_bfloat16 sh = __float2bfloat16(hsv), oh = __float2bfloat16(ho);
+        __nv_bfloat16* hs = h_state + size_t(b) * e.i[5] + u;
+        hs[0] = sh; hs[e.i[10]] = __float2bfloat16(hsv - __bfloat162float(sh)); hs[2 * e.i[10]] = sh;
+        __nv_bfloat16* hq = h_out + size_t(b) * e.i[6] + u;
+        hq[0] = oh; hq[e.i[2]] = __float2bfloat16(ho - __bfloat162float(oh));
+        if (split == 2) hq[2 * e.i[2]] = oh;
+        continue;
+      }
       h_state[size_t(b) * e.i[5] + u] = __float2bfloat16(hsv);
       h_out[size_t(b) * e.i[6] + u] = __float2bfloat16(ho);
       if (gst) {

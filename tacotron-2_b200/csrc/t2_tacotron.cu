@@ -63,6 +63,8 @@ struct TL {  // layout
   long long w_dencpre[2], w_dx3, w_encdh[2], w_encdc[2], w_encdg, w_demb, w_tiles, w_packjobs, w_regtab;
   long long w_ddecf, w_encdgall[2], w_dkeysb, w_dz, w_attU;
   long long w_tfsel, w_dfb;   // teacher_forcing_ratio < 1: per-step choices int32 [To], d(fed-back frame) fp32 [B][M]
+  // row pitches (elements) of the decoder-side bf16 rows; split_bf16 widens them (see build)
+  int ld_decin, ld_pn1, ld_pn2, ld_S1, ld_S2, ld_PI, ld_mem;
   std::vector<int> tile_off, tile_cnt;  // per wgrad launch (fixed order, see build_tiles)
   long long workspace_bytes;
   int n_packjobs, n_reg;
@@ -89,6 +91,8 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
              cfg->unmasked_encoder);
   T2_REQUIRE(cfg->noncumulative_weights == 0 || cfg->noncumulative_weights == 1, T2_ERR_INVALID_ARG, "noncumulative_weights %d is not 0 or 1",
              cfg->noncumulative_weights);
+  T2_REQUIRE(!cfg->split_bf16 || (lo.H % 64 == 0 && lo.D % 64 == 0), T2_ERR_UNSUPPORTED_SHAPE,
+             "split_bf16: the LSTM sizes must be multiples of 64 (the hi / lo halves of a state row are whole 64-wide K blocks)");
   // ---- parameters (order == oracle/tacotron.py:param_shapes) ----
   lo.n_params = 0; lo.params.clear(); lo.enc.clear(); lo.post.clear();
   lo.p_emb = add_param(lo.params, lo.n_params, "inputs_embedding", {lo.NS, lo.E});
@@ -147,30 +151,48 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
     lo.k_encWx[d] = pk.take(2LL * 4 * lo.H * lo.C * (split ? 3 : 1));            // [4H][C]  input projection (natural gate order)
     if (split) add_pack_split(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], 3 * lo.C, 0, 2 * lo.C, lo.C);
     else add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], lo.C, 1, 0);
-    lo.k_encWr[d] = pk.take(2LL * 4 * lo.H * lo.H);            // [4H perm][H] recurrent, rows permuted for EPI_LSTM
-    add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 1, 0, 1.f, lo.H);
+    lo.k_encWr[d] = pk.take(2LL * 4 * lo.H * lo.H * (split ? 3 : 1));   // [4H perm][H] recurrent, rows permuted for EPI_LSTM
+    if (split) add_pack_split(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], 3 * lo.H, 0, 2 * lo.H, lo.H, 1.f, lo.H);
+    else add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 1, 0, 1.f, lo.H);
     lo.k_encWrT[d] = pk.take(2LL * lo.H * 4 * lo.H);           // [H][4H] for the backward step
     add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWrT[d], 4 * lo.H, 0, 0);
   }
   lo.k_encWxT = pk.take(2LL * lo.C * 8 * lo.H);                // [C][fw 4H | bw 4H]
   for (int d = 0; d < 2; ++d) add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWxT, 8 * lo.H, 0, d * 4 * lo.H);
-  lo.k_mem = pk.take(2LL * lo.A * 2 * lo.H); add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 1, 0);
+  lo.k_mem = pk.take(2LL * lo.A * 2 * lo.H * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 6 * lo.H, 0, 4 * lo.H, 2 * lo.H);
+  else add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 1, 0);
   lo.k_memT = pk.take(2LL * 2 * lo.H * lo.A); add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_memT, lo.A, 0, 0);
   const int Mp = 128;  // mel channels padded for TMA boxes
-  lo.k_p1 = pk.take(2LL * lo.P1 * Mp); add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mp, 1, 0);
+  lo.k_p1 = pk.take(2LL * lo.P1 * Mp * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, 3 * Mp, 0, 2 * Mp, Mp);
+  else add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mp, 1, 0);
   lo.k_p1T = pk.take(2LL * lo.M * lo.P1); add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1T, lo.P1, 0, 0);
-  lo.k_p2 = pk.take(2LL * lo.P2 * lo.P1); add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 1, 0);
+  lo.k_p2 = pk.take(2LL * lo.P2 * lo.P1 * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, 3 * lo.P1, 0, 2 * lo.P1, lo.P1);
+  else add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 1, 0);
   lo.k_p2T = pk.take(2LL * lo.P1 * lo.P2); add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2T, lo.P2, 0, 0);
-  lo.k_l1x = pk.take(2LL * 4 * lo.D * lo.P2); add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 1, 0);
+  lo.k_l1x = pk.take(2LL * 4 * lo.D * lo.P2 * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, 3 * lo.P2, 0, 2 * lo.P2, lo.P2);
+  else add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 1, 0);
   lo.k_l1xT = pk.take(2LL * lo.P2 * 4 * lo.D); add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1xT, 4 * lo.D, 0, 0);
   const int K1r = 2 * lo.H + lo.D;
-  lo.k_l1r = pk.take(2LL * 4 * lo.D * K1r); add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 1, 0, 1.f, lo.D);
+  lo.k_l1r = pk.take(2LL * 4 * lo.D * K1r * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, 3 * K1r, 0, 2 * K1r, K1r, 1.f, lo.D);
+  else add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 1, 0, 1.f, lo.D);
   lo.k_l1rT = pk.take(2LL * K1r * 4 * lo.D); add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1rT, 4 * lo.D, 0, 0);
-  lo.k_l2 = pk.take(2LL * 4 * lo.D * K2); add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 1, 0, 1.f, lo.D);
+  lo.k_l2 = pk.take(2LL * 4 * lo.D * K2 * (split ? 3 : 1));
+  if (split) add_pack_split(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, 3 * K2, 0, 2 * K2, K2, 1.f, lo.D);
+  else add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 1, 0, 1.f, lo.D);
   lo.k_l2T = pk.take(2LL * K2 * 4 * lo.D); add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2T, 4 * lo.D, 0, 0);
-  lo.k_proj = pk.take(2LL * 128 * PIK);                         // rows 0..M-1 frame projection, row M stop projection
+  lo.k_proj = pk.take(2LL * 128 * PIK * (split ? 3 : 1));      // rows 0..M-1 frame projection, row M stop projection
+  if (split) {
+    add_pack_split(jobs, lo.p_fk, PIK, lo.M, lo.k_proj, 3 * PIK, 0, 2 * PIK, PIK);
+    add_pack_split(jobs, lo.p_sk, PIK, 1, lo.k_proj + 2LL * lo.M * 3 * PIK, 3 * PIK, 0, 2 * PIK, PIK);
+  } else {
   add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_proj, PIK, 1, 0);
   add_pack(jobs, lo.p_sk, PIK, 1, lo.k_proj + 2LL * lo.M * PIK, PIK, 1, 0);
+  }
   lo.k_projT = pk.take(2LL * PIK * 128);                        // [PIK][128]: cols 0..M-1 Wf, col M Ws
   add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_projT, 128, 0, 0);
   add_pack(jobs, lo.p_sk, PIK, 1, lo.k_projT, 128, 0, lo.M);
@@ -178,7 +200,9 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   if (split) add_pack_split(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, 3 * lo.PC, 0, 2 * lo.PC, lo.PC);
   else add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, lo.PC, 1, 0);
   lo.k_ppT = pk.take(2LL * lo.PC * 128); add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_ppT, 128, 0, 0);
-  lo.k_qT = pk.take(2LL * lo.A * lo.D); add_pack(jobs, lo.p_qry, lo.D, lo.A, lo.k_qT, lo.D, 1, 0);   // [A][D] for the attention kernel
+  lo.k_qT = pk.take(2LL * lo.A * lo.D * (split ? 2 : 1));     // [A][D] for the attention kernel; split: [A][hi(D) | lo(D)]
+  add_pack(jobs, lo.p_qry, lo.D, lo.A, lo.k_qT, split ? 2 * lo.D : lo.D, 1, 0);
+  if (split) { add_pack(jobs, lo.p_qry, lo.D, lo.A, lo.k_qT, 2 * lo.D, 1, lo.D); jobs.back().part = 2; }
   lo.packed_bytes = pk.used;
   lo.n_packjobs = int(jobs.size());
 
@@ -186,6 +210,9 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   Arena ws;
   const long long B = lo.B, Ti = lo.Ti, To = lo.To;
   const long long xm = split ? 2 : 1;       // split-bf16: stored conv-stack activations are [hi | lo]; pre-batch-norm activations fp32
+  const long long sm = split ? 3 : 1;       // split-bf16: recurrent state rows (the N operand of the swapped GEMMs) are [hi | lo | hi]
+  lo.ld_decin = split ? 2 * Mp : lo.M; lo.ld_pn1 = lo.P1 * int(xm); lo.ld_pn2 = lo.P2 * int(xm);
+  lo.ld_S1 = K1r * int(sm); lo.ld_S2 = K2 * int(sm); lo.ld_PI = PIK * int(xm); lo.ld_mem = 2 * lo.H * int(xm);
   lo.w_emb = ws.take(B * Ti * lo.E * 2 * xm);
   auto conv_ws = [&](ConvL& L, long long T) {
     L.w_y = ws.take(B * T * L.cout * (split ? 4 : 2)); L.w_x = ws.take(B * T * L.cout * 2 * xm); L.w_stats = ws.take(8LL * L.cout * 4);
@@ -193,21 +220,21 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   for (auto& L : lo.enc) conv_ws(L, Ti);
   for (int d = 0; d < 2; ++d) {
     lo.w_encpre[d] = ws.take(B * Ti * 4 * lo.H * 4);
-    lo.w_ench[d] = ws.take((Ti + 1) * B * lo.H * 2);      // h_state history, slot s = state after s processed steps
+    lo.w_ench[d] = ws.take((Ti + 1) * B * lo.H * 2 * sm);   // h_state history, slot s = state after s processed steps
     lo.w_encc[d] = ws.take((Ti + 1) * B * lo.H * 4);
     lo.w_encg[d] = ws.take(Ti * B * 4 * lo.H * 2);
     lo.w_enct[d] = ws.take(Ti * B * lo.H * 2);
   }
-  lo.w_memory = ws.take(B * Ti * 2 * lo.H * 2);
-  lo.w_values = ws.take(B * Ti * 2 * lo.H * 2);
+  lo.w_memory = ws.take(B * Ti * lo.ld_mem * 2);
+  lo.w_values = ws.take(B * Ti * lo.ld_mem * 2);
   lo.w_keys = ws.take(B * Ti * lo.A * 4);
-  lo.w_decin = ws.take(B * To * lo.M * 2);                  // time-major [To][B][M]
-  lo.w_pn1 = ws.take(To * B * lo.P1 * 2);
-  lo.w_pn2 = ws.take(To * B * lo.P2 * 2);
+  lo.w_decin = ws.take(B * To * lo.ld_decin * 2);           // time-major [To][B][M]; split: [hi(M) padded to 128 | lo(M) padded to 128]
+  lo.w_pn1 = ws.take(To * B * lo.ld_pn1 * 2);
+  lo.w_pn2 = ws.take(To * B * lo.ld_pn2 * 2);
   lo.w_pre1 = ws.take(To * B * 4 * lo.D * 4);
-  lo.w_S1 = ws.take((To + 1) * B * K1r * 2);
-  lo.w_S2 = ws.take((To + 1) * B * K2 * 2);
-  lo.w_PI = ws.take(To * B * PIK * 2);
+  lo.w_S1 = ws.take((To + 1) * B * lo.ld_S1 * 2);
+  lo.w_S2 = ws.take((To + 1) * B * lo.ld_S2 * 2);
+  lo.w_PI = ws.take(To * B * lo.ld_PI * 2);
   lo.w_c1 = ws.take((To + 1) * B * lo.D * 4); lo.w_c2 = ws.take((To + 1) * B * lo.D * 4);
   lo.w_g1 = ws.take(To * B * 4 * lo.D * 2); lo.w_g2 = ws.take(To * B * 4 * lo.D * 2);
   lo.w_t1 = ws.take(To * B * lo.D * 2); lo.w_t2 = ws.take(To * B * lo.D * 2);
@@ -288,11 +315,16 @@ __global__ void mask_values_kernel(const bf16* __restrict__ mem, const int* __re
   vals[e] = t < lens[b] ? mem[e] : __float2bfloat16(0.f);
 }
 // decoder inputs, time-major: dec_in[t][b][:] = t == 0 ? 0 : target[b][t-1][:]   (helpers.py:62-128, r = 1)
-__global__ void decin_kernel(const float* __restrict__ tgt, bf16* __restrict__ out, int B, int To, int M) {
+// split: rows [hi(M) | pad | lo(M) | pad] of pitch 256 (the padding stays zero from t2_taco_init)
+__global__ void decin_kernel(const float* __restrict__ tgt, bf16* __restrict__ out, int B, int To, int M, int split) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= (long long)To * B * M) return;
   const int m = int(e % M), b = int((e / M) % B), t = int(e / ((long long)M * B));
-  out[e] = __float2bfloat16(t == 0 ? 0.f : tgt[((long long)b * To + t - 1) * M + m]);
+  const float v = t == 0 ? 0.f : tgt[((long long)b * To + t - 1) * M + m];
+  if (!split) { out[e] = __float2bfloat16(v); return; }
+  const bf16 hi = __float2bfloat16(v);
+  bf16* row = out + (e / M) * 256 + m;
+  row[0] = hi; row[128] = __float2bfloat16(v - __bfloat162float(hi));
 }
 
 // ---- location-sensitive attention, one CTA per batch item per decoder step (attention.py:169-226) -------------
@@ -326,6 +358,10 @@ struct AttArgs {
   bf16* ctx_b; int ld_b;                    // context -> PI_all[t][b][D:]
   int B, Ti, D, A, KA, C2;
   int unmasked, noncumulative;              // t2_taco_config_t flags: pick the att_fwd_kernel instantiation (host side only)
+  // split (t2_taco_config_t.split_bf16): h2out / values / the context outputs are hi + lo pairs. The lo half of h2out sits at +lo_h2,
+  // of a values row at +C2 (row pitch 2 C2), of ctx_b at +lo_b; ctx_a is a swapped-GEMM state row: lo at +lo_a, hi again at +2 lo_a.
+  // WqT rows are [hi(D) | lo(D)].
+  int split = 0, lo_h2 = 0, lo_a = 0, lo_b = 0;
 };
 // q[a] = sum_k h[k] WqT[a][k]: one warp per output row (two rows in flight), lanes stride the row in 16-byte pieces so
 // that every load instruction reads 512 contiguous bytes (the 4-threads-per-output form touched 32 sectors per load)
@@ -340,19 +376,27 @@ __device__ __forceinline__ float dot8s(const uint4 u, const float* __restrict__ 
 }
 // q[a] = sum_k h[k] WqT[a][k]: one warp per output row (two rows in flight), lanes stride the row in 16-byte pieces so
 // that every load instruction reads 512 contiguous bytes; hs is in the split layout above
+// kSplit: WqT rows are [hi(D) | lo(D)] and q = sum_k h[k] (hi + lo)[a][k]
+template <bool kSplit>
 __device__ __forceinline__ void att_query(const bf16* __restrict__ WqT, const float* __restrict__ hs, float* __restrict__ q, int A, int D) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, NW = kAttThreads / 32;
   const int n16 = D >> 3;   // 16-byte pieces per row
+  const long long ldw = kSplit ? 2LL * D : D;
   for (int o = warp; o < A; o += 2 * NW) {
     const int o2 = o + NW;
-    const uint4* w0 = reinterpret_cast<const uint4*>(WqT + (long long)o * D);
-    const uint4* w1 = reinterpret_cast<const uint4*>(WqT + (long long)(o2 < A ? o2 : o) * D);
+    const uint4* w0 = reinterpret_cast<const uint4*>(WqT + (long long)o * ldw);
+    const uint4* w1 = reinterpret_cast<const uint4*>(WqT + (long long)(o2 < A ? o2 : o) * ldw);
     float a0 = 0.f, a1 = 0.f;
 #pragma unroll 4
     for (int i = lane; i < n16; i += 32) {
       const uint4 u0 = __ldg(w0 + i), u1 = __ldg(w1 + i);
       a0 += dot8s(u0, hs, i, D);
       a1 += dot8s(u1, hs, i, D);
+      if (kSplit) {
+        const uint4 l0 = __ldg(w0 + n16 + i), l1 = __ldg(w1 + n16 + i);
+        a0 += dot8s(l0, hs, i, D);
+        a1 += dot8s(l1, hs, i, D);
+      }
     }
     a0 = warp_sum(a0); a1 = warp_sum(a1);
     if (lane == 0) { q[o] = a0; if (o2 < A) q[o2] = a1; }
@@ -411,8 +455,8 @@ inline size_t att_fwd_smem(int Ti, int KA, int A, int D, int C2) {
 }
 // kMasked: the scores of positions past lens[b] are -inf (mask_encoder); otherwise the energies and the softmax cover all T_in
 // positions. The context sum stays bounded by lens[b] either way: the values rows past it are zero. kCumulative: the state after
-// the step is cum + alpha (cumulative_weights); otherwise alpha itself.
-template <bool kMasked, bool kCumulative>
+// the step is cum + alpha (cumulative_weights); otherwise alpha itself. kSplit: the split_bf16 operands (see AttArgs).
+template <bool kMasked, bool kCumulative, bool kSplit>
 __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
   extern __shared__ __align__(16) float sm[];
   pdl_wait();
@@ -433,11 +477,14 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
     const int j = i - half;
     cum[i] = (j >= 0 && j < Ti) ? a.cum[(long long)b * Ti + j] : 0.f;
   }
-  for (int i = tid; i < a.D; i += kAttThreads) hs[split8(i, a.D)] = __bfloat162float(a.h2out[(long long)b * a.ld_h2 + i]);
+  for (int i = tid; i < a.D; i += kAttThreads) {
+    const bf16* hp = a.h2out + (long long)b * a.ld_h2 + i;
+    hs[split8(i, a.D)] = kSplit ? __bfloat162float(hp[0]) + __bfloat162float(hp[a.lo_h2]) : __bfloat162float(hp[0]);
+  }
   for (int i = tid; i < Tip; i += kAttThreads) e[i] = 0.f;
   __syncthreads();
   ATT_STAMP(1);
-  att_query(a.WqT, hs, q, A, a.D);
+  att_query<kSplit>(a.WqT, hs, q, A, a.D);
   __syncthreads();
   ATT_STAMP(2);
   const int len = a.lens[b];
@@ -508,13 +555,19 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
       float acc[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-      const uint4* vp = reinterpret_cast<const uint4*>(a.values + (long long)b * Ti * a.C2) + ch;
+      const int ldv = kSplit ? 2 * nch : nch;  // uint4 chunks per values row ([hi | lo] in split mode)
+      const uint4* vp = reinterpret_cast<const uint4*>(a.values + (long long)b * Ti * ldv * 8) + ch;
 #pragma unroll 4
       for (int j = rg; j < len; j += 8) {
-        const uint4 u = __ldg(vp + (long long)j * nch);
+        const uint4 u = __ldg(vp + (long long)j * ldv);
         const float al = e[j];
         acc[0] += al * bf16lo(u.x); acc[1] += al * bf16hi(u.x); acc[2] += al * bf16lo(u.y); acc[3] += al * bf16hi(u.y);
         acc[4] += al * bf16lo(u.z); acc[5] += al * bf16hi(u.z); acc[6] += al * bf16lo(u.w); acc[7] += al * bf16hi(u.w);
+        if (kSplit) {
+          const uint4 w = __ldg(vp + (long long)j * ldv + nch);
+          acc[0] += al * bf16lo(w.x); acc[1] += al * bf16hi(w.x); acc[2] += al * bf16lo(w.y); acc[3] += al * bf16hi(w.y);
+          acc[4] += al * bf16lo(w.z); acc[5] += al * bf16hi(w.z); acc[6] += al * bf16lo(w.w); acc[7] += al * bf16hi(w.w);
+        }
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) part[rg * a.C2 + ch * 8 + i] = acc[i];
@@ -527,6 +580,16 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
 #pragma unroll
     for (int r = 0; r < 8; ++r) acc += part[r * a.C2 + c];
     const bf16 r16 = __float2bfloat16(acc);
+    if (kSplit) {
+      const bf16 l16 = __float2bfloat16(acc - __bfloat162float(r16));
+      if (a.ctx_a) {
+        bf16* ca = a.ctx_a + (long long)b * a.ld_a + c;
+        ca[0] = r16; ca[a.lo_a] = l16; ca[2 * a.lo_a] = r16;
+      }
+      bf16* cb = a.ctx_b + (long long)b * a.ld_b + c;
+      cb[0] = r16; cb[a.lo_b] = l16;
+      continue;
+    }
     if (a.ctx_a) a.ctx_a[(long long)b * a.ld_a + c] = r16;
     a.ctx_b[(long long)b * a.ld_b + c] = r16;
   }
@@ -535,19 +598,23 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
 // once per forward: the merged location filter bank U (from the conv kernel K [KA][F], its bias bK, the dense Wl [F][A] and the
 // attention bias) and the kernel's shared-memory opt-in
 using AttFwdFn = void (*)(AttArgs);
-AttFwdFn att_fwd_fn(int unmasked, int noncumulative) {
-  return unmasked ? (noncumulative ? att_fwd_kernel<false, false> : att_fwd_kernel<false, true>)
-                  : (noncumulative ? att_fwd_kernel<true, false> : att_fwd_kernel<true, true>);
+template <bool kSplit>
+AttFwdFn att_fwd_fn_t(int unmasked, int noncumulative) {
+  return unmasked ? (noncumulative ? att_fwd_kernel<false, false, kSplit> : att_fwd_kernel<false, true, kSplit>)
+                  : (noncumulative ? att_fwd_kernel<true, false, kSplit> : att_fwd_kernel<true, true, kSplit>);
+}
+AttFwdFn att_fwd_fn(int unmasked, int noncumulative, int split) {
+  return split ? att_fwd_fn_t<true>(unmasked, noncumulative) : att_fwd_fn_t<false>(unmasked, noncumulative);
 }
 int att_fwd_setup(const float* K, const float* bK, const float* Wl, const float* ba, float* U, int KA, int F, int A, size_t smem, int unmasked,
-                  int noncumulative, cudaStream_t st) {
+                  int noncumulative, int split, cudaStream_t st) {
   att_prep_kernel<<<grid1d((KA + 1) * A), 256, 0, st>>>(K, bK, Wl, ba, U, KA, F, A); t2_count_launch();
-  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_fn(unmasked, noncumulative), cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  T2_CHECK_CUDA(cudaFuncSetAttribute(att_fwd_fn(unmasked, noncumulative, split), cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
 int launch_att_fwd(const AttArgs& a, size_t smem, cudaStream_t st) {
-  T2_CHECK_CUDA(launch_pdl(att_fwd_fn(a.unmasked, a.noncumulative), dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
+  T2_CHECK_CUDA(launch_pdl(att_fwd_fn(a.unmasked, a.noncumulative, a.split), dim3(a.B), dim3(kAttThreads), smem, st, a)); t2_count_launch();
   return T2_OK;
 }
 
@@ -619,9 +686,10 @@ constexpr uint32_t kTfStream = 40;   // hash stream of the per-step teacher-forc
 // projo[t] += bias; next decoder input = the raw (un-clipped) frame just predicted (helpers.py:56). With tgt (TacoTrainingHelper at a
 // teacher-forcing ratio < 1, helpers.py:115-128): ONE draw u_t for the whole batch (stream kTfStream, element t, under seed + *step);
 // u_t < ratio feeds the target frame tgt[b][t] instead, and choice[t] records which of the two step t + 1 consumed.
+// split: next_in rows are the split decoder-input rows [hi(M) | pad | lo(M) | pad] of pitch 256 (decin_kernel)
 __global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __restrict__ fb, const float* __restrict__ sb, bf16* __restrict__ next_in,
                                           int B, int M, const float* __restrict__ tgt, int To, int t, float ratio, unsigned long long seed,
-                                          const unsigned long long* __restrict__ step, int* __restrict__ choice) {
+                                          const unsigned long long* __restrict__ step, int* __restrict__ choice, int split) {
   pdl_wait();
   pdl_launch_dependents();
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -634,7 +702,12 @@ __global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __
   const int m = e % (M + 1), b = e / (M + 1);
   const float v = p[b * 128 + m] + (m < M ? fb[m] : sb[0]);
   p[b * 128 + m] = v;
-  if (m < M && next_in) next_in[b * M + m] = __float2bfloat16(forced ? tgt[((long long)b * To + t) * M + m] : v);
+  if (m < M && next_in) {
+    const float x = forced ? tgt[((long long)b * To + t) * M + m] : v;
+    if (!split) { next_in[b * M + m] = __float2bfloat16(x); return; }
+    const bf16 hi = __float2bfloat16(x);
+    next_in[b * 256 + m] = hi; next_in[b * 256 + 128 + m] = __float2bfloat16(x - __bfloat162float(hi));
+  }
 }
 // normalisers -> s[5] (mel terms), s[6] (stop term); out (nullable) = the four normalised loss terms
 __global__ void loss_norm_kernel(float* s, float* out, float n_mel, float n_stop, float regw, const int* tlen, int B, int To, int M) {
@@ -667,7 +740,7 @@ int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, i
       g.seg[g.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, 2 * nkb, 0, 1};
       g.seg[g.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};
     }
-    T2_REQUIRE(g.nseg <= kMaxSeg && pdrop == 0.f, T2_ERR_UNSUPPORTED_SHAPE, "split conv_gemm: too many taps / dropout in the epilogue");
+    T2_REQUIRE(g.nseg <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "split conv_gemm: too many taps");
     g.epi.i[11] = 1;
   } else {
   g.a[0] = make_act(a, C, int(T), Bn, 1, C); g.na = 1;
@@ -688,14 +761,26 @@ struct StepCtx {
 };
 
 // one LSTM step on the swapped GEMM: gates^T = Wrec[4H perm][K] x S[B][K]^T (+ pre / bias) -> cell + zoneout
+// split_bf16: Wrec rows are [W_hi | W_hi | W_lo] (pitch 3K) and the state rows S [hi | lo | hi] (pitch 3K): one segment contracts
+// W_hi against [hi | lo], the next W_lo against the second hi copy. h_prev / h_state are state rows of this layout (lo at +K), h_out
+// gets its lo half at +out_lo and, when out_state, the second hi copy at +2 out_lo (see EPI_LSTM); the backward stashes are skipped.
 int lstm_step(const StepCtx& s, const void* wrec, int H, int K, const void* state, int B, const float* pre, int pre_stride, const float* bias,
               const float* c_prev, float* c_out, const bf16* h_prev, int ld_hp, bf16* h_state, int ld_hs, bf16* h_out, int ld_ho,
-              bf16* gst, bf16* tst, const int* lens, int t, int stream_id, float zone) {
+              bf16* gst, bf16* tst, const int* lens, int t, int stream_id, float zone, int out_lo = 0, int out_state = 0) {
   ActGemmCall g;
   memset(&g, 0, sizeof(g));
+  const int split = s.lo->c.split_bf16;
+  if (split) {
+    g.a[0] = make_act(wrec, 3 * K, 4 * H, 1, 1, 3 * K); g.na = 1;
+    g.seg[0] = Seg{0, 0, 0, 2 * K / kBK, 0, 1}; g.seg[1] = Seg{0, 0, 2 * K, K / kBK, 0, 1}; g.nseg = 2;
+    g.w = state; g.wN = B; g.wK = 3 * K; g.wL = 1;
+    gst = nullptr; tst = nullptr;
+    g.epi.i[2] = out_lo; g.epi.i[10] = K; g.epi.i[11] = out_state ? 2 : 1;
+  } else {
   g.a[0] = make_act(wrec, K, 4 * H, 1, 1, K); g.na = 1;
   g.seg[0] = Seg{0, 0, 0, K / kBK, 0, 1}; g.nseg = 1;
   g.w = state; g.wN = B; g.wK = K; g.wL = 1;
+  }
   g.T = 4 * H; g.B = 1; g.n_tiles = (B + 31) / 32;
   g.epi.ptr[0] = const_cast<float*>(pre); g.epi.ptr[1] = const_cast<float*>(bias); g.epi.ptr[2] = const_cast<float*>(c_prev); g.epi.ptr[3] = c_out;
   g.epi.ptr[4] = const_cast<bf16*>(h_prev); g.epi.ptr[5] = h_state; g.epi.ptr[6] = h_out; g.epi.ptr[7] = gst; g.epi.ptr[8] = tst;
@@ -976,7 +1061,7 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
   for (int i = tid * 4; i < RE * AP; i += kAttThreads * 4) *reinterpret_cast<float4*>(dE + i) = make_float4(0.f, 0.f, 0.f, 0.f);
   __syncthreads();
   ATT_STAMP(17);
-  att_query(a.WqT, hs, q, A, a.D);
+  att_query<false>(a.WqT, hs, q, A, a.D);
   ATT_STAMP(18);
   // d alpha[j] = dctx . values[j] + dcum[j] : one warp per row, 8-wide bf16 loads, four rows in flight
   float part = 0.f;
@@ -1338,16 +1423,18 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
     if (rc) return rc;
     bf16* hh = reinterpret_cast<bf16*>(ws + lo.w_ench[d]);
     float* cc = reinterpret_cast<float*>(ws + lo.w_encc[d]);
-    T2_CHECK_CUDA(cudaMemsetAsync(hh, 0, (size_t)B * H * 2, sx));
+    const int hw = lo.c.split_bf16 ? 3 * H : H;     // h history rows; split: state rows [hi | lo | hi]
+    T2_CHECK_CUDA(cudaMemsetAsync(hh, 0, (size_t)B * hw * 2, sx));
     T2_CHECK_CUDA(cudaMemsetAsync(cc, 0, (size_t)B * H * 4, sx));
     bf16* memory = reinterpret_cast<bf16*>(ws + lo.w_memory);
     for (int sidx = 0; sidx < Ti; ++sidx) {
       const int t = d == 0 ? sidx : Ti - 1 - sidx;
-      rc = lstm_step(sc, pk + lo.k_encWr[d], H, H, hh + (long long)sidx * B * H, B, pre + (long long)t * 4 * H, Ti * 4 * H, nullptr,
-                     cc + (long long)sidx * B * H, cc + (long long)(sidx + 1) * B * H, hh + (long long)sidx * B * H, H,
-                     hh + (long long)(sidx + 1) * B * H, H, memory + (long long)t * 2 * H + d * H, Ti * 2 * H,
+      rc = lstm_step(sc, pk + lo.k_encWr[d], H, H, hh + (long long)sidx * B * hw, B, pre + (long long)t * 4 * H, Ti * 4 * H, nullptr,
+                     cc + (long long)sidx * B * H, cc + (long long)(sidx + 1) * B * H, hh + (long long)sidx * B * hw, hw,
+                     hh + (long long)(sidx + 1) * B * hw, hw, memory + (long long)t * lo.ld_mem + d * H, Ti * lo.ld_mem,
                      reinterpret_cast<bf16*>(ws + lo.w_encg[d]) + (long long)sidx * B * 4 * H,
-                     reinterpret_cast<bf16*>(ws + lo.w_enct[d]) + (long long)sidx * B * H, d_input_lengths, t, 52 + d, lo.c.zoneout_rate);
+                     reinterpret_cast<bf16*>(ws + lo.w_enct[d]) + (long long)sidx * B * H, d_input_lengths, t, 52 + d, lo.c.zoneout_rate,
+                     2 * H, 0);
       if (rc) return rc;
     }
   }
@@ -1356,62 +1443,70 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
     T2_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
   }
   bf16* values = reinterpret_cast<bf16*>(ws + lo.w_values);
-  mask_values_kernel<<<grid1d((long long)B * Ti * 2 * H), 256, 0, st>>>(reinterpret_cast<bf16*>(ws + lo.w_memory), d_input_lengths, values, B, Ti, 2 * H);
+  mask_values_kernel<<<grid1d((long long)B * Ti * lo.ld_mem), 256, 0, st>>>(reinterpret_cast<bf16*>(ws + lo.w_memory), d_input_lengths, values, B, Ti,
+                                                                        lo.ld_mem);
   t2_count_launch();
   float* keys = reinterpret_cast<float*>(ws + lo.w_keys);
-  return conv_gemm(values, 2 * H, Ti, B, pk + lo.k_mem, lo.A, 2 * H, 1, nullptr, 128, nullptr, 0, nullptr, keys, lo.A, lo.A, 0.f, 0, 0, nullptr, st);
+  return conv_gemm(values, 2 * H, Ti, B, pk + lo.k_mem, lo.A, 2 * H * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, nullptr, 0, nullptr, keys, lo.A, lo.A,
+                   0.f, 0, 0, nullptr, st, lo.c.split_bf16);
 }
 
 struct DecBufs { bf16 *S1, *S2, *PI, *values; float *c1, *c2, *cum, *attU, *keys, *pre1; size_t att_smem; int K1r, K2, PIK; };
-// zero initial decoder state (Architecture_wrappers.py:134-167) + the merged location filter bank
-static int decoder_reset(const StepCtx& s, DecBufs& d) {
-  const TL& lo = *s.lo;
-  uint8_t* ws = s.ws; const float* d_params = s.params; cudaStream_t st = s.st;
-  const int B = lo.B, Ti = lo.Ti, H = lo.H, D = lo.D;
+static void decoder_bufs(const TL& lo, uint8_t* ws, DecBufs& d) {
+  const int H = lo.H, D = lo.D;
   d.K1r = 2 * H + D; d.K2 = 2 * D; d.PIK = D + 2 * H;
   d.S1 = reinterpret_cast<bf16*>(ws + lo.w_S1); d.S2 = reinterpret_cast<bf16*>(ws + lo.w_S2); d.PI = reinterpret_cast<bf16*>(ws + lo.w_PI);
   d.c1 = reinterpret_cast<float*>(ws + lo.w_c1); d.c2 = reinterpret_cast<float*>(ws + lo.w_c2);
   d.cum = reinterpret_cast<float*>(ws + lo.w_cum); d.attU = reinterpret_cast<float*>(ws + lo.w_attU);
   d.keys = reinterpret_cast<float*>(ws + lo.w_keys); d.values = reinterpret_cast<bf16*>(ws + lo.w_values);
   d.pre1 = reinterpret_cast<float*>(ws + lo.w_pre1);
-  T2_CHECK_CUDA(cudaMemsetAsync(d.S1, 0, (size_t)B * d.K1r * 2, st));
-  T2_CHECK_CUDA(cudaMemsetAsync(d.S2, 0, (size_t)B * d.K2 * 2, st));
+  d.att_smem = att_fwd_smem(lo.Ti, lo.KA, lo.A, D, 2 * H);
+}
+// zero initial decoder state (Architecture_wrappers.py:134-167) + the merged location filter bank
+static int decoder_reset(const StepCtx& s, DecBufs& d) {
+  const TL& lo = *s.lo;
+  const float* d_params = s.params; cudaStream_t st = s.st;
+  const int B = lo.B, Ti = lo.Ti, D = lo.D;
+  decoder_bufs(lo, s.ws, d);
+  T2_CHECK_CUDA(cudaMemsetAsync(d.S1, 0, (size_t)B * lo.ld_S1 * 2, st));
+  T2_CHECK_CUDA(cudaMemsetAsync(d.S2, 0, (size_t)B * lo.ld_S2 * 2, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.c1, 0, (size_t)B * D * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.c2, 0, (size_t)B * D * 4, st));
   T2_CHECK_CUDA(cudaMemsetAsync(d.cum, 0, (size_t)B * Ti * 4, st));
-  d.att_smem = att_fwd_smem(Ti, lo.KA, lo.A, D, 2 * H);
   return att_fwd_setup(d_params + lo.p_lck, d_params + lo.p_lcb, d_params + lo.p_lfl, d_params + lo.p_ba, d.attU, lo.KA, lo.F, lo.A, d.att_smem,
-                       lo.c.unmasked_encoder, lo.c.noncumulative_weights, st);
+                       lo.c.unmasked_encoder, lo.c.noncumulative_weights, lo.c.split_bf16, st);
 }
 // decoder step t: LSTM-1 (prenet part of its gates precomputed in pre1[t]), LSTM-2, attention (Architecture_wrappers.py:169-213)
 static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_lengths, int t) {
   const TL& lo = *s.lo;
   uint8_t* ws = s.ws; const uint8_t* pk = s.pk; const float* d_params = s.params; cudaStream_t st = s.st;
   const int B = lo.B, Ti = lo.Ti, H = lo.H, D = lo.D, K1r = d.K1r, K2 = d.K2, PIK = d.PIK;
-  bf16* S1t = d.S1 + (long long)t * B * K1r;
-  bf16* S1n = d.S1 + (long long)(t + 1) * B * K1r;
-  bf16* S2t = d.S2 + (long long)t * B * K2;
-  bf16* S2n = d.S2 + (long long)(t + 1) * B * K2;
-  bf16* PIt = d.PI + (long long)t * B * PIK;
+  const int ld1 = lo.ld_S1, ld2 = lo.ld_S2, ldp = lo.ld_PI;   // row pitches: K1r / K2 / PIK, split 3 K1r / 3 K2 / 2 PIK
+  bf16* S1t = d.S1 + (long long)t * B * ld1;
+  bf16* S1n = d.S1 + (long long)(t + 1) * B * ld1;
+  bf16* S2t = d.S2 + (long long)t * B * ld2;
+  bf16* S2n = d.S2 + (long long)(t + 1) * B * ld2;
+  bf16* PIt = d.PI + (long long)t * B * ldp;
   // LSTM 1: state operand [ctx_{t-1} | h1_{t-1}], input part precomputed in pre1[t]
   int rc = lstm_step(s, pk + lo.k_l1r, D, K1r, S1t, B, d.pre1 + (long long)t * B * 4 * D, 4 * D, nullptr, d.c1 + (long long)t * B * D,
-                     d.c1 + (long long)(t + 1) * B * D, S1t + 2 * H, K1r, S1n + 2 * H, K1r, S2t, K2,
+                     d.c1 + (long long)(t + 1) * B * D, S1t + 2 * H, ld1, S1n + 2 * H, ld1, S2t, ld2,
                      reinterpret_cast<bf16*>(ws + lo.w_g1) + (long long)t * B * 4 * D, reinterpret_cast<bf16*>(ws + lo.w_t1) + (long long)t * B * D,
-                     nullptr, t, 54, lo.c.zoneout_rate);
+                     nullptr, t, 54, lo.c.zoneout_rate, K2, 1);
   if (rc) return rc;
   // LSTM 2: state operand [h1out_t | h2_{t-1}]
   rc = lstm_step(s, pk + lo.k_l2, D, K2, S2t, B, nullptr, 0, d_params + lo.p_l2b, d.c2 + (long long)t * B * D, d.c2 + (long long)(t + 1) * B * D,
-                 S2t + D, K2, S2n + D, K2, PIt, PIK, reinterpret_cast<bf16*>(ws + lo.w_g2) + (long long)t * B * 4 * D,
-                 reinterpret_cast<bf16*>(ws + lo.w_t2) + (long long)t * B * D, nullptr, t, 55, lo.c.zoneout_rate);
+                 S2t + D, ld2, S2n + D, ld2, PIt, ldp, reinterpret_cast<bf16*>(ws + lo.w_g2) + (long long)t * B * 4 * D,
+                 reinterpret_cast<bf16*>(ws + lo.w_t2) + (long long)t * B * D, nullptr, t, 55, lo.c.zoneout_rate, PIK, 0);
   if (rc) return rc;
   AttArgs a;
-  a.h2out = PIt; a.ld_h2 = PIK; a.WqT = reinterpret_cast<const bf16*>(pk + lo.k_qT);
+  a.h2out = PIt; a.ld_h2 = ldp; a.WqT = reinterpret_cast<const bf16*>(pk + lo.k_qT);
   a.U = d.attU; a.v = d_params + lo.p_v;
   a.keys = d.keys; a.values = d.values; a.lens = d_input_lengths; a.cum = d.cum;
   a.alpha = reinterpret_cast<float*>(ws + lo.w_alpha) + (long long)t * B * Ti;
-  a.ctx_a = S1n; a.ld_a = K1r; a.ctx_b = PIt + D; a.ld_b = PIK;
+  a.ctx_a = S1n; a.ld_a = ld1; a.ctx_b = PIt + D; a.ld_b = ldp;
   a.B = B; a.Ti = Ti; a.D = D; a.A = lo.A; a.KA = lo.KA; a.C2 = 2 * H;
   a.unmasked = lo.c.unmasked_encoder; a.noncumulative = lo.c.noncumulative_weights;
+  a.split = lo.c.split_bf16; a.lo_h2 = PIK; a.lo_a = K1r; a.lo_b = PIK;
   return launch_att_fwd(a, d.att_smem, st);
 }
 
@@ -1436,24 +1531,25 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   if (rc) return rc;
   const void* x = nullptr;
   bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
-  decin_kernel<<<grid1d((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M); t2_count_launch();
+  decin_kernel<<<grid1d((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M, lo.c.split_bf16); t2_count_launch();
   const long long TB = (long long)To * B;
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
   float* pre1 = reinterpret_cast<float*>(ws + lo.w_pre1);
   float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
   const int PIK = D + 2 * H;
+  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1;   // split_bf16: packed forward operands are [W_hi | W_hi | W_lo]
   DecBufs db;
   if (lo.c.teacher_forcing_ratio >= 1.f) {
     // ---- decoder: everything that does not depend on the recurrence is batched over time (teacher forcing) ----
-    rc = conv_gemm(decin, lo.M, TB, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, pn1, nullptr, lo.P1,
-                   lo.P1, lo.c.dropout_rate, 20, seed, d_step, st);
+    rc = conv_gemm(decin, lo.M, TB, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, pn1, nullptr, lo.P1,
+                   lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, sp);
     if (rc) return rc;
-    rc = conv_gemm(pn1, lo.P1, TB, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, pn2, nullptr, lo.P2,
-                   lo.P2, lo.c.dropout_rate, 21, seed, d_step, st);
+    rc = conv_gemm(pn1, lo.P1, TB, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, pn2, nullptr, lo.P2,
+                   lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, sp);
     if (rc) return rc;
-    rc = conv_gemm(pn2, lo.P2, TB, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr, pre1, 4 * D, 4 * D, 0.f, 0, 0,
-                   nullptr, st);
+    rc = conv_gemm(pn2, lo.P2, TB, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr, pre1, 4 * D, 4 * D, 0.f, 0, 0,
+                   nullptr, st, sp);
     if (rc) return rc;
     rc = decoder_reset(s, db);
     if (rc) return rc;
@@ -1461,7 +1557,8 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
     T2_CHECK_CUDA(cudaGetLastError());
     // frame + stop projections for all steps at once
     // bias vector [M frames | 1 stop] lives in two parameter tensors: add them in the finishing kernel instead
-    rc = conv_gemm(db.PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st);
+    rc = conv_gemm(db.PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st,
+                   sp);
     if (rc) return rc;
     // add the projection biases in place (tiny), then clip / losses
     proj_bias_kernel<<<grid1d(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
@@ -1473,24 +1570,24 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
     if (rc) return rc;
     int* choice = reinterpret_cast<int*>(ws + lo.w_tfsel);
     for (int t = 0; t < To; ++t) {
-      rc = conv_gemm(decin + (long long)t * B * lo.M, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b,
-                     1, pn1 + (long long)t * B * lo.P1, nullptr, lo.P1, lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, 0, t * B);
+      rc = conv_gemm(decin + (long long)t * B * lo.ld_decin, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128,
+                     d_params + lo.p_p1b, 1, pn1 + (long long)t * B * lo.ld_pn1, nullptr, lo.P1, lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, sp, t * B);
       if (rc) return rc;
-      rc = conv_gemm(pn1 + (long long)t * B * lo.P1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128,
-                     d_params + lo.p_p2b, 1, pn2 + (long long)t * B * lo.P2, nullptr, lo.P2, lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, 0, t * B);
+      rc = conv_gemm(pn1 + (long long)t * B * lo.ld_pn1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128,
+                     d_params + lo.p_p2b, 1, pn2 + (long long)t * B * lo.ld_pn2, nullptr, lo.P2, lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, sp, t * B);
       if (rc) return rc;
-      rc = conv_gemm(pn2 + (long long)t * B * lo.P2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
-                     pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st);
+      rc = conv_gemm(pn2 + (long long)t * B * lo.ld_pn2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
+                     pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st, sp);
       if (rc) return rc;
       rc = decoder_step(s, db, d_input_lengths, t);
       if (rc) return rc;
       float* pt = projo + (long long)t * B * 128;
-      rc = conv_gemm(db.PI + (long long)t * B * PIK, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
-                     lo.M + 1, 0.f, 0, 0, nullptr, st);
+      rc = conv_gemm(db.PI + (long long)t * B * lo.ld_PI, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
+                     lo.M + 1, 0.f, 0, 0, nullptr, st, sp);
       if (rc) return rc;
       T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
-                               d_params + lo.p_sb, t + 1 < To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M, d_mel_targets, To, t,
-                               lo.c.teacher_forcing_ratio, seed, d_step, choice));
+                               d_params + lo.p_sb, t + 1 < To ? decin + (long long)(t + 1) * B * lo.ld_decin : (bf16*)nullptr, B, lo.M, d_mel_targets, To,
+                               t, lo.c.teacher_forcing_ratio, seed, d_step, choice, sp));
       t2_count_launch();
     }
     T2_CHECK_CUDA(cudaGetLastError());
@@ -1534,7 +1631,7 @@ extern "C" int t2_taco_infer_begin(const t2_taco_config_t* cfg, float* d_params,
   DecBufs db;
   rc = decoder_reset(s, db);
   if (rc) return rc;
-  T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_decin, 0, (size_t)lo.B * lo.M * 2, st));   // go frame (helpers.py:31)
+  T2_CHECK_CUDA(cudaMemsetAsync(ws + lo.w_decin, 0, (size_t)lo.B * lo.ld_decin * 2, st));   // go frame (helpers.py:31)
   return T2_OK;
 }
 
@@ -1552,41 +1649,36 @@ extern "C" int t2_taco_infer_steps(const t2_taco_config_t* cfg, float* d_params,
   const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
   StepCtx s{&lo, ws, pk, d_params, st, seed, nullptr, 0};
   const int B = lo.B, D = lo.D, H = lo.H, PIK = D + 2 * H;
+  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1;
   DecBufs db;
-  db.K1r = 2 * H + D; db.K2 = 2 * D; db.PIK = PIK;
-  db.S1 = reinterpret_cast<bf16*>(ws + lo.w_S1); db.S2 = reinterpret_cast<bf16*>(ws + lo.w_S2); db.PI = reinterpret_cast<bf16*>(ws + lo.w_PI);
-  db.c1 = reinterpret_cast<float*>(ws + lo.w_c1); db.c2 = reinterpret_cast<float*>(ws + lo.w_c2);
-  db.cum = reinterpret_cast<float*>(ws + lo.w_cum); db.attU = reinterpret_cast<float*>(ws + lo.w_attU);
-  db.keys = reinterpret_cast<float*>(ws + lo.w_keys); db.values = reinterpret_cast<bf16*>(ws + lo.w_values);
-  db.pre1 = reinterpret_cast<float*>(ws + lo.w_pre1);
-  db.att_smem = att_fwd_smem(lo.Ti, lo.KA, lo.A, D, 2 * H);
+  decoder_bufs(lo, ws, db);
   bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
   float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
   for (int t = t_begin; t < t_end; ++t) {
     const unsigned long long seed_t = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(t + 1);   // fresh prenet masks per step
-    bf16* x0 = decin + (long long)t * B * lo.M;
-    bf16* x1 = pn1 + (long long)t * B * lo.P1;
-    bf16* x2 = pn2 + (long long)t * B * lo.P2;
-    rc = conv_gemm(x0, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, x1, nullptr, lo.P1,
-                   lo.P1, lo.c.dropout_rate, 20, seed_t, nullptr, st);
+    bf16* x0 = decin + (long long)t * B * lo.ld_decin;
+    bf16* x1 = pn1 + (long long)t * B * lo.ld_pn1;
+    bf16* x2 = pn2 + (long long)t * B * lo.ld_pn2;
+    rc = conv_gemm(x0, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, x1, nullptr, lo.P1,
+                   lo.P1, lo.c.dropout_rate, 20, seed_t, nullptr, st, sp);
     if (rc) return rc;
-    rc = conv_gemm(x1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, x2, nullptr, lo.P2,
-                   lo.P2, lo.c.dropout_rate, 21, seed_t, nullptr, st);
+    rc = conv_gemm(x1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, x2, nullptr, lo.P2,
+                   lo.P2, lo.c.dropout_rate, 21, seed_t, nullptr, st, sp);
     if (rc) return rc;
-    rc = conv_gemm(x2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
-                   db.pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st);
+    rc = conv_gemm(x2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
+                   db.pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st, sp);
     if (rc) return rc;
     rc = decoder_step(s, db, d_input_lengths, t);
     if (rc) return rc;
     float* pt = projo + (long long)t * B * 128;
-    rc = conv_gemm(db.PI + (long long)t * B * PIK, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128, lo.M + 1,
-                   0.f, 0, 0, nullptr, st);
+    rc = conv_gemm(db.PI + (long long)t * B * lo.ld_PI, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
+                   lo.M + 1, 0.f, 0, 0, nullptr, st, sp);
     if (rc) return rc;
     T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
-                             d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.M : (bf16*)nullptr, B, lo.M,
-                             (const float*)nullptr, lo.To, t, 0.f, 0ull, (const unsigned long long*)nullptr, (int*)nullptr));
+                             d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.ld_decin : (bf16*)nullptr, B, lo.M,
+                             (const float*)nullptr, lo.To, t, 0.f, 0ull, (const unsigned long long*)nullptr, (int*)nullptr, sp));
     t2_count_launch();
   }
   T2_CHECK_CUDA(cudaGetLastError());
@@ -1639,9 +1731,9 @@ extern "C" int t2_taco_workspace_tensor(const t2_taco_config_t* cfg, void* d_wor
   const long long B = lo.B, Ti = lo.Ti, To = lo.To;
   struct E { const char* n; long long off, cnt; int eb; };
   const E table[] = {
-      {"memory", lo.w_memory, B * Ti * 2 * lo.H, 2}, {"keys", lo.w_keys, B * Ti * lo.A, 4}, {"alignments", lo.w_alpha, To * B * Ti, 4},
+      {"memory", lo.w_memory, B * Ti * lo.ld_mem, 2}, {"keys", lo.w_keys, B * Ti * lo.A, 4}, {"alignments", lo.w_alpha, To * B * Ti, 4},
       {"decoder_output", lo.w_decf, B * To * lo.M, 4}, {"mel_outputs", lo.w_mel, B * To * lo.M, 4}, {"stop_logits", lo.w_stop, B * To, 4},
-      {"projection_rows", lo.w_projo, To * B * 128, 4}, {"enc_conv_out", lo.enc.back().w_x, B * Ti * lo.C, 2}, {"prenet", lo.w_pn2, To * B * lo.P2, 2}, {"proj_in", lo.w_PI, To * B * (lo.D + 2 * lo.H), 2},
+      {"projection_rows", lo.w_projo, To * B * 128, 4}, {"enc_conv_out", lo.enc.back().w_x, B * Ti * lo.C, 2}, {"prenet", lo.w_pn2, To * B * lo.ld_pn2, 2}, {"proj_in", lo.w_PI, To * B * lo.ld_PI, 2},
       {"attention_filter_bank", lo.w_attU, (lo.KA + 1) * lo.A, 4},   // merged location filters U [KA][A] + offset row u0
       {"teacher_forced", lo.w_tfsel, To, 4},   // int32 per-step choices of the last forward at teacher_forcing_ratio < 1
   };
@@ -2010,7 +2102,7 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       a.ctx_a = static_cast<bf16*>(p[13]); a.ld_a = int(i[8]); a.ctx_b = static_cast<bf16*>(p[14]); a.ld_b = int(i[9]);
       a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2; a.unmasked = int(i[10]); a.noncumulative = int(i[11]);
       int rc = att_fwd_setup(static_cast<const float*>(p[2]), static_cast<const float*>(p[3]), static_cast<const float*>(p[4]),
-                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, a.unmasked, a.noncumulative, st);
+                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, a.unmasked, a.noncumulative, 0, st);
       return rc ? rc : launch_att_fwd(a, smem, st);
     }
     case T2_DBG_TACO_ATT_BWD: {

@@ -111,8 +111,9 @@ def make_config(hp, B, T_in, T_out, precision="bf16", teacher_forcing_ratio=None
 
 class Tacotron(object):
     def __init__(self, hparams, B, T_in, T_out, device="cuda", precision="bf16", teacher_forcing_ratio=None):
-        """precision 'fp32-class': the convolution stacks (encoder convs, postnet) run on bf16 hi + lo operand pairs with fp32
-        pre-batch-norm activations; forward / losses only (include/t2b200.h, t2_taco_config_t.split_bf16).
+        """precision 'fp32-class': every contraction of the forward and of synthesize() - convolution stacks, encoder BiLSTM, prenet,
+        decoder LSTMs, attention, frame / stop projection - runs on bf16 hi + lo operand pairs with hi + lo stored activations and
+        fp32 pre-batch-norm activations / cell states; forward / losses / synthesis only (include/t2b200.h, t2_taco_config_t.split_bf16).
         teacher_forcing_ratio (default hparams.tacotron_teacher_forcing_ratio): below 1, every decoder step of forward() draws whether
         the next step consumes the target frame or the frame just predicted, and backward() differentiates through the fed-back frames."""
         self.hp = hparams
