@@ -152,17 +152,22 @@ int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 /* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
  * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):
  * BN_FWD       bn_stats_kernel (training) + bn_apply_kernel. p: y, xb bf16 (nullable), xf fp32 [rows][C] (nullable), add fp32 [rows][C] (nullable),
- *              stats, gamma, beta, mm, mv. i: rows, C, ld, c0, Ct, training, y_fp32, stat_threads (128 or 256).
+ *              stats, gamma, beta, mm, mv. i: rows, C, ld, c0, Ct, training, y_fp32, stat_threads (128 or 256), split (0 / 1: xb rows are
+ *              [hi(ld) | lo(ld)] at pitch 2 ld).
  * BN_BWD       bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: g, y (both bf16, or both fp32 when i[9]), stats, bsum, gamma, dpre bf16, dgamma, dbeta.
  *              i: rows, C, ldg, ld, c0, Ct, ldd, act, stat_threads, fp32.
- * POOL_FWD     maxpool_fwd_k. p: x bf16 [N][C], out. i: N (= B T rows), T, C.
+ * POOL_FWD     maxpool_fwd_k. p: x bf16 [N][C], out. i: N (= B T rows), T, C, split (0 / 1: x and out are [N][hi(C) | lo(C)] rows, the
+ *              pair with the larger hi + lo wins).
  * POOL_BWD     maxpool_bwd_k. p: x, dout, dx. i: N, T, C.
- * HIGHWAY_FWD  highway_fwd_k. p: pre fp32 [N][2HU], bh, bt, h fp32 [N][HU], hf fp32, hb bf16, HT bf16 [N][2HU] (nullable). i: N, HU.
+ * HIGHWAY_FWD  highway_fwd_k. p: pre fp32 [N][2HU], bh, bt, h fp32 [N][HU], hf fp32, hb bf16, HT bf16 [N][2HU] (nullable). i: N, HU,
+ *              split (0 / 1: hb is [N][hi(HU) | lo(HU)]).
  * HIGHWAY_BWD  highway_bwd_k. p: dh fp32, HT bf16, h fp32, dHT bf16 [N][2HU], dcarry fp32. i: N, HU.
  * GRU_FWD      gru_fwd_kernel, both directions over the whole padded sequence (rows b T + t, N = B T). p: params fp32 (flat; the kernel
  *              reads the recurrent rows [HU, HU + RU) of the two kernels and the biases), XP fp32 [N][6RU] ([fw gates | fw cand | bw gates
  *              | bw cand], no biases), out bf16 [N][2RU], then the stashes bf16 [N][RU] r, u, c, rh of fw, then of bw (all eight present,
- *              or all null as in inference). i: B, T, HU, RU (= 128), then p_gk, p_ck, p_gb, p_cb of fw, then of bw (offsets into params).
+ *              or all null as in inference). i: B, T, HU, RU (= 128), then p_gk, p_ck, p_gb, p_cb of fw, then of bw (offsets into params),
+ *              then i[12] split (0 / 1: the recurrent weights are used as hi + lo pairs, out is [N][hi(2RU) | lo(2RU)] and the eight stashes
+ *              must be null).
  * GRU_BWD      gru_bwd_kernel (BPTT of both directions). p: params, dout fp32 [N][2RU], out bf16 [N][2RU] (h_prev, as GRU_FWD writes it),
  *              the stashes r, u, c of fw, then of bw, dXP bf16 [N][6RU] (out: [dr_pre | du_pre | dc_pre] per direction).
  *              i: B, T, HU, RU (= 128), then p_gk, p_ck of fw, then of bw. */
@@ -366,7 +371,7 @@ typedef struct {
   float max_abs_value, lower_bound_decay;
   int split_bf16;            /* 1 = "fp32-class" forward: every contraction of the training / GTA forward and of free-running synthesis
                               * (embedding, encoder conv blocks, encoder BiLSTM, memory layer, prenet, decoder LSTMs, attention query and
-                              * context, frame / stop projection, postnet) runs on bf16 hi + lo operand pairs (hi.hi + lo.hi + hi.lo, fp32
+                              * context, frame / stop projection, postnet; the CBHG head has its own t2_cbhg_config_t.split_bf16) runs on bf16 hi + lo operand pairs (hi.hi + lo.hi + hi.lo, fp32
                               * accumulate) and every stored activation / recurrent state is a hi + lo pair; pre-batch-norm activations and
                               * cell states are fp32. Forward / losses / synthesis only (no backward); the LSTM sizes must be multiples of 64. */
   int mask_decoder;          /* 1 = masked losses (tacotron/models/modules.py:412-455): MSE terms over the frames t < targets_lengths[b]
@@ -475,6 +480,11 @@ typedef struct {
   int n_priority_freq;       /* int(2000 / (sample_rate / 2) * num_freq): bins carrying the second half of the L1 weight */
   int clip_outputs, mask_decoder;
   float max_abs_value, lower_bound_decay, reg_weight;
+  int split_bf16;            /* 1 = "fp32-class" forward (t2_taco_config_t.split_bf16): every contraction - conv bank, projections,
+                              * dense, highway layers, GRU input projections and recurrence, linear projection - runs on bf16 hi + lo
+                              * operand pairs (hi.hi + lo.hi + hi.lo, fp32 accumulate; the recurrence h.W_hi + h.W_lo with the fp32 state)
+                              * and every stored bf16 activation is a hi + lo pair; pre-batch-norm activations are fp32. Forward / losses
+                              * only: t2_cbhg_backward returns T2_ERR_INVALID_ARG. 0 = bf16 operands; other values are T2_ERR_INVALID_ARG. */
 } t2_cbhg_config_t;
 int t2_cbhg_sizes(const t2_cbhg_config_t* cfg, long long* n_params, long long* packed_bytes, long long* workspace_bytes, int* n_tensors);
 int t2_cbhg_param_info(const t2_cbhg_config_t* cfg, int i, char* name, int name_cap, long long* offset, int* ndim, int* shape4,
@@ -493,6 +503,12 @@ int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, const void* d_
  * buffer; overwritten), d(loss)/d(mel_outputs) into d_mel_grad fp32 [B][T][num_mels] */
 int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_params, const void* d_packed, void* d_workspace, const float* d_mel,
                      float* d_grads, float* d_mel_grad, void* stream);
+/* debug / test access to workspace tensors by name: "linear_outputs" fp32 (as above), bf16 "rnn_outputs" [B][T][2 RU], "highway_input"
+ * [B][T][num_mels], "bank_outputs" / "pooled_outputs" [B][T][kernels * conv_channels] (after the batch norm / the max-pool), "gru_input"
+ * [B][T][highway_units], fp32 "gru_xp" [B][T][6 RU], and the training stashes. With split_bf16 = 1 the bf16 activation tensors double
+ * their rows: "rnn_outputs" [B][T][hi(2 RU) | lo(2 RU)], "bank_outputs" / "pooled_outputs" [B][T][hi(K CC) | lo(K CC)], "gru_input"
+ * [B][T][hi(HU) | lo(HU)] and "highway_input" [B][T][hi(Ms) | lo(Ms)] with num_mels zero-padded to Ms, the next multiple of 64 (count is the
+ * element count of those rows); the fp32 value of a channel is float(hi) + float(lo). "linear_outputs" and "gru_xp" stay fp32. */
 int t2_cbhg_workspace_tensor(const t2_cbhg_config_t* cfg, void* d_workspace, const char* name, void** ptr, long long* count);
 
 /* ---- optimizer: tf.train.AdamOptimizer + per-tensor clip_by_norm/clip_by_value + EMA ------------------------

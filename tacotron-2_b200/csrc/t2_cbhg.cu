@@ -68,6 +68,7 @@ struct CL {
 
 int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   T2_REQUIRE(cfg != nullptr, T2_ERR_INVALID_ARG, "null CBHG config");
+  T2_REQUIRE(cfg->split_bf16 == 0 || cfg->split_bf16 == 1, T2_ERR_INVALID_ARG, "split_bf16 %d is not 0 or 1", cfg->split_bf16);
   lo.c = *cfg;
   lo.B = cfg->B; lo.T = cfg->T; lo.M = cfg->num_mels; lo.K = cfg->kernels; lo.CC = cfg->conv_channels; lo.KC = lo.K * lo.CC;
   lo.PJc = cfg->projection; lo.PK = cfg->projection_kernel_size; lo.NH = cfg->highwaynet_layers; lo.HU = cfg->highway_units;
@@ -114,14 +115,22 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   lo.p_lk = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/kernel", {2 * lo.RU, lo.NF}); lo.p_lb = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/bias", {lo.NF});
 
   // ---- packed operands ----
+  // split_bf16: every forward operand is [W_hi | W_hi | W_lo] per K slot (add_pack_split; set_split_operand in t2_gemm.h), so its
+  // K pitch triples; the data-gradient operands of the backward pass keep their bf16 layout
+  const bool split = cfg->split_bf16 != 0;
+  const int s3 = split ? 3 : 1;
   std::vector<PackJob> jobs;
   Arena pk;
   auto conv_pack = [&](CConv& L, bool with_t) {
     const int rows_f = (L.cout + 127) / 128 * 128, rows_t = (L.cin + 127) / 128 * 128;
-    L.k_w = pk.take(2LL * rows_f * L.k * L.cinp);
+    L.k_w = pk.take(2LL * rows_f * L.k * L.cinp * s3);
     L.k_wT = with_t ? pk.take(2LL * rows_t * L.k * L.coutp) : 0;
     for (int j = 0; j < L.k; ++j) {
-      add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
+      if (split)
+        add_pack_split(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp,
+                       3 * j * L.cinp + 2 * L.cinp, L.cinp);
+      else
+        add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
       if (with_t) add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
     }
   };
@@ -142,28 +151,41 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
       for (int j = 0; j < lo.bank[l].k; ++j, ++slot)
         add_pack(jobs, lo.bank[l].p.kernel + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
   }
-  const int Mp = 128;
-  lo.k_dense = pk.take(2LL * lo.HU * Mp); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0);
+  const int Mp = 128, Ms = (lo.M + 63) / 64 * 64;     // Ms: the K slot of num_mels in the split operands
+  if (split) { lo.k_dense = pk.take(2LL * lo.HU * 3 * Ms); add_pack_split(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, 3 * Ms, 0, 2 * Ms, Ms); }
+  else { lo.k_dense = pk.take(2LL * lo.HU * Mp); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0); }
   lo.k_denseT = pk.take(2LL * 128 * lo.HU); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_denseT, lo.HU, 0, 0);
   for (int i = 0; i < lo.NH; ++i) {
-    lo.k_hw[i] = pk.take(2LL * 2 * lo.HU * lo.HU);             // rows [H units | T units][K = HU]
-    add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 1, 0);
-    add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * lo.HU, lo.HU, 1, 0);
+    lo.k_hw[i] = pk.take(2LL * 2 * lo.HU * lo.HU * s3);        // rows [H units | T units][K = HU]
+    if (split) {
+      add_pack_split(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
+      add_pack_split(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
+    } else {
+      add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 1, 0);
+      add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * lo.HU, lo.HU, 1, 0);
+    }
     lo.k_hwT[i] = pk.take(2LL * lo.HU * 2 * lo.HU);            // [HU in][H units | T units]
     add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, 0);
     add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, lo.HU);
   }
   // GRU input projections: output columns [fw gates 2RU | fw cand RU | bw gates 2RU | bw cand RU], K = HU (the first HU kernel rows)
   const int XPW = 6 * lo.RU;
-  lo.k_gx = pk.take(2LL * XPW * lo.HU);
+  lo.k_gx = pk.take(2LL * XPW * lo.HU * s3);
   lo.k_gxT = pk.take(2LL * lo.HU * XPW);
   for (int d = 0; d < 2; ++d) {
-    add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * lo.HU, lo.HU, 1, 0);
-    add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * lo.HU, lo.HU, 1, 0);
+    if (split) {
+      add_pack_split(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
+      add_pack_split(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
+    } else {
+      add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * lo.HU, lo.HU, 1, 0);
+      add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * lo.HU, lo.HU, 1, 0);
+    }
     add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU);
     add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU + 2 * lo.RU);
   }
-  lo.k_lin = pk.take(2LL * lo.NFR * 2 * lo.RU); add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 1, 0);
+  lo.k_lin = pk.take(2LL * lo.NFR * 2 * lo.RU * s3);
+  if (split) add_pack_split(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 6 * lo.RU, 0, 4 * lo.RU, 2 * lo.RU);
+  else add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 1, 0);
   const int NFK = (lo.NF + 63) / 64 * 64;
   lo.k_linT = pk.take(2LL * 2 * lo.RU * NFK); add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_linT, NFK, 0, 0);
   lo.packed_bytes = pk.used;
@@ -172,15 +194,17 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   // ---- workspace ----
   Arena ws;
   const long long N = lo.N;
-  lo.w_x0 = ws.take(N * lo.M * 2);
-  lo.w_Y = ws.take(N * lo.KC * 2); lo.w_Xb = ws.take(N * lo.KC * 2); lo.w_P = ws.take(N * lo.KC * 2); lo.w_stb = ws.take(8LL * lo.KC * 4);
-  lo.w_Y1 = ws.take(N * lo.PJc * 2); lo.w_X1 = ws.take(N * lo.PJc * 2); lo.w_st1 = ws.take(8LL * lo.PJc * 4);
+  // split_bf16: the bf16 operands become [hi | lo] rows (num_mels padded to Ms per half), the pre-batch-norm activations fp32
+  const long long xm = split ? 2 : 1, ym = split ? 4 : 2, mw = split ? 2LL * Ms : lo.M;
+  lo.w_x0 = ws.take(N * mw * 2);
+  lo.w_Y = ws.take(N * lo.KC * ym); lo.w_Xb = ws.take(N * lo.KC * 2 * xm); lo.w_P = ws.take(N * lo.KC * 2 * xm); lo.w_stb = ws.take(8LL * lo.KC * 4);
+  lo.w_Y1 = ws.take(N * lo.PJc * ym); lo.w_X1 = ws.take(N * lo.PJc * 2 * xm); lo.w_st1 = ws.take(8LL * lo.PJc * 4);
   lo.w_Y2 = ws.take(N * lo.M * 4); lo.w_st2 = ws.take(8LL * 128 * 4);
-  lo.w_hin = ws.take(N * lo.M * 2);
-  for (int i = 0; i <= lo.NH; ++i) { lo.w_hf[i] = ws.take(N * lo.HU * 4); lo.w_hb[i] = ws.take(N * lo.HU * 2); }
+  lo.w_hin = ws.take(N * mw * 2);
+  for (int i = 0; i <= lo.NH; ++i) { lo.w_hf[i] = ws.take(N * lo.HU * 4); lo.w_hb[i] = ws.take(N * lo.HU * 2 * xm); }
   for (int i = 0; i < lo.NH; ++i) lo.w_HT[i] = ws.take(N * 2 * lo.HU * 2);
   lo.w_XP = ws.take(N * XPW * 4);
-  lo.w_out = ws.take(N * 2 * lo.RU * 2);
+  lo.w_out = ws.take(N * 2 * lo.RU * 2 * xm);
   for (int d = 0; d < 2; ++d) { lo.w_gr[d] = ws.take(N * lo.RU * 2); lo.w_gu[d] = ws.take(N * lo.RU * 2); lo.w_gc[d] = ws.take(N * lo.RU * 2); lo.w_grh[d] = ws.take(N * lo.RU * 2); }
   lo.w_lin = ws.take(N * lo.NFP * 4);            // fp32 [N][NFP]: padded pitch (the epilogue stores whole float4s)
   lo.w_scal = ws.take(64 * 4);
@@ -211,11 +235,23 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
 // small kernels
 // ------------------------------------------------------------------------------------------------------
 // tf.layers.max_pooling1d(pool 2, stride 1, 'same'): out[t] = max(x[t], x[t + 1]) (last step: x[t])
+// kSplit: x / out rows are [hi(C) | lo(C)]; the recombined values hi + lo are compared and the winning pair is copied (exact)
+template <bool kSplit>
 __global__ void maxpool_fwd_k(const bf16* __restrict__ x, bf16* __restrict__ out, long long N, int T, int C) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= N * C) return;
   const long long r = e / C;
   const int t = int(r % T);
+  if (kSplit) {
+    const long long o = r * 2 * C + e % C;
+    bf16 h = x[o], l = x[o + C];
+    if (t + 1 < T) {
+      const bf16 h2 = x[o + 2 * C], l2 = x[o + 3 * C];
+      if (__bfloat162float(h2) + __bfloat162float(l2) > __bfloat162float(h) + __bfloat162float(l)) { h = h2; l = l2; }
+    }
+    out[o] = h; out[o + C] = l;
+    return;
+  }
   float v = __bfloat162float(x[e]);
   if (t + 1 < T) v = fmaxf(v, __bfloat162float(x[e + C]));
   out[e] = __float2bfloat16(v);
@@ -234,6 +270,8 @@ __global__ void maxpool_bwd_k(const bf16* __restrict__ x, const bf16* __restrict
 }
 // highway layer (modules.py:12-16): pre [N][2HU] = [H pre-activation | T pre-activation] (biases added here);
 // h' = relu(H) sigmoid(T) + h (1 - sigmoid(T)). Stashes relu(H) | sigmoid(T) in bf16 for the backward pass.
+// kSplit: hb rows are [hi(HU) | lo(HU)] (the split operand of the next GEMM); hf stays the fp32 carry.
+template <bool kSplit>
 __global__ void highway_fwd_k(const float* __restrict__ pre, const float* __restrict__ bh, const float* __restrict__ bt, const float* __restrict__ h,
                               float* __restrict__ hf, bf16* __restrict__ hb, bf16* __restrict__ HT, long long N, int HU) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -242,7 +280,13 @@ __global__ void highway_fwd_k(const float* __restrict__ pre, const float* __rest
   const float Hh = fmaxf(pre[r * 2 * HU + c] + bh[c], 0.f);
   const float Tt = 1.f / (1.f + __expf(-(pre[r * 2 * HU + HU + c] + bt[c])));
   const float v = Hh * Tt + h[e] * (1.f - Tt);
-  hf[e] = v; hb[e] = __float2bfloat16(v);
+  hf[e] = v;
+  if (kSplit) {
+    const bf16 hi = __float2bfloat16(v);
+    hb[r * 2 * HU + c] = hi; hb[r * 2 * HU + HU + c] = __float2bfloat16(v - __bfloat162float(hi));
+  } else {
+    hb[e] = __float2bfloat16(v);
+  }
   if (HT) { HT[r * 2 * HU + c] = __float2bfloat16(Hh); HT[r * 2 * HU + HU + c] = __float2bfloat16(Tt); }
 }
 // dh' -> d[H pre | T pre] (bf16, GEMM operand) and the carry part dh * (1 - T) written to dcarry (fp32)
@@ -257,14 +301,15 @@ __global__ void highway_bwd_k(const float* __restrict__ dh, const bf16* __restri
   dHT[r * 2 * HU + HU + c] = __float2bfloat16(g * (Hh - h[e]) * Tt * (1.f - Tt));
   dcarry[e] = g * (1.f - Tt);
 }
-void maxpool_fwd(const bf16* x, bf16* out, long long N, int T, int C, cudaStream_t st) {
-  maxpool_fwd_k<<<grid1d(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
+void maxpool_fwd(const bf16* x, bf16* out, long long N, int T, int C, int split, cudaStream_t st) {
+  (split ? maxpool_fwd_k<true> : maxpool_fwd_k<false>)<<<grid1d(N * C), 256, 0, st>>>(x, out, N, T, C); t2_count_launch();
 }
 void maxpool_bwd(const bf16* x, const bf16* dout, bf16* dx, long long N, int T, int C, cudaStream_t st) {
   maxpool_bwd_k<<<grid1d(N * C), 256, 0, st>>>(x, dout, dx, N, T, C); t2_count_launch();
 }
-void highway_fwd(const float* pre, const float* bh, const float* bt, const float* h, float* hf, bf16* hb, bf16* HT, long long N, int HU, cudaStream_t st) {
-  highway_fwd_k<<<grid1d(N * HU), 256, 0, st>>>(pre, bh, bt, h, hf, hb, HT, N, HU); t2_count_launch();
+void highway_fwd(const float* pre, const float* bh, const float* bt, const float* h, float* hf, bf16* hb, bf16* HT, long long N, int HU, int split,
+                 cudaStream_t st) {
+  (split ? highway_fwd_k<true> : highway_fwd_k<false>)<<<grid1d(N * HU), 256, 0, st>>>(pre, bh, bt, h, hf, hb, HT, N, HU); t2_count_launch();
 }
 void highway_bwd(const float* dh, const bf16* HT, const float* h, bf16* dHT, float* dcarry, long long N, int HU, cudaStream_t st) {
   highway_bwd_k<<<grid1d(N * HU), 256, 0, st>>>(dh, HT, h, dHT, dcarry, N, HU); t2_count_launch();
@@ -334,20 +379,29 @@ __global__ void dmel_k(const float* __restrict__ a, const float* __restrict__ b,
 //   r, u = sigmoid(xg + h Wg_h) ; c = tanh(xc + (r h) Wc_h) ; h' = u h + (1 - u) c        (xg, xc: input projections incl. biases)
 // One CTA = kGruItems batch items of one direction for all T steps; recurrent weights live in shared memory as bf16 PAIRS along k
 // ([k/2][col] of bf16x2) so that a 4-byte load feeds two FMAs; state in fp32.
+// kSplit (split_bf16): the lo halves W - bf16(W) of the recurrent weights are staged behind the hi halves in the same layouts and every
+// product is h W_hi + h W_lo; out rows are [hi(2RU) | lo(2RU)] and the backward stashes are not written.
 // ------------------------------------------------------------------------------------------------------
 struct GruArgs {
   const float* params; long long p_gk[2], p_ck[2], p_gb[2], p_cb[2];
   const float* XP;          // [N][6RU] fp32
-  bf16* out;                // [N][2RU]: h of direction d in columns [d RU, (d+1) RU)
+  bf16* out;                // [N][2RU]: h of direction d in columns [d RU, (d+1) RU); split: [N][4RU], the lo halves at +2RU
   bf16 *r[2], *u[2], *c[2], *rh[2];   // stashes [N][RU] (nullable)
   int B, T, HU, RU;
 };
 constexpr int kRU = 128;
+// the lo halves w - bf16(w) of a k pair (pack_bf16x2 layout)
+__device__ __forceinline__ uint32_t pack_lo_bf16x2(float w0, float w1) {
+  return pack_bf16x2(w0 - __bfloat162float(__float2bfloat16(w0)), w1 - __bfloat162float(__float2bfloat16(w1)));
+}
+template <bool kSplit>
 __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
   extern __shared__ __align__(16) uint8_t gsm[];
   uint32_t* Wg = reinterpret_cast<uint32_t*>(gsm);                 // [64][256] bf16x2 (k pairs)
   uint32_t* Wc = Wg + 64 * 256;                                    // [64][128]
-  float* h = reinterpret_cast<float*>(Wc + 64 * 128);              // [4][128]
+  uint32_t* Wgl = Wc + 64 * 128;                                   // kSplit: lo halves, [64][256] then [64][128]
+  uint32_t* Wcl = Wgl + 64 * 256;
+  float* h = reinterpret_cast<float*>(kSplit ? Wcl + 64 * 128 : Wgl);   // [4][128]
   float* rhs = h + kGruItems * kRU;                                // [4][128]
   float* us = rhs + kGruItems * kRU;                               // [4][128]
   const int d = blockIdx.y, b0 = blockIdx.x * kGruItems, tid = threadIdx.x;
@@ -356,10 +410,12 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
   for (int i = tid; i < 64 * 256; i += kGruThreads) {
     const int kp = i / 256, col = i % 256;
     Wg[i] = pack_bf16x2(gk[(2 * kp) * 256 + col], gk[(2 * kp + 1) * 256 + col]);
+    if (kSplit) Wgl[i] = pack_lo_bf16x2(gk[(2 * kp) * 256 + col], gk[(2 * kp + 1) * 256 + col]);
   }
   for (int i = tid; i < 64 * 128; i += kGruThreads) {
     const int kp = i / 128, col = i % 128;
     Wc[i] = pack_bf16x2(ck[(2 * kp) * 128 + col], ck[(2 * kp + 1) * 128 + col]);
+    if (kSplit) Wcl[i] = pack_lo_bf16x2(ck[(2 * kp) * 128 + col], ck[(2 * kp + 1) * 128 + col]);
   }
   for (int i = tid; i < kGruItems * kRU; i += kGruThreads) h[i] = 0.f;
   __syncthreads();
@@ -376,6 +432,16 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
     for (int kp = 0; kp < 64; ++kp) {
       const uint32_t w = Wg[kp * 256 + tid];
       const float w0 = bf16lo(w), w1 = bf16hi(w);
+      if (kSplit) {
+        const uint32_t wl = Wgl[kp * 256 + tid];
+        const float l0 = bf16lo(wl), l1 = bf16hi(wl);
+#pragma unroll
+        for (int i = 0; i < kGruItems; ++i) {
+          const float2 hv = *reinterpret_cast<const float2*>(h + i * kRU + 2 * kp);
+          acc[i] += hv.x * w0 + hv.y * w1 + (hv.x * l0 + hv.y * l1);
+        }
+        continue;
+      }
 #pragma unroll
       for (int i = 0; i < kGruItems; ++i) {
         const float2 hv = *reinterpret_cast<const float2*>(h + i * kRU + 2 * kp);
@@ -388,13 +454,13 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
       if (tid < kRU) {
         const float rhv = g * h[i * kRU + tid];
         rhs[i * kRU + tid] = rhv;
-        if (a.r[d] && b0 + i < a.B) {
+        if (!kSplit && a.r[d] && b0 + i < a.B) {
           const long long o = ((long long)(b0 + i) * a.T + t) * kRU + tid;
           a.r[d][o] = __float2bfloat16(g); a.rh[d][o] = __float2bfloat16(rhv);
         }
       } else {
         us[i * kRU + tid - kRU] = g;
-        if (a.u[d] && b0 + i < a.B) a.u[d][((long long)(b0 + i) * a.T + t) * kRU + tid - kRU] = __float2bfloat16(g);
+        if (!kSplit && a.u[d] && b0 + i < a.B) a.u[d][((long long)(b0 + i) * a.T + t) * kRU + tid - kRU] = __float2bfloat16(g);
       }
     }
     __syncthreads();
@@ -407,6 +473,16 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
     for (int kp = 0; kp < 64; ++kp) {
       const uint32_t w = Wc[kp * 128 + j2];
       const float w0 = bf16lo(w), w1 = bf16hi(w);
+      if (kSplit) {
+        const uint32_t wl = Wcl[kp * 128 + j2];
+        const float l0 = bf16lo(wl), l1 = bf16hi(wl);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const float2 v = *reinterpret_cast<const float2*>(rhs + (2 * half + q) * kRU + 2 * kp);
+          cc[q] += v.x * w0 + v.y * w1 + (v.x * l0 + v.y * l1);
+        }
+        continue;
+      }
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const float2 v = *reinterpret_cast<const float2*>(rhs + (2 * half + q) * kRU + 2 * kp);
@@ -421,7 +497,11 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_fwd_kernel(GruArgs a) {
       const float uv = us[i * kRU + j2];
       hn[q] = uv * h[i * kRU + j2] + (1.f - uv) * cv;
       const long long row = (long long)(b0 + i) * a.T + t;
-      if (b0 + i < a.B) {
+      if (b0 + i < a.B && kSplit) {
+        const bf16 hi = __float2bfloat16(hn[q]);
+        a.out[row * 4 * kRU + d * kRU + j2] = hi;
+        a.out[row * 4 * kRU + 2 * kRU + d * kRU + j2] = __float2bfloat16(hn[q] - __bfloat162float(hi));
+      } else if (b0 + i < a.B) {
         a.out[row * 2 * kRU + d * kRU + j2] = __float2bfloat16(hn[q]);
         if (a.c[d]) a.c[d][row * kRU + j2] = __float2bfloat16(cv);
       }
@@ -534,15 +614,22 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_bwd_kernel(GruBwdArgs a) {
 // host helpers
 // ------------------------------------------------------------------------------------------------------
 // out[pos][n] = act(sum_taps sum_k a[pos + shift][k0 + k] w[n][tap * Cp + k] + bias[n]) on the wgmma engine (EPI_BIAS_ACT)
+// split: `a` is a split-bf16 operand (set_split_operand, t2_gemm.h: ld, k0, k0s and Ctot are unused) against [W_hi | W_hi | W_lo] weights
 int gemm(const void* a, int C, int ld, int k0, long long T, int Bn, const void* w, int wN, int wK, int ntaps, const int* shifts, int BN,
-         const float* bias, int act, void* out_bf16, float* out_f32, int ldo, int nvalid, cudaStream_t st, const int* k0s = nullptr, int Ctot = 0) {
+         const float* bias, int act, void* out_bf16, float* out_f32, int ldo, int nvalid, cudaStream_t st, const int* k0s = nullptr, int Ctot = 0,
+         int split = 0) {
   ActGemmCall g;
   memset(&g, 0, sizeof(g));
-  const int nkb = (C + kBK - 1) / kBK;
-  g.a[0] = make_act(a, Ctot > 0 ? Ctot : k0 + C, int(T), Bn, 1, ld); g.na = 1;
-  T2_REQUIRE(ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "CBHG gemm: too many taps");
-  for (int s = 0; s < ntaps; ++s) g.seg[s] = Seg{0, shifts ? shifts[s] : 0, k0s ? k0s[s] : k0, nkb, 0, 1};
-  g.nseg = ntaps;
+  if (split) {
+    const int rc = set_split_operand(g, a, C, int(T), Bn, ntaps, shifts);
+    if (rc) return rc;
+  } else {
+    const int nkb = (C + kBK - 1) / kBK;
+    g.a[0] = make_act(a, Ctot > 0 ? Ctot : k0 + C, int(T), Bn, 1, ld); g.na = 1;
+    T2_REQUIRE(ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "CBHG gemm: too many taps");
+    for (int s = 0; s < ntaps; ++s) g.seg[s] = Seg{0, shifts ? shifts[s] : 0, k0s ? k0s[s] : k0, nkb, 0, 1};
+    g.nseg = ntaps;
+  }
   g.w = w; g.wN = wN; g.wK = wK; g.wL = 1;
   g.T = int(T); g.B = Bn; g.n_tiles = (nvalid + BN - 1) / BN;
   g.epi.ptr[0] = out_bf16; g.epi.ptr[1] = const_cast<float*>(bias); g.epi.ptr[2] = out_f32;
@@ -579,13 +666,15 @@ void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
     L.push_back(w); }
 }
 
-size_t gru_fwd_smem() { return (64 * 256 + 64 * 128) * 4 + 3 * kGruItems * kRU * 4; }
+// bf16 104,448 B; split 202,752 B (the lo halves of both weight blocks), under the 232,448 B opt-in limit of sm_90
+size_t gru_fwd_smem(int split) { return (64 * 256 + 64 * 128) * 4 * (split ? 2 : 1) + 3 * kGruItems * kRU * 4; }
 size_t gru_bwd_smem() { return (128 * 128 + 64 * 128) * 4 + (2 * kGruItems * kRU + kGruItems * 2 * kRU) * 4; }
 
 // launch helpers shared by t2_cbhg_forward / t2_cbhg_backward and t2_dbg_cbhg_kernel: one grid (B / 4 items x 2 directions), block and
 // shared-memory size. The checks run before any driver call.
 int gru_setup() {
-  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem())));
+  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem(0))));
+  T2_CHECK_CUDA(cudaFuncSetAttribute(gru_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_fwd_smem(1))));
   T2_CHECK_CUDA(cudaFuncSetAttribute(gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(gru_bwd_smem())));
   return T2_OK;
 }
@@ -594,10 +683,12 @@ int check_gru_shape(int B, int T, int HU, int RU, const char* what) {
   T2_REQUIRE(RU == kRU, T2_ERR_UNSUPPORTED_SHAPE, "%s: RU must be %d (got %d)", what, kRU, RU);
   return T2_OK;
 }
-int check_gru_fwd(const GruArgs& a) {
+int check_gru_fwd(const GruArgs& a, int split) {
   T2_REQUIRE(a.params && a.XP && a.out, T2_ERR_INVALID_ARG, "gru_fwd: null params / XP / out");
+  T2_REQUIRE(split == 0 || split == 1, T2_ERR_INVALID_ARG, "gru_fwd: split %d is not 0 or 1", split);
   int n = 0;
   for (int d = 0; d < 2; ++d) n += (a.r[d] != nullptr) + (a.u[d] != nullptr) + (a.c[d] != nullptr) + (a.rh[d] != nullptr);
+  T2_REQUIRE(!split || n == 0, T2_ERR_INVALID_ARG, "gru_fwd: the split mode writes no stashes (%d of 8 given)", n);
   T2_REQUIRE(n == 0 || n == 8, T2_ERR_INVALID_ARG, "gru_fwd: the r / u / c / rh stashes of both directions are all present or all null (%d of 8)", n);
   for (int d = 0; d < 2; ++d)
     T2_REQUIRE(a.p_gk[d] >= 0 && a.p_ck[d] >= 0 && a.p_gb[d] >= 0 && a.p_cb[d] >= 0, T2_ERR_INVALID_ARG, "gru_fwd: negative parameter offset");
@@ -611,10 +702,11 @@ int check_gru_bwd(const GruBwdArgs& a) {
   }
   return check_gru_shape(a.B, a.T, a.HU, a.RU, "gru_bwd");
 }
-int launch_gru_fwd(const GruArgs& a, cudaStream_t st) {
-  int rc = check_gru_fwd(a);
+int launch_gru_fwd(const GruArgs& a, int split, cudaStream_t st) {
+  int rc = check_gru_fwd(a, split);
   if (rc) return rc;
-  gru_fwd_kernel<<<dim3((a.B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_fwd_smem(), st>>>(a); t2_count_launch();
+  (split ? gru_fwd_kernel<true> : gru_fwd_kernel<false>)<<<dim3((a.B + kGruItems - 1) / kGruItems, 2), kGruThreads, gru_fwd_smem(split), st>>>(a);
+  t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
@@ -701,8 +793,9 @@ int conv_fwd(const Ctx& s, const CConv& L, const void* x, int ld_x, bf16* y_b, f
   int shifts[16];
   for (int j = 0; j < L.k; ++j) shifts[j] = conv_tap_shift(L.k, j);
   const int BN = L.cout % 256 == 0 ? 256 : 128;
-  return gemm(x, L.cin, ld_x, 0, s.lo->T, s.lo->B, s.pk + L.k_w, (L.cout + 127) / 128 * 128, L.k * L.cinp, L.k, shifts, BN, s.params + L.p.bias, L.act, y_b, y_f,
-              ldo, L.cout, s.st);
+  const int sp = s.lo->c.split_bf16;
+  return gemm(x, L.cin, ld_x, 0, s.lo->T, s.lo->B, s.pk + L.k_w, (L.cout + 127) / 128 * 128, L.k * L.cinp * (sp ? 3 : 1), L.k, shifts, BN,
+              s.params + L.p.bias, L.act, y_b, y_f, ldo, L.cout, s.st, nullptr, 0, sp);
 }
 }  // namespace
 
@@ -718,30 +811,43 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   const int T = lo.T, B = lo.B, M = lo.M, HU = lo.HU, RU = lo.RU, KC = lo.KC, PJc = lo.PJc;
   float* scal = W<float>(s, lo.w_scal);
   T2_CHECK_CUDA(cudaMemsetAsync(scal, 0, 16 * sizeof(float), st));
+  // split_bf16: every bf16 operand below is a [hi | lo] row pair, every contraction a split GEMM (set_split_operand), and the
+  // pre-batch-norm activations of the bank and of proj1 are fp32
+  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1, Ms = (M + 63) / 64 * 64;
   bf16* x0 = W<bf16>(s, lo.w_x0);
-  launch_f32_to_bf16(d_mel, x0, N * M, st);
+  if (sp) launch_f32_to_bf16_split(d_mel, x0, N, M, Ms, st);
+  else launch_f32_to_bf16(d_mel, x0, N * M, st);
   // ---- conv bank (each layer writes its 128-column slice) + per-layer batch norm ----
   bf16* Y = W<bf16>(s, lo.w_Y);
+  float* Yf = W<float>(s, lo.w_Y);
   bf16* Xb = W<bf16>(s, lo.w_Xb);
   float* stb = W<float>(s, lo.w_stb);
   if (training) T2_CHECK_CUDA(cudaMemsetAsync(stb, 0, 2LL * KC * sizeof(float), st));
   for (int k = 1; k <= lo.K; ++k) {
     const CConv& L = lo.bank[k - 1];
     const int c0 = (k - 1) * lo.CC;
-    rc = conv_fwd(s, L, x0, M, Y + c0, nullptr, KC);
+    rc = conv_fwd(s, L, x0, M, sp ? nullptr : Y + c0, sp ? Yf + c0 : nullptr, KC);
     if (rc) return rc;
-    bn_fwd(Y, KC, c0, Xb, 0, nullptr, nullptr, stb, KC, d_params + L.p.gamma, d_params + L.p.beta, d_params + L.p.mm, d_params + L.p.mv, N, lo.CC,
-           training, BnDropout{}, 128, st);
+    if (sp)
+      bn_fwd(Yf, KC, c0, Xb, 1, nullptr, nullptr, stb, KC, d_params + L.p.gamma, d_params + L.p.beta, d_params + L.p.mm, d_params + L.p.mv, N, lo.CC,
+             training, BnDropout{}, 128, st);
+    else
+      bn_fwd(Y, KC, c0, Xb, 0, nullptr, nullptr, stb, KC, d_params + L.p.gamma, d_params + L.p.beta, d_params + L.p.mm, d_params + L.p.mv, N, lo.CC,
+             training, BnDropout{}, 128, st);
   }
   bf16* P = W<bf16>(s, lo.w_P);
-  maxpool_fwd(Xb, P, N, T, KC, st);
+  maxpool_fwd(Xb, P, N, T, KC, sp, st);
   // ---- projections ----
-  bf16* Y1 = W<bf16>(s, lo.w_Y1); bf16* X1 = W<bf16>(s, lo.w_X1); float* st1 = W<float>(s, lo.w_st1);
-  rc = conv_fwd(s, lo.proj1, P, KC, Y1, nullptr, PJc);
+  bf16* Y1 = W<bf16>(s, lo.w_Y1); float* Y1f = W<float>(s, lo.w_Y1); bf16* X1 = W<bf16>(s, lo.w_X1); float* st1 = W<float>(s, lo.w_st1);
+  rc = conv_fwd(s, lo.proj1, P, KC, sp ? nullptr : Y1, sp ? Y1f : nullptr, PJc);
   if (rc) return rc;
   if (training) T2_CHECK_CUDA(cudaMemsetAsync(st1, 0, 2LL * PJc * sizeof(float), st));
-  bn_fwd(Y1, PJc, 0, X1, 0, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p.gamma, d_params + lo.proj1.p.beta, d_params + lo.proj1.p.mm,
-         d_params + lo.proj1.p.mv, N, PJc, training, BnDropout{}, 256, st);
+  if (sp)
+    bn_fwd(Y1f, PJc, 0, X1, 1, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p.gamma, d_params + lo.proj1.p.beta, d_params + lo.proj1.p.mm,
+           d_params + lo.proj1.p.mv, N, PJc, training, BnDropout{}, 256, st);
+  else
+    bn_fwd(Y1, PJc, 0, X1, 0, nullptr, nullptr, st1, PJc, d_params + lo.proj1.p.gamma, d_params + lo.proj1.p.beta, d_params + lo.proj1.p.mm,
+           d_params + lo.proj1.p.mv, N, PJc, training, BnDropout{}, 256, st);
   float* Y2 = W<float>(s, lo.w_Y2); float* st2 = W<float>(s, lo.w_st2);
   rc = conv_fwd(s, lo.proj2, X1, PJc, nullptr, Y2, M);
   if (rc) return rc;
@@ -751,21 +857,24 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   bf16* hin = W<bf16>(s, lo.w_hin);
   bn_fwd(Y2, M, 0, nullptr, 0, hin_f, d_mel, st2, M, d_params + lo.proj2.p.gamma, d_params + lo.proj2.p.beta, d_params + lo.proj2.p.mm,
          d_params + lo.proj2.p.mv, N, M, training, BnDropout{}, 128, st);
-  launch_f32_to_bf16(hin_f, hin, N * M, st);
+  if (sp) launch_f32_to_bf16_split(hin_f, hin, N, M, Ms, st);
+  else launch_f32_to_bf16(hin_f, hin, N * M, st);
   // ---- dense to the highway width, highway layers ----
-  rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]), HU, HU, st);
+  rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, sp ? 3 * Ms : 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]),
+            HU, HU, st, nullptr, 0, sp);
   if (rc) return rc;
   float* pre = W<float>(s, lo.w_XP);       // [N][2HU] scratch (the GRU input projections overwrite it afterwards)
   for (int i = 0; i < lo.NH; ++i) {
-    rc = gemm(W<bf16>(s, lo.w_hb[i]), HU, HU, 0, T, B, s.pk + lo.k_hw[i], 2 * HU, HU, 1, nullptr, 256, nullptr, 0, nullptr, pre, 2 * HU, 2 * HU, st);
+    rc = gemm(W<bf16>(s, lo.w_hb[i]), HU, HU, 0, T, B, s.pk + lo.k_hw[i], 2 * HU, HU * k3, 1, nullptr, 256, nullptr, 0, nullptr, pre, 2 * HU, 2 * HU, st,
+              nullptr, 0, sp);
     if (rc) return rc;
     highway_fwd(pre, d_params + lo.p_hb[i][0], d_params + lo.p_hb[i][1], W<float>(s, lo.w_hf[i]), W<float>(s, lo.w_hf[i + 1]), W<bf16>(s, lo.w_hb[i + 1]),
-                training ? W<bf16>(s, lo.w_HT[i]) : nullptr, N, HU, st);
+                (training && !sp) ? W<bf16>(s, lo.w_HT[i]) : nullptr, N, HU, sp, st);
   }
   // ---- bidirectional GRU ----
   const int XPW = 6 * RU;
   float* XP = W<float>(s, lo.w_XP);
-  rc = gemm(W<bf16>(s, lo.w_hb[lo.NH]), HU, HU, 0, T, B, s.pk + lo.k_gx, XPW, HU, 1, nullptr, 256, nullptr, 0, nullptr, XP, XPW, XPW, st);
+  rc = gemm(W<bf16>(s, lo.w_hb[lo.NH]), HU, HU, 0, T, B, s.pk + lo.k_gx, XPW, HU * k3, 1, nullptr, 256, nullptr, 0, nullptr, XP, XPW, XPW, st, nullptr, 0, sp);
   if (rc) return rc;
   {
     GruArgs a;
@@ -773,15 +882,16 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
     a.params = d_params;
     for (int d = 0; d < 2; ++d) {
       a.p_gk[d] = lo.p_gk[d]; a.p_ck[d] = lo.p_ck[d]; a.p_gb[d] = lo.p_gb[d]; a.p_cb[d] = lo.p_cb[d];
-      if (training) { a.r[d] = W<bf16>(s, lo.w_gr[d]); a.u[d] = W<bf16>(s, lo.w_gu[d]); a.c[d] = W<bf16>(s, lo.w_gc[d]); a.rh[d] = W<bf16>(s, lo.w_grh[d]); }
+      if (training && !sp) { a.r[d] = W<bf16>(s, lo.w_gr[d]); a.u[d] = W<bf16>(s, lo.w_gu[d]); a.c[d] = W<bf16>(s, lo.w_gc[d]); a.rh[d] = W<bf16>(s, lo.w_grh[d]); }
     }
     a.XP = XP; a.out = W<bf16>(s, lo.w_out); a.B = B; a.T = T; a.HU = HU; a.RU = RU;
-    rc = launch_gru_fwd(a, st);
+    rc = launch_gru_fwd(a, sp, st);
     if (rc) return rc;
   }
   // ---- linear projection, clip, loss ----
   float* lin = W<float>(s, lo.w_lin);
-  rc = gemm(W<bf16>(s, lo.w_out), 2 * RU, 2 * RU, 0, T, B, s.pk + lo.k_lin, lo.NFR, 2 * RU, 1, nullptr, 128, d_params + lo.p_lb, 0, nullptr, lin, lo.NFP, lo.NF, st);
+  rc = gemm(W<bf16>(s, lo.w_out), 2 * RU, 2 * RU, 0, T, B, s.pk + lo.k_lin, lo.NFR, 2 * RU * k3, 1, nullptr, 128, d_params + lo.p_lb, 0, nullptr, lin, lo.NFP,
+            lo.NF, st, nullptr, 0, sp);
   if (rc) return rc;
   const int* tlen = lo.c.mask_decoder ? W<int>(s, lo.w_tlen) : nullptr;
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
@@ -801,6 +911,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   CL lo;
   int rc = build(cfg, lo, nullptr);
   if (rc) return rc;
+  T2_REQUIRE(!lo.c.split_bf16, T2_ERR_INVALID_ARG, "split_bf16 (fp32-class) CBHG mode has no backward pass");
   T2_REQUIRE(d_params && d_packed && d_workspace && d_mel && d_grads && d_mel_grad, T2_ERR_INVALID_ARG, "cbhg_backward: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   Ctx s{&lo, static_cast<uint8_t*>(d_workspace), static_cast<const uint8_t*>(d_packed), const_cast<float*>(d_params), st, 1};
@@ -931,11 +1042,14 @@ extern "C" int t2_cbhg_workspace_tensor(const t2_cbhg_config_t* cfg, void* d_wor
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   const std::string n(name);
   long long off = -1, cnt = 0;
+  // split_bf16 doubles the rows of the bf16 tensors below to [hi | lo] (include/t2b200.h); highway_input pads M to a multiple of 64 per half
+  const long long xm = lo.c.split_bf16 ? 2 : 1, mw = lo.c.split_bf16 ? 2LL * ((lo.M + 63) / 64 * 64) : lo.M;
   if (n == "linear_outputs") { off = lo.w_lin; cnt = lo.N * lo.NFP; }           // fp32 [B][T][num_freq rounded up to 8] (row pitch!)
-  else if (n == "rnn_outputs") { off = lo.w_out; cnt = lo.N * 2 * lo.RU; }     // bf16 [B][T][2 RU]
-  else if (n == "highway_input") { off = lo.w_hin; cnt = lo.N * lo.M; }        // bf16 [B][T][M]
-  else if (n == "bank_outputs") { off = lo.w_Xb; cnt = lo.N * lo.KC; }         // bf16 [B][T][K CC] (after batch norm)
-  else if (n == "gru_input") { off = lo.w_hb[lo.NH]; cnt = lo.N * lo.HU; }     // bf16 [B][T][HU]: the last highway output
+  else if (n == "rnn_outputs") { off = lo.w_out; cnt = lo.N * 2 * lo.RU * xm; } // bf16 [B][T][2 RU]
+  else if (n == "highway_input") { off = lo.w_hin; cnt = lo.N * mw; }          // bf16 [B][T][M]
+  else if (n == "bank_outputs") { off = lo.w_Xb; cnt = lo.N * lo.KC * xm; }    // bf16 [B][T][K CC] (after batch norm)
+  else if (n == "pooled_outputs") { off = lo.w_P; cnt = lo.N * lo.KC * xm; }   // bf16 [B][T][K CC] (after the max-pool)
+  else if (n == "gru_input") { off = lo.w_hb[lo.NH]; cnt = lo.N * lo.HU * xm; } // bf16 [B][T][HU]: the last highway output
   // fp32 [B][T][6 RU] input projections [fw gates | fw cand | bw gates | bw cand] (no biases); valid between the forward and the
   // backward pass only: the highway backward reuses the buffer
   else if (n == "gru_xp") { off = lo.w_XP; cnt = lo.N * 6 * lo.RU; }
@@ -972,12 +1086,13 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_REQUIRE(rows >= 1 && C >= 1 && c0 >= 0 && c0 + C <= ld && c0 + C <= Ct && (thr == 128 || thr == 256) && p[0] && (p[1] || p[2]) && p[4] &&
                      p[5] && p[6] && p[7] && p[8],
                  T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_FWD: bad arguments");
+      T2_REQUIRE(i[8] == 0 || i[8] == 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel BN_FWD: split i[8] = %lld is not 0 or 1", i[8]);
       if (i[6])
-        bn_fwd(static_cast<const float*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), 0, static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+        bn_fwd(static_cast<const float*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), int(i[8]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
                static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
                static_cast<float*>(p[8]), rows, C, int(i[5]), BnDropout{}, thr, st);
       else
-        bn_fwd(static_cast<const bf16*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), 0, static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
+        bn_fwd(static_cast<const bf16*>(p[0]), ld, c0, static_cast<bf16*>(p[1]), int(i[8]), static_cast<float*>(p[2]), static_cast<const float*>(p[3]),
                static_cast<float*>(p[4]), Ct, static_cast<const float*>(p[5]), static_cast<const float*>(p[6]), static_cast<float*>(p[7]),
                static_cast<float*>(p[8]), rows, C, int(i[5]), BnDropout{}, thr, st);
       break;
@@ -1003,14 +1118,16 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
       const bool fwd = call->kernel == T2_DBG_CBHG_POOL_FWD;
       T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && i[0] % i[1] == 0 && i[2] >= 1 && p[0] && p[1] && (fwd || p[2]), T2_ERR_INVALID_ARG,
                  "dbg_cbhg_kernel POOL: bad arguments");
-      if (fwd) maxpool_fwd(static_cast<const bf16*>(p[0]), static_cast<bf16*>(p[1]), i[0], int(i[1]), int(i[2]), st);
+      T2_REQUIRE(!fwd || i[3] == 0 || i[3] == 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel POOL_FWD: split i[3] = %lld is not 0 or 1", i[3]);
+      if (fwd) maxpool_fwd(static_cast<const bf16*>(p[0]), static_cast<bf16*>(p[1]), i[0], int(i[1]), int(i[2]), int(i[3]), st);
       else maxpool_bwd(static_cast<const bf16*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<bf16*>(p[2]), i[0], int(i[1]), int(i[2]), st);
       break;
     }
     case T2_DBG_CBHG_HIGHWAY_FWD:
       T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && p[0] && p[1] && p[2] && p[3] && p[4] && p[5], T2_ERR_INVALID_ARG, "dbg_cbhg_kernel HIGHWAY_FWD: bad arguments");
+      T2_REQUIRE(i[2] == 0 || i[2] == 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel HIGHWAY_FWD: split i[2] = %lld is not 0 or 1", i[2]);
       highway_fwd(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]), static_cast<const float*>(p[3]),
-                  static_cast<float*>(p[4]), static_cast<bf16*>(p[5]), static_cast<bf16*>(p[6]), i[0], int(i[1]), st);
+                  static_cast<float*>(p[4]), static_cast<bf16*>(p[5]), static_cast<bf16*>(p[6]), i[0], int(i[1]), int(i[2]), st);
       break;
     case T2_DBG_CBHG_HIGHWAY_BWD:
       T2_REQUIRE(i[0] >= 1 && i[1] >= 1 && p[0] && p[1] && p[2] && p[3] && p[4], T2_ERR_INVALID_ARG, "dbg_cbhg_kernel HIGHWAY_BWD: bad arguments");
@@ -1029,9 +1146,10 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
       for (int k = 0; k < 4; ++k)   // B, T, HU, RU: in int range before the narrowing below
         T2_REQUIRE(i[k] >= 1 && i[k] <= (1 << 20), T2_ERR_UNSUPPORTED_SHAPE, "dbg_cbhg_kernel GRU_FWD: B, T, HU, RU must be in [1, 2^20] (i[%d] = %lld)", k, i[k]);
       a.B = int(i[0]); a.T = int(i[1]); a.HU = int(i[2]); a.RU = int(i[3]);
-      int rc = check_gru_fwd(a);
+      T2_REQUIRE(i[12] == 0 || i[12] == 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel GRU_FWD: split i[12] = %lld is not 0 or 1", i[12]);
+      int rc = check_gru_fwd(a, int(i[12]));
       if (!rc) rc = gru_setup();
-      return rc ? rc : launch_gru_fwd(a, st);
+      return rc ? rc : launch_gru_fwd(a, int(i[12]), st);
     }
     case T2_DBG_CBHG_GRU_BWD: {
       GruBwdArgs a;

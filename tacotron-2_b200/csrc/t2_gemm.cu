@@ -214,6 +214,19 @@ long long* take_timing_slice(long long n_slots) {
   return p;
 }
 
+int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts) {
+  const int nkb = (C + kBK - 1) / kBK, Cp = nkb * kBK;
+  T2_REQUIRE(2 * ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "split-bf16 GEMM: %d taps are more than %d segments", ntaps, kMaxSeg);
+  c.a[0] = make_act(a, 2 * Cp, T, B, 1, 2 * Cp); c.na = 1;
+  c.nseg = 0;
+  for (int s = 0; s < ntaps; ++s) {
+    c.seg[c.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, 2 * nkb, 0, 1};
+    c.seg[c.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};
+  }
+  c.epi.i[11] = 1;
+  return T2_OK;
+}
+
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used) {
   GemmArgs g;
   dim3 grid;

@@ -50,6 +50,10 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
+// split-bf16 ("fp32-class") operand A of an EPI_BIAS_ACT call: rows [hi | lo], each half C channels zero-padded to
+// Cp = ceil(C / kBK) * kBK (row pitch 2 Cp). Per tap one segment over both halves against [W_hi | W_hi] and one over the hi half
+// against [W_lo], so the packed weights hold 3 Cp K columns per tap (add_pack_split); a bf16 output is written as [hi(ldo) | lo(ldo)].
+int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts);
 // *cluster_used (nullable) receives the cluster size the kernel was launched with
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used = nullptr);
 // the checked kernel arguments (tensor maps encoded), grid and cluster size launch_act_gemm launches `c` with

@@ -143,9 +143,21 @@ __global__ void reg_grad_kernel(const float* __restrict__ params, float* __restr
     grads[off + i] += w * params[off + i];
 }
 
-__global__ void f32_to_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n) {
+// kSplit: n = rows * Cp elements of the split-bf16 operand rows [hi(Cp) | lo(Cp)] from fp32 [rows][C]; channels C..Cp-1 are zero
+template <bool kSplit>
+__global__ void f32_to_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, long long n, int C, int Cp) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < n) out[e] = __float2bfloat16(in[e]);
+  if (!kSplit) {
+    if (e < n) out[e] = __float2bfloat16(in[e]);
+    return;
+  }
+  if (e >= n) return;
+  const long long r = e / Cp;
+  const int c = int(e % Cp);
+  const float v = c < C ? in[r * C + c] : 0.f;
+  const bf16 hi = __float2bfloat16(v);
+  bf16* row = out + r * 2 * Cp + c;
+  row[0] = hi; row[Cp] = __float2bfloat16(v - __bfloat162float(hi));
 }
 
 }  // namespace
@@ -184,7 +196,12 @@ void launch_reg_grad(const float* params, float* grads, const long long* tab, in
 }
 
 void launch_f32_to_bf16(const float* in, __nv_bfloat16* out, long long n, cudaStream_t st) {
-  f32_to_bf16_kernel<<<grid1d(n), 256, 0, st>>>(in, out, n);
+  f32_to_bf16_kernel<false><<<grid1d(n), 256, 0, st>>>(in, out, n, 0, 0);
+  t2_count_launch();
+}
+
+void launch_f32_to_bf16_split(const float* in, __nv_bfloat16* out, long long rows, int C, int Cp, cudaStream_t st) {
+  f32_to_bf16_kernel<true><<<grid1d(rows * Cp), 256, 0, st>>>(in, out, rows * Cp, C, Cp);
   t2_count_launch();
 }
 

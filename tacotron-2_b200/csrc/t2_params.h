@@ -68,6 +68,8 @@ void launch_reg_loss(const float* params, const long long* tab, int n_reg, float
 void launch_reg_grad(const float* params, float* grads, const long long* tab, int n_reg, float weight, cudaStream_t st);
 
 void launch_f32_to_bf16(const float* in, __nv_bfloat16* out, long long n, cudaStream_t st);
+// fp32 [rows][C] -> split-bf16 operand rows [hi(Cp) | lo(Cp)] (row pitch 2 Cp, Cp >= C; the padding channels are written as zeros)
+void launch_f32_to_bf16_split(const float* in, __nv_bfloat16* out, long long rows, int C, int Cp, cudaStream_t st);
 
 // side stream with fork / join events for work that is independent of the caller's stream (created once per process;
 // T2_SIDE_STREAM=0 in the environment keeps everything on the caller's stream: nullptr)

@@ -722,10 +722,8 @@ __global__ void loss_norm_kernel(float* s, float* out, float n_mel, float n_stop
 }
 
 // generic helper: 1x1 / k-tap conv GEMM through the engine
-// split != 0 ("fp32-class" conv stacks): the input rows are [hi | lo], each half `C` channels zero-padded to Cp = ceil(C / 64) * 64; per
-// tap one segment over both halves against [W_hi | W_hi] and one over the hi half against [W_lo] (wK = 3 * ntaps * Cp); a bf16 output is
-// written as [hi(ldo) | lo(ldo)]. hash_row0: position offset of the dropout mask (a launch over the rows of one decoder step draws
-// the elements of those rows in the batched [T_out * B] launch)
+// split != 0 ("fp32-class" conv stacks): split-bf16 operands (set_split_operand, t2_gemm.h; wK = 3 * ntaps * Cp). hash_row0: position
+// offset of the dropout mask (a launch over the rows of one decoder step draws the elements of those rows in the batched [T_out * B] launch)
 int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, int wK, int ntaps, const int* shifts, int BN, float* bias,
               int act, void* out_bf16, float* out_f32, int ldo, int nvalid, float pdrop, int stream_id, unsigned long long seed,
               const unsigned long long* d_step, cudaStream_t st, int split = 0, int hash_row0 = 0) {
@@ -733,15 +731,8 @@ int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, i
   memset(&g, 0, sizeof(g));
   const int nkb = (C + kBK - 1) / kBK;
   if (split) {
-    const int Cp = nkb * kBK;
-    g.a[0] = make_act(a, 2 * Cp, int(T), Bn, 1, 2 * Cp); g.na = 1;
-    g.nseg = 0;
-    for (int s = 0; s < ntaps; ++s) {
-      g.seg[g.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, 2 * nkb, 0, 1};
-      g.seg[g.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};
-    }
-    T2_REQUIRE(g.nseg <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "split conv_gemm: too many taps");
-    g.epi.i[11] = 1;
+    const int rc = set_split_operand(g, a, C, int(T), Bn, ntaps, shifts);
+    if (rc) return rc;
   } else {
   g.a[0] = make_act(a, C, int(T), Bn, 1, C); g.na = 1;
   for (int s = 0; s < ntaps; ++s) g.seg[s] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};

@@ -24,7 +24,7 @@ class CbhgConfig(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int) for n in (
         "B", "T", "num_mels", "kernels", "conv_channels", "pool_size", "projection", "projection_kernel_size", "highwaynet_layers",
         "highway_units", "rnn_units", "num_freq", "n_priority_freq", "clip_outputs", "mask_decoder")] + [
-        (n, ctypes.c_float) for n in ("max_abs_value", "lower_bound_decay", "reg_weight")]
+        (n, ctypes.c_float) for n in ("max_abs_value", "lower_bound_decay", "reg_weight")] + [("split_bf16", ctypes.c_int)]
 
 
 def _decay_field(hp):
@@ -34,8 +34,11 @@ def _decay_field(hp):
     return hp.lower_bound_decay if hp.symmetric_mels else hp.lower_bound_decay - hp.max_abs_value
 
 
-def make_cbhg_config(hp, B, T, reg_weight):
-    """CBHG post-processing net + linear head (tacotron.py:203-219); the shapes the CUDA path implements are checked by t2_cbhg_sizes"""
+def make_cbhg_config(hp, B, T, reg_weight, precision="bf16"):
+    """CBHG post-processing net + linear head (tacotron.py:203-219); the shapes the CUDA path implements are checked by t2_cbhg_sizes.
+    precision 'fp32-class': split bf16 hi + lo operands, forward only (include/t2b200.h, t2_cbhg_config_t.split_bf16)."""
+    if precision not in ("bf16", "fp32-class"):
+        raise L.T2Error("precision must be 'bf16' or 'fp32-class'")
     c = CbhgConfig()
     c.B, c.T, c.num_mels = B, T, hp.num_mels
     c.kernels, c.conv_channels, c.pool_size = hp.cbhg_kernels, hp.cbhg_conv_channels, hp.cbhg_pool_size
@@ -45,6 +48,7 @@ def make_cbhg_config(hp, B, T, reg_weight):
     c.n_priority_freq = int(2000 / (hp.sample_rate * 0.5) * hp.num_freq)
     c.clip_outputs, c.mask_decoder = int(hp.clip_outputs), int(bool(hp.mask_decoder))
     c.max_abs_value, c.lower_bound_decay, c.reg_weight = hp.max_abs_value, _decay_field(hp), reg_weight
+    c.split_bf16 = int(precision == "fp32-class")
     return c
 
 
@@ -112,8 +116,9 @@ def make_config(hp, B, T_in, T_out, precision="bf16", teacher_forcing_ratio=None
 class Tacotron(object):
     def __init__(self, hparams, B, T_in, T_out, device="cuda", precision="bf16", teacher_forcing_ratio=None):
         """precision 'fp32-class': every contraction of the forward and of synthesize() - convolution stacks, encoder BiLSTM, prenet,
-        decoder LSTMs, attention, frame / stop projection - runs on bf16 hi + lo operand pairs with hi + lo stored activations and
-        fp32 pre-batch-norm activations / cell states; forward / losses / synthesis only (include/t2b200.h, t2_taco_config_t.split_bf16).
+        decoder LSTMs, attention, frame / stop projection, and with predict_linear the CBHG head and linear projection - runs on bf16
+        hi + lo operand pairs with hi + lo stored activations and fp32 pre-batch-norm activations / cell states; forward / losses /
+        synthesis / linear_from_mel only (include/t2b200.h, t2_taco_config_t.split_bf16 and t2_cbhg_config_t.split_bf16).
         teacher_forcing_ratio (default hparams.tacotron_teacher_forcing_ratio): below 1, every decoder step of forward() draws whether
         the next step consumes the target frame or the frame just predicted, and backward() differentiates through the fed-back frames."""
         self.hp = hparams
@@ -128,9 +133,7 @@ class Tacotron(object):
         self.cbhg = None
         n_cb = 0
         if getattr(hparams, "predict_linear", False):       # CBHG + linear head: a second engine chained on mel_outputs (include/t2b200.h)
-            if precision != "bf16":
-                raise L.T2Error("predict_linear has no fp32-class mode")
-            self.cbhg = make_cbhg_config(hparams, B, T_out, self.cfg.reg_weight)
+            self.cbhg = make_cbhg_config(hparams, B, T_out, self.cfg.reg_weight, precision)
             cn, cpb, cwb, cnt = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_int()
             L.check(self.lib.t2_cbhg_sizes(ctypes.byref(self.cbhg), ctypes.byref(cn), ctypes.byref(cpb), ctypes.byref(cwb), ctypes.byref(cnt)))
             n_cb = cn.value
@@ -244,7 +247,7 @@ class Tacotron(object):
         B = (B0 + 3) // 4 * 4                                   # the recurrent kernel takes items in fours; rows are independent here
         x = torch.zeros(B, max(T, 2), self.hp.num_mels, dtype=torch.float32, device=self.device)
         x[:B0, :T] = mel.float()
-        cfg = make_cbhg_config(self.hp, B, max(T, 2), 0.0)
+        cfg = make_cbhg_config(self.hp, B, max(T, 2), 0.0, self.precision)
         cfg.mask_decoder = 0
         pb, wb = ctypes.c_longlong(), ctypes.c_longlong()
         L.check(self.lib.t2_cbhg_sizes(ctypes.byref(cfg), None, ctypes.byref(pb), ctypes.byref(wb), None))
