@@ -187,7 +187,8 @@ int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream);
  * wavenet_vocoder/models/modules.py:184-521,539-654,736-817 and wavenet_vocoder/models/mixture.py:18-74.
  * Field names follow the reference's hparams.py:187-228. */
 typedef struct {
-  int layers, stacks, residual_channels, gate_channels, skip_out_channels, kernel_size;
+  int layers, stacks, residual_channels, gate_channels, skip_out_channels;
+  int kernel_size;           /* taps of the dilated causal convolution: 2, 3 or 4 (tap j reads x(t - (kernel_size-1-j) d)) */
   int cin_channels;          /* 80 (num_mels) or 0 = no local conditioning */
   int out_channels;          /* 256 (mu-law softmax), 3*nr_mix (MoL) or 2 (single Gaussian: mean, log-scale) */
   int quantize_channels;     /* 256 or 65536 */

@@ -6,7 +6,7 @@
 //   parameters   fp32 masters in TensorFlow variable layouts, concatenated (drop-in checkpoint order)
 //   packed       bf16 K-major GEMM operand copies of the masters, refreshed after every optimizer step
 // Per layer the forward is two GEMM launches:
-//   gate : [x(t-2d) | x(t-d) | x(t) | c(t)] (K = 3R + 128) x Wg -> tanh*sigmoid epilogue -> z (+ stashes)
+//   gate : [x(t-(k-1)d) | ... | x(t-d) | x(t) | c(t)] (K = kR + 128, k = kernel_size taps) x Wg -> tanh*sigmoid epilogue -> z (+ stashes)
 //   out  : z (K = G/2) x Wo -> (o + b + x) * sqrt(.5) epilogue -> x_next
 // the skip 1x1 of ALL layers is deferred into one K = L*G/2 GEMM (skips never round-trip through HBM).
 // Global (speaker) conditioning (gin_channels > 0) enters the gate GEMM's epilogue as a per-item bias, not as a GEMM operand.
@@ -43,6 +43,7 @@ struct ColsumJob {
 struct Layout {
   t2_wn_config_t c;
   int L, R, G, Gh, S, C, O, Q, B, T, Tc, Kg, ldo, Op;
+  int kw;       // taps of the dilated causal convolution (kernel_size): tap j reads x(t - (kw-1-j) d)
   bool split;   // split-bf16 forward (t2_wn_config_t.split_bf16)
   int xm;       // channel multiplier of the stored activations: 2 in split mode (hi | lo), else 1
   bool scalar_in, mol, gauss;   // mol: scalar-input head (mixture of logistics, or a single Gaussian when gauss)
@@ -88,10 +89,11 @@ struct Layout {
 // N), then the out tiles (none after the last layer); backward, from the top layer down, the dz tiles then the dx tiles. A ticket
 // waits only for the tiles whose outputs its GEMM reads (its A operand through the dilated taps, and its epilogue inputs), all of
 // them earlier in the order and inside its batch item (the taps' rows before 0 / past T are zero-filled, not read):
-//   gate(l, m) <- out(l-1, m-k..m)   rows [t0 - 2d, t0 + 128) of xd_l, k = ceil(2d / 128)   (out(l-1, m) also wrote x_l for out(l, m))
+//   gate(l, m) <- out(l-1, m-k..m)   rows [t0 - (kw-1)d, t0 + 128) of xd_l, k = ceil((kw-1)d / 128)   (out(l-1, m) also wrote x_l
+//                                     for out(l, m))
 //   out(l, m)  <- gate(l, m, every n)   z_l rows [t0, t0 + 128)
 //   dz(l, m)   <- dx(l+1, m)         dxin_{l+1} rows [t0, t0 + 128)   (and the dx epilogue's residual input of the same rows)
-//   dx(l, m)   <- dz(l, m..m+k, every n)   dg_l rows [t0, t0 + 128 + 2d)
+//   dx(l, m)   <- dz(l, m..m+k, every n)   dg_l rows [t0, t0 + 128 + (kw-1)d)
 // Every buffer a chain writes is per layer and read only by later tickets, so no ticket overwrites what an earlier one still reads.
 // dir 0: forward, 1: backward.
 void build_chain(const Layout& lo, int dir, std::vector<ChainTicket>& v) {
@@ -103,7 +105,7 @@ void build_chain(const Layout& lo, int dir, std::vector<ChainTicket>& v) {
   v.reserve(lo.n_chain[dir]);
   if (dir == 0) {
     for (int l = 0; l < lo.L; ++l) {
-      const int k = (2 * lo.dil(l) + kBM - 1) / kBM;
+      const int k = ((lo.kw - 1) * lo.dil(l) + kBM - 1) / kBM;
       for (int n = 0; n < ng; ++n)
         for (int m = 0; m < lo.MT; ++m) {
           const int m0 = m / tpb * tpb;                            // first M tile of this batch item
@@ -117,7 +119,7 @@ void build_chain(const Layout& lo, int dir, std::vector<ChainTicket>& v) {
     return;
   }
   for (int l = lo.L - 1; l >= 0; --l) {
-    const int k = (2 * lo.dil(l) + kBM - 1) / kBM;
+    const int k = ((lo.kw - 1) * lo.dil(l) + kBM - 1) / kBM;
     for (int n = 0; n < nz; ++n)
       for (int m = 0; m < lo.MT; ++m) {
         ChainTicket t{0, l, m, n, 0, -1, 0, idx(0, l, m)};
@@ -143,7 +145,9 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.scalar_in = cfg->input_type != 2;
   lo.mol = lo.scalar_in;
   T2_REQUIRE(lo.L >= 1 && cfg->stacks >= 1 && lo.L % cfg->stacks == 0, T2_ERR_INVALID_ARG, "layers %% stacks != 0");
-  T2_REQUIRE(cfg->kernel_size == 3, T2_ERR_UNSUPPORTED_SHAPE, "kernel_size must be 3");
+  T2_REQUIRE(cfg->kernel_size >= 2 && cfg->kernel_size <= 4, T2_ERR_UNSUPPORTED_SHAPE, "kernel_size must be 2, 3 or 4 (got %d)",
+             cfg->kernel_size);
+  lo.kw = cfg->kernel_size;
   T2_REQUIRE(lo.R == 128 || lo.R == 256, T2_ERR_UNSUPPORTED_SHAPE, "residual_channels must be 128 or 256 (got %d)", lo.R);
   T2_REQUIRE(lo.S == 128 || lo.S == 256, T2_ERR_UNSUPPORTED_SHAPE, "skip_out_channels must be 128 or 256 (got %d)", lo.S);
   T2_REQUIRE(lo.Gh == 128 || lo.Gh == 256, T2_ERR_UNSUPPORTED_SHAPE, "gate_channels must be 256 or 512 (got %d)", lo.G);
@@ -165,7 +169,7 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
              "upsample_activation must be 0 (ReLU), 1 (LeakyReLU) or 2 (none), got %d", cfg->upsample_activation);
   T2_REQUIRE(cfg->leaky_alpha >= 0.f && cfg->leaky_alpha <= 1.f, T2_ERR_INVALID_ARG, "leaky_alpha must be in [0, 1], got %g",
              double(cfg->leaky_alpha));
-  lo.Kg = 3 * lo.R + (lo.C > 0 ? 128 : 0);
+  lo.Kg = lo.kw * lo.R + (lo.C > 0 ? 128 : 0);
   lo.ldo = lo.mol ? 64 : 512;   // row pitch of dlog (bf16): MoL 32 values (+pad so a 64-wide TMA box fits); CE hi|lo pair
   lo.Op = lo.mol ? 64 : 512;    // K of Wf2T (CE: [Wf2^T | Wf2^T] against the hi|lo split of dlog)
   lo.res_scale = cfg->residual_legacy ? float(sqrt(0.5)) : 1.f;
@@ -196,7 +200,7 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     char p[64];
     snprintf(p, sizeof(p), "ResidualConv1DGLU_%d/", l);
     std::string s(p);
-    lo.p_dil_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_causal_conv/kernel", {3, lo.R, lo.G}));
+    lo.p_dil_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_causal_conv/kernel", {lo.kw, lo.R, lo.G}));
     lo.p_dil_b.push_back(add_param(lo.params, lo.n_params, s + "residual_block_causal_conv/bias", {lo.G}));
     if (lo.C > 0) {
       lo.p_c_k.push_back(add_param(lo.params, lo.n_params, s + "residual_block_cin_conv/kernel", {1, lo.C, lo.G}));
@@ -243,7 +247,7 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.k_Wf1 = pk.take((long long)lo.S * lo.S * km * 2);
   lo.k_Wf2 = pk.take((long long)(lo.O < 32 ? 32 : lo.O) * lo.S * km * 2);
   lo.k_WozT = pk.take(L * lo.Gh * (lo.R + lo.S) * 2);
-  lo.k_WdT = pk.take(L * lo.R * 3 * lo.G * 2);
+  lo.k_WdT = pk.take(L * lo.R * lo.kw * lo.G * 2);
   lo.k_WcT = pk.take((long long)(lo.C > 0 ? lo.C : 8) * L * lo.G * 2);
   lo.k_Wf1T = pk.take((long long)lo.S * lo.S * 2);
   lo.k_Wf2T = pk.take((long long)lo.S * lo.Op * 2);
@@ -282,22 +286,24 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     const long long wg = lo.k_Wg + (long long)l * lo.G * lo.Kg * km * 2;
     if (lo.split) {
       const int R = lo.R, Gh = lo.Gh;
-      for (int j = 0; j < 3; ++j) add_pack_split(pj, lo.p_dil_k[l] + (long long)j * R * lo.G, R, lo.G, wg, 3 * lo.Kg, j * 3 * R, j * 3 * R + 2 * R, R, 1.f, Gh);
-      if (lo.C > 0) add_pack_split(pj, lo.p_c_k[l], lo.C, lo.G, wg, 3 * lo.Kg, 9 * R, 9 * R + 256, 128, 1.f, Gh);
+      for (int j = 0; j < lo.kw; ++j)
+        add_pack_split(pj, lo.p_dil_k[l] + (long long)j * R * lo.G, R, lo.G, wg, 3 * lo.Kg, j * 3 * R, j * 3 * R + 2 * R, R, 1.f, Gh);
+      const int kc = 3 * lo.kw * R;   // the conditioning segment follows the kw tap segments of 3R each
+      if (lo.C > 0) add_pack_split(pj, lo.p_c_k[l], lo.C, lo.G, wg, 3 * lo.Kg, kc, kc + 256, 128, 1.f, Gh);
       add_pack_split(pj, lo.p_o_k[l], Gh, R, lo.k_Wo + (long long)l * R * Gh * 3 * 2, 3 * Gh, 0, 2 * Gh, Gh);
       // skip GEMM: K runs over [all layers: hi | hi] then [all layers: lo]
       add_pack_split(pj, lo.p_s_k[l], Gh, lo.S, lo.k_Ws, 3 * lo.L * Gh, l * 2 * Gh, 2 * lo.L * Gh + l * Gh, Gh, lo.skip_scale[l]);
     } else {
-    for (int j = 0; j < 3; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, 1, j * lo.R, 1.f, lo.Gh);
-    if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, 1, 3 * lo.R, 1.f, lo.Gh);
+    for (int j = 0; j < lo.kw; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, 1, j * lo.R, 1.f, lo.Gh);
+    if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, 1, lo.kw * lo.R, 1.f, lo.Gh);
     add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, lo.k_Wo + (long long)l * lo.R * lo.Gh * 2, lo.Gh, 1, 0);
     add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, lo.k_Ws, lo.L * lo.Gh, 1, l * lo.Gh, lo.skip_scale[l]);
     }
     const long long woz = lo.k_WozT + (long long)l * lo.Gh * (lo.R + lo.S) * 2;
     add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, woz, lo.R + lo.S, 0, 0, lo.res_scale);
     add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, woz, lo.R + lo.S, 0, lo.R, lo.skip_scale[l]);
-    const long long wd = lo.k_WdT + (long long)l * lo.R * 3 * lo.G * 2;
-    for (int j = 0; j < 3; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wd, 3 * lo.G, 0, j * lo.G);
+    const long long wd = lo.k_WdT + (long long)l * lo.R * lo.kw * lo.G * 2;
+    for (int j = 0; j < lo.kw; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wd, lo.kw * lo.G, 0, j * lo.G);
     if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, lo.k_WcT, lo.L * lo.G, 0, l * lo.G);
   }
   if (lo.split) {
@@ -324,8 +330,8 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   for (int l = 0; l < lo.L; ++l) {
     const int d = lo.dil(l);
     lo.tile_start[l] = int(lo.tiles_main.size());
-    for (int j = 0; j < 3; ++j)
-      append_wgrad_tiles(lo.tiles_main, proto(0, -(2 - j) * d, l, 1, l, 1.f), 0, lo.R, 0, lo.G, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.G);
+    for (int j = 0; j < lo.kw; ++j)
+      append_wgrad_tiles(lo.tiles_main, proto(0, -(lo.kw - 1 - j) * d, l, 1, l, 1.f), 0, lo.R, 0, lo.G, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.G);
     if (lo.C > 0) append_wgrad_tiles(lo.tiles_main, proto(2, 0, 0, 1, l, 1.f), 0, lo.C, 0, lo.G, lo.p_c_k[l], lo.G);
     for (int m0 = 0; m0 < lo.Gh; m0 += 128) {   // out and skip tiles of one row block side by side
       if (l < lo.L - 1)
@@ -1025,7 +1031,7 @@ __global__ void fx_finalize_kernel(const long long* __restrict__ acc, float* __r
   if (e < n && acc[e] != 0) grads[e] += fx_value(acc[e]);
 }
 
-// the per-layer gate GEMM: [x(t-2d) | x(t-d) | x(t) | c(t)] x Wg with the tanh*sigmoid epilogue
+// the per-layer gate GEMM: [x(t-(kw-1)d) | ... | x(t-d) | x(t) | c(t)] x Wg with the tanh*sigmoid epilogue
 ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l, bool save) {
   const long long BT = (long long)lo.B * lo.T;
   const int d = lo.dil(l);
@@ -1036,11 +1042,11 @@ ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int
     g.a[0] = make_act(ws + lo.w_xd, 2 * lo.R, lo.T, lo.B, lo.L);
     g.a[1] = make_act(ws + lo.w_cup, 256, lo.T, lo.B, 1);
     g.na = lo.C > 0 ? 2 : 1;
-    const int shifts[3] = {-2 * d, -d, 0};
     g.nseg = 0;
-    for (int j = 0; j < 3; ++j) {
-      g.seg[g.nseg++] = Seg{0, shifts[j], 0, 2 * lo.R / kBK, l, 1};
-      g.seg[g.nseg++] = Seg{0, shifts[j], 0, lo.R / kBK, l, 1};
+    for (int j = 0; j < lo.kw; ++j) {
+      const int shift = -(lo.kw - 1 - j) * d;
+      g.seg[g.nseg++] = Seg{0, shift, 0, 2 * lo.R / kBK, l, 1};
+      g.seg[g.nseg++] = Seg{0, shift, 0, lo.R / kBK, l, 1};
     }
     if (lo.C > 0) { g.seg[g.nseg++] = Seg{1, 0, 0, 4, 0, 1}; g.seg[g.nseg++] = Seg{1, 0, 0, 2, 0, 1}; }
     g.w = pk + lo.k_Wg; g.wN = lo.G; g.wK = 3 * lo.Kg; g.wL = lo.L; g.w_layer = l; g.w_k0 = 0;
@@ -1048,11 +1054,9 @@ ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int
   g.a[0] = make_act(ws + lo.w_xd, lo.R, lo.T, lo.B, lo.L);
   g.a[1] = make_act(ws + lo.w_cup, lo.C > 0 ? lo.C : 8, lo.T, lo.B, 1);
   g.na = lo.C > 0 ? 2 : 1;
-  g.seg[0] = Seg{0, -2 * d, 0, lo.R / kBK, l, 1};
-  g.seg[1] = Seg{0, -d, 0, lo.R / kBK, l, 1};
-  g.seg[2] = Seg{0, 0, 0, lo.R / kBK, l, 1};
-  g.nseg = 3;
-  if (lo.C > 0) { g.seg[3] = Seg{1, 0, 0, 2, 0, 1}; g.nseg = 4; }
+  for (int j = 0; j < lo.kw; ++j) g.seg[j] = Seg{0, -(lo.kw - 1 - j) * d, 0, lo.R / kBK, l, 1};
+  g.nseg = lo.kw;
+  if (lo.C > 0) g.seg[g.nseg++] = Seg{1, 0, 0, 2, 0, 1};
   g.w = pk + lo.k_Wg; g.wN = lo.G; g.wK = lo.Kg; g.wL = lo.L; g.w_layer = l; g.w_k0 = 0;
   }
   g.T = lo.T; g.B = lo.B; g.n_tiles = lo.G / 256;
@@ -1135,9 +1139,9 @@ ActGemmCall make_dx_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int l
   ActGemmCall g;
   memset(&g, 0, sizeof(g));
   g.a[0] = make_act(ws + lo.w_dg, lo.G, lo.T, lo.B, lo.L); g.na = 1;
-  for (int j = 0; j < 3; ++j) g.seg[j] = Seg{0, (2 - j) * d, 0, lo.G / kBK, l, 1};
-  g.nseg = 3;
-  g.w = pk + lo.k_WdT; g.wN = lo.R; g.wK = 3 * lo.G; g.wL = lo.L; g.w_layer = l;
+  for (int j = 0; j < lo.kw; ++j) g.seg[j] = Seg{0, (lo.kw - 1 - j) * d, 0, lo.G / kBK, l, 1};
+  g.nseg = lo.kw;
+  g.w = pk + lo.k_WdT; g.wN = lo.R; g.wK = lo.kw * lo.G; g.wL = lo.L; g.w_layer = l;
   g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
   g.epi.ptr[0] = top ? nullptr : dxin + (long long)(l + 1) * BT * lo.R;
   g.epi.ptr[1] = dxin + (long long)l * BT * lo.R;
@@ -2119,7 +2123,7 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
   T2_REQUIRE(CS == 1 || CS == 2 || CS == 4 || CS == 8 || CS == 16, T2_ERR_INVALID_ARG, "cluster size must be 1,2,4,8,16");
   a.CS = CS;
   a.ZC = lo.Gh / CS; a.RC = lo.R / CS; a.SC = lo.S / CS; a.FC = lo.S / CS; a.OC = (lo.O + CS - 1) / CS;
-  a.K1 = 3 * lo.R + lo.C;
+  a.K1 = lo.kw * lo.R + lo.C;
   a.per_rank_layer = 2LL * a.ZC * a.K1 + (long long)(a.RC + a.SC) * lo.Gh;
   a.o_head1 = a.per_rank_layer * CS * lo.L;
   a.o_head2 = a.o_head1 + (long long)CS * a.FC * lo.S;
@@ -2130,7 +2134,7 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
   a.ring_slots.clear(); a.ring_off.clear();
   long long off = 0;
   for (int l = 0; l < lo.L; ++l) {
-    int need = 2 * lo.dil(l) + 1, s = 1;
+    int need = (lo.kw - 1) * lo.dil(l) + 1, s = 1;   // x(t - (kw-1)d) .. x(t)
     while (s < need) s <<= 1;
     a.ring_slots.push_back(s);
     a.ring_off.push_back(int(off));
@@ -2170,8 +2174,9 @@ __global__ void ar_pack_kernel(ArPackArgs a) {
       if (i < 2LL * a.ZC * a.K1) {
         const int row = int(i / a.K1), k = int(i % a.K1);
         const int ch = (row < a.ZC) ? r * a.ZC + row : a.Gh + r * a.ZC + (row - a.ZC);
-        if (k < 3 * a.R) v = a.params[o[0] + (long long)(k / a.R) * a.R * a.G + (long long)(k % a.R) * a.G + ch];
-        else v = a.params[o[2] + (long long)(k - 3 * a.R) * a.G + ch];
+        const int kR = a.K1 - a.C;   // kernel_size taps of R
+        if (k < kR) v = a.params[o[0] + (long long)(k / a.R) * a.R * a.G + (long long)(k % a.R) * a.G + ch];
+        else v = a.params[o[2] + (long long)(k - kR) * a.G + ch];
       } else {
         i -= 2LL * a.ZC * a.K1;
         const int row = int(i / a.Gh), k = int(i % a.Gh);
@@ -2281,7 +2286,8 @@ __device__ __forceinline__ void ar_matvec(const bf16* __restrict__ W, int nout, 
   }
 }
 
-template <int NI>
+// NT: past taps of the dilated convolution (kernel_size - 1), read from the ring; the last tap is the current x
+template <int NI, int NT>
 __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = int(cluster.block_rank());
@@ -2293,7 +2299,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   extern __shared__ __align__(16) float sm[];
   const int ld1 = (a.K1 + 3) & ~3;
   const int nbs = 2 * a.ZC + a.RC;                  // bias slice per layer: a rows | b rows | residual-out rows
-  float* in1 = sm;                                  // [NI][ld1]  : x(t-2d) | x(t-d) | x(t) | c(t)
+  float* in1 = sm;                                  // [NI][ld1]  : x(t-NT*d) | ... | x(t-d) | x(t) | c(t)
   float* zbuf = in1 + NI * ld1;                     // [NI][Gh]   : full z vector (pulled from the cluster)
   float* xbuf = zbuf + NI * a.Gh;                   // [NI][R]    : current layer input (full vector)
   float* zsl = xbuf + NI * a.R;                     // [NI][ZC]   : this CTA's z slice, read remotely by the cluster
@@ -2338,7 +2344,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   uint32_t wphase = 0;            // bit s = parity to wait for on slot s
   long long seq = 0;              // (t, l) sequence number: slot = seq & 1
   // ring taps of the NEXT layer are fetched into registers one layer ahead (their producers ran >= one time step ago)
-  constexpr int kTapRegs = (NI * 2 * 512 + kArThreads - 1) / kArThreads;   // R <= 512
+  constexpr int kTapRegs = (NI * NT * 512 + kArThreads - 1) / kArThreads;   // R <= 512
   float tapv[kTapRegs];
   auto fetch_taps = [&](int tt0, int l) {
     const int d = 1 << (l % a.layers_per_stack);
@@ -2348,10 +2354,10 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
     for (int j = 0; j < kTapRegs; ++j) {
       const int i = tid + j * kArThreads;
       float v = 0.f;
-      if (i < ni * 2 * a.R) {
-        const int it = i / (2 * a.R), k = i % (2 * a.R);
+      if (i < ni * NT * a.R) {
+        const int it = i / (NT * a.R), k = i % (NT * a.R);
         const int tap = k / a.R, r = k % a.R;
-        const int tt = tt0 - (2 - tap) * d;
+        const int tt = tt0 - (NT - tap) * d;
         if (tt >= 0) v = __ldcg(a.ring + ((long long)(item0 + it) * rofs[2 * a.L] + roff + (tt & (slots - 1))) * a.R + r);
       }
       tapv[j] = v;
@@ -2380,13 +2386,13 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
 #pragma unroll
       for (int j = 0; j < kTapRegs; ++j) {
         const int i = tid + j * kArThreads;
-        if (i < ni * 2 * a.R) in1[(i / (2 * a.R)) * ld1 + i % (2 * a.R)] = tapv[j];
+        if (i < ni * NT * a.R) in1[(i / (NT * a.R)) * ld1 + i % (NT * a.R)] = tapv[j];
       }
-      for (int i = tid; i < ni * (ld1 - 2 * a.R); i += kArThreads) {
-        const int it = i / (ld1 - 2 * a.R), k = 2 * a.R + i % (ld1 - 2 * a.R);
+      for (int i = tid; i < ni * (ld1 - NT * a.R); i += kArThreads) {
+        const int it = i / (ld1 - NT * a.R), k = NT * a.R + i % (ld1 - NT * a.R);
         float v = 0.f;
-        if (k < 3 * a.R) v = xbuf[it * a.R + (k - 2 * a.R)];
-        else if (k < a.K1) v = cvec[it * ((a.C + 3) & ~3) + (k - 3 * a.R)];
+        if (k < (NT + 1) * a.R) v = xbuf[it * a.R + (k - NT * a.R)];
+        else if (k < a.K1) v = cvec[it * ((a.C + 3) & ~3) + (k - (NT + 1) * a.R)];
         in1[it * ld1 + k] = v;
       }
       __syncthreads();
@@ -2570,6 +2576,12 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   }
 }
 
+// the instantiation for NIt items per cluster pass and NT past taps
+template <int NT>
+void (*ar_kernel(int NIt))(ArArgs) {
+  return NIt == 1 ? wn_ar_kernel<1, NT> : (NIt == 2 ? wn_ar_kernel<2, NT> : wn_ar_kernel<kArMaxItems, NT>);
+}
+
 }  // namespace
 }  // namespace t2
 
@@ -2739,7 +2751,7 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
   a.prefetch = (al.per_rank_layer % 8 == 0 && smem + wslots <= 232448 - 1024) ? 1 : 0;
   if (const char* e = getenv("T2_AR_PREFETCH")) { if (e[0] == '0') a.prefetch = 0; }
   if (a.prefetch) smem += wslots;
-  void (*kern)(ArArgs) = NIt == 1 ? wn_ar_kernel<1> : (NIt == 2 ? wn_ar_kernel<2> : wn_ar_kernel<kArMaxItems>);
+  void (*kern)(ArArgs) = lo.kw == 2 ? ar_kernel<1>(NIt) : lo.kw == 3 ? ar_kernel<2>(NIt) : ar_kernel<3>(NIt);
   T2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (al.CS > 8) T2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   T2_CHECK_CUDA(cudaMemsetAsync(ws + al.w_ring, 0, (size_t)lo.B * al.ring_slots_total * lo.R * 4, st));

@@ -59,7 +59,7 @@ def unsupported_hparams(hp):
         need("use_speaker_embedding", lambda v: bool(v),
              "speaker ids fed straight into the gin convolution without an embedding: wavenet.py:151-158")
         need("n_speakers", lambda v: v is not None and v >= 1, "gin_channels > 0 needs n_speakers >= 1")
-    need("kernel_size", lambda v: v == 3, "kernel_size 3")
+    need("kernel_size", lambda v: v in (2, 3, 4), "kernel_size 2, 3 or 4")
     need("upsample_type", lambda v: v in _UPSAMPLE_TYPES or v == "NearestNeighbor", "Resize upsampler: modules.py:657-693")
     need("upsample_activation", lambda v: v in _UPSAMPLE_ACTIVATIONS, "Relu | LeakyRelu | None: wavenet.py:197-203")
     if getattr(hp, "upsample_activation", None) == "LeakyRelu":
