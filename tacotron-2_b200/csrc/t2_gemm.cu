@@ -334,23 +334,12 @@ __device__ __forceinline__ void red_release_gpu_add(int* p, int v) {
 // orders generic-proxy accesses (the counters) with async-proxy (TMA) accesses of global memory
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
-// the stage barriers of ActGemmCfg<BN> (full: 1 arrival, empty: one per consumer warp), as act_gemm_kernel sets them up
-template <int BN>
-__device__ __forceinline__ void chain_init_barriers(uint8_t* smem) {
-  using Cfg = ActGemmCfg<BN>;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
-  for (int i = 0; i < Cfg::kStages; ++i) {
-    mbar_init(&full_bar[i], 1);
-    mbar_init(&full_bar[Cfg::kStages + i], kActEpiWarps);
-  }
-  fence_barrier_init();
-}
 // the previous ticket's barriers are invalidated before their memory is initialised again (the two GEMMs of a chain may place
 // them differently: 4 stages at BN 256, 6 at BN 128)
 template <int BN>
 __device__ __forceinline__ void chain_inval_barriers(uint8_t* smem) {
   using Cfg = ActGemmCfg<BN>;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
+  uint64_t* full_bar = Cfg::full_bar(smem);
   for (int i = 0; i < 2 * Cfg::kStages; ++i)
     asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[i])) : "memory");
 }
@@ -396,8 +385,9 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) wn_chain_kernel(const __gr
         s_epi = e;
         if (prev_kind == 0) chain_inval_barriers<BN0>(smem);
         else if (prev_kind == 1) chain_inval_barriers<BN1>(smem);
-        if (k.kind == 0) chain_init_barriers<BN0>(smem);
-        else chain_init_barriers<BN1>(smem);
+        // one CTA per tile, no multicast: one empty-barrier arrival per consumer warp
+        if (k.kind == 0) C0::init_barriers(smem, kActEpiWarps);
+        else C1::init_barriers(smem, kActEpiWarps);
         prev_kind = k.kind;
       } else {
         t = a.n_tix;
@@ -418,8 +408,9 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) wn_chain_kernel(const __gr
       fence_proxy_async_global();
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (k.kind == 0) act_gemm_tile<E0, BN0, true>(g, s_epi, smem, k.m, k.n, 0, all_kb, 1, 0, 1, nullptr);
-    else act_gemm_tile<E1, BN1, true>(g, s_epi, smem, k.m, k.n, 0, all_kb, 1, 0, 1, nullptr);
+    const int b = k.m / g.tiles_per_b, t0 = (k.m - b * g.tiles_per_b) * kBM;
+    if (k.kind == 0) act_gemm_tile<E0, BN0, true>(g, s_epi, smem, k.m, k.n, b, t0, 0, all_kb, 1, 0, 1, nullptr);
+    else act_gemm_tile<E1, BN1, true>(g, s_epi, smem, k.m, k.n, b, t0, 0, all_kb, 1, 0, 1, nullptr);
     // the tile's TMA stores are complete in the threads that issued them: publish them to the tiles that wait for this one
     fence_proxy_async_global();
     __syncthreads();

@@ -1028,30 +1028,49 @@ struct ActGemmCfg {
   static constexpr int kSmemBytes = kPipeBytes + kEpiBytes + 1024 + 256;
   static_assert(kStages >= 2 && kPipeBytes <= kPipeBudget && kSmemBytes <= 232448, "shared memory budget");
   static_assert(kPipeBytes % 1024 == 0, "staging tiles must be aligned to the 1024-byte swizzle atom");
+
+  // `smem` is the 1024-byte aligned base of the dynamic shared memory.
+  // the stage barriers follow the dedicated staging tile: kStages full barriers, then kStages empty barriers
+  static __device__ __forceinline__ uint64_t* full_bar(uint8_t* smem) {
+    return reinterpret_cast<uint64_t*>(smem + kPipeBytes + kEpiBytes);
+  }
+  static __device__ __forceinline__ uint64_t* empty_bar(uint8_t* smem) { return full_bar(smem) + kStages; }
+  // One thread initialises the stage barriers. A full barrier takes the producer's one arrival (plus the stage's TMA bytes), an
+  // empty barrier `empty_count` arrivals: one per consumer warp of every CTA that multicasts into the stage.
+  static __device__ __forceinline__ void init_barriers(uint8_t* smem, uint32_t empty_count) {
+    uint64_t* full = full_bar(smem);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&full[kStages + i], empty_count);
+    }
+    fence_barrier_init();
+  }
 };
 
-// One (m_tile, n_tile) output tile of `g`, exactly as one CTA of act_gemm_kernel computes it, for the tickets of the persistent WaveNet
-// layer chains. act_gemm_kernel keeps its own copy of these lines: calling this function from it gives the same PTX up to where the
-// tile-index arithmetic is placed, but ptxas then allocates its 96 registers differently and the per-layer gate GEMM spills more
-// (72 instead of 24 stack bytes) and runs 3.6 % slower on an H100. Keep the two in step: TMA producer loop, wgmma mainloop over k-blocks [kb_lo, kb_hi), the fp32 accumulator
-// tile, the fused epilogue (on `epi`) and the drain of its TMA stores. The caller has initialised the stage barriers of
-// ActGemmCfg<BN> (full: 1 arrival, empty: kActEpiWarps * cs) behind a CTA barrier and has made the tile's inputs visible; the
-// tile ends with every store's global writes complete in the threads that issued them (no CTA barrier at its end).
+// One (m_tile, n_tile) output tile of `g`: the body of every act_gemm_kernel CTA and of every ticket of the persistent WaveNet layer
+// chains. TMA producer loop, wgmma mainloop over k-blocks [kb_lo, kb_hi), the fp32 accumulator tile, the fused epilogue (on `epi`)
+// and the drain of its TMA stores. The caller has initialised the stage barriers (ActGemmCfg<BN>::init_barriers, empty count
+// kActEpiWarps * cs) behind a CTA barrier and has made the tile's inputs visible; the tile ends with every store's global writes
+// complete in the threads that issued them (no CTA barrier at its end).
 // `smem` is the 1024-byte aligned base of the dynamic shared memory; cs / crank / cmask describe the multicast cluster.
+// b / t0: the batch item and first time step of m_tile (m_tile = b * g.tiles_per_b + t0 / kBM). The caller divides, so that
+// act_gemm_kernel can do it before its PDL wait, off the path from the previous kernel's end to this tile's first TMA load.
+// ptxas allocates the 96 registers by how the tile indices and the k-block range reach this body: act_gemm_kernel reads blockIdx.x
+// and computes b / t0 and the split-K range at its entry. Reading blockIdx.x / .y in here instead spills the gate GEMM's epilogue to a 72-byte
+// stack (24 as it is; DESIGN §4), so check `-Xptxas -v` for every instantiation after changing how the arguments arrive.
 // kChain: the tile is a ticket of a persistent layer chain, whose epilogue inputs may come from other CTAs of the same grid
 template <int EPI, int BN, bool kChain = false>
 __device__ __forceinline__ void act_gemm_tile(const GemmArgs& g, const EpiArgs& epi, uint8_t* smem, int m_tile, int n_tile,
-                                              int kb_lo, int kb_hi, uint32_t cs, uint32_t crank, uint16_t cmask, long long* dbg) {
+                                              int b, int t0, int kb_lo, int kb_hi, uint32_t cs, uint32_t crank, uint16_t cmask,
+                                              long long* dbg) {
   using Cfg = ActGemmCfg<BN>;
   constexpr int WN = BN / 2;          // columns per consumer warpgroup
   float* acc_s = reinterpret_cast<float*>(smem);
   // staging tiles, tile-major over the row quarters: tiles 0 and 1 end the ring, the dedicated tile 2 follows it
   uint8_t* staging = smem + Cfg::kPipeBytes - Cfg::kTailBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
+  uint64_t* full_bar = Cfg::full_bar(smem);
+  uint64_t* empty_bar = Cfg::empty_bar(smem);
   const int warp = threadIdx.x >> 5;
-  const int b = m_tile / g.tiles_per_b;
-  const int t0 = (m_tile - b * g.tiles_per_b) * kBM;
   const int total_kb = kb_hi - kb_lo;
 
   if (warp == kActEpiWarps) {
@@ -1165,42 +1184,31 @@ __device__ __forceinline__ void act_gemm_tile(const GemmArgs& g, const EpiArgs& 
 template <int EPI, int BN>
 __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __grid_constant__ GemmArgs g) {
   using Cfg = ActGemmCfg<BN>;
-  constexpr int WN = BN / 2;          // columns per consumer warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* acc_s = reinterpret_cast<float*>(smem);
-  // staging tiles, tile-major over the row quarters: tiles 0 and 1 end the ring, the dedicated tile 2 follows it
-  uint8_t* staging = smem + Cfg::kPipeBytes - Cfg::kTailBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kPipeBytes + Cfg::kEpiBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
-
-  const int warp = threadIdx.x >> 5;
+  // the M tile, its batch item / first time step and the k-block range are taken here, first: before the PDL wait, and where they
+  // are computed decides the tile body's spills (act_gemm_tile)
   const int m_tile = blockIdx.x;
+  const int b = m_tile / g.tiles_per_b;
+  const int t0 = (m_tile - b * g.tiles_per_b) * kBM;
+  int all_kb = 0;
+  for (int s = 0; s < g.nseg; ++s) all_kb += g.seg[s].nkb * g.seg[s].nlayers;
+  // split-K: gridDim.z CTAs share one output tile, each reducing a contiguous slice of the k-blocks (the epilogue must
+  // then accumulate atomically)
+  const int kb_lo = int((long long)all_kb * blockIdx.z / gridDim.z), kb_hi = int((long long)all_kb * (blockIdx.z + 1) / gridDim.z);
+
   // Thread-block cluster along M (launch attribute; 1 = no cluster): the weight tile of a pipeline stage is identical for every M
   // tile, so each CTA of the cluster fetches 1/cs of its rows and MULTICASTS them to all peers (one L2 read feeds cs SMs).
   const uint32_t cs = cluster_nctarank(), crank = cluster_ctarank();
   const uint16_t cmask = uint16_t((1u << cs) - 1u);
   long long* dbg = g.dbg ? g.dbg + ((size_t(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * kDbgSlots : nullptr;
   if (dbg && threadIdx.x == 0) { dbg[0] = clock64(); dbg[8] = globaltimer_ns(); dbg[11] = smid(); }
-  const int b = m_tile / g.tiles_per_b;
-  const int t0 = (m_tile - b * g.tiles_per_b) * kBM;
 
-  int all_kb = 0;
-  for (int s = 0; s < g.nseg; ++s) all_kb += g.seg[s].nkb * g.seg[s].nlayers;
-  // split-K: gridDim.z CTAs share one output tile, each reducing a contiguous slice of the k-blocks (the epilogue must
-  // then accumulate atomically)
-  const int kb_lo = int((long long)all_kb * blockIdx.z / gridDim.z), kb_hi = int((long long)all_kb * (blockIdx.z + 1) / gridDim.z);
-  const int total_kb = kb_hi - kb_lo;
-
-  if (warp == kActEpiWarps && elect_one()) {
+  if ((threadIdx.x >> 5) == kActEpiWarps && elect_one()) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&g.amap[i]);
     tma_prefetch_desc(&g.bmap);
-    for (int i = 0; i < Cfg::kStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      // a stage is free once every consumer warp of EVERY CTA of the cluster has consumed it (peers multicast into it)
-      mbar_init(&empty_bar[i], kActEpiWarps * cs);
-    }
-    fence_barrier_init();
+    // a stage is free once every consumer warp of EVERY CTA of the cluster has consumed it (peers multicast into it)
+    Cfg::init_barriers(smem, kActEpiWarps * cs);
   }
   __syncthreads();
   if (cs > 1) cluster_sync_all();      // peers' barriers are initialised before any remote arrive / multicast write
@@ -1209,110 +1217,7 @@ __global__ void __launch_bounds__(kActGemmThreads, 1) act_gemm_kernel(const __gr
   pdl_launch_dependents();
   if (dbg && threadIdx.x == 0) { dbg[1] = clock64(); dbg[9] = globaltimer_ns(); }
 
-  if (warp == kActEpiWarps) {
-    if (elect_one()) {
-      const int n_tile = blockIdx.y;
-      int stage = 0;
-      uint32_t phase = 0;
-      int kb_global = 0;
-      for (int s = 0; s < g.nseg; ++s) {
-        const Seg sg = g.seg[s];
-        for (int l = 0; l < sg.nlayers; ++l) {
-          for (int kb = 0; kb < sg.nkb; ++kb, ++kb_global) {
-            if (kb_global < kb_lo || kb_global >= kb_hi) continue;
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-            uint8_t* sa = smem + stage * Cfg::kStageBytes;
-            uint8_t* sb = sa + Cfg::kABytes;
-            tma_load_4d(sa, &g.amap[sg.map], &full_bar[stage], sg.k0 + kb * kBK, t0 + sg.shift, b, sg.layer0 + l);
-            if (cs == 1) {
-              tma_load_3d(sb, &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK, n_tile * BN, g.b_layer);
-            } else {
-              const int rows = BN / int(cs);     // this CTA's slice of the weight tile (whole 8-row swizzle atoms: 1024-byte aligned)
-              tma_load_3d_mc(sb + crank * rows * (kBK * 2), &g.bmap, &full_bar[stage], g.b_k0 + kb_global * kBK,
-                             n_tile * BN + int(crank) * rows, g.b_layer, cmask);
-            }
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;  // row quarter of this warp in the epilogue
-    const int lane = threadIdx.x & 31;
-    EpiCtx c;
-    c.lane = lane;
-    c.cg = warp >> 2;
-    c.qbar = 1 + q;
-    c.b = b; c.T = g.T;
-    const int tw = t0 + q * 32;          // first time step of this warp
-    c.t = tw + c.lane;
-    c.valid = c.t < g.T;
-    c.row0 = size_t(b) * g.T + tw;
-    c.nrows = g.T - tw < 0 ? 0 : (g.T - tw > 32 ? 32 : g.T - tw);
-    c.stg = staging + q * kSTileBytes;
-    c.smem_all = smem + Cfg::kAccBytes;
-    c.m_tile = m_tile;
-    c.omap = g.omap; c.tq = tw; c.sk = 0;
-    c.n_tile = blockIdx.y;
-    if constexpr (EpiHasPrefetch<EPI>::value) Epilogue<EPI, BN>::prefetch(g.epi, c);
-
-    // ---- mainloop: this warpgroup's 64 x WN quarter of the tile
-    const int wg = warp >> 2, mh = wg >> 1, nh = wg & 1;
-    float d[WN / 2];
-#pragma unroll
-    for (int i = 0; i < WN / 2; ++i) d[i] = 0.f;
-    int stage = 0, prev = 0;
-    uint32_t phase = 0;
-    for (int kb = 0; kb < total_kb; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      __syncwarp();                    // wgmma is warp-aligned: reconverge after the spin-wait
-      if (dbg && kb == 0 && threadIdx.x == 0) dbg[2] = clock64();
-      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes) + uint32_t(mh * 64 * 128);
-      const uint32_t sb = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes) + uint32_t(nh * WN * 128);
-      const uint64_t adesc = make_gdesc_sw128(sa, 16, 1024);
-      const uint64_t bdesc = make_gdesc_sw128(sb, 16, 1024);
-      wgmma_fence();
-      wgmma_fence_regs(d);
-#pragma unroll
-      for (int k = 0; k < kBK / 16; ++k)
-        // advancing K by 16 bf16 = 32 bytes inside the 128-byte swizzle row: +2 in the (addr>>4) field
-        Wgmma<WN, 0, 0>::mma(d, adesc + uint64_t(k * 2), bdesc + uint64_t(k * 2), (kb > 0 || k > 0) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_fence_regs(d);
-      // the previous k-block's MMAs have finished reading their stage: hand it back to the producer(s)
-      wgmma_wait<1>();
-      if (kb > 0 && lane == 0) {
-        if (cs == 1) mbar_arrive(&empty_bar[prev]);
-        else for (uint32_t r = 0; r < cs; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
-      }
-      prev = stage;
-      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(d);
-    if (dbg && threadIdx.x == 0) dbg[3] = clock64();
-    // every warpgroup's MMAs are done with the stages: the accumulator tile may overwrite them
-    asm volatile("bar.sync 6, 512;\n" ::: "memory");
-    {
-      const int r0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
-#pragma unroll
-      for (int j = 0; j < WN / 8; ++j)
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int r = r0 + 8 * i, col = nh * WN + 8 * j + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(acc_s + r * BN + ((((col >> 2) ^ (r & 7)) << 2) | (col & 3))) =
-              make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
-        }
-    }
-    asm volatile("bar.sync 6, 512;\n" ::: "memory");
-    const int row = q * 32 + lane;
-    c.trow = AccRow{acc_s + row * BN, 0, row & 7};
-    if (dbg && threadIdx.x == 0) dbg[4] = clock64();
-    Epilogue<EPI, BN>::run(g.epi, c);
-    if (dbg && threadIdx.x == 0) dbg[5] = clock64();
-    tile_store_drain(c);
-  }
+  act_gemm_tile<EPI, BN>(g, g.epi, smem, m_tile, blockIdx.y, b, t0, kb_lo, kb_hi, cs, crank, cmask, dbg);
   __syncthreads();
   if (dbg && threadIdx.x == 0) { dbg[6] = clock64(); dbg[10] = globaltimer_ns(); }
   // no CTA may leave while a peer can still arrive on its barriers or multicast into its shared memory
