@@ -121,7 +121,10 @@ typedef struct {
  *          K fp32 [KA][F], bK [F], Wl [F][A], ba [A], U fp32 [(KA+1)][A] (out: merged filter bank), v [A], keys fp32 [B][Ti][A],
  *          values bf16 [B][Ti][C2], lens int32 [B], cum fp32 [B][Ti] (in/out: the attention state), alpha fp32 [B][Ti] (out), ctx_a
  *          bf16 (nullable), ctx_b bf16. i: B, Ti, D, A, KA, F, C2, ld_h2, ld_a, ld_b, unmasked, noncumulative (the two
- *          t2_taco_config_t flags; 0 = masked scores and cum + alpha as the new state, 1 = all T_in scores and alpha as the new state).
+ *          t2_taco_config_t flags; 0 = masked scores and cum + alpha as the new state, 1 = all T_in scores and alpha as the new state),
+ *          split (t2_taco_config_t.split_bf16: WqT rows are [hi(D) | lo(D)], values rows [hi(C2) | lo(C2)]), then lo_h2, lo_a, lo_b (0
+ *          unless split): the lo half of the query source sits at +lo_h2, ctx_a is written [hi | lo at +lo_a | hi again at +2 lo_a],
+ *          ctx_b [hi | lo at +lo_b].
  * BN_FWD   bn_stats_kernel (training) + bn_apply_kernel (conv-block batch norm). p: y (bf16, or fp32 when i[3]), x bf16 [rows][C] (split: [rows][2C]),
  *          stats fp32 [4C], gamma, beta, moving mean, moving variance. i: rows, C, training, y_fp32, stream, split. f: dropout p.
  * BN_BWD   bn_bwd_stats_kernel + bn_bwd_apply_kernel. p: dout bf16, y bf16, stats fp32 [6C] (mean / rstd at [2C, 4C); [4C, 6C) receives
@@ -148,6 +151,36 @@ typedef struct {
 #define T2_DBG_TACO_ATT_FINISH 5
 #define T2_DBG_TACO_DVALUES 6
 #define T2_DBG_TACO_ATT_BWD 7
+/* CONV_GEMM   conv_gemm: a k-tap 'same' convolution / projection through the GEMM engine and EPI_BIAS_ACT, tap j reading row
+ *             t + conv_tap_shift(ntaps, j) of the same item. p: a bf16 [Bn][T][C] (split: [Bn][T][hi(Cp) | lo(Cp)], Cp = C rounded up
+ *             to 64), packed weight bf16 [N][wK] (split: [W_hi | W_hi | W_lo] per tap, wK >= 3 ntaps Cp), bias fp32 [N] (nullable),
+ *             out bf16 [Bn T][ldo] (split: [hi(ldo) | lo(ldo)], pitch 2 ldo; nullable), out fp32 [Bn T][ldo] (nullable; one of the two
+ *             outputs is required). i: C, T, Bn, N, wK, ntaps (<= 16; split <= 8), BN (128 / 256), act (0 none, 1 relu, 2 tanh), ldo,
+ *             nvalid, dropout stream, split, hash_row0 (position offset of the dropout mask). f: dropout rate. seed / step: dropout seed.
+ * LSTM_STEP   lstm_step: one recurrent step on the swapped GEMM (EPI_LSTM). p: wrec bf16 [4H][K] (split: [4H][W_hi | W_hi | W_lo]),
+ *             state bf16 [B][K] (split: [B][hi | lo | hi]), pre fp32 (row b at + b pre_stride, nullable), bias fp32 [4H] (nullable),
+ *             c_prev fp32 [B][H], c_out fp32 [B][H], h_prev bf16 (+ b ld_hp; split: lo at +K), h_state bf16 (+ b ld_hs; split: written
+ *             [hi | lo at +K | hi at +2K]), h_out bf16 (+ b ld_ho; split: lo at +out_lo, and the second hi copy at +2 out_lo when
+ *             out_state), gate stash bf16 [B][4H] (nullable), tanh(c) stash bf16 [B][H] (nullable; neither stash is written in split
+ *             mode), lens int32 [B] (nullable). i: H, K, B, pre_stride, ld_hp, ld_hs, ld_ho, t, zoneout stream, out_lo, out_state,
+ *             training, split. f: zoneout rate. seed / step: zoneout seed.
+ * ROWS        one of the small row writers, i[0] selecting it and i[1] = split (0: bf16 rows, 1: split-bf16 [hi | lo] rows):
+ *             0 embed_fwd_kernel    p: idx int32 [npos], table fp32 [NS][E], out bf16 ([npos][E]; split [npos][hi(E) | lo(E)]).
+ *                                   i: -, -, npos, E.
+ *             1 decin_kernel        p: target fp32 [B][To][M], out bf16 ([To][B][M]; split: rows [hi(M) | pad | lo(M) | pad] of pitch
+ *                                   256, the padding is not written). i: -, -, B, To, M.
+ *             2 dec_finish_kernel   p: projo fp32 [To][B][128], target fp32 [B][To][M] (nullable), stop target (nullable), dec bf16
+ *                                   ([B][To][M]; split: rows [hi(M) | pad | lo(M) | pad] of pitch 256), dec fp32 [B][To][M], stop fp32
+ *                                   [B][To], loss sums fp32 [5] (accumulated), target lengths int32 [B] (nullable). i: -, -, B, To, M,
+ *                                   clip. f: clip low, clip high, stop positive weight.
+ *             3 proj_bias_feedback_kernel  p: projection fp32 [B][128] (in / out), frame bias [M], stop bias [1], next input bf16
+ *                                   (nullable; [B][M], split: decin rows of pitch 256), target fp32 [B][To][M] (nullable), choice int32
+ *                                   [To] (required with a target). i: -, -, B, M, To, t. f: teacher-forcing ratio. seed / step: its draw.
+ *             4 f32_to_bf16_kernel  p: in fp32 [rows][C], out bf16 ([rows][C]; split [rows][hi(Cp) | lo(Cp)], channels C..Cp-1
+ *                                   zero). i: -, -, rows, C, Cp (= C unless split). */
+#define T2_DBG_TACO_CONV_GEMM 8
+#define T2_DBG_TACO_LSTM_STEP 9
+#define T2_DBG_TACO_ROWS 10
 int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 /* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
  * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):

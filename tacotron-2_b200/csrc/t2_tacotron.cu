@@ -429,7 +429,13 @@ constexpr int kAttPad = 8;   // row padding (floats) of the filter bank / dE til
 __device__ __forceinline__ float toep(const float* __restrict__ cum, int j, int k, int KA) {
   return k < KA ? cum[j + k] : (k == KA ? 1.f : 0.f);
 }
+// the TF32 remainder of x: tf32(x - tf32(x)) (the subtraction is exact in fp32)
+__device__ __forceinline__ uint32_t tf32_rest(float x, uint32_t big) { return f2tf32(x - __uint_as_float(big)); }
 // pl for the 16 rows j0.. and the 64 channels n0..: acc[nt] = C fragment of n-tile nt (8 channels each)
+// kSplit (split_bf16): 3xTF32. Both operands are split as big = tf32(x), small = tf32(x - big) and the three products
+// small.big + big.small + big.big are accumulated; the dropped small.small and the remainders past small are <= ~2^-21 of |cum| |U|,
+// where one TF32 product alone rounds each operand by up to 2^-11.
+template <bool kSplit>
 __device__ __forceinline__ void loc_tile(const float* __restrict__ Us, int AP, const float* __restrict__ cum, int KA, int j0, int n0,
                                          float (&acc)[8][4]) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -441,11 +447,20 @@ __device__ __forceinline__ void loc_tile(const float* __restrict__ Us, int AP, c
     uint32_t af[4];
     af[0] = f2tf32(toep(cum, j0 + g, k, KA)); af[1] = f2tf32(toep(cum, j0 + g + 8, k, KA));
     af[2] = f2tf32(toep(cum, j0 + g, k + 4, KA)); af[3] = f2tf32(toep(cum, j0 + g + 8, k + 4, KA));
+    uint32_t as[4];
+    if (kSplit) {
+      as[0] = tf32_rest(toep(cum, j0 + g, k, KA), af[0]); as[1] = tf32_rest(toep(cum, j0 + g + 8, k, KA), af[1]);
+      as[2] = tf32_rest(toep(cum, j0 + g, k + 4, KA), af[2]); as[3] = tf32_rest(toep(cum, j0 + g + 8, k + 4, KA), af[3]);
+    }
     const bool v0 = k <= KA, v1 = k + 4 <= KA;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
       const int n = n0 + nt * 8 + g;
       const uint32_t b0 = v0 ? f2tf32(Us[k * AP + n]) : 0u, b1 = v1 ? f2tf32(Us[(k + 4) * AP + n]) : 0u;
+      if (kSplit) {
+        mma_tf32(acc[nt], as, b0, b1);
+        mma_tf32(acc[nt], af, v0 ? tf32_rest(Us[k * AP + n], b0) : 0u, v1 ? tf32_rest(Us[(k + 4) * AP + n], b1) : 0u);
+      }
       mma_tf32(acc[nt], af, b0, b1);
     }
   }
@@ -496,7 +511,7 @@ __global__ void __launch_bounds__(kAttThreads) att_fwd_kernel(AttArgs a) {
     for (int u = warp; u < n_units; u += NW) {
       const int j0 = (u / n_nh) * 16, n0 = (u % n_nh) * 64;
       float acc[8][4];
-      loc_tile(Us, AP, cum, a.KA, j0, n0, acc);
+      loc_tile<kSplit>(Us, AP, cum, a.KA, j0, n0, acc);
       const int r0 = j0 + g, r1 = r0 + 8;
       const float* k0p = a.keys + ((long long)b * Ti + (r0 < el ? r0 : 0)) * A + n0 + 2 * t;
       const float* k1p = a.keys + ((long long)b * Ti + (r1 < el ? r1 : 0)) * A + n0 + 2 * t;
@@ -1104,7 +1119,7 @@ __global__ void __launch_bounds__(kAttThreads) att_bwd_kernel(AttBwd a) {
     for (int u = warp; u < n_units; u += NW) {
       const int j0 = (u / n_nh) * 16, n0 = (u % n_nh) * 64;
       float acc[8][4];
-      loc_tile(Us, AP, cum, a.KA, j0, n0, acc);
+      loc_tile<false>(Us, AP, cum, a.KA, j0, n0, acc);
       const int r0 = j0 + g, r1 = r0 + 8;
       const bool ok0 = r0 < el, ok1 = r1 < el;
       const long long kr0 = ((long long)b * Ti + (ok0 ? r0 : 0)) * A + n0 + 2 * t, kr1 = ((long long)b * Ti + (ok1 ? r1 : 0)) * A + n0 + 2 * t;
@@ -2083,9 +2098,15 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
                  T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FWD: bad pitch or alignment");
       T2_REQUIRE((i[10] == 0 || i[10] == 1) && (i[11] == 0 || i[11] == 1), T2_ERR_INVALID_ARG,
                  "dbg_taco_kernel ATT_FWD: unmasked / noncumulative must be 0 or 1");
+      const int split = int(i[12]);
+      T2_REQUIRE(split == 0 ? i[13] == 0 && i[14] == 0 && i[15] == 0
+                            : split == 1 && i[13] >= D && i[7] >= i[13] + D && i[14] >= C2 && (!p[13] || i[8] >= 2 * i[14] + C2) &&
+                                  i[15] >= C2 && i[9] >= i[15] + C2,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel ATT_FWD: bad split flag or lo offsets");
       const size_t smem = att_fwd_smem(Ti, KA, A, D, C2);
       T2_REQUIRE(smem <= kSmemOptin, T2_ERR_UNSUPPORTED_SHAPE, "dbg_taco_kernel ATT_FWD: %zu B of shared memory", smem);
       AttArgs a;
+      a.split = split; a.lo_h2 = int(i[13]); a.lo_a = int(i[14]); a.lo_b = int(i[15]);
       a.h2out = static_cast<const bf16*>(p[0]); a.ld_h2 = int(i[7]); a.WqT = static_cast<const bf16*>(p[1]);
       a.U = static_cast<float*>(p[6]); a.v = static_cast<const float*>(p[7]);
       a.keys = static_cast<const float*>(p[8]); a.values = static_cast<const bf16*>(p[9]); a.lens = static_cast<const int*>(p[10]);
@@ -2093,8 +2114,92 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       a.ctx_a = static_cast<bf16*>(p[13]); a.ld_a = int(i[8]); a.ctx_b = static_cast<bf16*>(p[14]); a.ld_b = int(i[9]);
       a.B = B; a.Ti = Ti; a.D = D; a.A = A; a.KA = KA; a.C2 = C2; a.unmasked = int(i[10]); a.noncumulative = int(i[11]);
       int rc = att_fwd_setup(static_cast<const float*>(p[2]), static_cast<const float*>(p[3]), static_cast<const float*>(p[4]),
-                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, a.unmasked, a.noncumulative, 0, st);
+                             static_cast<const float*>(p[5]), static_cast<float*>(p[6]), KA, F, A, smem, a.unmasked, a.noncumulative, split, st);
       return rc ? rc : launch_att_fwd(a, smem, st);
+    }
+    case T2_DBG_TACO_CONV_GEMM: {
+      const int C = int(i[0]), T = int(i[1]), Bn = int(i[2]), N = int(i[3]), wK = int(i[4]), ntaps = int(i[5]), BN = int(i[6]);
+      const int act = int(i[7]), ldo = int(i[8]), nvalid = int(i[9]), sid = int(i[10]), split = int(i[11]), row0 = int(i[12]);
+      const float pdrop = call->f[0];
+      const int Cp = (C + kBK - 1) / kBK * kBK;
+      T2_REQUIRE(p[0] && p[1] && (p[3] || p[4]) && aligned16(p[0]) && aligned16(p[1]) && (split == 0 || split == 1) &&
+                     ntaps >= 1 && ntaps <= (split ? kMaxSeg / 2 : kMaxSeg),
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel CONV_GEMM: bad pointers, split flag or tap count");
+      T2_REQUIRE(C >= 1 && C <= 4096 && (split || C % 8 == 0) && T >= 1 && Bn >= 1 && Bn <= 65535 && N >= 1 && wK % 8 == 0 &&
+                     wK >= ntaps * Cp * (split ? 3 : 1) && (BN == 128 || BN == 256) && act >= 0 && act <= 2 && nvalid >= 1 && nvalid <= N &&
+                     ldo >= nvalid && sid >= 0 && row0 >= 0 && pdrop >= 0.f && pdrop < 1.f && (ldo % 8 == 0 || !split),
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel CONV_GEMM: bad shape");
+      int shifts[kMaxSeg];
+      for (int j = 0; j < ntaps; ++j) shifts[j] = conv_tap_shift(ntaps, j);
+      int rc = conv_gemm(p[0], C, T, Bn, p[1], N, wK, ntaps, shifts, BN, static_cast<float*>(p[2]), act, p[3], static_cast<float*>(p[4]), ldo,
+                         nvalid, pdrop, sid, call->seed, call->step, st, split, row0);
+      if (rc) return rc;
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
+    }
+    case T2_DBG_TACO_LSTM_STEP: {
+      const int H = int(i[0]), K = int(i[1]), B = int(i[2]), pre_stride = int(i[3]), ld_hp = int(i[4]), ld_hs = int(i[5]), ld_ho = int(i[6]);
+      const int t = int(i[7]), sid = int(i[8]), out_lo = int(i[9]), out_state = int(i[10]), training = int(i[11]), split = int(i[12]);
+      const float zone = call->f[0];
+      T2_REQUIRE(p[0] && p[1] && p[4] && p[5] && p[6] && p[7] && p[8] && aligned16(p[0]) && aligned16(p[1]) && (split == 0 || split == 1) &&
+                     (training == 0 || training == 1) && (out_state == 0 || out_state == 1) && zone >= 0.f && zone < 1.f && t >= 0 && sid >= 0,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel LSTM_STEP: bad pointers or flags");
+      T2_REQUIRE(H >= 32 && H % 32 == 0 && K >= 64 && K % 64 == 0 && B >= 1 && B <= 65535 && (!p[2] || pre_stride >= 4 * H) &&
+                     (split ? ld_hp >= K + H && ld_hs >= 2 * K + H && out_lo >= H && ld_ho >= (out_state ? 2 : 1) * out_lo + H
+                            : ld_hp >= H && ld_hs >= H && ld_ho >= H && out_lo == 0 && out_state == 0),
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel LSTM_STEP: bad shape or pitch");
+      TL lo{};
+      lo.c.split_bf16 = split;
+      StepCtx s{&lo, nullptr, nullptr, nullptr, st, call->seed, call->step, training};
+      int rc = lstm_step(s, p[0], H, K, p[1], B, static_cast<const float*>(p[2]), pre_stride, static_cast<const float*>(p[3]),
+                         static_cast<const float*>(p[4]), static_cast<float*>(p[5]), static_cast<const bf16*>(p[6]), ld_hp,
+                         static_cast<bf16*>(p[7]), ld_hs, static_cast<bf16*>(p[8]), ld_ho, static_cast<bf16*>(p[9]), static_cast<bf16*>(p[10]),
+                         static_cast<const int*>(p[11]), t, sid, zone, out_lo, out_state);
+      if (rc) return rc;
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
+    }
+    case T2_DBG_TACO_ROWS: {
+      const int which = int(i[0]), split = int(i[1]);
+      T2_REQUIRE(which >= 0 && which <= 4 && (split == 0 || split == 1), T2_ERR_INVALID_ARG, "dbg_taco_kernel ROWS: bad writer or split flag");
+      if (which == 0) {   // embed_fwd_kernel
+        const long long npos = i[2];
+        const int E = int(i[3]);
+        T2_REQUIRE(p[0] && p[1] && p[2] && npos >= 1 && E >= 1, T2_ERR_INVALID_ARG, "dbg_taco_kernel ROWS embed: bad arguments");
+        embed_fwd_kernel<<<grid1d(npos * E), 256, 0, st>>>(static_cast<const int*>(p[0]), static_cast<const float*>(p[1]), static_cast<bf16*>(p[2]),
+                                                           npos, E, split);
+      } else if (which == 1) {   // decin_kernel
+        const int B = int(i[2]), To = int(i[3]), M = int(i[4]);
+        T2_REQUIRE(p[0] && p[1] && B >= 1 && To >= 1 && M >= 1 && (!split || M <= 128), T2_ERR_INVALID_ARG,
+                   "dbg_taco_kernel ROWS decin: bad arguments");
+        decin_kernel<<<grid1d((long long)To * B * M), 256, 0, st>>>(static_cast<const float*>(p[0]), static_cast<bf16*>(p[1]), B, To, M, split);
+      } else if (which == 2) {   // dec_finish_kernel
+        const int B = int(i[2]), To = int(i[3]), M = int(i[4]), clip = int(i[5]);
+        T2_REQUIRE(p[0] && p[3] && p[4] && p[5] && p[6] && B >= 1 && To >= 1 && M >= 1 && M + 1 <= 128 && (clip == 0 || clip == 1),
+                   T2_ERR_INVALID_ARG, "dbg_taco_kernel ROWS dec_finish: bad arguments");
+        dec_finish_kernel<<<grid1d((long long)B * To * (M + 1)), 256, 0, st>>>(
+            static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]), static_cast<bf16*>(p[3]),
+            static_cast<float*>(p[4]), static_cast<float*>(p[5]), static_cast<float*>(p[6]), B, To, M, clip, call->f[0], call->f[1], split,
+            static_cast<const int*>(p[7]), call->f[2]);
+      } else if (which == 3) {   // proj_bias_feedback_kernel
+        const int B = int(i[2]), M = int(i[3]), To = int(i[4]), t = int(i[5]);
+        T2_REQUIRE(p[0] && p[1] && p[2] && (!p[4] || p[5]) && B >= 1 && M >= 1 && M + 1 <= 128 && To >= 1 && t >= 0 && t < To &&
+                       call->f[0] >= 0.f && call->f[0] <= 1.f,
+                   T2_ERR_INVALID_ARG, "dbg_taco_kernel ROWS proj_bias_feedback: bad arguments");
+        T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (M + 1))), dim3(256), 0, st, static_cast<float*>(p[0]),
+                                 static_cast<const float*>(p[1]), static_cast<const float*>(p[2]), static_cast<bf16*>(p[3]), B, M,
+                                 static_cast<const float*>(p[4]), To, t, call->f[0], call->seed, call->step, static_cast<int*>(p[5]), split));
+      } else {   // f32_to_bf16_kernel
+        const long long rows = i[2];
+        const int C = int(i[3]), Cp = int(i[4]);
+        T2_REQUIRE(p[0] && p[1] && rows >= 1 && C >= 1 && (split ? Cp >= C : Cp == C), T2_ERR_INVALID_ARG,
+                   "dbg_taco_kernel ROWS f32_to_bf16: bad arguments");
+        if (split) launch_f32_to_bf16_split(static_cast<const float*>(p[0]), static_cast<bf16*>(p[1]), rows, C, Cp, st);
+        else launch_f32_to_bf16(static_cast<const float*>(p[0]), static_cast<bf16*>(p[1]), rows * C, st);
+      }
+      if (which <= 3) t2_count_launch();
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
     }
     case T2_DBG_TACO_ATT_BWD: {
       const int B = int(i[0]), Ti = int(i[1]), D = int(i[2]), A = int(i[3]), KA = int(i[4]), C2 = int(i[5]);

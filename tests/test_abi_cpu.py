@@ -246,3 +246,85 @@ def test_training_rejects_t_in_past_the_attention_backward_limit():
             assert rc == -2, (T_in, rc, lib.t2_last_error())
             msg = lib.t2_last_error()
             assert b"T_in <= 336" in msg and b"232448" in msg, msg
+
+
+def _taco_hook(kernel, p, i, f=()):
+    from t2_import import t2
+    lib = t2.lib.load()
+    c = t2.lib.DbgKernel()
+    c.kernel = kernel
+    for k, v in enumerate(p):
+        c.p[k] = v
+    for k, v in enumerate(i):
+        c.i[k] = v
+    for k, v in enumerate(f):
+        c.f[k] = v
+    return lib.t2_dbg_taco_kernel(ctypes.byref(c), None), lib.t2_last_error()
+
+
+# the fp32-class (split-bf16) hooks of tests/test_split_operands_gpu.py: each call below breaks exactly one argument of an otherwise
+# valid launch, and is refused before any driver call (the fake pointers are never dereferenced)
+_FAKE = [16 * (k + 1) for k in range(16)]
+CONV_GOOD = [128, 40, 2, 128, 3 * 3 * 128, 3, 128, 0, 128, 128, 0, 1, 0]   # C, T, Bn, N, wK, ntaps, BN, act, ldo, nvalid, stream, split, row0
+LSTM_GOOD = [64, 64, 2, 256, 192, 192, 256, 0, 0, 128, 0, 1, 1]            # H, K, B, pre_stride, ld_hp, ld_hs, ld_ho, t, stream, out_lo,
+                                                                           # out_state, training, split
+ATT_GOOD = [2, 40, 256, 128, 31, 32, 512, 520, 1040 + 512, 1040, 0, 0, 1, 264, 520, 520]
+
+
+@pytest.mark.parametrize("k,v,msg", [(5, 9, b"tap count"), (5, 0, b"tap count"), (11, 2, b"split flag"), (6, 64, b"bad shape"),
+                                     (4, 3 * 3 * 128 - 8, b"bad shape"), (7, 3, b"bad shape"), (9, 129, b"bad shape"),
+                                     (8, 120, b"bad shape"), (12, -1, b"bad shape")])
+def test_conv_gemm_hook_rejects_bad_arguments(k, v, msg):
+    """ntaps = 9 is 18 segments in split mode, more than kMaxSeg = 16"""
+    i = list(CONV_GOOD)
+    i[k] = v
+    rc, err = _taco_hook(8, _FAKE[:5], i)
+    assert rc == -1 and msg in err, err
+
+
+def test_conv_gemm_hook_needs_an_output_and_nine_taps_are_fine_only_in_bf16_mode():
+    i = list(CONV_GOOD)
+    rc, err = _taco_hook(8, _FAKE[:3] + [0, 0], i)
+    assert rc == -1 and b"bad pointers" in err
+    i[5], i[4], i[11] = 9, 9 * 128, 0
+    i[0] = 100                                    # bf16 mode: 9 segments pass the tap check; C % 8 != 0 is refused next
+    rc, err = _taco_hook(8, _FAKE[:5], i)
+    assert rc == -1 and b"bad shape" in err, err
+
+
+@pytest.mark.parametrize("k,v,msg", [(12, 2, b"flags"), (11, 2, b"flags"), (10, 2, b"flags"), (0, 48, b"pitch"), (1, 96, b"pitch"),
+                                     (4, 64 + 63, b"pitch"), (5, 128 + 63, b"pitch"), (9, 63, b"pitch"), (6, 128 + 63, b"pitch"),
+                                     (3, 255, b"pitch"), (7, -1, b"flags")])
+def test_lstm_step_hook_rejects_bad_arguments(k, v, msg):
+    i = list(LSTM_GOOD)
+    i[k] = v
+    rc, err = _taco_hook(9, _FAKE[:12], i, [0.1])
+    assert rc == -1 and msg in err, err
+
+
+def test_lstm_step_hook_rejects_split_offsets_in_bf16_mode_and_a_bad_zoneout_rate():
+    i = list(LSTM_GOOD)
+    i[12] = 0                                     # bf16 mode with out_lo / out_state set
+    rc, err = _taco_hook(9, _FAKE[:12], i, [0.1])
+    assert rc == -1 and b"pitch" in err, err
+    rc, err = _taco_hook(9, _FAKE[:12], LSTM_GOOD, [1.0])
+    assert rc == -1 and b"flags" in err, err
+
+
+@pytest.mark.parametrize("k,v", [(12, 2), (13, 255), (15, 511), (14, 511), (9, 1031), (7, 519)])
+def test_att_fwd_hook_checks_the_split_offsets(k, v):
+    i = list(ATT_GOOD)
+    i[k] = v
+    rc, err = _taco_hook(1, _FAKE[:15], i)
+    assert rc == -1 and b"lo offsets" in err, err
+
+
+def test_att_fwd_hook_rejects_lo_offsets_in_bf16_mode_and_rows_rejects_a_bad_writer():
+    i = list(ATT_GOOD)
+    i[12] = 0
+    rc, err = _taco_hook(1, _FAKE[:15], i)
+    assert rc == -1 and b"lo offsets" in err, err
+    rc, err = _taco_hook(10, _FAKE[:8], [5, 1, 2, 8, 80])
+    assert rc == -1 and b"bad writer" in err, err
+    rc, err = _taco_hook(10, _FAKE[:8], [1, 1, 2, 8, 129])        # split decoder-input rows hold at most 128 mels per half
+    assert rc == -1 and b"decin" in err, err

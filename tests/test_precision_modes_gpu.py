@@ -5,7 +5,8 @@ SAME wgmma kernels (three products per contraction), forward + loss only:
 
   WaveNet fp32-class   logits max abs err <= 1e-4 (measured 6e-6), loss (CE / MoL NLL) abs err <= 1e-4   -> north-star 1e-3 met
   WaveNet bf16         logits max abs err <= 5e-3, loss abs err <= 1e-3 (measured: 1.7e-3 / 3e-5 at the 24-layer Cfg-2 shape)
-  Tacotron             the convolution stacks have the fp32-class mode, the recurrences do not: see the Tacotron test below
+  Tacotron fp32-class  every contraction (convolution stacks, recurrences, attention, projections) on split operands:
+                       mel-L1 <= 1e-3 at the Cfg-3 widths, against ~2.5e-2 in bf16 mode (the Tacotron test below)
 
 so the bf16-mode deviation is operand / storage rounding, not a difference in the algorithm."""
 import math
@@ -72,21 +73,21 @@ def test_wavenet_fp32_class_vs_bf16(shape):
 @pytest.mark.parametrize("stochastic", [False, True])
 def test_tacotron_fp32_class_conv_stacks_vs_bf16(stochastic):
     """mel-L1 on `mel_outputs` (the north-star parity metric) at the Cfg-3 widths, B = 32, T_in 160, T_out 200.
-    bf16 mode: ~2.5e-2 at random init. Two contributions (tools/taco_layer_diag.py): (i) every batch-normalised postnet layer adds
-    ~0.2 % of a unit-variance activation through bf16 storage of operands / activations; (ii) at random init the decoder outputs are
-    nearly constant over (batch, time) (per-channel std 0.06), so the FIRST postnet batch norm divides by a pre-norm std of 0.03 and
-    amplifies the decoder-output deviation (4e-4, bf16 recurrence GEMMs) ~30x. The 'fp32-class' mode runs the convolution stacks on
-    bf16 hi + lo operand pairs with fp32 pre-norm activations and removes (i) - mel-L1 halves to ~1.2e-2; (ii) remains because the
-    recurrences keep bf16 operands (a split-operand decoder is not implemented; DESIGN.md §4c). Asserted: the measured values with
-    2x margin, alignments / decoder output / losses unchanged or better."""
+    bf16 mode: ~2.5e-2 at random init (bound 5e-2). Two contributions (tools/taco_layer_diag.py): (i) every batch-normalised postnet
+    layer adds ~0.2 % of a unit-variance activation through bf16 storage of operands / activations; (ii) at random init the decoder
+    outputs are nearly constant over (batch, time) (per-channel std 0.06), so the FIRST postnet batch norm divides by a pre-norm std of
+    0.03 and amplifies the decoder-output deviation (bf16 recurrence GEMMs) ~30x. The 'fp32-class' mode carries every operand of the
+    forward as a bf16 hi + lo pair - the convolution stacks, the encoder and decoder recurrences, the attention and the projections -
+    and removes both: asserted at the parity target mel-L1 <= 1e-3 and below a tenth of the bf16 mode's, with alignments / decoder
+    output no worse."""
     from hparams import hparams as hp0
     hp = hp0.copy()
     hp.parse("predict_linear=False" + ("" if stochastic else ",tacotron_dropout_rate=0.0,tacotron_zoneout_rate=0.0"))
     tol = dict(align=6e-4, dec_l1=1.6e-3, stop=5e-3, loss=2e-3, grad_rel=1.0, grad_cos=0.0)
     tag = "tacotron_precision_modes_%s_" % ("stochastic" if stochastic else "deterministic")
-    a = taco_compare(tag + "fp32_class", hp, 32, 160, 200, 54, dict(tol, mel_l1=2.5e-2), backward=False, precision="fp32-class").measured
+    a = taco_compare(tag + "fp32_class", hp, 32, 160, 200, 54, dict(tol, mel_l1=1e-3), backward=False, precision="fp32-class").measured
     b = taco_compare(tag + "bf16", hp, 32, 160, 200, 54, dict(tol, mel_l1=5e-2), backward=False, precision="bf16").measured
-    assert a["mel_l1"] <= 0.7 * b["mel_l1"], (a["mel_l1"], b["mel_l1"])
+    assert a["mel_l1"] <= 0.1 * b["mel_l1"], (a["mel_l1"], b["mel_l1"])
     assert a["dec_l1"] <= b["dec_l1"] * 1.05 and a["align_max_err"] <= b["align_max_err"] * 1.5
 
 

@@ -30,7 +30,8 @@ still be NaN (or exactly 0 where the kernel promises it), and NaN in the unread 
 COVERAGE maps every __global__ kernel of the two files and of the kernels they share (t2_params.cu, t2_batchnorm.cu) to the test here that
 launches it (the shared batch-norm kernels are launched by both the Tacotron and the CBHG batch-norm tests);
 a COVERAGE value is either the name of a test here or `file::test` for a per-kernel test in another module (att_bwd_kernel:
-tests/test_attention_state_gpu.py; the two GRU kernels: tests/test_cbhg_gru_gpu.py). EXEMPT names the existing end-to-end test that covers
+tests/test_attention_state_gpu.py; the two GRU kernels: tests/test_cbhg_gru_gpu.py; the split row writers:
+tests/test_split_operands_gpu.py). EXEMPT names the existing end-to-end test that covers
 each plumbing kernel (packing, embedding, losses, column sums).
 test_every_engine_and_shared_kernel_is_covered (CPU) fails for a kernel added without an entry."""
 import ctypes
@@ -67,18 +68,20 @@ COVERAGE = {
     "lstm_cell_bwd_kernel": "test_lstm_cell_bwd", "att_finish_kernel": "test_att_finish", "att_finish2_kernel": "test_att_finish",
     "dvalues_ctx_kernel": "test_dvalues_ctx", "att_bwd_kernel": "test_attention_state_gpu.py::test_att_bwd",
     "gru_fwd_kernel": "test_cbhg_gru_gpu.py::test_gru_fwd", "gru_bwd_kernel": "test_cbhg_gru_gpu.py::test_gru_bwd",
+    "embed_fwd_kernel": "test_split_operands_gpu.py::test_embed_fwd_split", "decin_kernel": "test_split_operands_gpu.py::test_decin_split",
+    "dec_finish_kernel": "test_split_operands_gpu.py::test_dec_finish_split",
+    "proj_bias_feedback_kernel": "test_split_operands_gpu.py::test_proj_bias_feedback_split",
+    "f32_to_bf16_kernel": "test_split_operands_gpu.py::test_f32_to_bf16_split",
 }
 _TACO_E2E = "test_tacotron_gpu.py::test_backward_matches_oracle"
 _CBHG_E2E = "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle"
 EXEMPT = {
-    "pack_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "embed_fwd_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
+    "pack_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
     "embed_bwd_kernel": _TACO_E2E, "bias_colsum_kernel": _TACO_E2E, "mask_values_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
-    "decin_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "dec_finish_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
     "mel_finish_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "reg_loss_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
     "proj_bias_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "loss_norm_kernel": "test_tacotron_gpu.py::test_masked_decoder_losses_match_oracle",
     "loss_seed_kernel": _TACO_E2E, "ddec_tm_kernel": _TACO_E2E, "relu_drop_bwd_kernel": "test_parity_full_gpu.py::test_tacotron_training_mode_stochastic_paths_small",
-    "f32_to_bf16_kernel": _CBHG_E2E, "reg_grad_kernel": _TACO_E2E,
-    "proj_bias_feedback_kernel": "test_tacotron_gpu.py::test_free_running_synthesis_matches_oracle",
+    "reg_grad_kernel": _TACO_E2E,
     "add_k": _CBHG_E2E, "lin_finish_k": _CBHG_E2E,
     "lin_norm_k": "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle", "loss_out_k": _CBHG_E2E, "dmel_k": _CBHG_E2E,
 }
