@@ -239,8 +239,10 @@ typedef struct {
   float log_scale_min_gauss; /* single-Gaussian head (out_channels == 2): clamp of the predicted log-scale (hparams.py:196) */
   int cdf_loss;              /* Gaussian head: 1 = log(CDF+ - CDF-) loss, 0 = log-density (gaussian.py:18-33) */
   int split_bf16;            /* 1 = "fp32-class" forward: activations and weights travel as bf16 hi + lo pairs (3 tensor-core products per
-                              * contraction, fp32 accumulate; ~2^-17 relative operand error instead of 2^-9). Forward / loss only, dropout 0:
-                              * the parity mode that shows the bf16-mode deviation from the reference's fp32 graph is storage rounding. */
+                              * contraction, fp32 accumulate; ~2^-17 relative operand error instead of 2^-9). Forward / loss and AR synthesis
+                              * only, dropout 0: the parity mode that shows the bf16-mode deviation from the reference's fp32 graph is storage
+                              * rounding. In AR synthesis (t2_wn_ar_*) it stores the synthesis weights as plain fp32 and reads the conditioning
+                              * in fp32 (CUDA-core FMA: exact products without a hi + lo pair). */
   int gin_channels;          /* global (speaker) conditioning: width of the speaker embedding (wavenet.py:151-158), 0 = off */
   int n_speakers;            /* rows of gc_embedding (>= 1 when gin_channels > 0) */
   int upsample_activation;   /* after each learnable upsampling layer (wavenet.py:197-203): 0 ReLU, 1 LeakyReLU max(alpha x, x), 2 none */
@@ -370,10 +372,13 @@ int t2_dbg_wn_kernel(const t2_dbg_kernel_t* call, void* stream);
  * (modules.py:273-303) and sample_from_discretized_mix_logistic (mixture.py:76-107). cfg->B = synthesis batch,
  * cfg->T = samples to generate. cluster_size in {1,2,4,8,16}: CTAs per thread-block cluster sharing one batch group. */
 int t2_wn_ar_sizes(const t2_wn_config_t* cfg, int cluster_size, long long* packed_bytes, long long* workspace_bytes);
-/* fp32 masters -> slice-major bf16 synthesis weights + ring tables; run once per checkpoint; synchronises */
+/* fp32 masters -> slice-major synthesis weights (bf16, or fp32 when cfg->split_bf16 = 1: packed_bytes then holds 4 bytes per weight)
+ * + ring tables; run once per checkpoint; synchronises */
 int t2_wn_ar_pack(const t2_wn_config_t* cfg, int cluster_size, const float* d_params, void* d_packed_ar,
                   void* d_workspace, void* stream);
 /* d_c: fp32 [B,cin,Tc] (feeder-normalised mels); d_initial: int32[B] (mu-law index, 127 = silence) or fp32[B];
+ * conditioning: cfg->split_bf16 = 0 rounds the upsampled conditioning to a bf16 [B,T,cin] workspace copy; = 1 reads it in fp32 where it
+ * lies - d_c [B,T,cin] itself when c_pre_upsampled, else the last upsampling layer's fp32 output [B,cin,T] in the workspace;
  * d_test_inputs: NULL or int32/fp32 [B,T] teacher-forcing inputs (the reference's wavenet_synth_debug path);
  * d_u_a / d_u_b: NULL (on-device counter RNG from `seed`) or injected uniforms in (0,1): MoL d_u_a [B,T,nr_mix] mixture
  * selection and d_u_b [B,T] logistic draw; mu-law d_u_a [B,T]. d_out_samples: int32 / fp32 [B,T];

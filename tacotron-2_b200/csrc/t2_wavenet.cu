@@ -2108,13 +2108,14 @@ constexpr int kArMaxItems = 4;
 
 struct ArLayout {
   int CS, ZC, RC, SC, FC, OC, K1;
-  long long per_rank_layer;        // bf16 elements per (layer, rank): 2*ZC*K1 + (RC+SC)*Gh
+  int esize;                       // bytes per stored weight: 2 (bf16), or 4 (fp32) in the fp32-class mode (split_bf16)
+  long long per_rank_layer;        // weight elements per (layer, rank): 2*ZC*K1 + (RC+SC)*Gh
   long long o_head1, o_head2;      // element offsets of the head blocks (after all layers)
-  long long n_weights;             // bf16 elements
+  long long n_weights;             // weight elements
   long long o_bias;                // byte offset of the fp32 bias block
   long long packed_bytes;
   long long ring_slots_total;      // sum over layers of slots
-  long long workspace_bytes, w_cup, w_upout_base, w_ring, w_ringoff;
+  long long workspace_bytes, w_cup, w_upout_base, w_ring, w_ringoff;   // w_cup: bf16 mode only (-1 in the fp32-class mode)
   long long w_gbias;               // Gi > 0: fp32 [B][L][G] per-item gate biases (t2_wn_ar_set_speakers), else -1
   std::vector<int> ring_slots, ring_off;
 };
@@ -2128,7 +2129,8 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
   a.o_head1 = a.per_rank_layer * CS * lo.L;
   a.o_head2 = a.o_head1 + (long long)CS * a.FC * lo.S;
   a.n_weights = a.o_head2 + (long long)CS * a.OC * lo.S;
-  a.o_bias = align_up(a.n_weights * 2, 256);
+  a.esize = lo.split ? 4 : 2;
+  a.o_bias = align_up(a.n_weights * a.esize, 256);
   // biases fp32: per layer [G gate | R out], then skip_total [S], f1 [S], f2 [O padded to CS*OC]
   a.packed_bytes = a.o_bias + 4LL * ((long long)lo.L * (lo.G + lo.R) + 2 * lo.S + CS * a.OC);
   a.ring_slots.clear(); a.ring_off.clear();
@@ -2143,7 +2145,8 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
   a.ring_slots_total = off;
   Arena ws;
   const long long BT = (long long)lo.B * lo.T;
-  a.w_cup = ws.take(BT * (lo.C > 0 ? lo.C : 8) * 2);
+  // the fp32-class mode reads the fp32 conditioning where it lies (d_c, or the last upsampling layer's output): no c_up copy
+  a.w_cup = lo.split ? -1 : ws.take(BT * (lo.C > 0 ? lo.C : 8) * 2);
   a.w_upout_base = ws.used;
   for (size_t i = 0; i < lo.up_w.size(); ++i) ws.take((long long)lo.B * lo.C * lo.up_w[i] * 4);
   a.w_ring = ws.take((long long)lo.B * off * lo.R * 4);
@@ -2155,13 +2158,17 @@ int build_ar_layout(const Layout& lo, int CS, ArLayout& a) {
 
 struct ArPackArgs {
   const float* params;
-  bf16* w;
+  void* w;                 // WT (bf16, or fp32 in the fp32-class mode) [n_weights], slice-major
   float* bias;
   const long long* offs;   // per layer: dil_k, dil_b, c_k, c_b, s_k, s_b, o_k, o_b  (8 per layer); then f1_k,f1_b,f2_k,f2_b
   const float* skip_scale;
   int L, R, G, Gh, S, C, O, CS, ZC, RC, SC, FC, OC, K1;
   long long per_rank_layer, o_head1, o_head2, n_weights;
 };
+__device__ __forceinline__ void ar_store(bf16* p, float v) { *p = __float2bfloat16(v); }
+__device__ __forceinline__ void ar_store(float* p, float v) { *p = v; }
+
+template <typename WT>
 __global__ void ar_pack_kernel(ArPackArgs a) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e < a.n_weights) {
@@ -2192,7 +2199,7 @@ __global__ void ar_pack_kernel(ArPackArgs a) {
       const int row = int(i / a.S), k = int(i % a.S);
       if (row < a.O) v = a.params[a.offs[8 * a.L + 2] + (long long)k * a.O + row];
     }
-    a.w[e] = __float2bfloat16(v);
+    ar_store(static_cast<WT*>(a.w) + e, v);
   }
   // biases
   const long long nb = (long long)a.L * (a.G + a.R) + 2 * a.S + a.CS * a.OC;
@@ -2218,12 +2225,12 @@ __global__ void ar_pack_kernel(ArPackArgs a) {
 }
 
 struct ArArgs {
-  const bf16* w;            // slice-major weights
+  const void* w;            // slice-major weights, WT (bf16, or fp32 in the fp32-class mode)
   const float* bias;
   const float* gbias;       // nullable: per-item gate biases [B][L][G] replacing the shared gate rows of `bias` (speaker conditioning)
   const float* in_k;        // input_convolution kernel fp32 [cin][R]
   const float* in_b;
-  const bf16* c_up;         // [B][T][C]
+  const void* c_up;         // bf16 mode: bf16 [B][T][C]; fp32-class mode: fp32, element (b, t, ch) at b*c_sb + t*c_st + ch*c_sc
   float* ring;              // [B][ring_slots_total][R]
   const int* ring_off;      // [L] then ring_slots [L]
   const void* initial;      // int32 [B] or f32 [B]
@@ -2239,18 +2246,53 @@ struct ArArgs {
   float res_scale, log_scale_min, log_scale_min_gauss;
   int items_per_cluster;
   int prefetch;             // 1: this CTA's per-layer weight slice is double-buffered in shared memory (bulk async copies)
+  long long c_sb, c_st, c_sc;   // fp32-class mode: element strides of the fp32 conditioning (item, time, channel)
 };
 
 // y[it][o] = sum_k W[o][k] * x[it][k] for o in [0, nout): all outputs of a pass run side by side - a group of GS lanes
 // (GS = 512 / nout rounded down to a power of two, <= 32) owns one output row and strides its 16-byte chunks, the partial
 // sums meet in log2(GS) shuffles. (The warp-per-output form serialised 2 rows x 5 shuffle levels x NI per warp.)
-template <int NI>
-__device__ __forceinline__ void ar_matvec(const bf16* __restrict__ W, int nout, int K, const float* __restrict__ x /*[NI][ldx]*/,
+// WT: stored weight type; a 16-byte chunk holds 8 bf16 weights or 4 fp32 weights (the fp32-class mode: exact fp32 products).
+template <int NI, typename WT>
+__device__ __forceinline__ void ar_matvec(const WT* __restrict__ W, int nout, int K, const float* __restrict__ x /*[NI][ldx]*/,
                                           int ldx, float* __restrict__ y /*[NI][ldy]*/, int ldy, int ni) {
   int gs = 32;
   while (gs > 1 && gs * nout > kArThreads) gs >>= 1;
   const int per_pass = kArThreads / gs;
   const int sub = threadIdx.x % gs;
+  if constexpr (sizeof(WT) == 4) {
+    const int nchunk = K >> 2;
+    for (int o0 = 0; o0 < nout; o0 += per_pass) {
+      const int o = o0 + threadIdx.x / gs;
+      const bool live = o < nout;
+      float acc[NI];
+#pragma unroll
+      for (int it = 0; it < NI; ++it) acc[it] = 0.f;
+      if (live) {
+        const float4* wr = reinterpret_cast<const float4*>(W + (size_t)o * K);
+#pragma unroll 2
+        for (int c = sub; c < nchunk; c += gs) {
+          const float4 w = wr[c];
+#pragma unroll
+          for (int it = 0; it < NI; ++it) {
+            if (it < ni) {
+              const float4 p = *reinterpret_cast<const float4*>(x + it * ldx + c * 4);
+              acc[it] += w.x * p.x + w.y * p.y + w.z * p.z + w.w * p.w;
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int it = 0; it < NI; ++it) {
+        if (it < ni) {
+          float v = acc[it];
+          for (int m = gs >> 1; m > 0; m >>= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
+          if (live && sub == 0) y[it * ldy + o] = v;
+        }
+      }
+    }
+    return;
+  }
   const int nchunk = K >> 3;
   for (int o0 = 0; o0 < nout; o0 += per_pass) {
     const int o = o0 + threadIdx.x / gs;
@@ -2286,8 +2328,9 @@ __device__ __forceinline__ void ar_matvec(const bf16* __restrict__ W, int nout, 
   }
 }
 
-// NT: past taps of the dilated convolution (kernel_size - 1), read from the ring; the last tap is the current x
-template <int NI, int NT>
+// NT: past taps of the dilated convolution (kernel_size - 1), read from the ring; the last tap is the current x.
+// WT: stored weight type, bf16 or fp32 (the fp32-class mode, which also reads its conditioning in fp32).
+template <int NI, int NT, typename WT>
 __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = int(cluster.block_rank());
@@ -2312,10 +2355,10 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   float* cvec = bsl + a.L * nbs;                    // [NI][C]    : conditioning frame of the current step
   int* rofs = reinterpret_cast<int*>(cvec + NI * ((a.C + 3) & ~3));   // [2L+1] ring offsets / slots / total
   float* cur = reinterpret_cast<float*>(rofs + ((2 * a.L + 1 + 3) & ~3));   // [NI] current input sample (scalar) or index
-  // weight prefetch: two slots of per_rank_layer bf16 + two mbarriers behind the activation buffers (16-byte aligned)
+  // weight prefetch: two slots of per_rank_layer WT + two mbarriers behind the activation buffers (16-byte aligned)
   uint64_t* wbar = reinterpret_cast<uint64_t*>((reinterpret_cast<uintptr_t>(cur + NI) + 15) & ~uintptr_t(15));
-  bf16* wslot = reinterpret_cast<bf16*>(wbar + 2);
-  const uint32_t wbytes = uint32_t(a.per_rank_layer * 2);
+  WT* wslot = reinterpret_cast<WT*>(wbar + 2);
+  const uint32_t wbytes = uint32_t(a.per_rank_layer * (long long)sizeof(WT));
   const int tid = threadIdx.x;
   if (a.prefetch && tid == 0) {
     mbar_init(&wbar[0], 1); mbar_init(&wbar[1], 1);
@@ -2339,7 +2382,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   __syncthreads();
   if (a.prefetch && tid == 0) {   // slice of layer 0 -> slot 0
     mbar_expect_tx(&wbar[0], wbytes);
-    bulk_load_1d(wslot, a.w + (long long)rank * a.per_rank_layer, wbytes, &wbar[0]);
+    bulk_load_1d(wslot, static_cast<const WT*>(a.w) + (long long)rank * a.per_rank_layer, wbytes, &wbar[0]);
   }
   uint32_t wphase = 0;            // bit s = parity to wait for on slot s
   long long seq = 0;              // (t, l) sequence number: slot = seq & 1
@@ -2375,8 +2418,14 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
       xbuf[it * a.R + r] = v;
     }
     for (int i = tid; i < ni * a.SC; i += kArThreads) skip[i] = 0.f;
-    for (int i = tid; i < ni * a.C; i += kArThreads)     // conditioning frame of this step, once (not once per layer)
-      cvec[(i / a.C) * ((a.C + 3) & ~3) + i % a.C] = __bfloat162float(a.c_up[((long long)(item0 + i / a.C) * a.T + t) * a.C + i % a.C]);
+    for (int i = tid; i < ni * a.C; i += kArThreads) {   // conditioning frame of this step, once (not once per layer)
+      if constexpr (sizeof(WT) == 4)
+        cvec[(i / a.C) * ((a.C + 3) & ~3) + i % a.C] =
+            static_cast<const float*>(a.c_up)[(item0 + i / a.C) * a.c_sb + t * a.c_st + (i % a.C) * a.c_sc];
+      else
+        cvec[(i / a.C) * ((a.C + 3) & ~3) + i % a.C] =
+            __bfloat162float(static_cast<const bf16*>(a.c_up)[((long long)(item0 + i / a.C) * a.T + t) * a.C + i % a.C]);
+    }
     __syncthreads();
     for (int l = 0; l < a.L; ++l) {
       const int slots = rofs[a.L + l];
@@ -2404,7 +2453,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
           a.ring[((long long)(item0 + it) * rofs[2 * a.L] + roff + (t & (slots - 1))) * a.R + r] = xbuf[i];
         }
       // ---- stage 1: gate pre-activations for this CTA's ZC z-channels (a rows then b rows) ----
-      const bf16* w1 = a.w + ((long long)l * a.CS + rank) * a.per_rank_layer;
+      const WT* w1 = static_cast<const WT*>(a.w) + ((long long)l * a.CS + rank) * a.per_rank_layer;
       if (a.prefetch) {
         const int slot = int(seq & 1);
         mbar_wait(&wbar[slot], (wphase >> slot) & 1u);       // this layer's slice has landed
@@ -2413,7 +2462,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
         if (tid == 0 && (t + 1 < a.T || l + 1 < a.L)) {      // next layer's slice -> the other slot (free since the last cluster.sync)
           const int ln = l + 1 < a.L ? l + 1 : 0;
           mbar_expect_tx(&wbar[slot ^ 1], wbytes);
-          bulk_load_1d(wslot + (long long)(slot ^ 1) * a.per_rank_layer, a.w + ((long long)ln * a.CS + rank) * a.per_rank_layer, wbytes,
+          bulk_load_1d(wslot + (long long)(slot ^ 1) * a.per_rank_layer, static_cast<const WT*>(a.w) + ((long long)ln * a.CS + rank) * a.per_rank_layer, wbytes,
                        &wbar[slot ^ 1]);
         }
       }
@@ -2449,7 +2498,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
       }
       __syncthreads();
       // ---- stage 2: this CTA's RC residual-out channels and SC skip channels ----
-      const bf16* w2 = w1 + 2LL * a.ZC * a.K1;
+      const WT* w2 = w1 + 2LL * a.ZC * a.K1;
       ar_matvec<NI>(w2, a.RC + a.SC, a.Gh, zbuf, a.Gh, loc, a.RC + a.SC, ni);
       __syncthreads();
       AR_STAMP(6);
@@ -2479,7 +2528,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
       for (int r = 0; r < a.CS; ++r) cluster.map_shared_rank(hbuf, r)[it * a.S + ch] = v;
     }
     cluster.sync();
-    ar_matvec<NI>(a.w + a.o_head1 + (long long)rank * a.FC * a.S, a.FC, a.S, hbuf, a.S, loc, a.FC, ni);
+    ar_matvec<NI>(static_cast<const WT*>(a.w) + a.o_head1 + (long long)rank * a.FC * a.S, a.FC, a.S, hbuf, a.S, loc, a.FC, ni);
     __syncthreads();
     cluster.sync();   // every CTA has finished reading hbuf (h1) before it is overwritten with h2
     for (int i = tid; i < ni * a.FC; i += kArThreads) {
@@ -2488,7 +2537,7 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
       for (int r = 0; r < a.CS; ++r) cluster.map_shared_rank(hbuf, r)[it * a.S + ch] = v;
     }
     cluster.sync();
-    ar_matvec<NI>(a.w + a.o_head2 + (long long)rank * a.OC * a.S, a.OC, a.S, hbuf, a.S, loc, a.OC, ni);
+    ar_matvec<NI>(static_cast<const WT*>(a.w) + a.o_head2 + (long long)rank * a.OC * a.S, a.OC, a.S, hbuf, a.S, loc, a.OC, ni);
     __syncthreads();
     for (int i = tid; i < ni * a.OC; i += kArThreads) {
       const int it = i / a.OC, j = i % a.OC, ch = rank * a.OC + j;
@@ -2576,10 +2625,14 @@ __global__ void __launch_bounds__(kArThreads, 1) wn_ar_kernel(ArArgs a) {
   }
 }
 
-// the instantiation for NIt items per cluster pass and NT past taps
-template <int NT>
+// the instantiation for NIt items per cluster pass, NT past taps and stored weight type WT
+template <int NT, typename WT>
 void (*ar_kernel(int NIt))(ArArgs) {
-  return NIt == 1 ? wn_ar_kernel<1, NT> : (NIt == 2 ? wn_ar_kernel<2, NT> : wn_ar_kernel<kArMaxItems, NT>);
+  return NIt == 1 ? wn_ar_kernel<1, NT, WT> : (NIt == 2 ? wn_ar_kernel<2, NT, WT> : wn_ar_kernel<kArMaxItems, NT, WT>);
+}
+template <typename WT>
+void (*ar_kernel_kw(int kw, int NIt))(ArArgs) {
+  return kw == 2 ? ar_kernel<1, WT>(NIt) : kw == 3 ? ar_kernel<2, WT>(NIt) : ar_kernel<3, WT>(NIt);
 }
 
 }  // namespace
@@ -2617,6 +2670,7 @@ extern "C" int t2_wn_ar_pack(const t2_wn_config_t* cfg, int cluster_size, const 
   ArLayout a;
   rc = build_ar_layout(lo, cluster_size, a);
   if (rc) return rc;
+  T2_REQUIRE(d_params && d_packed_ar && d_workspace, T2_ERR_INVALID_ARG, "t2_wn_ar_pack: null buffer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   std::vector<long long> offs(8 * lo.L + 4);
   for (int l = 0; l < lo.L; ++l) {
@@ -2633,13 +2687,15 @@ extern "C" int t2_wn_ar_pack(const t2_wn_config_t* cfg, int cluster_size, const 
   T2_CHECK_CUDA(cudaMemcpyAsync(d_offs, offs.data(), offs.size() * sizeof(long long), cudaMemcpyHostToDevice, st));
   T2_CHECK_CUDA(cudaMemcpyAsync(d_scale, lo.skip_scale.data(), lo.L * sizeof(float), cudaMemcpyHostToDevice, st));
   ArPackArgs p;
-  p.params = d_params; p.w = static_cast<bf16*>(d_packed_ar);
+  p.params = d_params; p.w = d_packed_ar;
   p.bias = reinterpret_cast<float*>(static_cast<uint8_t*>(d_packed_ar) + a.o_bias);
   p.offs = d_offs; p.skip_scale = d_scale;
   p.L = lo.L; p.R = lo.R; p.G = lo.G; p.Gh = lo.Gh; p.S = lo.S; p.C = lo.C; p.O = lo.O; p.CS = a.CS; p.ZC = a.ZC; p.RC = a.RC;
   p.SC = a.SC; p.FC = a.FC; p.OC = a.OC; p.K1 = a.K1; p.per_rank_layer = a.per_rank_layer; p.o_head1 = a.o_head1;
   p.o_head2 = a.o_head2; p.n_weights = a.n_weights;
-  ar_pack_kernel<<<grid1d(a.n_weights), 256, 0, st>>>(p); t2_count_launch();
+  if (lo.split) ar_pack_kernel<float><<<grid1d(a.n_weights), 256, 0, st>>>(p);
+  else ar_pack_kernel<bf16><<<grid1d(a.n_weights), 256, 0, st>>>(p);
+  t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   // ring tables
   std::vector<int> rt(2 * lo.L + 1);
@@ -2687,14 +2743,18 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
   if (rc) return rc;
   T2_REQUIRE(lo.C > 0, T2_ERR_UNSUPPORTED_SHAPE, "AR synthesis needs local conditioning");
   T2_REQUIRE(lo.R <= lo.S, T2_ERR_UNSUPPORTED_SHAPE, "AR synthesis needs residual_channels <= skip_out_channels");
+  T2_REQUIRE(d_params && d_packed_ar && d_workspace && d_c && d_initial && d_out_samples, T2_ERR_INVALID_ARG,
+             "t2_wn_ar_generate: null buffer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   const uint8_t* pk = static_cast<const uint8_t*>(d_packed_ar);
   const long long BT = (long long)lo.B * lo.T;
-  // conditioning -> c_up (bf16 channels-last), same kernels as the training path
-  bf16* c_up = reinterpret_cast<bf16*>(ws + al.w_cup);
+  // conditioning -> c_up (bf16 channels-last), same kernels as the training path. The fp32-class mode reads the fp32 conditioning
+  // in place instead: d_c [B][T][C] when pre-upsampled, else the last upsampling layer's output [B][C][T]
+  bf16* c_up = lo.split ? nullptr : reinterpret_cast<bf16*>(ws + al.w_cup);
+  const float* c32 = d_c;
   if (cfg->c_pre_upsampled) {
-    launch_f32_to_bf16(d_c, c_up, BT * lo.C, st);
+    if (!lo.split) launch_f32_to_bf16(d_c, c_up, BT * lo.C, st);
   } else {
     const float* in = d_c;
     int W = lo.Tc;
@@ -2710,15 +2770,22 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
       in = out;
       W *= s;
     }
+    c32 = in;
   }
   T2_CHECK_CUDA(cudaGetLastError());
   ArArgs a;
   memset(&a, 0, sizeof(a));
-  a.w = reinterpret_cast<const bf16*>(pk);
+  a.w = pk;
   a.bias = reinterpret_cast<const float*>(pk + al.o_bias);
   a.gbias = lo.Gi > 0 ? reinterpret_cast<const float*>(ws + al.w_gbias) : nullptr;
   a.in_k = d_params + lo.p_in_k; a.in_b = d_params + lo.p_in_b;
-  a.c_up = c_up;
+  if (lo.split) {
+    a.c_up = c32;
+    const bool cl = cfg->c_pre_upsampled != 0;
+    a.c_sb = (long long)lo.T * lo.C; a.c_st = cl ? lo.C : 1; a.c_sc = cl ? 1 : lo.T;
+  } else {
+    a.c_up = c_up;
+  }
   a.ring = reinterpret_cast<float*>(ws + al.w_ring);
   a.ring_off = reinterpret_cast<const int*>(ws + al.w_ringoff);
   a.initial = d_initial; a.test_inputs = d_test_inputs; a.u_a = d_u_a; a.u_b = d_u_b;
@@ -2746,12 +2813,13 @@ extern "C" int t2_wn_ar_generate(const t2_wn_config_t* cfg, int cluster_size, co
   size_t smem = sizeof(float) * (size_t(NIt) * (ld1 + lo.Gh + lo.R + al.ZC + al.RC + locw + al.SC + lo.S + al.CS * al.OC + ((lo.C + 3) & ~3) + 1) +
                                  size_t(lo.L) * (2 * al.ZC + al.RC) + ((2 * lo.L + 1 + 3) & ~3)) + 64;
   // double-buffered shared-memory copy of this CTA's per-layer weight slice when it fits next to the activations
-  // (paper widths: 70.6 KB per slice at cluster size 16); otherwise the slices stream from L2 as before
-  const size_t wslots = 2 * size_t(al.per_rank_layer) * 2 + 64;
-  a.prefetch = (al.per_rank_layer % 8 == 0 && smem + wslots <= 232448 - 1024) ? 1 : 0;
+  // (paper widths at cluster size 16: 70.6 KB per bf16 slice; the fp32 slices, 141 KB, do not fit twice); otherwise the slices
+  // stream from L2 as before
+  const size_t wslots = 2 * size_t(al.per_rank_layer) * al.esize + 64;
+  a.prefetch = ((al.per_rank_layer * al.esize) % 16 == 0 && smem + wslots <= 232448 - 1024) ? 1 : 0;
   if (const char* e = getenv("T2_AR_PREFETCH")) { if (e[0] == '0') a.prefetch = 0; }
   if (a.prefetch) smem += wslots;
-  void (*kern)(ArArgs) = lo.kw == 2 ? ar_kernel<1>(NIt) : lo.kw == 3 ? ar_kernel<2>(NIt) : ar_kernel<3>(NIt);
+  void (*kern)(ArArgs) = lo.split ? ar_kernel_kw<float>(lo.kw, NIt) : ar_kernel_kw<bf16>(lo.kw, NIt);
   T2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   if (al.CS > 8) T2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   T2_CHECK_CUDA(cudaMemsetAsync(ws + al.w_ring, 0, (size_t)lo.B * al.ring_slots_total * lo.R * 4, st));

@@ -448,11 +448,14 @@ class WaveNet(object):
 class WaveNetSynthesizer(object):
     """Fast-WaveNet autoregressive generation on the H100 (wavenet_vocoder/synthesizer.py + WaveNet.incremental)."""
 
-    def __init__(self, hparams, B, T, cluster_size=8, device="cuda"):
+    def __init__(self, hparams, B, T, cluster_size=8, device="cuda", precision="bf16"):
+        """precision: 'bf16' (synthesis weights and conditioning stored in bf16, fp32 arithmetic) or 'fp32-class' (fp32 weights and
+        conditioning: the raw outputs differ from the fp32 network only by fp32 accumulation order)."""
         self.hp = hparams
         self.lib = L.load()
         self.device = torch.device(device)
-        self.cfg = make_config(hparams, B, T, False, 0.0)
+        self.precision = precision
+        self.cfg = make_config(hparams, B, T, False, 0.0, precision)
         self.cs = cluster_size
         sz = WnSizes()
         L.check(self.lib.t2_wn_sizes(ctypes.byref(self.cfg), ctypes.byref(sz)))

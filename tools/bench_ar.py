@@ -6,14 +6,14 @@ import torch
 from hparams import hparams
 from t2_import import t2
 
-def run(input_type, B, cs, T=22000):
+def run(input_type, B, cs, T=22000, precision="bf16"):
     hp = hparams.copy()
     hp.parse("layers=24,stacks=4,residual_channels=256,gate_channels=512,skip_out_channels=256,upsample_scales=[11,25]")
     if input_type == "mulaw-quantize":
         hp.parse("input_type=mulaw-quantize,quantize_channels=256,out_channels=256")
     else:
         hp.parse("input_type=raw,quantize_channels=65536,out_channels=30")
-    syn = t2.wavenet.WaveNetSynthesizer(hp, B, T, cluster_size=cs)
+    syn = t2.wavenet.WaveNetSynthesizer(hp, B, T, cluster_size=cs, precision=precision)
     syn.init_variables(seed=5)
     c = torch.rand(B, 80, T // 275, device="cuda")
     init = (torch.full((B,), 127, dtype=torch.int32) if input_type == "mulaw-quantize" else torch.zeros(B)).cuda()
