@@ -151,7 +151,7 @@ typedef struct {
 #define T2_DBG_TACO_ATT_FINISH 5
 #define T2_DBG_TACO_DVALUES 6
 #define T2_DBG_TACO_ATT_BWD 7
-/* CONV_GEMM   conv_gemm: a k-tap 'same' convolution / projection through the GEMM engine and EPI_BIAS_ACT, tap j reading row
+/* CONV_GEMM   launch_bias_act: a k-tap 'same' convolution / projection through the GEMM engine and EPI_BIAS_ACT, tap j reading row
  *             t + conv_tap_shift(ntaps, j) of the same item. p: a bf16 [Bn][T][C] (split: [Bn][T][hi(Cp) | lo(Cp)], Cp = C rounded up
  *             to 64), packed weight bf16 [N][wK] (split: [W_hi | W_hi | W_lo] per tap, wK >= 3 ntaps Cp), bias fp32 [N] (nullable),
  *             out bf16 [Bn T][ldo] (split: [hi(ldo) | lo(ldo)], pitch 2 ldo; nullable), out fp32 [Bn T][ldo] (nullable; one of the two

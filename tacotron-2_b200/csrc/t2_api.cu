@@ -34,18 +34,10 @@ extern "C" int t2_dbg_conv_gemm(const void* a, int B, int T, int C, int ld, cons
   using namespace t2;
   T2_REQUIRE(nshift >= 1 && nshift <= kMaxSeg, T2_ERR_INVALID_ARG, "nshift out of range");
   T2_REQUIRE(BN == 128 || BN == 256, T2_ERR_UNSUPPORTED_SHAPE, "BN must be 128 or 256");
-  ActGemmCall c;
-  memset(&c, 0, sizeof(c));
-  c.a[0] = make_act(a, C, T, B, 1, ld);
-  c.na = 1;
   const int nkb = (C + kBK - 1) / kBK;
-  for (int s = 0; s < nshift; ++s) c.seg[s] = Seg{0, shifts[s], 0, nkb, 0, 1};
-  c.nseg = nshift;
-  c.w = w; c.wN = N; c.wK = nshift * nkb * kBK; c.wL = 1; c.w_layer = 0;
-  c.T = T; c.B = B; c.n_tiles = (N + BN - 1) / BN;
-  c.epi.ptr[0] = out_bf16; c.epi.ptr[1] = const_cast<float*>(bias); c.epi.ptr[2] = out_f32;
-  c.epi.i[0] = N; c.epi.i[1] = relu; c.epi.i[2] = N;
-  return launch_act_gemm(EPI_BIAS_ACT, BN, c, static_cast<cudaStream_t>(stream));
+  return launch_bias_act({.a = a, .C = C, .ld = ld, .T = T, .B = B, .ntaps = nshift, .shifts = shifts, .w = w, .N = N, .wK = nshift * nkb * kBK,
+                          .BN = BN, .bias = bias, .act = relu, .out_bf16 = out_bf16, .out_f32 = out_f32, .ldo = N, .nvalid = N},
+                         static_cast<cudaStream_t>(stream));
 }
 
 // dW[m, n] = scale * sum_{b,t} A[b, t + shift_a, m] * Bm[b, t, n]   (fp32 out [Ca, Cb])

@@ -115,7 +115,7 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   lo.p_lk = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/kernel", {2 * lo.RU, lo.NF}); lo.p_lb = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/bias", {lo.NF});
 
   // ---- packed operands ----
-  // split_bf16: every forward operand is [W_hi | W_hi | W_lo] per K slot (add_pack_split; set_split_operand in t2_gemm.h), so its
+  // split_bf16: every forward operand is [W_hi | W_hi | W_lo] per K slot (add_pack_split; the split operand of launch_bias_act, t2_gemm.h), so its
   // K pitch triples; the data-gradient operands of the backward pass keep their bf16 layout
   const bool split = cfg->split_bf16 != 0;
   const int s3 = split ? 3 : 1;
@@ -613,30 +613,6 @@ __global__ void __launch_bounds__(kGruThreads, 1) gru_bwd_kernel(GruBwdArgs a) {
 // ------------------------------------------------------------------------------------------------------
 // host helpers
 // ------------------------------------------------------------------------------------------------------
-// out[pos][n] = act(sum_taps sum_k a[pos + shift][k0 + k] w[n][tap * Cp + k] + bias[n]) on the wgmma engine (EPI_BIAS_ACT)
-// split: `a` is a split-bf16 operand (set_split_operand, t2_gemm.h: ld, k0, k0s and Ctot are unused) against [W_hi | W_hi | W_lo] weights
-int gemm(const void* a, int C, int ld, int k0, long long T, int Bn, const void* w, int wN, int wK, int ntaps, const int* shifts, int BN,
-         const float* bias, int act, void* out_bf16, float* out_f32, int ldo, int nvalid, cudaStream_t st, const int* k0s = nullptr, int Ctot = 0,
-         int split = 0) {
-  ActGemmCall g;
-  memset(&g, 0, sizeof(g));
-  if (split) {
-    const int rc = set_split_operand(g, a, C, int(T), Bn, ntaps, shifts);
-    if (rc) return rc;
-  } else {
-    const int nkb = (C + kBK - 1) / kBK;
-    g.a[0] = make_act(a, Ctot > 0 ? Ctot : k0 + C, int(T), Bn, 1, ld); g.na = 1;
-    T2_REQUIRE(ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "CBHG gemm: too many taps");
-    for (int s = 0; s < ntaps; ++s) g.seg[s] = Seg{0, shifts ? shifts[s] : 0, k0s ? k0s[s] : k0, nkb, 0, 1};
-    g.nseg = ntaps;
-  }
-  g.w = w; g.wN = wN; g.wK = wK; g.wL = 1;
-  g.T = int(T); g.B = Bn; g.n_tiles = (nvalid + BN - 1) / BN;
-  g.epi.ptr[0] = out_bf16; g.epi.ptr[1] = const_cast<float*>(bias); g.epi.ptr[2] = out_f32;
-  g.epi.i[0] = ldo; g.epi.i[1] = act; g.epi.i[2] = nvalid;
-  return launch_act_gemm(EPI_BIAS_ACT, BN, g, st);
-}
-
 // wgrad launches, in the order t2_cbhg_backward issues them
 enum { WG_LIN = 0, WG_GRU = 1, WG_HW0 = 2 /* NH launches, last highway layer first */ };
 void build_tiles(const CL& lo, std::vector<std::vector<WgradTile>>& L) {
@@ -794,8 +770,10 @@ int conv_fwd(const Ctx& s, const CConv& L, const void* x, int ld_x, bf16* y_b, f
   for (int j = 0; j < L.k; ++j) shifts[j] = conv_tap_shift(L.k, j);
   const int BN = L.cout % 256 == 0 ? 256 : 128;
   const int sp = s.lo->c.split_bf16;
-  return gemm(x, L.cin, ld_x, 0, s.lo->T, s.lo->B, s.pk + L.k_w, (L.cout + 127) / 128 * 128, L.k * L.cinp * (sp ? 3 : 1), L.k, shifts, BN,
-              s.params + L.p.bias, L.act, y_b, y_f, ldo, L.cout, s.st, nullptr, 0, sp);
+  return launch_bias_act({.a = x, .C = L.cin, .ld = ld_x, .T = s.lo->T, .B = s.lo->B, .ntaps = L.k, .shifts = shifts, .split = sp, .w = s.pk + L.k_w,
+                          .N = (L.cout + 127) / 128 * 128, .wK = L.k * L.cinp * (sp ? 3 : 1), .BN = BN, .bias = s.params + L.p.bias, .act = L.act,
+                          .out_bf16 = y_b, .out_f32 = y_f, .ldo = ldo, .nvalid = L.cout},
+                         s.st);
 }
 }  // namespace
 
@@ -811,7 +789,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   const int T = lo.T, B = lo.B, M = lo.M, HU = lo.HU, RU = lo.RU, KC = lo.KC, PJc = lo.PJc;
   float* scal = W<float>(s, lo.w_scal);
   T2_CHECK_CUDA(cudaMemsetAsync(scal, 0, 16 * sizeof(float), st));
-  // split_bf16: every bf16 operand below is a [hi | lo] row pair, every contraction a split GEMM (set_split_operand), and the
+  // split_bf16: every bf16 operand below is a [hi | lo] row pair, every contraction a split GEMM (launch_bias_act), and the
   // pre-batch-norm activations of the bank and of proj1 are fp32
   const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1, Ms = (M + 63) / 64 * 64;
   bf16* x0 = W<bf16>(s, lo.w_x0);
@@ -860,13 +838,15 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   if (sp) launch_f32_to_bf16_split(hin_f, hin, N, M, Ms, st);
   else launch_f32_to_bf16(hin_f, hin, N * M, st);
   // ---- dense to the highway width, highway layers ----
-  rc = gemm(hin, M, M, 0, T, B, s.pk + lo.k_dense, HU, sp ? 3 * Ms : 128, 1, nullptr, 128, d_params + lo.p_db, 0, W<bf16>(s, lo.w_hb[0]), W<float>(s, lo.w_hf[0]),
-            HU, HU, st, nullptr, 0, sp);
+  rc = launch_bias_act({.a = hin, .C = M, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_dense, .N = HU, .wK = sp ? 3 * Ms : 128, .BN = 128,
+                        .bias = d_params + lo.p_db, .out_bf16 = W<bf16>(s, lo.w_hb[0]), .out_f32 = W<float>(s, lo.w_hf[0]), .ldo = HU, .nvalid = HU},
+                       st);
   if (rc) return rc;
   float* pre = W<float>(s, lo.w_XP);       // [N][2HU] scratch (the GRU input projections overwrite it afterwards)
   for (int i = 0; i < lo.NH; ++i) {
-    rc = gemm(W<bf16>(s, lo.w_hb[i]), HU, HU, 0, T, B, s.pk + lo.k_hw[i], 2 * HU, HU * k3, 1, nullptr, 256, nullptr, 0, nullptr, pre, 2 * HU, 2 * HU, st,
-              nullptr, 0, sp);
+    rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[i]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_hw[i], .N = 2 * HU, .wK = HU * k3,
+                          .BN = 256, .out_f32 = pre, .ldo = 2 * HU, .nvalid = 2 * HU},
+                         st);
     if (rc) return rc;
     highway_fwd(pre, d_params + lo.p_hb[i][0], d_params + lo.p_hb[i][1], W<float>(s, lo.w_hf[i]), W<float>(s, lo.w_hf[i + 1]), W<bf16>(s, lo.w_hb[i + 1]),
                 (training && !sp) ? W<bf16>(s, lo.w_HT[i]) : nullptr, N, HU, sp, st);
@@ -874,7 +854,9 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   // ---- bidirectional GRU ----
   const int XPW = 6 * RU;
   float* XP = W<float>(s, lo.w_XP);
-  rc = gemm(W<bf16>(s, lo.w_hb[lo.NH]), HU, HU, 0, T, B, s.pk + lo.k_gx, XPW, HU * k3, 1, nullptr, 256, nullptr, 0, nullptr, XP, XPW, XPW, st, nullptr, 0, sp);
+  rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[lo.NH]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_gx, .N = XPW, .wK = HU * k3, .BN = 256,
+                        .out_f32 = XP, .ldo = XPW, .nvalid = XPW},
+                       st);
   if (rc) return rc;
   {
     GruArgs a;
@@ -890,8 +872,9 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   }
   // ---- linear projection, clip, loss ----
   float* lin = W<float>(s, lo.w_lin);
-  rc = gemm(W<bf16>(s, lo.w_out), 2 * RU, 2 * RU, 0, T, B, s.pk + lo.k_lin, lo.NFR, 2 * RU * k3, 1, nullptr, 128, d_params + lo.p_lb, 0, nullptr, lin, lo.NFP,
-            lo.NF, st, nullptr, 0, sp);
+  rc = launch_bias_act({.a = W<bf16>(s, lo.w_out), .C = 2 * RU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_lin, .N = lo.NFR, .wK = 2 * RU * k3,
+                        .BN = 128, .bias = d_params + lo.p_lb, .out_f32 = lin, .ldo = lo.NFP, .nvalid = lo.NF},
+                       st);
   if (rc) return rc;
   const int* tlen = lo.c.mask_decoder ? W<int>(s, lo.w_tlen) : nullptr;
   const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
@@ -934,7 +917,9 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   bf16* out = W<bf16>(s, lo.w_out);
   float* dout = W<float>(s, lo.w_dout);
   const int NFK = (lo.NF + 63) / 64 * 64;
-  rc = gemm(dlin, lo.NF, lo.NFP, 0, T, B, s.pk + lo.k_linT, 2 * RU, NFK, 1, nullptr, 256, nullptr, 0, nullptr, dout, 2 * RU, 2 * RU, st);
+  rc = launch_bias_act({.a = dlin, .C = lo.NF, .ld = lo.NFP, .T = T, .B = B, .w = s.pk + lo.k_linT, .N = 2 * RU, .wK = NFK, .BN = 256, .out_f32 = dout,
+                        .ldo = 2 * RU, .nvalid = 2 * RU},
+                       st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(out, 2 * RU, T, B), make_act(dlin, lo.NF, T, B, 1, lo.NFP)}; rc = wgrad(maps, 2); if (rc) return rc; }
   colsum(dlin, N, lo.NF, lo.NFP, d_grads + lo.p_lb, 256, st);
@@ -962,14 +947,16 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     colsum(dXP + d * 3 * RU + 2 * RU, N, RU, XPW, d_grads + lo.p_cb[d], 128, st);
   }
   float* dh = W<float>(s, lo.w_dh);
-  rc = gemm(dXP, XPW, XPW, 0, T, B, s.pk + lo.k_gxT, HU, XPW, 1, nullptr, 128, nullptr, 0, nullptr, dh, HU, HU, st);
+  rc = launch_bias_act({.a = dXP, .C = XPW, .T = T, .B = B, .w = s.pk + lo.k_gxT, .N = HU, .wK = XPW, .BN = 128, .out_f32 = dh, .ldo = HU, .nvalid = HU}, st);
   if (rc) return rc;
   // ---- highway layers (last first) ----
   bf16* dHT = W<bf16>(s, lo.w_dHT);
   float* dcar = W<float>(s, lo.w_XP);        // [N][HU] fp32 scratch (the forward input projections are no longer needed)
   for (int i = lo.NH - 1; i >= 0; --i) {
     highway_bwd(dh, W<bf16>(s, lo.w_HT[i]), W<float>(s, lo.w_hf[i]), dHT, dcar, N, HU, st);
-    rc = gemm(dHT, 2 * HU, 2 * HU, 0, T, B, s.pk + lo.k_hwT[i], HU, 2 * HU, 1, nullptr, 128, nullptr, 0, nullptr, dh, HU, HU, st);
+    rc = launch_bias_act({.a = dHT, .C = 2 * HU, .T = T, .B = B, .w = s.pk + lo.k_hwT[i], .N = HU, .wK = 2 * HU, .BN = 128, .out_f32 = dh, .ldo = HU,
+                          .nvalid = HU},
+                         st);
     if (rc) return rc;
     add_k<<<grid1d(N * HU), 256, 0, st>>>(dh, dcar, i == 0 ? W<bf16>(s, lo.w_dhb) : nullptr, N * HU); t2_count_launch();
     { ActT maps[2] = {make_act(W<bf16>(s, lo.w_hb[i]), HU, T, B), make_act(dHT, 2 * HU, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
@@ -979,7 +966,7 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   // ---- dense ----
   bf16* dhb = W<bf16>(s, lo.w_dhb);
   float* dhin = W<float>(s, lo.w_dhin);
-  rc = gemm(dhb, HU, HU, 0, T, B, s.pk + lo.k_denseT, 128, HU, 1, nullptr, 128, nullptr, 0, nullptr, dhin, M, M, st);
+  rc = launch_bias_act({.a = dhb, .C = HU, .T = T, .B = B, .w = s.pk + lo.k_denseT, .N = 128, .wK = HU, .BN = 128, .out_f32 = dhin, .ldo = M, .nvalid = M}, st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_hin), M, T, B), make_act(dhb, HU, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
   colsum(dhb, N, HU, HU, d_grads + lo.p_db, 128, st);
@@ -992,7 +979,9 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   int sh[16];
   bf16* d2 = W<bf16>(s, lo.w_d2);
   for (int j = 0; j < lo.PK; ++j) sh[j] = -conv_tap_shift(lo.PK, j);
-  rc = gemm(dY2b, lo.proj2.coutp, 128, 0, T, B, s.pk + lo.proj2.k_wT, (PJc + 127) / 128 * 128, lo.PK * lo.proj2.coutp, lo.PK, sh, 256, nullptr, 0, d2, nullptr, PJc, PJc, st);
+  rc = launch_bias_act({.a = dY2b, .C = lo.proj2.coutp, .ld = 128, .T = T, .B = B, .ntaps = lo.PK, .shifts = sh, .w = s.pk + lo.proj2.k_wT,
+                        .N = (PJc + 127) / 128 * 128, .wK = lo.PK * lo.proj2.coutp, .BN = 256, .out_bf16 = d2, .ldo = PJc, .nvalid = PJc},
+                       st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_X1), PJc, T, B), make_act(dY2b, M, T, B, 1, 128)}; rc = wgrad(maps, 2); if (rc) return rc; }
   colsum(dY2b, N, M, 128, d_grads + lo.proj2.p.bias, 128, st);
@@ -1002,7 +991,9 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
   bn_bwd(d2, PJc, W<bf16>(s, lo.w_Y1), PJc, 0, W<float>(s, lo.w_st1), PJc, bsum, d_params + lo.proj1.p.gamma, d1, PJc, d_grads + lo.proj1.p.gamma,
          d_grads + lo.proj1.p.beta, N, PJc, 1, BnDropout{}, 256, st);
   bf16* dP = W<bf16>(s, lo.w_dP);
-  rc = gemm(d1, PJc, PJc, 0, T, B, s.pk + lo.proj1.k_wT, KC, lo.PK * lo.proj1.coutp, lo.PK, sh, 256, nullptr, 0, dP, nullptr, KC, KC, st);
+  rc = launch_bias_act({.a = d1, .C = PJc, .T = T, .B = B, .ntaps = lo.PK, .shifts = sh, .w = s.pk + lo.proj1.k_wT, .N = KC, .wK = lo.PK * lo.proj1.coutp,
+                        .BN = 256, .out_bf16 = dP, .ldo = KC, .nvalid = KC},
+                       st);
   if (rc) return rc;
   { ActT maps[2] = {make_act(W<bf16>(s, lo.w_P), KC, T, B), make_act(d1, PJc, T, B)}; rc = wgrad(maps, 2); if (rc) return rc; }
   colsum(d1, N, PJc, PJc, d_grads + lo.proj1.p.bias, 256, st);
@@ -1025,7 +1016,9 @@ extern "C" int t2_cbhg_backward(const t2_cbhg_config_t* cfg, const float* d_para
     int shifts[16], k0s[16], n = 0;
     for (int l = lo.grp_first[g]; l < lo.grp_first[g + 1]; ++l)
       for (int j = 0; j < lo.bank[l].k; ++j, ++n) { shifts[n] = -conv_tap_shift(lo.bank[l].k, j); k0s[n] = l * lo.CC; }
-    rc = gemm(dpre, lo.CC, KC, 0, T, B, s.pk + lo.k_bankT[g], 128, n * lo.CC, n, shifts, 128, nullptr, 0, nullptr, dx, 128, M, st, k0s, KC);
+    rc = launch_bias_act({.a = dpre, .C = lo.CC, .k0s = k0s, .Ctot = KC, .T = T, .B = B, .ntaps = n, .shifts = shifts, .w = s.pk + lo.k_bankT[g], .N = 128,
+                          .wK = n * lo.CC, .BN = 128, .out_f32 = dx, .ldo = 128, .nvalid = M},
+                         st);
     if (rc) return rc;
   }
   dmel_k<<<grid1d(N * M), 256, 0, st>>>(W<float>(s, lo.w_dx0[0]), W<float>(s, lo.w_dx0[1]), W<float>(s, lo.w_dx0[2]), dhin, d_mel_grad, N, M); t2_count_launch();

@@ -214,7 +214,10 @@ long long* take_timing_slice(long long n_slots) {
   return p;
 }
 
-int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts) {
+// split-bf16 ("fp32-class") operand A of an EPI_BIAS_ACT call: rows [hi | lo], each half C channels zero-padded to
+// Cp = ceil(C / kBK) * kBK (row pitch 2 Cp). Per tap one segment over both halves against [W_hi | W_hi] and one over the hi half
+// against [W_lo], so the packed weights hold 3 Cp K columns per tap (add_pack_split).
+static int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts) {
   const int nkb = (C + kBK - 1) / kBK, Cp = nkb * kBK;
   T2_REQUIRE(2 * ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "split-bf16 GEMM: %d taps are more than %d segments", ntaps, kMaxSeg);
   c.a[0] = make_act(a, 2 * Cp, T, B, 1, 2 * Cp); c.na = 1;
@@ -225,6 +228,28 @@ int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int nt
   }
   c.epi.i[11] = 1;
   return T2_OK;
+}
+
+int launch_bias_act(const BiasActGemm& g, cudaStream_t st) {
+  ActGemmCall c;
+  memset(&c, 0, sizeof(c));
+  if (g.split) {
+    const int rc = set_split_operand(c, g.a, g.C, g.T, g.B, g.ntaps, g.shifts);
+    if (rc) return rc;
+  } else {
+    T2_REQUIRE(g.ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "bias-act GEMM: %d taps are more than %d segments", g.ntaps, kMaxSeg);
+    const int Ctot = g.Ctot > 0 ? g.Ctot : g.C, nkb = (g.C + kBK - 1) / kBK;
+    c.a[0] = make_act(g.a, Ctot, g.T, g.B, 1, g.ld > 0 ? g.ld : Ctot); c.na = 1;
+    for (int s = 0; s < g.ntaps; ++s) c.seg[s] = Seg{0, g.shifts ? g.shifts[s] : 0, g.k0s ? g.k0s[s] : 0, nkb, 0, 1};
+    c.nseg = g.ntaps;
+  }
+  c.w = g.w; c.wN = g.N; c.wK = g.wK; c.wL = 1;
+  c.T = g.T; c.B = g.B; c.n_tiles = (g.nvalid + g.BN - 1) / g.BN;
+  c.epi.ptr[0] = g.out_bf16; c.epi.ptr[1] = const_cast<float*>(g.bias); c.epi.ptr[2] = g.out_f32;
+  c.epi.ptr[7] = const_cast<unsigned long long*>(g.step);
+  c.epi.i[0] = g.ldo; c.epi.i[1] = g.act; c.epi.i[2] = g.nvalid; c.epi.i[3] = g.stream; c.epi.i[4] = g.hash_row0; c.epi.f[1] = g.pdrop;
+  c.epi.seed = g.seed;
+  return launch_act_gemm(EPI_BIAS_ACT, g.BN, c, st);
 }
 
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used) {

@@ -50,12 +50,27 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
-// split-bf16 ("fp32-class") operand A of an EPI_BIAS_ACT call: rows [hi | lo], each half C channels zero-padded to
-// Cp = ceil(C / kBK) * kBK (row pitch 2 Cp). Per tap one segment over both halves against [W_hi | W_hi] and one over the hi half
-// against [W_lo], so the packed weights hold 3 Cp K columns per tap (add_pack_split); a bf16 output is written as [hi(ldo) | lo(ldo)].
-int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts);
 // *cluster_used (nullable) receives the cluster size the kernel was launched with
 int launch_act_gemm(int epi, int BN, const ActGemmCall& c, cudaStream_t stream, int* cluster_used = nullptr);
+// One EPI_BIAS_ACT launch: a k-tap 'same' convolution or a projection over the [B][T] rows of a channels-last bf16 operand,
+//   out[b][t][n] = act(sum_tap sum_k a[b][t + shifts[tap]][k0s[tap] + k] w[n][tap * Cp + k] + bias[n]),   Cp = ceil(C / kBK) * kBK,
+// then dropout at rate pdrop with the mask of hash stream `stream` under seed + *step (step nullable), drawn at row hash_row0 + row,
+// so a launch over some rows of a larger matrix draws that matrix's mask (Epilogue<EPI_BIAS_ACT>, t2_gemm.cuh). Call sites name the
+// fields with designated initialisers, in declaration order.
+struct BiasActGemm {
+  const void* a; int C;                    // operand A: C channels per tap
+  int ld = 0;                              // row pitch (0 = Ctot)
+  const int* k0s = nullptr; int Ctot = 0;  // per-tap first channel (null = 0) of rows of Ctot addressable channels (0 = C)
+  int T; int B;
+  int ntaps = 1; const int* shifts = nullptr;   // tap j reads row t + shifts[j] (null = 0)
+  int split = 0;     // split-bf16 ("fp32-class") operand: rows [hi | lo] of pitch 2 Cp (ld, k0s and Ctot unused) against packed weights
+                     // [W_hi | W_hi | W_lo] (wK = 3 ntaps Cp, add_pack_split); a bf16 output is written as [hi(ldo) | lo(ldo)]
+  const void* w; int N; int wK; int BN;    // packed bf16 weights [N][wK]; BN 128 or 256
+  const float* bias = nullptr; int act = 0;
+  void* out_bf16 = nullptr; float* out_f32 = nullptr; int ldo; int nvalid;   // columns [0, nvalid) of output rows of pitch ldo
+  float pdrop = 0.f; int stream = 0; unsigned long long seed = 0; const unsigned long long* step = nullptr; int hash_row0 = 0;
+};
+int launch_bias_act(const BiasActGemm& g, cudaStream_t st);
 // the checked kernel arguments (tensor maps encoded), grid and cluster size launch_act_gemm launches `c` with
 int make_gemm_args(int epi, int BN, const ActGemmCall& c, GemmArgs& g, dim3& grid, int& cs);
 // one persistent layer chain (wn_chain_kernel): kind 0 / 1 tiles are EPI_GATE (BN 256) / EPI_RES (BN bn1) when fwd, else

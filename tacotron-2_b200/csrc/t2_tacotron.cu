@@ -736,31 +736,6 @@ __global__ void loss_norm_kernel(float* s, float* out, float n_mel, float n_stop
   if (out) { out[0] = s[0] / n_mel; out[1] = s[1] / n_mel; out[2] = s[2] / n_stop; out[3] = s[3] * regw; }
 }
 
-// generic helper: 1x1 / k-tap conv GEMM through the engine
-// split != 0 ("fp32-class" conv stacks): split-bf16 operands (set_split_operand, t2_gemm.h; wK = 3 * ntaps * Cp). hash_row0: position
-// offset of the dropout mask (a launch over the rows of one decoder step draws the elements of those rows in the batched [T_out * B] launch)
-int conv_gemm(const void* a, int C, long long T, int Bn, const void* w, int N, int wK, int ntaps, const int* shifts, int BN, float* bias,
-              int act, void* out_bf16, float* out_f32, int ldo, int nvalid, float pdrop, int stream_id, unsigned long long seed,
-              const unsigned long long* d_step, cudaStream_t st, int split = 0, int hash_row0 = 0) {
-  ActGemmCall g;
-  memset(&g, 0, sizeof(g));
-  const int nkb = (C + kBK - 1) / kBK;
-  if (split) {
-    const int rc = set_split_operand(g, a, C, int(T), Bn, ntaps, shifts);
-    if (rc) return rc;
-  } else {
-  g.a[0] = make_act(a, C, int(T), Bn, 1, C); g.na = 1;
-  for (int s = 0; s < ntaps; ++s) g.seg[s] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};
-  g.nseg = ntaps;
-  }
-  g.w = w; g.wN = N; g.wK = wK; g.wL = 1;
-  g.T = int(T); g.B = Bn; g.n_tiles = (nvalid + BN - 1) / BN;
-  g.epi.ptr[0] = out_bf16; g.epi.ptr[1] = bias; g.epi.ptr[2] = out_f32; g.epi.ptr[7] = const_cast<unsigned long long*>(d_step);
-  g.epi.i[0] = ldo; g.epi.i[1] = act; g.epi.i[2] = nvalid; g.epi.i[3] = stream_id; g.epi.i[4] = hash_row0; g.epi.f[1] = pdrop;
-  g.epi.seed = seed;
-  return launch_act_gemm(EPI_BIAS_ACT, BN, g, st);
-}
-
 struct StepCtx {
   const TL* lo; uint8_t* ws; const uint8_t* pk; const float* params; cudaStream_t st; unsigned long long seed;
   const unsigned long long* d_step; int training;
@@ -796,16 +771,17 @@ int lstm_step(const StepCtx& s, const void* wrec, int H, int K, const void* stat
   return launch_act_gemm(EPI_LSTM, 32, g, s.st);
 }
 
-int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, long long T, int training) {
+int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, int T, int training) {
   const TL& lo = *s.lo;
   int shifts[8];
   for (int j = 0; j < L.k; ++j) shifts[j] = conv_tap_shift(L.k, j);
   const int split = lo.c.split_bf16;
   bf16* y = reinterpret_cast<bf16*>(s.ws + L.w_y);
   float* yf = reinterpret_cast<float*>(s.ws + L.w_y);     // split mode keeps the pre-batch-norm activation in fp32
-  int rc = conv_gemm(x_in, L.cin, T, lo.B, s.pk + L.k_w, L.cout, L.k * L.cinp * (split ? 3 : 1), L.k, shifts, L.cout % 256 == 0 ? 256 : 128,
-                     const_cast<float*>(s.params + L.p.bias), L.act, split ? nullptr : y,
-                     split ? yf : nullptr, L.cout, L.cout, 0.f, 0, 0, nullptr, s.st, split);
+  int rc = launch_bias_act({.a = x_in, .C = L.cin, .T = T, .B = lo.B, .ntaps = L.k, .shifts = shifts, .split = split, .w = s.pk + L.k_w, .N = L.cout,
+                            .wK = L.k * L.cinp * (split ? 3 : 1), .BN = L.cout % 256 == 0 ? 256 : 128, .bias = s.params + L.p.bias, .act = L.act,
+                            .out_bf16 = split ? nullptr : y, .out_f32 = split ? yf : nullptr, .ldo = L.cout, .nvalid = L.cout},
+                           s.st);
   if (rc) return rc;
   float* stats = reinterpret_cast<float*>(s.ws + L.w_stats);
   const long long rows = (long long)lo.B * T;
@@ -1323,7 +1299,7 @@ void launch_dvalues_ctx(const float* alpha, const bf16* dctx, const int* lens, f
   dvalues_ctx_kernel<<<dim3(Ti, B), 256, 0, st>>>(alpha, dctx, lens, dvalues, B, Ti, To, C2); t2_count_launch();
 }
 
-int conv_block_bwd(const StepCtx& s, const ConvL& L, const void* x_in, long long T, const bf16* dout, bf16* dpre, bf16* dx, float* grads,
+int conv_block_bwd(const StepCtx& s, const ConvL& L, const void* x_in, int T, const bf16* dout, bf16* dpre, bf16* dx, float* grads,
                    const WgradTile* tiles, int ntiles) {
   const TL& lo = *s.lo;
   const long long rows = (long long)lo.B * T;
@@ -1335,14 +1311,15 @@ int conv_block_bwd(const StepCtx& s, const ConvL& L, const void* x_in, long long
          BnDropout{lo.c.dropout_rate, s.seed, s.d_step, L.stream}, 256, s.st);
   colsum(dpre, rows, L.cout, L.cout, grads + L.p.bias, 256, s.st);
   T2_CHECK_CUDA(cudaGetLastError());
-  ActT maps[2] = {make_act(x_in, L.cin, int(T), lo.B), make_act(dpre, L.cout, int(T), lo.B)};
-  int rc = launch_wgrad(maps, 2, tiles, ntiles, grads, int(T), lo.B, s.st);
+  ActT maps[2] = {make_act(x_in, L.cin, T, lo.B), make_act(dpre, L.cout, T, lo.B)};
+  int rc = launch_wgrad(maps, 2, tiles, ntiles, grads, T, lo.B, s.st);
   if (rc) return rc;
   if (dx) {
     int shifts[8];
     for (int j = 0; j < L.k; ++j) shifts[j] = -conv_tap_shift(L.k, j);
-    rc = conv_gemm(dpre, L.cout, T, lo.B, s.pk + L.k_wT, L.cin, L.k * L.cout, L.k, shifts, L.cin % 256 == 0 ? 256 : 128, nullptr, 0, dx, nullptr, L.cin,
-                   L.cin, 0.f, 0, 0, nullptr, s.st);
+    rc = launch_bias_act({.a = dpre, .C = L.cout, .T = T, .B = lo.B, .ntaps = L.k, .shifts = shifts, .w = s.pk + L.k_wT, .N = L.cin, .wK = L.k * L.cout,
+                          .BN = L.cin % 256 == 0 ? 256 : 128, .out_bf16 = dx, .ldo = L.cin, .nvalid = L.cin},
+                         s.st);
     if (rc) return rc;
   }
   return T2_OK;
@@ -1424,8 +1401,9 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
     cudaStream_t sx = (d == 1 && side) ? side->s : st;
     StepCtx sc = s; sc.st = sx;
     float* pre = reinterpret_cast<float*>(ws + lo.w_encpre[d]);
-    rc = conv_gemm(x, lo.C, Ti, B, pk + lo.k_encWx[d], 4 * H, lo.C * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 256, const_cast<float*>(d_params) + lo.p_elb[d], 0,
-                   nullptr, pre, 4 * H, 4 * H, 0.f, 0, 0, nullptr, sx, lo.c.split_bf16);
+    rc = launch_bias_act({.a = x, .C = lo.C, .T = Ti, .B = B, .split = lo.c.split_bf16, .w = pk + lo.k_encWx[d], .N = 4 * H,
+                          .wK = lo.C * (lo.c.split_bf16 ? 3 : 1), .BN = 256, .bias = d_params + lo.p_elb[d], .out_f32 = pre, .ldo = 4 * H, .nvalid = 4 * H},
+                         sx);
     if (rc) return rc;
     bf16* hh = reinterpret_cast<bf16*>(ws + lo.w_ench[d]);
     float* cc = reinterpret_cast<float*>(ws + lo.w_encc[d]);
@@ -1453,8 +1431,9 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
                                                                         lo.ld_mem);
   t2_count_launch();
   float* keys = reinterpret_cast<float*>(ws + lo.w_keys);
-  return conv_gemm(values, 2 * H, Ti, B, pk + lo.k_mem, lo.A, 2 * H * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, nullptr, 0, nullptr, keys, lo.A, lo.A,
-                   0.f, 0, 0, nullptr, st, lo.c.split_bf16);
+  return launch_bias_act({.a = values, .C = 2 * H, .T = Ti, .B = B, .split = lo.c.split_bf16, .w = pk + lo.k_mem, .N = lo.A,
+                          .wK = 2 * H * (lo.c.split_bf16 ? 3 : 1), .BN = 128, .out_f32 = keys, .ldo = lo.A, .nvalid = lo.A},
+                         st);
 }
 
 struct DecBufs { bf16 *S1, *S2, *PI, *values; float *c1, *c2, *cum, *attU, *keys, *pre1; size_t att_smem; int K1r, K2, PIK; };
@@ -1515,6 +1494,85 @@ static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_l
   a.split = lo.c.split_bf16; a.lo_h2 = PIK; a.lo_a = K1r; a.lo_b = PIK;
   return launch_att_fwd(a, d.att_smem, st);
 }
+// prenet (two ReLU + dropout layers) and the prenet part of LSTM-1's gates (pre1) over rows [row0, row0 + nrows) of the [T_out * B]
+// decoder buffers; the dropout masks are drawn under seed + *step (step nullable) at hash row offset hash_row0
+static int prenet_fwd(const StepCtx& s, int row0, int nrows, unsigned long long seed, const unsigned long long* step, int hash_row0) {
+  const TL& lo = *s.lo;
+  const uint8_t* pk = s.pk; const float* d_params = s.params;
+  const int D = lo.D, sp = lo.c.split_bf16, k3 = sp ? 3 : 1;   // split_bf16: packed forward operands are [W_hi | W_hi | W_lo]
+  bf16* decin = reinterpret_cast<bf16*>(s.ws + lo.w_decin) + (long long)row0 * lo.ld_decin;
+  bf16* pn1 = reinterpret_cast<bf16*>(s.ws + lo.w_pn1) + (long long)row0 * lo.ld_pn1;
+  bf16* pn2 = reinterpret_cast<bf16*>(s.ws + lo.w_pn2) + (long long)row0 * lo.ld_pn2;
+  float* pre1 = reinterpret_cast<float*>(s.ws + lo.w_pre1) + (long long)row0 * 4 * D;
+  int rc = launch_bias_act({.a = decin, .C = lo.M, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p1, .N = lo.P1, .wK = 128 * k3,
+                            .BN = lo.P1 >= 256 ? 256 : 128, .bias = d_params + lo.p_p1b, .act = 1, .out_bf16 = pn1, .ldo = lo.P1, .nvalid = lo.P1,
+                            .pdrop = lo.c.dropout_rate, .stream = 20, .seed = seed, .step = step, .hash_row0 = hash_row0},
+                           s.st);
+  if (rc) return rc;
+  rc = launch_bias_act({.a = pn1, .C = lo.P1, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p2, .N = lo.P2, .wK = lo.P1 * k3,
+                        .BN = lo.P2 >= 256 ? 256 : 128, .bias = d_params + lo.p_p2b, .act = 1, .out_bf16 = pn2, .ldo = lo.P2, .nvalid = lo.P2,
+                        .pdrop = lo.c.dropout_rate, .stream = 21, .seed = seed, .step = step, .hash_row0 = hash_row0},
+                       s.st);
+  if (rc) return rc;
+  return launch_bias_act({.a = pn2, .C = lo.P2, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_l1x, .N = 4 * D, .wK = lo.P2 * k3, .BN = 256,
+                          .bias = d_params + lo.p_l1b, .out_f32 = pre1, .ldo = 4 * D, .nvalid = 4 * D},
+                         s.st);
+}
+// frame + stop projections of rows [row0, row0 + nrows) into projo; the bias vector [M frames | 1 stop] lives in two parameter
+// tensors, so the caller's finishing kernel adds it
+static int proj_fwd(const StepCtx& s, const DecBufs& d, int row0, int nrows) {
+  const TL& lo = *s.lo;
+  return launch_bias_act({.a = d.PI + (long long)row0 * lo.ld_PI, .C = d.PIK, .T = nrows, .B = 1, .split = lo.c.split_bf16, .w = s.pk + lo.k_proj,
+                          .N = lo.M + 1, .wK = d.PIK * (lo.c.split_bf16 ? 3 : 1), .BN = 128,
+                          .out_f32 = reinterpret_cast<float*>(s.ws + lo.w_projo) + (long long)row0 * 128, .ldo = 128, .nvalid = lo.M + 1},
+                         s.st);
+}
+// decoder step t of a decoder that feeds its own frames back: prenet(t), decoder_step, projection(t), then proj_bias_feedback_kernel
+// adds the biases and writes step t + 1's input. With tgt (teacher-forcing ratio < 1) one draw under seed + *step picks the target frame
+// instead when it falls below ratio, and choice[t] records it.
+static int decoder_step_fed(const StepCtx& s, const DecBufs& d, const int* d_input_lengths, int t, const float* tgt, float ratio,
+                            unsigned long long seed, const unsigned long long* step, int* choice, int hash_row0) {
+  const TL& lo = *s.lo;
+  const int B = lo.B;
+  int rc = prenet_fwd(s, t * B, B, seed, step, hash_row0);
+  if (rc) return rc;
+  rc = decoder_step(s, d, d_input_lengths, t);
+  if (rc) return rc;
+  rc = proj_fwd(s, d, t * B, B);
+  if (rc) return rc;
+  bf16* decin = reinterpret_cast<bf16*>(s.ws + lo.w_decin);
+  T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, s.st,
+                           reinterpret_cast<float*>(s.ws + lo.w_projo) + (long long)t * B * 128, s.params + lo.p_fb, s.params + lo.p_sb,
+                           t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.ld_decin : (bf16*)nullptr, B, lo.M, tgt, lo.To, t, ratio, seed, step,
+                           choice, lo.c.split_bf16));
+  t2_count_launch();
+  return T2_OK;
+}
+// clip the T decoded frames of every item (dec_finish_kernel), the postnet conv blocks (batch norm in training mode when s.training)
+// and the residual projection (mel_finish_kernel). With targets the losses go to the workspace scalars: tlen (nullable) masks frames,
+// pos_weight weighs the stop loss.
+static int postnet_fwd(const StepCtx& s, int T, const float* mel_tgt, const float* stop_tgt, const int* tlen, float pos_weight) {
+  const TL& lo = *s.lo;
+  uint8_t* ws = s.ws; cudaStream_t st = s.st;
+  const int B = lo.B;
+  float* scal = reinterpret_cast<float*>(ws + lo.w_scal);
+  const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
+  bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
+  float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
+  dec_finish_kernel<<<grid1d((long long)B * T * (lo.M + 1)), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_projo), mel_tgt, stop_tgt, dec_bm, dec_f,
+                                                                       reinterpret_cast<float*>(ws + lo.w_stop), scal, B, T, lo.M, lo.c.clip_outputs,
+                                                                       lo_c, hi_c, lo.c.split_bf16, tlen, pos_weight); t2_count_launch();
+  const void* x = dec_bm;
+  for (auto& L : lo.post) { int rc = conv_block_fwd(s, L, x, T, s.training); if (rc) return rc; x = ws + L.w_x; }
+  float* resid = reinterpret_cast<float*>(ws + lo.w_resid);
+  int rc = launch_bias_act({.a = x, .C = lo.PC, .T = T, .B = B, .split = lo.c.split_bf16, .w = s.pk + lo.k_pp, .N = lo.M,
+                            .wK = lo.PC * (lo.c.split_bf16 ? 3 : 1), .BN = 128, .bias = s.params + lo.p_ppb, .out_f32 = resid, .ldo = 128, .nvalid = lo.M},
+                           st);
+  if (rc) return rc;
+  mel_finish_kernel<<<grid1d((long long)B * T * lo.M), 256, 0, st>>>(dec_f, resid, mel_tgt, reinterpret_cast<float*>(ws + lo.w_mel), scal, (long long)B * T,
+                                                                 lo.M, lo.c.clip_outputs, lo_c, hi_c, tlen, T); t2_count_launch();
+  return T2_OK;
+}
 
 // forward + losses. d_inputs int32 [B][T_in]; d_input_lengths int32 [B]; d_mel_targets fp32 [B][T_out][M];
 // d_stop_targets fp32 [B][T_out]. d_loss fp32[4] = {before, after, stop, regularisation} (already normalised).
@@ -1527,92 +1585,45 @@ extern "C" int t2_taco_forward(const t2_taco_config_t* cfg, float* d_params, con
   if (training) { rc = check_att_bwd_fits(lo); if (rc) return rc; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
-  const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
-  StepCtx s{&lo, ws, pk, d_params, st, seed, d_step, training};
-  const int B = lo.B, Ti = lo.Ti, To = lo.To, H = lo.H, D = lo.D;
+  StepCtx s{&lo, ws, static_cast<const uint8_t*>(d_packed), d_params, st, seed, d_step, training};
+  const int B = lo.B, To = lo.To;
   float* scal = reinterpret_cast<float*>(ws + lo.w_scal);
   T2_CHECK_CUDA(cudaMemsetAsync(scal, 0, 16 * sizeof(float), st));
   const int* tlen = lo.c.mask_decoder ? reinterpret_cast<const int*>(ws + lo.w_tlen) : nullptr;     // t2_taco_set_target_lengths
   rc = encoder_fwd(s, d_inputs, d_input_lengths, training);
   if (rc) return rc;
-  const void* x = nullptr;
   bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
   decin_kernel<<<grid1d((long long)To * B * lo.M), 256, 0, st>>>(d_mel_targets, decin, B, To, lo.M, lo.c.split_bf16); t2_count_launch();
   const long long TB = (long long)To * B;
-  bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
-  bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
-  float* pre1 = reinterpret_cast<float*>(ws + lo.w_pre1);
-  float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
-  const int PIK = D + 2 * H;
-  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1;   // split_bf16: packed forward operands are [W_hi | W_hi | W_lo]
   DecBufs db;
   if (lo.c.teacher_forcing_ratio >= 1.f) {
     // ---- decoder: everything that does not depend on the recurrence is batched over time (teacher forcing) ----
-    rc = conv_gemm(decin, lo.M, TB, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, pn1, nullptr, lo.P1,
-                   lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, sp);
-    if (rc) return rc;
-    rc = conv_gemm(pn1, lo.P1, TB, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, pn2, nullptr, lo.P2,
-                   lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, sp);
-    if (rc) return rc;
-    rc = conv_gemm(pn2, lo.P2, TB, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr, pre1, 4 * D, 4 * D, 0.f, 0, 0,
-                   nullptr, st, sp);
+    rc = prenet_fwd(s, 0, int(TB), seed, d_step, 0);
     if (rc) return rc;
     rc = decoder_reset(s, db);
     if (rc) return rc;
     for (int t = 0; t < To; ++t) { rc = decoder_step(s, db, d_input_lengths, t); if (rc) return rc; }
     T2_CHECK_CUDA(cudaGetLastError());
-    // frame + stop projections for all steps at once
-    // bias vector [M frames | 1 stop] lives in two parameter tensors: add them in the finishing kernel instead
-    rc = conv_gemm(db.PI, PIK, TB, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, projo, 128, lo.M + 1, 0.f, 0, 0, nullptr, st,
-                   sp);
+    // frame + stop projections for all steps at once, then their biases in place (tiny)
+    rc = proj_fwd(s, db, 0, int(TB));
     if (rc) return rc;
-    // add the projection biases in place (tiny), then clip / losses
-    proj_bias_kernel<<<grid1d(TB * (lo.M + 1)), 256, 0, st>>>(projo, d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M); t2_count_launch();
+    proj_bias_kernel<<<grid1d(TB * (lo.M + 1)), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_projo), d_params + lo.p_fb, d_params + lo.p_sb, TB, lo.M);
+    t2_count_launch();
   } else {
     // ---- decoder at a teacher-forcing ratio < 1: step t + 1's input is known only once step t has drawn and projected, so the
-    // prenet, the LSTM-1 input projection and the projections run per step (the loop of t2_taco_infer_steps). The prenet masks are the
+    // prenet, the LSTM-1 input projection and the projections run per step (the steps of t2_taco_infer_steps). The prenet masks are the
     // elements the batched launches draw (hash row offset t * B), so a step that takes the target repeats the batched arithmetic. ----
     rc = decoder_reset(s, db);
     if (rc) return rc;
     int* choice = reinterpret_cast<int*>(ws + lo.w_tfsel);
     for (int t = 0; t < To; ++t) {
-      rc = conv_gemm(decin + (long long)t * B * lo.ld_decin, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128,
-                     d_params + lo.p_p1b, 1, pn1 + (long long)t * B * lo.ld_pn1, nullptr, lo.P1, lo.P1, lo.c.dropout_rate, 20, seed, d_step, st, sp, t * B);
+      rc = decoder_step_fed(s, db, d_input_lengths, t, d_mel_targets, lo.c.teacher_forcing_ratio, seed, d_step, choice, t * B);
       if (rc) return rc;
-      rc = conv_gemm(pn1 + (long long)t * B * lo.ld_pn1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128,
-                     d_params + lo.p_p2b, 1, pn2 + (long long)t * B * lo.ld_pn2, nullptr, lo.P2, lo.P2, lo.c.dropout_rate, 21, seed, d_step, st, sp, t * B);
-      if (rc) return rc;
-      rc = conv_gemm(pn2 + (long long)t * B * lo.ld_pn2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
-                     pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st, sp);
-      if (rc) return rc;
-      rc = decoder_step(s, db, d_input_lengths, t);
-      if (rc) return rc;
-      float* pt = projo + (long long)t * B * 128;
-      rc = conv_gemm(db.PI + (long long)t * B * lo.ld_PI, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
-                     lo.M + 1, 0.f, 0, 0, nullptr, st, sp);
-      if (rc) return rc;
-      T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
-                               d_params + lo.p_sb, t + 1 < To ? decin + (long long)(t + 1) * B * lo.ld_decin : (bf16*)nullptr, B, lo.M, d_mel_targets, To,
-                               t, lo.c.teacher_forcing_ratio, seed, d_step, choice, sp));
-      t2_count_launch();
     }
     T2_CHECK_CUDA(cudaGetLastError());
   }
-  const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
-  bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
-  float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
-  dec_finish_kernel<<<grid1d((long long)B * To * (lo.M + 1)), 256, 0, st>>>(projo, d_mel_targets, d_stop_targets, dec_bm, dec_f,
-                                                                        reinterpret_cast<float*>(ws + lo.w_stop), scal, B, To, lo.M,
-                                                                        lo.c.clip_outputs, lo_c, hi_c, lo.c.split_bf16, tlen, lo.c.cross_entropy_pos_weight); t2_count_launch();
-  // ---- postnet ----
-  x = dec_bm;
-  for (auto& L : lo.post) { rc = conv_block_fwd(s, L, x, To, training); if (rc) return rc; x = ws + L.w_x; }
-  float* resid = reinterpret_cast<float*>(ws + lo.w_resid);
-  rc = conv_gemm(x, lo.PC, To, B, pk + lo.k_pp, lo.M, lo.PC * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, d_params + lo.p_ppb, 0, nullptr, resid, 128, lo.M,
-                 0.f, 0, 0, nullptr, st, lo.c.split_bf16);
+  rc = postnet_fwd(s, To, d_mel_targets, d_stop_targets, tlen, lo.c.cross_entropy_pos_weight);
   if (rc) return rc;
-  mel_finish_kernel<<<grid1d((long long)B * To * lo.M), 256, 0, st>>>(dec_f, resid, d_mel_targets, reinterpret_cast<float*>(ws + lo.w_mel), scal,
-                                                                  (long long)B * To, lo.M, lo.c.clip_outputs, lo_c, hi_c, tlen, To); t2_count_launch();
   launch_reg_loss(d_params, reinterpret_cast<const long long*>(ws + lo.w_regtab), lo.n_reg, scal + 3, st);
   T2_CHECK_CUDA(cudaGetLastError());
   loss_norm_kernel<<<1, 1, 0, st>>>(scal, d_loss, float((long long)B * To * lo.M), float((long long)B * To), lo.c.reg_weight, tlen, B, To, lo.M);
@@ -1652,40 +1663,13 @@ extern "C" int t2_taco_infer_steps(const t2_taco_config_t* cfg, float* d_params,
   T2_REQUIRE(t_begin >= 0 && t_begin <= t_end && t_end <= lo.To, T2_ERR_INVALID_ARG, "bad step range [%d, %d)", t_begin, t_end);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
-  const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
-  StepCtx s{&lo, ws, pk, d_params, st, seed, nullptr, 0};
-  const int B = lo.B, D = lo.D, H = lo.H, PIK = D + 2 * H;
-  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1;
+  StepCtx s{&lo, ws, static_cast<const uint8_t*>(d_packed), d_params, st, seed, nullptr, 0};
   DecBufs db;
   decoder_bufs(lo, ws, db);
-  bf16* decin = reinterpret_cast<bf16*>(ws + lo.w_decin);
-  bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
-  bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
-  float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
   for (int t = t_begin; t < t_end; ++t) {
     const unsigned long long seed_t = seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(t + 1);   // fresh prenet masks per step
-    bf16* x0 = decin + (long long)t * B * lo.ld_decin;
-    bf16* x1 = pn1 + (long long)t * B * lo.ld_pn1;
-    bf16* x2 = pn2 + (long long)t * B * lo.ld_pn2;
-    rc = conv_gemm(x0, lo.M, B, 1, pk + lo.k_p1, lo.P1, 128 * k3, 1, nullptr, lo.P1 >= 256 ? 256 : 128, d_params + lo.p_p1b, 1, x1, nullptr, lo.P1,
-                   lo.P1, lo.c.dropout_rate, 20, seed_t, nullptr, st, sp);
+    rc = decoder_step_fed(s, db, d_input_lengths, t, nullptr, 0.f, seed_t, nullptr, nullptr, 0);
     if (rc) return rc;
-    rc = conv_gemm(x1, lo.P1, B, 1, pk + lo.k_p2, lo.P2, lo.P1 * k3, 1, nullptr, lo.P2 >= 256 ? 256 : 128, d_params + lo.p_p2b, 1, x2, nullptr, lo.P2,
-                   lo.P2, lo.c.dropout_rate, 21, seed_t, nullptr, st, sp);
-    if (rc) return rc;
-    rc = conv_gemm(x2, lo.P2, B, 1, pk + lo.k_l1x, 4 * D, lo.P2 * k3, 1, nullptr, 256, d_params + lo.p_l1b, 0, nullptr,
-                   db.pre1 + (long long)t * B * 4 * D, 4 * D, 4 * D, 0.f, 0, 0, nullptr, st, sp);
-    if (rc) return rc;
-    rc = decoder_step(s, db, d_input_lengths, t);
-    if (rc) return rc;
-    float* pt = projo + (long long)t * B * 128;
-    rc = conv_gemm(db.PI + (long long)t * B * lo.ld_PI, PIK, B, 1, pk + lo.k_proj, lo.M + 1, PIK * k3, 1, nullptr, 128, nullptr, 0, nullptr, pt, 128,
-                   lo.M + 1, 0.f, 0, 0, nullptr, st, sp);
-    if (rc) return rc;
-    T2_CHECK_CUDA(launch_pdl(proj_bias_feedback_kernel, dim3(grid1d((long long)B * (lo.M + 1))), dim3(256), 0, st, pt, d_params + lo.p_fb,
-                             d_params + lo.p_sb, t + 1 < lo.To ? decin + (long long)(t + 1) * B * lo.ld_decin : (bf16*)nullptr, B, lo.M,
-                             (const float*)nullptr, lo.To, t, 0.f, 0ull, (const unsigned long long*)nullptr, (int*)nullptr, sp));
-    t2_count_launch();
   }
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
@@ -1700,24 +1684,9 @@ extern "C" int t2_taco_infer_finish(const t2_taco_config_t* cfg, float* d_params
   T2_REQUIRE(T_used >= 1 && T_used <= lo.To, T2_ERR_INVALID_ARG, "T_used %d outside [1, %d]", T_used, lo.To);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
-  const uint8_t* pk = static_cast<const uint8_t*>(d_packed);
-  StepCtx s{&lo, ws, pk, d_params, st, 0ull, nullptr, 0};
-  const int B = lo.B;
-  float* scal = reinterpret_cast<float*>(ws + lo.w_scal);
-  const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
-  bf16* dec_bm = reinterpret_cast<bf16*>(ws + lo.w_decbm);
-  float* dec_f = reinterpret_cast<float*>(ws + lo.w_decf);
-  dec_finish_kernel<<<grid1d((long long)B * T_used * (lo.M + 1)), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_projo), nullptr, nullptr, dec_bm, dec_f,
-                                                                            reinterpret_cast<float*>(ws + lo.w_stop), scal, B, T_used, lo.M,
-                                                                            lo.c.clip_outputs, lo_c, hi_c, lo.c.split_bf16, nullptr, 1.f); t2_count_launch();
-  const void* x = dec_bm;
-  for (auto& L : lo.post) { rc = conv_block_fwd(s, L, x, T_used, 0); if (rc) return rc; x = ws + L.w_x; }
-  float* resid = reinterpret_cast<float*>(ws + lo.w_resid);
-  rc = conv_gemm(x, lo.PC, T_used, B, pk + lo.k_pp, lo.M, lo.PC * (lo.c.split_bf16 ? 3 : 1), 1, nullptr, 128, d_params + lo.p_ppb, 0, nullptr, resid, 128, lo.M,
-                 0.f, 0, 0, nullptr, st, lo.c.split_bf16);
+  StepCtx s{&lo, ws, static_cast<const uint8_t*>(d_packed), d_params, st, 0ull, nullptr, 0};
+  rc = postnet_fwd(s, T_used, nullptr, nullptr, nullptr, 1.f);
   if (rc) return rc;
-  mel_finish_kernel<<<grid1d((long long)B * T_used * lo.M), 256, 0, st>>>(dec_f, resid, nullptr, reinterpret_cast<float*>(ws + lo.w_mel), scal,
-                                                                      (long long)B * T_used, lo.M, lo.c.clip_outputs, lo_c, hi_c, nullptr, T_used); t2_count_launch();
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
@@ -1774,6 +1743,51 @@ extern "C" int t2_taco_set_target_lengths(const t2_taco_config_t* cfg, void* d_w
   return T2_OK;
 }
 
+// prenet backward over rows [row0, row0 + nrows) of the [T_out * B] decoder buffers: the input part of LSTM-1's gate gradient (dg1)
+// through the input projection and both prenet layers (ReLU + dropout) into dz2 (w_dz) and dpn1 (in place)
+static int prenet_bwd(const StepCtx& s, int row0, int nrows) {
+  const TL& lo = *s.lo;
+  uint8_t* ws = s.ws; cudaStream_t st = s.st;
+  const int D = lo.D;
+  const long long r2 = (long long)row0 * lo.P2, r1 = (long long)row0 * lo.P1;
+  const bf16* dg1 = reinterpret_cast<const bf16*>(ws + lo.w_dg1) + (long long)row0 * 4 * D;
+  const bf16* pn1 = reinterpret_cast<const bf16*>(ws + lo.w_pn1) + r1;
+  const bf16* pn2 = reinterpret_cast<const bf16*>(ws + lo.w_pn2) + r2;
+  bf16* dpn2 = reinterpret_cast<bf16*>(ws + lo.w_dpn2) + r2;
+  bf16* dpn1 = reinterpret_cast<bf16*>(ws + lo.w_dpn1) + r1;
+  bf16* dz2 = reinterpret_cast<bf16*>(ws + lo.w_dz) + r2;
+  int rc = launch_bias_act({.a = dg1, .C = 4 * D, .T = nrows, .B = 1, .w = s.pk + lo.k_l1xT, .N = lo.P2, .wK = 4 * D, .BN = lo.P2 % 256 == 0 ? 256 : 128,
+                            .out_bf16 = dpn2, .ldo = lo.P2, .nvalid = lo.P2},
+                           st);
+  if (rc) return rc;
+  relu_drop_bwd_kernel<<<grid1d((long long)nrows * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, (long long)nrows * lo.P2, lo.c.dropout_rate); t2_count_launch();
+  rc = launch_bias_act({.a = dz2, .C = lo.P2, .T = nrows, .B = 1, .w = s.pk + lo.k_p2T, .N = lo.P1, .wK = lo.P2, .BN = lo.P1 % 256 == 0 ? 256 : 128,
+                        .out_bf16 = dpn1, .ldo = lo.P1, .nvalid = lo.P1},
+                       st);
+  if (rc) return rc;
+  relu_drop_bwd_kernel<<<grid1d((long long)nrows * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, (long long)nrows * lo.P1, lo.c.dropout_rate); t2_count_launch();
+  return T2_OK;
+}
+// loss gradient of the projection outputs of steps [t0, t1) into ddec_tm (ddec_tm_kernel; fb / choice: the gradient of the frame a
+// per-step decoder fed back, both nullable) and its product with the transposed frame / stop projections into dPI
+static int proj_bwd(const StepCtx& s, const bf16* ddec_post, const float* stop_tgt, int t0, int t1, const float* fb, const int* choice) {
+  const TL& lo = *s.lo;
+  uint8_t* ws = s.ws; cudaStream_t st = s.st;
+  const int B = lo.B, PIK = lo.D + 2 * lo.H;
+  const float lo_c = -lo.c.max_abs_value - lo.c.lower_bound_decay, hi_c = lo.c.max_abs_value;
+  const int* tlen = lo.c.mask_decoder ? reinterpret_cast<const int*>(ws + lo.w_tlen) : nullptr;
+  bf16* ddec_tm = reinterpret_cast<bf16*>(ws + lo.w_ddec_tm);
+  ddec_tm_kernel<<<grid1d((long long)(t1 - t0) * B * 128), 256, 0, st>>>(reinterpret_cast<const float*>(ws + lo.w_ddecf), ddec_post,
+                                                                       reinterpret_cast<const float*>(ws + lo.w_projo), stop_tgt, ddec_tm, B, lo.To, lo.M,
+                                                                       lo.c.clip_outputs, lo_c, hi_c, tlen, lo.c.cross_entropy_pos_weight,
+                                                                       reinterpret_cast<const float*>(ws + lo.w_scal), t0, t1, fb, choice);
+  t2_count_launch();
+  return launch_bias_act({.a = ddec_tm + (long long)t0 * B * 128, .C = 128, .T = (t1 - t0) * B, .B = 1, .w = s.pk + lo.k_projT, .N = PIK, .wK = 128,
+                          .BN = PIK % 256 == 0 ? 256 : 128, .out_f32 = reinterpret_cast<float*>(ws + lo.w_dPI) + (long long)t0 * B * PIK, .ldo = PIK,
+                          .nvalid = PIK},
+                         st);
+}
+
 // backward of the last t2_taco_forward(training=1): writes d(total loss)/d(theta) for every trainable tensor
 extern "C" int t2_taco_backward(const t2_taco_config_t* cfg, const float* d_params, const void* d_packed, void* d_workspace,
                                 const int* d_inputs, const int* d_input_lengths, const float* d_mel_targets, const float* d_stop_targets,
@@ -1820,8 +1834,9 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   loss_seed_kernel<<<grid1d(BTo * 128), 256, 0, st>>>(reinterpret_cast<float*>(ws + lo.w_decf), reinterpret_cast<float*>(ws + lo.w_resid),
                                                   reinterpret_cast<float*>(ws + lo.w_mel), d_mel_targets, dmel, ddecf, BTo, M, lo.c.clip_outputs,
                                                   lo_c, hi_c, tlen, To, scal, d_mel_outputs_grad); t2_count_launch();
-  rc = conv_gemm(dmel, 128, To, B, pk + lo.k_ppT, lo.PC, 128, 1, nullptr, lo.PC % 256 == 0 ? 256 : 128, nullptr, 0, dY0, nullptr, lo.PC, lo.PC, 0.f, 0, 0,
-                 nullptr, st);
+  rc = launch_bias_act({.a = dmel, .C = 128, .T = To, .B = B, .w = pk + lo.k_ppT, .N = lo.PC, .wK = 128, .BN = lo.PC % 256 == 0 ? 256 : 128, .out_bf16 = dY0,
+                        .ldo = lo.PC, .nvalid = lo.PC},
+                       st);
   if (rc) return rc;
   {
     ActT maps[2] = {make_act(ws + lo.post.back().w_x, lo.PC, To, B), make_act(dmel, 128, To, B)};
@@ -1843,7 +1858,6 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   }
   // ---- projections ----
   bf16* ddec_tm = reinterpret_cast<bf16*>(ws + lo.w_ddec_tm);
-  float* projo = reinterpret_cast<float*>(ws + lo.w_projo);
   float* dPI = reinterpret_cast<float*>(ws + lo.w_dPI);
   bf16* PI = reinterpret_cast<bf16*>(ws + lo.w_PI);
   auto proj_wgrad = [&]() -> int {
@@ -1854,11 +1868,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     return T2_OK;
   };
   if (!per_step) {
-    ddec_tm_kernel<<<grid1d(TB * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c, hi_c, tlen,
-                                                 lo.c.cross_entropy_pos_weight, scal, 0, To, nullptr, nullptr);
-    t2_count_launch();
-    rc = conv_gemm(ddec_tm, 128, TB, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dPI, PIK, PIK, 0.f, 0, 0,
-                   nullptr, st);
+    rc = proj_bwd(s, ddec_post, d_stop_targets, 0, To, nullptr, nullptr);
     if (rc) return rc;
     rc = proj_wgrad();
     if (rc) return rc;
@@ -1897,7 +1907,6 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   if (rc) return rc;
   bf16* pn1 = reinterpret_cast<bf16*>(ws + lo.w_pn1);
   bf16* pn2 = reinterpret_cast<bf16*>(ws + lo.w_pn2);
-  bf16* dpn2 = reinterpret_cast<bf16*>(ws + lo.w_dpn2);
   bf16* dpn1 = reinterpret_cast<bf16*>(ws + lo.w_dpn1);
   bf16* dz2 = reinterpret_cast<bf16*>(ws + lo.w_dz);
   float* dfb = reinterpret_cast<float*>(ws + lo.w_dfb);
@@ -1906,12 +1915,7 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     if (per_step) {
       // loss gradient of step t's projection outputs + (when step t + 1 consumed step t's frame) the gradient of step t + 1's input,
       // left in dfb by the previous iteration; then dPI_t through the frame / stop projections
-      ddec_tm_kernel<<<grid1d((long long)B * 128), 256, 0, st>>>(ddecf, ddec_post, projo, d_stop_targets, ddec_tm, B, To, M, lo.c.clip_outputs, lo_c,
-                                                            hi_c, tlen, lo.c.cross_entropy_pos_weight, scal, t, t + 1,
-                                                            t + 1 < To ? dfb : nullptr, choice);
-      t2_count_launch();
-      rc = conv_gemm(ddec_tm + (long long)t * B * 128, 128, B, 1, pk + lo.k_projT, PIK, 128, 1, nullptr, PIK % 256 == 0 ? 256 : 128, nullptr, 0,
-                     nullptr, dPI + (long long)t * B * PIK, PIK, PIK, 0.f, 0, 0, nullptr, st);
+      rc = proj_bwd(s, ddec_post, d_stop_targets, t, t + 1, t + 1 < To ? dfb : nullptr, choice);
       if (rc) return rc;
     }
     AttBwd a;
@@ -1943,19 +1947,12 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     if (per_step) {
       // the input part of LSTM-1's gate gradient back through the input projection and both prenet layers (ReLU + dropout), into the
       // [T_out * B] buffers of the batched path; for t >= 1 on to d(input frame of step t) = dfb
-      const long long r2 = (long long)t * B * lo.P2, r1 = (long long)t * B * lo.P1;
-      rc = conv_gemm(c1.dg_a, 4 * D, B, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2 + r2, nullptr,
-                     lo.P2, lo.P2, 0.f, 0, 0, nullptr, st);
+      rc = prenet_bwd(s, t * B, B);
       if (rc) return rc;
-      relu_drop_bwd_kernel<<<grid1d((long long)B * lo.P2), 256, 0, st>>>(dpn2 + r2, pn2 + r2, dz2 + r2, (long long)B * lo.P2, lo.c.dropout_rate);
-      t2_count_launch();
-      rc = conv_gemm(dz2 + r2, lo.P2, B, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1 + r1, nullptr,
-                     lo.P1, lo.P1, 0.f, 0, 0, nullptr, st);
-      if (rc) return rc;
-      relu_drop_bwd_kernel<<<grid1d((long long)B * lo.P1), 256, 0, st>>>(dpn1 + r1, pn1 + r1, dpn1 + r1, (long long)B * lo.P1, lo.c.dropout_rate);
-      t2_count_launch();
       if (t >= 1) {
-        rc = conv_gemm(dpn1 + r1, lo.P1, B, 1, pk + lo.k_p1T, M, lo.P1, 1, nullptr, 128, nullptr, 0, nullptr, dfb, M, M, 0.f, 0, 0, nullptr, st);
+        rc = launch_bias_act({.a = dpn1 + (long long)t * B * lo.P1, .C = lo.P1, .T = B, .B = 1, .w = pk + lo.k_p1T, .N = M, .wK = lo.P1, .BN = 128,
+                              .out_f32 = dfb, .ldo = M, .nvalid = M},
+                             st);
         if (rc) return rc;
       }
     }
@@ -1971,14 +1968,8 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
     colsum(dg1, TB, 4 * D, 4 * D, d_grads + lo.p_l1b, 256, st);
   }
   if (!per_step) {   // prenet data gradients over all steps (the per-step path wrote them inside the loop)
-    rc = conv_gemm(dg1, 4 * D, TB, 1, pk + lo.k_l1xT, lo.P2, 4 * D, 1, nullptr, lo.P2 % 256 == 0 ? 256 : 128, nullptr, 0, dpn2, nullptr, lo.P2, lo.P2, 0.f,
-                   0, 0, nullptr, st);
+    rc = prenet_bwd(s, 0, int(TB));
     if (rc) return rc;
-    relu_drop_bwd_kernel<<<grid1d(TB * lo.P2), 256, 0, st>>>(dpn2, pn2, dz2, TB * lo.P2, lo.c.dropout_rate); t2_count_launch();
-    rc = conv_gemm(dz2, lo.P2, TB, 1, pk + lo.k_p2T, lo.P1, lo.P2, 1, nullptr, lo.P1 % 256 == 0 ? 256 : 128, nullptr, 0, dpn1, nullptr, lo.P1, lo.P1, 0.f, 0,
-                   0, nullptr, st);
-    if (rc) return rc;
-    relu_drop_bwd_kernel<<<grid1d(TB * lo.P1), 256, 0, st>>>(dpn1, pn1, dpn1, TB * lo.P1, lo.c.dropout_rate); t2_count_launch();
   }
   {
     ActT maps[6] = {make_act(pn1, lo.P1, int(TB), 1), make_act(dz2, lo.P2, int(TB), 1), make_act(ws + lo.w_decin, M, int(TB), 1),
@@ -1996,8 +1987,9 @@ extern "C" int t2_taco_backward_ex(const t2_taco_config_t* cfg, const float* d_p
   bf16* dkeysb = reinterpret_cast<bf16*>(ws + lo.w_dkeysb);
   launch_f32_to_bf16(dkeys, dkeysb, (long long)B * Ti * A, st);
   float* dvalues = reinterpret_cast<float*>(ws + lo.w_dvalues);
-  rc = conv_gemm(dkeysb, A, Ti, B, pk + lo.k_memT, 2 * H, A, 1, nullptr, (2 * H) % 256 == 0 ? 256 : 128, nullptr, 0, nullptr, dvalues, 2 * H, 2 * H, 0.f, 0, 0,
-                 nullptr, st);
+  rc = launch_bias_act({.a = dkeysb, .C = A, .T = Ti, .B = B, .w = pk + lo.k_memT, .N = 2 * H, .wK = A, .BN = (2 * H) % 256 == 0 ? 256 : 128,
+                        .out_f32 = dvalues, .ldo = 2 * H, .nvalid = 2 * H},
+                       st);
   if (rc) return rc;
   {
     ActT maps[2] = {make_act(ws + lo.w_values, 2 * H, Ti, B), make_act(dkeysb, A, Ti, B)};
@@ -2131,8 +2123,10 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
                  T2_ERR_INVALID_ARG, "dbg_taco_kernel CONV_GEMM: bad shape");
       int shifts[kMaxSeg];
       for (int j = 0; j < ntaps; ++j) shifts[j] = conv_tap_shift(ntaps, j);
-      int rc = conv_gemm(p[0], C, T, Bn, p[1], N, wK, ntaps, shifts, BN, static_cast<float*>(p[2]), act, p[3], static_cast<float*>(p[4]), ldo,
-                         nvalid, pdrop, sid, call->seed, call->step, st, split, row0);
+      int rc = launch_bias_act({.a = p[0], .C = C, .T = T, .B = Bn, .ntaps = ntaps, .shifts = shifts, .split = split, .w = p[1], .N = N, .wK = wK, .BN = BN,
+                                .bias = static_cast<const float*>(p[2]), .act = act, .out_bf16 = p[3], .out_f32 = static_cast<float*>(p[4]), .ldo = ldo,
+                                .nvalid = nvalid, .pdrop = pdrop, .stream = sid, .seed = call->seed, .step = call->step, .hash_row0 = row0},
+                               st);
       if (rc) return rc;
       T2_CHECK_CUDA(cudaGetLastError());
       return T2_OK;

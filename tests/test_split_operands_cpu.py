@@ -28,7 +28,7 @@ SPLIT_COVERAGE = {
     "first_conv_kernel": "test_wavenet_kernels_gpu.py::test_first_conv",
     "up1d_fwd_kernel": "test_wavenet_upsample_gpu.py::test_1d_split_rows",
     "upsample_fwd_kernel": "test_wavenet_upsample_gpu.py::test_1d_split_rows",
-    # epilogues branching on e.i[11]; EPI_BIAS_ACT and EPI_LSTM through the production helpers conv_gemm / lstm_step
+    # epilogues branching on e.i[11]; EPI_BIAS_ACT and EPI_LSTM through the production helpers launch_bias_act / lstm_step
     "EPI_GATE": _GEMM + "test_gate",
     "EPI_RES": _GEMM + "test_res",
     "EPI_BIAS_ACT": _SPLIT + "test_conv_gemm_split",

@@ -121,7 +121,7 @@ def seed_offset(v):
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# a. split conv / projection GEMMs through conv_gemm(..., split = 1)
+# a. split conv / projection GEMMs through launch_bias_act(.split = 1)
 # ------------------------------------------------------------------------------------------------------------------------------
 def conv_inputs(B, T, C, N, ntaps, gen, signed=False):
     """activation rows [hi(Cp) | lo(Cp)] (zero channels C..Cp-1 in both halves, as f32_to_bf16_kernel<true> writes them) and packed

@@ -320,3 +320,31 @@ def test_dropin_training_loop_at_ratio_half():
     torch.cuda.synchronize()
     print("drop-in losses at ratio 0.5:", losses)
     assert all(math.isfinite(l) for l in losses) and torch.isfinite(m.gradients).all()
+
+
+@pytest.mark.parametrize("precision", ["bf16", "fp32-class"])
+def test_synthesis_is_bitwise_the_ratio_zero_evaluation_forward(precision):
+    """free-running synthesis (t2_taco_infer_*) and an evaluation forward at teacher-forcing ratio 0 run the same decoder step: each
+    feeds the frame it just predicted to the next step. With prenet dropout off nothing random is left, so over the T_used steps
+    synthesis ran both give the same decoder outputs, alignments and stop logits bit for bit. The postnet's 'same' convolutions read
+    past T_used, so mel_outputs agree only when synthesis ran all T_out steps."""
+    hp = _hp(tacotron_zoneout_rate=0.1)
+    B, T_in, T_out, M = 3, 40, 24, hp.num_mels
+    params = ot.init_params(hp, seed=68, random_bias=True)
+    inputs, lens, mel, stop = [x.cuda() for x in _batch(hp, B, T_in, T_out, 68)]
+    model = t2.tacotron.Tacotron(hp, B, T_in, T_out, precision=precision, teacher_forcing_ratio=0.0)
+    model.load_params(params)
+    model.forward(inputs.int(), lens.int(), mel, stop, training=False, seed=5)
+    torch.cuda.synchronize()
+    fwd = _outputs(model, B, T_in, T_out, M)
+    syn = model.synthesize(inputs.int(), lens.int(), max_iters=T_out, seed=5)
+    T = syn["T"]
+    syn_stop = model.workspace_tensor("stop_logits", (B, T)).cpu()
+    same = dict(decoder_output=torch.equal(syn["decoder_output"].cpu(), fwd["decoder_output"][:, :T]),
+                alignments=torch.equal(syn["alignments"].cpu(), fwd["alignments"][:, :T]),
+                stop_logits=torch.equal(syn_stop, fwd["stop_logits"][:, :T]))
+    if T == T_out:
+        same["mel_outputs"] = torch.equal(syn["mel_outputs"].cpu(), fwd["mel_outputs"])
+    print("synthesis (T_used %d of %d) vs ratio-0 evaluation forward, %s: bitwise" % (T, T_out, precision), same)
+    record("tacotron_synthesis_vs_ratio0_fwd_%s" % precision, T_used=T, bitwise=all(same.values()))
+    assert all(same.values()), same
