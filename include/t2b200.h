@@ -181,6 +181,40 @@ typedef struct {
 #define T2_DBG_TACO_CONV_GEMM 8
 #define T2_DBG_TACO_LSTM_STEP 9
 #define T2_DBG_TACO_ROWS 10
+/* LOSS        one of the loss / gradient-seed kernels, i[0] selecting it. The decoder-output kernels (0-3) take i: -, B, To, M (M + 1
+ *             <= 128), clip, and f: clip low, clip high, stop positive weight; frames are batch-major [B][To][M], projection rows
+ *             time-major [To][B][128] (col M: stop logit), the loss scalars fp32 [16] as the engine keeps them ([0] before, [1] after,
+ *             [2] stop, [3] regulariser, [4] masked stop count: accumulated; [5] / [6] mel / stop normalisers).
+ *             0 mel_finish_kernel   p: dec fp32, residual fp32 [B To][128], target (nullable), mel fp32 (out), scal, target lengths
+ *                                   int32 [B] (nullable).
+ *             1 loss_norm_kernel    p: scal, out fp32 [4] (nullable: the four normalised loss terms), target lengths (nullable).
+ *                                   f[0]: regulariser weight (clip unused).
+ *             2 loss_seed_kernel    p: dec fp32, residual, mel, target, dmel bf16 [B To][128] (out), ddec fp32 [B][To][M] (out),
+ *                                   target lengths (nullable), scal (reads [5]), extra fp32 [B][To][M] (nullable; d loss / d mel
+ *                                   outputs from a later head).
+ *             3 ddec_tm_kernel      p: ddec fp32 [B][To][M], dpost bf16 [B][To][M], projection rows, stop target fp32 [B][To], out bf16
+ *                                   [To][B][128] (rows of steps [t0, t1) written), target lengths (nullable), scal (reads [6]), fb fp32
+ *                                   [B][M] (nullable), choice int32 [To] (required with fb). i[5], i[6]: t0, t1.
+ *             4 proj_bias_kernel    p: projection rows fp32 [rows][128] (in / out), frame bias [M], stop bias [1]. i: -, rows, M.
+ *             5 relu_drop_bwd_kernel  p: d bf16 [n], y bf16 [n], dz bf16 [n] (may be d). i: -, n. f[0]: dropout rate.
+ *             6 embed_bwd_kernel    p: idx int32 [npos], dx bf16 [npos][E], dtable fp32 (accumulated). i: -, npos, E.
+ *             7 mask_values_kernel  p: memory bf16 [B][Ti][C2], lengths int32 [B], values bf16 [B][Ti][C2]. i: -, B, Ti, C2.
+ *             8 bias_colsum_kernel<bf16> (colsum)  p: src bf16 [rows][ld], dst fp32 [C] (accumulated). i: -, rows, C, ld, threads
+ *                                   (128 / 256).
+ * PARAMS      the parameter-table kernels, i[0] selecting one.
+ *             0 pack_kernel, one job (add_pack)  p: params fp32, packed bf16, job buffer (device, >= sizeof(PackJob) B; filled
+ *                                   stream-ordered). i: -, job buffer bytes, W (32: four LSTM gates, 128: two WaveNet gate halves),
+ *                                   grid_x, src_off, K, N, dst_off (bf16 elements), dst_ld, transpose, col0, perm, part (0 / 2).
+ *                                   f[0]: scale.
+ *             1 pack_kernel, the three jobs of add_pack_split in one launch  p: as 0 (>= 3 sizeof(PackJob) B). i: -, bytes, W,
+ *                                   grid_x, src_off, K, N, dst_off, dst_ld, col_hi, col_lo, slot, perm. f[0]: scale.
+ *                                   A job with perm > 0 must transpose, with N = gates * perm (gates = 4 for W = 32, 2 for W = 128)
+ *                                   and perm % W == 0.
+ *             2 reg_loss_kernel     p: params fp32, table int64 [n_reg][2] (offset, elements), dst fp32 (accumulated: 0.5 sum w^2).
+ *                                   i: -, n_reg.
+ *             3 reg_grad_kernel     p: params, grads fp32 (accumulated: weight w), table. i: -, n_reg. f[0]: weight. */
+#define T2_DBG_TACO_LOSS 11
+#define T2_DBG_TACO_PARAMS 12
 int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 /* t2_dbg_cbhg_kernel ids (the batch-norm pair works on the column slice [c0, c0 + C) of pitch-ld matrices; statistics / sums are
  * [4 Ct] / [2 Ct] indexed by absolute column, and the caller zeroes the sum sections first, as the engine does):
@@ -203,7 +237,14 @@ int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
  *              must be null).
  * GRU_BWD      gru_bwd_kernel (BPTT of both directions). p: params, dout fp32 [N][2RU], out bf16 [N][2RU] (h_prev, as GRU_FWD writes it),
  *              the stashes r, u, c of fw, then of bw, dXP bf16 [N][6RU] (out: [dr_pre | du_pre | dc_pre] per direction).
- *              i: B, T, HU, RU (= 128), then p_gk, p_ck of fw, then of bw. */
+ *              i: B, T, HU, RU (= 128), then p_gk, p_ck of fw, then of bw.
+ * LINEAR       lin_norm_k, lin_finish_k, then loss_out_k (the linear-spectrogram clip, L1 loss and gradient seed; rows r = b T + t,
+ *              N = B T). p: lin fp32 [N][NFP] (in / out: columns [0, NF) clipped), target fp32 [N][NF] (nullable: inference), dlin bf16
+ *              [N][NFP] (nullable; written only with a target, as the engine does), scal fp32 [10] ([0] / [1] accumulated L1 sums, [2]
+ *              regulariser sum, [8] / [9] normalisers), out fp32 [2] (nullable: loss_out_k skipped), target lengths int32 [B] (nullable).
+ *              i: B, T, NF, NFP, n_prio, clip. f: clip low, clip high, regulariser weight.
+ * ADD          i[0] selecting: 0 add_k  p: acc fp32 [n] (in / out: acc + a), a fp32 [n], out bf16 [n] (nullable). i: -, n.
+ *                              1 dmel_k p: a, b, c fp32 [N][128], dhin fp32 [N][M], out fp32 [N][M]. i: -, N, M (<= 128). */
 #define T2_DBG_CBHG_BN_FWD 1
 #define T2_DBG_CBHG_BN_BWD 2
 #define T2_DBG_CBHG_POOL_FWD 3
@@ -212,6 +253,8 @@ int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream);
 #define T2_DBG_CBHG_HIGHWAY_BWD 6
 #define T2_DBG_CBHG_GRU_FWD 7
 #define T2_DBG_CBHG_GRU_BWD 8
+#define T2_DBG_CBHG_LINEAR 9
+#define T2_DBG_CBHG_ADD 10
 int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream);
 
 

@@ -1160,6 +1160,36 @@ extern "C" int t2_dbg_cbhg_kernel(const t2_dbg_kernel_t* call, void* stream) {
       if (!rc) rc = gru_setup();
       return rc ? rc : launch_gru_bwd(a, st);
     }
+    case T2_DBG_CBHG_LINEAR: {
+      const long long B = i[0], T = i[1];
+      const int NF = int(i[2]), NFP = int(i[3]), n_prio = int(i[4]), clip = int(i[5]);
+      T2_REQUIRE(p[0] && p[3] && B >= 1 && B <= 65535 && T >= 1 && T <= 65535 && NF >= 1 && NFP >= NF && n_prio >= 1 && n_prio <= NF &&
+                     (clip == 0 || clip == 1),
+                 T2_ERR_INVALID_ARG, "dbg_cbhg_kernel LINEAR: bad arguments");
+      float* scal = static_cast<float*>(p[3]);
+      const float* tgt = static_cast<const float*>(p[1]);
+      const long long N = B * T;
+      lin_norm_k<<<1, 1, 0, st>>>(scal, static_cast<const int*>(p[5]), int(B), int(T), NF, n_prio); t2_count_launch();
+      lin_finish_k<<<grid1d(N * NFP), 256, 0, st>>>(static_cast<float*>(p[0]), tgt, tgt ? static_cast<bf16*>(p[2]) : nullptr, scal, N, int(T), NF, NFP,
+                                                    n_prio, clip, call->f[0], call->f[1], static_cast<const int*>(p[5]));
+      t2_count_launch();
+      if (p[4]) { loss_out_k<<<1, 1, 0, st>>>(scal, static_cast<float*>(p[4]), call->f[2]); t2_count_launch(); }
+      break;
+    }
+    case T2_DBG_CBHG_ADD: {
+      T2_REQUIRE(i[0] == 0 || i[0] == 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel ADD: bad kernel selector %lld", i[0]);
+      if (i[0] == 0) {
+        T2_REQUIRE(p[0] && p[1] && i[1] >= 1, T2_ERR_INVALID_ARG, "dbg_cbhg_kernel ADD add_k: bad arguments");
+        add_k<<<grid1d(i[1]), 256, 0, st>>>(static_cast<float*>(p[0]), static_cast<const float*>(p[1]), static_cast<bf16*>(p[2]), i[1]);
+      } else {
+        T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && i[1] >= 1 && i[2] >= 1 && i[2] <= 128, T2_ERR_INVALID_ARG,
+                   "dbg_cbhg_kernel ADD dmel_k: bad arguments");
+        dmel_k<<<grid1d(i[1] * i[2]), 256, 0, st>>>(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]), static_cast<const float*>(p[2]),
+                                                  static_cast<const float*>(p[3]), static_cast<float*>(p[4]), i[1], int(i[2]));
+      }
+      t2_count_launch();
+      break;
+    }
     default:
       return t2_set_error(T2_ERR_INVALID_ARG, "dbg_cbhg_kernel: unknown kernel id %d", call->kernel);
   }

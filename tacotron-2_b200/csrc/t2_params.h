@@ -58,7 +58,9 @@ void add_pack_split(std::vector<PackJob>& jobs, long long src, int K, int N, lon
                     float scale = 1.f, int perm = 0);
 // runs the jobs_dev[0, n_jobs) table at grid (grid_x, n_jobs) x (32, 8). W is the row block width of the gate permutation:
 // row = (u / W) * (gates * W) + g * W + u % W, with W = 128 for WaveNet's two gate halves (tanh | sigmoid) and W = 32 for the four
-// LSTM gates of the EPI_LSTM rows.
+// LSTM gates of the EPI_LSTM rows. The permutation is a bijection of the job's N rows only when the job transposes, N == gates * perm
+// and perm % W == 0; the kernel does not check this, and a job that breaks it writes rows outside its block, so every job with
+// perm > 0 must be built to meet it.
 int launch_pack(const float* params, void* packed, const PackJob* jobs_dev, int n_jobs, int W, int grid_x, cudaStream_t st);
 
 // L2 regulariser: the table holds (offset, elements) of every tensor with reg set; reg_loss adds 0.5 sum w^2 to *dst,

@@ -2293,6 +2293,111 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_CHECK_CUDA(cudaGetLastError());
       return T2_OK;
     }
+    case T2_DBG_TACO_LOSS: {
+      const int which = int(i[0]);
+      const float* f = call->f;
+      T2_REQUIRE(which >= 0 && which <= 8, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS: bad kernel selector %d", which);
+      if (which <= 3) {   // the decoder-output losses: B, To, M (+ clip) as the engine passes them, rows of pitch 128
+        const int B = int(i[1]), To = int(i[2]), M = int(i[3]), clip = int(i[4]);
+        T2_REQUIRE(i[1] >= 1 && i[1] <= 65535 && i[2] >= 1 && i[2] <= 65535 && M >= 1 && M + 1 <= 128 && (which == 1 || clip == 0 || clip == 1),
+                   T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS: bad shape or clip flag");
+        const long long BTo = (long long)B * To;
+        if (which == 0) {
+          T2_REQUIRE(p[0] && p[1] && p[3] && p[4], T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS mel_finish: null pointer");
+          mel_finish_kernel<<<grid1d(BTo * M), 256, 0, st>>>(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]),
+                                                             static_cast<const float*>(p[2]), static_cast<float*>(p[3]), static_cast<float*>(p[4]),
+                                                             BTo, M, clip, f[0], f[1], static_cast<const int*>(p[5]), To);
+        } else if (which == 1) {
+          T2_REQUIRE(p[0], T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS loss_norm: null pointer");
+          loss_norm_kernel<<<1, 1, 0, st>>>(static_cast<float*>(p[0]), static_cast<float*>(p[1]), float(BTo * M), float(BTo), f[0],
+                                            static_cast<const int*>(p[2]), B, To, M);
+        } else if (which == 2) {
+          T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[5] && p[7], T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS loss_seed: null pointer");
+          loss_seed_kernel<<<grid1d(BTo * 128), 256, 0, st>>>(static_cast<const float*>(p[0]), static_cast<const float*>(p[1]),
+                                                              static_cast<const float*>(p[2]), static_cast<const float*>(p[3]), static_cast<bf16*>(p[4]),
+                                                              static_cast<float*>(p[5]), BTo, M, clip, f[0], f[1], static_cast<const int*>(p[6]), To,
+                                                              static_cast<const float*>(p[7]), static_cast<const float*>(p[8]));
+        } else {
+          const int t0 = int(i[5]), t1 = int(i[6]);
+          T2_REQUIRE(p[0] && p[1] && p[2] && p[3] && p[4] && p[6] && (!p[7] || p[8]), T2_ERR_INVALID_ARG,
+                     "dbg_taco_kernel LOSS ddec_tm: null pointer (choice is required with fb)");
+          T2_REQUIRE(t0 >= 0 && t0 < t1 && t1 <= To, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS ddec_tm: bad step range [%d, %d)", t0, t1);
+          ddec_tm_kernel<<<grid1d((long long)(t1 - t0) * B * 128), 256, 0, st>>>(
+              static_cast<const float*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<const float*>(p[2]), static_cast<const float*>(p[3]),
+              static_cast<bf16*>(p[4]), B, To, M, clip, f[0], f[1], static_cast<const int*>(p[5]), f[2], static_cast<const float*>(p[6]), t0, t1,
+              static_cast<const float*>(p[7]), static_cast<const int*>(p[8]));
+        }
+      } else if (which == 4) {   // proj_bias_kernel
+        const long long rows = i[1];
+        const int M = int(i[2]);
+        T2_REQUIRE(p[0] && p[1] && p[2] && rows >= 1 && M >= 1 && M + 1 <= 128, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS proj_bias: bad arguments");
+        proj_bias_kernel<<<grid1d(rows * (M + 1)), 256, 0, st>>>(static_cast<float*>(p[0]), static_cast<const float*>(p[1]),
+                                                                 static_cast<const float*>(p[2]), rows, M);
+      } else if (which == 5) {   // relu_drop_bwd_kernel (dz may alias d, as the engine's second call does)
+        const long long n = i[1];
+        T2_REQUIRE(p[0] && p[1] && p[2] && n >= 1 && f[0] >= 0.f && f[0] < 1.f, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS relu_drop_bwd: bad arguments");
+        relu_drop_bwd_kernel<<<grid1d(n), 256, 0, st>>>(static_cast<const bf16*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<bf16*>(p[2]), n, f[0]);
+      } else if (which == 6) {   // embed_bwd_kernel
+        const long long npos = i[1];
+        const int E = int(i[2]);
+        T2_REQUIRE(p[0] && p[1] && p[2] && npos >= 1 && E >= 1, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS embed_bwd: bad arguments");
+        embed_bwd_kernel<<<grid1d(npos * E), 256, 0, st>>>(static_cast<const int*>(p[0]), static_cast<const bf16*>(p[1]), static_cast<float*>(p[2]), npos, E);
+      } else if (which == 7) {   // mask_values_kernel
+        const int B = int(i[1]), Ti = int(i[2]), C2 = int(i[3]);
+        T2_REQUIRE(p[0] && p[1] && p[2] && B >= 1 && Ti >= 1 && C2 >= 1, T2_ERR_INVALID_ARG, "dbg_taco_kernel LOSS mask_values: bad arguments");
+        mask_values_kernel<<<grid1d((long long)B * Ti * C2), 256, 0, st>>>(static_cast<const bf16*>(p[0]), static_cast<const int*>(p[1]),
+                                                                          static_cast<bf16*>(p[2]), B, Ti, C2);
+      } else {   // bias_colsum_kernel<bf16> through colsum
+        const long long rows = i[1];
+        const int C = int(i[2]), ld = int(i[3]), threads = int(i[4]);
+        T2_REQUIRE(p[0] && p[1] && rows >= 1 && C >= 1 && ld >= C && (threads == 128 || threads == 256), T2_ERR_INVALID_ARG,
+                   "dbg_taco_kernel LOSS bias_colsum: bad arguments");
+        colsum(static_cast<const bf16*>(p[0]), rows, C, ld, static_cast<float*>(p[1]), threads, st);
+      }
+      if (which <= 7) t2_count_launch();
+      T2_CHECK_CUDA(cudaGetLastError());
+      return T2_OK;
+    }
+    case T2_DBG_TACO_PARAMS: {
+      const int which = int(i[0]);
+      T2_REQUIRE(which >= 0 && which <= 3, T2_ERR_INVALID_ARG, "dbg_taco_kernel PARAMS: bad kernel selector %d", which);
+      if (which >= 2) {   // reg_loss_kernel / reg_grad_kernel over a caller (offset, elements) table of i[1] tensors
+        const long long n_reg = i[1];
+        T2_REQUIRE(p[0] && p[1] && p[2] && n_reg >= 1 && n_reg <= 65535, T2_ERR_INVALID_ARG, "dbg_taco_kernel PARAMS reg: bad arguments");
+        if (which == 2)
+          launch_reg_loss(static_cast<const float*>(p[0]), static_cast<const long long*>(p[1]), int(n_reg), static_cast<float*>(p[2]), st);
+        else
+          launch_reg_grad(static_cast<const float*>(p[0]), static_cast<float*>(p[1]), static_cast<const long long*>(p[2]), int(n_reg), call->f[0], st);
+        T2_CHECK_CUDA(cudaGetLastError());
+        return T2_OK;
+      }
+      // pack_kernel: one job (add_pack) or the three jobs of add_pack_split, built here and copied into the caller's job buffer
+      const int split = which == 1, W = int(i[2]), grid_x = int(i[3]);
+      const long long src = i[4], dst = i[7];
+      const int K = int(i[5]), N = int(i[6]), ld = int(i[8]), perm = int(i[split ? 12 : 11]);
+      const int transpose = split ? 1 : int(i[9]), col0 = int(i[split ? 9 : 10]), part = split ? 0 : int(i[12]);
+      const int col_lo = split ? int(i[10]) : 0, slot = split ? int(i[11]) : 0;
+      T2_REQUIRE(p[0] && p[1] && p[2] && (W == 32 || W == 128) && grid_x >= 1 && grid_x <= 65535 && src >= 0 && dst >= 0 && i[5] >= 1 &&
+                     i[5] <= (1 << 20) && i[6] >= 1 && i[6] <= (1 << 20) && col0 >= 0 && (transpose == 0 || transpose == 1) &&
+                     (part == 0 || part == 2) && col_lo >= 0 && slot >= 0,
+                 T2_ERR_INVALID_ARG, "dbg_taco_kernel PARAMS pack: bad arguments");
+      const int gates = W == 32 ? 4 : 2;
+      T2_REQUIRE(perm == 0 || (perm > 0 && transpose && perm % W == 0 && (long long)gates * perm == N), T2_ERR_INVALID_ARG,
+                 "dbg_taco_kernel PARAMS pack: gate permutation %d needs a transposing job with N = %d * perm and perm %% %d == 0", perm, gates, W);
+      const int extent = transpose ? K : N;     // columns each destination row receives from col0 on
+      T2_REQUIRE(ld >= col0 + extent && (!split || (ld >= col0 + slot + extent && ld >= col_lo + extent)), T2_ERR_INVALID_ARG,
+                 "dbg_taco_kernel PARAMS pack: destination columns beyond the leading dimension %d", ld);
+      std::vector<PackJob> jobs;
+      if (split) add_pack_split(jobs, src, K, N, 2 * dst, ld, col0, col_lo, slot, call->f[0], perm);
+      else {
+        add_pack(jobs, src, K, N, 2 * dst, ld, transpose, col0, call->f[0], perm);
+        jobs.back().part = part;
+      }
+      T2_REQUIRE(i[1] >= (long long)(jobs.size() * sizeof(PackJob)), T2_ERR_INVALID_ARG, "dbg_taco_kernel PARAMS pack: job buffer of %lld B < %zu B",
+                 i[1], jobs.size() * sizeof(PackJob));
+      T2_CHECK_CUDA(cudaMemcpyAsync(p[2], jobs.data(), jobs.size() * sizeof(PackJob), cudaMemcpyHostToDevice, st));
+      return launch_pack(static_cast<const float*>(p[0]), p[1], static_cast<const PackJob*>(p[2]), int(jobs.size()), W, grid_x, st);
+    }
     default:
       return t2_set_error(T2_ERR_INVALID_ARG, "dbg_taco_kernel: unknown kernel id %d", call->kernel);
   }

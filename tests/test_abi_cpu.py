@@ -328,3 +328,101 @@ def test_att_fwd_hook_rejects_lo_offsets_in_bf16_mode_and_rows_rejects_a_bad_wri
     assert rc == -1 and b"bad writer" in err, err
     rc, err = _taco_hook(10, _FAKE[:8], [1, 1, 2, 8, 129])        # split decoder-input rows hold at most 128 mels per half
     assert rc == -1 and b"decin" in err, err
+
+
+def _cbhg_hook(kernel, p, i, f=()):
+    from t2_import import t2
+    lib = t2.lib.load()
+    c = t2.lib.DbgKernel()
+    c.kernel = kernel
+    for k, v in enumerate(p):
+        c.p[k] = v
+    for k, v in enumerate(i):
+        c.i[k] = v
+    for k, v in enumerate(f):
+        c.f[k] = v
+    return lib.t2_dbg_cbhg_kernel(ctypes.byref(c), None), lib.t2_last_error()
+
+
+# the loss / parameter-table hooks of tests/test_taco_loss_kernels_gpu.py: one broken argument each, refused before any driver call
+LOSS_GOOD = {0: [0, 2, 5, 80, 1], 1: [1, 2, 5, 80, 0], 2: [2, 2, 5, 80, 1], 3: [3, 2, 5, 80, 1, 0, 5], 4: [4, 10, 80], 5: [5, 100],
+             6: [6, 10, 512], 7: [7, 2, 5, 512], 8: [8, 100, 80, 128, 256]}
+
+
+@pytest.mark.parametrize("i,p_null,msg", [
+    ([0, 2, 5, 128, 1], None, b"bad shape"), ([2, 2, 5, 80, 2], None, b"clip flag"), ([0, 0, 5, 80, 1], None, b"bad shape"),
+    (LOSS_GOOD[0], 0, b"mel_finish: null"), (LOSS_GOOD[1], 0, b"loss_norm: null"), (LOSS_GOOD[2], 7, b"loss_seed: null"),
+    ([3, 2, 5, 80, 1, 3, 3], None, b"step range"), ([3, 2, 5, 80, 1, 0, 6], None, b"step range"), (LOSS_GOOD[3], 8, b"choice is required"),
+    ([4, 10, 128], None, b"proj_bias"), (LOSS_GOOD[4], 2, b"proj_bias"), ([5, 0], None, b"relu_drop_bwd"), ([6, 10, 0], None, b"embed_bwd"),
+    (LOSS_GOOD[7], 1, b"mask_values"), ([8, 100, 80, 64, 256], None, b"bias_colsum"), ([8, 100, 80, 128, 64], None, b"bias_colsum"),
+    ([9, 1, 1, 1, 1], None, b"selector")])
+def test_loss_hook_rejects_bad_arguments(i, p_null, msg):
+    p = list(_FAKE[:9])
+    if p_null is not None:
+        p[p_null] = 0
+    rc, err = _taco_hook(11, p, i, [-4.1, 4.0, 1.0])
+    assert rc == -1 and msg in err, err
+
+
+def test_loss_hook_accepts_nothing_but_the_documented_rates_and_lengths():
+    rc, err = _taco_hook(11, _FAKE[:3], [5, 100], [1.0])              # relu_drop_bwd: dropout rate 1 divides by 0
+    assert rc == -1 and b"relu_drop_bwd" in err, err
+    rc, err = _taco_hook(11, _FAKE[:3], [6, 0, 8])
+    assert rc == -1 and b"embed_bwd" in err, err
+
+
+PACK_GOOD = [0, 4096, 32, 32, 0, 64, 128, 0, 64, 1, 0, 32, 0]         # -, bytes, W, grid_x, src, K, N, dst, ld, transpose, col0, perm, part
+PACK_SPLIT_GOOD = [1, 4096, 32, 32, 0, 64, 128, 0, 192, 0, 128, 64, 32]  # -, bytes, W, grid_x, src, K, N, dst, ld, col_hi, col_lo, slot, perm
+
+
+@pytest.mark.parametrize("split,k,v,msg", [
+    (0, 11, 16, b"gate permutation"), (0, 11, 64, b"gate permutation"), (0, 9, 0, b"gate permutation"), (0, 6, 129, b"gate permutation"),
+    (0, 2, 64, b"bad arguments"), (0, 12, 1, b"bad arguments"), (0, 5, 0, b"bad arguments"), (0, 3, 0, b"bad arguments"),
+    (0, 8, 63, b"leading dimension"), (0, 1, 47, b"job buffer"), (1, 12, 96, b"gate permutation"), (1, 2, 128, b"gate permutation"),
+    (1, 8, 191, b"leading dimension"), (1, 1, 143, b"job buffer"), (1, 11, -1, b"bad arguments")])
+def test_pack_hook_rejects_bad_jobs(split, k, v, msg):
+    """a gate permutation must transpose, with N = gates * perm and perm % W == 0 (W = 32: 4 gates, W = 128: 2 halves); a PackJob is
+    48 bytes, so one job needs 48 B of job buffer and a split triple 144 B"""
+    i = list(PACK_SPLIT_GOOD if split else PACK_GOOD)
+    i[k] = v
+    rc, err = _taco_hook(12, _FAKE[:3], i, [1.0])
+    assert rc == -1 and msg in err, err
+
+
+def test_params_hook_rejects_null_pointers_and_empty_tables():
+    rc, err = _taco_hook(12, [_FAKE[0], 0, _FAKE[2]], PACK_GOOD, [1.0])
+    assert rc == -1 and b"pack: bad arguments" in err, err
+    for which in (2, 3):
+        rc, err = _taco_hook(12, _FAKE[:3], [which, 0], [1e-6])
+        assert rc == -1 and b"reg" in err, err
+        rc, err = _taco_hook(12, [_FAKE[0], 0, _FAKE[2]], [which, 4], [1e-6])
+        assert rc == -1 and b"reg" in err, err
+    rc, err = _taco_hook(12, _FAKE[:3], [4, 1])
+    assert rc == -1 and b"selector" in err, err
+
+
+LIN_GOOD = [2, 5, 1025, 1032, 185, 1]                                # B, T, NF, NFP, n_prio, clip
+
+
+@pytest.mark.parametrize("k,v", [(3, 1024), (4, 0), (4, 1026), (5, 2), (0, 0), (1, 0), (2, 0)])
+def test_linear_hook_rejects_bad_arguments(k, v):
+    i = list(LIN_GOOD)
+    i[k] = v
+    rc, err = _cbhg_hook(9, _FAKE[:6], i, [-4.1, 4.0, 1e-6])
+    assert rc == -1 and b"LINEAR" in err, err
+
+
+def test_linear_and_add_hooks_reject_null_pointers_and_bad_selectors():
+    for null in (0, 3):
+        p = list(_FAKE[:6])
+        p[null] = 0
+        rc, err = _cbhg_hook(9, p, LIN_GOOD, [-4.1, 4.0, 1e-6])
+        assert rc == -1 and b"LINEAR" in err, err
+    rc, err = _cbhg_hook(10, _FAKE[:5], [2, 10])
+    assert rc == -1 and b"selector" in err, err
+    rc, err = _cbhg_hook(10, [0] + _FAKE[1:3], [0, 10])
+    assert rc == -1 and b"add_k" in err, err
+    rc, err = _cbhg_hook(10, _FAKE[:5], [1, 10, 129])
+    assert rc == -1 and b"dmel_k" in err, err
+    rc, err = _cbhg_hook(10, _FAKE[:4] + [0], [1, 10, 80])
+    assert rc == -1 and b"dmel_k" in err, err

@@ -31,8 +31,9 @@ COVERAGE maps every __global__ kernel of the two files and of the kernels they s
 launches it (the shared batch-norm kernels are launched by both the Tacotron and the CBHG batch-norm tests);
 a COVERAGE value is either the name of a test here or `file::test` for a per-kernel test in another module (att_bwd_kernel:
 tests/test_attention_state_gpu.py; the two GRU kernels: tests/test_cbhg_gru_gpu.py; the split row writers:
-tests/test_split_operands_gpu.py). EXEMPT names the existing end-to-end test that covers
-each plumbing kernel (packing, embedding, losses, column sums).
+tests/test_split_operands_gpu.py; the loss, gradient-seed, parameter-packing, regulariser and column-sum kernels:
+tests/test_taco_loss_kernels_gpu.py). EXEMPT, which would name an end-to-end test covering a kernel without a per-launch test, is
+empty.
 test_every_engine_and_shared_kernel_is_covered (CPU) fails for a kernel added without an entry."""
 import ctypes
 import math
@@ -69,27 +70,25 @@ COVERAGE = {
     "dvalues_ctx_kernel": "test_dvalues_ctx", "att_bwd_kernel": "test_attention_state_gpu.py::test_att_bwd",
     "gru_fwd_kernel": "test_cbhg_gru_gpu.py::test_gru_fwd", "gru_bwd_kernel": "test_cbhg_gru_gpu.py::test_gru_bwd",
     "embed_fwd_kernel": "test_split_operands_gpu.py::test_embed_fwd_split", "decin_kernel": "test_split_operands_gpu.py::test_decin_split",
-    "dec_finish_kernel": "test_split_operands_gpu.py::test_dec_finish_split",
     "proj_bias_feedback_kernel": "test_split_operands_gpu.py::test_proj_bias_feedback_split",
     "f32_to_bf16_kernel": "test_split_operands_gpu.py::test_f32_to_bf16_split",
 }
-_TACO_E2E = "test_tacotron_gpu.py::test_backward_matches_oracle"
-_CBHG_E2E = "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle"
-EXEMPT = {
-    "pack_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
-    "embed_bwd_kernel": _TACO_E2E, "bias_colsum_kernel": _TACO_E2E, "mask_values_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
-    "mel_finish_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "reg_loss_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle",
-    "proj_bias_kernel": "test_tacotron_gpu.py::test_forward_matches_oracle", "loss_norm_kernel": "test_tacotron_gpu.py::test_masked_decoder_losses_match_oracle",
-    "loss_seed_kernel": _TACO_E2E, "ddec_tm_kernel": _TACO_E2E, "relu_drop_bwd_kernel": "test_parity_full_gpu.py::test_tacotron_training_mode_stochastic_paths_small",
-    "reg_grad_kernel": _TACO_E2E,
-    "add_k": _CBHG_E2E, "lin_finish_k": _CBHG_E2E,
-    "lin_norm_k": "test_cbhg_gpu.py::test_cbhg_engine_matches_oracle", "loss_out_k": _CBHG_E2E, "dmel_k": _CBHG_E2E,
-}
+_LK = "test_taco_loss_kernels_gpu.py::"
+COVERAGE.update({
+    "dec_finish_kernel": _LK + "test_decoder_loss_chain", "mel_finish_kernel": _LK + "test_decoder_loss_chain",
+    "loss_norm_kernel": _LK + "test_decoder_loss_chain", "loss_seed_kernel": _LK + "test_decoder_loss_chain",
+    "ddec_tm_kernel": _LK + "test_decoder_loss_chain", "proj_bias_kernel": _LK + "test_proj_bias",
+    "relu_drop_bwd_kernel": _LK + "test_relu_drop_bwd", "embed_bwd_kernel": _LK + "test_embed_bwd", "mask_values_kernel": _LK + "test_mask_values",
+    "lin_norm_k": _LK + "test_linear_loss", "lin_finish_k": _LK + "test_linear_loss", "loss_out_k": _LK + "test_linear_loss",
+    "add_k": _LK + "test_add_k", "dmel_k": _LK + "test_dmel_k", "pack_kernel": _LK + "test_pack",
+    "reg_loss_kernel": _LK + "test_reg_loss_and_grad", "reg_grad_kernel": _LK + "test_reg_loss_and_grad",
+    "bias_colsum_kernel": _LK + "test_bias_colsum",
+})
+EXEMPT = {}
 
 
 def test_every_engine_and_shared_kernel_is_covered():
-    """CPU: every __global__ kernel of t2_tacotron.cu / t2_cbhg.cu / t2_params.cu / t2_batchnorm.cu is launched by a test here, or exempted
-    with the name of an existing test that covers it end to end"""
+    """CPU: every __global__ kernel of t2_tacotron.cu / t2_cbhg.cu / t2_params.cu / t2_batchnorm.cu is launched by a per-kernel test"""
     names = set()
     for f in ("t2_tacotron.cu", "t2_cbhg.cu", "t2_params.cu", "t2_batchnorm.cu"):
         src = open(os.path.join(ROOT, "tacotron-2_b200", "csrc", f)).read()
@@ -97,7 +96,7 @@ def test_every_engine_and_shared_kernel_is_covered():
     assert len(names) >= 39
     missing = sorted(n for n in names if n not in COVERAGE and n not in EXEMPT)
     assert not missing, "kernels without a test: %s" % missing
-    assert not set(COVERAGE) & set(EXEMPT)
+    assert not set(COVERAGE) & set(EXEMPT) and not EXEMPT
     for k, t in list(COVERAGE.items()) + list(EXEMPT.items()):
         f, name = t.split("::") if "::" in t else (os.path.basename(__file__), t)
         assert re.search(r"^def %s\(" % name, open(os.path.join(ROOT, "tests", f)).read(), re.M), (k, t)
