@@ -646,6 +646,24 @@ int t2_mel_basis_f64(const t2_audio_config_t* cfg, double* h_basis);
 int t2_griffin_lim_bytes(const t2_audio_config_t* cfg, int B, int frames, long long* bytes);
 int t2_griffin_lim_f32(const t2_audio_config_t* cfg, const void* d_plan, const float* d_mag, float* d_phase_io, int B, int frames,
                        int iters, unsigned long long seed, void* d_workspace, float* d_wav, void* stream);
+/* One launch of an audio front-end kernel on caller buffers (t2_dbg_kernel_t above), through the launcher t2_stft_mel_f32 /
+ * t2_griffin_lim_f32 use, so grid, block and shared memory are the product's (tests/test_audio_kernels_gpu.py). cfg must pass the
+ * plan checks of t2_stft_mel_plan_bytes; plan is a device plan built for cfg by t2_stft_mel_plan_init; bins = n_fft/2 + 1. Every
+ * argument is checked before any driver call; no temporaries are allocated. Does not synchronise.
+ * STFT_MEL       stft_mel_kernel_v2. p: plan, wav fp32 [B][n_samples], mel fp32, lin fp32 (nullable), laid out as t2_stft_mel_f32's.
+ *                i: B (1..65535), n_samples (1..2^30), time_major (0 / 1). f: preemphasis, gain (finite).
+ * GL_INIT_PHASE  gl_init_phase_kernel. p: phase float2 [n] (out: exp(2 pi i u), u the counter hash of the element index under seed).
+ *                i: n (1..2^36). seed.
+ * GL_ISTFT       gl_istft_kernel. p: plan, mag fp32 [B][frames][bins], phase float2 [B][frames][bins], frames fp32 [B][frames][win_size]
+ *                (out: the windowed inverse transforms). i: B (1..65535), frames (2..2^24, hop (frames - 1) < 2^31).
+ * GL_OLA         gl_ola_kernel. p: plan, frames fp32 [B][frames][win_size], y fp32 [B][hop (frames - 1)] (out). i: as GL_ISTFT.
+ * GL_STFT        gl_stft_kernel. p: plan, y fp32 [B][hop (frames - 1)], phase float2 [B][frames][bins] (out: unit phases). i: as GL_ISTFT. */
+#define T2_DBG_AUDIO_STFT_MEL 1
+#define T2_DBG_AUDIO_GL_INIT_PHASE 2
+#define T2_DBG_AUDIO_GL_ISTFT 3
+#define T2_DBG_AUDIO_GL_OLA 4
+#define T2_DBG_AUDIO_GL_STFT 5
+int t2_dbg_audio_kernel(const t2_audio_config_t* cfg, const t2_dbg_kernel_t* call, void* stream);
 int t2_preemphasis_f32(const float* d_x, float* d_y, int B, int n_samples, float k, void* stream);
 /* mu-law (mu forced to 255 like util.py:48,67,99,127); quantise truncates toward zero */
 int t2_mulaw_quantize_f32_i32(const float* d_in, int* d_out, long long n, void* stream);

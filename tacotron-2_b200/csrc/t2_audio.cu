@@ -4,18 +4,19 @@
 // librosa.stft, center=True, pad_mode='constant'), :225-270 (_linear_to_mel, _amp_to_db, _normalize) and
 // wavenet_vocoder/util.py:30-129 (mu-law family) of the reference.
 //
-// One CTA transforms one frame at a time: the Hann-windowed frame (only win_size of the n_fft samples are non-zero)
-// is packed as n_fft/2 complex points, run through a shared-memory radix-4 Stockham FFT, untangled into the
-// n_fft/2+1 real-FFT bins, squared, contracted with the SPARSE triangular mel filters, converted to dB and
-// normalised — one HBM read of the samples, one HBM write of num_mels floats per frame, nothing in between.
+// Each frame is transformed by its own n_fft/32 threads of a 256-thread CTA: the Hann-windowed frame (only win_size of the
+// n_fft samples are non-zero) is packed as n_fft/2 complex points, run through a register-radix Stockham FFT, untangled into
+// the n_fft/2+1 real-FFT bins, raised to magnitude_power, contracted with the SPARSE triangular mel filters, converted to dB
+// and normalised — one HBM read of the samples, one HBM write of num_mels floats per frame, nothing in between.
 // The FFT runs in fp64: the reference's spectra come from a double-precision FFT (numpy) and the dB floor sits
 // ~100 dB under the spectral peak, which fp32 butterflies cannot resolve to the 1e-3 parity tolerance.
 // n_fft is 512, 1024, 2048 or 4096 (the reference's advice, hparams.py:52: the first power of two above win_size,
 // i.e. 8, 16, 22.05-24 and 44.1-48 kHz audio); the FFT kernels are instantiated once per complex length N = n_fft / 2.
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/t2b200.h"
@@ -24,10 +25,22 @@
 namespace t2 {
 namespace {
 
-constexpr int kV1Nfft = 2048;     // the v1 kernel (T2_STFT_V1=1) is sized for this n_fft only
 constexpr int kMaxMels = 128;
 
 bool nfft_supported(int n_fft) { return n_fft == 512 || n_fft == 1024 || n_fft == 2048 || n_fft == 4096; }
+bool in_range(long long v, long long lo, long long hi) { return v >= lo && v <= hi; }
+
+// calls f(std::integral_constant<int, N>) for the complex FFT length N = n_fft / 2 of a supported n_fft
+template <class F>
+int by_nfft(int n_fft, F&& f) {
+  switch (n_fft) {
+    case 512: return f(std::integral_constant<int, 256>());
+    case 1024: return f(std::integral_constant<int, 512>());
+    case 2048: return f(std::integral_constant<int, 1024>());
+    case 4096: return f(std::integral_constant<int, 2048>());
+    default: return t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "no audio kernel for n_fft %d", n_fft);
+  }
+}
 
 struct Plan {
   // byte offsets inside the device plan buffer
@@ -121,118 +134,13 @@ __device__ __forceinline__ float finish(const StftArgs& a, double v) {
   return r;
 }
 
-__global__ void __launch_bounds__(256) stft_mel_kernel(StftArgs a) {
-  constexpr int kNfft = kV1Nfft, kN = kNfft / 2, kBins = kN + 1;
-  __shared__ double2 buf0[kN];
-  __shared__ double2 buf1[kN];
-  __shared__ double pw[kBins + 7];
-  const int j = threadIdx.x;  // 256 threads = one radix-4 butterfly each per pass
-  const long long total = (long long)a.B * a.frames;
-  const int lpad = (kNfft - a.win_size) / 2;
-  for (long long fr = blockIdx.x; fr < total; fr += gridDim.x) {
-    const int b = int(fr / a.frames), f = int(fr % a.frames);
-    const float* w = a.wav + (long long)b * a.n_samples;
-    // 1. load + window, packed as z[n] = x[2n] + i x[2n+1]
-    for (int n = j; n < kN; n += 256) {
-      double v[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int q = 2 * n + h;            // position inside the n_fft frame
-        const int wi = q - lpad;            // position inside the window
-        double s = 0.0;
-        if (wi >= 0 && wi < a.win_size) {
-          const long long si = (long long)f * a.hop - kNfft / 2 + q;  // centred, zero-padded signal
-          if (si >= 0 && si < a.n_samples) {
-            double x = double(w[si]);
-            if (a.preemph != 0.f) x -= double(a.preemph) * (si > 0 ? double(w[si - 1]) : 0.0);
-            s = x * double(a.gain) * a.win[wi];
-          }
-        }
-        v[h] = s;
-      }
-      buf0[n] = make_double2(v[0], v[1]);
-    }
-    __syncthreads();
-    // 2. radix-4 Stockham autosort FFT, 5 passes (Ns = 1, 4, 16, 64, 256)
-    double2* src = buf0;
-    double2* dst = buf1;
-#pragma unroll 1
-    for (int Ns = 1; Ns < kN; Ns *= 4) {
-      const int k = j & (Ns - 1);
-      const int step = kN / (4 * Ns);
-      double2 v0 = src[j], v1 = src[j + kN / 4], v2 = src[j + kN / 2], v3 = src[j + 3 * kN / 4];
-      if (Ns > 1) {
-        v1 = cmul(v1, a.tw[k * step]);
-        v2 = cmul(v2, a.tw[2 * k * step]);
-        v3 = cmul(v3, a.tw[3 * k * step]);
-      }
-      // DFT-4 (forward): [1,1,1,1; 1,-i,-1,i; 1,-1,1,-1; 1,i,-1,-i]
-      const double2 s02 = make_double2(v0.x + v2.x, v0.y + v2.y), d02 = make_double2(v0.x - v2.x, v0.y - v2.y);
-      const double2 s13 = make_double2(v1.x + v3.x, v1.y + v3.y), d13 = make_double2(v1.x - v3.x, v1.y - v3.y);
-      const int j0 = ((j - k) << 2) + k;  // (j / Ns) * Ns * 4 + k
-      dst[j0] = make_double2(s02.x + s13.x, s02.y + s13.y);
-      dst[j0 + Ns] = make_double2(d02.x + d13.y, d02.y - d13.x);       // d02 - i d13
-      dst[j0 + 2 * Ns] = make_double2(s02.x - s13.x, s02.y - s13.y);
-      dst[j0 + 3 * Ns] = make_double2(d02.x - d13.y, d02.y + d13.x);   // d02 + i d13
-      __syncthreads();
-      double2* t = src; src = dst; dst = t;
-    }
-    // 3. untangle to the real-FFT bins and take |X|^p
-    for (int k = j; k <= kN; k += 256) {
-      const double2 zk = src[k & (kN - 1)];
-      const double2 zn = src[(kN - k) & (kN - 1)];
-      const double2 e = make_double2(0.5 * (zk.x + zn.x), 0.5 * (zk.y - zn.y));
-      const double2 o = make_double2(0.5 * (zk.y + zn.y), -0.5 * (zk.x - zn.x));  // -i/2 (zk - conj zn)
-      const int kk = k <= kN / 2 ? k : kN - k;
-      double2 t2w = a.tw2[kk];
-      if (k > kN / 2) t2w = make_double2(-t2w.x, t2w.y);  // W^(N-kk) = -conj(W^kk)
-      const double2 ow = cmul(o, t2w);
-      const double re = e.x + ow.x, im = e.y + ow.y;
-      // librosa stores the STFT as complex64 before |.|: round the components like the reference does
-      const float ref = float(re), imf = float(im);
-      double mag2 = double(ref) * double(ref) + double(imf) * double(imf);
-      double val;
-      if (a.mag_power == 2.f) {
-        const float m = sqrtf(float(mag2));  // np.abs(complex64) -> float32, then ** 2 in float32
-        val = double(m * m);
-      } else {
-        val = double(powf(sqrtf(float(mag2)), a.mag_power));
-      }
-      pw[k] = val;
-      if (a.lin) {
-        const float r = finish(a, val);
-        if (a.time_major) a.lin[((long long)b * a.frames + f) * kBins + k] = r;
-        else a.lin[((long long)b * kBins + k) * a.frames + f] = r;
-      }
-    }
-    __syncthreads();
-    // 4. sparse mel filterbank (fp64 accumulate, like np.dot with the float64 basis) + dB + normalise
-    const int warp = j >> 5, lane = j & 31;
-    for (int m = warp; m < a.nm; m += 8) {
-      const int s = a.fstart[m], n = a.fcount[m];
-      const double* fw = a.fw + a.foff[m];
-      double acc = 0.0;
-      for (int i = lane; i < n; i += 32) acc += fw[i] * pw[s + i];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-      if (lane == 0) {
-        const float r = finish(a, acc);
-        if (a.time_major) a.mel[((long long)b * a.frames + f) * a.nm + m] = r;
-        else a.mel[((long long)b * a.nm + m) * a.frames + f] = r;
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// ---- v2: register-radix FFT, 4096 / N frames per CTA ------------------------------------------------------------------------
+// ---- register-radix FFT, 4096 / N frames per CTA ----------------------------------------------------------------------------
 // N / 16 threads own one frame (16 complex points each); N = 16 x 16 x R Stockham passes (R = N / 256 = 1, 2, 4 or 8) with the
-// radix-16 butterflies held in registers, so a frame crosses shared memory at most three times (n_fft = 2048: instead of ten,
-// 5 radix-4 passes x read + write) and never needs a CTA-wide barrier: the threads of a frame meet on their own named barrier,
-// or on a half-warp __syncwarp when a frame is 16 threads. The first pass reads the windowed samples straight from global memory
-// (no staging pass). Shared-memory rows are padded by one element per 16 (17 j + r) so that the transposing stores of the
-// radix-16 passes are conflict-free for 16-byte elements. Post-FFT arithmetic is the v1 arithmetic. The CTA is 256 threads for
-// every N and a frame's shared memory grows with N, so every size keeps ~102.5 KB per CTA and 2 CTAs per SM.
+// radix-16 butterflies held in registers, so a frame crosses shared memory at most three times and never needs a CTA-wide
+// barrier: the threads of a frame meet on their own named barrier, or on a half-warp __syncwarp when a frame is 16 threads. The
+// first pass reads the windowed samples straight from global memory (no staging pass). Shared-memory rows are padded by one
+// element per 16 (17 j + r) so that the transposing stores of the radix-16 passes are conflict-free for 16-byte elements. The
+// CTA is 256 threads for every N and a frame's shared memory grows with N, so every size keeps ~102.5 KB per CTA and 2 CTAs per SM.
 constexpr int kCtaThreads = 256;
 template <int N>
 struct FftShape {
@@ -383,7 +291,8 @@ __global__ void __launch_bounds__(kCtaThreads, 2) stft_mel_kernel_v2(StftArgs a)
       v[r] = make_double2(c[0], c[1]);
     }
     fft_passes<N>(v, buf, a.tw, slot, j);
-    // untangle to the real-FFT bins and take |X|^p (v1 arithmetic)
+    // untangle to the real-FFT bins and take |X|^p; librosa stores the STFT as complex64 before |.|: round the components like the
+    // reference does, then np.abs(complex64) -> float32 and ** p in float32
     for (int k = j; k <= N; k += T) {
       const double2 zk = buf[padi(k & (N - 1))];
       const double2 zn = buf[padi((N - k) & (N - 1))];
@@ -626,24 +535,88 @@ int launch_stft_mel(const StftArgs& a, int sms, cudaStream_t st) {
   return T2_OK;
 }
 
+// One launcher per Griffin-Lim kernel, shared by launch_griffin_lim and t2_dbg_audio_kernel.
 template <int N>
-int launch_griffin_lim(const GlArgs& a, int iters, bool init_phase, unsigned long long seed, int sms, cudaStream_t st) {
+int launch_gl_istft(const GlArgs& a, int sms, cudaStream_t st) {
   constexpr int smem = FftShape<N>::kSmemBytes;
   static bool configured = false;
   if (!configured) {
     T2_CHECK_CUDA(cudaFuncSetAttribute(gl_istft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = true;
+  }
+  gl_istft_kernel<N><<<frame_grid<N>((long long)a.B * a.frames, sms), kCtaThreads, smem, st>>>(a); t2_count_launch();
+  return T2_OK;
+}
+template <int N>
+int launch_gl_stft(const GlArgs& a, int sms, cudaStream_t st) {
+  constexpr int smem = FftShape<N>::kSmemBytes;
+  static bool configured = false;
+  if (!configured) {
     T2_CHECK_CUDA(cudaFuncSetAttribute(gl_stft_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  const long long total = (long long)a.B * a.frames, ny = (long long)a.B * a.n_out;
-  const unsigned grid = frame_grid<N>(total, sms);
-  if (init_phase) { gl_init_phase_kernel<<<nblk(total * (N + 1)), 256, 0, st>>>(a.phase, total * (N + 1), seed); t2_count_launch(); }
+  gl_stft_kernel<N><<<frame_grid<N>((long long)a.B * a.frames, sms), kCtaThreads, smem, st>>>(a); t2_count_launch();
+  return T2_OK;
+}
+void launch_gl_ola(const GlArgs& a, cudaStream_t st) {
+  const long long ny = (long long)a.B * a.n_out;
+  gl_ola_kernel<<<nblk(ny), 256, 0, st>>>(a); t2_count_launch();
+}
+void launch_gl_init_phase(float2* ph, long long n, unsigned long long seed, cudaStream_t st) {
+  gl_init_phase_kernel<<<nblk(n), 256, 0, st>>>(ph, n, seed); t2_count_launch();
+}
+
+template <int N>
+int launch_griffin_lim(const GlArgs& a, int iters, bool init_phase, unsigned long long seed, int sms, cudaStream_t st) {
+  if (init_phase) launch_gl_init_phase(a.phase, (long long)a.B * a.frames * (N + 1), seed, st);
   for (int it = 0; it <= iters; ++it) {
-    gl_istft_kernel<N><<<grid, kCtaThreads, smem, st>>>(a); t2_count_launch();
-    gl_ola_kernel<<<nblk(ny), 256, 0, st>>>(a); t2_count_launch();
-    if (it < iters) { gl_stft_kernel<N><<<grid, kCtaThreads, smem, st>>>(a); t2_count_launch(); }
+    int rc = launch_gl_istft<N>(a, sms, st);
+    if (rc) return rc;
+    launch_gl_ola(a, st);
+    if (it < iters && (rc = launch_gl_stft<N>(a, sms, st))) return rc;
   }
   return T2_OK;
+}
+
+int device_sms() {
+  int dev = 0, sms = 148;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+// the kernel arguments of t2_stft_mel_f32 / t2_griffin_lim_f32 for a checked config, its plan and the caller's buffers
+StftArgs stft_args(const t2_audio_config_t* cfg, const Plan& p, const void* d_plan, const float* wav, int B, int n_samples,
+                   float preemphasis, float gain, float* mel, float* lin, int time_major) {
+  const uint8_t* pl = static_cast<const uint8_t*>(d_plan);
+  StftArgs a;
+  memset(&a, 0, sizeof(a));
+  a.wav = wav; a.mel = mel; a.lin = lin;
+  a.tw = reinterpret_cast<const double2*>(pl + p.o_tw);
+  a.tw2 = reinterpret_cast<const double2*>(pl + p.o_tw2);
+  a.win = reinterpret_cast<const double*>(pl + p.o_win);
+  a.fstart = reinterpret_cast<const int*>(pl + p.o_fstart);
+  a.fcount = reinterpret_cast<const int*>(pl + p.o_fcount);
+  a.foff = reinterpret_cast<const int*>(pl + p.o_foff);
+  a.fw = reinterpret_cast<const double*>(pl + p.o_fw);
+  a.B = B; a.n_samples = n_samples; a.frames = 1 + n_samples / cfg->hop_size; a.hop = cfg->hop_size;
+  a.win_size = cfg->win_size; a.nm = cfg->num_mels; a.time_major = time_major;
+  a.preemph = preemphasis; a.gain = gain; a.mag_power = cfg->magnitude_power;
+  a.min_level = float(exp(double(cfg->min_level_db) / 20.0 * log(10.0)));
+  a.min_level_db = cfg->min_level_db; a.ref_level_db = cfg->ref_level_db; a.max_abs = cfg->max_abs_value;
+  a.normalize = cfg->signal_normalization; a.symmetric = cfg->symmetric_mels; a.clip = cfg->allow_clipping_in_normalization;
+  return a;
+}
+GlArgs gl_args(const t2_audio_config_t* cfg, const Plan& p, const void* d_plan, int B, int frames) {
+  const uint8_t* pl = static_cast<const uint8_t*>(d_plan);
+  GlArgs a;
+  memset(&a, 0, sizeof(a));
+  a.tw = reinterpret_cast<const double2*>(pl + p.o_tw);
+  a.tw2 = reinterpret_cast<const double2*>(pl + p.o_tw2);
+  a.win = reinterpret_cast<const double*>(pl + p.o_win);
+  a.B = B; a.frames = frames; a.hop = cfg->hop_size; a.win_size = cfg->win_size; a.n_out = cfg->hop_size * (frames - 1);
+  a.n_fft = cfg->n_fft;
+  return a;
 }
 
 }  // namespace
@@ -706,45 +679,11 @@ extern "C" int t2_stft_mel_f32(const t2_audio_config_t* cfg, const void* d_plan,
   int rc = make_plan(cfg, p, nullptr);
   if (rc) return rc;
   T2_REQUIRE(d_plan && d_wav && d_mel && B >= 1 && n_samples >= 1, T2_ERR_INVALID_ARG, "stft_mel: bad arguments");
-  const uint8_t* pl = static_cast<const uint8_t*>(d_plan);
-  StftArgs a;
-  memset(&a, 0, sizeof(a));
-  a.wav = d_wav; a.mel = d_mel; a.lin = d_linear;
-  a.tw = reinterpret_cast<const double2*>(pl + p.o_tw);
-  a.tw2 = reinterpret_cast<const double2*>(pl + p.o_tw2);
-  a.win = reinterpret_cast<const double*>(pl + p.o_win);
-  a.fstart = reinterpret_cast<const int*>(pl + p.o_fstart);
-  a.fcount = reinterpret_cast<const int*>(pl + p.o_fcount);
-  a.foff = reinterpret_cast<const int*>(pl + p.o_foff);
-  a.fw = reinterpret_cast<const double*>(pl + p.o_fw);
-  a.B = B; a.n_samples = n_samples; a.frames = 1 + n_samples / cfg->hop_size; a.hop = cfg->hop_size;
-  a.win_size = cfg->win_size; a.nm = cfg->num_mels; a.time_major = time_major;
-  a.preemph = preemphasis; a.gain = gain; a.mag_power = cfg->magnitude_power;
-  a.min_level = float(exp(double(cfg->min_level_db) / 20.0 * log(10.0)));
-  a.min_level_db = cfg->min_level_db; a.ref_level_db = cfg->ref_level_db; a.max_abs = cfg->max_abs_value;
-  a.normalize = cfg->signal_normalization; a.symmetric = cfg->symmetric_mels; a.clip = cfg->allow_clipping_in_normalization;
-  const long long total = (long long)B * a.frames;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const StftArgs a = stft_args(cfg, p, d_plan, d_wav, B, n_samples, preemphasis, gain, d_mel, d_linear, time_major);
+  const int sms = device_sms();
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  static int use_v1 = -1;
-  if (use_v1 < 0) { const char* e = getenv("T2_STFT_V1"); use_v1 = (e && e[0] == '1') ? 1 : 0; }
-  if (use_v1) {
-    T2_REQUIRE(cfg->n_fft == kV1Nfft, T2_ERR_UNSUPPORTED_SHAPE, "T2_STFT_V1=1: the v1 kernel runs n_fft = %d only (got %d)", kV1Nfft, cfg->n_fft);
-    const long long cap = (long long)sms * 4;  // 4 resident CTAs per SM (41 KB smem, 256 threads each)
-    const unsigned grid = (unsigned)(total < cap ? total : cap);
-    stft_mel_kernel<<<grid, 256, 0, st>>>(a); t2_count_launch();
-  } else {
-    switch (cfg->n_fft) {
-      case 512: rc = launch_stft_mel<256>(a, sms, st); break;
-      case 1024: rc = launch_stft_mel<512>(a, sms, st); break;
-      case 2048: rc = launch_stft_mel<1024>(a, sms, st); break;
-      case 4096: rc = launch_stft_mel<2048>(a, sms, st); break;
-      default: rc = t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "stft_mel: no kernel for n_fft %d", cfg->n_fft);
-    }
-    if (rc) return rc;
-  }
+  rc = by_nfft(cfg->n_fft, [&](auto n) { return launch_stft_mel<decltype(n)::value>(a, sms, st); });
+  if (rc) return rc;
   T2_CHECK_CUDA(cudaGetLastError());
   return T2_OK;
 }
@@ -771,30 +710,71 @@ extern "C" int t2_griffin_lim_f32(const t2_audio_config_t* cfg, const void* d_pl
   int rc = make_plan(cfg, p, nullptr);
   if (rc) return rc;
   T2_REQUIRE(d_plan && d_mag && d_workspace && d_wav && B >= 1 && frames >= 2 && iters >= 0, T2_ERR_INVALID_ARG, "griffin_lim: bad arguments");
-  const uint8_t* pl = static_cast<const uint8_t*>(d_plan);
   uint8_t* ws = static_cast<uint8_t*>(d_workspace);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  GlArgs a;
-  memset(&a, 0, sizeof(a));
+  GlArgs a = gl_args(cfg, p, d_plan, B, frames);
   a.mag = d_mag;
   a.phase = d_phase_io ? reinterpret_cast<float2*>(d_phase_io) : reinterpret_cast<float2*>(ws);
   a.fr = reinterpret_cast<float*>(ws + al((long long)B * frames * (cfg->n_fft / 2 + 1) * 8));
   a.y = d_wav;
-  a.tw = reinterpret_cast<const double2*>(pl + p.o_tw);
-  a.tw2 = reinterpret_cast<const double2*>(pl + p.o_tw2);
-  a.win = reinterpret_cast<const double*>(pl + p.o_win);
-  a.B = B; a.frames = frames; a.hop = cfg->hop_size; a.win_size = cfg->win_size; a.n_out = cfg->hop_size * (frames - 1);
-  a.n_fft = cfg->n_fft;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = device_sms();
   const bool init_phase = d_phase_io == nullptr;
-  switch (cfg->n_fft) {
-    case 512: rc = launch_griffin_lim<256>(a, iters, init_phase, seed, sms, st); break;
-    case 1024: rc = launch_griffin_lim<512>(a, iters, init_phase, seed, sms, st); break;
-    case 2048: rc = launch_griffin_lim<1024>(a, iters, init_phase, seed, sms, st); break;
-    case 4096: rc = launch_griffin_lim<2048>(a, iters, init_phase, seed, sms, st); break;
-    default: rc = t2_set_error(T2_ERR_UNSUPPORTED_SHAPE, "griffin_lim: no kernel for n_fft %d", cfg->n_fft);
+  rc = by_nfft(cfg->n_fft, [&](auto n) { return launch_griffin_lim<decltype(n)::value>(a, iters, init_phase, seed, sms, st); });
+  if (rc) return rc;
+  T2_CHECK_CUDA(cudaGetLastError());
+  return T2_OK;
+}
+
+extern "C" int t2_dbg_audio_kernel(const t2_audio_config_t* cfg, const t2_dbg_kernel_t* call, void* stream) {
+  T2_REQUIRE(call != nullptr, T2_ERR_INVALID_ARG, "dbg_audio_kernel: null call");
+  Plan p;
+  int rc = make_plan(cfg, p, nullptr);
+  if (rc) return rc;
+  void* const* q = call->p;
+  const long long* i = call->i;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  switch (call->kernel) {
+    case T2_DBG_AUDIO_STFT_MEL: {
+      T2_REQUIRE(q[0] && q[1] && q[2], T2_ERR_INVALID_ARG, "dbg_audio_kernel STFT_MEL: null plan, wav or mel");
+      T2_REQUIRE(in_range(i[0], 1, 65535) && in_range(i[1], 1, 1 << 30), T2_ERR_UNSUPPORTED_SHAPE,
+                 "dbg_audio_kernel STFT_MEL: B must be in [1, 65535], n_samples in [1, 2^30]");
+      T2_REQUIRE(in_range(i[2], 0, 1) && std::isfinite(call->f[0]) && std::isfinite(call->f[1]), T2_ERR_INVALID_ARG,
+                 "dbg_audio_kernel STFT_MEL: time_major is 0 / 1, preemphasis and gain are finite");
+      const StftArgs a = stft_args(cfg, p, q[0], static_cast<const float*>(q[1]), int(i[0]), int(i[1]), call->f[0], call->f[1],
+                                   static_cast<float*>(q[2]), static_cast<float*>(q[3]), int(i[2]));
+      const int sms = device_sms();
+      rc = by_nfft(cfg->n_fft, [&](auto n) { return launch_stft_mel<decltype(n)::value>(a, sms, st); });
+      break;
+    }
+    case T2_DBG_AUDIO_GL_INIT_PHASE:
+      T2_REQUIRE(q[0] && in_range(i[0], 1, 1LL << 36), T2_ERR_INVALID_ARG, "dbg_audio_kernel GL_INIT_PHASE: null phase or n outside [1, 2^36]");
+      launch_gl_init_phase(static_cast<float2*>(q[0]), i[0], call->seed, st);
+      break;
+    case T2_DBG_AUDIO_GL_ISTFT:
+    case T2_DBG_AUDIO_GL_OLA:
+    case T2_DBG_AUDIO_GL_STFT: {
+      const int id = call->kernel;
+      const char* what = id == T2_DBG_AUDIO_GL_ISTFT ? "GL_ISTFT" : id == T2_DBG_AUDIO_GL_OLA ? "GL_OLA" : "GL_STFT";
+      T2_REQUIRE(q[0] && q[1] && q[2] && (id != T2_DBG_AUDIO_GL_ISTFT || q[3]), T2_ERR_INVALID_ARG, "dbg_audio_kernel %s: null pointer argument",
+                 what);
+      T2_REQUIRE(in_range(i[0], 1, 65535) && in_range(i[1], 2, 1 << 24) && (long long)cfg->hop_size * (i[1] - 1) < (1LL << 31),
+                 T2_ERR_UNSUPPORTED_SHAPE, "dbg_audio_kernel %s: B must be in [1, 65535], frames in [2, 2^24], hop (frames - 1) < 2^31", what);
+      GlArgs a = gl_args(cfg, p, q[0], int(i[0]), int(i[1]));
+      const int sms = device_sms();
+      if (id == T2_DBG_AUDIO_GL_ISTFT) {
+        a.mag = static_cast<const float*>(q[1]); a.phase = static_cast<float2*>(q[2]); a.fr = static_cast<float*>(q[3]);
+        rc = by_nfft(cfg->n_fft, [&](auto n) { return launch_gl_istft<decltype(n)::value>(a, sms, st); });
+      } else if (id == T2_DBG_AUDIO_GL_OLA) {
+        a.fr = static_cast<float*>(q[1]); a.y = static_cast<float*>(q[2]);
+        launch_gl_ola(a, st);
+      } else {
+        a.y = static_cast<float*>(q[1]); a.phase = static_cast<float2*>(q[2]);
+        rc = by_nfft(cfg->n_fft, [&](auto n) { return launch_gl_stft<decltype(n)::value>(a, sms, st); });
+      }
+      break;
+    }
+    default:
+      return t2_set_error(T2_ERR_INVALID_ARG, "dbg_audio_kernel: unknown kernel id %d", call->kernel);
   }
   if (rc) return rc;
   T2_CHECK_CUDA(cudaGetLastError());

@@ -78,3 +78,56 @@ def test_win_size_none_means_n_fft():
         cfg = t2.audio.make_config(hp)
         assert cfg.win_size == n_fft
         assert _plan_bytes(hp)[0] == 0
+
+
+# t2_dbg_audio_kernel (tests/test_audio_kernels_gpu.py): each call breaks one argument of an otherwise valid launch and is refused before
+# any driver call; the fake pointers are never dereferenced and nothing is launched
+_FAKE = [256 * (k + 1) for k in range(4)]
+_HOOK_GOOD = {1: (_FAKE, [3, 5000, 1]), 2: (_FAKE[:1], [1000]), 3: (_FAKE, [3, 40]), 4: (_FAKE[:3], [3, 40]), 5: (_FAKE[:3], [3, 40])}
+
+
+def _audio_hook(kernel, p, i, f=(0.97, 1.0), n_fft=1024):
+    lib = t2.lib.load()
+    hp = hp_for(16000, 1024, 200, 800)
+    hp.set_hparam("n_fft", n_fft)
+    cfg = t2.audio.make_config(hp)
+    c = t2.lib.DbgKernel()
+    c.kernel = kernel
+    for k, v in enumerate(p):
+        c.p[k] = v
+    for k, v in enumerate(i):
+        c.i[k] = v
+    for k, v in enumerate(f):
+        c.f[k] = v
+    return lib.t2_dbg_audio_kernel(ctypes.byref(cfg), ctypes.byref(c), None), lib.t2_last_error()
+
+
+@pytest.mark.parametrize("kernel,change,msg", [
+    (9, None, b"unknown kernel id"), (0, None, b"unknown kernel id"),
+    (1, ("p", 0), b"STFT_MEL: null"), (1, ("p", 1), b"STFT_MEL: null"), (1, ("p", 2), b"STFT_MEL: null"),
+    (1, ("i", 0, 0), b"STFT_MEL: B"), (1, ("i", 1, 0), b"STFT_MEL: B"), (1, ("i", 2, 2), b"time_major"), (1, ("i", 2, -1), b"time_major"),
+    (1, ("f", 0, float("nan")), b"finite"), (1, ("f", 1, float("inf")), b"finite"),
+    (2, ("p", 0), b"GL_INIT_PHASE"), (2, ("i", 0, 0), b"GL_INIT_PHASE"),
+    (3, ("p", 0), b"GL_ISTFT: null"), (3, ("p", 3), b"GL_ISTFT: null"), (3, ("i", 0, 0), b"GL_ISTFT: B"), (3, ("i", 1, 1), b"GL_ISTFT: B"),
+    (4, ("p", 2), b"GL_OLA: null"), (4, ("i", 0, 0), b"GL_OLA: B"), (4, ("i", 1, 1), b"GL_OLA: B"),
+    (5, ("p", 1), b"GL_STFT: null"), (5, ("i", 0, 0), b"GL_STFT: B"), (5, ("i", 1, 1), b"GL_STFT: B")])
+def test_audio_hook_refuses_bad_arguments_before_any_launch(kernel, change, msg):
+    lib = t2.lib.load()
+    n0 = lib.t2_launch_count()
+    p, i = _HOOK_GOOD.get(kernel, (_FAKE, [1, 1]))
+    p, i, f = list(p), list(i), [0.97, 1.0]
+    if change is not None:
+        if change[0] == "p":
+            p[change[1]] = 0
+        else:
+            {"i": i, "f": f}[change[0]][change[1]] = change[2]
+    rc, err = _audio_hook(kernel, p, i, f)
+    assert rc in (-1, -2) and msg in err, (rc, err)
+    assert lib.t2_launch_count() == n0
+
+
+@pytest.mark.parametrize("kernel", [1, 2, 3, 4, 5])
+def test_audio_hook_refuses_an_unsupported_n_fft(kernel):
+    p, i = _HOOK_GOOD[kernel]
+    rc, err = _audio_hook(kernel, list(p), list(i), n_fft=8192)
+    assert rc == T2_ERR_UNSUPPORTED_SHAPE and b"got 8192" in err, err
