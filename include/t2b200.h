@@ -206,7 +206,7 @@ typedef struct {
  *                                   stream-ordered). i: -, job buffer bytes, W (32: four LSTM gates, 128: two WaveNet gate halves),
  *                                   grid_x, src_off, K, N, dst_off (bf16 elements), dst_ld, transpose, col0, perm, part (0 / 2).
  *                                   f[0]: scale.
- *             1 pack_kernel, the three jobs of add_pack_split in one launch  p: as 0 (>= 3 sizeof(PackJob) B). i: -, bytes, W,
+ *             1 pack_kernel, the three jobs of a split-bf16 slot in one launch p: as 0 (>= 3 sizeof(PackJob) B). i: -, bytes, W,
  *                                   grid_x, src_off, K, N, dst_off, dst_ld, col_hi, col_lo, slot, perm. f[0]: scale.
  *                                   A job with perm > 0 must transpose, with N = gates * perm (gates = 4 for W = 32, 2 for W = 128)
  *                                   and perm % W == 0.

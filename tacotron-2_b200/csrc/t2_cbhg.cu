@@ -115,22 +115,17 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
   lo.p_lk = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/kernel", {2 * lo.RU, lo.NF}); lo.p_lb = add_param(lo.params, lo.n_params, "cbhg_linear_specs_projection/bias", {lo.NF});
 
   // ---- packed operands ----
-  // split_bf16: every forward operand is [W_hi | W_hi | W_lo] per K slot (add_pack_split; the split operand of launch_bias_act, t2_gemm.h), so its
-  // K pitch triples; the data-gradient operands of the backward pass keep their bf16 layout
+  // split_bf16: the forward operands take the split-bf16 layout (add_pack_fwd); the data-gradient operands of the backward pass keep
+  // their bf16 layout
   const bool split = cfg->split_bf16 != 0;
-  const int s3 = split ? 3 : 1;
   std::vector<PackJob> jobs;
   Arena pk;
   auto conv_pack = [&](CConv& L, bool with_t) {
     const int rows_f = (L.cout + 127) / 128 * 128, rows_t = (L.cin + 127) / 128 * 128;
-    L.k_w = pk.take(2LL * rows_f * L.k * L.cinp * s3);
+    L.k_w = pk.take(fwd_operand_bytes(rows_f, L.k * L.cinp, split));
     L.k_wT = with_t ? pk.take(2LL * rows_t * L.k * L.coutp) : 0;
     for (int j = 0; j < L.k; ++j) {
-      if (split)
-        add_pack_split(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp,
-                       3 * j * L.cinp + 2 * L.cinp, L.cinp);
-      else
-        add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd [cout][tap j | cin]
+      add_pack_fwd(jobs, split, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, j * L.cinp, L.cinp);   // fwd [cout][tap j | cin]
       if (with_t) add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.coutp, 0, j * L.coutp);   // dgrad [cin][tap j | cout]
     }
   };
@@ -151,41 +146,30 @@ int build(const t2_cbhg_config_t* cfg, CL& lo, std::vector<PackJob>* jobs_out) {
       for (int j = 0; j < lo.bank[l].k; ++j, ++slot)
         add_pack(jobs, lo.bank[l].p.kernel + (long long)j * lo.M * lo.CC, lo.M, lo.CC, lo.k_bankT[g], lo.grp_taps[g] * lo.CC, 0, slot * lo.CC);
   }
-  const int Mp = 128, Ms = (lo.M + 63) / 64 * 64;     // Ms: the K slot of num_mels in the split operands
-  if (split) { lo.k_dense = pk.take(2LL * lo.HU * 3 * Ms); add_pack_split(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, 3 * Ms, 0, 2 * Ms, Ms); }
-  else { lo.k_dense = pk.take(2LL * lo.HU * Mp); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_dense, Mp, 1, 0); }
+  const int Ms = (lo.M + 63) / 64 * 64;     // the K slot of num_mels: the half width of the split mel rows
+  lo.k_dense = pk.take(fwd_operand_bytes(lo.HU, Ms, split));
+  add_pack_fwd(jobs, split, lo.p_dk, lo.M, lo.HU, lo.k_dense, Ms, 0, Ms);
   lo.k_denseT = pk.take(2LL * 128 * lo.HU); add_pack(jobs, lo.p_dk, lo.M, lo.HU, lo.k_denseT, lo.HU, 0, 0);
   for (int i = 0; i < lo.NH; ++i) {
-    lo.k_hw[i] = pk.take(2LL * 2 * lo.HU * lo.HU * s3);        // rows [H units | T units][K = HU]
-    if (split) {
-      add_pack_split(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
-      add_pack_split(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
-    } else {
-      add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 1, 0);
-      add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + 2LL * lo.HU * lo.HU, lo.HU, 1, 0);
-    }
+    lo.k_hw[i] = pk.take(fwd_operand_bytes(2 * lo.HU, lo.HU, split));        // rows [H units | T units][K = HU]
+    add_pack_fwd(jobs, split, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hw[i], lo.HU, 0, lo.HU);
+    add_pack_fwd(jobs, split, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hw[i] + fwd_operand_bytes(lo.HU, lo.HU, split), lo.HU, 0, lo.HU);
     lo.k_hwT[i] = pk.take(2LL * lo.HU * 2 * lo.HU);            // [HU in][H units | T units]
     add_pack(jobs, lo.p_hk[i][0], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, 0);
     add_pack(jobs, lo.p_hk[i][1], lo.HU, lo.HU, lo.k_hwT[i], 2 * lo.HU, 0, lo.HU);
   }
   // GRU input projections: output columns [fw gates 2RU | fw cand RU | bw gates 2RU | bw cand RU], K = HU (the first HU kernel rows)
   const int XPW = 6 * lo.RU;
-  lo.k_gx = pk.take(2LL * XPW * lo.HU * s3);
+  lo.k_gx = pk.take(fwd_operand_bytes(XPW, lo.HU, split));
   lo.k_gxT = pk.take(2LL * lo.HU * XPW);
   for (int d = 0; d < 2; ++d) {
-    if (split) {
-      add_pack_split(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
-      add_pack_split(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * 3 * lo.HU, 3 * lo.HU, 0, 2 * lo.HU, lo.HU);
-    } else {
-      add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU) * lo.HU, lo.HU, 1, 0);
-      add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + 2LL * (d * 3 * lo.RU + 2 * lo.RU) * lo.HU, lo.HU, 1, 0);
-    }
+    add_pack_fwd(jobs, split, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gx + fwd_operand_bytes(d * 3 * lo.RU, lo.HU, split), lo.HU, 0, lo.HU);
+    add_pack_fwd(jobs, split, lo.p_ck[d], lo.HU, lo.RU, lo.k_gx + fwd_operand_bytes(d * 3 * lo.RU + 2 * lo.RU, lo.HU, split), lo.HU, 0, lo.HU);
     add_pack(jobs, lo.p_gk[d], lo.HU, 2 * lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU);
     add_pack(jobs, lo.p_ck[d], lo.HU, lo.RU, lo.k_gxT, XPW, 0, d * 3 * lo.RU + 2 * lo.RU);
   }
-  lo.k_lin = pk.take(2LL * lo.NFR * 2 * lo.RU * s3);
-  if (split) add_pack_split(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 6 * lo.RU, 0, 4 * lo.RU, 2 * lo.RU);
-  else add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 1, 0);
+  lo.k_lin = pk.take(fwd_operand_bytes(lo.NFR, 2 * lo.RU, split));
+  add_pack_fwd(jobs, split, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_lin, 2 * lo.RU, 0, 2 * lo.RU);
   const int NFK = (lo.NF + 63) / 64 * 64;
   lo.k_linT = pk.take(2LL * 2 * lo.RU * NFK); add_pack(jobs, lo.p_lk, 2 * lo.RU, lo.NF, lo.k_linT, NFK, 0, 0);
   lo.packed_bytes = pk.used;
@@ -771,7 +755,7 @@ int conv_fwd(const Ctx& s, const CConv& L, const void* x, int ld_x, bf16* y_b, f
   const int BN = L.cout % 256 == 0 ? 256 : 128;
   const int sp = s.lo->c.split_bf16;
   return launch_bias_act({.a = x, .C = L.cin, .ld = ld_x, .T = s.lo->T, .B = s.lo->B, .ntaps = L.k, .shifts = shifts, .split = sp, .w = s.pk + L.k_w,
-                          .N = (L.cout + 127) / 128 * 128, .wK = L.k * L.cinp * (sp ? 3 : 1), .BN = BN, .bias = s.params + L.p.bias, .act = L.act,
+                          .N = (L.cout + 127) / 128 * 128, .wK = L.k * L.cinp, .BN = BN, .bias = s.params + L.p.bias, .act = L.act,
                           .out_bf16 = y_b, .out_f32 = y_f, .ldo = ldo, .nvalid = L.cout},
                          s.st);
 }
@@ -791,7 +775,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   T2_CHECK_CUDA(cudaMemsetAsync(scal, 0, 16 * sizeof(float), st));
   // split_bf16: every bf16 operand below is a [hi | lo] row pair, every contraction a split GEMM (launch_bias_act), and the
   // pre-batch-norm activations of the bank and of proj1 are fp32
-  const int sp = lo.c.split_bf16, k3 = sp ? 3 : 1, Ms = (M + 63) / 64 * 64;
+  const int sp = lo.c.split_bf16, Ms = (M + 63) / 64 * 64;
   bf16* x0 = W<bf16>(s, lo.w_x0);
   if (sp) launch_f32_to_bf16_split(d_mel, x0, N, M, Ms, st);
   else launch_f32_to_bf16(d_mel, x0, N * M, st);
@@ -838,13 +822,13 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   if (sp) launch_f32_to_bf16_split(hin_f, hin, N, M, Ms, st);
   else launch_f32_to_bf16(hin_f, hin, N * M, st);
   // ---- dense to the highway width, highway layers ----
-  rc = launch_bias_act({.a = hin, .C = M, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_dense, .N = HU, .wK = sp ? 3 * Ms : 128, .BN = 128,
+  rc = launch_bias_act({.a = hin, .C = M, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_dense, .N = HU, .wK = Ms, .BN = 128,
                         .bias = d_params + lo.p_db, .out_bf16 = W<bf16>(s, lo.w_hb[0]), .out_f32 = W<float>(s, lo.w_hf[0]), .ldo = HU, .nvalid = HU},
                        st);
   if (rc) return rc;
   float* pre = W<float>(s, lo.w_XP);       // [N][2HU] scratch (the GRU input projections overwrite it afterwards)
   for (int i = 0; i < lo.NH; ++i) {
-    rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[i]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_hw[i], .N = 2 * HU, .wK = HU * k3,
+    rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[i]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_hw[i], .N = 2 * HU, .wK = HU,
                           .BN = 256, .out_f32 = pre, .ldo = 2 * HU, .nvalid = 2 * HU},
                          st);
     if (rc) return rc;
@@ -854,7 +838,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   // ---- bidirectional GRU ----
   const int XPW = 6 * RU;
   float* XP = W<float>(s, lo.w_XP);
-  rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[lo.NH]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_gx, .N = XPW, .wK = HU * k3, .BN = 256,
+  rc = launch_bias_act({.a = W<bf16>(s, lo.w_hb[lo.NH]), .C = HU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_gx, .N = XPW, .wK = HU, .BN = 256,
                         .out_f32 = XP, .ldo = XPW, .nvalid = XPW},
                        st);
   if (rc) return rc;
@@ -872,7 +856,7 @@ extern "C" int t2_cbhg_forward(const t2_cbhg_config_t* cfg, float* d_params, con
   }
   // ---- linear projection, clip, loss ----
   float* lin = W<float>(s, lo.w_lin);
-  rc = launch_bias_act({.a = W<bf16>(s, lo.w_out), .C = 2 * RU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_lin, .N = lo.NFR, .wK = 2 * RU * k3,
+  rc = launch_bias_act({.a = W<bf16>(s, lo.w_out), .C = 2 * RU, .T = T, .B = B, .split = sp, .w = s.pk + lo.k_lin, .N = lo.NFR, .wK = 2 * RU,
                         .BN = 128, .bias = d_params + lo.p_lb, .out_f32 = lin, .ldo = lo.NFP, .nvalid = lo.NF},
                        st);
   if (rc) return rc;

@@ -150,7 +150,41 @@ static int launch_one(const GemmArgs& g, dim3 grid, int cs, cudaStream_t stream)
   return T2_OK;
 }
 
-int make_gemm_args(int epi, int BN, const ActGemmCall& c, GemmArgs& g, dim3& grid, int& cs) {
+// the split-bf16 form of a plain call (ActGemmCall::split)
+static int split_form(ActGemmCall& c) {
+  T2_REQUIRE(c.na >= 1 && c.na <= 4 && c.nseg >= 1 && 2 * c.nseg <= kMaxSeg && c.w_k0 == 0, T2_ERR_UNSUPPORTED_SHAPE,
+             "split-bf16 GEMM: %d maps and %d segments (at most %d) from K column %d", c.na, c.nseg, kMaxSeg / 2, c.w_k0);
+  int nkb[4] = {0, 0, 0, 0}, ktot = 0;
+  for (int s = 0; s < c.nseg; ++s) {
+    const Seg& p = c.seg[s];
+    T2_REQUIRE(p.map >= 0 && p.map < c.na && p.k0 == 0 && p.nkb > 0 && (nkb[p.map] == 0 || nkb[p.map] == p.nkb), T2_ERR_INVALID_ARG,
+               "split-bf16 GEMM: segment %d must read its map from channel 0, as wide as the other segments of that map", s);
+    nkb[p.map] = p.nkb;
+    ktot += p.nkb * p.nlayers * kBK;
+  }
+  for (int i = 0; i < c.na; ++i) {
+    const int Cp = nkb[i] * kBK;
+    if (Cp) c.a[i] = make_act(c.a[i].ptr, 2 * Cp, c.a[i].T, c.a[i].B, c.a[i].L, 2 * Cp);
+  }
+  for (int s = c.nseg - 1; s >= 0; --s) {
+    const Seg p = c.seg[s];
+    c.seg[2 * s] = Seg{p.map, p.shift, 0, 2 * p.nkb, p.layer0, p.nlayers};
+    c.seg[2 * s + 1] = Seg{p.map, p.shift, 0, p.nkb, p.layer0, p.nlayers};
+  }
+  c.nseg *= 2;
+  c.wK = 3 * ktot;
+  c.epi.i[11] = 1;
+  return T2_OK;
+}
+
+int make_gemm_args(int epi, int BN, const ActGemmCall& call, GemmArgs& g, dim3& grid, int& cs) {
+  ActGemmCall split;
+  if (call.split) {
+    split = call;
+    const int rc = split_form(split);
+    if (rc) return rc;
+  }
+  const ActGemmCall& c = call.split ? split : call;
   // argument checks first: they touch neither the device nor the driver
   T2_REQUIRE(c.na >= 1 && c.na <= 4 && c.nseg >= 1 && c.nseg <= kMaxSeg, T2_ERR_INVALID_ARG,
              "act_gemm: bad map/segment count (%d, %d)", c.na, c.nseg);
@@ -214,35 +248,15 @@ long long* take_timing_slice(long long n_slots) {
   return p;
 }
 
-// split-bf16 ("fp32-class") operand A of an EPI_BIAS_ACT call: rows [hi | lo], each half C channels zero-padded to
-// Cp = ceil(C / kBK) * kBK (row pitch 2 Cp). Per tap one segment over both halves against [W_hi | W_hi] and one over the hi half
-// against [W_lo], so the packed weights hold 3 Cp K columns per tap (add_pack_split).
-static int set_split_operand(ActGemmCall& c, const void* a, int C, int T, int B, int ntaps, const int* shifts) {
-  const int nkb = (C + kBK - 1) / kBK, Cp = nkb * kBK;
-  T2_REQUIRE(2 * ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "split-bf16 GEMM: %d taps are more than %d segments", ntaps, kMaxSeg);
-  c.a[0] = make_act(a, 2 * Cp, T, B, 1, 2 * Cp); c.na = 1;
-  c.nseg = 0;
-  for (int s = 0; s < ntaps; ++s) {
-    c.seg[c.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, 2 * nkb, 0, 1};
-    c.seg[c.nseg++] = Seg{0, shifts ? shifts[s] : 0, 0, nkb, 0, 1};
-  }
-  c.epi.i[11] = 1;
-  return T2_OK;
-}
-
 int launch_bias_act(const BiasActGemm& g, cudaStream_t st) {
   ActGemmCall c;
   memset(&c, 0, sizeof(c));
-  if (g.split) {
-    const int rc = set_split_operand(c, g.a, g.C, g.T, g.B, g.ntaps, g.shifts);
-    if (rc) return rc;
-  } else {
-    T2_REQUIRE(g.ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "bias-act GEMM: %d taps are more than %d segments", g.ntaps, kMaxSeg);
-    const int Ctot = g.Ctot > 0 ? g.Ctot : g.C, nkb = (g.C + kBK - 1) / kBK;
-    c.a[0] = make_act(g.a, Ctot, g.T, g.B, 1, g.ld > 0 ? g.ld : Ctot); c.na = 1;
-    for (int s = 0; s < g.ntaps; ++s) c.seg[s] = Seg{0, g.shifts ? g.shifts[s] : 0, g.k0s ? g.k0s[s] : 0, nkb, 0, 1};
-    c.nseg = g.ntaps;
-  }
+  T2_REQUIRE(g.ntaps <= kMaxSeg, T2_ERR_UNSUPPORTED_SHAPE, "bias-act GEMM: %d taps are more than %d segments", g.ntaps, kMaxSeg);
+  const int Ctot = g.Ctot > 0 ? g.Ctot : g.C, nkb = (g.C + kBK - 1) / kBK;
+  c.a[0] = make_act(g.a, Ctot, g.T, g.B, g.layers, g.ld > 0 ? g.ld : Ctot); c.na = 1;
+  for (int s = 0; s < g.ntaps; ++s) c.seg[s] = Seg{0, g.shifts ? g.shifts[s] : 0, g.k0s ? g.k0s[s] : 0, nkb, 0, g.layers};
+  c.nseg = g.ntaps;
+  c.split = g.split;
   c.w = g.w; c.wN = g.N; c.wK = g.wK; c.wL = 1;
   c.T = g.T; c.B = g.B; c.n_tiles = (g.nvalid + g.BN - 1) / g.BN;
   c.epi.ptr[0] = g.out_bf16; c.epi.ptr[1] = const_cast<float*>(g.bias); c.epi.ptr[2] = g.out_f32;

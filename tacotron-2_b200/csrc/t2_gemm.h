@@ -31,6 +31,11 @@ struct ActGemmCall {
   int n_tiles;     // grid.y
   int ksplit;      // grid.z: CTAs sharing one output tile over slices of K (0/1 = off; epilogue must accumulate atomically)
   int cluster;     // requested weight-multicast cluster size along M: 0 = T2_CLUSTER / default, else 1, 2, 4 or 8
+  // split-bf16 ("fp32-class") operands. The call is given in its plain form; make_gemm_args launches its split form: every map
+  // becomes rows [hi(Cp) | lo(Cp)] of pitch 2 Cp, with Cp = nkb * kBK of the segments that read it (k0 = 0), every segment one of
+  // 2 nkb blocks over both halves and one of nkb blocks over the hi half, wK three times the segments' width (the packing of
+  // add_pack_fwd, t2_params.h; w_k0 = 0), and epi.i[11] = 1
+  int split;
   EpiArgs epi;
 };
 
@@ -63,8 +68,9 @@ struct BiasActGemm {
   const int* k0s = nullptr; int Ctot = 0;  // per-tap first channel (null = 0) of rows of Ctot addressable channels (0 = C)
   int T; int B;
   int ntaps = 1; const int* shifts = nullptr;   // tap j reads row t + shifts[j] (null = 0)
-  int split = 0;     // split-bf16 ("fp32-class") operand: rows [hi | lo] of pitch 2 Cp (ld, k0s and Ctot unused) against packed weights
-                     // [W_hi | W_hi | W_lo] (wK = 3 ntaps Cp, add_pack_split); a bf16 output is written as [hi(ldo) | lo(ldo)]
+  int layers = 1;    // K runs over the [layers][B][T] slabs of the operand, layers outer
+  int split = 0;     // split-bf16 ("fp32-class") operand (ActGemmCall::split): rows [hi | lo] of pitch 2 Cp (ld, k0s and Ctot unused)
+                     // against weights packed by add_pack_fwd; wK stays the plain one; a bf16 output is written as [hi(ldo) | lo(ldo)]
   const void* w; int N; int wK; int BN;    // packed bf16 weights [N][wK]; BN 128 or 256
   const float* bias = nullptr; int act = 0;
   void* out_bf16 = nullptr; float* out_f32 = nullptr; int ldo; int nvalid;   // columns [0, nvalid) of output rows of pitch ldo

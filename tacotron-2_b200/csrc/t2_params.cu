@@ -62,11 +62,14 @@ void add_pack(std::vector<PackJob>& jobs, long long src, int K, int N, long long
   jobs.push_back(j);
 }
 
-void add_pack_split(std::vector<PackJob>& jobs, long long src, int K, int N, long long dst_bytes, int ld, int col_hi, int col_lo, int slot,
-                    float scale, int perm) {
-  add_pack(jobs, src, K, N, dst_bytes, ld, 1, col_hi, scale, perm);
-  add_pack(jobs, src, K, N, dst_bytes, ld, 1, col_hi + slot, scale, perm);
-  add_pack(jobs, src, K, N, dst_bytes, ld, 1, col_lo, scale, perm);
+void add_pack_fwd(std::vector<PackJob>& jobs, bool split, long long src, int K, int N, long long dst_bytes, int Kw, int c, int Cp,
+                  float scale, int perm, int layer, int layers) {
+  const int x = layer * Cp, Ks = layers * Cp;
+  if (!split) {
+    add_pack(jobs, src, K, N, dst_bytes, Kw, 1, c + x, scale, perm);
+    return;
+  }
+  for (int col : {3 * c + 2 * x, 3 * c + 2 * x + Cp, 3 * c + 2 * Ks + x}) add_pack(jobs, src, K, N, dst_bytes, 3 * Kw, 1, col, scale, perm);
   jobs.back().part = 2;
 }
 

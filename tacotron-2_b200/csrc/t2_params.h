@@ -53,9 +53,17 @@ struct PackJob {
 };
 void add_pack(std::vector<PackJob>& jobs, long long src, int K, int N, long long dst_bytes, int ld, int transpose, int col0, float scale = 1.f,
               int perm = 0);
-// split-bf16 forward operand: the K slot of the plain layout becomes [W_hi | W_hi | W_lo] at columns col_hi, col_hi + slot and col_lo
-void add_pack_split(std::vector<PackJob>& jobs, long long src, int K, int N, long long dst_bytes, int ld, int col_hi, int col_lo, int slot,
-                    float scale = 1.f, int perm = 0);
+// Forward GEMM operands: packed bf16 weights [rows][Kw], K contiguous, whose columns the GEMM reads as plain segments of nkb 64-wide
+// blocks over nlayers layer slabs (Seg, t2_gemm_types.h). In the split-bf16 ("fp32-class") mode the operand is [rows][3 Kw]: a plain
+// segment that starts at column c and is Ks = nkb * 64 * nlayers wide has weight slots of Cp = nkb * 64 columns, and the slot at plain
+// column c + x is packed at split columns 3c + 2x and 3c + 2x + Cp (W_hi, both read against activation rows [hi | lo]) and 3c + 2Ks + x
+// (W_lo, read against the hi half). With one layer that is [W_hi | W_hi | W_lo] per slot; over layers, every layer's [W_hi | W_hi] and
+// then every layer's W_lo. The GEMM side of the rule is ActGemmCall::split (t2_gemm.h).
+inline long long fwd_operand_bytes(long long rows, long long Kw, bool split) { return 2 * rows * Kw * (split ? 3 : 1); }
+// fp32 [K][N] -> rows [0, N) of the forward operand at dst_bytes: the weight slot of `layer` in the plain segment that starts at column
+// c and loops over `layers` slots of Cp columns
+void add_pack_fwd(std::vector<PackJob>& jobs, bool split, long long src, int K, int N, long long dst_bytes, int Kw, int c, int Cp,
+                  float scale = 1.f, int perm = 0, int layer = 0, int layers = 1);
 // runs the jobs_dev[0, n_jobs) table at grid (grid_x, n_jobs) x (32, 8). W is the row block width of the gate permutation:
 // row = (u / W) * (gates * W) + g * W + u % W, with W = 128 for WaveNet's two gate halves (tanh | sigmoid) and W = 32 for the four
 // LSTM gates of the EPI_LSTM rows. The permutation is a bijection of the job's N rows only when the job transposes, N == gates * perm

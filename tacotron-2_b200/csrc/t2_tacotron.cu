@@ -136,69 +136,53 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   const bool split = cfg->split_bf16 != 0;
   auto conv_pack = [&](ConvL& L) {
     L.cinp = (L.cin + 63) / 64 * 64;
-    L.k_w = pk.take(2LL * L.cout * L.k * L.cinp * (split ? 3 : 1));
+    L.k_w = pk.take(fwd_operand_bytes(L.cout, L.k * L.cinp, split));
     L.k_wT = pk.take(2LL * L.cinp * L.k * L.cout);
     for (int j = 0; j < L.k; ++j) {
-      if (split) add_pack_split(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, 3 * L.k * L.cinp, 3 * j * L.cinp, 3 * j * L.cinp + 2 * L.cinp, L.cinp);
-      else
-      add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, 1, j * L.cinp);      // fwd: [cout][tap j | cin]
+      add_pack_fwd(jobs, split, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_w, L.k * L.cinp, j * L.cinp, L.cinp);   // fwd: [cout][tap j | cin]
       add_pack(jobs, L.p.kernel + (long long)j * L.cin * L.cout, L.cin, L.cout, L.k_wT, L.k * L.cout, 0, j * L.cout);     // dgrad: [cin][tap j | cout]
     }
   };
   for (auto& L : lo.enc) conv_pack(L);
   for (auto& L : lo.post) conv_pack(L);
   for (int d = 0; d < 2; ++d) {
-    lo.k_encWx[d] = pk.take(2LL * 4 * lo.H * lo.C * (split ? 3 : 1));            // [4H][C]  input projection (natural gate order)
-    if (split) add_pack_split(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], 3 * lo.C, 0, 2 * lo.C, lo.C);
-    else add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], lo.C, 1, 0);
-    lo.k_encWr[d] = pk.take(2LL * 4 * lo.H * lo.H * (split ? 3 : 1));   // [4H perm][H] recurrent, rows permuted for EPI_LSTM
-    if (split) add_pack_split(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], 3 * lo.H, 0, 2 * lo.H, lo.H, 1.f, lo.H);
-    else add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 1, 0, 1.f, lo.H);
+    lo.k_encWx[d] = pk.take(fwd_operand_bytes(4 * lo.H, lo.C, split));            // [4H][C]  input projection (natural gate order)
+    add_pack_fwd(jobs, split, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWx[d], lo.C, 0, lo.C);
+    lo.k_encWr[d] = pk.take(fwd_operand_bytes(4 * lo.H, lo.H, split));   // [4H perm][H] recurrent, rows permuted for EPI_LSTM
+    add_pack_fwd(jobs, split, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWr[d], lo.H, 0, lo.H, 1.f, lo.H);
     lo.k_encWrT[d] = pk.take(2LL * lo.H * 4 * lo.H);           // [H][4H] for the backward step
     add_pack(jobs, lo.p_elk[d] + (long long)lo.C * 4 * lo.H, lo.H, 4 * lo.H, lo.k_encWrT[d], 4 * lo.H, 0, 0);
   }
   lo.k_encWxT = pk.take(2LL * lo.C * 8 * lo.H);                // [C][fw 4H | bw 4H]
   for (int d = 0; d < 2; ++d) add_pack(jobs, lo.p_elk[d], lo.C, 4 * lo.H, lo.k_encWxT, 8 * lo.H, 0, d * 4 * lo.H);
-  lo.k_mem = pk.take(2LL * lo.A * 2 * lo.H * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 6 * lo.H, 0, 4 * lo.H, 2 * lo.H);
-  else add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 1, 0);
+  lo.k_mem = pk.take(fwd_operand_bytes(lo.A, 2 * lo.H, split));
+  add_pack_fwd(jobs, split, lo.p_mem, 2 * lo.H, lo.A, lo.k_mem, 2 * lo.H, 0, 2 * lo.H);
   lo.k_memT = pk.take(2LL * 2 * lo.H * lo.A); add_pack(jobs, lo.p_mem, 2 * lo.H, lo.A, lo.k_memT, lo.A, 0, 0);
-  const int Mp = 128;  // mel channels padded for TMA boxes
-  lo.k_p1 = pk.take(2LL * lo.P1 * Mp * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, 3 * Mp, 0, 2 * Mp, Mp);
-  else add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mp, 1, 0);
+  const int Mc = (lo.M + 63) / 64 * 64;   // the K slot of num_mels: the half width of the split mel rows
+  lo.k_p1 = pk.take(fwd_operand_bytes(lo.P1, Mc, split));
+  add_pack_fwd(jobs, split, lo.p_p1k, lo.M, lo.P1, lo.k_p1, Mc, 0, Mc);
   lo.k_p1T = pk.take(2LL * lo.M * lo.P1); add_pack(jobs, lo.p_p1k, lo.M, lo.P1, lo.k_p1T, lo.P1, 0, 0);
-  lo.k_p2 = pk.take(2LL * lo.P2 * lo.P1 * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, 3 * lo.P1, 0, 2 * lo.P1, lo.P1);
-  else add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 1, 0);
+  lo.k_p2 = pk.take(fwd_operand_bytes(lo.P2, lo.P1, split));
+  add_pack_fwd(jobs, split, lo.p_p2k, lo.P1, lo.P2, lo.k_p2, lo.P1, 0, lo.P1);
   lo.k_p2T = pk.take(2LL * lo.P1 * lo.P2); add_pack(jobs, lo.p_p2k, lo.P1, lo.P2, lo.k_p2T, lo.P2, 0, 0);
-  lo.k_l1x = pk.take(2LL * 4 * lo.D * lo.P2 * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, 3 * lo.P2, 0, 2 * lo.P2, lo.P2);
-  else add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 1, 0);
+  lo.k_l1x = pk.take(fwd_operand_bytes(4 * lo.D, lo.P2, split));
+  add_pack_fwd(jobs, split, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1x, lo.P2, 0, lo.P2);
   lo.k_l1xT = pk.take(2LL * lo.P2 * 4 * lo.D); add_pack(jobs, lo.p_l1k, lo.P2, 4 * lo.D, lo.k_l1xT, 4 * lo.D, 0, 0);
   const int K1r = 2 * lo.H + lo.D;
-  lo.k_l1r = pk.take(2LL * 4 * lo.D * K1r * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, 3 * K1r, 0, 2 * K1r, K1r, 1.f, lo.D);
-  else add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 1, 0, 1.f, lo.D);
+  lo.k_l1r = pk.take(fwd_operand_bytes(4 * lo.D, K1r, split));
+  add_pack_fwd(jobs, split, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1r, K1r, 0, K1r, 1.f, lo.D);
   lo.k_l1rT = pk.take(2LL * K1r * 4 * lo.D); add_pack(jobs, lo.p_l1k + (long long)lo.P2 * 4 * lo.D, K1r, 4 * lo.D, lo.k_l1rT, 4 * lo.D, 0, 0);
-  lo.k_l2 = pk.take(2LL * 4 * lo.D * K2 * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, 3 * K2, 0, 2 * K2, K2, 1.f, lo.D);
-  else add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 1, 0, 1.f, lo.D);
+  lo.k_l2 = pk.take(fwd_operand_bytes(4 * lo.D, K2, split));
+  add_pack_fwd(jobs, split, lo.p_l2k, K2, 4 * lo.D, lo.k_l2, K2, 0, K2, 1.f, lo.D);
   lo.k_l2T = pk.take(2LL * K2 * 4 * lo.D); add_pack(jobs, lo.p_l2k, K2, 4 * lo.D, lo.k_l2T, 4 * lo.D, 0, 0);
-  lo.k_proj = pk.take(2LL * 128 * PIK * (split ? 3 : 1));      // rows 0..M-1 frame projection, row M stop projection
-  if (split) {
-    add_pack_split(jobs, lo.p_fk, PIK, lo.M, lo.k_proj, 3 * PIK, 0, 2 * PIK, PIK);
-    add_pack_split(jobs, lo.p_sk, PIK, 1, lo.k_proj + 2LL * lo.M * 3 * PIK, 3 * PIK, 0, 2 * PIK, PIK);
-  } else {
-  add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_proj, PIK, 1, 0);
-  add_pack(jobs, lo.p_sk, PIK, 1, lo.k_proj + 2LL * lo.M * PIK, PIK, 1, 0);
-  }
+  lo.k_proj = pk.take(fwd_operand_bytes(128, PIK, split));      // rows 0..M-1 frame projection, row M stop projection
+  add_pack_fwd(jobs, split, lo.p_fk, PIK, lo.M, lo.k_proj, PIK, 0, PIK);
+  add_pack_fwd(jobs, split, lo.p_sk, PIK, 1, lo.k_proj + fwd_operand_bytes(lo.M, PIK, split), PIK, 0, PIK);
   lo.k_projT = pk.take(2LL * PIK * 128);                        // [PIK][128]: cols 0..M-1 Wf, col M Ws
   add_pack(jobs, lo.p_fk, PIK, lo.M, lo.k_projT, 128, 0, 0);
   add_pack(jobs, lo.p_sk, PIK, 1, lo.k_projT, 128, 0, lo.M);
-  lo.k_pp = pk.take(2LL * 128 * lo.PC * (split ? 3 : 1));
-  if (split) add_pack_split(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, 3 * lo.PC, 0, 2 * lo.PC, lo.PC);
-  else add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_pp, lo.PC, 1, 0);
+  lo.k_pp = pk.take(fwd_operand_bytes(128, lo.PC, split));
+  add_pack_fwd(jobs, split, lo.p_ppk, lo.PC, lo.M, lo.k_pp, lo.PC, 0, lo.PC);
   lo.k_ppT = pk.take(2LL * lo.PC * 128); add_pack(jobs, lo.p_ppk, lo.PC, lo.M, lo.k_ppT, 128, 0, 0);
   lo.k_qT = pk.take(2LL * lo.A * lo.D * (split ? 2 : 1));     // [A][D] for the attention kernel; split: [A][hi(D) | lo(D)]
   add_pack(jobs, lo.p_qry, lo.D, lo.A, lo.k_qT, split ? 2 * lo.D : lo.D, 1, 0);
@@ -211,7 +195,7 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   const long long B = lo.B, Ti = lo.Ti, To = lo.To;
   const long long xm = split ? 2 : 1;       // split-bf16: stored conv-stack activations are [hi | lo]; pre-batch-norm activations fp32
   const long long sm = split ? 3 : 1;       // split-bf16: recurrent state rows (the N operand of the swapped GEMMs) are [hi | lo | hi]
-  lo.ld_decin = split ? 2 * Mp : lo.M; lo.ld_pn1 = lo.P1 * int(xm); lo.ld_pn2 = lo.P2 * int(xm);
+  lo.ld_decin = split ? 2 * Mc : lo.M; lo.ld_pn1 = lo.P1 * int(xm); lo.ld_pn2 = lo.P2 * int(xm);
   lo.ld_S1 = K1r * int(sm); lo.ld_S2 = K2 * int(sm); lo.ld_PI = PIK * int(xm); lo.ld_mem = 2 * lo.H * int(xm);
   lo.w_emb = ws.take(B * Ti * lo.E * 2 * xm);
   auto conv_ws = [&](ConvL& L, long long T) {
@@ -228,7 +212,7 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   lo.w_memory = ws.take(B * Ti * lo.ld_mem * 2);
   lo.w_values = ws.take(B * Ti * lo.ld_mem * 2);
   lo.w_keys = ws.take(B * Ti * lo.A * 4);
-  lo.w_decin = ws.take(B * To * lo.ld_decin * 2);           // time-major [To][B][M]; split: [hi(M) padded to 128 | lo(M) padded to 128]
+  lo.w_decin = ws.take(B * To * lo.ld_decin * 2);           // time-major [To][B][M]; split: [hi(M) padded to Mc | lo(M) padded to Mc]
   lo.w_pn1 = ws.take(To * B * lo.ld_pn1 * 2);
   lo.w_pn2 = ws.take(To * B * lo.ld_pn2 * 2);
   lo.w_pre1 = ws.take(To * B * 4 * lo.D * 4);
@@ -241,7 +225,7 @@ int build(const t2_taco_config_t* cfg, TL& lo, std::vector<PackJob>* jobs_out) {
   lo.w_cum = ws.take(B * Ti * 4);
   lo.w_alpha = ws.take(To * B * Ti * 4);
   lo.w_projo = ws.take(To * B * 128 * 4);
-  lo.w_decbm = ws.take(split ? B * To * 256 * 2 : B * To * lo.M * 2);     /* split: [hi(M) padded to 128 | lo(M) padded to 128] */ lo.w_decf = ws.take(B * To * lo.M * 4); lo.w_stop = ws.take(B * To * 4);
+  lo.w_decbm = ws.take(B * To * lo.ld_decin * 2);     /* split: [hi(M) padded to Mc | lo(M) padded to Mc] */ lo.w_decf = ws.take(B * To * lo.M * 4); lo.w_stop = ws.take(B * To * 4);
   for (auto& L : lo.post) conv_ws(L, To);
   lo.w_tlen = ws.take(B * 4);
   lo.w_resid = ws.take(B * To * 128 * 4); lo.w_mel = ws.take(B * To * lo.M * 4);
@@ -315,16 +299,17 @@ __global__ void mask_values_kernel(const bf16* __restrict__ mem, const int* __re
   vals[e] = t < lens[b] ? mem[e] : __float2bfloat16(0.f);
 }
 // decoder inputs, time-major: dec_in[t][b][:] = t == 0 ? 0 : target[b][t-1][:]   (helpers.py:62-128, r = 1)
-// split: rows [hi(M) | pad | lo(M) | pad] of pitch 256 (the padding stays zero from t2_taco_init)
+// split: rows [hi(M) | pad | lo(M) | pad] of pitch 2 Cp, Cp = ceil(M / 64) * 64 (the padding stays zero from t2_taco_init)
 __global__ void decin_kernel(const float* __restrict__ tgt, bf16* __restrict__ out, int B, int To, int M, int split) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (e >= (long long)To * B * M) return;
   const int m = int(e % M), b = int((e / M) % B), t = int(e / ((long long)M * B));
   const float v = t == 0 ? 0.f : tgt[((long long)b * To + t - 1) * M + m];
   if (!split) { out[e] = __float2bfloat16(v); return; }
+  const int Cp = (M + 63) / 64 * 64;
   const bf16 hi = __float2bfloat16(v);
-  bf16* row = out + (e / M) * 256 + m;
-  row[0] = hi; row[128] = __float2bfloat16(v - __bfloat162float(hi));
+  bf16* row = out + (e / M) * 2 * Cp + m;
+  row[0] = hi; row[Cp] = __float2bfloat16(v - __bfloat162float(hi));
 }
 
 // ---- location-sensitive attention, one CTA per batch item per decoder step (attention.py:169-226) -------------
@@ -650,10 +635,11 @@ __global__ void dec_finish_kernel(const float* __restrict__ projo, const float* 
       const long long o = ((long long)b * To + t) * M + m;
       dec_f[o] = d;
       if (!split) dec_bm[o] = __float2bfloat16(d);
-      else {   // rows [hi(M) zero-padded to 128 | lo(M) zero-padded to 128] (the buffer is cleared once at init)
+      else {   // rows [hi(M) zero-padded to Cp | lo(M) zero-padded to Cp], Cp = ceil(M / 64) * 64 (the buffer is cleared once at init)
+        const int Cp = (M + 63) / 64 * 64;
         const bf16 h = __float2bfloat16(d);
-        bf16* row = dec_bm + ((long long)b * To + t) * 256 + m;
-        row[0] = h; row[128] = __float2bfloat16(d - __bfloat162float(h));
+        bf16* row = dec_bm + ((long long)b * To + t) * 2 * Cp + m;
+        row[0] = h; row[Cp] = __float2bfloat16(d - __bfloat162float(h));
       }
       if (tgt && live) { const float df = d - tgt[o]; l0 = df * df; }
     } else {
@@ -701,7 +687,7 @@ constexpr uint32_t kTfStream = 40;   // hash stream of the per-step teacher-forc
 // projo[t] += bias; next decoder input = the raw (un-clipped) frame just predicted (helpers.py:56). With tgt (TacoTrainingHelper at a
 // teacher-forcing ratio < 1, helpers.py:115-128): ONE draw u_t for the whole batch (stream kTfStream, element t, under seed + *step);
 // u_t < ratio feeds the target frame tgt[b][t] instead, and choice[t] records which of the two step t + 1 consumed.
-// split: next_in rows are the split decoder-input rows [hi(M) | pad | lo(M) | pad] of pitch 256 (decin_kernel)
+// split: next_in rows are the split decoder-input rows [hi(M) | pad | lo(M) | pad] of pitch 2 Cp (decin_kernel)
 __global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __restrict__ fb, const float* __restrict__ sb, bf16* __restrict__ next_in,
                                           int B, int M, const float* __restrict__ tgt, int To, int t, float ratio, unsigned long long seed,
                                           const unsigned long long* __restrict__ step, int* __restrict__ choice, int split) {
@@ -720,8 +706,9 @@ __global__ void proj_bias_feedback_kernel(float* __restrict__ p, const float* __
   if (m < M && next_in) {
     const float x = forced ? tgt[((long long)b * To + t) * M + m] : v;
     if (!split) { next_in[b * M + m] = __float2bfloat16(x); return; }
+    const int Cp = (M + 63) / 64 * 64;
     const bf16 hi = __float2bfloat16(x);
-    next_in[b * 256 + m] = hi; next_in[b * 256 + 128 + m] = __float2bfloat16(x - __bfloat162float(hi));
+    next_in[b * 2 * Cp + m] = hi; next_in[b * 2 * Cp + Cp + m] = __float2bfloat16(x - __bfloat162float(hi));
   }
 }
 // normalisers -> s[5] (mel terms), s[6] (stop term); out (nullable) = the four normalised loss terms
@@ -779,7 +766,7 @@ int conv_block_fwd(const StepCtx& s, const ConvL& L, const void* x_in, int T, in
   bf16* y = reinterpret_cast<bf16*>(s.ws + L.w_y);
   float* yf = reinterpret_cast<float*>(s.ws + L.w_y);     // split mode keeps the pre-batch-norm activation in fp32
   int rc = launch_bias_act({.a = x_in, .C = L.cin, .T = T, .B = lo.B, .ntaps = L.k, .shifts = shifts, .split = split, .w = s.pk + L.k_w, .N = L.cout,
-                            .wK = L.k * L.cinp * (split ? 3 : 1), .BN = L.cout % 256 == 0 ? 256 : 128, .bias = s.params + L.p.bias, .act = L.act,
+                            .wK = L.k * L.cinp, .BN = L.cout % 256 == 0 ? 256 : 128, .bias = s.params + L.p.bias, .act = L.act,
                             .out_bf16 = split ? nullptr : y, .out_f32 = split ? yf : nullptr, .ldo = L.cout, .nvalid = L.cout},
                            s.st);
   if (rc) return rc;
@@ -1402,7 +1389,7 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
     StepCtx sc = s; sc.st = sx;
     float* pre = reinterpret_cast<float*>(ws + lo.w_encpre[d]);
     rc = launch_bias_act({.a = x, .C = lo.C, .T = Ti, .B = B, .split = lo.c.split_bf16, .w = pk + lo.k_encWx[d], .N = 4 * H,
-                          .wK = lo.C * (lo.c.split_bf16 ? 3 : 1), .BN = 256, .bias = d_params + lo.p_elb[d], .out_f32 = pre, .ldo = 4 * H, .nvalid = 4 * H},
+                          .wK = lo.C, .BN = 256, .bias = d_params + lo.p_elb[d], .out_f32 = pre, .ldo = 4 * H, .nvalid = 4 * H},
                          sx);
     if (rc) return rc;
     bf16* hh = reinterpret_cast<bf16*>(ws + lo.w_ench[d]);
@@ -1432,7 +1419,7 @@ static int encoder_fwd(const StepCtx& s, const int* d_inputs, const int* d_input
   t2_count_launch();
   float* keys = reinterpret_cast<float*>(ws + lo.w_keys);
   return launch_bias_act({.a = values, .C = 2 * H, .T = Ti, .B = B, .split = lo.c.split_bf16, .w = pk + lo.k_mem, .N = lo.A,
-                          .wK = 2 * H * (lo.c.split_bf16 ? 3 : 1), .BN = 128, .out_f32 = keys, .ldo = lo.A, .nvalid = lo.A},
+                          .wK = 2 * H, .BN = 128, .out_f32 = keys, .ldo = lo.A, .nvalid = lo.A},
                          st);
 }
 
@@ -1499,22 +1486,22 @@ static int decoder_step(const StepCtx& s, const DecBufs& d, const int* d_input_l
 static int prenet_fwd(const StepCtx& s, int row0, int nrows, unsigned long long seed, const unsigned long long* step, int hash_row0) {
   const TL& lo = *s.lo;
   const uint8_t* pk = s.pk; const float* d_params = s.params;
-  const int D = lo.D, sp = lo.c.split_bf16, k3 = sp ? 3 : 1;   // split_bf16: packed forward operands are [W_hi | W_hi | W_lo]
+  const int D = lo.D, sp = lo.c.split_bf16;
   bf16* decin = reinterpret_cast<bf16*>(s.ws + lo.w_decin) + (long long)row0 * lo.ld_decin;
   bf16* pn1 = reinterpret_cast<bf16*>(s.ws + lo.w_pn1) + (long long)row0 * lo.ld_pn1;
   bf16* pn2 = reinterpret_cast<bf16*>(s.ws + lo.w_pn2) + (long long)row0 * lo.ld_pn2;
   float* pre1 = reinterpret_cast<float*>(s.ws + lo.w_pre1) + (long long)row0 * 4 * D;
-  int rc = launch_bias_act({.a = decin, .C = lo.M, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p1, .N = lo.P1, .wK = 128 * k3,
+  int rc = launch_bias_act({.a = decin, .C = lo.M, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p1, .N = lo.P1, .wK = (lo.M + 63) / 64 * 64,
                             .BN = lo.P1 >= 256 ? 256 : 128, .bias = d_params + lo.p_p1b, .act = 1, .out_bf16 = pn1, .ldo = lo.P1, .nvalid = lo.P1,
                             .pdrop = lo.c.dropout_rate, .stream = 20, .seed = seed, .step = step, .hash_row0 = hash_row0},
                            s.st);
   if (rc) return rc;
-  rc = launch_bias_act({.a = pn1, .C = lo.P1, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p2, .N = lo.P2, .wK = lo.P1 * k3,
+  rc = launch_bias_act({.a = pn1, .C = lo.P1, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_p2, .N = lo.P2, .wK = lo.P1,
                         .BN = lo.P2 >= 256 ? 256 : 128, .bias = d_params + lo.p_p2b, .act = 1, .out_bf16 = pn2, .ldo = lo.P2, .nvalid = lo.P2,
                         .pdrop = lo.c.dropout_rate, .stream = 21, .seed = seed, .step = step, .hash_row0 = hash_row0},
                        s.st);
   if (rc) return rc;
-  return launch_bias_act({.a = pn2, .C = lo.P2, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_l1x, .N = 4 * D, .wK = lo.P2 * k3, .BN = 256,
+  return launch_bias_act({.a = pn2, .C = lo.P2, .T = nrows, .B = 1, .split = sp, .w = pk + lo.k_l1x, .N = 4 * D, .wK = lo.P2, .BN = 256,
                           .bias = d_params + lo.p_l1b, .out_f32 = pre1, .ldo = 4 * D, .nvalid = 4 * D},
                          s.st);
 }
@@ -1523,7 +1510,7 @@ static int prenet_fwd(const StepCtx& s, int row0, int nrows, unsigned long long 
 static int proj_fwd(const StepCtx& s, const DecBufs& d, int row0, int nrows) {
   const TL& lo = *s.lo;
   return launch_bias_act({.a = d.PI + (long long)row0 * lo.ld_PI, .C = d.PIK, .T = nrows, .B = 1, .split = lo.c.split_bf16, .w = s.pk + lo.k_proj,
-                          .N = lo.M + 1, .wK = d.PIK * (lo.c.split_bf16 ? 3 : 1), .BN = 128,
+                          .N = lo.M + 1, .wK = d.PIK, .BN = 128,
                           .out_f32 = reinterpret_cast<float*>(s.ws + lo.w_projo) + (long long)row0 * 128, .ldo = 128, .nvalid = lo.M + 1},
                          s.st);
 }
@@ -1566,7 +1553,7 @@ static int postnet_fwd(const StepCtx& s, int T, const float* mel_tgt, const floa
   for (auto& L : lo.post) { int rc = conv_block_fwd(s, L, x, T, s.training); if (rc) return rc; x = ws + L.w_x; }
   float* resid = reinterpret_cast<float*>(ws + lo.w_resid);
   int rc = launch_bias_act({.a = x, .C = lo.PC, .T = T, .B = B, .split = lo.c.split_bf16, .w = s.pk + lo.k_pp, .N = lo.M,
-                            .wK = lo.PC * (lo.c.split_bf16 ? 3 : 1), .BN = 128, .bias = s.params + lo.p_ppb, .out_f32 = resid, .ldo = 128, .nvalid = lo.M},
+                            .wK = lo.PC, .BN = 128, .bias = s.params + lo.p_ppb, .out_f32 = resid, .ldo = 128, .nvalid = lo.M},
                            st);
   if (rc) return rc;
   mel_finish_kernel<<<grid1d((long long)B * T * lo.M), 256, 0, st>>>(dec_f, resid, mel_tgt, reinterpret_cast<float*>(ws + lo.w_mel), scal, (long long)B * T,
@@ -2371,7 +2358,7 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
         T2_CHECK_CUDA(cudaGetLastError());
         return T2_OK;
       }
-      // pack_kernel: one job (add_pack) or the three jobs of add_pack_split, built here and copied into the caller's job buffer
+      // pack_kernel: one job (add_pack) or the three jobs of a split-bf16 slot, built here and copied into the caller's job buffer
       const int split = which == 1, W = int(i[2]), grid_x = int(i[3]);
       const long long src = i[4], dst = i[7];
       const int K = int(i[5]), N = int(i[6]), ld = int(i[8]), perm = int(i[split ? 12 : 11]);
@@ -2388,8 +2375,10 @@ extern "C" int t2_dbg_taco_kernel(const t2_dbg_kernel_t* call, void* stream) {
       T2_REQUIRE(ld >= col0 + extent && (!split || (ld >= col0 + slot + extent && ld >= col_lo + extent)), T2_ERR_INVALID_ARG,
                  "dbg_taco_kernel PARAMS pack: destination columns beyond the leading dimension %d", ld);
       std::vector<PackJob> jobs;
-      if (split) add_pack_split(jobs, src, K, N, 2 * dst, ld, col0, col_lo, slot, call->f[0], perm);
-      else {
+      if (split) {   // the three jobs of one split-bf16 weight slot (add_pack_fwd): W_hi at col_hi and col_hi + slot, W_lo at col_lo
+        for (int col : {col0, col0 + slot, col_lo}) add_pack(jobs, src, K, N, 2 * dst, ld, 1, col, call->f[0], perm);
+        jobs.back().part = 2;
+      } else {
         add_pack(jobs, src, K, N, 2 * dst, ld, transpose, col0, call->f[0], perm);
         jobs.back().part = part;
       }

@@ -240,12 +240,11 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   // ---- packed ----
   Arena pk;
   const long long L = lo.L;
-  const long long km = lo.split ? 3 : 1;   // split-bf16: every forward K segment becomes [W_hi | W_hi | W_lo]
-  lo.k_Wg = pk.take(L * lo.G * lo.Kg * km * 2);
-  lo.k_Wo = pk.take(L * lo.R * lo.Gh * km * 2);
-  lo.k_Ws = pk.take((long long)lo.S * L * lo.Gh * km * 2);
-  lo.k_Wf1 = pk.take((long long)lo.S * lo.S * km * 2);
-  lo.k_Wf2 = pk.take((long long)(lo.O < 32 ? 32 : lo.O) * lo.S * km * 2);
+  lo.k_Wg = pk.take(fwd_operand_bytes(L * lo.G, lo.Kg, lo.split));
+  lo.k_Wo = pk.take(fwd_operand_bytes(L * lo.R, lo.Gh, lo.split));
+  lo.k_Ws = pk.take(fwd_operand_bytes(lo.S, L * lo.Gh, lo.split));
+  lo.k_Wf1 = pk.take(fwd_operand_bytes(lo.S, lo.S, lo.split));
+  lo.k_Wf2 = pk.take(fwd_operand_bytes(lo.O < 32 ? 32 : lo.O, lo.S, lo.split));
   lo.k_WozT = pk.take(L * lo.Gh * (lo.R + lo.S) * 2);
   lo.k_WdT = pk.take(L * lo.R * lo.kw * lo.G * 2);
   lo.k_WcT = pk.take((long long)(lo.C > 0 ? lo.C : 8) * L * lo.G * 2);
@@ -283,22 +282,13 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
   lo.packjobs.clear();
   std::vector<PackJob>& pj = lo.packjobs;
   for (int l = 0; l < lo.L; ++l) {
-    const long long wg = lo.k_Wg + (long long)l * lo.G * lo.Kg * km * 2;
-    if (lo.split) {
-      const int R = lo.R, Gh = lo.Gh;
-      for (int j = 0; j < lo.kw; ++j)
-        add_pack_split(pj, lo.p_dil_k[l] + (long long)j * R * lo.G, R, lo.G, wg, 3 * lo.Kg, j * 3 * R, j * 3 * R + 2 * R, R, 1.f, Gh);
-      const int kc = 3 * lo.kw * R;   // the conditioning segment follows the kw tap segments of 3R each
-      if (lo.C > 0) add_pack_split(pj, lo.p_c_k[l], lo.C, lo.G, wg, 3 * lo.Kg, kc, kc + 256, 128, 1.f, Gh);
-      add_pack_split(pj, lo.p_o_k[l], Gh, R, lo.k_Wo + (long long)l * R * Gh * 3 * 2, 3 * Gh, 0, 2 * Gh, Gh);
-      // skip GEMM: K runs over [all layers: hi | hi] then [all layers: lo]
-      add_pack_split(pj, lo.p_s_k[l], Gh, lo.S, lo.k_Ws, 3 * lo.L * Gh, l * 2 * Gh, 2 * lo.L * Gh + l * Gh, Gh, lo.skip_scale[l]);
-    } else {
-    for (int j = 0; j < lo.kw; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, 1, j * lo.R, 1.f, lo.Gh);
-    if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, 1, lo.kw * lo.R, 1.f, lo.Gh);
-    add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, lo.k_Wo + (long long)l * lo.R * lo.Gh * 2, lo.Gh, 1, 0);
-    add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, lo.k_Ws, lo.L * lo.Gh, 1, l * lo.Gh, lo.skip_scale[l]);
-    }
+    // gate GEMM: one segment per tap, then the conditioning segment (128 columns wide); the skip GEMM loops K over the layers
+    const long long wg = lo.k_Wg + fwd_operand_bytes((long long)l * lo.G, lo.Kg, lo.split);
+    for (int j = 0; j < lo.kw; ++j)
+      add_pack_fwd(pj, lo.split, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wg, lo.Kg, j * lo.R, lo.R, 1.f, lo.Gh);
+    if (lo.C > 0) add_pack_fwd(pj, lo.split, lo.p_c_k[l], lo.C, lo.G, wg, lo.Kg, lo.kw * lo.R, 128, 1.f, lo.Gh);
+    add_pack_fwd(pj, lo.split, lo.p_o_k[l], lo.Gh, lo.R, lo.k_Wo + fwd_operand_bytes((long long)l * lo.R, lo.Gh, lo.split), lo.Gh, 0, lo.Gh);
+    add_pack_fwd(pj, lo.split, lo.p_s_k[l], lo.Gh, lo.S, lo.k_Ws, lo.L * lo.Gh, 0, lo.Gh, lo.skip_scale[l], 0, l, lo.L);
     const long long woz = lo.k_WozT + (long long)l * lo.Gh * (lo.R + lo.S) * 2;
     add_pack(pj, lo.p_o_k[l], lo.Gh, lo.R, woz, lo.R + lo.S, 0, 0, lo.res_scale);
     add_pack(pj, lo.p_s_k[l], lo.Gh, lo.S, woz, lo.R + lo.S, 0, lo.R, lo.skip_scale[l]);
@@ -306,13 +296,8 @@ int build_layout(const t2_wn_config_t* cfg, Layout& lo) {
     for (int j = 0; j < lo.kw; ++j) add_pack(pj, lo.p_dil_k[l] + (long long)j * lo.R * lo.G, lo.R, lo.G, wd, lo.kw * lo.G, 0, j * lo.G);
     if (lo.C > 0) add_pack(pj, lo.p_c_k[l], lo.C, lo.G, lo.k_WcT, lo.L * lo.G, 0, l * lo.G);
   }
-  if (lo.split) {
-    add_pack_split(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, 3 * lo.S, 0, 2 * lo.S, lo.S);
-    add_pack_split(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, 3 * lo.S, 0, 2 * lo.S, lo.S);
-  } else {
-    add_pack(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, lo.S, 1, 0);
-    add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, lo.S, 1, 0);
-  }
+  add_pack_fwd(pj, lo.split, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1, lo.S, 0, lo.S);
+  add_pack_fwd(pj, lo.split, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2, lo.S, 0, lo.S);
   add_pack(pj, lo.p_f1_k, lo.S, lo.S, lo.k_Wf1T, lo.S, 0, 0);
   add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 0);
   if (!lo.mol) add_pack(pj, lo.p_f2_k, lo.S, lo.O, lo.k_Wf2T, lo.Op, 0, 256);
@@ -1037,20 +1022,6 @@ ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int
   const int d = lo.dil(l);
   ActGemmCall g;
   memset(&g, 0, sizeof(g));
-  if (lo.split) {
-    // rows [hi | lo]: per tap one segment over both halves against [W_hi | W_hi] and one over the hi half against [W_lo]
-    g.a[0] = make_act(ws + lo.w_xd, 2 * lo.R, lo.T, lo.B, lo.L);
-    g.a[1] = make_act(ws + lo.w_cup, 256, lo.T, lo.B, 1);
-    g.na = lo.C > 0 ? 2 : 1;
-    g.nseg = 0;
-    for (int j = 0; j < lo.kw; ++j) {
-      const int shift = -(lo.kw - 1 - j) * d;
-      g.seg[g.nseg++] = Seg{0, shift, 0, 2 * lo.R / kBK, l, 1};
-      g.seg[g.nseg++] = Seg{0, shift, 0, lo.R / kBK, l, 1};
-    }
-    if (lo.C > 0) { g.seg[g.nseg++] = Seg{1, 0, 0, 4, 0, 1}; g.seg[g.nseg++] = Seg{1, 0, 0, 2, 0, 1}; }
-    g.w = pk + lo.k_Wg; g.wN = lo.G; g.wK = 3 * lo.Kg; g.wL = lo.L; g.w_layer = l; g.w_k0 = 0;
-  } else {
   g.a[0] = make_act(ws + lo.w_xd, lo.R, lo.T, lo.B, lo.L);
   g.a[1] = make_act(ws + lo.w_cup, lo.C > 0 ? lo.C : 8, lo.T, lo.B, 1);
   g.na = lo.C > 0 ? 2 : 1;
@@ -1058,13 +1029,12 @@ ActGemmCall make_gate_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, int
   g.nseg = lo.kw;
   if (lo.C > 0) g.seg[g.nseg++] = Seg{1, 0, 0, 2, 0, 1};
   g.w = pk + lo.k_Wg; g.wN = lo.G; g.wK = lo.Kg; g.wL = lo.L; g.w_layer = l; g.w_k0 = 0;
-  }
+  g.split = lo.split;
   g.T = lo.T; g.B = lo.B; g.n_tiles = lo.G / 256;
   const long long lofs = (long long)l * BT * lo.Gh;
   g.epi.ptr[0] = save ? reinterpret_cast<bf16*>(ws + lo.w_ta) + lofs : nullptr;
   g.epi.ptr[1] = save ? reinterpret_cast<bf16*>(ws + lo.w_sb) + lofs : nullptr;
   g.epi.ptr[2] = reinterpret_cast<bf16*>(ws + lo.w_z) + lofs * lo.xm;
-  g.epi.i[11] = lo.split ? 1 : 0;
   g.epi.ptr[3] = const_cast<float*>(reinterpret_cast<const float*>(pk + lo.k_bias_g) + (long long)l * lo.G);
   if (lo.Gi > 0) {   // per-item gate biases (gin_bias_kernel): item b's row at + b * G
     g.epi.ptr[3] = reinterpret_cast<float*>(ws + lo.w_gbias) + (long long)l * lo.B * lo.G;
@@ -1081,14 +1051,13 @@ ActGemmCall make_out_call(const Layout& lo, uint8_t* ws, const uint8_t* pk, cons
   bf16* xd_all = reinterpret_cast<bf16*>(ws + lo.w_xd);
   ActGemmCall o;
   memset(&o, 0, sizeof(o));
-  o.a[0] = make_act(ws + lo.w_z, lo.Gh * lo.xm, lo.T, lo.B, lo.L); o.na = 1;
-  o.seg[0] = Seg{0, 0, 0, lo.Gh * lo.xm / kBK, l, 1}; o.nseg = 1;
-  if (lo.split) { o.seg[1] = Seg{0, 0, 0, lo.Gh / kBK, l, 1}; o.nseg = 2; }
-  o.w = pk + lo.k_Wo; o.wN = lo.R; o.wK = lo.Gh * (lo.split ? 3 : 1); o.wL = lo.L; o.w_layer = l;
+  o.a[0] = make_act(ws + lo.w_z, lo.Gh, lo.T, lo.B, lo.L); o.na = 1;
+  o.seg[0] = Seg{0, 0, 0, lo.Gh / kBK, l, 1}; o.nseg = 1;
+  o.w = pk + lo.k_Wo; o.wN = lo.R; o.wK = lo.Gh; o.wL = lo.L; o.w_layer = l;
+  o.split = lo.split;
   o.T = lo.T; o.B = lo.B; o.n_tiles = 1;
   o.epi.ptr[0] = x_all + (long long)l * BT * lo.R * lo.xm;
   o.epi.ptr[1] = x_all + (long long)(l + 1) * BT * lo.R * lo.xm;
-  o.epi.i[11] = lo.split ? 1 : 0;
   o.epi.ptr[2] = p > 0.f ? xd_all + (long long)(l + 1) * BT * lo.R : nullptr;
   o.epi.ptr[3] = const_cast<float*>(params + lo.p_o_b[l]);
   o.epi.f[0] = lo.res_scale; o.epi.f[1] = p; o.epi.i[1] = l + 1; o.epi.seed = seed;
@@ -1509,7 +1478,6 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   T2_CHECK_CUDA(cudaGetLastError());
   // 3. residual stack
   bf16* z_all = reinterpret_cast<bf16*>(ws + lo.w_z);
-  const ActT a_z = make_act(z_all, lo.Gh * lo.xm, lo.T, lo.B, lo.L);
   if (use_chain(lo)) {
     rc = launch_chain(lo, 0, ws, pk, d_params, save_for_backward != 0, seed, d_step, 0, st);
     if (rc) return rc;
@@ -1528,40 +1496,23 @@ extern "C" int t2_wn_forward(const t2_wn_config_t* cfg, const float* d_params, c
   // 4. all skip 1x1s as one K = L*Gh GEMM, + ReLU
   bf16* h1 = reinterpret_cast<bf16*>(ws + lo.w_h1);
   bf16* h2 = reinterpret_cast<bf16*>(ws + lo.w_h2);
-  {
-    ActGemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.a[0] = a_z; g.na = 1;
-    g.seg[0] = Seg{0, 0, 0, lo.Gh * lo.xm / kBK, 0, lo.L}; g.nseg = 1;
-    if (lo.split) { g.seg[1] = Seg{0, 0, 0, lo.Gh / kBK, 0, lo.L}; g.nseg = 2; }
-    g.w = pk + lo.k_Ws; g.wN = lo.S; g.wK = lo.L * lo.Gh * (lo.split ? 3 : 1); g.wL = 1;
-    g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
-    g.epi.ptr[0] = h1; g.epi.ptr[1] = const_cast<float*>(reinterpret_cast<const float*>(pk + lo.k_bias_skip));
-    g.epi.i[0] = lo.S; g.epi.i[1] = 1; g.epi.i[2] = lo.S; g.epi.i[11] = lo.split ? 1 : 0;
-    rc = launch_act_gemm(EPI_BIAS_ACT, lo.S, g, st);
-    if (rc) return rc;
-  }
-  {
-    ActGemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.a[0] = make_act(h1, lo.S * lo.xm, lo.T, lo.B); g.na = 1;
-    g.seg[0] = Seg{0, 0, 0, lo.S * lo.xm / kBK, 0, 1}; g.nseg = 1;
-    if (lo.split) { g.seg[1] = Seg{0, 0, 0, lo.S / kBK, 0, 1}; g.nseg = 2; }
-    g.w = pk + lo.k_Wf1; g.wN = lo.S; g.wK = lo.S * (lo.split ? 3 : 1); g.wL = 1;
-    g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
-    g.epi.ptr[0] = h2; g.epi.ptr[1] = const_cast<float*>(d_params + lo.p_f1_b);
-    g.epi.i[0] = lo.S; g.epi.i[1] = 1; g.epi.i[2] = lo.S; g.epi.i[11] = lo.split ? 1 : 0;
-    rc = launch_act_gemm(EPI_BIAS_ACT, lo.S, g, st);
-    if (rc) return rc;
-  }
+  rc = launch_bias_act({.a = z_all, .C = lo.Gh, .T = lo.T, .B = lo.B, .layers = lo.L, .split = lo.split, .w = pk + lo.k_Ws, .N = lo.S,
+                        .wK = lo.L * lo.Gh, .BN = lo.S, .bias = reinterpret_cast<const float*>(pk + lo.k_bias_skip), .act = 1, .out_bf16 = h1,
+                        .ldo = lo.S, .nvalid = lo.S},
+                       st);
+  if (rc) return rc;
+  rc = launch_bias_act({.a = h1, .C = lo.S, .T = lo.T, .B = lo.B, .split = lo.split, .w = pk + lo.k_Wf1, .N = lo.S, .wK = lo.S, .BN = lo.S,
+                        .bias = d_params + lo.p_f1_b, .act = 1, .out_bf16 = h2, .ldo = lo.S, .nvalid = lo.S},
+                       st);
+  if (rc) return rc;
   // 5. output projection fused with the loss
   {
     ActGemmCall g;
     memset(&g, 0, sizeof(g));
-    g.a[0] = make_act(h2, lo.S * lo.xm, lo.T, lo.B); g.na = 1;
-    g.seg[0] = Seg{0, 0, 0, lo.S * lo.xm / kBK, 0, 1}; g.nseg = 1;
-    if (lo.split) { g.seg[1] = Seg{0, 0, 0, lo.S / kBK, 0, 1}; g.nseg = 2; }
-    g.w = pk + lo.k_Wf2; g.wN = lo.O; g.wK = lo.S * (lo.split ? 3 : 1); g.wL = 1;
+    g.a[0] = make_act(h2, lo.S, lo.T, lo.B); g.na = 1;
+    g.seg[0] = Seg{0, 0, 0, lo.S / kBK, 0, 1}; g.nseg = 1;
+    g.w = pk + lo.k_Wf2; g.wN = lo.O; g.wK = lo.S; g.wL = 1;
+    g.split = lo.split;
     g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
     g.epi.ptr[0] = const_cast<void*>(d_targets);
     g.epi.ptr[1] = const_cast<int*>(d_lengths);
@@ -1742,15 +1693,9 @@ extern "C" int t2_wn_backward_phased(const t2_wn_config_t* cfg, const float* d_p
   // conditioning path
   if (lo.C > 0 && !cfg->c_pre_upsampled) {
     float* dcup = reinterpret_cast<float*>(ws + lo.w_dcup);
-    ActGemmCall g;
-    memset(&g, 0, sizeof(g));
-    g.a[0] = a_dg; g.na = 1;
-    g.seg[0] = Seg{0, 0, 0, lo.G / kBK, 0, lo.L}; g.nseg = 1;
-    g.w = pk + lo.k_WcT; g.wN = lo.C; g.wK = lo.L * lo.G; g.wL = 1;
-    g.T = lo.T; g.B = lo.B; g.n_tiles = 1;
-    g.epi.ptr[0] = nullptr; g.epi.ptr[1] = nullptr; g.epi.ptr[2] = dcup;
-    g.epi.i[0] = lo.C; g.epi.i[1] = 0; g.epi.i[2] = lo.C;
-    rc = launch_act_gemm(EPI_BIAS_ACT, 128, g, sb);
+    rc = launch_bias_act({.a = dg, .C = lo.G, .T = lo.T, .B = lo.B, .layers = lo.L, .w = pk + lo.k_WcT, .N = lo.C, .wK = lo.L * lo.G, .BN = 128,
+                          .out_f32 = dcup, .ldo = lo.C, .nvalid = lo.C},
+                         sb);
     if (rc) return rc;
     // dc_up arrives channels-last from the GEMM: transpose once into [B][C][T]
     float* dchw = reinterpret_cast<float*>(ws + lo.w_upgrad[1]);

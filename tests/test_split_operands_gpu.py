@@ -477,22 +477,24 @@ def test_embed_fwd_split():
 def test_decin_split():
     g = torch.Generator().manual_seed(2)
     B, To, M = 3, 21, 80
+    Cp = (M + 63) // 64 * 64
     tgt = (torch.randn(B, To, M, generator=g) * 2).to(DEV)
-    out = nan_buf((To * B + 1, 256), torch.bfloat16)
+    out = nan_buf((To * B + 1, 2 * Cp), torch.bfloat16)
     ref = nan_buf((To * B, M), torch.bfloat16)
     rows(1, 1, [tgt, out], [B, To, M])
     rows(1, 0, [tgt, ref], [B, To, M])
     v = torch.cat([torch.zeros(1, B, M, device=DEV), tgt.transpose(0, 1)[:-1]]).reshape(To * B, M)   # row t b: target[b][t - 1]
-    assert_split_exact("decin", out[:To * B, :M], out[:To * B, 128:128 + M], v)
+    assert_split_exact("decin", out[:To * B, :M], out[:To * B, Cp:Cp + M], v)
     assert torch.equal(out[:To * B, :M].view(torch.int16), ref.view(torch.int16))
-    # [hi(M) | pad | lo(M) | pad] at pitch 256: the padding is the engine's zero-initialised workspace and is never written
-    all_nan("decin padding", torch.cat([out[:, M:128].flatten(), out[:, 128 + M:].flatten(), out[To * B:].flatten()]))
+    # [hi(M) | pad | lo(M) | pad] at pitch 2 Cp: the padding is the engine's zero-initialised workspace and is never written
+    all_nan("decin padding", torch.cat([out[:, M:Cp].flatten(), out[:, Cp + M:].flatten(), out[To * B:].flatten()]))
 
 
 @pytest.mark.parametrize("clip,with_tgt", [(1, True), (0, False)])
 def test_dec_finish_split(clip, with_tgt):
     g = torch.Generator().manual_seed(3 + clip)
     B, To, M = 3, 19, 80
+    Cp = (M + 63) // 64 * 64
     projo = torch.full((To, B, 128), NAN)
     projo[..., :M + 1] = torch.randn(To, B, M + 1, generator=g) * 3
     projo = projo.to(DEV)
@@ -501,7 +503,7 @@ def test_dec_finish_split(clip, with_tgt):
     lo_c, hi_c = -4.1, 4.0
     outs = {}
     for sm in (1, 0):
-        dec_bm = nan_buf((B * To + 1, 256 if sm else M), torch.bfloat16)
+        dec_bm = nan_buf((B * To + 1, 2 * Cp if sm else M), torch.bfloat16)
         dec_f, stop = nan_buf((B, To, M), torch.float32), nan_buf((B, To), torch.float32)
         scal = torch.zeros(5, device=DEV)
         rows(2, sm, [projo, tgt, stop_t, dec_bm, dec_f, stop, scal, None], [B, To, M, clip], [lo_c, hi_c, 1.0])
@@ -512,9 +514,9 @@ def test_dec_finish_split(clip, with_tgt):
     v = projo[..., :M].transpose(0, 1).reshape(B * To, M)
     v = v.clamp(lo_c, hi_c) if clip else v
     assert torch.equal(sf.view(B * To, M), v)
-    assert_split_exact("dec_finish", sb[:B * To, :M], sb[:B * To, 128:128 + M], v)
+    assert_split_exact("dec_finish", sb[:B * To, :M], sb[:B * To, Cp:Cp + M], v)
     assert torch.equal(sb[:B * To, :M].view(torch.int16), bb[:B * To].view(torch.int16))
-    all_nan("dec_finish padding", torch.cat([sb[:, M:128].flatten(), sb[:, 128 + M:].flatten(), sb[B * To:].flatten()]))
+    all_nan("dec_finish padding", torch.cat([sb[:, M:Cp].flatten(), sb[:, Cp + M:].flatten(), sb[B * To:].flatten()]))
 
 
 @pytest.mark.parametrize("ratio", [None, 0.0, 1.0, 0.5])
@@ -522,6 +524,7 @@ def test_proj_bias_feedback_split(ratio):
     """the next decoder input row, from the predicted frame or (teacher-forcing ratio < 1) the target frame the draw picks"""
     g = torch.Generator().manual_seed(4)
     B, M, To, t, seed, off = 5, 80, 9, 3, 99, 4
+    Cp = (M + 63) // 64 * 64
     p0 = torch.full((B, 128), NAN)
     p0[:, :M + 1] = torch.randn(B, M + 1, generator=g) * 2
     fb, sb = (torch.randn(M, generator=g) * 0.1).to(DEV), (torch.randn(1, generator=g)).to(DEV)
@@ -529,7 +532,7 @@ def test_proj_bias_feedback_split(ratio):
     res = {}
     for sm in (1, 0):
         p = p0.clone().to(DEV)
-        nxt = nan_buf((B, 256 if sm else M), torch.bfloat16)
+        nxt = nan_buf((B, 2 * Cp if sm else M), torch.bfloat16)
         choice = torch.full((To,), -1, dtype=torch.int32, device=DEV) if ratio is not None else None
         rows(3, sm, [p, fb, sb, nxt, tgt, choice], [B, M, To, t], [ratio or 0.0], seed=seed, step=seed_offset(off))
         res[sm] = (p, nxt, choice)
@@ -542,9 +545,9 @@ def test_proj_bias_feedback_split(ratio):
         forced = bool(mh.hash_uniform32(mh.hash_seed(seed + off, 40), np.array([t], dtype=np.uint64))[0] < np.float32(ratio))
         assert int(sch[t]) == int(forced) and int(bch[t]) == int(forced)
     x = tgt[:, t] if forced else pv[:, :M]
-    assert_split_exact("feedback", sn[:, :M], sn[:, 128:128 + M], x)
+    assert_split_exact("feedback", sn[:, :M], sn[:, Cp:Cp + M], x)
     assert torch.equal(sn[:, :M].view(torch.int16), bn.view(torch.int16))
-    all_nan("feedback padding", torch.cat([sn[:, M:128].flatten(), sn[:, 128 + M:].flatten()]))
+    all_nan("feedback padding", torch.cat([sn[:, M:Cp].flatten(), sn[:, Cp + M:].flatten()]))
 
 
 @pytest.mark.parametrize("C,Cp", [(80, 128), (128, 128), (1025, 1088)])

@@ -482,7 +482,7 @@ def run_pack(which, K, N, src_off, dst_off, ld, cols, transpose, perm, W, part, 
     ref = torch.full((size,), NAN, dtype=torch.bfloat16)
     if which == 0:
         cover = pack_expect(ref, src, K, N, dst_off, ld, transpose, cols[0], perm, W, part, scale)
-    else:                                                          # add_pack_split: hi at col_hi and col_hi + slot, lo at col_lo
+    else:                                                          # split slot: hi at col_hi and col_hi + slot, lo at col_lo
         cover = pack_expect(ref, src, K, N, dst_off, ld, 1, cols[0], perm, W, 0, scale)
         cover |= pack_expect(ref, src, K, N, dst_off, ld, 1, cols[0] + cols[2], perm, W, 0, scale)
         cover |= pack_expect(ref, src, K, N, dst_off, ld, 1, cols[1], perm, W, 2, scale)
@@ -518,7 +518,7 @@ PACK_SPLIT_CASES = [  # K, N, src_off, dst_off, dst_ld, col_hi, col_lo, slot, pe
 @GPU
 @pytest.mark.parametrize("K,N,src_off,dst_off,ld,col_hi,col_lo,slot,perm,W,scale,grid_x", PACK_SPLIT_CASES)
 def test_pack_split(K, N, src_off, dst_off, ld, col_hi, col_lo, slot, perm, W, scale, grid_x):
-    """the three jobs of add_pack_split in one launch (grid.y = 3): [W_hi | W_hi | W_lo] of the scaled weights"""
+    """the three jobs of one split-bf16 weight slot in one launch (grid.y = 3): [W_hi | W_hi | W_lo] of the scaled weights"""
     run_pack(1, K, N, src_off, dst_off, ld, (col_hi, col_lo, slot), 1, perm, W, 0, scale, grid_x, K + N + slot)
 
 

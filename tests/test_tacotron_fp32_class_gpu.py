@@ -36,11 +36,12 @@ def _tol(align, dec_l1, stop, loss):
     return dict(align=align, dec_l1=dec_l1, mel_l1=MEL_L1, stop=stop, loss=loss, grad_rel=1.0, grad_cos=0.0)
 
 
-@pytest.mark.parametrize("stochastic", [False, True])
-def test_teacher_forced_cfg3(stochastic):
-    """B = 32, T_in 160, T_out 200; stochastic: conv / prenet dropout 0.5 and zoneout 0.1 with the device's masks injected"""
-    hp = _hp(stochastic)
-    tag = "tacotron_fp32_class_cfg3_%s" % ("stochastic" if stochastic else "deterministic")
+@pytest.mark.parametrize("stochastic,num_mels", [(False, 80), (True, 80), (False, 40)], ids=["False", "True", "num_mels40"])
+def test_teacher_forced_cfg3(stochastic, num_mels):
+    """B = 32, T_in 160, T_out 200; stochastic: conv / prenet dropout 0.5 and zoneout 0.1 with the device's masks injected. 40 mels fill
+    one 64-wide K block per half of the split mel rows (decoder input, postnet input) instead of two."""
+    hp = _hp(stochastic, num_mels=num_mels)
+    tag = "tacotron_fp32_class_cfg3_%s%s" % ("stochastic" if stochastic else "deterministic", "" if num_mels == 80 else "_mels%d" % num_mels)
     m = taco_compare(tag, hp, 32, 160, 200, 61, _tol(2.7e-5, 5.5e-6, 3e-5, 5e-5), backward=False, precision="fp32-class").measured
     assert m["mel_l1"] <= MEL_L1, m
 
